@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- the measure-query hot path on B200: scanned datapoints/s and achieved HBM GB/s.
+"""bench.py -- the measure-query hot path on H100: scanned datapoints/s and achieved HBM GB/s.
 
 Workload = BASELINE.json's north-star configuration (configs[2] / configs[3], SURVEY.md 8d C3 / C4):
     1e9 datapoints (10 000 series x 100 000 points), 4 float64 fields (latency, walk, ints, uniform) + a dictionary tag,
     query  GROUP BY service_id (1000 services x 10 series)  sum(latency), count(latency)  ->  Top 100 by the sum.
 A "step" is one pass of the hot path (block selection -> page decode -> filter -> aggregate -> Top-N) over all of it.
 
-``--gpus 1``  one part of 1e9 datapoints resident in one B200's HBM.
+``--gpus 1``  one part of 1e9 datapoints resident in one H100's HBM (12.8 GB of part files).
 ``--gpus N``  (torchrun) the SAME 1e9 datapoints sharded by series range over N ranks -- STRONG scaling (C4): every rank
               scans its shard into a partial table on its GPU, the tables meet on rank 0, which finalises (MEAN / Top-N).
 
@@ -14,13 +14,16 @@ A "step" is one pass of the hot path (block selection -> page decode -> filter -
 ``e2e``          the same metric through the host-buffer entry point of the C ABI (bydb_scan_agg_host): part file images in
                  HOST memory in, result out, every step; legs for a caller whose images are pinned and for one whose are not.
 ``roofline``     algorithmic bytes (SURVEY.md 8d: 8 B per scanned datapoint for this query -- one float64 column; the group
-                 id is per series, never read per row) / the scan kernel's CUDA-event time, against MEASURED_PEAKS.json.
+                 id is per series, never read per row) / the scan kernel's CUDA-event time, against the H100 SXM data-sheet HBM
+                 bandwidth (3.35 TB/s; a bound, not a measured peak).
 ``c2_query``     second leg on the same part: BASELINE configs[1]'s query (time range AND region == "r3", avg(latency) +
                  max(walk)), 25 algorithmic B per datapoint.
 ``cpu_baseline`` the oracle (C restatement of the reference's Go path; Go cannot be built in this image) on the host cores
                  over a stated sample of the same series, reference-shaped and all-core, with the GPU's answer on exactly
                  that sample compared against it (``agrees_with_gpu``).
 ``--impl reference`` times that CPU port alone on parts written by the oracle's own writer; the product library is not loaded.
+``--dump-outputs DIR`` writes the result of the last timed step (the arrays a caller receives) as DIR/<name>.npy, float64, so that
+                 two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -44,6 +47,7 @@ SEED = 0xB200
 B_ALG_C3 = 8    # sum(latency): one float64 column per scanned row (SURVEY.md 8d, C3)
 B_ALG_C2 = 25   # 8 (timestamp) + 1 (dictionary tag) + 2 x 8 (fields)            (SURVEY.md 8d, C2)
 METRIC = "measure datapoints scanned+aggregated/sec"
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet, HBM3
 
 
 def parse_args():
@@ -60,6 +64,7 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the sustained / graph / C2-query legs (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's result arrays as DIR/<name>.npy (float64)")
     return ap.parse_args()
 
 
@@ -78,14 +83,12 @@ def workload_text(n_series, n_points, services, world):
     return s
 
 
-def traffic_from_profile():
-    """dram__bytes_read.sum + dram__bytes_write.sum of one scan launch of this query, from the committed
-    ncu --set full capture (profiles/traffic.json names it); None when there is none."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        return int(t["dram_bytes_read"]) + int(t["dram_bytes_write"])
-    except Exception:
-        return None
+def dump_outputs(out_dir, r):
+    """The arrays a caller of the timed path receives (capi.Result), as float64 .npy files; all values are small integers or
+    float64, so the conversion is exact."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name in ("group_id", "rows", "is_float", "val_i64", "val_f64"):
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(getattr(r, name)).astype(np.float64))
 
 
 FIELD_KINDS = ("latency", "walk", "ints", "uniform")
@@ -111,8 +114,15 @@ def c2_query(pkg, handles, sids, n_points):
                      tmax=T0 + (3 * n_points // 4) * STEP, preds=[pkg.Pred("default", "region", pkg.OP_EQ, b"r3")])
 
 
+def _die_with_parent():
+    """Child-side hook: the sampler is killed with the bench if the bench exits without stopping it (error, signal)."""
+    import ctypes
+    import signal
+    ctypes.CDLL(None).prctl(1, signal.SIGTERM)  # PR_SET_PDEATHSIG
+
+
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed regions (B200_PROFILING.md)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed regions."""
 
     def __init__(self, index: int):
         self.index = index
@@ -125,7 +135,8 @@ class ClockSampler:
                 ["nvidia-smi", "-i", str(self.index),
                  "--query-gpu=clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
                  "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap",
-                 "--format=csv,noheader,nounits", "-lms", "100"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+                 "--format=csv,noheader,nounits", "-lms", "100"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True,
+                preexec_fn=_die_with_parent)
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
         except Exception:
@@ -313,7 +324,7 @@ def main():
     cores = os.cpu_count() or 1
     cfg = {"workload": workload_text(n_series, n_points, services, world), "n_series": n_series, "n_points": n_points, "services": services,
            "query": "sum(latency), count(latency) GROUP BY service_id, Top 100",
-           "timing": "inputs larger than L2 (no flush needed): the encoded latency pages of one step are ~1.9 GB per 1e9 datapoints vs 126 MB L2"}
+           "timing": "inputs larger than L2 (no flush needed): the encoded latency pages of one step are ~1.9 GB per 1e9 datapoints vs 50 MB L2"}
 
     if args.impl == "reference":
         if rank == 0:
@@ -461,6 +472,8 @@ def main():
     except Exception as ex:  # noqa: BLE001 -- keep the bench line alive: the plain call is then the timed one
         graph_note = {"error": str(ex)[:200]}
         dt, last, timed_step = d_plain, last_plain, step
+    if args.dump_outputs and last is not None:
+        dump_outputs(args.dump_outputs, last)
     kernel_timing = "cuda events inside the plain calls of the same step (a graph replay has no per-kernel events); value is timed on the prepared-query path"
     rows_step = stats_acc[-1].rows_scanned
     scan_ms = float(np.mean([s.scan_kernel_ms for s in stats_acc]))
@@ -630,22 +643,17 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = HBM_PEAK_GBS
     achieved = rows_step * B_ALG_C3 / (scan_ms * 1e-3) / 1e9
-    roofline = {"bound": "hbm", "kernel": "scan_sum_express_kernel (timed with the two empty lanes launched behind it, ~6 us)",
+    roofline = {"bound": "hbm", "kernel": "scan_sum_express_kernel (timed with the two empty lanes launched behind it)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (burst copy)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)",
+                "peak_source": "H100 SXM data sheet (HBM3, 3.35 TB/s); not a measured peak",
                 "algorithmic_bytes_per_datapoint": B_ALG_C3, "algorithmic_bytes_per_launch": int(rows_step * B_ALG_C3), "kernel_ms": scan_ms,
                 "kernel_ms_max_over_ranks": scan_ms_max, "encoded_page_bytes_per_launch": int(page_bytes),
                 "encoded_GBps": page_bytes / (scan_ms * 1e-3) / 1e9, "frac_encoded": page_bytes / (scan_ms * 1e-3) / 1e9 / peak,
-                "traffic": traffic_from_profile() if world == 1 else None, "kernel_timing": kernel_timing,
+                "kernel_timing": kernel_timing,
                 "reading": "frac counts SURVEY 8(d)'s 8 decoded bytes per datapoint; the pages hold ~1.9 encoded bytes per datapoint, so frac can "
-                           "pass 1 while DRAM runs at frac_encoded of the copy peak: the kernel is bound by the ALU pipe (ncu: 74 % busy), not by HBM",
+                           "pass 1 while DRAM runs at frac_encoded of the peak",
                 "note": "per launch on rank 0's shard" if world > 1 else "per launch"}
     out = {"metric": METRIC, "value": value, "unit": "datapoints/s", "n_gpus": world, "steps": args.steps, "warmup": warm,
            "ms_per_step": dt / args.steps * 1e3, "higher_is_better": True, "scaling": "strong" if world > 1 else "n/a", "vs_baseline": None,

@@ -1,5 +1,5 @@
 /*
- * bydb_gpu.h -- C ABI of libbydbgpu.so: the B200-native measure scan -> filter -> aggregate path.
+ * bydb_gpu.h -- C ABI of libbydbgpu.so: the H100-native (sm_90a) measure scan -> filter -> aggregate path.
  *
  * This is the drop-in boundary a cgo binding in BanyanDB would bind (see INTEGRATION.md).  It
  * replaces, for one query, the reference's HOT LOOPS 1-3 (SURVEY.md section 3.1):

@@ -2,7 +2,7 @@
  * bydb_oracle.h -- CPU ORACLE for the BanyanDB measure-query hot path.
  *
  * TEST INFRASTRUCTURE ONLY.  This is a plain-C restatement of the reference's
- * Go algorithm (apache/skywalking-banyandb @ /root/reference).  Only tests/,
+ * Go algorithm (apache/skywalking-banyandb, commit 0dd5d684).  Only tests/,
  * __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs
  * may load this library.  The product (libbydbgpu.so) never links, loads or
  * calls anything in oracle/.

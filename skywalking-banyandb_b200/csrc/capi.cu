@@ -132,7 +132,7 @@ struct ExecSlot {
 }  // namespace
 
 // A few persistent host threads for the cold path's block-index parsing: creating a dozen threads per query costs
-// more (~0.5 ms, serialised on the calling thread) than parsing the first primary block.
+// more (serialised on the calling thread) than parsing the first primary block.
 class WorkPool {
   public:
     ~WorkPool() {
@@ -1384,7 +1384,7 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
 extern "C" {
 
 const char *bydb_last_error(void) { return g_last_error.c_str(); }
-const char *bydb_version(void) { return "bydb-b200 0.1 (sm_100a)"; }
+const char *bydb_version(void) { return "bydb-b200 0.1 (sm_90a)"; }
 
 int bydb_init(const bydb_cfg *cfg, bydb_ctx **out) {
     return guarded([&]() -> int {
@@ -1397,7 +1397,9 @@ int bydb_init(const bydb_cfg *cfg, bydb_ctx **out) {
     CUDA_TRY(cudaSetDevice(dev));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major < 10) return fail(BYDB_ENOTSUP, std::string("device '") + prop.name + "' is not sm_100 (Blackwell); this library is built for sm_100a only");
+    // sm_90a code (arch-specific: TMA bulk copies, mbarrier transaction counts) loads on compute capability 9.0 only
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(BYDB_ENOTSUP, std::string("device '") + prop.name + "' is not sm_90 (Hopper); this library is built for sm_90a only");
     auto ctx = new bydb_ctx();
     ctx->device = dev;
     ctx->sm_count = prop.multiProcessorCount;
@@ -1586,7 +1588,7 @@ int bydb_scan_agg(bydb_ctx *ctx, const bydb_query *q, bydb_result *out) {
 
 // ------------------------------------------------------------------------------------------------
 // Gather path of the cold query (host images in pageable memory, e.g. BanyanDB's mmap'd part files): instead of copying
-// every file of the part to HBM (12.8 GB for the 1e9 bench part, 1.1 s from pageable memory), the host selects the blocks
+// every file of the part to HBM (12.8 GB for the 1e9 bench part), the host selects the blocks
 // like plan_blocks does and collects ONLY the pages the query reads -- the timestamps page, the aggregated fields, the
 // predicate tags -- into one arena image per slice: [DevBlock[] | DevCol[] | file table | pages], every page offset
 // rewritten into the arena.  The image goes up through the pinned staging ring in 64 MB chunks.
@@ -2150,8 +2152,8 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
         std::string err;
         int rc = 0;
     };
-    // pieces of one or two primary blocks: the first piece (= the first slice the GPU can start on) is parsed in well under a
-    // millisecond; with 32 pieces it took 4.8 ms of a 45 ms step before anything was launched (traced step, r02n)
+    // pieces of one or two primary blocks: the first piece (= the first slice the GPU can start on) is parsed quickly; with
+    // fewer, larger pieces the GPU waits for the first big one before anything is launched
     const size_t T = std::max<size_t>(1, std::min<size_t>(n_primary, 128));
     const bool trace = getenv("BYDB_TRACE") != nullptr;  // host-side timeline of the cold path on stderr (read per call: a caller can trace one step)
     const auto t_begin = std::chrono::steady_clock::now();

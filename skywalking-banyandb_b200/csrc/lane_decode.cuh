@@ -64,7 +64,7 @@ constexpr uint32_t kFastChunkBytes = 32 * kFastLaneBytes;  // 1 KB per warp iter
 BYDB_LANE_FN uint32_t low_bits(uint32_t n) { return n >= 32 ? 0xffffffffu : ((1u << n) - 1u); }
 
 // 32-bit multiply-add that stays a multiply-add: IMAD runs on the FMA pipe, which this integer kernel otherwise
-// leaves idle while LOP3/SHF/SEL/IADD3 saturate the ALU pipe (ncu r01h: alu 82 %, fma 17 %).  Written as inline PTX
+// leaves idle while LOP3/SHF/SEL/IADD3 saturate the ALU pipe.  Written as inline PTX
 // so that neither the front end nor ptxas turns a multiply by a 0/1 flag back into logic ops.
 BYDB_LANE_FN uint32_t imad_u32(uint32_t a, uint32_t b, uint32_t c) {
     uint32_t d;
@@ -230,7 +230,7 @@ BYDB_LANE_FN void swar_begin(SwarLane &s, uint32_t prev_w) {
 }
 // kMasked: first / last chunk of a page -- vm is 0xff for the bytes of the word that belong to the page; the others
 // neither terminate, nor carry payload, nor continue anything.
-// Pipe balance (ncu r01: this integer kernel is bound by the ALU pipe, LOP3/PRMT/SHF, while the FMA pipe idles): everything
+// Pipe balance (this integer kernel loads the ALU pipe, LOP3/PRMT/SHF, while the FMA pipe idles): everything
 // that can be a multiply-add is one -- the shifts by constants (IMAD / IMAD.HI), the in-word prefix sum, the running
 // terminator count (a dot product with 1s) and its broadcast.
 template <bool kMasked>

@@ -1,4 +1,4 @@
-// scan_kernels.cu -- hand-written sm_100a kernels of the measure scan -> filter -> aggregate path.
+// scan_kernels.cu -- hand-written sm_90a kernels of the measure scan -> filter -> aggregate path.
 //
 //   plan_blocks    a1-a3  block selection: sid in query set AND [ts_min,ts_max] overlaps [tmin,tmax]
 //                         (banyand/measure/part_iter.go:79-250, query.go:594-639)
@@ -1099,8 +1099,8 @@ __device__ __noinline__ int delta_page_sparse(WarpSmem *sm, int lane) {
         SwarLite sl;
         uint32_t lastw;
         // the word loops stay ROLLED (4 words per trip): unrolled, the two light passes and the two decode variants of one
-        // instantiation are ~25 KB of hot code, and a query with two aggregated fields runs two instantiations -- ncu r02l: the
-        // warps then wait for instructions 6.8 cycles per issue
+        // instantiation are ~25 KB of hot code, and a query with two aggregated fields runs two instantiations: the warps then
+        // stall on instruction fetch
         if (interior) {
             lastw = *reinterpret_cast<const uint32_t *>(src + kSwarLaneBytes - 4);
             uint32_t pw = __shfl_up_sync(0xffffffffu, lastw, 1);
@@ -2006,8 +2006,8 @@ __device__ __forceinline__ uint32_t grab_work(uint32_t *cursor, uint32_t nwork, 
 
 // The value type of aggregated field c must be the same in every block of the query (kErrTypeMix otherwise).  One global word
 // per field records it; `known` caches what this thread has already seen (4 bits per field), so the common case costs no
-// memory access at all -- a compare-and-swap per block on one hot address used to be a fifth of the kernel's stall samples
-// once the page decode got cheap (ncu r02b).  Returns false on a mismatch.
+// memory access at all -- a compare-and-swap per block on one hot address is a serialising round trip to L2 that shows once
+// the page decode is cheap.  Returns false on a mismatch.
 __device__ __forceinline__ bool check_col_type(const ScanParams &p, uint32_t c, uint8_t vt, uint32_t &known) {
     const uint32_t have = (known >> (4 * c)) & 0xfu;
     if (have == vt) return true;
@@ -2392,7 +2392,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kFastLane ? BYDB_FAST_CTAS 
 // Express lane: the all-rows SUM / MEAN / COUNT scan (BASELINE configs 3/4: group-by sum, no row predicate) without the
 // per-block latency chain.  With the SWAR decoder a 16 KB page costs ~5 k warp instructions, so the dependent loads in front
 // of every page (work cursor -> work list -> DevBlock -> DevCol -> page header -> first TMA stage) weighed as much as the
-// decode (ncu r02b: issue slots 46 % busy, long-scoreboard stalls 8 per issue).  Here a warp takes kExpressBatch blocks per
+// decode (the warps wait on long-scoreboard stalls instead of issuing).  Here a warp takes kExpressBatch blocks per
 // cursor increment; lane l resolves block l (directory entry, column lookup, page header) -- eight dependent chains overlap in
 // the lanes of one warp -- and then the warp streams the batch's pages through ONE continuous TMA ring: the first stages of
 // page k+1 are in flight while page k is being decoded.  Blocks that are not plain (cut by the time range, a page that is not

@@ -1,18 +1,19 @@
 #!/usr/bin/env python
 """Generates tests/golden/e2e_cases.json from the reference's own end-to-end measure cases
-(/root/reference/test/cases/measure/data/{input,want,testdata} + pkg/test/measure/testdata/measures): the data points
+(<reference>/test/cases/measure/data/{input,want,testdata} + pkg/test/measure/testdata/measures): the data points
 the integration suite writes, the query of each case and the rows it expects.  Only cases inside the hot path are
-taken (group-by + aggregation, optional Top / tag filter).  Run in the build container (the reference tree is not
-on the GPU box); the JSON it writes is the committed fixture.
+taken (group-by + aggregation, optional Top / tag filter).  Run it against a checkout of apache/skywalking-banyandb;
+the JSON it writes is the committed fixture, so the tests never need the reference tree.
 
-    python tests/golden/make_e2e_fixtures.py
+    python tests/golden/make_e2e_fixtures.py <path to a skywalking-banyandb checkout>
 """
 import json
 import os
+import sys
 
 import yaml
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "."
 DATA = os.path.join(REF, "test/cases/measure/data")
 SCHEMAS = os.path.join(REF, "pkg/test/measure/testdata/measures")
 # case -> data file written by test/cases/init.go:88,105 for that measure (group sw_metric)

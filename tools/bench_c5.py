@@ -124,12 +124,7 @@ def main():
                  "int64_bit_equal": bool(got.val_i64.tolist() == want.val_i64.tolist()),
                  "float_max_rel_err": float(np.max(np.abs(got.val_f64 - want.val_f64) / np.maximum(np.abs(want.val_f64), 1e-300))) if want.val_f64.size else 0.0}
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = B.HBM_PEAK_GBS
         ach = rows * b_alg / (scan_ms * 1e-3) / 1e9
         print(json.dumps({"metric": B.METRIC, "value": total * args.steps / dt, "unit": "datapoints/s", "n_gpus": world, "steps": args.steps,
                           "ms_per_step": dt / args.steps * 1e3, "scaling": "strong" if world > 1 else "n/a", "dtype": "i64+f64", "data": "synthetic",

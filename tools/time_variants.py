@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""time_variants.py -- times several builds of libbydbgpu.so (kernel experiments, scripts/build_variants.sh) in ONE
+"""time_variants.py -- times several builds of libbydbgpu.so (kernel experiments, `make variant` in skywalking-banyandb_b200/) in ONE
 process on one GPU: the synthetic part is generated once, every variant registers it, runs two queries of the bench
 shape and must return bit-identical results to the first library given.
 
