@@ -1,7 +1,7 @@
 // lane_decode.cuh -- the per-lane part of the fast varint decoders of scan_kernels.cu.
 //
 // Everything here is a plain function of one lane's registers (no shuffles, no shared memory), so the very same source is
-// also compiled for the host: tests/native/lane_decode_test.cc runs it against a byte-at-a-time reference decoder
+// also compiled for the host: tests/native/lane_decode_test.cc (and lane_switch_test.cc for swar_word2) runs it against a byte-at-a-time reference decoder
 // (full chunks, chunks with bytes outside the page, and the two-chain experiment) without a GPU.
 #pragma once
 
@@ -218,15 +218,17 @@ BYDB_LANE_FN uint32_t mulhi_u32(uint32_t a, uint32_t b) {  // IMAD.HI: a right s
 
 struct SwarLane {
     int32_t T0, T1, T2, R0, R1, R2;
-    uint32_t wide;     // msb set in some byte <=> a varint of 4 or more bytes was seen
+    uint32_t wide;     // msb set in some byte <=> swar_word: a varint of 4 or more bytes was seen; swar_word2: 3 or more
     int32_t nterm;     // 1 + terminators seen so far in this lane
     uint32_t prev_w;   // the word before the current one (the previous lane's last word for the first)
+    uint32_t prev_sb;  // prev_w * 128 (swar_word2 carries it instead of recomputing it)
 };
 BYDB_LANE_FN void swar_begin(SwarLane &s, uint32_t prev_w) {
     s.T0 = s.T1 = s.T2 = s.R0 = s.R1 = s.R2 = 0;
     s.wide = 0;
     s.nterm = 1;
     s.prev_w = prev_w;
+    s.prev_sb = imad_u32(prev_w, 128u, 0u);
 }
 // kMasked: first / last chunk of a page -- vm is 0xff for the bytes of the word that belong to the page; the others
 // neither terminate, nor carry payload, nor continue anything.
@@ -265,6 +267,40 @@ BYDB_LANE_FN void swar_word(SwarLane &s, uint32_t w_in, uint32_t vm) {
     s.R2 = dp4a_us(q2, wR, s.R2);
     s.wide |= q2;
     s.prev_w = w;
+}
+// Two-class word: swar_word for pages whose varints are at most 2 bytes long -- the common case of slowly varying metrics
+// (a zig-zag varint needs 3 bytes only for |delta| >= 8192).  Class 0 is unchanged; every byte after the first of a varint is
+// class 1, signed by S1.  M2, S2, S12, q2 and the class-2 dot products are gone, and psb is carried from the previous word.
+// The flag (s.wide) is a continuation byte in class-1 position: a varint of 3 or more bytes, for which this word is wrong.
+// Where the flag stays clear the result is exactly swar_word's: the class-0 bytes and the terminator ranks are the same in
+// both words, and a class-1 byte of a varint of at most 2 bytes has M2 = 0 (the byte two back is a terminator or lies
+// outside the page), so swar_word's p1 / S12 are this word's p1 / S1 and its q2 is 0.  The caller (swar_chunk_sum in
+// scan_kernels.cu) decodes a flagged chunk again with swar_word.
+template <bool kMasked>
+BYDB_LANE_FN void swar_word2(SwarLane &s, uint32_t w_in, uint32_t vm) {
+    const uint32_t w = kMasked ? (w_in & vm) : w_in;
+    const uint32_t p = w & 0x7f7f7f7fu;
+    const uint32_t M1 = lane_prmt(w, s.prev_w, 0xA98Fu);   // 0xff = not the first byte of a varint
+    const uint32_t sb = imad_u32(w, 128u, 0u);
+    const uint32_t S0 = lane_prmt(sb, 0u, 0xBA98u);
+    const uint32_t S1 = lane_prmt(sb, s.prev_sb, 0xA98Fu);
+    const uint32_t x0 = (p ^ S0) & ~M1;
+    const uint32_t p1 = p & M1;
+    const uint32_t wT = S1 | 0x01010101u;
+    uint32_t t01 = ~mulhi_u32(w, 1u << 25) & 0x01010101u;
+    if (kMasked) t01 &= vm;
+    const uint32_t base = imad_u32(static_cast<uint32_t>(s.nterm), 0x01010101u, 0u);
+    const uint32_t rinc = imad_u32(t01, 0x01010101u, base);
+    const uint32_t rank1 = imad_u32(t01, 0xffffffffu, rinc);
+    s.nterm = dp4a_su(0x01010101u, t01, s.nterm);
+    const uint32_t wR = imad_u32(S1 & 0x01010101u, 1u, rank1 ^ S1);
+    s.T0 = dp4a_su(x0, 0x01010101u, s.T0);
+    s.R0 = dp4a_su(x0, rank1, s.R0);
+    s.T1 = dp4a_us(p1, wT, s.T1);
+    s.R1 = dp4a_us(p1, wR, s.R1);
+    s.wide |= w & M1;
+    s.prev_w = w;
+    s.prev_sb = sb;
 }
 // -> number of terminators of the lane; T and R' as defined above
 BYDB_LANE_FN uint32_t swar_end(const SwarLane &s, int32_t &T, int32_t &Rp) {

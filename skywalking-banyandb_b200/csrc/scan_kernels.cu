@@ -703,6 +703,13 @@ struct SwarChunk {
 constexpr uint32_t kSwarLaneBytes = 64;
 constexpr uint32_t kSwarChunkBytes = 32 * kSwarLaneBytes;
 static_assert(kStageBytes % kSwarChunkBytes == 0, "a TMA stage holds whole SWAR chunks");
+// kClasses: 2 = swar_word2 (wide: a varint of 3+ bytes), 3 = swar_word (wide: a varint of 4+ bytes)
+template <int kClasses, bool kMasked>
+__device__ __forceinline__ void swar_step(SwarLane &sl, uint32_t w, uint32_t vm) {
+    if (kClasses == 2) swar_word2<kMasked>(sl, w, vm);
+    else swar_word<kMasked>(sl, w, vm);
+}
+template <int kClasses>
 __device__ __forceinline__ SwarChunk swar_chunk(const uint8_t *buf, uint32_t c, uint32_t pstart, uint32_t pend, uint32_t total, uint32_t &carry_w, int lane) {
     const uint32_t o = c * kSwarChunkBytes + lane * kSwarLaneBytes;
     const bool interior = c * kSwarChunkBytes >= pstart && (c + 1) * kSwarChunkBytes <= pend;  // warp-uniform
@@ -719,14 +726,14 @@ __device__ __forceinline__ SwarChunk swar_chunk(const uint8_t *buf, uint32_t c, 
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
             const uint4 wa = *reinterpret_cast<const uint4 *>(src + 32 * half), wb = *reinterpret_cast<const uint4 *>(src + 32 * half + 16);
-            swar_word<false>(sl, wa.x, 0u);
-            swar_word<false>(sl, wa.y, 0u);
-            swar_word<false>(sl, wa.z, 0u);
-            swar_word<false>(sl, wa.w, 0u);
-            swar_word<false>(sl, wb.x, 0u);
-            swar_word<false>(sl, wb.y, 0u);
-            swar_word<false>(sl, wb.z, 0u);
-            swar_word<false>(sl, wb.w, 0u);
+            swar_step<kClasses, false>(sl, wa.x, 0u);
+            swar_step<kClasses, false>(sl, wa.y, 0u);
+            swar_step<kClasses, false>(sl, wa.z, 0u);
+            swar_step<kClasses, false>(sl, wa.w, 0u);
+            swar_step<kClasses, false>(sl, wb.x, 0u);
+            swar_step<kClasses, false>(sl, wb.y, 0u);
+            swar_step<kClasses, false>(sl, wb.z, 0u);
+            swar_step<kClasses, false>(sl, wb.w, 0u);
         }
     } else {
         uint4 w[4];
@@ -749,10 +756,10 @@ __device__ __forceinline__ SwarChunk swar_chunk(const uint8_t *buf, uint32_t c, 
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             const uint32_t v = (q < 2 ? va : vb) >> (16 * (q & 1));
-            swar_word<true>(sl, w[q].x, expand4(v));
-            swar_word<true>(sl, w[q].y, expand4(v >> 4));
-            swar_word<true>(sl, w[q].z, expand4(v >> 8));
-            swar_word<true>(sl, w[q].w, expand4(v >> 12));
+            swar_step<kClasses, true>(sl, w[q].x, expand4(v));
+            swar_step<kClasses, true>(sl, w[q].y, expand4(v >> 4));
+            swar_step<kClasses, true>(sl, w[q].z, expand4(v >> 8));
+            swar_step<kClasses, true>(sl, w[q].w, expand4(v >> 12));
         }
     }
     SwarChunk r;
@@ -760,12 +767,29 @@ __device__ __forceinline__ SwarChunk swar_chunk(const uint8_t *buf, uint32_t c, 
     r.n = swar_end(sl, r.T, r.Rp);
     return r;
 }
+// One chunk of a page for the express lane's SWAR sum: a page starts on the two-class word (three = false).  A chunk whose vote
+// raises the two-class flag is decoded again, from the same stage and the same carry word, with the three-class word, which
+// then takes the rest of the page; there `wide` means a varint of 4+ bytes (the page bails out).  Exact: a varint of 3+ bytes
+// raises the flag in the chunk that holds its second byte, never later than the chunk of its third byte, so every chunk the
+// two-class word keeps has only bytes on which both words agree (lane_decode.cuh, swar_word2).  A page with a 3-byte varint
+// pays at most one extra chunk.  The stage is released only after its chunks, so the redone chunk's bytes are still staged.
+__device__ __forceinline__ SwarChunk swar_chunk_sum(const uint8_t *buf, uint32_t c, uint32_t pstart, uint32_t pend, uint32_t total, uint32_t &carry_w,
+                                                    bool &three, int lane) {
+    if (!three) {
+        const uint32_t cw = carry_w;
+        const SwarChunk ch = swar_chunk<2>(buf, c, pstart, pend, total, carry_w, lane);
+        if (!ch.wide) return ch;
+        three = true;
+        carry_w = cw;
+    }
+    return swar_chunk<3>(buf, c, pstart, pend, total, carry_w, lane);
+}
 
 // ------------------------------------------------------------------------------------------------
 // SWAR sum decoder: EncodeTypeDelta page, every row active, only SUM / MEAN / COUNT wanted (the group-by-sum shape of
 // BASELINE configs 3/4).  See lane_decode.cuh (swar_word): the page sum is a weighted sum over BYTES, so nothing is
-// carried from byte to byte or from lane to lane except the count of terminators; per 1 KB chunk the warp does one
-// shuffle of the neighbour's last word, 8 x swar_word per lane, one scan of the lanes' terminator counts and one
+// carried from byte to byte or from lane to lane except the count of terminators; per 2 KB chunk the warp does one
+// shuffle of the neighbour's last word, 16 x swar_word per lane, one scan of the lanes' terminator counts and one
 // 64-bit multiply-add.  Returns like delta_page_fast (0 done / 1 a varint of 4+ bytes was met / 2 corrupt).
 // ------------------------------------------------------------------------------------------------
 __device__ __noinline__ int delta_page_sum_all(WarpSmem *sm, int lane) {
@@ -793,7 +817,10 @@ __device__ __noinline__ int delta_page_sum_all(WarpSmem *sm, int lane) {
     for (uint32_t c = 0; c < nchunks; ++c) {
         const uint32_t k = c / kChunksPerStage;
         if ((c % kChunksPerStage) == 0) buf = stream_wait(st, sm, k);
-        const SwarChunk ch = swar_chunk(buf, c, st.pstart, st.pend, st.total, carry_w, lane);
+        // three-class word only: the two-class switch (swar_chunk_sum) adds a second copy of the chunk decode to this
+        // function, which changed the register allocation of the whole fast-lane kernel and made the masked scan of
+        // bench.py's C2 query 4 % slower on an H100 (3.52 against 3.38 ms); every-row pages seldom reach the fast lane
+        const SwarChunk ch = swar_chunk<3>(buf, c, st.pstart, st.pend, st.total, carry_w, lane);
         if (ch.wide) {
             // a varint of four or more bytes: the general decoder takes the page (same bail-out as delta_page_fast)
             stream_drain(st, sm, k);
@@ -2544,13 +2571,14 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_ex
                     const uint32_t nchunks = (tot_k + kSwarChunkBytes - 1) / kSwarChunkBytes;
                     int64_t S = 0;
                     uint32_t tb = 0, carry_w = 0, last_byte = 0;
+                    bool three = false;
                     for (uint32_t j = 0; j < nst_k; ++j) {
                         const uint32_t s = sb_k + j;
                         const uint8_t *buf = ring_wait(sm, seq0 + s);
                         const uint32_t c1 = min(nchunks, (j + 1) * kChunksPerStage);
                         for (uint32_t cc = j * kChunksPerStage; cc < c1; ++cc) {
                             if (good) {
-                                const SwarChunk ch = swar_chunk(buf, cc, ps_k, pe_k, tot_k, carry_w, lane);
+                                const SwarChunk ch = swar_chunk_sum(buf, cc, ps_k, pe_k, tot_k, carry_w, three, lane);
                                 if (ch.wide) {
                                     good = false;  // keep consuming the page's stages (the ring stays in step), stop decoding
                                 } else {
