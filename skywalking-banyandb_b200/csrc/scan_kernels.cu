@@ -1589,8 +1589,10 @@ __global__ void plan_blocks_kernel(const __grid_constant__ ScanParams p) {
         }
         int32_t qi = -1;
         if (lo < p.n_series && p.q_sids[lo] == sid) qi = static_cast<int32_t>(lo);
-        // part_iter.go:232-241: the block must overlap the inclusive time range
-        sel = qi >= 0 && !(b.ts_max < p.tmin || b.ts_min > p.tmax);
+        // part_iter.go:232-241: the block must overlap the inclusive time range.  An empty range (tmin > tmax) holds no row of
+        // any block, so it selects none: a block spanning it would otherwise reach series_reduce, whose overlap check then
+        // sees parts that the host-side overlap precheck (empty intersection with the range) never sent through dedup
+        sel = qi >= 0 && p.tmin <= p.tmax && !(b.ts_max < p.tmin || b.ts_min > p.tmax);
         p.block_qsid[g] = sel ? qi : -1;
         p.Prows[g] = 0;
         // head of this series' run of blocks inside the part: lets series_reduce skip its binary search
@@ -3504,7 +3506,7 @@ __global__ void __launch_bounds__(256) key_values_kernel(const __grid_constant__
             if (p.q_sids[mid] < blk.sid) lo = mid + 1;
             else hi = mid;
         }
-        if (!(lo < p.n_series && p.q_sids[lo] == blk.sid) || blk.ts_max < p.tmin || blk.ts_min > p.tmax) continue;
+        if (!(lo < p.n_series && p.q_sids[lo] == blk.sid) || p.tmin > p.tmax || blk.ts_max < p.tmin || blk.ts_min > p.tmax) continue;
         DevCol col;
         if (!find_col(part, blk, p.key_name, col, lane)) {
             if (lane == 0) key_insert(p, nullptr, 0, g);  // column absent in this block: every cell is nil (block.go:226-233)
