@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <chrono>
 #include <condition_variable>
+#include <cstddef>
 #include <cstdlib>
 #include <deque>
 #include <functional>
@@ -84,6 +85,23 @@ struct Part {
     }
 };
 
+// The zero page of a scan: zeroed on the device before plan_blocks, written by the kernels, and read back whole behind the
+// last kernel of the step (errors + counters).
+struct ZeroPage {
+    uint32_t work_count, work_next;   // work list cursor
+    uint32_t err[2];                  // DevErr (first error wins), block / series index
+    unsigned long long stats[6];      // see ScanParams::stats
+    int32_t col_type[kMaxFcols];
+    unsigned long long dd_counts[2];  // version dedup: flagged blocks, flagged rows
+    uint32_t slow_count, slow_next;   // slow-lane list cursor
+    uint32_t rest_count, rest_next;   // express lane only: cursor of the blocks it left to the regular fast lane
+};
+static_assert(offsetof(ZeroPage, err) == 8 && offsetof(ZeroPage, stats) == 16 && offsetof(ZeroPage, col_type) == 64 &&
+                  offsetof(ZeroPage, dd_counts) == 96 && offsetof(ZeroPage, slow_count) == 112 && offsetof(ZeroPage, rest_count) == 120,
+              "zero page layout");
+constexpr size_t kZeroPageBytes = 256;  // zeroed and read back per scan
+static_assert(sizeof(ZeroPage) <= kZeroPageBytes, "zero page size");
+
 // One in-flight call: stream, events and a pinned staging buffer.
 struct ExecSlot {
     cudaStream_t stream = nullptr;
@@ -91,7 +109,8 @@ struct ExecSlot {
     cudaEvent_t ev[4 * kMaxBatches] = {};
     uint8_t *pinned = nullptr;
     size_t pinned_bytes = 0;
-    uint8_t *zpage = nullptr;  // 256 B pinned: read-back of the per-query zero page (errors + counters)
+    uint8_t *zpage = nullptr;  // pinned, kZeroPageBytes per batch: read-back of the zero pages
+    ZeroPage *page(int batch) { return reinterpret_cast<ZeroPage *>(zpage + kZeroPageBytes * static_cast<size_t>(batch)); }
     bool express[kMaxBatches] = {};  // per batch: run_scan launched the express lane (its zero-page counter is meaningful)
     cudaEvent_t busy = nullptr;  // recorded by a call that returned before its work finished (asynchronous scan_partials)
     bool busy_pending = false;
@@ -124,7 +143,7 @@ struct ExecSlot {
         if (cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess) return -1;
         for (auto &e : ev)
             if (cudaEventCreate(&e) != cudaSuccess) return -1;
-        if (cudaMallocHost(reinterpret_cast<void **>(&zpage), 256 * kMaxBatches) != cudaSuccess) return -1;
+        if (cudaMallocHost(reinterpret_cast<void **>(&zpage), kZeroPageBytes * kMaxBatches) != cudaSuccess) return -1;
         if (cudaEventCreateWithFlags(&busy, cudaEventDisableTiming) != cudaSuccess) return -1;
         return ensure_pinned(kInitialPinned);
     }
@@ -350,24 +369,16 @@ void distinct_fields(const bydb_query *q, std::vector<std::string> &fcols, std::
     }
 }
 
-// partial-table layout for (G groups, F fields); see bydb_gpu.h
-struct TableLayout {
-    size_t G, F, GF;
-    size_t off_sum_f64, off_max_f64, off_negmin_f64, off_sum_i64, off_cnt, off_rows, off_max_i64, off_notmin_i64, off_coltype, total;
-    TableLayout(size_t g, size_t f) : G(g), F(f), GF(g * f) {
-        size_t o = 0;
-        off_sum_f64 = o; o += GF * 8;
-        off_max_f64 = o; o += GF * 8;
-        off_negmin_f64 = o; o += GF * 8;
-        off_sum_i64 = o; o += GF * 8;
-        off_cnt = o; o += GF * 8;
-        off_rows = o; o += G * 8;
-        off_max_i64 = o; o += GF * 8;
-        off_notmin_i64 = o; o += GF * 8;
-        off_coltype = o; o += F * 8;
-        total = o;
+// the caller's file list of one part, checked
+int file_images(const bydb_part_files *files, std::vector<FileImage> &imgs) {
+    if (!files || files->n_files == 0 || !files->files) return fail(BYDB_EINVAL, "no files");
+    for (uint32_t i = 0; i < files->n_files; ++i) {
+        const bydb_file &f = files->files[i];
+        if (!f.name || (!f.data && f.len)) return fail(BYDB_EINVAL, "file without name/data");
+        imgs.push_back(FileImage{f.name, f.data, f.len});
     }
-};
+    return 0;
+}
 
 // zero_copy: the data files stay in (pinned, device-mapped) host memory and the kernels read the
 // pages they need straight over PCIe; only the block directory is uploaded.
@@ -376,21 +387,15 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
                           size_t *dir_bytes_out);
 
 int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_files *files, std::shared_ptr<Part> &out, uint64_t *h2d,
-                              bool zero_copy = false, bool transient = false, size_t batch = 0, size_t n_batches = 1, bool unpack = false,
-                              PartDir *parsed = nullptr, bool device_index = false) {
-    if (!files || files->n_files == 0 || !files->files) return fail(BYDB_EINVAL, "no files");
+                              bool zero_copy = false, bool transient = false, bool unpack = false, PartDir *parsed = nullptr, bool device_index = false) {
     std::vector<FileImage> imgs;
-    for (uint32_t i = 0; i < files->n_files; ++i) {
-        const bydb_file &f = files->files[i];
-        if (!f.name || (!f.data && f.len)) return fail(BYDB_EINVAL, "file without name/data");
-        imgs.push_back(FileImage{f.name, f.data, f.len});
-    }
+    if (int rc = file_images(files, imgs)) return rc;
     auto part = std::make_shared<Part>();
     part->id = part_id;
     part->device = ctx->device;
     std::string err;
     // resident parts: the block index is inflated and parsed by kernels (index_kernels.cu); the host only decides the file table
-    const bool dev_index = device_index && !parsed && n_batches == 1 && !zero_copy;
+    const bool dev_index = device_index && !parsed && !zero_copy;
     std::vector<std::string> families;
     if (dev_index) {
         for (const auto &f : imgs)
@@ -402,7 +407,7 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
     } else if (parsed) {
         part->dir = std::move(*parsed);  // the caller parsed this slice of the block index already (cold path, in the background)
     } else {
-        int rc = build_part_dir(imgs, ctx->names, part->dir, err, batch, n_batches);
+        int rc = build_part_dir(imgs, ctx->names, part->dir, err);
         if (rc) return fail(rc, "part " + std::to_string(part_id) + ": " + err);
     }
     // arena: each data file 256 B aligned with >= 256 B of slack after it (TMA over-read, bit windows)
@@ -547,15 +552,16 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
 // the handful of interned column names to the context's ids.  Fills part.dir (host copy of the directory) and writes
 // DevBlock[] / DevCol[] straight into the part's device directory.
 // ------------------------------------------------------------------------------------------------
-struct DevTmp {
-    uint8_t *p = nullptr;
-    cudaStream_t s = nullptr;
-    ~DevTmp() {
-        if (p) cudaFreeAsync(p, s);
+// device memory from the stream-ordered pool, freed on its stream (behind the work that uses it) when this goes out of scope
+struct Scratch {
+    uint8_t *base = nullptr;
+    cudaStream_t stream = nullptr;
+    ~Scratch() {
+        if (base) cudaFreeAsync(base, stream);
     }
-    int alloc(size_t n, cudaStream_t st) {
-        s = st;
-        return cudaMallocAsync(reinterpret_cast<void **>(&p), n ? n : 256, st) == cudaSuccess ? 0 : -1;
+    cudaError_t alloc(size_t n, cudaStream_t s) {
+        stream = s;
+        return cudaMallocAsync(reinterpret_cast<void **>(&base), n ? n : 256, s);
     }
 };
 
@@ -609,79 +615,79 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
     up += kIndexMaxNames * sizeof(IndexName);
     const size_t off_map = up;
     up += align_up(kIndexMaxNames * sizeof(uint16_t), 256);
-    DevTmp in;
+    Scratch in;
     if (in.alloc(up, s)) return fail(BYDB_ENOMEM, "device allocation failed (index files)");
-    CUDA_TRY(cudaMemsetAsync(in.p + off_ctl, 0, 256 + kIndexMaxNames * sizeof(IndexName), s));
-    if (meta->len) CUDA_TRY(cudaMemcpyAsync(in.p, meta->data, meta->len, cudaMemcpyHostToDevice, s));
-    if (primary->len) CUDA_TRY(cudaMemcpyAsync(in.p + off_primary, primary->data, primary->len, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemsetAsync(in.base + off_ctl, 0, 256 + kIndexMaxNames * sizeof(IndexName), s));
+    if (meta->len) CUDA_TRY(cudaMemcpyAsync(in.base, meta->data, meta->len, cudaMemcpyHostToDevice, s));
+    if (primary->len) CUDA_TRY(cudaMemcpyAsync(in.base + off_primary, primary->data, primary->len, cudaMemcpyHostToDevice, s));
     std::vector<IndexFamily> fams(families.size());
     for (size_t i = 0; i < families.size(); ++i) {
-        if (tfm[i]->len) CUDA_TRY(cudaMemcpyAsync(in.p + off_tfm[i], tfm[i]->data, tfm[i]->len, cudaMemcpyHostToDevice, s));
-        CUDA_TRY(cudaMemcpyAsync(in.p + off_name[i], families[i].data(), families[i].size(), cudaMemcpyHostToDevice, s));
+        if (tfm[i]->len) CUDA_TRY(cudaMemcpyAsync(in.base + off_tfm[i], tfm[i]->data, tfm[i]->len, cudaMemcpyHostToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(in.base + off_name[i], families[i].data(), families[i].size(), cudaMemcpyHostToDevice, s));
         memset(&fams[i], 0, sizeof fams[i]);
-        fams[i].name = in.p + off_name[i];
+        fams[i].name = in.base + off_name[i];
         fams[i].name_len = static_cast<uint32_t>(families[i].size());
-        fams[i].tfm = in.p + off_tfm[i];
+        fams[i].tfm = in.base + off_tfm[i];
         fams[i].tfm_len = tfm[i]->len;
         fams[i].tf_len = tf[i]->len;
         fams[i].file_id = static_cast<uint8_t>(2 + i);
     }
-    if (!fams.empty()) CUDA_TRY(cudaMemcpyAsync(in.p + off_fams, fams.data(), fams.size() * sizeof(IndexFamily), cudaMemcpyHostToDevice, s));
+    if (!fams.empty()) CUDA_TRY(cudaMemcpyAsync(in.base + off_fams, fams.data(), fams.size() * sizeof(IndexFamily), cudaMemcpyHostToDevice, s));
     IndexCtl ctl0;
     memset(&ctl0, 0, sizeof ctl0);
     ctl0.min_ts = INT64_MAX;
     ctl0.max_ts = INT64_MIN;
-    CUDA_TRY(cudaMemcpyAsync(in.p + off_ctl, &ctl0, sizeof ctl0, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(in.base + off_ctl, &ctl0, sizeof ctl0, cudaMemcpyHostToDevice, s));
     IndexParams ip;
     memset(&ip, 0, sizeof ip);
-    ip.meta = in.p;
-    ip.primary = in.p + off_primary;
+    ip.meta = in.base;
+    ip.primary = in.base + off_primary;
     ip.meta_len = meta->len;
     ip.primary_len = primary->len;
     ip.ts_len = tsf->len;
     ip.fv_len = fvf->len;
     ip.n_families = static_cast<uint32_t>(families.size());
-    ip.families = reinterpret_cast<const IndexFamily *>(in.p + off_fams);
-    ip.ctl = reinterpret_cast<IndexCtl *>(in.p + off_ctl);
-    ip.names = reinterpret_cast<IndexName *>(in.p + off_names);
-    ip.name_map = reinterpret_cast<const uint16_t *>(in.p + off_map);
+    ip.families = reinterpret_cast<const IndexFamily *>(in.base + off_fams);
+    ip.ctl = reinterpret_cast<IndexCtl *>(in.base + off_ctl);
+    ip.names = reinterpret_cast<IndexName *>(in.base + off_names);
+    ip.name_map = reinterpret_cast<const uint16_t *>(in.base + off_map);
     IndexCtl ctl;
     auto read_ctl = [&]() -> int {
-        CUDA_TRY(cudaMemcpyAsync(&ctl, in.p + off_ctl, sizeof ctl, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(&ctl, in.base + off_ctl, sizeof ctl, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(cudaStreamSynchronize(s));
         if (ctl.err) return fail(BYDB_EINVAL, "part " + std::to_string(part.id) + ": " + index_err_text(ctl.err) + " (#" + std::to_string(ctl.err_where) + ")");
         return 0;
     };
     // ---- meta.bin: size, then inflate + the primary frames' sizes
-    DevTmp scratch0;
+    Scratch scratch0;
     if (scratch0.alloc(index_scratch_stride(), s)) return fail(BYDB_ENOMEM, "device allocation failed (index scratch)");
-    ip.scratch = scratch0.p;
+    ip.scratch = scratch0.base;
     launch_index_meta(ip, 0, s);
     int rc = read_ctl();
     if (rc) return rc;
     const size_t n_primary = static_cast<size_t>(ctl.meta_raw / 40);
-    DevTmp meta_raw, pbs;
+    Scratch meta_raw, pbs;
     if (meta_raw.alloc(ctl.meta_raw, s) || pbs.alloc(n_primary * sizeof(IndexPrimary), s)) return fail(BYDB_ENOMEM, "device allocation failed (index)");
-    CUDA_TRY(cudaMemsetAsync(pbs.p, 0, n_primary ? n_primary * sizeof(IndexPrimary) : 256, s));
-    ip.meta_raw = meta_raw.p;
+    CUDA_TRY(cudaMemsetAsync(pbs.base, 0, n_primary ? n_primary * sizeof(IndexPrimary) : 256, s));
+    ip.meta_raw = meta_raw.base;
     ip.meta_raw_cap = ctl.meta_raw;
-    ip.pb = reinterpret_cast<IndexPrimary *>(pbs.p);
+    ip.pb = reinterpret_cast<IndexPrimary *>(pbs.base);
     launch_index_meta(ip, 1, s);
     rc = read_ctl();
     if (rc) return rc;
     // ---- primary blocks: inflate, count
     ip.n_primary = static_cast<uint32_t>(n_primary);
-    DevTmp raw, scratch;
+    Scratch raw, scratch;
     if (raw.alloc(ctl.raw_total + 256, s) || scratch.alloc(std::max<size_t>(1, n_primary) * index_scratch_stride(), s))
         return fail(BYDB_ENOMEM, "device allocation failed (inflated index)");
-    ip.raw = raw.p;
-    ip.scratch = scratch.p;
+    ip.raw = raw.base;
+    ip.scratch = scratch.base;
     launch_index_inflate(ip, s);
     launch_index_walk(ip, false, s);
     std::vector<IndexPrimary> hpb(n_primary);
     std::vector<IndexName> hnames(kIndexMaxNames);
-    if (n_primary) CUDA_TRY(cudaMemcpyAsync(hpb.data(), pbs.p, n_primary * sizeof(IndexPrimary), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hnames.data(), in.p + off_names, kIndexMaxNames * sizeof(IndexName), cudaMemcpyDeviceToHost, s));
+    if (n_primary) CUDA_TRY(cudaMemcpyAsync(hpb.data(), pbs.base, n_primary * sizeof(IndexPrimary), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(hnames.data(), in.base + off_names, kIndexMaxNames * sizeof(IndexName), cudaMemcpyDeviceToHost, s));
     rc = read_ctl();
     if (rc) return rc;
     uint64_t nb = 0, nc = 0;
@@ -700,8 +706,8 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
         key.append(reinterpret_cast<const char *>(e.bytes), e.len);
         map[i] = ctx->names.intern(key);
     }
-    if (n_primary) CUDA_TRY(cudaMemcpyAsync(pbs.p, hpb.data(), n_primary * sizeof(IndexPrimary), cudaMemcpyHostToDevice, s));
-    CUDA_TRY(cudaMemcpyAsync(in.p + off_map, map.data(), kIndexMaxNames * sizeof(uint16_t), cudaMemcpyHostToDevice, s));
+    if (n_primary) CUDA_TRY(cudaMemcpyAsync(pbs.base, hpb.data(), n_primary * sizeof(IndexPrimary), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(in.base + off_map, map.data(), kIndexMaxNames * sizeof(uint16_t), cudaMemcpyHostToDevice, s));
     // ---- the part's device directory, filled by the second walk
     const size_t off_cols = align_up(nb * sizeof(DevBlock), 256);
     const size_t off_files = off_cols + align_up(nc * sizeof(DevCol), 256);
@@ -745,29 +751,22 @@ int unpack_fallback_pages(bydb_ctx *ctx, Part &part, size_t n_files, cudaStream_
     const size_t nb = part.dir.blocks.size(), nc = part.dir.cols.size();
     if (nb == 0 || nc == 0) return 0;
     if (n_files >= 255) return 0;
-    struct Tmp {
-        uint8_t *p = nullptr;
-        cudaStream_t s = nullptr;
-        ~Tmp() {
-            if (p) cudaFreeAsync(p, s);
-        }
-    } jobs, scratch;
-    jobs.s = scratch.s = s;
+    Scratch jobs, scratch;
     const size_t jobs_off = 256;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&jobs.p), jobs_off + nc * sizeof(UnpackJob), s));
-    CUDA_TRY(cudaMemsetAsync(jobs.p, 0, jobs_off, s));
+    CUDA_TRY(jobs.alloc(jobs_off + nc * sizeof(UnpackJob), s));
+    CUDA_TRY(cudaMemsetAsync(jobs.base, 0, jobs_off, s));
     UnpackParams up{};
     up.blocks = part.d_blocks;
     up.cols = const_cast<DevCol *>(part.d_cols);
     up.files = part.d_files;
     up.n_blocks = static_cast<uint32_t>(nb);
     up.arena_file_id = static_cast<uint32_t>(n_files);
-    up.counters = reinterpret_cast<unsigned long long *>(jobs.p);
-    up.jobs = reinterpret_cast<UnpackJob *>(jobs.p + jobs_off);
+    up.counters = reinterpret_cast<unsigned long long *>(jobs.base);
+    up.jobs = reinterpret_cast<UnpackJob *>(jobs.base + jobs_off);
     up.max_jobs = nc;
     launch_classify_pages(up, s);
     unsigned long long cnt[5] = {0, 0, 0, 0, 0};
-    CUDA_TRY(cudaMemcpyAsync(cnt, jobs.p, sizeof cnt, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(cnt, jobs.base, sizeof cnt, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     part.unpack_skipped = cnt[3];
     if (cnt[0] == 0) return 0;
@@ -783,30 +782,118 @@ int unpack_fallback_pages(bydb_ctx *ctx, Part &part, size_t n_files, cudaStream_
     if (e != cudaSuccess) return fail(BYDB_ENOMEM, "device allocation failed for the unpack arena");
     const int n_warps = static_cast<int>(std::min<unsigned long long>(cnt[0], 8ull * static_cast<unsigned long long>(ctx->sm_count)));
     const int n_warps4 = (n_warps + 3) / 4 * 4;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&scratch.p), static_cast<size_t>(n_warps4) * unpack_scratch_stride(), s));
+    CUDA_TRY(scratch.alloc(static_cast<size_t>(n_warps4) * unpack_scratch_stride(), s));
     // publish the arena as one more file of the part
     const uint8_t *ap = part.d_unpack;
     CUDA_TRY(cudaMemcpyAsync(const_cast<uint8_t **>(reinterpret_cast<const uint8_t *const *>(part.d_files)) + n_files, &ap, sizeof ap,
                              cudaMemcpyHostToDevice, s));
     up.n_jobs = cnt[0];
     up.arena = part.d_unpack;
-    up.scratch = scratch.p;
+    up.scratch = scratch.base;
     launch_unpack_pages(up, n_warps4, s);
-    CUDA_TRY(cudaMemcpyAsync(cnt, jobs.p, sizeof cnt, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(cnt, jobs.base, sizeof cnt, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     part.unpacked_pages = cnt[4];
     part.unpack_skipped = cnt[3];
     return 0;
 }
 
-struct Scratch {
-    uint8_t *base = nullptr;
-    size_t bytes = 0;
-    cudaStream_t stream = nullptr;
-    ~Scratch() {
-        if (base) cudaFreeAsync(base, stream);
-    }
+// staging of one step, in pinned memory and on the device alike: series ids | order (query-series indices sorted by
+// (group, series)) | group_start (where each group begins in order), back to back so that one copy takes all three
+struct StageLayout {
+    size_t NS, G, off_order, off_gstart, bytes, stride;
 };
+StageLayout stage_layout(size_t NS, size_t G) {
+    const size_t bytes = NS * 12 + (G + 1) * 4;
+    return StageLayout{NS, G, NS * 8, NS * 12, bytes, align_up(bytes, 256)};
+}
+
+void stage_series(const bydb_query *q, const StageLayout &st, uint8_t *h) {
+    int32_t *order = reinterpret_cast<int32_t *>(h + st.off_order), *gstart = reinterpret_cast<int32_t *>(h + st.off_gstart);
+    if (st.NS) memcpy(h, q->series_ids, st.NS * 8);
+    std::fill(gstart, gstart + st.G + 1, 0);
+    if (q->series_group) {
+        for (size_t i = 0; i < st.NS; ++i) gstart[static_cast<size_t>(q->series_group[i]) + 1]++;
+        for (size_t g = 0; g < st.G; ++g) gstart[g + 1] += gstart[g];
+        std::vector<int32_t> cur(gstart, gstart + st.G);
+        for (size_t i = 0; i < st.NS; ++i) order[cur[q->series_group[i]]++] = static_cast<int32_t>(i);
+    } else {
+        for (size_t i = 0; i < st.NS; ++i) order[i] = static_cast<int32_t>(i);
+        gstart[1] = static_cast<int32_t>(st.NS);
+    }
+}
+
+// device scratch of the finalisation and row selection; [o_out, o_out + out_bytes) is read back: selected-row count and the
+// table's status word (o_cnt) | is_float | the selected rows
+struct FinalLayout {
+    size_t o_vi, o_vf, o_keys, o_kst, o_out, o_cnt, o_isf, o_sg, o_sr, o_si, o_sf, out_bytes, total, cap, A;
+};
+FinalLayout final_layout(size_t G, size_t A, int32_t top_n) {
+    FinalLayout fl;
+    size_t o = 0;
+    auto carve = [&](size_t bytes) {
+        size_t at = o;
+        o = align_up(o + bytes, 256);
+        return at;
+    };
+    fl.cap = top_n > 0 ? std::min<size_t>(static_cast<size_t>(top_n), G) : G;
+    fl.A = A;
+    fl.o_vi = carve(G * A * 8);
+    fl.o_vf = carve(G * A * 8);
+    fl.o_keys = carve(G * 8);
+    fl.o_kst = carve(G);
+    fl.o_out = o;
+    fl.o_cnt = carve(16);
+    fl.o_isf = carve(A);
+    fl.o_sg = carve(fl.cap * 4);
+    fl.o_sr = carve(fl.cap * 8);
+    fl.o_si = carve(fl.cap * A * 8);
+    fl.o_sf = carve(fl.cap * A * 8);
+    fl.out_bytes = o - fl.o_out;
+    fl.total = o;
+    return fl;
+}
+
+// pinned bytes of a step over G series groups whose finalisation sees out_groups groups: run_scan's staging of each batch, then
+// the read-back of the results.  A prepared graph keeps the two apart (its results land at host_off = the staging's stride).
+size_t step_pinned_bytes(const bydb_query *q, size_t G, size_t out_groups, size_t batches = 1) {
+    return stage_layout(q->n_series, G).stride * batches + final_layout(out_groups, q->n_aggs, q->top_n).out_bytes;
+}
+
+// the partial-table pointers of ReduceParams / FinalizeParams (the names and order of TablePtrs)
+template <class P>
+void set_table(P &p, const TablePtrs &t) {
+    p.sum_f64 = t.sum_f64;
+    p.max_f64 = t.max_f64;
+    p.negmin_f64 = t.negmin_f64;
+    p.sum_i64 = t.sum_i64;
+    p.cnt = t.cnt;
+    p.rows = t.rows;
+    p.max_i64 = t.max_i64;
+    p.notmin_i64 = t.notmin_i64;
+    p.coltype = t.coltype;
+}
+
+// the parts of a query as the kernels see them: blocks numbered globally in part order
+void part_refs(const std::vector<std::shared_ptr<Part>> &parts, DevPartRef *out) {
+    uint32_t base = 0;
+    for (size_t i = 0; i < parts.size(); ++i) {
+        const Part &p = *parts[i];
+        out[i] = DevPartRef{p.d_blocks, p.d_cols, p.d_files, static_cast<uint32_t>(p.dir.blocks.size()), base};
+        base += out[i].n_blocks;
+    }
+}
+
+// two parts hold rows of one time span inside [tmin, tmax]: the scan then runs the version dedup, whose precheck synchronises
+bool parts_overlap(const std::vector<std::shared_ptr<Part>> &parts, int64_t tmin, int64_t tmax) {
+    for (size_t a = 0; a < parts.size(); ++a)
+        for (size_t b = a + 1; b < parts.size(); ++b) {
+            const PartDir &x = parts[a]->dir, &y = parts[b]->dir;
+            if (x.blocks.empty() || y.blocks.empty()) continue;
+            if (std::max(std::max(x.min_ts, y.min_ts), tmin) <= std::min(std::min(x.max_ts, y.max_ts), tmax)) return true;
+        }
+    return false;
+}
 
 // Runs plan -> scan -> series_reduce -> group_reduce on `stream`, leaving the partial table at
 // `d_table` (device).  Synchronises the stream.  Fills stats.
@@ -819,25 +906,19 @@ struct KeyedPass {
 };
 
 int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cudaStream_t stream, uint8_t *d_table, const TableLayout &tl,
-             bydb_stats *stats, int batch = 0, bool presized = false, const KeyedPass *kp = nullptr) {
+             bydb_stats *stats, int batch = 0, const KeyedPass *kp = nullptr) {
     cudaEvent_t *ev = slot.ev + 4 * batch;
-    uint8_t *zpage = slot.zpage + 256 * batch;
-    memset(zpage, 0, 256);  // a failure before the read-back is enqueued must not leave a previous call's status behind
+    ZeroPage *hz = slot.page(batch);
+    memset(hz, 0, kZeroPageBytes);  // a failure before the read-back is enqueued must not leave a previous call's status behind
     const size_t F = plan.fcols.size();
     const size_t NS = q->n_series;
     const size_t NB = plan.total_blocks;
     const int32_t G = plan.n_groups;
     // ---- host staging: sids | order | group_start
-    std::vector<int32_t> order(NS), gstart(static_cast<size_t>(G) + 1, 0);
-    if (q->series_group) {
-        for (size_t i = 0; i < NS; ++i) gstart[static_cast<size_t>(q->series_group[i]) + 1]++;
-        for (int32_t g = 0; g < G; ++g) gstart[g + 1] += gstart[g];
-        std::vector<int32_t> cur(gstart.begin(), gstart.end() - 1);
-        for (size_t i = 0; i < NS; ++i) order[cur[q->series_group[i]]++] = static_cast<int32_t>(i);
-    } else {
-        for (size_t i = 0; i < NS; ++i) order[i] = static_cast<int32_t>(i);
-        gstart[1] = static_cast<int32_t>(NS);
-    }
+    const StageLayout st = stage_layout(NS, static_cast<size_t>(G));
+    if (slot.ensure_pinned(st.stride * static_cast<size_t>(batch + 1))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    uint8_t *h = slot.pinned + st.stride * static_cast<size_t>(batch);
+    stage_series(q, st, h);
     // ---- device scratch layout
     size_t o = 0;
     auto carve = [&](size_t bytes) {
@@ -845,11 +926,8 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
         o = align_up(o + bytes, 256);
         return at;
     };
-    const size_t off_zero = carve(256);  // work_count, work_next, err[2], stats[4], col_type[F]
-    // sids | order | group_start sit back to back, exactly like in the pinned staging: one copy brings all three
-    const size_t off_sids = carve(NS * 12 + (static_cast<size_t>(G) + 1) * 4);
-    const size_t off_order = off_sids + NS * 8;
-    const size_t off_gstart = off_sids + NS * 12;
+    const size_t off_zero = carve(kZeroPageBytes);
+    const size_t off_sids = carve(st.bytes);  // the staging as it is: one copy brings sids, order and group_start
     const size_t off_worklist = carve(NB * 4);
     const size_t off_slowlist = carve(NB * 4);
     const size_t off_restlist = carve(NB * 4);
@@ -864,40 +942,20 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     const size_t off_first = carve(use_first ? n_first * 4 : 0);
     const size_t off_dd_index = carve(NB * 4), off_dd_rowoff = carve(NB * 8), off_dd_list = carve(NB * 4);
     Scratch sc;
-    sc.stream = stream;
-    sc.bytes = o;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&sc.base), o, stream));
+    CUDA_TRY(sc.alloc(o, stream));
     uint8_t *d = sc.base;
-    const size_t stage_bytes = NS * 8 + NS * 4 + (static_cast<size_t>(G) + 1) * 4;
-    const size_t stage_stride = align_up(stage_bytes + 256, 256);
-    if (!presized && slot.ensure_pinned(stage_stride * static_cast<size_t>(batch + 1))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    uint8_t *h = slot.pinned + stage_stride * static_cast<size_t>(batch);
-    if (NS) memcpy(h, q->series_ids, NS * 8);
-    if (NS) memcpy(h + NS * 8, order.data(), NS * 4);
-    memcpy(h + NS * 12, gstart.data(), (static_cast<size_t>(G) + 1) * 4);
-    CUDA_TRY(cudaMemsetAsync(d + off_zero, 0, 256, stream));
+    ZeroPage *z = reinterpret_cast<ZeroPage *>(d + off_zero);
+    CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
     if (use_first) CUDA_TRY(cudaMemsetAsync(d + off_first, 0xff, n_first * 4, stream));
-    CUDA_TRY(cudaMemcpyAsync(d + off_sids, h, stage_bytes, cudaMemcpyHostToDevice, stream));
-    if (stats) stats->h2d_bytes += stage_bytes;
+    CUDA_TRY(cudaMemcpyAsync(d + off_sids, h, st.bytes, cudaMemcpyHostToDevice, stream));
+    if (stats) stats->h2d_bytes += st.bytes;
 
-    // zero page: [0] work_count [1] work_next [2..3] err [4..11] stats (u64 x4) [16..] col_type
-    uint32_t *z32 = reinterpret_cast<uint32_t *>(d + off_zero);
     ScanParams sp;
     memset(&sp, 0, sizeof sp);
     ReduceParams rp;
     memset(&rp, 0, sizeof rp);
-    uint32_t base = 0;
-    for (size_t i = 0; i < plan.parts.size(); ++i) {
-        DevPartRef r;
-        r.blocks = plan.parts[i]->d_blocks;
-        r.cols = plan.parts[i]->d_cols;
-        r.files = plan.parts[i]->d_files;
-        r.n_blocks = static_cast<uint32_t>(plan.parts[i]->dir.blocks.size());
-        r.block_base = base;
-        base += r.n_blocks;
-        sp.parts[i] = r;
-        rp.parts[i] = r;
-    }
+    part_refs(plan.parts, sp.parts);
+    std::copy(sp.parts, sp.parts + plan.parts.size(), rp.parts);
     sp.n_parts = rp.n_parts = static_cast<uint32_t>(plan.parts.size());
     sp.total_blocks = static_cast<uint32_t>(NB);
     sp.q_sids = reinterpret_cast<const uint64_t *>(d + off_sids);
@@ -926,14 +984,14 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
         }
     }
     sp.worklist = reinterpret_cast<uint32_t *>(d + off_worklist);
-    sp.work_count = z32 + 0;
-    sp.work_next = z32 + 1;
+    sp.work_count = &z->work_count;
+    sp.work_next = &z->work_next;
     sp.slow_list = reinterpret_cast<uint32_t *>(d + off_slowlist);
-    sp.slow_count = z32 + 28;  // bytes 112..119 of the zero page
-    sp.slow_next = z32 + 29;
-    sp.err = z32 + 2;
-    sp.stats = reinterpret_cast<unsigned long long *>(d + off_zero + 16);
-    sp.col_type = reinterpret_cast<int32_t *>(d + off_zero + 64);
+    sp.slow_count = &z->slow_count;
+    sp.slow_next = &z->slow_next;
+    sp.err = z->err;
+    sp.stats = z->stats;
+    sp.col_type = z->col_type;
     sp.block_qsid = reinterpret_cast<int32_t *>(d + off_qsid);
     sp.first_block = use_first ? reinterpret_cast<uint32_t *>(d + off_first) : nullptr;
     sp.P = reinterpret_cast<BlockPartial *>(d + off_P);
@@ -944,8 +1002,8 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     rp.n_fcols = static_cast<uint32_t>(F);
     rp.n_groups = G;
     rp.q_sids = sp.q_sids;
-    rp.order = reinterpret_cast<const int32_t *>(d + off_order);
-    rp.group_start = reinterpret_cast<const int32_t *>(d + off_gstart);
+    rp.order = reinterpret_cast<const int32_t *>(d + off_sids + st.off_order);
+    rp.group_start = reinterpret_cast<const int32_t *>(d + off_sids + st.off_gstart);
     rp.block_qsid = sp.block_qsid;
     rp.first_block = sp.first_block;
     rp.P = sp.P;
@@ -954,57 +1012,37 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     rp.S = reinterpret_cast<BlockPartial *>(d + off_S);
     rp.Srows = reinterpret_cast<int64_t *>(d + off_Srows);
     rp.err = sp.err;
-    rp.sum_f64 = reinterpret_cast<double *>(d_table + tl.off_sum_f64);
-    rp.max_f64 = reinterpret_cast<double *>(d_table + tl.off_max_f64);
-    rp.negmin_f64 = reinterpret_cast<double *>(d_table + tl.off_negmin_f64);
-    rp.sum_i64 = reinterpret_cast<int64_t *>(d_table + tl.off_sum_i64);
-    rp.cnt = reinterpret_cast<int64_t *>(d_table + tl.off_cnt);
-    rp.rows = reinterpret_cast<int64_t *>(d_table + tl.off_rows);
-    rp.max_i64 = reinterpret_cast<int64_t *>(d_table + tl.off_max_i64);
-    rp.notmin_i64 = reinterpret_cast<int64_t *>(d_table + tl.off_notmin_i64);
-    rp.coltype = reinterpret_cast<int64_t *>(d_table + tl.off_coltype);
+    TablePtrs table = tl.at(d_table, kp ? kp->group_off : 0);
     if (kp) {
-        const size_t go = kp->group_off, gf = kp->group_off * F;
-        rp.sum_f64 += gf, rp.max_f64 += gf, rp.negmin_f64 += gf;
-        rp.sum_i64 += gf, rp.cnt += gf, rp.max_i64 += gf, rp.notmin_i64 += gf;
-        rp.rows += go;
-        rp.coltype = kp->coltype;
+        table.coltype = kp->coltype;
         rp.Pfirst = sp.Pfirst;
         rp.Kts = kp->kts;
         rp.Krow = kp->krow;
     }
+    set_table(rp, table);
 
     CUDA_TRY(cudaEventRecord(ev[0], stream));
     launch_plan_blocks(sp, stream);
     // ---- version dedup: only when two parts of the query overlap in time at all (host-side precheck on
     //      the part directories); then the device finds the series that really overlap
     Scratch dd_scratch;
-    dd_scratch.stream = stream;
     uint32_t extra_launches = 0;
-    bool parts_overlap = false;
-    for (size_t a = 0; a < plan.parts.size() && !parts_overlap; ++a)
-        for (size_t b = a + 1; b < plan.parts.size() && !parts_overlap; ++b) {
-            const PartDir &x = plan.parts[a]->dir, &y = plan.parts[b]->dir;
-            if (x.blocks.empty() || y.blocks.empty()) continue;
-            const int64_t lo = std::max(std::max(x.min_ts, y.min_ts), q->tmin), hi = std::min(std::min(x.max_ts, y.max_ts), q->tmax);
-            parts_overlap = lo <= hi;
-        }
-    if (parts_overlap && NB > 0 && NS > 0) {
+    const bool overlap = parts_overlap(plan.parts, q->tmin, q->tmax);
+    if (overlap && NB > 0 && NS > 0) {
         sp.dd_index = reinterpret_cast<int32_t *>(d + off_dd_index);
         sp.dd_row_off = reinterpret_cast<unsigned long long *>(d + off_dd_rowoff);
         sp.dd_list = reinterpret_cast<uint32_t *>(d + off_dd_list);
-        sp.dd_counts = reinterpret_cast<unsigned long long *>(d + off_zero + 96);
+        sp.dd_counts = z->dd_counts;
         CUDA_TRY(cudaMemsetAsync(sp.dd_index, 0xff, NB * 4, stream));
         launch_detect_overlap(sp, stream);
-        CUDA_TRY(cudaMemcpyAsync(zpage + 128, d + off_zero + 96, 16, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaMemcpyAsync(hz->dd_counts, z->dd_counts, sizeof hz->dd_counts, cudaMemcpyDeviceToHost, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
-        const unsigned long long n_ddb = reinterpret_cast<unsigned long long *>(zpage + 128)[0];
-        const unsigned long long n_ddr = reinterpret_cast<unsigned long long *>(zpage + 128)[1];
+        const unsigned long long n_ddb = hz->dd_counts[0], n_ddr = hz->dd_counts[1];
         extra_launches += 1;
-        if (stats) stats->d2h_bytes += 16;
+        if (stats) stats->d2h_bytes += sizeof hz->dd_counts;
         if (n_ddb > 0) {
             const size_t b_ts = align_up(n_ddr * 8, 256), b_sh = align_up(n_ddb * kMaskWords * 4, 256);
-            CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&dd_scratch.base), 2 * b_ts + b_sh, stream));
+            CUDA_TRY(dd_scratch.alloc(2 * b_ts + b_sh, stream));
             sp.dd_ts = reinterpret_cast<int64_t *>(dd_scratch.base);
             sp.dd_ver = reinterpret_cast<int64_t *>(dd_scratch.base + b_ts);
             sp.dd_shadow = reinterpret_cast<uint32_t *>(dd_scratch.base + 2 * b_ts);
@@ -1017,14 +1055,13 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     {
         // express lane (scan_sum_express_kernel): all-rows SUM / MEAN / COUNT without row predicates or version dedup -- the
         // group-by-sum shape; every block it cannot take (time-range cut, non-delta page, ...) goes on to the regular lane
-        bool sums_only = q->n_preds == 0 && !parts_overlap && NB > 0;
+        bool sums_only = q->n_preds == 0 && !overlap && NB > 0;
         for (size_t c = 0; c < F; ++c) sums_only = sums_only && (sp.fcol_need[c] & 2) == 0;
-        static const bool no_express = getenv("BYDB_NO_EXPRESS") != nullptr;  // A/B timing of the two lanes
-        slot.express[batch] = sums_only && !no_express;
-        if (sums_only && !no_express) {
+        slot.express[batch] = sums_only;
+        if (sums_only) {
             sp.rest_list = reinterpret_cast<uint32_t *>(d + off_restlist);
-            sp.rest_count = z32 + 30;  // bytes 120..127 of the zero page
-            sp.rest_next = z32 + 31;
+            sp.rest_count = &z->rest_count;
+            sp.rest_next = &z->rest_next;
             if (stats) stats->kernel_launches += 1;
         }
     }
@@ -1032,88 +1069,70 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     launch_scan_blocks(sp, ctx->sm_count * ctx->ctas_per_sm_fast, ctx->sm_count * ctx->ctas_per_sm, stream);
     CUDA_TRY(cudaEventRecord(ev[2], stream));
     launch_series_reduce(rp, stream);
+    const int32_t *gstart = reinterpret_cast<const int32_t *>(h + st.off_gstart);
     bool small_groups = true;  // every group has at most 32 series: the warp-per-group reduce (bit-identical sums)
     for (int32_t g = 0; g < G && small_groups; ++g) small_groups = gstart[g + 1] - gstart[g] <= 32;
     launch_group_reduce(rp, stream, small_groups);
     CUDA_TRY(cudaEventRecord(ev[3], stream));
     // read back the zero page (errors + counters); the caller synchronises and then calls collect_scan
-    CUDA_TRY(cudaMemcpyAsync(zpage, d + off_zero, 256, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(hz, z, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
     if (stats) {
         stats->kernel_launches += (NB ? 1u : 0u) + 2u + (NS ? 1u : 0u) + 1u + extra_launches;
-        stats->d2h_bytes += 256;
+        stats->d2h_bytes += kZeroPageBytes;
     }
     // the scratch must outlive the kernels: it is freed stream-ordered (after them) when `sc` goes out of scope
     return 0;
 }
 
-// blocks the express lane finished, from a read-back zero page: it takes the whole work list (word 0) and hands on what it
-// cannot finish (word 30).  Word 30 is only written when the express kernel ran, so the caller says whether it did.
-uint32_t express_blocks(const uint8_t *zpage, bool launched) {
-    const uint32_t *hz = reinterpret_cast<const uint32_t *>(zpage);
-    return launched ? hz[0] - hz[30] : 0u;
+// a read-back zero page: its counters into `stats` (when given) and its device error as the result.  `express`: the step
+// launched the express lane, which takes the whole work list and hands on to the regular lane what it cannot finish.
+int read_zero_page(const ZeroPage &z, bool express, bydb_stats *stats) {
+    if (stats) {
+        stats->rows_scanned += z.stats[0];
+        stats->rows_matched += z.stats[1];
+        stats->page_bytes += z.stats[2];
+        stats->blocks_scanned += z.stats[3];
+        stats->blocks_slow_lane += static_cast<uint32_t>(z.stats[4]);
+        stats->slow_lane_reasons |= static_cast<uint32_t>(z.stats[5]);
+        stats->blocks_express_lane += express ? z.work_count - z.rest_count : 0u;
+    }
+    if (z.err[0] == 0) return 0;
+    g_last_dev_err = z.err[0];  // reset by the API entry points; a later clean slice must not hide it
+    char buf[96];
+    snprintf(buf, sizeof buf, " (block/series #%u)", z.err[1]);
+    return fail(dev_err_code(z.err[0]), std::string(dev_err_text(z.err[0])) + buf);
 }
 
 // after the stream is synchronised: device errors + counters of the scan
 int collect_scan(ExecSlot &slot, bydb_stats *stats, int batch = 0) {
-    cudaEvent_t *ev = slot.ev + 4 * batch;
-    const uint32_t *hz = reinterpret_cast<const uint32_t *>(slot.zpage + 256 * batch);
     if (stats) {
-        const unsigned long long *hs = reinterpret_cast<const unsigned long long *>(slot.zpage + 256 * batch + 16);
-        stats->rows_scanned += hs[0];
-        stats->rows_matched += hs[1];
-        stats->page_bytes += hs[2];
-        stats->blocks_scanned += hs[3];
-        stats->blocks_slow_lane += static_cast<uint32_t>(hs[4]);
-        stats->slow_lane_reasons |= static_cast<uint32_t>(hs[5]);
-        stats->blocks_express_lane += express_blocks(slot.zpage + 256 * batch, slot.express[batch]);
+        cudaEvent_t *ev = slot.ev + 4 * batch;
         float ms = 0;
         cudaEventElapsedTime(&ms, ev[1], ev[2]);
         stats->scan_kernel_ms += ms;
         cudaEventElapsedTime(&ms, ev[0], ev[3]);
         stats->device_ms += ms;
     }
-    if (hz[2] != 0) g_last_dev_err = hz[2];  // reset by the API entry points; a later clean slice must not hide it
-    if (hz[2] != 0) {
-        char buf[96];
-        snprintf(buf, sizeof buf, " (block/series #%u)", hz[3]);
-        return fail(dev_err_code(hz[2]), std::string(dev_err_text(hz[2])) + buf);
-    }
-    return 0;
+    return read_zero_page(*slot.page(batch), slot.express[batch], stats);
 }
 
-struct FinalLayout {
-    size_t o_out = 0, o_cnt = 0, o_isf = 0, o_sg = 0, o_sr = 0, o_si = 0, o_sf = 0, out_bytes = 0, cap = 0, A = 0;
-    uint32_t launches = 0;
-};
+// the status a partial table carries in its coltype words (DevErr, 0 = none): tables of bydb_scan_partials and the peers'
+// mailbox slots, possibly another rank's
+int table_status(uint32_t e) {
+    if (e == 0) return 0;
+    g_last_dev_err = e;
+    return fail(dev_err_code(e), std::string(dev_err_text(e)) + " (status carried in a partial table)");
+}
 
-// finalize_to_host up to (and including) the read-back copy, without the synchronisation and the parsing; the result
-// lands at slot.pinned + host_off so that the staging area of run_scan (at the start of slot.pinned) stays intact
+// finalisation + row selection of the table at d_table, up to and including the read-back copy to slot.pinned + host_off;
+// fl = final_layout() of the query, launches = kernels launched
 int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t stream, const uint8_t *d_table, const TableLayout &tl,
-                     size_t host_off, FinalLayout &fl, Scratch &sc) {
+                     size_t host_off, Scratch &sc, FinalLayout &fl, uint32_t &launches) {
     const size_t F = plan.fcols.size();
     const int32_t G = plan.n_groups;
     const size_t A = q->n_aggs;
-    const size_t cap = q->top_n > 0 ? std::min<size_t>(static_cast<size_t>(q->top_n), static_cast<size_t>(G)) : static_cast<size_t>(G);
-    size_t o = 0;
-    auto carve = [&](size_t bytes) {
-        size_t at = o;
-        o = align_up(o + bytes, 256);
-        return at;
-    };
-    const size_t o_vi = carve(static_cast<size_t>(G) * A * 8), o_vf = carve(static_cast<size_t>(G) * A * 8), o_keys = carve(static_cast<size_t>(G) * 8),
-                 o_kst = carve(static_cast<size_t>(G));
-    fl.o_out = o;
-    fl.o_cnt = carve(16);
-    fl.o_isf = carve(A);
-    fl.o_sg = carve(cap * 4);
-    fl.o_sr = carve(cap * 8);
-    fl.o_si = carve(cap * A * 8);
-    fl.o_sf = carve(cap * A * 8);
-    fl.out_bytes = o - fl.o_out;
-    fl.cap = cap;
-    fl.A = A;
-    sc.stream = stream;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&sc.base), o, stream));
+    fl = final_layout(static_cast<size_t>(G), A, q->top_n);
+    CUDA_TRY(sc.alloc(fl.total, stream));
     uint8_t *d = sc.base;
     FinalizeParams fp;
     memset(&fp, 0, sizeof fp);
@@ -1125,17 +1144,9 @@ int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
         fp.agg_fcol[a] = plan.agg_fcol[a];
         fp.agg_func[a] = q->aggs[a].func;
     }
-    fp.sum_f64 = reinterpret_cast<const double *>(d_table + tl.off_sum_f64);
-    fp.max_f64 = reinterpret_cast<const double *>(d_table + tl.off_max_f64);
-    fp.negmin_f64 = reinterpret_cast<const double *>(d_table + tl.off_negmin_f64);
-    fp.sum_i64 = reinterpret_cast<const int64_t *>(d_table + tl.off_sum_i64);
-    fp.cnt = reinterpret_cast<const int64_t *>(d_table + tl.off_cnt);
-    fp.rows = reinterpret_cast<const int64_t *>(d_table + tl.off_rows);
-    fp.max_i64 = reinterpret_cast<const int64_t *>(d_table + tl.off_max_i64);
-    fp.notmin_i64 = reinterpret_cast<const int64_t *>(d_table + tl.off_notmin_i64);
-    fp.coltype = reinterpret_cast<const int64_t *>(d_table + tl.off_coltype);
-    fp.out_i64 = reinterpret_cast<int64_t *>(d + o_vi);
-    fp.out_f64 = reinterpret_cast<double *>(d + o_vf);
+    set_table(fp, tl.at(const_cast<uint8_t *>(d_table)));  // read only
+    fp.out_i64 = reinterpret_cast<int64_t *>(d + fl.o_vi);
+    fp.out_f64 = reinterpret_cast<double *>(d + fl.o_vf);
     fp.out_is_float = d + fl.o_isf;
     fp.err_out = reinterpret_cast<uint32_t *>(d + fl.o_cnt + 8);
     SelectParams sp;
@@ -1153,20 +1164,26 @@ int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
     sp.val_i64 = fp.out_i64;
     sp.val_f64 = fp.out_f64;
     sp.is_float = fp.out_is_float;
-    sp.keys = reinterpret_cast<uint64_t *>(d + o_keys);
-    sp.kstate = d + o_kst;
+    sp.keys = reinterpret_cast<uint64_t *>(d + fl.o_keys);
+    sp.kstate = d + fl.o_kst;
     sp.sel_count = reinterpret_cast<uint32_t *>(d + fl.o_cnt);
     sp.sel_group = reinterpret_cast<int32_t *>(d + fl.o_sg);
     sp.sel_rows = reinterpret_cast<int64_t *>(d + fl.o_sr);
     sp.sel_i64 = reinterpret_cast<int64_t *>(d + fl.o_si);
     sp.sel_f64 = reinterpret_cast<double *>(d + fl.o_sf);
-    fl.launches = launch_finalize_select(fp, sp, stream);
+    launches = launch_finalize_select(fp, sp, stream);
     if (slot.ensure_pinned(host_off + fl.out_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     CUDA_TRY(cudaMemcpyAsync(slot.pinned + host_off, d + fl.o_out, fl.out_bytes, cudaMemcpyDeviceToHost, stream));
     return 0;
 }
 
-void finalize_parse(const uint8_t *h, const FinalLayout &fl, bydb_result *out) {
+// the read-back at h into *out; carried_status: the table came from bydb_scan_partials or a mailbox slot, so the status it
+// carries is the outcome
+int finalize_parse(const uint8_t *h, const FinalLayout &fl, bool carried_status, bydb_result *out) {
+    if (carried_status) {
+        const int rc = table_status(*reinterpret_cast<const uint32_t *>(h + (fl.o_cnt - fl.o_out) + 8));
+        if (rc) return rc;
+    }
     const size_t A = fl.A;
     const size_t R = std::min<size_t>(*reinterpret_cast<const uint32_t *>(h + (fl.o_cnt - fl.o_out)), fl.cap);
     auto owner = new ResultOwner();
@@ -1187,31 +1204,24 @@ void finalize_parse(const uint8_t *h, const FinalLayout &fl, bydb_result *out) {
     out->val_i64 = owner->val_i64.data();
     out->val_f64 = owner->val_f64.data();
     out->owner = owner;
+    return 0;
 }
 
 
 // finalisation + row selection + read-back of the result rows, synchronised and parsed
-int finalize_to_host(bydb_ctx *ctx, const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t stream, const uint8_t *d_table,
-                     const TableLayout &tl, bydb_result *out, bool check_inband_status = false) {
-    (void)ctx;
+int finalize_to_host(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t stream, const uint8_t *d_table, const TableLayout &tl,
+                     bydb_result *out, bool carried_status = false) {
     FinalLayout fl;
+    uint32_t launches = 0;
     Scratch sc;
-    int rc = finalize_enqueue(q, plan, slot, stream, d_table, tl, 0, fl, sc);
+    int rc = finalize_enqueue(q, plan, slot, stream, d_table, tl, 0, sc, fl, launches);
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(stream));
     CUDA_TRY(cudaGetLastError());
     out->stats.d2h_bytes += fl.out_bytes;
-    out->stats.kernel_launches += fl.launches;
-    if (check_inband_status) {
-        // the table came from bydb_scan_partials / a peer's mailbox slot (possibly another rank's): its status is in the table
-        const uint32_t e = *reinterpret_cast<const uint32_t *>(slot.pinned + (fl.o_cnt - fl.o_out) + 8);
-        g_last_dev_err = e;
-        if (e != 0) return fail(dev_err_code(e), std::string(dev_err_text(e)) + " (status carried in a partial table)");
-    }
-    finalize_parse(slot.pinned, fl, out);
-    return 0;
+    out->stats.kernel_launches += launches;
+    return finalize_parse(slot.pinned, fl, carried_status, out);
 }
-
 int make_plan(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::shared_ptr<Part>> *given, Plan &plan) {
     if (given) {
         plan.parts = *given;
@@ -1244,18 +1254,14 @@ int scan_agg_impl(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::sha
     ExecSlot &slot = *lease.slot;
     TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
     Scratch table;
-    table.stream = slot.stream;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&table.base), tl.total, slot.stream));
+    CUDA_TRY(table.alloc(tl.total, slot.stream));
     memset(&out->stats, 0, sizeof out->stats);
     out->stats.h2d_bytes = h2d_pre;
-    {
-        // size the pinned staging once: it must not be reallocated while copies from/to it are in flight
-        const size_t G = static_cast<size_t>(plan.n_groups), A = q->n_aggs, NS = q->n_series;
-        if (slot.ensure_pinned(NS * 12 + (G + 1) * 4 + G * (12 + 16 * A) + 16 * A + 8192)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    }
+    // size the pinned staging once: it must not be reallocated while copies from/to it are in flight
+    if (slot.ensure_pinned(step_pinned_bytes(q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     rc = run_scan(ctx, q, plan, slot, slot.stream, table.base, tl, &out->stats);
     // finalisation is enqueued behind the scan; one synchronisation covers both
-    if (!rc) rc = finalize_to_host(ctx, q, plan, slot, slot.stream, table.base, tl, out);
+    if (!rc) rc = finalize_to_host(q, plan, slot, slot.stream, table.base, tl, out);
     if (rc) {
         // a failure after something was enqueued: the slot (and, on the host path, the transient parts the kernels read)
         // go back to their pools when this returns, so nothing may still be in flight
@@ -1337,37 +1343,49 @@ void prepared_destroy(bydb_prepared *p) {
     delete p;
 }
 
+// A graph reads its parts through the device pointers captured with it, so it may only replay while every handle still names
+// the very part object it captured (`held`).  Otherwise the graph is dropped, to be captured again; returns false when a handle
+// names no part any more (a released part makes the call fail like the plain path would).
+bool check_held_parts(bydb_ctx *ctx, const std::vector<bydb_part_h> &parts, cudaGraphExec_t &exec, std::vector<std::shared_ptr<Part>> &held) {
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    bool same = held.size() == parts.size(), missing = false;
+    for (size_t i = 0; i < parts.size(); ++i) {
+        auto it = ctx->parts.find(parts[i]);
+        if (it == ctx->parts.end()) missing = true;
+        else if (same && it->second != held[i]) same = false;
+    }
+    if (missing || !same) {
+        cudaGraphExecDestroy(exec);
+        exec = nullptr;
+        held.clear();
+    }
+    return !missing;
+}
+
 // captures one step into p->exec; returns 0, or a code after leaving the stream out of capture mode
 int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
     Plan plan;
     int rc = make_plan(ctx, &p->q, nullptr, plan);
     if (rc) return rc;
     // the version-dedup precheck of run_scan synchronises: parts that overlap in time keep the uncaptured path
-    for (size_t a = 0; a < plan.parts.size(); ++a)
-        for (size_t b = a + 1; b < plan.parts.size(); ++b) {
-            const PartDir &x = plan.parts[a]->dir, &y = plan.parts[b]->dir;
-            if (x.blocks.empty() || y.blocks.empty()) continue;
-            if (std::max(std::max(x.min_ts, y.min_ts), p->q.tmin) <= std::min(std::min(x.max_ts, y.max_ts), p->q.tmax)) {
-                p->capturable = false;
-                return 0;
-            }
-        }
+    if (parts_overlap(plan.parts, p->q.tmin, p->q.tmax)) {
+        p->capturable = false;
+        return 0;
+    }
     ExecSlot &slot = *p->slot;
     TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
-    const size_t G = static_cast<size_t>(plan.n_groups), A = p->q.n_aggs, NS = p->q.n_series;
-    const size_t stage = align_up(NS * 12 + (G + 1) * 4 + 512, 256);
-    p->host_off = stage;  // results land behind the staging area, which must survive from replay to replay
-    if (slot.ensure_pinned(stage + G * (12 + 16 * A) + 16 * A + 16384)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    p->host_off = stage_layout(p->q.n_series, tl.G).stride;  // results land behind the staging area, which must survive from replay to replay
+    if (slot.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     memset(&p->captured, 0, sizeof p->captured);
     cudaError_t e = cudaStreamBeginCapture(slot.stream, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) return fail(BYDB_EIO, std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(e));
+    uint32_t fin_launches = 0;
     {
         Scratch table, fin;
-        table.stream = slot.stream;
-        rc = cudaMallocAsync(reinterpret_cast<void **>(&table.base), tl.total, slot.stream) == cudaSuccess ? 0 : fail(BYDB_ENOMEM, "cudaMallocAsync (capture)");
-        if (!rc) rc = run_scan(ctx, &p->q, plan, slot, slot.stream, table.base, tl, &p->captured, 0, true);
+        rc = table.alloc(tl.total, slot.stream) == cudaSuccess ? 0 : fail(BYDB_ENOMEM, "cudaMallocAsync (capture)");
+        if (!rc) rc = run_scan(ctx, &p->q, plan, slot, slot.stream, table.base, tl, &p->captured);
         p->express = slot.express[0];
-        if (!rc) rc = finalize_enqueue(&p->q, plan, slot, slot.stream, table.base, tl, p->host_off, p->fl, fin);
+        if (!rc) rc = finalize_enqueue(&p->q, plan, slot, slot.stream, table.base, tl, p->host_off, fin, p->fl, fin_launches);
         // table / fin are released here: inside the capture, i.e. as free nodes of the graph
     }
     cudaGraph_t graph = nullptr;
@@ -1385,7 +1403,7 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
         p->exec = nullptr;
         p->capturable = false;
     }
-    p->captured.kernel_launches += p->fl.launches;  // finalize + select_rows (one fused launch for few groups)
+    p->captured.kernel_launches += fin_launches;  // finalize + select_rows (one fused launch for few groups)
     p->captured.d2h_bytes += p->fl.out_bytes;
     p->held = plan.parts;
     return 0;
@@ -1499,7 +1517,7 @@ int bydb_part_register(bydb_ctx *ctx, uint64_t part_id, const bydb_part_files *f
     }
     CUDA_TRY(cudaSetDevice(ctx->device));
     std::shared_ptr<Part> part;
-    int rc = register_part_locked_free(ctx, part_id, files, part, nullptr, false, false, 0, 1, true, nullptr, !ctx->host_index);
+    int rc = register_part_locked_free(ctx, part_id, files, part, nullptr, false, false, true, nullptr, !ctx->host_index);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     auto again = ctx->by_id.find(part_id);
@@ -1633,13 +1651,8 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     Plan plan;
     rc = make_plan(ctx, q, nullptr, plan);
     if (rc) return rc;
-    for (size_t a = 0; a < plan.parts.size(); ++a)
-        for (size_t b = a + 1; b < plan.parts.size(); ++b) {
-            const PartDir &x = plan.parts[a]->dir, &y = plan.parts[b]->dir;
-            if (x.blocks.empty() || y.blocks.empty()) continue;
-            if (std::max(std::max(x.min_ts, y.min_ts), q->tmin) <= std::min(std::min(x.max_ts, y.max_ts), q->tmax))
-                return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
-        }
+    if (parts_overlap(plan.parts, q->tmin, q->tmax))
+        return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
     CUDA_TRY(cudaSetDevice(ctx->device));
     SlotLease lease(ctx);
     if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
@@ -1659,8 +1672,7 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
                  a_lens = carve(static_cast<size_t>(cap) * 4);
     const size_t a_total = o;
     Scratch ka;
-    ka.stream = stream;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&ka.base), a_total, stream));
+    CUDA_TRY(ka.alloc(a_total, stream));
     const size_t back_bytes = a_total - a_ctl;  // ctl | vals | lens come back in one copy
     if (slot.ensure_pinned(std::max(back_bytes, NS * 8) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     if (NS) memcpy(slot.pinned, q->series_ids, NS * 8);
@@ -1668,19 +1680,7 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     CUDA_TRY(cudaMemsetAsync(ka.base + a_slots, 0, a_total - a_slots, stream));
     KeyParams kpar;
     memset(&kpar, 0, sizeof kpar);
-    {
-        uint32_t base = 0;
-        for (size_t i = 0; i < plan.parts.size(); ++i) {
-            DevPartRef r;
-            r.blocks = plan.parts[i]->d_blocks;
-            r.cols = plan.parts[i]->d_cols;
-            r.files = plan.parts[i]->d_files;
-            r.n_blocks = static_cast<uint32_t>(plan.parts[i]->dir.blocks.size());
-            r.block_base = base;
-            base += r.n_blocks;
-            kpar.parts[i] = r;
-        }
-    }
+    part_refs(plan.parts, kpar.parts);
     kpar.n_parts = static_cast<uint32_t>(plan.parts.size());
     kpar.total_blocks = static_cast<uint32_t>(NB);
     kpar.q_sids = reinterpret_cast<const uint64_t *>(ka.base + a_sids);
@@ -1749,14 +1749,10 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     const size_t b_src = carve(tlc.total), b_dst = carve(tlc.total), b_ct = carve(V * F * 8), b_kts = carve(V * NS * 8), b_krow = carve(V * NS * 4),
                  b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16);
     Scratch kb;
-    kb.stream = stream;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&kb.base), o, stream));
+    CUDA_TRY(kb.alloc(o, stream));
     CUDA_TRY(cudaMemsetAsync(kb.base + b_ct, 0, V * F * 8, stream));
     CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
-    {
-        const size_t A = q->n_aggs;
-        if (slot.ensure_pinned(NS * 12 + (G + 1) * 4 + GP * (12 + 16 * A) + 16 * A + 8192)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    }
+    if (slot.ensure_pinned(step_pinned_bytes(q, G, GP))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     std::vector<bydb_pred> preds(q->preds, q->preds + q->n_preds);
     preds.emplace_back();
     bydb_query qv = *q;
@@ -1776,7 +1772,7 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
         pass.coltype = reinterpret_cast<int64_t *>(kb.base + b_ct) + v * F;
         pass.kts = reinterpret_cast<int64_t *>(kb.base + b_kts) + v * NS;
         pass.krow = reinterpret_cast<uint32_t *>(kb.base + b_krow) + v * NS;
-        rc = run_scan(ctx, &qv, plan, slot, stream, kb.base + b_src, tlc, &out->base.stats, 0, true, &pass);
+        rc = run_scan(ctx, &qv, plan, slot, stream, kb.base + b_src, tlc, &out->base.stats, 0, &pass);
         cudaError_t ce = cudaStreamSynchronize(stream);  // also on failure: nothing may be in flight when the slot goes back
         if (!rc && ce != cudaSuccess) rc = fail(BYDB_EIO, cudaGetErrorString(ce));
         if (!rc) rc = collect_scan(slot, &out->base.stats);
@@ -1789,26 +1785,14 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     ko.n_groups = static_cast<int32_t>(G);
     ko.n_values = static_cast<uint32_t>(V);
     ko.n_series = static_cast<uint32_t>(NS);
-    // order | group_start of the series groups: rebuilt here (run_scan's copies live in its own scratch)
-    std::vector<int32_t> order(NS), gstart(G + 1, 0);
-    if (q->series_group) {
-        for (size_t i = 0; i < NS; ++i) gstart[static_cast<size_t>(q->series_group[i]) + 1]++;
-        for (size_t g = 0; g < G; ++g) gstart[g + 1] += gstart[g];
-        std::vector<int32_t> cur(gstart.begin(), gstart.end() - 1);
-        for (size_t i = 0; i < NS; ++i) order[cur[q->series_group[i]]++] = static_cast<int32_t>(i);
-    } else {
-        for (size_t i = 0; i < NS; ++i) order[i] = static_cast<int32_t>(i);
-        gstart[1] = static_cast<int32_t>(NS);
-    }
+    // order | group_start of the series groups: staged again (run_scan's copies live in its own scratch)
+    const StageLayout st = stage_layout(NS, G);
     Scratch kc;
-    kc.stream = stream;
-    const size_t c_order = 0, c_gstart = align_up(NS * 4, 256);
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&kc.base), c_gstart + (G + 1) * 4, stream));
-    if (NS) memcpy(slot.pinned, order.data(), NS * 4);
-    memcpy(slot.pinned + c_gstart, gstart.data(), (G + 1) * 4);
-    CUDA_TRY(cudaMemcpyAsync(kc.base, slot.pinned, c_gstart + (G + 1) * 4, cudaMemcpyHostToDevice, stream));
-    ko.order = reinterpret_cast<const int32_t *>(kc.base + c_order);
-    ko.group_start = reinterpret_cast<const int32_t *>(kc.base + c_gstart);
+    CUDA_TRY(kc.alloc(st.bytes, stream));
+    stage_series(q, st, slot.pinned);
+    CUDA_TRY(cudaMemcpyAsync(kc.base, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream));
+    ko.order = reinterpret_cast<const int32_t *>(kc.base + st.off_order);
+    ko.group_start = reinterpret_cast<const int32_t *>(kc.base + st.off_gstart);
     ko.Kts = reinterpret_cast<const int64_t *>(kb.base + b_kts);
     ko.Krow = reinterpret_cast<const uint32_t *>(kb.base + b_krow);
     ko.slot = reinterpret_cast<int32_t *>(kb.base + b_slot);
@@ -1816,26 +1800,13 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     ko.perm = reinterpret_cast<int32_t *>(kb.base + b_perm);
     ko.n_present = reinterpret_cast<uint32_t *>(kb.base + b_np);
     launch_key_order(ko, stream);
-    auto table_ptrs = [&](uint8_t *t) {
-        TablePtrs tp;
-        tp.sum_f64 = reinterpret_cast<double *>(t + tlc.off_sum_f64);
-        tp.max_f64 = reinterpret_cast<double *>(t + tlc.off_max_f64);
-        tp.negmin_f64 = reinterpret_cast<double *>(t + tlc.off_negmin_f64);
-        tp.sum_i64 = reinterpret_cast<int64_t *>(t + tlc.off_sum_i64);
-        tp.cnt = reinterpret_cast<int64_t *>(t + tlc.off_cnt);
-        tp.rows = reinterpret_cast<int64_t *>(t + tlc.off_rows);
-        tp.max_i64 = reinterpret_cast<int64_t *>(t + tlc.off_max_i64);
-        tp.notmin_i64 = reinterpret_cast<int64_t *>(t + tlc.off_notmin_i64);
-        tp.coltype = reinterpret_cast<int64_t *>(t + tlc.off_coltype);
-        return tp;
-    };
-    launch_permute_table(table_ptrs(kb.base + b_dst), table_ptrs(kb.base + b_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F),
+    launch_permute_table(tlc.at(kb.base + b_dst), tlc.at(kb.base + b_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F),
                          reinterpret_cast<const int64_t *>(kb.base + b_ct), static_cast<uint32_t>(V), stream);
     CUDA_TRY(cudaStreamSynchronize(stream));  // the staging above is reused by the finalisation's read-back
     out->base.stats.kernel_launches += 3;
     Plan planc = plan;
     planc.n_groups = static_cast<int32_t>(GP);
-    rc = finalize_to_host(ctx, q, planc, slot, stream, kb.base + b_dst, tlc, &out->base, true);
+    rc = finalize_to_host(q, planc, slot, stream, kb.base + b_dst, tlc, &out->base, true);
     if (rc) {
         cudaStreamSynchronize(stream);
         return rc;
@@ -1921,8 +1892,7 @@ int bydb_encode_pages(bydb_ctx *ctx, const bydb_encode_input *in, bydb_encoded_p
     const size_t d_vals = carve(NV * 8), d_boff = carve((NB + 1) * 8), d_soff = carve((NB + 1) * 8), d_scr = carve(is_float ? NV * 8 : 0),
                  d_exp = carve(is_float ? NV * 2 : 0), d_len = carve(NB * 4), d_st = carve(NB), d_ooff = carve((NB + 1) * 8), d_slots = carve(slot_off[NB]);
     Scratch sc;
-    sc.stream = stream;
-    if (cudaMallocAsync(reinterpret_cast<void **>(&sc.base), o, stream) != cudaSuccess) {
+    if (sc.alloc(o, stream) != cudaSuccess) {
         cudaGetLastError();
         return fail(BYDB_ENOMEM, "bydb_encode_pages: device allocation failed");
     }
@@ -1960,8 +1930,7 @@ int bydb_encode_pages(bydb_ctx *ctx, const bydb_encode_input *in, bydb_encoded_p
     owner->bytes.assign(std::max<size_t>(total, 1), 0);
     out->bytes = owner->bytes.data();
     Scratch compact;
-    compact.stream = stream;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&compact.base), std::max<size_t>(total, 256), stream));
+    CUDA_TRY(compact.alloc(std::max<size_t>(total, 256), stream));
     CUDA_TRY(cudaMemcpyAsync(d + d_ooff, owner->page_off.data(), (NB + 1) * 8, cudaMemcpyHostToDevice, stream));
     CUDA_TRY(cudaEventRecord(ev2, stream));
     launch_gather_pages(ep, reinterpret_cast<const uint64_t *>(d + d_ooff), compact.base, grid, stream);
@@ -2136,11 +2105,7 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
     base.n_series = q->n_series;
     TableLayout tl(static_cast<size_t>(base.n_groups), base.fcols.size());
     std::vector<FileImage> imgs;
-    for (uint32_t i = 0; i < files->n_files; ++i) {
-        const bydb_file &f = files->files[i];
-        if (!f.name || (!f.data && f.len)) return fail(BYDB_EINVAL, "file without name/data");
-        imgs.push_back(FileImage{f.name, f.data, f.len});
-    }
+    if (int frc = file_images(files, imgs)) return frc;
     size_t n_primary = 0;
     {
         std::string err;
@@ -2148,13 +2113,8 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
         if (rc0) return fail(rc0, err);
     }
     Scratch tables;
-    tables.stream = slot.stream;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&tables.base), tl.total * K, slot.stream));
-    {
-        const size_t G = static_cast<size_t>(base.n_groups), A = q->n_aggs, NS = q->n_series;
-        const size_t stage_stride = align_up(NS * 12 + (G + 1) * 4 + 256, 256);
-        if (slot.ensure_pinned(std::max(stage_stride * K, G * (12 + 16 * A) + 16 * A + 8192))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    }
+    CUDA_TRY(tables.alloc(tl.total * K, slot.stream));
+    if (slot.ensure_pinned(step_pinned_bytes(q, tl.G, tl.G, K))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     memset(&out->stats, 0, sizeof out->stats);
     // The block index is parsed in the background from the start, one task per group of primary blocks (they are
     // independent zstd frames).  The main thread takes the pieces in order: whatever is parsed by the time the GPU can
@@ -2253,7 +2213,7 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
             h2d = gi->bytes;
             gathered.push_back(gi);                  // the directory vectors feed the staged copies: keep them until the end
         } else {
-            rc = register_part_locked_free(ctx, ~0ull - static_cast<uint64_t>(k), files, p, &h2d, true, true, 0, 1, false, &merged);
+            rc = register_part_locked_free(ctx, ~0ull - static_cast<uint64_t>(k), files, p, &h2d, true, true, false, &merged);
             if (rc) continue;
             keep.push_back(p);
         }
@@ -2261,17 +2221,15 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
         Plan plan = base;
         plan.parts = {p};
         plan.total_blocks = static_cast<uint32_t>(p->dir.blocks.size());
-        rc = run_scan(ctx, q, plan, slot, slot.stream, tables.base + tl.total * static_cast<size_t>(k), tl, &out->stats, k, true);
+        rc = run_scan(ctx, q, plan, slot, slot.stream, tables.base + tl.total * static_cast<size_t>(k), tl, &out->stats, k);
         if (trace) fprintf(stderr, "[bydb cold] slice %d enqueued at %.0f us\n", k, since());
     }
     while (next < T) (void)parses[next++].get();
     if (!rc && n_slices > 0) {
-        launch_combine_tables(reinterpret_cast<uint64_t *>(tables.base), static_cast<uint32_t>(n_slices), tl.total / 8, tl.off_sum_f64 / 8,
-                              tl.off_max_f64 / 8, tl.off_max_f64 / 8, tl.off_sum_i64 / 8, tl.off_sum_i64 / 8, tl.off_max_i64 / 8, tl.off_max_i64 / 8,
-                              tl.total / 8, slot.stream);
+        launch_combine_tables(tables.base, static_cast<uint32_t>(n_slices), tl, slot.stream);
         out->stats.kernel_launches += 1;
         // the pinned staging of the last slices may still be in flight: finalize copies into it only after the kernels
-        rc = finalize_to_host(ctx, q, base, slot, slot.stream, tables.base, tl, out);
+        rc = finalize_to_host(q, base, slot, slot.stream, tables.base, tl, out);
         if (rc) cudaStreamSynchronize(slot.stream);  // nothing of this call may be in flight when the slot and the parts go back
         if (trace) fprintf(stderr, "[bydb cold] finalized at %.0f us\n", since());
     } else {
@@ -2319,7 +2277,7 @@ int bydb_scan_agg_host(bydb_ctx *ctx, uint32_t n_parts, const bydb_part_files *p
         memset(out, 0, sizeof *out);
         for (uint32_t i = 0; i < n_parts; ++i) {
             std::shared_ptr<Part> p;
-            rc = register_part_locked_free(ctx, ~0ull - i, &parts[i], p, &h2d, (q->flags & BYDB_Q_HOST_ZERO_COPY) != 0, true, 0, 1, attempt == 1);
+            rc = register_part_locked_free(ctx, ~0ull - i, &parts[i], p, &h2d, (q->flags & BYDB_Q_HOST_ZERO_COPY) != 0, true, attempt == 1);
             if (rc) break;
             tmp.push_back(p);
         }
@@ -2408,9 +2366,7 @@ int bydb_partials_combine(bydb_ctx *ctx, const bydb_query *q, void *d_tables, ui
     TableLayout tl(static_cast<size_t>(q->series_group ? q->n_groups : 1), fcols.size());
     if (bytes_each != tl.total) return fail(BYDB_EINVAL, "partial tables must be exactly bydb_partials_layout().total_bytes each");
     CUDA_TRY(cudaSetDevice(ctx->device));
-    launch_combine_tables(static_cast<uint64_t *>(d_tables), n_tables, tl.total / 8, tl.off_sum_f64 / 8, tl.off_max_f64 / 8, tl.off_max_f64 / 8,
-                          tl.off_sum_i64 / 8, tl.off_sum_i64 / 8, tl.off_max_i64 / 8, tl.off_max_i64 / 8, tl.total / 8,
-                          static_cast<cudaStream_t>(stream));
+    launch_combine_tables(static_cast<uint8_t *>(d_tables), n_tables, tl, static_cast<cudaStream_t>(stream));
     CUDA_TRY(cudaGetLastError());
     return 0;
     });
@@ -2431,7 +2387,7 @@ int bydb_reduce_finalize(bydb_ctx *ctx, const bydb_query *q, const void *d_parti
     SlotLease lease(ctx);
     if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
     cudaStream_t s = static_cast<cudaStream_t>(stream);  // NULL = the legacy default stream, like every partial-table call
-    return finalize_to_host(ctx, q, plan, *lease.slot, s, static_cast<const uint8_t *>(d_partials), tl, out, true);
+    return finalize_to_host(q, plan, *lease.slot, s, static_cast<const uint8_t *>(d_partials), tl, out, true);
     });
 }
 
@@ -2476,8 +2432,8 @@ int bydb_query_prepare(bydb_ctx *ctx, const bydb_query *q, bydb_prepared **out) 
     bool ok = p->slot->create() == 0;  // with its pinned staging: nothing page-locked is allocated inside an execution
     if (ok) {
         // sized for this query now (see ExecSlot::ensure_pinned: a page-locked allocation inside a collective can stall the peers)
-        const size_t G = q->series_group ? static_cast<size_t>(q->n_groups) : 1, A = q->n_aggs, NS = q->n_series;
-        ok = p->slot->ensure_pinned(NS * 12 + (G + 1) * 4 + G * (12 + 16 * A) + 16 * A + 16384) == 0;
+        const size_t G = q->series_group ? static_cast<size_t>(q->n_groups) : 1;
+        ok = p->slot->ensure_pinned(step_pinned_bytes(q, G, G)) == 0;
     }
     ok = ok && cudaEventCreate(&p->t0) == cudaSuccess && cudaEventCreate(&p->t1) == cudaSuccess;
     if (!ok) {
@@ -2510,25 +2466,7 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
         if (rc) return rc;
         if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
     }
-    {
-        // the graph reads the parts through the device pointers captured with it: every handle must still name the very
-        // part object that was captured (a released part makes the call fail like bydb_scan_agg would, a re-registered one
-        // drops the graph and captures again)
-        std::lock_guard<std::mutex> lk2(ctx->mu);
-        bool same = p->held.size() == p->parts.size();
-        bool missing = false;
-        for (size_t i = 0; i < p->parts.size(); ++i) {
-            auto it = ctx->parts.find(p->parts[i]);
-            if (it == ctx->parts.end()) missing = true;
-            else if (same && it->second != p->held[i]) same = false;
-        }
-        if (missing || !same) {
-            cudaGraphExecDestroy(p->exec);
-            p->exec = nullptr;
-            p->held.clear();
-            if (missing) return fail(BYDB_ENOENT, "unknown part handle");
-        }
-    }
+    if (!check_held_parts(ctx, p->parts, p->exec, p->held)) return fail(BYDB_ENOENT, "unknown part handle");
     if (!p->exec) {
         const int rc = prepared_capture(ctx, p);
         if (rc) return rc;
@@ -2540,28 +2478,14 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
     CUDA_TRY(cudaEventRecord(p->t1, slot.stream));
     CUDA_TRY(cudaStreamSynchronize(slot.stream));
     CUDA_TRY(cudaGetLastError());
-    out->stats = p->captured;
-    const uint32_t *hz = reinterpret_cast<const uint32_t *>(slot.zpage);
-    const unsigned long long *hs = reinterpret_cast<const unsigned long long *>(slot.zpage + 16);
-    out->stats.rows_scanned = hs[0];
-    out->stats.rows_matched = hs[1];
-    out->stats.page_bytes = hs[2];
-    out->stats.blocks_scanned = hs[3];
-    out->stats.blocks_slow_lane = static_cast<uint32_t>(hs[4]);
-    out->stats.slow_lane_reasons = static_cast<uint32_t>(hs[5]);
-    out->stats.blocks_express_lane = express_blocks(slot.zpage, p->express);
+    out->stats = p->captured;  // host-side counters; the zero-page counters are still 0 there
     float ms = 0;
     cudaEventElapsedTime(&ms, p->t0, p->t1);
     out->stats.device_ms = ms;
     out->stats.scan_kernel_ms = 0;  // per-kernel events are not available inside a graph replay
-    if (hz[2] != 0) {
-        g_last_dev_err = hz[2];
-        char buf[96];
-        snprintf(buf, sizeof buf, " (block/series #%u)", hz[3]);
-        return fail(dev_err_code(hz[2]), std::string(dev_err_text(hz[2])) + buf);
-    }
-    finalize_parse(slot.pinned + p->host_off, p->fl, out);
-    return 0;
+    const int rc = read_zero_page(*slot.page(0), p->express, &out->stats);
+    if (rc) return rc;
+    return finalize_parse(slot.pinned + p->host_off, p->fl, false, out);
     });
 }
 
@@ -2590,32 +2514,29 @@ int bydb_partials_rows(bydb_ctx *ctx, const bydb_query *q, const void *d_partial
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaMemcpyAsync(h.data(), d_partials, tl.total, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
-    const double *sum_f = reinterpret_cast<const double *>(h.data() + tl.off_sum_f64), *max_f = reinterpret_cast<const double *>(h.data() + tl.off_max_f64),
-                 *negmin_f = reinterpret_cast<const double *>(h.data() + tl.off_negmin_f64);
-    const int64_t *sum_i = reinterpret_cast<const int64_t *>(h.data() + tl.off_sum_i64), *cnt = reinterpret_cast<const int64_t *>(h.data() + tl.off_cnt),
-                  *rows = reinterpret_cast<const int64_t *>(h.data() + tl.off_rows), *max_i = reinterpret_cast<const int64_t *>(h.data() + tl.off_max_i64),
-                  *notmin_i = reinterpret_cast<const int64_t *>(h.data() + tl.off_notmin_i64), *coltype = reinterpret_cast<const int64_t *>(h.data() + tl.off_coltype);
+    const TablePtrs t = tl.at(h.data());
     uint32_t dev_err = 0;
-    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(coltype[c] >> 8));
-    if (dev_err) return fail(dev_err_code(dev_err), std::string(dev_err_text(dev_err)) + " (status carried in a partial table)");
+    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(t.coltype[c] >> 8));
+    rc = table_status(dev_err);
+    if (rc) return rc;
     auto owner = std::make_unique<PartialRowsOwner>();
     owner->is_float.resize(A);
-    for (size_t a = 0; a < A; ++a) owner->is_float[a] = (coltype[agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
+    for (size_t a = 0; a < A; ++a) owner->is_float[a] = (t.coltype[agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
     for (size_t g = 0; g < G; ++g) {
-        if (rows[g] <= 0) continue;  // the group never appeared on this node
+        if (t.rows[g] <= 0) continue;  // the group never appeared on this node
         owner->group_id.push_back(static_cast<int32_t>(g));
         for (size_t a = 0; a < A; ++a) {
             const size_t o = g * F + static_cast<size_t>(agg_fcol[a]);
             const bool isf = owner->is_float[a] != 0;
-            const int64_t n = cnt[o];
+            const int64_t n = t.cnt[o];
             int64_t vi = 0, ci = 0;
             double vf = 0.0, cf = 0.0;
             switch (q->aggs[a].func) {
-                case BYDB_AGG_SUM: vi = sum_i[o]; vf = sum_f[o]; break;
+                case BYDB_AGG_SUM: vi = t.sum_i64[o]; vf = t.sum_f64[o]; break;
                 case BYDB_AGG_COUNT: vi = n; vf = static_cast<double>(n); break;
-                case BYDB_AGG_MAX: vi = n > 0 ? max_i[o] : INT64_MIN; vf = n > 0 ? max_f[o] : -1.7976931348623157e308; break;
-                case BYDB_AGG_MIN: vi = n > 0 ? ~notmin_i[o] : INT64_MAX; vf = n > 0 ? -negmin_f[o] : 1.7976931348623157e308; break;
-                case BYDB_AGG_MEAN: vi = sum_i[o]; vf = sum_f[o]; ci = n; cf = static_cast<double>(n); break;
+                case BYDB_AGG_MAX: vi = n > 0 ? t.max_i64[o] : INT64_MIN; vf = n > 0 ? t.max_f64[o] : -1.7976931348623157e308; break;
+                case BYDB_AGG_MIN: vi = n > 0 ? ~t.notmin_i64[o] : INT64_MAX; vf = n > 0 ? -t.negmin_f64[o] : 1.7976931348623157e308; break;
+                case BYDB_AGG_MEAN: vi = t.sum_i64[o]; vf = t.sum_f64[o]; ci = n; cf = static_cast<double>(n); break;
             }
             owner->val_i64.push_back(isf ? 0 : vi);
             owner->val_f64.push_back(isf ? vf : 0.0);
@@ -2820,10 +2741,7 @@ static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vecto
     if (!rc) rc = make_plan(ctx, q, given, plan);
     TableLayout tl(static_cast<size_t>(rc ? 1 : plan.n_groups), rc ? 1 : plan.fcols.size());
     if (!rc && tl.total > slot) rc = fail(BYDB_EINVAL, "partial table larger than the mailbox slots (bydb_comm_export max_table_bytes)");
-    if (!rc) {
-        const size_t G = static_cast<size_t>(plan.n_groups), A = q->n_aggs, NS = q->n_series;
-        if (es.ensure_pinned(NS * 12 + (G + 1) * 4 + G * (12 + 16 * A) + 16 * A + 8192)) rc = fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    }
+    if (!rc && es.ensure_pinned(step_pinned_bytes(q, tl.G, tl.G))) rc = fail(BYDB_ENOMEM, "cudaMallocHost failed");
     memset(&out->stats, 0, sizeof out->stats);
     out->stats.h2d_bytes = h2d_pre;
     // the slots' previous use -- the last collective with THIS root and parity, the same epoch on every rank -- must have been
@@ -2853,11 +2771,9 @@ static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vecto
             launch_comm_wait(flags, static_cast<uint32_t>(cm.nranks), epoch, my_err, kErrPeerTimeout, s);
         }
         if (!rc) {
-            launch_combine_tables(reinterpret_cast<uint64_t *>(slots0), static_cast<uint32_t>(cm.nranks), tl.total / 8, tl.off_sum_f64 / 8, tl.off_max_f64 / 8,
-                                  tl.off_max_f64 / 8, tl.off_sum_i64 / 8, tl.off_sum_i64 / 8, tl.off_max_i64 / 8, tl.off_max_i64 / 8, tl.total / 8, s,
-                                  slot / 8);
+            launch_combine_tables(slots0, static_cast<uint32_t>(cm.nranks), tl, s, slot);
             out->stats.kernel_launches += 3;
-            frc = finalize_to_host(ctx, q, plan, es, s, slots0, tl, out, true);  // synchronises
+            frc = finalize_to_host(q, plan, es, s, slots0, tl, out, true);  // synchronises
             finalized = frc == 0;
         }
         cudaStreamSynchronize(s);
@@ -2927,28 +2843,15 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
     CommArgs *d_args = reinterpret_cast<CommArgs *>(cm.mine + kCommArgsOff);
     ExecSlot &es = *p->slot;
     // pinned words of this prepared query that the graph's memcpy nodes read / write: the last two zero pages of its slot
-    CommArgs *h_args = reinterpret_cast<CommArgs *>(es.zpage + 256 * 7);
-    uint8_t *h_back = es.zpage + 256 * 6;  // [0,4) this rank's wait-kernel error word, [8, 8 + 8 * nranks) the status words (root)
-    if (static_cast<size_t>(cm.nranks) * 8 + 8 > 256) {  // more ranks than the pinned read-back page holds status words for
+    CommArgs *h_args = reinterpret_cast<CommArgs *>(es.page(7));
+    uint8_t *h_back = reinterpret_cast<uint8_t *>(es.page(6));  // [0,4) this rank's wait-kernel error word, [8, 8 + 8 * nranks) the status words (root)
+    if (static_cast<size_t>(cm.nranks) * 8 + 8 > kZeroPageBytes) {  // more ranks than the pinned read-back page holds status words for
         lk.unlock();
         return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
     }
     auto &rg = p->reduce_graphs[root * 2 + static_cast<int>(parity)];
     // a graph reads its parts through the pointers captured with it (same rule as bydb_scan_agg_prepared)
-    if (rg.exec) {
-        std::lock_guard<std::mutex> lk2(ctx->mu);
-        bool same = rg.held.size() == p->parts.size(), missing = false;
-        for (size_t i = 0; i < p->parts.size(); ++i) {
-            auto it = ctx->parts.find(p->parts[i]);
-            if (it == ctx->parts.end()) missing = true;
-            else if (same && it->second != rg.held[i]) same = false;
-        }
-        if (missing || !same) {
-            cudaGraphExecDestroy(rg.exec);
-            rg.exec = nullptr;
-            rg.held.clear();
-        }
-    }
+    if (rg.exec) (void)check_held_parts(ctx, p->parts, rg.exec, rg.held);  // a missing part fails in make_plan below
     if (!rg.exec) {
         Plan plan;
         int rc = make_plan(ctx, &p->q, nullptr, plan);
@@ -2956,18 +2859,10 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
             lk.unlock();
             return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);  // takes part in the collective and reports the failure
         }
-        bool overlap = false;  // the version-dedup precheck synchronises: such queries keep the plain path
-        for (size_t a = 0; a < plan.parts.size(); ++a)
-            for (size_t b = a + 1; b < plan.parts.size(); ++b) {
-                const PartDir &x = plan.parts[a]->dir, &y = plan.parts[b]->dir;
-                if (x.blocks.empty() || y.blocks.empty()) continue;
-                if (std::max(std::max(x.min_ts, y.min_ts), p->q.tmin) <= std::min(std::min(x.max_ts, y.max_ts), p->q.tmax)) overlap = true;
-            }
         TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
-        const size_t G = static_cast<size_t>(plan.n_groups), A = p->q.n_aggs, NS = p->q.n_series;
-        const size_t stage = align_up(NS * 12 + (G + 1) * 4 + 512, 256);
-        p->host_off = stage;
-        if (overlap || tl.total > slot_bytes || es.ensure_pinned(stage + G * (12 + 16 * A) + 16 * A + 16384)) {
+        p->host_off = stage_layout(p->q.n_series, tl.G).stride;
+        // the version-dedup precheck synchronises: such queries keep the plain path
+        if (parts_overlap(plan.parts, p->q.tmin, p->q.tmax) || tl.total > slot_bytes || es.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) {
             p->reduce_capturable = false;
             lk.unlock();
             return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
@@ -2989,23 +2884,22 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
             step("args copy", cudaMemcpyAsync(d_args, h_args, sizeof(CommArgs), cudaMemcpyHostToDevice, s) == cudaSuccess);
             launch_comm_wait_args(done, 1, d_args, 1, my_err, kErrPeerTimeout, s);
             step("wait for the slots", true);
-            step("scan", run_scan(ctx, &p->q, plan, es, s, my_slot, tl, &rg.captured, 0, true) == 0);
+            step("scan", run_scan(ctx, &p->q, plan, es, s, my_slot, tl, &rg.captured) == 0);
             rg.express = es.express[0];
             launch_comm_signal_args(flags + cm.rank, status + cm.rank, d_args, s);
             step("signal", true);
             if (cm.rank == root) {
                 launch_comm_wait_args(flags, static_cast<uint32_t>(cm.nranks), d_args, 0, my_err, kErrPeerTimeout, s);
                 step("wait for the ranks", true);
-                launch_combine_tables(reinterpret_cast<uint64_t *>(slots0), static_cast<uint32_t>(cm.nranks), tl.total / 8, tl.off_sum_f64 / 8,
-                                      tl.off_max_f64 / 8, tl.off_max_f64 / 8, tl.off_sum_i64 / 8, tl.off_sum_i64 / 8, tl.off_max_i64 / 8, tl.off_max_i64 / 8,
-                                      tl.total / 8, s, slot_bytes / 8);
+                launch_combine_tables(slots0, static_cast<uint32_t>(cm.nranks), tl, s, slot_bytes);
                 step("combine", true);
-                step("finalize", finalize_enqueue(&p->q, plan, es, s, slots0, tl, p->host_off, rg.fl, fin) == 0);
+                uint32_t fin_launches = 0;
+                step("finalize", finalize_enqueue(&p->q, plan, es, s, slots0, tl, p->host_off, fin, rg.fl, fin_launches) == 0);
                 launch_comm_done_args(done, d_args, s);
                 step("done word", true);
                 step("status read-back",
                      cudaMemcpyAsync(h_back + 8, status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost, s) == cudaSuccess);
-                rg.captured.kernel_launches += 3 + rg.fl.launches;
+                rg.captured.kernel_launches += 3 + fin_launches;
             }
             step("error read-back", cudaMemcpyAsync(h_back, my_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, s) == cudaSuccess);
             rg.captured.kernel_launches += 2;
@@ -3041,36 +2935,23 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
     cm.last_use[2 * static_cast<size_t>(root) + parity] = epoch;
     h_args->epoch = epoch;
     h_args->prev_use = prev_use;
-    memset(h_back, 0, 256);
-    memset(es.zpage, 0, 256);
+    memset(h_back, 0, kZeroPageBytes);
+    memset(es.page(0), 0, kZeroPageBytes);
     cudaStream_t s = es.stream;
     CUDA_TRY(cudaEventRecord(p->t0, s));
     CUDA_TRY(cudaGraphLaunch(rg.exec, s));
     CUDA_TRY(cudaEventRecord(p->t1, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     CUDA_TRY(cudaGetLastError());
-    out->stats = rg.captured;
-    const uint32_t *hz = reinterpret_cast<const uint32_t *>(es.zpage);
-    const unsigned long long *hs = reinterpret_cast<const unsigned long long *>(es.zpage + 16);
-    out->stats.rows_scanned = hs[0];
-    out->stats.rows_matched = hs[1];
-    out->stats.page_bytes = hs[2];
-    out->stats.blocks_scanned = hs[3];
-    out->stats.blocks_slow_lane = static_cast<uint32_t>(hs[4]);
-    out->stats.slow_lane_reasons = static_cast<uint32_t>(hs[5]);
-    out->stats.blocks_express_lane = express_blocks(es.zpage, rg.express);
+    out->stats = rg.captured;  // host-side counters; the zero-page counters are still 0 there
     float ms = 0;
     cudaEventElapsedTime(&ms, p->t0, p->t1);
     out->stats.device_ms = ms;
     out->stats.scan_kernel_ms = 0;  // per-kernel events are not available inside a graph replay
     const uint32_t perr = *reinterpret_cast<const uint32_t *>(h_back);
     if (perr != 0) cudaMemset(my_err, 0, sizeof perr);
-    if (hz[2] != 0) {
-        g_last_dev_err = hz[2];
-        char buf[96];
-        snprintf(buf, sizeof buf, " (block/series #%u)", hz[3]);
-        return fail(dev_err_code(hz[2]), std::string(dev_err_text(hz[2])) + buf);
-    }
+    const int rc = read_zero_page(*es.page(0), rg.express, &out->stats);
+    if (rc) return rc;
     if (perr != 0) return fail(dev_err_code(perr), dev_err_text(perr));
     if (cm.rank != root) return 0;
     const unsigned long long *peer_status = reinterpret_cast<const unsigned long long *>(h_back + 8);
@@ -3079,14 +2960,7 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
         if ((w >> 32) == (epoch & 0xffffffffull) && static_cast<uint32_t>(w) != 0)
             return fail(-static_cast<int>(static_cast<uint32_t>(w)), "multi-GPU reduce: rank " + std::to_string(r) + " failed before its scan");
     }
-    const uint8_t *h = es.pinned + p->host_off;
-    const uint32_t e_in = *reinterpret_cast<const uint32_t *>(h + (rg.fl.o_cnt - rg.fl.o_out) + 8);
-    if (e_in != 0) {
-        g_last_dev_err = e_in;
-        return fail(dev_err_code(e_in), std::string(dev_err_text(e_in)) + " (status carried in a partial table)");
-    }
-    finalize_parse(h, rg.fl, out);
-    return 0;
+    return finalize_parse(es.pinned + p->host_off, rg.fl, true, out);
     });
 }
 
@@ -3107,7 +2981,7 @@ int bydb_scan_reduce_host(bydb_ctx *ctx, uint32_t n_parts, const bydb_part_files
     for (uint32_t i = 0; i < n_parts && !rc; ++i) {
         std::shared_ptr<Part> p;
         // fallback pages are unpacked up front here: a collective cannot be re-run by one rank alone
-        rc = register_part_locked_free(ctx, ~0ull - i, &parts[i], p, &h2d, zc, true, 0, 1, !zc);
+        rc = register_part_locked_free(ctx, ~0ull - i, &parts[i], p, &h2d, zc, true, !zc);
         if (!rc) tmp.push_back(p);
     }
     rc = scan_reduce_impl(ctx, q, &tmp, rc, h2d, root, out);

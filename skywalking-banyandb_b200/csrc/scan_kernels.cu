@@ -3742,13 +3742,13 @@ void launch_group_reduce(const ReduceParams &p, cudaStream_t s, bool small_group
     if (small_groups) group_reduce_small_kernel<<<(p.n_groups + 7) / 8, 256, 0, s>>>(p);
     else group_reduce_kernel<<<p.n_groups, 256, 0, s>>>(p);
 }
-void launch_combine_tables(uint64_t *tables, uint32_t n_tables, uint64_t words, uint64_t sum_f64_lo, uint64_t sum_f64_hi, uint64_t max_f64_lo,
-                           uint64_t max_f64_hi, uint64_t sum_i64_lo, uint64_t sum_i64_hi, uint64_t max_i64_lo, uint64_t max_i64_hi, cudaStream_t s,
-                           uint64_t stride_words) {
+void launch_combine_tables(uint8_t *tables, uint32_t n_tables, const TableLayout &tl, cudaStream_t s, size_t stride_bytes) {
+    const uint64_t words = tl.total / 8;
     if (words == 0 || n_tables < 2) return;
-    combine_tables_kernel<<<static_cast<unsigned>((words + 255) / 256), 256, 0, s>>>(tables, n_tables, words, stride_words ? stride_words : words, sum_f64_lo,
-                                                                                  sum_f64_hi, max_f64_lo, max_f64_hi, sum_i64_lo, sum_i64_hi, max_i64_lo,
-                                                                                  max_i64_hi);
+    // word ranges by how they combine: float sums | float maxima (max, -min) | int64 sums (sum, count, rows) | int64 maxima (max, ~min, coltype)
+    combine_tables_kernel<<<static_cast<unsigned>((words + 255) / 256), 256, 0, s>>>(
+        reinterpret_cast<uint64_t *>(tables), n_tables, words, stride_bytes ? stride_bytes / 8 : words, tl.off_sum_f64 / 8, tl.off_max_f64 / 8,
+        tl.off_max_f64 / 8, tl.off_sum_i64 / 8, tl.off_sum_i64 / 8, tl.off_max_i64 / 8, tl.off_max_i64 / 8, words);
 }
 
 // ------------------------------------------------------------------------------------------------

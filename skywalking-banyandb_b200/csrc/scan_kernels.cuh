@@ -107,7 +107,7 @@ struct ScanParams {
     uint32_t *Pfirst;             // [total_blocks] first surviving row of the block (group-key passes only, else NULL)
     int32_t *col_type;            // [n_fcols] 0 unknown / BYDB_VT_INT64 / BYDB_VT_FLOAT64
     uint32_t *err;                // [2]
-    unsigned long long *stats;    // [0] rows_scanned [1] rows_matched [2] page_bytes [3] blocks
+    unsigned long long *stats;    // [0] rows_scanned [1] rows_matched [2] page_bytes [3] blocks [4] slow-lane blocks [5] slow-lane reasons
     // ---- version dedup across overlapping parts (query.go:995-1004); all NULL when no parts overlap
     int32_t *dd_index;            // [total_blocks] compact index of a block that needs dedup, or -1
     unsigned long long *dd_row_off; // [total_blocks] offset of the block's rows in dd_ts / dd_ver
@@ -220,16 +220,41 @@ struct TablePtrs {
     double *sum_f64, *max_f64, *negmin_f64;
     int64_t *sum_i64, *cnt, *rows, *max_i64, *notmin_i64, *coltype;
 };
+// partial-table layout for (G groups, F fields); see bydb_gpu.h
+struct TableLayout {
+    size_t G, F, GF;
+    size_t off_sum_f64, off_max_f64, off_negmin_f64, off_sum_i64, off_cnt, off_rows, off_max_i64, off_notmin_i64, off_coltype, total;
+    TableLayout(size_t g, size_t f) : G(g), F(f), GF(g * f) {
+        size_t o = 0;
+        off_sum_f64 = o; o += GF * 8;
+        off_max_f64 = o; o += GF * 8;
+        off_negmin_f64 = o; o += GF * 8;
+        off_sum_i64 = o; o += GF * 8;
+        off_cnt = o; o += GF * 8;
+        off_rows = o; o += G * 8;
+        off_max_i64 = o; o += GF * 8;
+        off_notmin_i64 = o; o += GF * 8;
+        off_coltype = o; o += F * 8;
+        total = o;
+    }
+    // the regions of the table at `base`, each from group row g0 on (the coltype words belong to no row)
+    TablePtrs at(uint8_t *base, size_t g0 = 0) const {
+        const size_t gf = g0 * F;
+        return TablePtrs{reinterpret_cast<double *>(base + off_sum_f64) + gf, reinterpret_cast<double *>(base + off_max_f64) + gf,
+                         reinterpret_cast<double *>(base + off_negmin_f64) + gf, reinterpret_cast<int64_t *>(base + off_sum_i64) + gf,
+                         reinterpret_cast<int64_t *>(base + off_cnt) + gf, reinterpret_cast<int64_t *>(base + off_rows) + g0,
+                         reinterpret_cast<int64_t *>(base + off_max_i64) + gf, reinterpret_cast<int64_t *>(base + off_notmin_i64) + gf,
+                         reinterpret_cast<int64_t *>(base + off_coltype)};
+    }
+};
 // dst[j] = src[perm[j]] for every group row of a partial table; coltype = the passes' column types merged
 void launch_permute_table(const TablePtrs &dst, const TablePtrs &src, const int32_t *perm, uint32_t n_groups, uint32_t n_fcols,
                           const int64_t *pass_coltype, uint32_t n_passes, cudaStream_t s);
 constexpr int kFusedFinalizeGroups = 8192;  // up to here one CTA finalises and selects in a single launch
 struct FinalizeParams;
 uint32_t launch_finalize_select(const FinalizeParams &fp, const SelectParams &p, cudaStream_t s);  // -> kernels launched
-// combines n partial tables (each `words` 8-byte words, laid out back to back) into the first one, rank order
-void launch_combine_tables(uint64_t *tables, uint32_t n_tables, uint64_t words, uint64_t sum_f64_lo, uint64_t sum_f64_hi, uint64_t max_f64_lo,
-                           uint64_t max_f64_hi, uint64_t sum_i64_lo, uint64_t sum_i64_hi, uint64_t max_i64_lo, uint64_t max_i64_hi, cudaStream_t s,
-                           uint64_t stride_words = 0);
+// combines n partial tables of layout `tl`, stride_bytes apart (0 = back to back), into the first one, rank order
+void launch_combine_tables(uint8_t *tables, uint32_t n_tables, const TableLayout &tl, cudaStream_t s, size_t stride_bytes = 0);
 // peer-mailbox reduce (bydb_comm_*): bounded wait for n epoch flags, release-store of one
 void launch_comm_wait(const unsigned long long *flags, uint32_t n, unsigned long long epoch, uint32_t *err, uint32_t err_code, cudaStream_t s);
 void launch_comm_signal(unsigned long long *flag, unsigned long long epoch, cudaStream_t s);
