@@ -241,6 +241,7 @@ struct bydb_ctx {
     int sm_count = 0;
     int ctas_per_sm = 2;       // slow lane (general decoder)
     int ctas_per_sm_fast = 2;  // fast lane
+    int ctas_per_sm_express = 2;  // express lane (its own shared-memory ring)
     uint64_t hbm_budget = 0;
     uint64_t hbm_used = 0;
     bool host_index = false;   // BYDB_CFG_HOST_INDEX: parse the block index of resident parts on the host (part_dir.cc)
@@ -1066,7 +1067,7 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
         }
     }
     CUDA_TRY(cudaEventRecord(ev[1], stream));
-    launch_scan_blocks(sp, ctx->sm_count * ctx->ctas_per_sm_fast, ctx->sm_count * ctx->ctas_per_sm, stream);
+    launch_scan_blocks(sp, ctx->sm_count * ctx->ctas_per_sm_express, ctx->sm_count * ctx->ctas_per_sm_fast, ctx->sm_count * ctx->ctas_per_sm, stream);
     CUDA_TRY(cudaEventRecord(ev[2], stream));
     launch_series_reduce(rp, stream);
     const int32_t *gstart = reinterpret_cast<const int32_t *>(h + st.off_gstart);
@@ -1467,11 +1468,12 @@ int bydb_init(const bydb_cfg *cfg, bydb_ctx **out) {
     preload_unpack_kernels();
     preload_index_kernels();
     preload_encode_kernels();
-    int occ_fast = 1, occ_slow = 1;
-    scan_max_ctas_per_sm(&occ_fast, &occ_slow);
+    int occ_express = 1, occ_fast = 1, occ_slow = 1;
+    scan_max_ctas_per_sm(&occ_express, &occ_fast, &occ_slow);
     int want = (cfg && cfg->warps_per_sm > 0) ? (cfg->warps_per_sm + kWarpsPerCta - 1) / kWarpsPerCta : 64;
     ctx->ctas_per_sm = std::max(1, std::min(want, occ_slow));
     ctx->ctas_per_sm_fast = std::max(1, std::min(want, occ_fast));
+    ctx->ctas_per_sm_express = std::max(1, std::min(want, occ_express));
     *out = ctx;
     return 0;
     });

@@ -219,7 +219,8 @@ BYDB_LANE_FN uint32_t mulhi_u32(uint32_t a, uint32_t b) {  // IMAD.HI: a right s
 struct SwarLane {
     int32_t T0, T1, T2, R0, R1, R2;
     uint32_t wide;     // msb set in some byte <=> swar_word: a varint of 4 or more bytes was seen; swar_word2: 3 or more
-    int32_t nterm;     // 1 + terminators seen so far in this lane
+    int32_t nterm;     // swar_word: 1 + terminators seen so far in this lane
+    uint32_t base;     // swar_word2: the same count replicated into every byte (carried instead of nterm)
     uint32_t prev_w;   // the word before the current one (the previous lane's last word for the first)
     uint32_t prev_sb;  // prev_w * 128 (swar_word2 carries it instead of recomputing it)
 };
@@ -227,6 +228,7 @@ BYDB_LANE_FN void swar_begin(SwarLane &s, uint32_t prev_w) {
     s.T0 = s.T1 = s.T2 = s.R0 = s.R1 = s.R2 = 0;
     s.wide = 0;
     s.nterm = 1;
+    s.base = 0x01010101u;
     s.prev_w = prev_w;
     s.prev_sb = imad_u32(prev_w, 128u, 0u);
 }
@@ -274,8 +276,8 @@ BYDB_LANE_FN void swar_word(SwarLane &s, uint32_t w_in, uint32_t vm) {
 // The flag (s.wide) is a continuation byte in class-1 position: a varint of 3 or more bytes, for which this word is wrong.
 // Where the flag stays clear the result is exactly swar_word's: the class-0 bytes and the terminator ranks are the same in
 // both words, and a class-1 byte of a varint of at most 2 bytes has M2 = 0 (the byte two back is a terminator or lies
-// outside the page), so swar_word's p1 / S12 are this word's p1 / S1 and its q2 is 0.  The caller (swar_chunk_sum in
-// scan_kernels.cu) decodes a flagged chunk again with swar_word.
+// outside the page), so swar_word's p1 / S12 are this word's p1 / S1 and its q2 is 0.  The caller (the express lane in
+// scan_kernels.cu) decodes a flagged unit again with swar_word.
 template <bool kMasked>
 BYDB_LANE_FN void swar_word2(SwarLane &s, uint32_t w_in, uint32_t vm) {
     const uint32_t w = kMasked ? (w_in & vm) : w_in;
@@ -289,10 +291,9 @@ BYDB_LANE_FN void swar_word2(SwarLane &s, uint32_t w_in, uint32_t vm) {
     const uint32_t wT = S1 | 0x01010101u;
     uint32_t t01 = ~mulhi_u32(w, 1u << 25) & 0x01010101u;
     if (kMasked) t01 &= vm;
-    const uint32_t base = imad_u32(static_cast<uint32_t>(s.nterm), 0x01010101u, 0u);
-    const uint32_t rinc = imad_u32(t01, 0x01010101u, base);
+    const uint32_t rinc = imad_u32(t01, 0x01010101u, s.base);
     const uint32_t rank1 = imad_u32(t01, 0xffffffffu, rinc);
-    s.nterm = dp4a_su(0x01010101u, t01, s.nterm);
+    s.base = lane_prmt(rinc, 0u, 0x3333u);  // byte 3 of rinc = base + the word's terminators, replicated: the next word's base
     const uint32_t wR = imad_u32(S1 & 0x01010101u, 1u, rank1 ^ S1);
     s.T0 = dp4a_su(x0, 0x01010101u, s.T0);
     s.R0 = dp4a_su(x0, rank1, s.R0);
@@ -302,11 +303,12 @@ BYDB_LANE_FN void swar_word2(SwarLane &s, uint32_t w_in, uint32_t vm) {
     s.prev_w = w;
     s.prev_sb = sb;
 }
-// -> number of terminators of the lane; T and R' as defined above
+// -> number of terminators of the lane; T and R' as defined above.  One lane runs one kind of word between swar_begin and
+// swar_end, so one of the two counters is still at its start value (and folds away where the word is known at compile time).
 BYDB_LANE_FN uint32_t swar_end(const SwarLane &s, int32_t &T, int32_t &Rp) {
     T = (s.T0 >> 1) + 64 * s.T1 + 8192 * s.T2;
     Rp = (s.R0 >> 1) + 64 * s.R1 + 8192 * s.R2;
-    return static_cast<uint32_t>(s.nterm - 1);
+    return static_cast<uint32_t>(s.nterm - 1) + ((s.base & 0xffu) - 1u);
 }
 
 // ------------------------------------------------------------------------------------------------

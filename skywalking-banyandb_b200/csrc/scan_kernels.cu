@@ -767,24 +767,6 @@ __device__ __forceinline__ SwarChunk swar_chunk(const uint8_t *buf, uint32_t c, 
     r.n = swar_end(sl, r.T, r.Rp);
     return r;
 }
-// One chunk of a page for the express lane's SWAR sum: a page starts on the two-class word (three = false).  A chunk whose vote
-// raises the two-class flag is decoded again, from the same stage and the same carry word, with the three-class word, which
-// then takes the rest of the page; there `wide` means a varint of 4+ bytes (the page bails out).  Exact: a varint of 3+ bytes
-// raises the flag in the chunk that holds its second byte, never later than the chunk of its third byte, so every chunk the
-// two-class word keeps has only bytes on which both words agree (lane_decode.cuh, swar_word2).  A page with a 3-byte varint
-// pays at most one extra chunk.  The stage is released only after its chunks, so the redone chunk's bytes are still staged.
-__device__ __forceinline__ SwarChunk swar_chunk_sum(const uint8_t *buf, uint32_t c, uint32_t pstart, uint32_t pend, uint32_t total, uint32_t &carry_w,
-                                                    bool &three, int lane) {
-    if (!three) {
-        const uint32_t cw = carry_w;
-        const SwarChunk ch = swar_chunk<2>(buf, c, pstart, pend, total, carry_w, lane);
-        if (!ch.wide) return ch;
-        three = true;
-        carry_w = cw;
-    }
-    return swar_chunk<3>(buf, c, pstart, pend, total, carry_w, lane);
-}
-
 // ------------------------------------------------------------------------------------------------
 // SWAR sum decoder: EncodeTypeDelta page, every row active, only SUM / MEAN / COUNT wanted (the group-by-sum shape of
 // BASELINE configs 3/4).  See lane_decode.cuh (swar_word): the page sum is a weighted sum over BYTES, so nothing is
@@ -2430,9 +2412,25 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kFastLane ? BYDB_FAST_CTAS 
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kExpressBatch = 8;
 
-__device__ __forceinline__ const uint8_t *ring_wait(WarpSmem *sm, uint32_t n) {
-    const uint32_t slot = n % kStages;
-    const uint32_t parity = (n / kStages) & 1u;
+// One express stage is one decode unit: two 2 KB halves, lane l decoding the 64 bytes at l * 64 of each.  Keeping a lane's
+// window at 64 bytes keeps its terminator ranks <= 65 (they must fit the signed bytes of swar_word's wR) and the shared-memory
+// loads as conflict-free as the 2 KB chunk's; the per-unit work (neighbour shuffles, vote, scan, 64-bit multiply-add, ring
+// wait and refill) is paid once per 32 words per lane.
+constexpr int kExpressStageBytes = 2 * kSwarChunkBytes;
+constexpr int kExpressStages = BYDB_EXPRESS_STAGES;
+static_assert(kExpressStages >= 2, "the express ring refills a stage while the other is decoded");
+
+// the express lane's per-warp shared memory: its ring only (8 warps x 8 KB + barriers: three CTAs per SM)
+struct __align__(128) ExpressSmem {
+    uint8_t stage[kExpressStages][kExpressStageBytes];
+    uint64_t bar[kExpressStages];
+    uint32_t fault;  // set when a TMA wait timed out
+};
+size_t express_smem_bytes() { return sizeof(ExpressSmem) * kWarpsPerCta; }
+
+__device__ __forceinline__ uint8_t *ring_wait(ExpressSmem *sm, uint32_t n) {
+    const uint32_t slot = n % kExpressStages;
+    const uint32_t parity = (n / kExpressStages) & 1u;
     for (uint32_t spins = 0; !mbar_try_wait(&sm->bar[slot], parity); ++spins) {
         if (spins > (1u << 24)) {
             sm->fault = 1;
@@ -2441,23 +2439,88 @@ __device__ __forceinline__ const uint8_t *ring_wait(WarpSmem *sm, uint32_t n) {
     }
     return sm->stage[slot];
 }
+// one stage of the ring: `bytes` from `src` into ring position n (one lane)
+__device__ __forceinline__ void ring_fill(ExpressSmem *sm, uint32_t n, const uint8_t *src, uint32_t bytes) {
+    const uint32_t slot = n % kExpressStages;
+    mbar_expect_tx(&sm->bar[slot], bytes);
+    tma_load_1d(sm->stage[slot], src, bytes, &sm->bar[slot]);
+}
+
+// a 16-byte piece of a stage with only the bytes of `keep` (bit i = byte i) left
+__device__ __forceinline__ void keep_bytes(uint8_t *piece, uint32_t keep) {
+    uint4 v = *reinterpret_cast<const uint4 *>(piece);
+    v.x &= expand4(keep);
+    v.y &= expand4(keep >> 4);
+    v.z &= expand4(keep >> 8);
+    v.w &= expand4(keep >> 12);
+    *reinterpret_cast<uint4 *>(piece) = v;
+}
+// The express lane decodes every unit with the unmasked word, so the bytes of a unit outside the body are made zeros in the
+// stage before it is read: the <= 15 bytes in front of the body (first unit), and behind it the rest of its last 16-byte piece
+// (the next column's bytes) and whatever an earlier copy left beyond the bytes copied.  u0: the unit's offset in the page
+// window; called by the whole warp on a unit that holds pstart or pend.  The stores are fenced against the TMA unit's refill of
+// the stage (generic-proxy writes before async-proxy writes) and made visible to the warp.
+__device__ __forceinline__ void express_zero_edges(uint8_t *buf, uint32_t u0, uint32_t pstart, uint32_t pend, int lane) {
+    if (u0 == 0 && pstart > 0 && lane == 0) keep_bytes(buf, 0xffffu & ~low_bits(pstart));
+    if (u0 + kExpressStageBytes > pend) {
+        const uint32_t e = pend - u0, p0 = e >> 4;  // the piece that holds pend
+        for (uint32_t p = p0 + lane; p < kExpressStageBytes / 16; p += 32) {
+            if (p == p0 && (e & 15u)) keep_bytes(buf + 16 * p, low_bits(e & 15u));  // lane 0, after its head cut of the same piece
+            else *reinterpret_cast<uint4 *>(buf + 16 * p) = make_uint4(0u, 0u, 0u, 0u);
+        }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+}
+// one lane's 64-byte window of a half
+template <int kClasses>
+__device__ __forceinline__ void express_half(SwarLane &sl, const uint8_t *src, uint32_t pw) {
+    swar_begin(sl, pw);
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const uint4 wa = *reinterpret_cast<const uint4 *>(src + 32 * q), wb = *reinterpret_cast<const uint4 *>(src + 32 * q + 16);
+        swar_step<kClasses, false>(sl, wa.x, 0u);
+        swar_step<kClasses, false>(sl, wa.y, 0u);
+        swar_step<kClasses, false>(sl, wa.z, 0u);
+        swar_step<kClasses, false>(sl, wa.w, 0u);
+        swar_step<kClasses, false>(sl, wb.x, 0u);
+        swar_step<kClasses, false>(sl, wb.y, 0u);
+        swar_step<kClasses, false>(sl, wb.z, 0u);
+        swar_step<kClasses, false>(sl, wb.w, 0u);
+    }
+}
+struct ExpressUnit {
+    int32_t Ta, Ra, Tb, Rb;  // T and R' of the lane's windows in half a / b
+    uint32_t n;              // their terminator counts, packed: n_a | n_b << 16
+    bool wide;               // warp vote of the word's flag
+};
+// src: the lane's window in half a; pwa / pwb: the words in front of its windows in half a / b
+template <int kClasses>
+__device__ __forceinline__ ExpressUnit express_unit(const uint8_t *src, uint32_t pwa, uint32_t pwb) {
+    ExpressUnit r;
+    SwarLane sl;
+    express_half<kClasses>(sl, src, pwa);
+    uint32_t wide = sl.wide;
+    const uint32_t na = swar_end(sl, r.Ta, r.Ra);
+    express_half<kClasses>(sl, src + kSwarChunkBytes, pwb);
+    wide |= sl.wide;
+    r.n = na | (swar_end(sl, r.Tb, r.Rb) << 16);
+    r.wide = __any_sync(0xffffffffu, (wide & 0x80808080u) != 0);
+    return r;
+}
 
 __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_express_kernel(const __grid_constant__ ScanParams p) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
-    WarpSmem *sm = reinterpret_cast<WarpSmem *>(smem_raw) + warp;
+    ExpressSmem *sm = reinterpret_cast<ExpressSmem *>(smem_raw) + warp;
     if (lane == 0) {
         sm->fault = 0;
-        sm->seq = 0;
-        sm->st_rows = sm->st_matched = sm->st_bytes = 0;
-        sm->st_blocks = sm->st_deferred = sm->st_why = 0;
-        for (int s = 0; s < kStages; ++s) mbar_init(&sm->bar[s], 1);
+        for (int s = 0; s < kExpressStages; ++s) mbar_init(&sm->bar[s], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     const uint32_t nwork = *p.work_count;
-    constexpr uint32_t kChunksPerStage = kStageBytes / kSwarChunkBytes;
     uint32_t seq = 0;  // stages issued so far by this warp (mbarrier phase bookkeeping; the kernel owns the ring from start to end)
     unsigned long long st_rows = 0, st_bytes = 0;  // per-warp statistics, flushed once at the end
     uint32_t st_blocks = 0, known_types = 0;
@@ -2522,7 +2585,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_ex
                             pstart = static_cast<uint32_t>(a & 15);
                             pend = pstart + (col.size - hdr);
                             total = (pend + 15u) & ~15u;
-                            nst = pend > pstart ? (total + kStageBytes - 1) / kStageBytes : 0;
+                            nst = pend > pstart ? (total + kExpressStageBytes - 1) / kExpressStageBytes : 0;
                             has_page = true;
                             page_bytes += col.size;
                         }
@@ -2540,21 +2603,17 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_ex
             const uint32_t ts = __shfl_sync(0xffffffffu, sb, kExpressBatch - 1);  // stages of the whole batch
             sb -= streams ? nst : 0;                                               // exclusive
             const uint32_t seq0 = seq;
+            // stage s of the batch, from whichever lane's page it belongs to
             auto issue = [&](uint32_t s) {
                 const uint32_t bal = __ballot_sync(0xffffffffu, streams && s >= sb && s < sb + nst);
                 const int src = __ffs(bal) - 1;
                 const uint64_t ab = shfl_u64(reinterpret_cast<uint64_t>(abase), src);
                 const uint32_t tot = __shfl_sync(0xffffffffu, total, src);
-                const uint32_t off = (s - __shfl_sync(0xffffffffu, sb, src)) * kStageBytes;
-                if (lane == 0) {
-                    const uint32_t bytes = min(static_cast<uint32_t>(kStageBytes), tot - off);
-                    const uint32_t slot = (seq0 + s) % kStages;
-                    mbar_expect_tx(&sm->bar[slot], bytes);
-                    tma_load_1d(sm->stage[slot], reinterpret_cast<const uint8_t *>(ab) + off, bytes, &sm->bar[slot]);
-                }
+                const uint32_t off = (s - __shfl_sync(0xffffffffu, sb, src)) * kExpressStageBytes;
+                if (lane == 0) ring_fill(sm, seq0 + s, reinterpret_cast<const uint8_t *>(ab) + off, min(static_cast<uint32_t>(kExpressStageBytes), tot - off));
             };
             __syncwarp();
-            for (uint32_t s = 0; s < ts && s < static_cast<uint32_t>(kStages); ++s) issue(s);
+            for (uint32_t s = 0; s < ts && s < static_cast<uint32_t>(kExpressStages); ++s) issue(s);
             seq += ts;
             for (uint32_t k = 0; k < nb; ++k) {
                 const bool okk = __shfl_sync(0xffffffffu, ok, k);
@@ -2570,39 +2629,75 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_ex
                     const uint32_t ps_k = __shfl_sync(0xffffffffu, pstart, k), pe_k = __shfl_sync(0xffffffffu, pend, k);
                     const uint32_t tot_k = __shfl_sync(0xffffffffu, total, k);
                     const int64_t first_k = static_cast<int64_t>(shfl_u64(static_cast<uint64_t>(first), k));
-                    const uint32_t nchunks = (tot_k + kSwarChunkBytes - 1) / kSwarChunkBytes;
+                    const uint8_t *ab_k = reinterpret_cast<const uint8_t *>(shfl_u64(reinterpret_cast<uint64_t>(abase), k));
                     int64_t S = 0;
-                    uint32_t tb = 0, carry_w = 0, last_byte = 0;
+                    // terminators before the unit.  Every byte of every unit is decoded, and the zeros that stand in for the
+                    // bytes outside the body are one-byte varints of delta 0: they add nothing to T or R' and one terminator
+                    // each.  So tb starts at minus the zeros in front of the body (all of them come before every body byte and
+                    // would otherwise lower its weight), and the zeros behind it are taken off before the count check.
+                    int32_t tb = -static_cast<int32_t>(ps_k);
+                    uint32_t carry_w = 0, last_byte = 0;
+                    // A page starts on the two-class word.  A unit whose vote raises its flag is decoded again, from the same
+                    // stage and the same neighbour words, with the three-class word, which then takes the rest of the page;
+                    // there the flag means a varint of 4+ bytes (the page bails out).  Exact: a varint of 3+ bytes raises the
+                    // flag in the unit that holds its second byte, never later than the unit of its third byte, so every unit
+                    // the two-class word keeps has only bytes on which both words agree (lane_decode.cuh, swar_word2).  The
+                    // stage is refilled only after its unit, so the redone unit's bytes are still staged.
                     bool three = false;
                     for (uint32_t j = 0; j < nst_k; ++j) {
                         const uint32_t s = sb_k + j;
-                        const uint8_t *buf = ring_wait(sm, seq0 + s);
-                        const uint32_t c1 = min(nchunks, (j + 1) * kChunksPerStage);
-                        for (uint32_t cc = j * kChunksPerStage; cc < c1; ++cc) {
-                            if (good) {
-                                const SwarChunk ch = swar_chunk_sum(buf, cc, ps_k, pe_k, tot_k, carry_w, three, lane);
-                                if (ch.wide) {
-                                    good = false;  // keep consuming the page's stages (the ring stays in step), stop decoding
-                                } else {
-                                    uint32_t n_in = ch.n;
-#pragma unroll
-                                    for (int sft = 1; sft < 32; sft <<= 1) {
-                                        const uint32_t on = __shfl_up_sync(0xffffffffu, n_in, sft);
-                                        if (lane >= sft) n_in += on;
-                                    }
-                                    const int64_t A1 = static_cast<int64_t>(count_k) - static_cast<int64_t>(tb) - static_cast<int64_t>(n_in - ch.n);
-                                    S += A1 * static_cast<int64_t>(ch.T) - static_cast<int64_t>(ch.Rp);
-                                    tb += __shfl_sync(0xffffffffu, n_in, 31);
-                                }
+                        uint8_t *buf = ring_wait(sm, seq0 + s);
+                        if (good) {
+                            if (j == 0 || (j + 1) * kExpressStageBytes > pe_k) express_zero_edges(buf, j * kExpressStageBytes, ps_k, pe_k, lane);
+                            const uint8_t *src = buf + lane * kSwarLaneBytes;
+                            // the word in front of each window: lane l-1's last word of the same half; for lane 0, the
+                            // previous unit's last word (half a) and lane 31's last word of half a (half b)
+                            const uint32_t la = *reinterpret_cast<const uint32_t *>(src + kSwarLaneBytes - 4);
+                            const uint32_t lb = *reinterpret_cast<const uint32_t *>(src + kSwarChunkBytes + kSwarLaneBytes - 4);
+                            const uint32_t xa = __shfl_sync(0xffffffffu, la, (lane + 31) & 31), xb = __shfl_sync(0xffffffffu, lb, (lane + 31) & 31);
+                            const uint32_t pwa = lane == 0 ? carry_w : xa, pwb = lane == 0 ? xa : xb;
+                            carry_w = xb;  // lane 0: lane 31's last word of half b
+                            ExpressUnit eu;
+                            if (!three) {
+                                eu = express_unit<2>(src, pwa, pwb);
+                                three = eu.wide;
                             }
-                            if (cc == nchunks - 1 && lane == 0) last_byte = buf[(pe_k - 1) % kStageBytes];
+                            if (three) eu = express_unit<3>(src, pwa, pwb);
+                            if (eu.wide) {
+                                good = false;  // keep consuming the page's stages (the ring stays in step), stop decoding
+                            } else {
+                                // one scan of both halves' terminator counts (<= 2048 per half: 16 bits each)
+                                uint32_t n_in = eu.n;
+#pragma unroll
+                                for (int sft = 1; sft < 32; sft <<= 1) {
+                                    const uint32_t on = __shfl_up_sync(0xffffffffu, n_in, sft);
+                                    if (lane >= sft) n_in += on;
+                                }
+                                const uint32_t tot_n = __shfl_sync(0xffffffffu, n_in, 31), ex = n_in - eu.n;
+                                // weight of a byte = (count - 1) - terminators before it = (count - tb - before the lane) - (rank + 1)
+                                const int32_t Aa = static_cast<int32_t>(count_k) - tb - static_cast<int32_t>(ex & 0xffffu);
+                                const int32_t Ab = Aa - static_cast<int32_t>(tot_n & 0xffffu) + static_cast<int32_t>(ex & 0xffffu) - static_cast<int32_t>(ex >> 16);
+                                S += static_cast<int64_t>(Aa) * eu.Ta + static_cast<int64_t>(Ab) * eu.Tb - static_cast<int64_t>(eu.Ra) - static_cast<int64_t>(eu.Rb);
+                                tb += static_cast<int32_t>((tot_n & 0xffffu) + (tot_n >> 16));
+                            }
                         }
+                        if (j == nst_k - 1 && lane == 0) last_byte = buf[(pe_k - 1) % kExpressStageBytes];
                         __syncwarp();
-                        if (s + kStages < ts) issue(s + kStages);
+                        const uint32_t nx = s + kExpressStages;
+                        if (nx < ts) {
+                            if (j + kExpressStages < nst_k) {
+                                // the common case: the next stage to fill is this page's own
+                                const uint32_t off = (j + kExpressStages) * kExpressStageBytes;
+                                if (lane == 0) ring_fill(sm, seq0 + nx, ab_k + off, min(static_cast<uint32_t>(kExpressStageBytes), tot_k - off));
+                            } else {
+                                issue(nx);
+                            }
+                        }
                     }
                     last_byte = __shfl_sync(0xffffffffu, last_byte, 0);
+                    const int32_t zeros_after = static_cast<int32_t>(nst_k * kExpressStageBytes - pe_k);
                     if (nst_k == 0) good = count_k == 1;  // an empty body: the page holds `first` alone
-                    else good = good && tb + 1 == count_k && last_byte < 0x80u;
+                    else good = good && tb - zeros_after + 1 == static_cast<int32_t>(count_k) && last_byte < 0x80u;
 #pragma unroll
                     for (int m = 16; m >= 1; m >>= 1) S += static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(S), m));
                     acc.add_scaled(first_k, count_k);
@@ -3698,24 +3793,27 @@ static void scan_set_attrs() {
     const int smem = static_cast<int>(scan_smem_bytes());
     cudaFuncSetAttribute(scan_blocks_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(scan_blocks_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    cudaFuncSetAttribute(scan_sum_express_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(scan_sum_express_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(express_smem_bytes()));
     cudaFuncSetAttribute(dedup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (dev >= 0 && dev < 64) g_attr_set[dev].store(true, std::memory_order_release);
 }
-// fast lane over the planned blocks, then the slow lane over whatever the fast lane deferred
-void launch_scan_blocks(const ScanParams &p, int grid_fast, int grid_slow, cudaStream_t s) {
+// express lane (when the query has its shape), fast lane over the planned blocks or what the express lane left, then the
+// slow lane over whatever the fast lane deferred
+void launch_scan_blocks(const ScanParams &p, int grid_express, int grid_fast, int grid_slow, cudaStream_t s) {
     scan_set_attrs();
     const size_t smem = scan_smem_bytes();
-    if (p.rest_list) scan_sum_express_kernel<<<grid_fast, kWarpsPerCta * 32, smem, s>>>(p);
+    if (p.rest_list) scan_sum_express_kernel<<<grid_express, kWarpsPerCta * 32, express_smem_bytes(), s>>>(p);
     scan_blocks_kernel<true><<<grid_fast, kWarpsPerCta * 32, smem, s>>>(p);
     scan_blocks_kernel<false><<<grid_slow, kWarpsPerCta * 32, smem, s>>>(p);
 }
 
-void scan_max_ctas_per_sm(int *fast, int *slow) {
+void scan_max_ctas_per_sm(int *express, int *fast, int *slow) {
     scan_set_attrs();
-    int a = 1, b = 1;
+    int e = 1, a = 1, b = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e, scan_sum_express_kernel, kWarpsPerCta * 32, express_smem_bytes());
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, scan_blocks_kernel<true>, kWarpsPerCta * 32, scan_smem_bytes());
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, scan_blocks_kernel<false>, kWarpsPerCta * 32, scan_smem_bytes());
+    *express = e < 1 ? 1 : e;
     *fast = a < 1 ? 1 : a;
     *slow = b < 1 ? 1 : b;
 }

@@ -17,6 +17,9 @@ constexpr int kWarpsPerCta = 8;          // 256 threads; every warp is an indepe
 #ifndef BYDB_STAGES
 #define BYDB_STAGES 2
 #endif
+#ifndef BYDB_EXPRESS_STAGES
+#define BYDB_EXPRESS_STAGES 2            // the express lane's own ring depth (its stages are 4 KB decode units)
+#endif
 #ifndef BYDB_SPARSE
 #define BYDB_SPARSE 0                    // 1: masked / ranged delta pages take delta_page_sparse (measured slower, see DESIGN.md 4.2; make variant EXTRA="-DBYDB_SPARSE=1 -DBYDB_STAGES=3")
 #endif
@@ -311,15 +314,17 @@ void launch_gather_pages(const EncodeParams &p, const uint64_t *out_off, uint8_t
 void preload_encode_kernels();   // encode_kernels.cu
 
 size_t scan_smem_bytes();
+size_t express_smem_bytes();
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s);
-void launch_scan_blocks(const ScanParams &p, int grid_fast, int grid_slow, cudaStream_t s);
+// grid_express: the express lane's grid (launched when p.rest_list is set), grid_fast / grid_slow: the regular lanes'
+void launch_scan_blocks(const ScanParams &p, int grid_express, int grid_fast, int grid_slow, cudaStream_t s);
 void launch_series_reduce(const ReduceParams &p, cudaStream_t s);
 void launch_group_reduce(const ReduceParams &p, cudaStream_t s, bool small_groups = false);  // small_groups: no group has more than 32 series
 void launch_finalize(const FinalizeParams &p, cudaStream_t s);
 void launch_detect_overlap(const ScanParams &p, cudaStream_t s);
 void launch_dedup(const ScanParams &p, int grid, cudaStream_t s);
 int upload_pow10_table();
-void scan_max_ctas_per_sm(int *fast, int *slow);
+void scan_max_ctas_per_sm(int *express, int *fast, int *slow);
 void preload_kernels();          // scan_kernels.cu: forces the (lazily loaded) code of every kernel onto the current device
 void preload_unpack_kernels();   // unpack_kernels.cu
 void preload_index_kernels();    // index_kernels.cu
