@@ -2974,8 +2974,10 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
         acc[c].cnt = 0;
     }
     int64_t rows = 0;
-    int64_t kts = INT64_MAX;  // group-key passes: (ts_min, row) of the first surviving row of the series, lane-local until the end
-    uint32_t krow = 0;
+    // group-key passes: (ts_min, row) of the first surviving row of the series, lane-local until the end; krow == kKeyAbsent
+    // while the series has shown no row (every timestamp, INT64_MAX included, is a valid ts_min)
+    int64_t kts = INT64_MAX;
+    uint32_t krow = kKeyAbsent;
     int64_t span_lo[4], span_hi[4];
     int nspan = 0;
     bool overlap = false;
@@ -3004,7 +3006,7 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
                 tlo = part.blocks[b].ts_min;
                 thi = part.blocks[b].ts_max;
             }
-            if (p.Kts && r > 0 && tlo < kts) {
+            if (p.Kts && r > 0 && (krow == kKeyAbsent || tlo < kts)) {
                 kts = tlo;
                 krow = p.Pfirst[g];
             }
@@ -3050,7 +3052,7 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
         for (int m = 16; m >= 1; m >>= 1) {
             const int64_t ot = static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(kts), m));
             const uint32_t orow = __shfl_xor_sync(0xffffffffu, krow, m);
-            if (ot < kts) {
+            if (orow != kKeyAbsent && (krow == kKeyAbsent || ot < kts)) {
                 kts = ot;
                 krow = orow;
             }
@@ -3684,10 +3686,11 @@ __global__ void __launch_bounds__(256) key_order_kernel(const __grid_constant__ 
     if (gp >= G * p.n_values) return;
     const uint32_t v = gp / G, g = gp % G;
     const int64_t *kts = p.Kts + static_cast<size_t>(v) * p.n_series;
+    const uint32_t *krow = p.Krow + static_cast<size_t>(v) * p.n_series;
     int32_t best = INT32_MAX;
     for (int32_t k = p.group_start[g] + lane; k < p.group_start[g + 1]; k += 32) {
         const int32_t i = p.order[k];
-        if (kts[i] != INT64_MAX && i < best) best = i;
+        if (krow[i] != kKeyAbsent && i < best) best = i;
     }
     best = __reduce_min_sync(0xffffffffu, best);
     if (best == INT32_MAX) {
@@ -3695,11 +3698,12 @@ __global__ void __launch_bounds__(256) key_order_kernel(const __grid_constant__ 
         return;
     }
     const int64_t mts = kts[best];
-    const uint32_t mrow = p.Krow[static_cast<size_t>(v) * p.n_series + best];
+    const uint32_t mrow = krow[best];
     uint32_t rank = 0;
     for (uint32_t v2 = lane; v2 < p.n_values; v2 += 32) {
         const int64_t t = p.Kts[static_cast<size_t>(v2) * p.n_series + best];
-        if (t != INT64_MAX && (t < mts || (t == mts && p.Krow[static_cast<size_t>(v2) * p.n_series + best] < mrow))) ++rank;
+        const uint32_t r2 = p.Krow[static_cast<size_t>(v2) * p.n_series + best];
+        if (r2 != kKeyAbsent && (t < mts || (t == mts && r2 < mrow))) ++rank;
     }
     rank = __reduce_add_sync(0xffffffffu, rank);
     if (lane == 0) {

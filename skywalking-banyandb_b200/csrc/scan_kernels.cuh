@@ -56,6 +56,7 @@ enum DevErr : uint32_t {
     kErrKeyLong = 13,       // per-row group key: a value longer than kMaxLit bytes
 };
 constexpr int kOpEqOrNil = 7;  // internal predicate operator of the group-key passes: the cell is nil or equals the literal
+constexpr uint32_t kKeyAbsent = 0xffffffffu;  // Krow of a series that never shows the value (a block's first row is below it)
 
 struct DevPartRef {
     const DevBlock *blocks;
