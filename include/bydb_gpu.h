@@ -195,18 +195,26 @@ int bydb_scan_agg(bydb_ctx *ctx, const bydb_query *q, bydb_result *out);
  * (series_group of its series, value of the key tag in that row); groups come back in insertion order -- the scan order is
  * series by series (ascending series id), by time inside a series -- or in rank order when top_n > 0 (ties: the group
  * inserted first, top.go:62-76).  A nil cell and "" are the same key (groupby.go:226-254 encodes a string / bytes key as
- * length + raw bytes).  The key must be a string / binary tag stored with the dictionary encoding (<= 256 distinct values
- * per block, pkg/encoding/dictionary.go); a block that fell back to the plain bytes block makes the call return
- * BYDB_ENOTSUP, more than max_values distinct values over the selected blocks BYDB_ENOMEM (the reference's aggregation
- * memory budget), a value longer than 64 bytes BYDB_ENOTSUP.  Device side: one pass collects the distinct values from the
- * dictionary pages, then ONE SCAN PASS PER VALUE (the key as an extra predicate) fills that value's slice of a composite
- * partial table; stats count every pass.  Not available through the prepared / partial-table / multi-GPU entry points,
+ * length + raw bytes).  value_type declares the key tag's type, from the schema the caller holds (as bydb_pred.value_type):
+ *   0, BYDB_VT_STR or BYDB_VT_BINARY: a string / binary tag stored with the dictionary encoding (<= 256 distinct values per
+ *     block, pkg/encoding/dictionary.go); a block that fell back to the plain bytes block makes the call return
+ *     BYDB_ENOTSUP, a value longer than 64 bytes BYDB_ENOTSUP, a tag stored as int64 BYDB_EINVAL.
+ *   BYDB_VT_INT64: an int64 tag.  A key value is 8 bytes of little-endian two's complement (the reference's key bytes), so
+ *     key_off advances in steps of 8; a nil cell, or a block without the column, is the key 0 (the column's zero value,
+ *     typed_column.go:49-53).  A tag stored as a string gives BYDB_EINVAL, a numeric fallback page that admission left
+ *     packed BYDB_ENOTSUP.
+ *   any other value: BYDB_EINVAL.
+ * n_keys counts the distinct values over ALL rows of the selected blocks (series in the query, time span meeting the
+ * range), before the time trim and the predicates.  More than max_values of them give BYDB_ENOMEM (the reference's
+ * aggregation memory budget).  Device side: one pass collects the distinct values, then ONE SCAN PASS PER VALUE (the key as
+ * an extra predicate) fills that value's slice of a composite partial table; stats count every pass.  A group-key query
+ * takes at most 7 predicates of its own.  Not available through the prepared / partial-table / multi-GPU entry points,
  * and not over parts that overlap in time. */
 typedef struct {
     const char *family;    /* tag family of the key tag                                      */
     const char *tag;       /* tag name                                                       */
     uint32_t max_values;   /* distinct key values accepted over the whole query; 0 = 64, at most 256 */
-    uint32_t reserved;
+    uint32_t value_type;   /* 0 / BYDB_VT_STR / BYDB_VT_BINARY (string key) or BYDB_VT_INT64 */
 } bydb_group_key;
 
 typedef struct {

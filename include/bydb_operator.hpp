@@ -17,6 +17,9 @@
 // buildAggOutputSchema's (aggregation.go:402-418): the projected tag columns in schema order, then one RoleField column per
 // AggSpec typed by aggOutputType (COUNT -> int64, otherwise the input field's type); group rows come in first-appearance
 // order of the scan (reversed for an order-by DESC request), non-key projected tags carry the first-seen value.
+// A GroupBy key column with per-series values (ScanSpec::SeriesTags: entity / indexed tags) is densified per series; at most
+// one key column may be a stored tag (a tag column absent from SeriesTags), and then the operator calls bydb_scan_agg_keyed, which adds
+// the row's value of that tag to the group.  Such a key takes the ascending series order only (no OrderDesc).
 // tests/native/operator_test.cc drives it; the Python mirror (skywalking-banyandb_b200/scan_operator.py) follows the same code.
 #pragma once
 
@@ -111,6 +114,7 @@ struct ScanSpec {
     int64_t TMin = INT64_MIN, TMax = INT64_MAX;
     std::vector<Pred> Preds;
     bool OrderDesc = false;
+    uint32_t MaxKeyValues = 0;  // distinct values of a stored-tag GroupBy key (bydb_group_key.max_values; 0 = the library's 64)
 };
 
 struct Error {
@@ -174,6 +178,7 @@ class GPUScanAgg final : public PullOperator {
             }
         }
         if (cursor_ >= row_end_) return std::nullopt;  // EOF
+        const bydb_result &res = result();
         const size_t lo = cursor_, hi = std::min(cursor_ + static_cast<size_t>(batch_), row_end_);
         cursor_ = hi;
         auto b = std::make_unique<RecordBatch>();
@@ -183,9 +188,26 @@ class GPUScanAgg final : public PullOperator {
             const ColumnDef &cd = in_.Columns[static_cast<size_t>(ti)];
             Column col;
             col.Type = cd.Type;
+            if (ti == stored_key_) {
+                for (size_t r = lo; r < hi; ++r) {  // the row's key bytes (groupby.go:226-254); a nil cell came back as 0 / ""
+                    const int32_t k = kres_.key_id[r];
+                    const uint8_t *kb = kres_.key_bytes + kres_.key_off[k];
+                    const size_t klen = kres_.key_off[k + 1] - kres_.key_off[k];
+                    if (cd.Type == ColumnType::ColumnTypeInt64) {
+                        uint64_t u = 0;
+                        for (size_t i = 0; i < klen && i < 8; ++i) u |= static_cast<uint64_t>(kb[i]) << (8 * i);
+                        col.Int64.push_back(static_cast<int64_t>(u));
+                    } else {
+                        col.Bytes.emplace_back(reinterpret_cast<const char *>(kb), klen);
+                    }
+                    col.Valid.push_back(1);
+                }
+                b->Columns.push_back(std::move(col));
+                continue;
+            }
             const auto it = scan_.SeriesTags.find({cd.TagFamily, cd.Name});
             for (size_t r = lo; r < hi; ++r) {
-                const int g = res_.group_id[r];
+                const int g = res.group_id[r];
                 if (it == scan_.SeriesTags.end()) {
                     col.Bytes.emplace_back();
                     col.Valid.push_back(0);
@@ -199,11 +221,11 @@ class GPUScanAgg final : public PullOperator {
         const size_t A = aggs_.size();
         for (size_t a = 0; a < A; ++a) {
             Column col;
-            const bool isf = res_.is_float[a] != 0;
+            const bool isf = res.is_float[a] != 0;
             col.Type = isf ? ColumnType::ColumnTypeFloat64 : ColumnType::ColumnTypeInt64;
             for (size_t r = lo; r < hi; ++r) {
-                if (isf) col.Float64.push_back(res_.val_f64[r * A + a]);
-                else col.Int64.push_back(res_.val_i64[r * A + a]);
+                if (isf) col.Float64.push_back(res.val_f64[r * A + a]);
+                else col.Int64.push_back(res.val_i64[r * A + a]);
                 col.Valid.push_back(1);
             }
             b->Columns.push_back(std::move(col));
@@ -214,7 +236,8 @@ class GPUScanAgg final : public PullOperator {
 
     Status Close() override {  // idempotent; releases the result exactly once
         if (have_result_) {
-            bydb_result_free(ctx_, &res_);
+            if (stored_key_ >= 0) bydb_keyed_result_free(ctx_, &kres_);
+            else bydb_result_free(ctx_, &res_);
             have_result_ = false;
         }
         closed_ = true;
@@ -225,6 +248,7 @@ class GPUScanAgg final : public PullOperator {
 
   private:
     Status fail(int code, std::string msg) { return Error{code, std::move(msg)}; }
+    const bydb_result &result() const { return stored_key_ >= 0 ? kres_.base : res_; }
 
     Status run() {
         ran_ = true;
@@ -233,14 +257,23 @@ class GPUScanAgg final : public PullOperator {
         const size_t ns = scan_.SeriesIDs.size();
         // group key per series = tuple of the key columns' values; dense ids in first-appearance order of the scan
         // (aggregation.go:211-213); an order-by DESC request visits the series list backwards
+        // A tag key column without per-series values is a stored tag: bydb_scan_agg_keyed adds its row value to the group.
+        // Any other key column (a field) still needs per-series values.
         std::vector<const std::vector<std::string> *> keyvals;
+        stored_key_ = -1;
         for (int ki : keys_) {
             const ColumnDef &cd = in_.Columns[static_cast<size_t>(ki)];
             const auto it = scan_.SeriesTags.find({cd.TagFamily, cd.Name});
+            if (it == scan_.SeriesTags.end() && cd.Role == ColumnRole::RoleTag) {
+                if (stored_key_ >= 0) return fail(BYDB_ENOTSUP, "GroupBy key " + cd.TagFamily + "/" + cd.Name + ": at most one stored-tag key per query");
+                stored_key_ = ki;
+                continue;
+            }
             if (it == scan_.SeriesTags.end() || it->second.size() != ns)
                 return fail(BYDB_EINVAL, "GroupBy key " + cd.TagFamily + "/" + cd.Name + " needs one value per series (entity / indexed tag)");
             keyvals.push_back(&it->second);
         }
+        if (stored_key_ >= 0 && scan_.OrderDesc) return fail(BYDB_ENOTSUP, "a stored-tag GroupBy key takes the ascending series order only (OrderDesc)");
         std::map<std::vector<std::string>, int32_t> group_of;
         std::vector<int32_t> gids(ns, 0);
         group_first_series_.clear();
@@ -303,12 +336,23 @@ class GPUScanAgg final : public PullOperator {
         q.top_n = top_ ? top_->N : 0;
         q.top_agg = top_ ? top_->AggIndex : 0;
         q.top_desc = top_ ? (top_->Desc ? 1 : 0) : 1;
-        const int rc = bydb_scan_agg(ctx_, &q, &res_);
+        int rc;
+        if (stored_key_ < 0) {
+            rc = bydb_scan_agg(ctx_, &q, &res_);
+        } else {
+            const ColumnDef &cd = in_.Columns[static_cast<size_t>(stored_key_)];
+            bydb_group_key key{};
+            key.family = cd.TagFamily.c_str();
+            key.tag = cd.Name.c_str();
+            key.max_values = scan_.MaxKeyValues;
+            key.value_type = cd.Type == ColumnType::ColumnTypeInt64 ? BYDB_VT_INT64 : 0;
+            rc = bydb_scan_agg_keyed(ctx_, &q, &key, &kres_);
+        }
         if (rc != 0) return fail(rc, bydb_last_error() ? bydb_last_error() : "bydb_scan_agg failed");
         have_result_ = true;
-        stats_ = res_.stats;
+        stats_ = result().stats;
         // offset / limit window over the (Top-ordered) output rows, limit.go:56-73
-        const size_t n = static_cast<size_t>(res_.n_rows);
+        const size_t n = static_cast<size_t>(result().n_rows);
         if (limit_) {
             cursor_ = std::min<size_t>(limit_->Offset, n);
             row_end_ = std::min<size_t>(cursor_ + limit_->Limit, n);
@@ -328,6 +372,8 @@ class GPUScanAgg final : public PullOperator {
     std::optional<TopSpec> top_;
     std::optional<LimitSpec> limit_;
     bydb_result res_{};
+    bydb_keyed_result kres_{};  // the result when a GroupBy key is a stored tag
+    int stored_key_ = -1;       // input column of that key, -1 = none
     bydb_stats stats_{};
     std::vector<int> group_first_series_;
     size_t cursor_ = 0, row_end_ = 0;

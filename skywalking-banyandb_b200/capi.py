@@ -70,7 +70,7 @@ class _Result(C.Structure):
 
 
 class _GroupKey(C.Structure):
-    _fields_ = [("family", C.c_char_p), ("tag", C.c_char_p), ("max_values", C.c_uint32), ("reserved", C.c_uint32)]
+    _fields_ = [("family", C.c_char_p), ("tag", C.c_char_p), ("max_values", C.c_uint32), ("value_type", C.c_uint32)]
 
 
 class _KeyedResult(C.Structure):
@@ -432,12 +432,13 @@ class Context:
         finally:
             self._L.bydb_result_free(self._h, C.byref(r))
 
-    def scan_agg_keyed(self, q: Query, family: str, tag: str, max_values: int = 0) -> Result:
-        """Group-by on a stored tag (bydb_scan_agg_keyed): rows carry (series group, key value)."""
+    def scan_agg_keyed(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> Result:
+        """Group-by on a stored tag (bydb_scan_agg_keyed): rows carry (series group, key value).  value_type: 0 / VT_STR /
+        VT_BINARY for a string tag, VT_INT64 for an int64 tag (key values are then 8 little-endian bytes)."""
         keep: list = []
         cq = _mk_query(q, keep)
         fb, tb = family.encode(), tag.encode()
-        gk = _GroupKey(fb, tb, max_values, 0)
+        gk = _GroupKey(fb, tb, max_values, value_type)
         r = _KeyedResult()
         _check(self._L.bydb_scan_agg_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
         try:

@@ -1646,6 +1646,9 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     int rc = validate_query(q, true);
     if (rc) return rc;
     if (!key || !key->family || !key->tag) return fail(BYDB_EINVAL, "group key without family/tag");
+    if (key->value_type != 0 && key->value_type != BYDB_VT_STR && key->value_type != BYDB_VT_BINARY && key->value_type != BYDB_VT_INT64)
+        return fail(BYDB_EINVAL, "bydb_group_key.value_type must be 0, BYDB_VT_STR, BYDB_VT_BINARY or BYDB_VT_INT64");
+    const bool int64_key = key->value_type == BYDB_VT_INT64;
     const uint32_t cap = key->max_values ? key->max_values : 64u;
     if (cap > kMaxKeyValues) return fail(BYDB_EINVAL, "bydb_group_key.max_values above 256");
     if (q->n_preds + 1 > kMaxPreds) return fail(BYDB_ENOTSUP, "a group-key query takes at most 7 predicates");
@@ -1694,9 +1697,10 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     kpar.slots = reinterpret_cast<unsigned long long *>(ka.base + a_slots);
     kpar.count = reinterpret_cast<uint32_t *>(ka.base + a_ctl);
     kpar.err = reinterpret_cast<uint32_t *>(ka.base + a_ctl) + 1;
+    kpar.zero = reinterpret_cast<uint32_t *>(ka.base + a_ctl) + 3;
     kpar.vals = ka.base + a_vals;
     kpar.lens = reinterpret_cast<uint32_t *>(ka.base + a_lens);
-    launch_key_values(kpar, ctx->sm_count * 4, stream);
+    launch_key_values(kpar, int64_key, ctx->sm_count * 4, stream);
     CUDA_TRY(cudaStreamSynchronize(stream));  // the staging of the series ids must be consumed before the read-back reuses it
     CUDA_TRY(cudaMemcpyAsync(slot.pinned, ka.base + a_ctl, back_bytes, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
@@ -1716,7 +1720,10 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     {
         const uint8_t *hv = slot.pinned + (a_vals - a_ctl);
         const uint32_t *hl = reinterpret_cast<const uint32_t *>(slot.pinned + (a_lens - a_ctl));
-        for (size_t v = 0; v < V; ++v) values[v].assign(hv + v * kMaxLit, hv + v * kMaxLit + hl[v]);
+        for (size_t v = 0; v < V; ++v) {
+            if (int64_key) values[v].assign(hv + v * 8, hv + v * 8 + 8);  // the reference's key bytes: little-endian int64
+            else values[v].assign(hv + v * kMaxLit, hv + v * kMaxLit + hl[v]);
+        }
     }
     auto owner = new KeyedOwner();
     out->owner = owner;
@@ -1764,10 +1771,18 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
         memset(&kpred, 0, sizeof kpred);
         kpred.family = key->family;
         kpred.tag = key->tag;
-        kpred.op = values[v].empty() ? kOpEqOrNil : BYDB_OP_EQ;  // a nil cell and "" are the same key (groupby.go:226-254)
-        kpred.value_type = BYDB_VT_STR;
-        kpred.lit = values[v].data();
-        kpred.lit_len = values[v].size();
+        if (int64_key) {
+            int64_t lit = 0;
+            memcpy(&lit, values[v].data(), 8);
+            kpred.op = lit == 0 ? kOpEqOrNil : BYDB_OP_EQ;  // a nil cell is the column's zero value (typed_column.go:49-53)
+            kpred.value_type = BYDB_VT_INT64;
+            kpred.lit_i64 = lit;
+        } else {
+            kpred.op = values[v].empty() ? kOpEqOrNil : BYDB_OP_EQ;  // a nil cell and "" are the same key (groupby.go:226-254)
+            kpred.value_type = BYDB_VT_STR;
+            kpred.lit = values[v].data();
+            kpred.lit_len = values[v].size();
+        }
         qv.preds = preds.data();
         KeyedPass pass;
         pass.group_off = v * G;

@@ -1554,6 +1554,24 @@ __device__ __forceinline__ void agg_arith_page(AggAcc &acc, int64_t first, int64
 // ------------------------------------------------------------------------------------------------
 // plan_blocks: block selection
 // ------------------------------------------------------------------------------------------------
+// Is block b selected?  qi = index of its series in the query's ascending series list, -1 when the series is not queried
+// (binary search, query.go:601).  part_iter.go:232-241: the block must overlap the inclusive time range.  An empty range
+// (tmin > tmax) holds no row of any block, so it selects none: a block spanning it would otherwise reach series_reduce,
+// whose overlap check then sees parts that the host-side overlap precheck (empty intersection with the range) never sent
+// through dedup.  The group-key discovery kernels select with the same test.
+__device__ __forceinline__ bool select_block(const uint64_t *q_sids, uint32_t n_series, int64_t tmin, int64_t tmax, const DevBlock &b,
+                                             int32_t &qi) {
+    uint32_t lo = 0, hi = n_series;
+    const uint64_t sid = b.sid;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (q_sids[mid] < sid) lo = mid + 1;
+        else hi = mid;
+    }
+    qi = lo < n_series && q_sids[lo] == sid ? static_cast<int32_t>(lo) : -1;
+    return qi >= 0 && tmin <= tmax && !(b.ts_max < tmin || b.ts_min > tmax);
+}
+
 __global__ void plan_blocks_kernel(const __grid_constant__ ScanParams p) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     bool sel = false;
@@ -1561,20 +1579,9 @@ __global__ void plan_blocks_kernel(const __grid_constant__ ScanParams p) {
         uint32_t pi = 0;
         while (pi + 1 < p.n_parts && g >= p.parts[pi + 1].block_base) ++pi;
         const DevBlock &b = p.parts[pi].blocks[g - p.parts[pi].block_base];
-        // binary search of the block's series in the query's ascending series list (query.go:601)
-        uint32_t lo = 0, hi = p.n_series;
         const uint64_t sid = b.sid;
-        while (lo < hi) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (p.q_sids[mid] < sid) lo = mid + 1;
-            else hi = mid;
-        }
-        int32_t qi = -1;
-        if (lo < p.n_series && p.q_sids[lo] == sid) qi = static_cast<int32_t>(lo);
-        // part_iter.go:232-241: the block must overlap the inclusive time range.  An empty range (tmin > tmax) holds no row of
-        // any block, so it selects none: a block spanning it would otherwise reach series_reduce, whose overlap check then
-        // sees parts that the host-side overlap precheck (empty intersection with the range) never sent through dedup
-        sel = qi >= 0 && p.tmin <= p.tmax && !(b.ts_max < p.tmin || b.ts_min > p.tmax);
+        int32_t qi;
+        sel = select_block(p.q_sids, p.n_series, p.tmin, p.tmax, b, qi);
         p.block_qsid[g] = sel ? qi : -1;
         p.Prows[g] = 0;
         // head of this series' run of blocks inside the part: lets series_reduce skip its binary search
@@ -3543,7 +3550,8 @@ __global__ void combine_tables_kernel(uint64_t *t, uint32_t n, uint64_t words, u
 // insertion list; groupby.go:226-254: a string / bytes key is its length + raw bytes, so a nil cell and "" are one key).
 //   1. key_values_kernel: one warp per selected block reads the tag's dictionary page (<= 256 values per block,
 //      pkg/encoding/dictionary.go:52-88) and enters every value into a small open-addressing table in global memory; a
-//      slot holds the device address and length of the bytes inside the part, the bytes themselves never move.
+//      slot holds the device address and length of the bytes inside the part, the bytes themselves never move.  An int64
+//      key takes key_values_i64_kernel instead (below): every value of the block's int64 page, the value itself in the slot.
 //   2. the host runs one ordinary scan pass per distinct value v (predicate "tag is v"); group_reduce of pass v writes
 //      slice v of a composite partial table of V x G groups, series_reduce records where each series first shows v.
 //   3. key_order_kernel / key_perm_kernel put the composite groups into insertion order: the scan order is series by
@@ -3596,14 +3604,8 @@ __global__ void __launch_bounds__(256) key_values_kernel(const __grid_constant__
         while (pi + 1 < p.n_parts && g >= p.parts[pi + 1].block_base) ++pi;
         const DevPartRef &part = p.parts[pi];
         const DevBlock blk = part.blocks[g - part.block_base];
-        // the selection of plan_blocks_kernel
-        uint32_t lo = 0, hi = p.n_series;
-        while (lo < hi) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (p.q_sids[mid] < blk.sid) lo = mid + 1;
-            else hi = mid;
-        }
-        if (!(lo < p.n_series && p.q_sids[lo] == blk.sid) || p.tmin > p.tmax || blk.ts_max < p.tmin || blk.ts_min > p.tmax) continue;
+        int32_t qi;
+        if (!select_block(p.q_sids, p.n_series, p.tmin, p.tmax, blk, qi)) continue;
         DevCol col;
         if (!find_col(part, blk, p.key_name, col, lane)) {
             if (lane == 0) key_insert(p, nullptr, 0, g);  // column absent in this block: every cell is nil (block.go:226-233)
@@ -3673,9 +3675,189 @@ __global__ void key_pack_kernel(const __grid_constant__ KeyParams p) {
     }
 }
 
-void launch_key_values(const KeyParams &p, int grid, cudaStream_t s) {
-    if (p.total_blocks) key_values_kernel<<<grid, 256, 0, s>>>(p);
-    key_pack_kernel<<<1, 32, 0, s>>>(p);
+// ---- int64 key: groupby.go:226-254 appends the 8 little-endian bytes of the value, and a nil cell reaches it as the
+// column's zero value (typed_column.go:49-53), so nil and 0 are one key.  The values have no address in the part, so a slot
+// holds the value itself: 0 marks an empty slot and the value 0 is recorded in a flag word of its own (p.zero).  The home
+// slot is key_insert's, FNV-1a over the 8 key bytes.
+__device__ __forceinline__ uint32_t key_slot_i64(unsigned long long u) {
+    uint64_t h = 0xcbf29ce484222325ull;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) h = (h ^ ((u >> (8 * i)) & 0xffu)) * 0x100000001b3ull;
+    return static_cast<uint32_t>(h ^ (h >> 32)) & (kKeySlots - 1);
+}
+// u enters the table from its home slot s; false = an error was raised (the caller stops inserting)
+__device__ __noinline__ bool key_insert_i64(const KeyParams &p, unsigned long long u, uint32_t s, uint32_t g) {
+    if (u == 0ull) {
+        if (*reinterpret_cast<volatile uint32_t *>(p.zero) != 0u || atomicExch(p.zero, 1u) != 0u) return true;
+        if (atomicAdd(p.count, 1u) < p.cap) return true;
+        key_err(p, kErrKeyCap, g);
+        return false;
+    }
+    for (uint32_t probe = 0; probe < kKeySlots; ++probe) {
+        unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.slots[s]);
+        if (cur == 0ull) {
+            cur = atomicCAS(&p.slots[s], 0ull, u);
+            if (cur == 0ull) {
+                if (atomicAdd(p.count, 1u) < p.cap) return true;
+                key_err(p, kErrKeyCap, g);
+                return false;
+            }
+        }
+        if (cur == u) return true;
+        s = (s + 1) & (kKeySlots - 1);
+    }
+    key_err(p, kErrKeyCap, g);
+    return false;
+}
+
+// Per-warp cache in shared memory of values already in the table, direct-mapped by the home slot: a value that changes
+// every row (the common shape of a status code) then reaches the global table once per warp and slot, not once per row.
+// An entry is written only after its value is in the table, so a hit never skips an insert; lanes racing on an entry at
+// worst cause a miss.
+constexpr uint32_t kKeyCacheSlots = 128;
+constexpr size_t kKeyCacheBytes = sizeof(unsigned long long) * kKeyCacheSlots * kWarpsPerCta;
+
+// the values of one lane: a value equal to the last one this lane entered is skipped (runs), then the warp's cache is asked
+struct KeyI64Cons {
+    const KeyParams *p;
+    volatile unsigned long long *cache;  // [kKeyCacheSlots] of this warp, 0 = empty
+    uint32_t g;
+    bool have, ok, zero_done;
+    int64_t last;
+    __device__ __forceinline__ void put(int64_t v) {
+        if (!ok || (have && v == last)) return;
+        have = true;
+        last = v;
+        const unsigned long long u = static_cast<unsigned long long>(v);
+        if (u == 0ull) {  // the value 0 has its own flag word: once per lane and block
+            if (!zero_done) ok = key_insert_i64(*p, 0ull, 0u, g);
+            zero_done = true;
+            return;
+        }
+        const uint32_t s = key_slot_i64(u);
+        volatile unsigned long long *c = cache + (s & (kKeyCacheSlots - 1));
+        if (*c == u) return;
+        ok = key_insert_i64(*p, u, s, g);
+        if (ok) *c = u;
+    }
+    __device__ __forceinline__ void operator()(uint32_t, int64_t v) { put(v); }
+};
+
+// one warp per selected block: every value of the key tag's int64 page, over all rows of the block
+__global__ void __launch_bounds__(kWarpsPerCta * 32) key_values_i64_kernel(const __grid_constant__ KeyParams p) {
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    WarpSmem *sm = reinterpret_cast<WarpSmem *>(smem_raw) + warp;
+    // the cache follows the warps' WarpSmem slots
+    volatile unsigned long long *cache =
+        reinterpret_cast<unsigned long long *>(smem_raw + sizeof(WarpSmem) * kWarpsPerCta) + static_cast<size_t>(warp) * kKeyCacheSlots;
+    for (uint32_t i = lane; i < kKeyCacheSlots; i += 32) cache[i] = 0ull;
+    if (lane == 0) {
+        sm->fault = 0;
+        sm->seq = 0;
+        for (int s = 0; s < kStages; ++s) mbar_init(&sm->bar[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const uint32_t n_warps = gridDim.x * kWarpsPerCta;
+    for (uint32_t g = blockIdx.x * kWarpsPerCta + warp; g < p.total_blocks; g += n_warps) {
+        uint32_t stop = lane == 0 ? *reinterpret_cast<volatile uint32_t *>(&p.err[0]) : 0u;
+        stop = __shfl_sync(0xffffffffu, stop, 0);
+        if (stop != 0u) return;  // warp-uniform
+        uint32_t pi = 0;
+        while (pi + 1 < p.n_parts && g >= p.parts[pi + 1].block_base) ++pi;
+        const DevPartRef &part = p.parts[pi];
+        const DevBlock blk = part.blocks[g - part.block_base];
+        int32_t qi;
+        if (!select_block(p.q_sids, p.n_series, p.tmin, p.tmax, blk, qi)) continue;
+        KeyI64Cons kc{&p, cache, g, false, true, false, 0};
+        DevCol col;
+        if (!find_col(part, blk, p.key_name, col, lane)) {
+            if (lane == 0) kc.put(0);  // column absent in this block: every cell is nil (block.go:226-233)
+            continue;
+        }
+        const uint8_t *page = part.files[col.file_id] + col.off;
+        const uint32_t count = blk.count;
+        const uint32_t enc = col.size >= 1 ? __ldg(page) : 0u;
+        uint32_t err = kErrNone;
+        if (col.value_type != BYDB_VT_INT64) {
+            err = kErrPredType;
+        } else if (col.size < 1) {
+            err = kErrCorrupt;
+        } else if (enc == kEncRawCells) {
+            if (col.size < 8 + 9ull * count || (reinterpret_cast<uintptr_t>(page) & 7)) {
+                err = kErrCorrupt;
+            } else {
+                const bool nulls = __ldg(page + 1) != 0;
+                const long long *vals = reinterpret_cast<const long long *>(page + 8);
+                const uint8_t *valid = page + 8 + 8ull * count;
+                for (uint32_t row = lane; row < count; row += 32) kc.put(!nulls || __ldg(valid + row) != 0 ? __ldg(vals + row) : 0);
+            }
+        } else if (enc == 9) {
+            err = kErrPlainPage;
+        } else if (col.size < 9) {
+            err = kErrCorrupt;
+        } else {
+            const int64_t first = conv_bytes_to_int64(page + 1);
+            const uint8_t *body = page + 9;
+            const uint32_t blen = col.size - 9;
+            if (enc == 1) {
+                if (blen != 0) err = kErrCorrupt;
+                else if (lane == 0) kc.put(first);
+            } else if (enc == 2) {
+                int64_t d = 0;
+                uint32_t used = 0;
+                if (!read_varint_seq(body, blen, d, used) || used != blen) {
+                    err = kErrCorrupt;
+                } else {
+                    // first + d*r (mod 2^64) repeats after 2^(64 - ctz(d)) rows: d = 2^63 gives two values
+                    const uint64_t ud = static_cast<uint64_t>(d);
+                    const int period_log2 = ud == 0 ? 0 : 64 - (__ffsll(static_cast<long long>(ud)) - 1);
+                    const uint32_t distinct = period_log2 < 32 ? min(count, 1u << period_log2) : count;
+                    if (distinct > p.cap) err = kErrKeyCap;
+                    else
+                        for (uint32_t r = lane; r < distinct; r += 32) kc.put(static_cast<int64_t>(static_cast<uint64_t>(first) + ud * r));
+                }
+            } else if (enc == 3 || enc == 4) {
+                bool ok;
+                if (enc == 3) ok = decode_varint_page<false>(sm, body, blen, count, first, kc, lane);
+                else ok = decode_varint_page<true>(sm, body, blen, count, first, kc, lane);
+                if (!__all_sync(0xffffffffu, ok)) err = kErrCorrupt;
+                else if (sm->fault) err = kErrTmaTimeout;
+            } else {
+                err = kErrBadEnc;
+            }
+        }
+        if (err != kErrNone && lane == 0) key_err(p, err, g);
+    }
+}
+
+// one warp: the value 0 first when it occurs, then the occupied slots in slot order, each as 8 little-endian bytes in vals
+__global__ void key_pack_i64_kernel(const __grid_constant__ KeyParams p) {
+    const int lane = threadIdx.x;
+    unsigned long long *out = reinterpret_cast<unsigned long long *>(p.vals);
+    uint32_t n = *p.zero != 0u ? 1u : 0u;
+    if (lane == 0 && n) out[0] = 0ull;
+    for (uint32_t base = 0; base < kKeySlots; base += 32) {
+        const unsigned long long cur = p.slots[base + lane];
+        const uint32_t bal = __ballot_sync(0xffffffffu, cur != 0ull);
+        const uint32_t at = n + __popc(bal & ((1u << lane) - 1u));
+        if (cur != 0ull && at < p.cap) out[at] = cur;
+        n += __popc(bal);
+    }
+}
+
+static void scan_set_attrs();
+void launch_key_values(const KeyParams &p, bool int64_key, int grid, cudaStream_t s) {
+    if (!int64_key) {
+        if (p.total_blocks) key_values_kernel<<<grid, 256, 0, s>>>(p);
+        key_pack_kernel<<<1, 32, 0, s>>>(p);
+        return;
+    }
+    scan_set_attrs();
+    if (p.total_blocks) key_values_i64_kernel<<<grid, kWarpsPerCta * 32, scan_smem_bytes() + kKeyCacheBytes, s>>>(p);
+    key_pack_i64_kernel<<<1, 32, 0, s>>>(p);
 }
 
 // one warp per composite group (v, g): its first series and the rank of v among that series' values
@@ -3799,6 +3981,7 @@ static void scan_set_attrs() {
     cudaFuncSetAttribute(scan_blocks_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(scan_sum_express_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(express_smem_bytes()));
     cudaFuncSetAttribute(dedup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(key_values_i64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem + static_cast<int>(kKeyCacheBytes));
     if (dev >= 0 && dev < 64) g_attr_set[dev].store(true, std::memory_order_release);
 }
 // express lane (when the query has its shape), fast lane over the planned blocks or what the express lane left, then the
@@ -3970,6 +4153,8 @@ void preload_kernels() {
     cudaFuncAttributes ka;
     (void)cudaFuncGetAttributes(&ka, key_values_kernel);
     (void)cudaFuncGetAttributes(&ka, key_pack_kernel);
+    (void)cudaFuncGetAttributes(&ka, key_values_i64_kernel);
+    (void)cudaFuncGetAttributes(&ka, key_pack_i64_kernel);
     (void)cudaFuncGetAttributes(&ka, key_order_kernel);
     (void)cudaFuncGetAttributes(&ka, key_perm_kernel);
     (void)cudaFuncGetAttributes(&ka, permute_table_kernel);

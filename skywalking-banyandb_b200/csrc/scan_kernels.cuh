@@ -199,13 +199,16 @@ struct KeyParams {
     int64_t tmin, tmax;
     uint16_t key_name;
     uint16_t pad[3];
-    unsigned long long *slots;    // [kKeySlots] 0 = empty, else bit63 | len << 48 | device address of the bytes
+    unsigned long long *slots;    // [kKeySlots] 0 = empty, else bit63 | len << 48 | device address of the bytes;
+                                  // int64 key: 0 = empty, else the value itself
     uint32_t *count;              // distinct values found
     uint32_t *err;                // [2]
-    uint8_t *vals;                // [cap * kMaxLit] packed by key_pack
+    uint32_t *zero;               // int64 key: 1 = the value 0 occurs (it cannot take a slot)
+    uint8_t *vals;                // [cap * kMaxLit] packed by key_pack (int64 key: [cap] values, 8 little-endian bytes each)
     uint32_t *lens;               // [cap]
 };
-void launch_key_values(const KeyParams &p, int grid, cudaStream_t s);
+// int64_key: the key tag is an int64 column (key_values_i64_kernel), else a dictionary string tag (key_values_kernel)
+void launch_key_values(const KeyParams &p, bool int64_key, int grid, cudaStream_t s);
 struct KeyOrderParams {
     int32_t n_groups;             // G: groups of series
     uint32_t n_values;            // V

@@ -8,6 +8,10 @@ into libbydbgpu.so.  Names and contracts follow the reference:
   PullOperator {Init, OutputSchema, NextBatch, Close} pkg/query/vectorized/operator.go:34-52
   output schema = buildAggOutputSchema               aggregation.go:402-418
   Top semantics                                       pkg/query/vectorized/measure/top.go:145-214
+
+A GroupBy key column with per-series values (ScanSpec.series_tags: entity / indexed tags) is densified per series.  At most
+one key column may be a stored tag (a tag column absent from series_tags): the operator then calls bydb_scan_agg_keyed, which adds the
+row's value of that tag to the group (include/bydb_operator.hpp follows the same rules).
 """
 from __future__ import annotations
 
@@ -112,6 +116,17 @@ class ScanSpec:
     order_desc: bool = False
     # ^ orderBy sort of the request: the scan visits the series list backwards, so groups are numbered (and non-key
     #   projected tags take their first-seen value) from the far end -- aggregation.go:211-213 on a reversed stream
+    max_key_values: int = 0
+    # ^ distinct values a stored-tag GroupBy key may take over the query (bydb_group_key.max_values; 0 = the library's 64)
+
+
+def _key_cell(t: ColumnType, k: bytes):
+    """a row's stored-tag key bytes (groupby.go:226-254) as a cell of the key column; a nil cell came back as 0 / \"\" """
+    if t == ColumnType.ColumnTypeInt64:
+        return int.from_bytes(k, "little", signed=True)
+    if t == ColumnType.ColumnTypeString:
+        return k.decode("utf-8", "surrogateescape")
+    return k
 
 
 class GPUScanAgg:
@@ -140,6 +155,7 @@ class GPUScanAgg:
         self._out = BatchSchema(defs)
         self._result: Optional[capi.Result] = None
         self._group_first_series: List[int] = []
+        self._stored_key: Optional[int] = None   # input column of the stored-tag GroupBy key, if any
         self._cursor = 0
         self._closed = False
         self._err: Optional[Exception] = None
@@ -177,6 +193,9 @@ class GPUScanAgg:
         cols: List[object] = []
         for ti in self._tag_idx:
             cdef = self._in.Columns[ti]
+            if ti == self._stored_key:
+                cols.append([_key_cell(cdef.Type, k) for k in r.key[lo:hi]])
+                continue
             vals = self._scan.series_tags.get((cdef.TagFamily, cdef.Name))
             cols.append([None if vals is None else vals[self._group_first_series[g]] for g in r.group_id[lo:hi]])
         for ai, _ in enumerate(self._aggs):
@@ -187,14 +206,24 @@ class GPUScanAgg:
         sc = self._scan
         sids = np.asarray(sc.series_ids, dtype=np.uint64)
         # group key per series = tuple of key-column values; dense ids in first-appearance order
-        # (aggregation.go:211-213; series-major scan order for group-by-entity)
+        # (aggregation.go:211-213; series-major scan order for group-by-entity).  A tag key column without per-series values
+        # is a stored tag: its value changes from row to row, and bydb_scan_agg_keyed adds it to the series group.  Any other
+        # key column (a field) still needs per-series values.
         keyvals = []
+        self._stored_key = None
         for ki in self._keys:
             cdef = self._in.Columns[ki]
             vals = sc.series_tags.get((cdef.TagFamily, cdef.Name))
+            if vals is None and cdef.Role == ColumnRole.RoleTag:
+                if self._stored_key is not None:
+                    raise capi.BydbError(capi.ENOTSUP, f"GroupBy key {cdef.TagFamily}/{cdef.Name}: at most one stored-tag key per query")
+                self._stored_key = ki
+                continue
             if vals is None or len(vals) != len(sids):
                 raise ValueError(f"GroupBy key {cdef.TagFamily}/{cdef.Name} needs one value per series (entity / indexed tag)")
             keyvals.append(vals)
+        if self._stored_key is not None and sc.order_desc:
+            raise capi.BydbError(capi.ENOTSUP, "a stored-tag GroupBy key takes the ascending series order only (order_desc)")
         group_of: Dict[tuple, int] = {}
         gids = np.zeros(len(sids), dtype=np.int32)
         self._group_first_series = []
@@ -215,7 +244,12 @@ class GPUScanAgg:
                        top_desc=self._top.Desc if self._top else True)
         if not self._keys:
             self._group_first_series = ([len(sids) - 1] if sc.order_desc else [0]) if len(sids) else []
-        self._result = self._ctx.scan_agg(q)
+        if self._stored_key is None:
+            self._result = self._ctx.scan_agg(q)
+        else:
+            cdef = self._in.Columns[self._stored_key]
+            vt = capi.VT_INT64 if cdef.Type == ColumnType.ColumnTypeInt64 else 0
+            self._result = self._ctx.scan_agg_keyed(q, cdef.TagFamily, cdef.Name, sc.max_key_values, vt)
         self.stats = self._result.stats
         # offset / limit window over the (Top-ordered) output rows, limit.go:56-73
         n = len(self._result.group_id)
