@@ -208,8 +208,8 @@ int bydb_scan_agg(bydb_ctx *ctx, const bydb_query *q, bydb_result *out);
  * range), before the time trim and the predicates.  More than max_values of them give BYDB_ENOMEM (the reference's
  * aggregation memory budget).  Device side: one pass collects the distinct values, then ONE SCAN PASS PER VALUE (the key as
  * an extra predicate) fills that value's slice of a composite partial table; stats count every pass.  A group-key query
- * takes at most 7 predicates of its own.  Not available through the prepared / partial-table / multi-GPU entry points,
- * and not over parts that overlap in time. */
+ * takes at most 7 predicates of its own.  Not available through the prepared / partial-table entry points, and not over
+ * parts that overlap in time; its multi-GPU form is bydb_scan_reduce_keyed (below). */
 typedef struct {
     const char *family;    /* tag family of the key tag                                      */
     const char *tag;       /* tag name                                                       */
@@ -355,6 +355,29 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *pq, int32_t root, by
  * the duration of the call (with BYDB_Q_HOST_ZERO_COPY only the block directory is uploaded and the scan pulls the pages it
  * touches over PCIe), scanned into the root's mailbox, dropped.  q->parts / q->n_parts are ignored. */
 int bydb_scan_reduce_host(bydb_ctx *ctx, uint32_t n_parts, const bydb_part_files *parts, const bydb_query *q, int32_t root, bydb_result *out);
+
+/* Group-by on a stored tag over the same peer mailboxes: the collective form of bydb_scan_agg_keyed.  Every rank runs key
+ * discovery and one scan pass per key value over ITS parts, straight into its slot of the root's mailbox; the root builds the
+ * union of the ranks' values, combines their composite tables in rank order (deterministic float sums) and finalises once.
+ *   - Every rank passes the SAME series_ids, series_group, n_groups, tmin / tmax, predicates, aggregations, Top-N, flags and
+ *     *key (max_values included); only `parts` differ -- they are the rank's shard.  A rank that selects no block of a series
+ *     contributes nothing to it.  Each rank hashes those fields; a rank whose hash differs from the root's makes the root fail
+ *     with BYDB_EINVAL.
+ *   - The root's answer is the answer of bydb_scan_agg_keyed over all ranks' parts: rows in insertion order of the whole scan
+ *     (or Top-N order, ties to the group inserted first); n_keys counts the distinct values over all ranks' selected blocks, and
+ *     more than max_values of them give BYDB_ENOMEM even when every rank alone is under the cap.  The order of the key table
+ *     (key_off / key_bytes) is not part of the contract: identify rows by their key bytes.
+ *   - Non-root ranks get n_rows = 0, n_keys = 0 and their own scan statistics.
+ *   - Within a rank the rules of bydb_scan_agg_keyed hold (its parts must not overlap in time: BYDB_ENOTSUP; same caps, key-type
+ *     errors and predicate limit).  Across ranks, one series may live on several ranks only over time spans that do not
+ *     intersect -- the span being the series' selected blocks clipped to [tmin, tmax] -- which covers sharding by series range
+ *     and by time window; an intersection makes the root fail with BYDB_ENOTSUP naming the series.
+ *   - A rank whose slot is too small for its value count fails with BYDB_EINVAL (and so does the root).  Every failure keeps the
+ *     ranks' epochs in step: keyed and plain collectives may alternate, with any roots.
+ * Size the mailboxes with bydb_keyed_reduce_slot_bytes (host only, like bydb_partials_layout): the slot a rank needs at
+ * max_values key values; pass it (or the largest over the queries to come) to bydb_comm_export as max_table_bytes. */
+int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t *out);
+int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out);
 
 const char *bydb_last_error(void);
 const char *bydb_version(void);

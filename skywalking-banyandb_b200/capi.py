@@ -105,6 +105,7 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_query_release", "bydb_partials_layout",
            "bydb_scan_partials", "bydb_partials_combine", "bydb_reduce_finalize", "bydb_partials_rows", "bydb_partial_rows_free", "bydb_comm_export", "bydb_comm_connect",
            "bydb_scan_reduce", "bydb_scan_reduce_prepared", "bydb_scan_reduce_host", "bydb_scan_agg_keyed", "bydb_keyed_result_free",
+           "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -159,6 +160,8 @@ def load_library():
     L.bydb_scan_reduce.argtypes = [C.c_void_p, C.POINTER(_Query), C.c_int32, C.POINTER(_Result)]
     L.bydb_scan_reduce_prepared.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(_Result)]
     L.bydb_scan_reduce_host.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(_PartFiles), C.POINTER(_Query), C.c_int32, C.POINTER(_Result)]
+    L.bydb_keyed_reduce_slot_bytes.argtypes = [C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(C.c_uint64)]
+    L.bydb_scan_reduce_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32, C.POINTER(_KeyedResult)]
     _lib = L
     return L
 
@@ -368,6 +371,16 @@ class GraphQuery:
             self._h = None
 
 
+def keyed_reduce_slot_bytes(q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> int:
+    """bydb_keyed_reduce_slot_bytes (host only): the mailbox slot a rank of a keyed collective needs at max_values key values."""
+    keep: list = []
+    cq = _mk_query(q, keep)
+    gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+    out = C.c_uint64()
+    _check(load_library().bydb_keyed_reduce_slot_bytes(C.byref(cq), C.byref(gk), C.byref(out)))
+    return out.value
+
+
 class Context:
     """bydb_ctx: one device, its streams and the HBM part cache."""
 
@@ -441,6 +454,9 @@ class Context:
         gk = _GroupKey(fb, tb, max_values, value_type)
         r = _KeyedResult()
         _check(self._L.bydb_scan_agg_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
+        return self._read_keyed(q, r)
+
+    def _read_keyed(self, q: Query, r: "_KeyedResult") -> Result:
         try:
             if r.base.n_rows == 0 and not r.base.owner:
                 a = len(q.aggs)
@@ -565,6 +581,20 @@ class Context:
             return _read_result(r)
         finally:
             self._L.bydb_result_free(self._h, C.byref(r))
+
+    def keyed_reduce_slot_bytes(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> int:
+        """Mailbox slot bytes a keyed collective needs (bydb_keyed_reduce_slot_bytes): pass it to comm_export."""
+        return keyed_reduce_slot_bytes(q, family, tag, max_values, value_type)
+
+    def scan_reduce_keyed(self, q: Query, family: str, tag: str, root: int = 0, max_values: int = 0, value_type: int = 0) -> Result:
+        """Collective group-by on a stored tag (bydb_scan_reduce_keyed): every rank passes the same query but its parts.  The
+        root gets scan_agg_keyed's answer over all ranks' parts; the others an empty result with their own scan statistics."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        r = _KeyedResult()
+        _check(self._L.bydb_scan_reduce_keyed(self._h, C.byref(cq), C.byref(gk), root, C.byref(r)))
+        return self._read_keyed(q, r)
 
     def partials_combine(self, q, d_ptr: int, n_tables: int, bytes_each: int, stream: int = 0) -> None:
         cq, keep = _cq(q)

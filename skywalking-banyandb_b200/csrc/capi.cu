@@ -316,6 +316,7 @@ const char *dev_err_text(uint32_t code) {
         case kErrPeerTimeout: return "multi-GPU reduce: a peer rank did not deliver its partial table in time";
         case kErrKeyCap: return "per-row group key: more distinct key values than bydb_group_key.max_values";
         case kErrKeyLong: return "per-row group key: a key value longer than 64 bytes";
+        case kErrRankOverlap: return "keyed collective: a series lives on several ranks over time spans that intersect";
     }
     return "unknown device error";
 }
@@ -904,6 +905,7 @@ struct KeyedPass {
     int64_t *coltype;   // [F] the pass's own column types + status (merged by permute_table)
     int64_t *kts;       // [n_series] see ReduceParams::Kts
     uint32_t *krow;     // [n_series]
+    int64_t *span;      // [2 * n_series] see ReduceParams::span, or NULL
 };
 
 int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cudaStream_t stream, uint8_t *d_table, const TableLayout &tl,
@@ -1019,6 +1021,7 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
         rp.Pfirst = sp.Pfirst;
         rp.Kts = kp->kts;
         rp.Krow = kp->krow;
+        rp.span = kp->span;
     }
     set_table(rp, table);
 
@@ -1633,40 +1636,25 @@ struct KeyedOwner {
     std::vector<uint32_t> key_off;
     std::vector<uint8_t> key_bytes;
 };
-}  // namespace
+using KeyValues = std::vector<std::vector<uint8_t>>;
 
-void bydb_keyed_result_free(bydb_ctx *ctx, bydb_keyed_result *r);
-void bydb_encoded_pages_free(bydb_ctx *ctx, bydb_encoded_pages *r);
-
-// Group-by on a stored tag (per-row key): see "Group key" in scan_kernels.cu for the device side.
-int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out) {
-    return guarded([&]() -> int {
-    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
-    memset(out, 0, sizeof *out);
-    int rc = validate_query(q, true);
-    if (rc) return rc;
+// the checks of a group key that need no device; cap = the distinct values accepted (max_values, 0 = 64)
+int check_group_key(const bydb_query *q, const bydb_group_key *key, uint32_t &cap) {
     if (!key || !key->family || !key->tag) return fail(BYDB_EINVAL, "group key without family/tag");
     if (key->value_type != 0 && key->value_type != BYDB_VT_STR && key->value_type != BYDB_VT_BINARY && key->value_type != BYDB_VT_INT64)
         return fail(BYDB_EINVAL, "bydb_group_key.value_type must be 0, BYDB_VT_STR, BYDB_VT_BINARY or BYDB_VT_INT64");
-    const bool int64_key = key->value_type == BYDB_VT_INT64;
-    const uint32_t cap = key->max_values ? key->max_values : 64u;
+    cap = key->max_values ? key->max_values : 64u;
     if (cap > kMaxKeyValues) return fail(BYDB_EINVAL, "bydb_group_key.max_values above 256");
     if (q->n_preds + 1 > kMaxPreds) return fail(BYDB_ENOTSUP, "a group-key query takes at most 7 predicates");
-    g_last_dev_err = 0;
-    Plan plan;
-    rc = make_plan(ctx, q, nullptr, plan);
-    if (rc) return rc;
-    if (parts_overlap(plan.parts, q->tmin, q->tmax))
-        return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    SlotLease lease(ctx);
-    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
-    ExecSlot &slot = *lease.slot;
-    cudaStream_t stream = slot.stream;
-    const size_t F = plan.fcols.size(), NS = q->n_series, NB = plan.total_blocks, G = static_cast<size_t>(plan.n_groups);
-    memset(&out->base.stats, 0, sizeof out->base.stats);
+    return 0;
+}
 
-    // ---- 1. the distinct key values of the selected blocks
+// 1. the distinct key values of the selected blocks, on the slot's stream, synchronised
+int discover_keys(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats *stats,
+                  KeyValues &values) {
+    const bool int64_key = key->value_type == BYDB_VT_INT64;
+    const size_t NS = q->n_series, NB = plan.total_blocks;
+    cudaStream_t stream = slot.stream;
     size_t o = 0;
     auto carve = [&](size_t bytes) {
         size_t at = o;
@@ -1693,7 +1681,10 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     kpar.cap = cap;
     kpar.tmin = q->tmin;
     kpar.tmax = q->tmax;
-    kpar.key_name = ctx->names.find(std::string("t:") + key->family + "/" + key->tag);
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        kpar.key_name = ctx->names.find(std::string("t:") + key->family + "/" + key->tag);
+    }
     kpar.slots = reinterpret_cast<unsigned long long *>(ka.base + a_slots);
     kpar.count = reinterpret_cast<uint32_t *>(ka.base + a_ctl);
     kpar.err = reinterpret_cast<uint32_t *>(ka.base + a_ctl) + 1;
@@ -1705,9 +1696,9 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     CUDA_TRY(cudaMemcpyAsync(slot.pinned, ka.base + a_ctl, back_bytes, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     CUDA_TRY(cudaGetLastError());
-    out->base.stats.kernel_launches += 2;
-    out->base.stats.h2d_bytes += NS * 8;
-    out->base.stats.d2h_bytes += back_bytes;
+    stats->kernel_launches += 2;
+    stats->h2d_bytes += NS * 8;
+    stats->d2h_bytes += back_bytes;
     const uint32_t *ctl = reinterpret_cast<const uint32_t *>(slot.pinned);
     if (ctl[1] != 0) {
         g_last_dev_err = ctl[1];
@@ -1716,57 +1707,28 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
         return fail(dev_err_code(ctl[1]), std::string(dev_err_text(ctl[1])) + buf);
     }
     const size_t V = std::min<size_t>(ctl[0], cap);
-    std::vector<std::vector<uint8_t>> values(V);
-    {
-        const uint8_t *hv = slot.pinned + (a_vals - a_ctl);
-        const uint32_t *hl = reinterpret_cast<const uint32_t *>(slot.pinned + (a_lens - a_ctl));
-        for (size_t v = 0; v < V; ++v) {
-            if (int64_key) values[v].assign(hv + v * 8, hv + v * 8 + 8);  // the reference's key bytes: little-endian int64
-            else values[v].assign(hv + v * kMaxLit, hv + v * kMaxLit + hl[v]);
-        }
-    }
-    auto owner = new KeyedOwner();
-    out->owner = owner;
-    bool done = false;
-    struct Undo {  // a failure past this point must not leave a half-filled result with the caller
-        bydb_ctx *ctx;
-        bydb_keyed_result *out;
-        bool *done;
-        ~Undo() {
-            if (!*done) bydb_keyed_result_free(ctx, out);
-        }
-    } undo{ctx, out, &done};
-    owner->key_off.push_back(0);
+    values.assign(V, {});
+    const uint8_t *hv = slot.pinned + (a_vals - a_ctl);
+    const uint32_t *hl = reinterpret_cast<const uint32_t *>(slot.pinned + (a_lens - a_ctl));
     for (size_t v = 0; v < V; ++v) {
-        owner->key_bytes.insert(owner->key_bytes.end(), values[v].begin(), values[v].end());
-        owner->key_off.push_back(static_cast<uint32_t>(owner->key_bytes.size()));
+        if (int64_key) values[v].assign(hv + v * 8, hv + v * 8 + 8);  // the reference's key bytes: little-endian int64
+        else values[v].assign(hv + v * kMaxLit, hv + v * kMaxLit + hl[v]);
     }
-    if (owner->key_bytes.empty()) owner->key_bytes.push_back(0);
-    out->n_keys = static_cast<int32_t>(V);
-    out->key_off = owner->key_off.data();
-    out->key_bytes = owner->key_bytes.data();
-    if (V == 0) {  // no block selected: no rows (n_rows = 0)
-        done = true;
-        return 0;
-    }
+    return 0;
+}
 
-    // ---- 2. one scan pass per value into slice v of the composite table (V x G groups, value-major)
-    const size_t GP = G * V;
-    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
-    TableLayout tlc(GP, F);
-    o = 0;
-    const size_t b_src = carve(tlc.total), b_dst = carve(tlc.total), b_ct = carve(V * F * 8), b_kts = carve(V * NS * 8), b_krow = carve(V * NS * 4),
-                 b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16);
-    Scratch kb;
-    CUDA_TRY(kb.alloc(o, stream));
-    CUDA_TRY(cudaMemsetAsync(kb.base + b_ct, 0, V * F * 8, stream));
-    CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
-    if (slot.ensure_pinned(step_pinned_bytes(q, G, GP))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+// 2. one scan pass per value v (the key as an extra predicate) into slice v of the composite table tlc (V x G groups, value-major)
+// at `table`, with the pass's column types at coltype + v * F and where each series first shows v at kts / krow + v * NS; the
+// first pass also writes the series' spans when `span` is set.  Every pass is synchronised and its device errors collected.
+int run_keyed_passes(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Plan &plan, ExecSlot &slot, const KeyValues &values,
+                     const TableLayout &tlc, uint8_t *table, int64_t *coltype, int64_t *kts, uint32_t *krow, int64_t *span, bydb_stats *stats) {
+    const bool int64_key = key->value_type == BYDB_VT_INT64;
+    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
     std::vector<bydb_pred> preds(q->preds, q->preds + q->n_preds);
     preds.emplace_back();
     bydb_query qv = *q;
     qv.n_preds = q->n_preds + 1;
-    for (size_t v = 0; v < V; ++v) {
+    for (size_t v = 0; v < values.size(); ++v) {
         bydb_pred &kpred = preds.back();
         memset(&kpred, 0, sizeof kpred);
         kpred.family = key->family;
@@ -1786,44 +1748,76 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
         qv.preds = preds.data();
         KeyedPass pass;
         pass.group_off = v * G;
-        pass.coltype = reinterpret_cast<int64_t *>(kb.base + b_ct) + v * F;
-        pass.kts = reinterpret_cast<int64_t *>(kb.base + b_kts) + v * NS;
-        pass.krow = reinterpret_cast<uint32_t *>(kb.base + b_krow) + v * NS;
-        rc = run_scan(ctx, &qv, plan, slot, stream, kb.base + b_src, tlc, &out->base.stats, 0, &pass);
-        cudaError_t ce = cudaStreamSynchronize(stream);  // also on failure: nothing may be in flight when the slot goes back
+        pass.coltype = coltype + v * F;
+        pass.kts = kts + v * NS;
+        pass.krow = krow + v * NS;
+        pass.span = v == 0 ? span : nullptr;
+        int rc = run_scan(ctx, &qv, plan, slot, slot.stream, table, tlc, stats, 0, &pass);
+        cudaError_t ce = cudaStreamSynchronize(slot.stream);  // also on failure: nothing may be in flight when the slot goes back
         if (!rc && ce != cudaSuccess) rc = fail(BYDB_EIO, cudaGetErrorString(ce));
-        if (!rc) rc = collect_scan(slot, &out->base.stats);
+        if (!rc) rc = collect_scan(slot, stats);
         if (rc) return rc;
     }
+    return 0;
+}
 
-    // ---- 3. insertion order of the composite groups, table reordered, ordinary finalisation / Top-N on it
+// the key table of a keyed result: value k is `values[k]`
+void set_key_table(bydb_keyed_result *out, KeyedOwner *owner, const KeyValues &values) {
+    owner->key_off.assign(1, 0);
+    owner->key_bytes.clear();
+    for (const auto &v : values) {
+        owner->key_bytes.insert(owner->key_bytes.end(), v.begin(), v.end());
+        owner->key_off.push_back(static_cast<uint32_t>(owner->key_bytes.size()));
+    }
+    if (owner->key_bytes.empty()) owner->key_bytes.push_back(0);
+    out->n_keys = static_cast<int32_t>(values.size());
+    out->key_off = owner->key_off.data();
+    out->key_bytes = owner->key_bytes.data();
+}
+
+// 3. insertion order of the V x G composite groups from where each series first shows each value (kts / krow), the table at
+// `table` reordered, the ordinary finalisation / Top-N on it, and the rows mapped back to (series group, key value).  The
+// caller sized the slot's pinned staging with step_pinned_bytes(q, G, V * G).
+int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
+                 const int64_t *kts, const uint32_t *krow, bydb_keyed_result *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    const StageLayout st = stage_layout(NS, G);
+    size_t o = 0;
+    auto carve = [&](size_t bytes) {
+        size_t at = o;
+        o = align_up(o + bytes, 256);
+        return at;
+    };
+    const size_t b_dst = carve(tlc.total), b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16),
+                 b_stage = carve(st.bytes);
+    Scratch kb;
+    CUDA_TRY(kb.alloc(o, stream));
+    CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
     KeyOrderParams ko;
     memset(&ko, 0, sizeof ko);
     ko.n_groups = static_cast<int32_t>(G);
     ko.n_values = static_cast<uint32_t>(V);
     ko.n_series = static_cast<uint32_t>(NS);
     // order | group_start of the series groups: staged again (run_scan's copies live in its own scratch)
-    const StageLayout st = stage_layout(NS, G);
-    Scratch kc;
-    CUDA_TRY(kc.alloc(st.bytes, stream));
     stage_series(q, st, slot.pinned);
-    CUDA_TRY(cudaMemcpyAsync(kc.base, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream));
-    ko.order = reinterpret_cast<const int32_t *>(kc.base + st.off_order);
-    ko.group_start = reinterpret_cast<const int32_t *>(kc.base + st.off_gstart);
-    ko.Kts = reinterpret_cast<const int64_t *>(kb.base + b_kts);
-    ko.Krow = reinterpret_cast<const uint32_t *>(kb.base + b_krow);
+    CUDA_TRY(cudaMemcpyAsync(kb.base + b_stage, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream));
+    ko.order = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_order);
+    ko.group_start = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_gstart);
+    ko.Kts = kts;
+    ko.Krow = krow;
     ko.slot = reinterpret_cast<int32_t *>(kb.base + b_slot);
     ko.first_series = reinterpret_cast<int32_t *>(kb.base + b_first);
     ko.perm = reinterpret_cast<int32_t *>(kb.base + b_perm);
     ko.n_present = reinterpret_cast<uint32_t *>(kb.base + b_np);
     launch_key_order(ko, stream);
-    launch_permute_table(tlc.at(kb.base + b_dst), tlc.at(kb.base + b_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F),
-                         reinterpret_cast<const int64_t *>(kb.base + b_ct), static_cast<uint32_t>(V), stream);
+    launch_permute_table(tlc.at(kb.base + b_dst), tlc.at(table), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), coltype,
+                         static_cast<uint32_t>(V), stream);
     CUDA_TRY(cudaStreamSynchronize(stream));  // the staging above is reused by the finalisation's read-back
     out->base.stats.kernel_launches += 3;
     Plan planc = plan;
     planc.n_groups = static_cast<int32_t>(GP);
-    rc = finalize_to_host(q, planc, slot, stream, kb.base + b_dst, tlc, &out->base, true);
+    int rc = finalize_to_host(q, planc, slot, stream, kb.base + b_dst, tlc, &out->base, true);
     if (rc) {
         cudaStreamSynchronize(stream);
         return rc;
@@ -1841,7 +1835,79 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
         ro->group_id[r] = comp % static_cast<int32_t>(G);
     }
     out->key_id = owner->key_id.data();
-    done = true;
+    return 0;
+}
+
+// a failure past the point where the result owns memory must not leave a half-filled result with the caller
+struct KeyedUndo {
+    bydb_ctx *ctx;
+    bydb_keyed_result *out;
+    bool done = false;
+    ~KeyedUndo() {
+        if (!done) bydb_keyed_result_free(ctx, out);
+    }
+};
+}  // namespace
+
+void bydb_encoded_pages_free(bydb_ctx *ctx, bydb_encoded_pages *r);
+
+// Group-by on a stored tag (per-row key): see "Group key" in scan_kernels.cu for the device side.
+int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out) {
+    return guarded([&]() -> int {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    memset(out, 0, sizeof *out);
+    int rc = validate_query(q, true);
+    if (rc) return rc;
+    uint32_t cap = 0;
+    rc = check_group_key(q, key, cap);
+    if (rc) return rc;
+    g_last_dev_err = 0;
+    Plan plan;
+    rc = make_plan(ctx, q, nullptr, plan);
+    if (rc) return rc;
+    if (parts_overlap(plan.parts, q->tmin, q->tmax))
+        return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    SlotLease lease(ctx);
+    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
+    ExecSlot &slot = *lease.slot;
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
+    memset(&out->base.stats, 0, sizeof out->base.stats);
+
+    KeyValues values;
+    rc = discover_keys(ctx, q, key, cap, plan, slot, &out->base.stats, values);
+    if (rc) return rc;
+    const size_t V = values.size();
+    auto owner = new KeyedOwner();
+    out->owner = owner;
+    KeyedUndo undo{ctx, out};
+    set_key_table(out, owner, values);
+    if (V == 0) {  // no block selected: no rows (n_rows = 0)
+        undo.done = true;
+        return 0;
+    }
+
+    const size_t GP = G * V;
+    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
+    TableLayout tlc(GP, F);
+    size_t o = 0;
+    auto carve = [&](size_t bytes) {
+        size_t at = o;
+        o = align_up(o + bytes, 256);
+        return at;
+    };
+    const size_t b_src = carve(tlc.total), b_ct = carve(V * F * 8), b_kts = carve(V * NS * 8), b_krow = carve(V * NS * 4);
+    Scratch kb;
+    CUDA_TRY(kb.alloc(o, stream));
+    CUDA_TRY(cudaMemsetAsync(kb.base + b_ct, 0, V * F * 8, stream));
+    if (slot.ensure_pinned(step_pinned_bytes(q, G, GP))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    int64_t *ct = reinterpret_cast<int64_t *>(kb.base + b_ct), *kts = reinterpret_cast<int64_t *>(kb.base + b_kts);
+    uint32_t *krow = reinterpret_cast<uint32_t *>(kb.base + b_krow);
+    rc = run_keyed_passes(ctx, q, key, plan, slot, values, tlc, kb.base + b_src, ct, kts, krow, nullptr, &out->base.stats);
+    if (!rc) rc = keyed_finish(q, plan, slot, V, kb.base + b_src, tlc, ct, kts, krow, out, owner);
+    if (rc) return rc;
+    undo.done = true;
     return 0;
     });
 }
@@ -2707,8 +2773,6 @@ int bydb_comm_connect(bydb_ctx *ctx, int32_t rank, int32_t nranks, const bydb_co
     });
 }
 
-// given: the parts to scan instead of q->parts (the host-buffer form); pre_rc: a failure that already happened on this
-// rank (its transient parts could not be admitted) -- the rank still takes part in the collective and reports it
 // Host-side form of comm_wait_kernel for ranks that share a device (Comm::shared_device): polls n words until all have reached
 // `epoch`; bounded like the kernel (60 s).  Returns 0 or kErrPeerTimeout.
 static uint32_t comm_wait_host(Comm &cm, const unsigned long long *dev_words, uint32_t n, unsigned long long epoch) {
@@ -2728,9 +2792,29 @@ static uint32_t comm_wait_host(Comm &cm, const unsigned long long *dev_words, ui
     }
 }
 
-static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::shared_ptr<Part>> *given, int pre_rc, uint64_t h2d_pre, int32_t root,
-                            bydb_result *out) {
-    {
+// One collective call of the peer-mailbox reduce, shared by bydb_scan_reduce and bydb_scan_reduce_keyed: the epoch and slot
+// parity, the wait for the slots' previous use, this rank's status word and arrival flag, on the root the wait for every rank
+// and the `done` word, and the outcome, most specific first.  What differs between the two forms comes in as hooks:
+//   prepare(es, slot_bytes)     host-side work before the slots' previous use is awaited: validation, planning, sizing, the
+//                               pinned staging (no page-locked allocation may follow: see ExecSlot::kInitialPinned)
+//   contribute(es, my_slot)     this rank's share, on es.stream, into its slot of the root's mailbox
+//   collect(es)                 once the stream is synchronised: this rank's own device-side errors and counters
+//   reduce(es, slots0, slot_bytes, settle, finalized)
+//                               root only, enqueued behind the wait for every rank: combine and finalise into the result
+//                               (finalized = it holds memory).  settle() synchronises and returns the first failure of any
+//                               rank; a reduce that must not read a failed rank's slot calls it first
+//   discard()                   frees the result when a later check fails
+// pre_rc: a failure that already happened on this rank (its transient parts could not be admitted) -- the rank still takes
+// part in the collective and reports it.
+struct CollectiveHooks {
+    std::function<int(ExecSlot &, size_t)> prepare;
+    std::function<int(ExecSlot &, uint8_t *)> contribute;
+    std::function<int(ExecSlot &)> collect;
+    std::function<int(ExecSlot &, uint8_t *, size_t, const std::function<int()> &, bool &)> reduce;
+    std::function<void()> discard;
+};
+
+static int run_collective(bydb_ctx *ctx, int32_t root, int pre_rc, const CollectiveHooks &h) {
     const std::string pre_msg = pre_rc ? g_last_error : std::string();
     Comm &cm = ctx->comm;
     std::lock_guard<std::mutex> lk(cm.mu);
@@ -2753,14 +2837,7 @@ static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vecto
     unsigned long long *status = reinterpret_cast<unsigned long long *>(root_mb + kCommStatusOff);
     unsigned long long *done = reinterpret_cast<unsigned long long *>(root_mb + kCommDoneOff);
     uint32_t *my_err = reinterpret_cast<uint32_t *>(cm.mine + kCommErrOff);
-    Plan plan;
-    int rc = pre_rc ? fail(pre_rc, pre_msg) : validate_query(q, given == nullptr);
-    if (!rc) rc = make_plan(ctx, q, given, plan);
-    TableLayout tl(static_cast<size_t>(rc ? 1 : plan.n_groups), rc ? 1 : plan.fcols.size());
-    if (!rc && tl.total > slot) rc = fail(BYDB_EINVAL, "partial table larger than the mailbox slots (bydb_comm_export max_table_bytes)");
-    if (!rc && es.ensure_pinned(step_pinned_bytes(q, tl.G, tl.G))) rc = fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    memset(&out->stats, 0, sizeof out->stats);
-    out->stats.h2d_bytes = h2d_pre;
+    int rc = pre_rc ? fail(pre_rc, pre_msg) : h.prepare(es, slot);
     // the slots' previous use -- the last collective with THIS root and parity, the same epoch on every rank -- must have been
     // consumed by the root (its `done` word only ever grows) before they are overwritten
     const uint64_t prev_use = cm.last_use[2 * static_cast<size_t>(root) + parity];
@@ -2770,29 +2847,40 @@ static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vecto
         if (cm.shared_device) host_perr = comm_wait_host(cm, done, 1, prev_use);
         else launch_comm_wait(done, 1, prev_use, my_err, kErrPeerTimeout, s);
     }
-    // map: this rank's group_reduce writes the table straight into the root's memory (P2P stores over NVLink)
-    if (!rc) rc = run_scan(ctx, q, plan, es, s, my_slot, tl, &out->stats);
+    if (!rc) rc = h.contribute(es, my_slot);
     const std::string my_msg = rc ? g_last_error : std::string();
     const unsigned long long st_word = (epoch << 32) | static_cast<unsigned long long>(static_cast<uint32_t>(-rc));
     cudaMemcpyAsync(status + cm.rank, &st_word, sizeof st_word, cudaMemcpyHostToDevice, s);  // pageable source: staged before the call returns
     launch_comm_signal(flags + cm.rank, epoch, s);
     unsigned long long peer_status[kCommMaxRanks] = {0};
+    // the first failure of a rank, from the status words the root holds
+    auto peer_failure = [&]() -> int {
+        for (int r = 0; r < cm.nranks; ++r) {
+            const unsigned long long w = peer_status[r];
+            if ((w >> 32) == (epoch & 0xffffffffull) && static_cast<uint32_t>(w) != 0)
+                return fail(-static_cast<int>(static_cast<uint32_t>(w)), "multi-GPU reduce: rank " + std::to_string(r) + " failed on its side of the collective");
+        }
+        return 0;
+    };
     bool finalized = false;
     int frc = 0;
     if (cm.rank == root) {
-        // reduce: wait for every rank's table, combine in rank order (deterministic float sums), finalise
+        // reduce: wait for every rank's share, then the form's own combine and finalisation
         if (cm.shared_device) {
-            const uint32_t e2 = comm_wait_host(cm, flags, static_cast<uint32_t>(cm.nranks), epoch);  // own flag included: own table is complete
+            const uint32_t e2 = comm_wait_host(cm, flags, static_cast<uint32_t>(cm.nranks), epoch);  // own flag included: own share is complete
             host_perr = host_perr ? host_perr : e2;
         } else {
             launch_comm_wait(flags, static_cast<uint32_t>(cm.nranks), epoch, my_err, kErrPeerTimeout, s);
         }
-        if (!rc) {
-            launch_combine_tables(slots0, static_cast<uint32_t>(cm.nranks), tl, s, slot);
-            out->stats.kernel_launches += 3;
-            frc = finalize_to_host(q, plan, es, s, slots0, tl, out, true);  // synchronises
-            finalized = frc == 0;
-        }
+        const std::function<int()> settle = [&]() -> int {
+            cudaStreamSynchronize(s);
+            uint32_t e = 0;
+            if (cudaMemcpy(&e, my_err, sizeof e, cudaMemcpyDeviceToHost) != cudaSuccess || e == 0) e = host_perr;
+            if (e) return fail(dev_err_code(e), dev_err_text(e));
+            cudaMemcpy(peer_status, status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost);
+            return peer_failure();
+        };
+        if (!rc) frc = h.reduce(es, slots0, slot, settle, finalized);
         cudaStreamSynchronize(s);
         cudaMemcpy(peer_status, status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost);
         // the slots of this parity are free again: nothing reads them any more
@@ -2802,24 +2890,267 @@ static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vecto
     uint32_t perr = 0;
     if (cudaMemcpy(&perr, my_err, sizeof perr, cudaMemcpyDeviceToHost) == cudaSuccess && perr != 0) cudaMemset(my_err, 0, sizeof perr);
     if (!perr) perr = host_perr;
-    // ---- outcome, most specific first: this rank's own host-side failure, its device-side scan error, a peer's failure
+    // ---- outcome, most specific first: this rank's own host-side failure, its device-side errors, a peer's failure
     if (rc) {
-        if (finalized) bydb_result_free(ctx, out);
+        if (finalized) h.discard();
         return fail(rc, my_msg);
     }
-    int crc = collect_scan(es, &out->stats);
+    int crc = h.collect(es);
     if (!crc && perr) crc = fail(dev_err_code(perr), dev_err_text(perr));
     if (!crc && cm.rank == root) {
-        for (int r = 0; r < cm.nranks && !crc; ++r) {
-            const unsigned long long w = peer_status[r];
-            if ((w >> 32) == (epoch & 0xffffffffull) && static_cast<uint32_t>(w) != 0)
-                crc = fail(-static_cast<int>(static_cast<uint32_t>(w)), "multi-GPU reduce: rank " + std::to_string(r) + " failed before its scan");
-        }
+        crc = peer_failure();
         if (!crc) crc = frc;
     }
-    if (crc && finalized) bydb_result_free(ctx, out);
+    if (crc && finalized) h.discard();
     return crc;
+}
+
+// given: the parts to scan instead of q->parts (the host-buffer form); pre_rc: see run_collective
+static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::shared_ptr<Part>> *given, int pre_rc, uint64_t h2d_pre, int32_t root,
+                            bydb_result *out) {
+    Plan plan;
+    TableLayout tl(1, 1);
+    memset(&out->stats, 0, sizeof out->stats);
+    out->stats.h2d_bytes = h2d_pre;
+    CollectiveHooks h;
+    h.prepare = [&](ExecSlot &es, size_t slot) -> int {
+        int rc = validate_query(q, given == nullptr);
+        if (!rc) rc = make_plan(ctx, q, given, plan);
+        if (rc) return rc;
+        tl = TableLayout(static_cast<size_t>(plan.n_groups), plan.fcols.size());
+        if (tl.total > slot) return fail(BYDB_EINVAL, "partial table larger than the mailbox slots (bydb_comm_export max_table_bytes)");
+        if (es.ensure_pinned(step_pinned_bytes(q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+        return 0;
+    };
+    // map: this rank's group_reduce writes the table straight into the root's memory (P2P stores over NVLink)
+    h.contribute = [&](ExecSlot &es, uint8_t *my_slot) { return run_scan(ctx, q, plan, es, es.stream, my_slot, tl, &out->stats); };
+    h.collect = [&](ExecSlot &es) { return collect_scan(es, &out->stats); };
+    // reduce: combine the slots in rank order (deterministic float sums), finalise; a failed rank's status travels in its table
+    h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &, bool &finalized) -> int {
+        launch_combine_tables(slots0, static_cast<uint32_t>(ctx->comm.nranks), tl, es.stream, slot);
+        out->stats.kernel_launches += 3;
+        const int frc = finalize_to_host(q, plan, es, es.stream, slots0, tl, out, true);  // synchronises
+        finalized = frc == 0;
+        return frc;
+    };
+    h.discard = [&] { bydb_result_free(ctx, out); };
+    return run_collective(ctx, root, pre_rc, h);
+}
+
+// A hash of what every rank of a keyed collective must pass alike: the whole query but its parts, and the group key.
+static uint64_t keyed_fingerprint(const bydb_query *q, const bydb_group_key *key, uint32_t cap) {
+    uint64_t h = 0xcbf29ce484222325ull;  // FNV-1a
+    auto mix = [&](const void *p, size_t n) {
+        const uint8_t *b = static_cast<const uint8_t *>(p);
+        for (size_t i = 0; i < n; ++i) h = (h ^ b[i]) * 0x100000001b3ull;
+    };
+    auto mix_u64 = [&](uint64_t v) { mix(&v, sizeof v); };
+    auto mix_str = [&](const char *s) {
+        const size_t n = s ? strlen(s) : 0;
+        mix_u64(n);
+        mix(s, n);
+    };
+    mix_u64(q->n_series);
+    mix(q->series_ids, q->n_series * 8);
+    mix_u64(q->series_group ? static_cast<uint64_t>(static_cast<uint32_t>(q->n_groups)) : ~0ull);
+    if (q->series_group) mix(q->series_group, q->n_series * 4);
+    mix_u64(static_cast<uint64_t>(q->tmin));
+    mix_u64(static_cast<uint64_t>(q->tmax));
+    mix_u64(q->n_preds);
+    for (uint32_t i = 0; i < q->n_preds; ++i) {
+        const bydb_pred &p = q->preds[i];
+        mix_str(p.family);
+        mix_str(p.tag);
+        mix_u64(static_cast<uint64_t>(p.op) << 32 | static_cast<uint32_t>(p.value_type));
+        if (p.value_type == BYDB_VT_INT64) {
+            mix_u64(static_cast<uint64_t>(p.lit_i64));
+        } else {
+            mix_u64(p.lit_len);
+            mix(p.lit, p.lit_len);
+        }
     }
+    mix_u64(q->n_aggs);
+    for (uint32_t a = 0; a < q->n_aggs; ++a) {
+        mix_str(q->aggs[a].field);
+        mix_u64(static_cast<uint64_t>(q->aggs[a].func));
+    }
+    mix_u64(static_cast<uint64_t>(static_cast<uint32_t>(q->top_n)) << 32 | static_cast<uint32_t>(q->top_agg));
+    mix_u64(static_cast<uint64_t>(static_cast<uint32_t>(q->top_desc)) << 32 | q->flags);
+    mix_str(key->family);
+    mix_str(key->tag);
+    mix_u64(static_cast<uint64_t>(cap) << 32 | key->value_type);
+    return h;
+}
+
+// the slot of a rank of a keyed collective that found V key values
+static KeyedSlot keyed_slot(const bydb_query *q, size_t n_fields, size_t V) {
+    return KeyedSlot(static_cast<size_t>(q->series_group ? q->n_groups : 1), n_fields, q->n_series, V);
+}
+
+int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t *out) {
+    return guarded([&]() -> int {
+    if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
+    int rc = validate_query(q, false);
+    uint32_t cap = 0;
+    if (!rc) rc = check_group_key(q, key, cap);
+    if (rc) return rc;
+    std::vector<std::string> fcols;
+    std::vector<int> agg_fcol;
+    distinct_fields(q, fcols, agg_fcol);
+    if (fcols.size() > kMaxFcols) return fail(BYDB_EINVAL, "too many distinct aggregated fields (max 8)");
+    *out = keyed_slot(q, fcols.size(), cap).total;
+    return 0;
+    });
+}
+
+// The keyed collective: discovery and the per-value passes of bydb_scan_agg_keyed on every rank, written into its slot of the
+// root's mailbox (layout KeyedSlot); on the root the union of the values, the cross-rank span check, the union table and first
+// appearances (key_union / rank_span_check / combine_keyed / merge_first kernels), then bydb_scan_agg_keyed's ordering and
+// finalisation.
+int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out) {
+    return guarded([&]() -> int {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    memset(out, 0, sizeof *out);
+    g_last_dev_err = 0;
+    auto owner = new KeyedOwner();
+    out->owner = owner;
+    KeyedUndo undo{ctx, out};
+    set_key_table(out, owner, {});
+    bydb_stats &stats = out->base.stats;
+    Plan plan;
+    uint32_t cap = 0;
+    KeyValues values;
+    std::vector<uint8_t> header;
+    KeyedSlot ks(0, 0, 0, 0);
+    uint64_t fp = 0;
+    CollectiveHooks h;
+    h.prepare = [&](ExecSlot &es, size_t slot) -> int {
+        int rc = validate_query(q, true);
+        if (!rc) rc = check_group_key(q, key, cap);
+        if (!rc) rc = make_plan(ctx, q, nullptr, plan);
+        if (rc) return rc;
+        if (parts_overlap(plan.parts, q->tmin, q->tmax))
+            return fail(BYDB_ENOTSUP, "group-key query over parts of one rank that overlap in time (version dedup) is not supported on the device path");
+        rc = discover_keys(ctx, q, key, cap, plan, es, &stats, values);
+        if (rc) return rc;
+        const size_t V = values.size(), G = static_cast<size_t>(plan.n_groups), F = plan.fcols.size();
+        if (G * cap > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
+        ks = keyed_slot(q, F, V);
+        if (ks.total > slot)
+            return fail(BYDB_EINVAL, "keyed collective: this rank's " + std::to_string(V) + " key values need " + std::to_string(ks.total) +
+                                         " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keyed_reduce_slot_bytes)");
+        // sized for the union (at most cap values) now: the root's finalisation may not allocate page-locked memory later
+        if (es.ensure_pinned(step_pinned_bytes(q, G, G * cap))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+        fp = keyed_fingerprint(q, key, cap);
+        header.assign(ks.off_vals + V * kMaxLit, 0);
+        const uint32_t v32 = static_cast<uint32_t>(V);
+        memcpy(header.data(), &fp, 8);
+        memcpy(header.data() + 8, &v32, 4);
+        for (size_t v = 0; v < V; ++v) {
+            const uint32_t len = static_cast<uint32_t>(values[v].size());
+            memcpy(header.data() + ks.off_lens + 4 * v, &len, 4);
+            if (len) memcpy(header.data() + ks.off_vals + v * kMaxLit, values[v].data(), len);
+        }
+        return 0;
+    };
+    h.contribute = [&](ExecSlot &es, uint8_t *my_slot) -> int {
+        const size_t V = values.size();
+        if (V) {
+            int rc = run_keyed_passes(ctx, q, key, plan, es, values, TableLayout(V * plan.n_groups, plan.fcols.size()), my_slot + ks.off_table,
+                                      reinterpret_cast<int64_t *>(my_slot + ks.off_coltype), reinterpret_cast<int64_t *>(my_slot + ks.off_kts),
+                                      reinterpret_cast<uint32_t *>(my_slot + ks.off_krow), reinterpret_cast<int64_t *>(my_slot + ks.off_span), &stats);
+            if (rc) return rc;
+        }
+        CUDA_TRY(cudaMemcpyAsync(my_slot, header.data(), header.size(), cudaMemcpyHostToDevice, es.stream));  // pageable: staged before it returns
+        return 0;
+    };
+    h.collect = [&](ExecSlot &) { return 0; };  // every pass was collected as it ran
+    h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &settle, bool &) -> int {
+        int rc = settle();  // a failed rank's slot holds nothing to read
+        if (rc) return rc;
+        cudaStream_t s = es.stream;
+        const uint32_t R = static_cast<uint32_t>(ctx->comm.nranks);
+        for (uint32_t r = 0; r < R; ++r) {
+            uint64_t theirs = 0;
+            CUDA_TRY(cudaMemcpy(&theirs, slots0 + r * slot, 8, cudaMemcpyDeviceToHost));
+            if (theirs != fp)
+                return fail(BYDB_EINVAL, "keyed collective: rank " + std::to_string(r) +
+                                             " passed another query or group key (only the parts may differ between ranks)");
+        }
+        // ---- union of the ranks' values, cross-rank span check
+        const size_t NS = q->n_series, G = static_cast<size_t>(plan.n_groups), F = plan.fcols.size();
+        size_t o = 0;
+        auto carve = [&](size_t bytes) {
+            size_t at = o;
+            o = align_up(o + bytes, 256);
+            return at;
+        };
+        const size_t u_ctl = carve(16), u_vals = carve(static_cast<size_t>(cap) * kMaxLit), u_lens = carve(static_cast<size_t>(cap) * 4),
+                     u_inv = carve(static_cast<size_t>(R) * cap * 4);
+        const size_t back_bytes = u_inv - u_ctl;  // ctl | vals | lens come back in one copy
+        Scratch us;
+        CUDA_TRY(us.alloc(o, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl, 0, 8, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl + 8, 0xff, 4, s));
+        KeyedUnionParams up;
+        memset(&up, 0, sizeof up);
+        up.slots = slots0;
+        up.slot_stride = slot;
+        up.G = static_cast<uint32_t>(G);
+        up.F = static_cast<uint32_t>(F);
+        up.NS = static_cast<uint32_t>(NS);
+        up.cap = cap;
+        up.n_ranks = R;
+        up.tmin = q->tmin;
+        up.tmax = q->tmax;
+        up.vals = us.base + u_vals;
+        up.lens = reinterpret_cast<uint32_t *>(us.base + u_lens);
+        up.inv = reinterpret_cast<int32_t *>(us.base + u_inv);
+        up.ctl = reinterpret_cast<uint32_t *>(us.base + u_ctl);
+        launch_key_union(up, s);
+        CUDA_TRY(cudaMemcpyAsync(es.pinned, us.base + u_ctl, back_bytes, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaGetLastError());
+        stats.kernel_launches += NS && R > 1 ? 2 : 1;
+        stats.d2h_bytes += back_bytes;
+        const uint32_t *ctl = reinterpret_cast<const uint32_t *>(es.pinned);
+        if (ctl[1] == kErrKeyCap)
+            return fail(BYDB_ENOMEM, "keyed collective: more distinct key values over all ranks than bydb_group_key.max_values (" + std::to_string(cap) + ")");
+        if (ctl[1] == kErrRankOverlap) {
+            const uint32_t i = ctl[2];
+            return fail(BYDB_ENOTSUP, "keyed collective: series #" + std::to_string(i) + " (id " + std::to_string(i < NS ? q->series_ids[i] : 0) +
+                                          ") lives on several ranks over time spans that intersect");
+        }
+        const size_t V = std::min<size_t>(ctl[0], cap);
+        KeyValues uvals(V);
+        const uint32_t *hl = reinterpret_cast<const uint32_t *>(es.pinned + (u_lens - u_ctl));
+        for (size_t u = 0; u < V; ++u) {
+            const uint8_t *b = es.pinned + (u_vals - u_ctl) + u * kMaxLit;
+            uvals[u].assign(b, b + std::min<uint32_t>(hl[u], kMaxLit));
+        }
+        set_key_table(out, owner, uvals);
+        if (V == 0) return 0;  // no rank selected a block: no rows
+        // ---- the ranks' tables, column types and first appearances folded into the union arrays
+        const TableLayout tlu(V * G, F);
+        o = 0;
+        const size_t c_table = carve(tlu.total), c_ct = carve(V * F * 8), c_kts = carve(V * NS * 8), c_krow = carve(V * NS * 4);
+        Scratch uc;
+        CUDA_TRY(uc.alloc(o, s));
+        up.n_values = static_cast<uint32_t>(V);
+        up.table = reinterpret_cast<uint64_t *>(uc.base + c_table);
+        up.coltype = reinterpret_cast<int64_t *>(uc.base + c_ct);
+        up.Kts = reinterpret_cast<int64_t *>(uc.base + c_kts);
+        up.Krow = reinterpret_cast<uint32_t *>(uc.base + c_krow);
+        launch_combine_keyed(up, s);
+        stats.kernel_launches += NS ? 2 : 1;
+        return keyed_finish(q, plan, es, V, uc.base + c_table, tlu, up.coltype, up.Kts, up.Krow, out, owner);
+    };
+    h.discard = [] {};  // the result of a failed call is freed by `undo`
+    const int rc = run_collective(ctx, root, 0, h);
+    if (rc) return rc;
+    undo.done = true;
+    return 0;
+    });
 }
 
 int bydb_scan_reduce(bydb_ctx *ctx, const bydb_query *q, int32_t root, bydb_result *out) {

@@ -2987,6 +2987,7 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
     uint32_t krow = kKeyAbsent;
     int64_t span_lo[4], span_hi[4];
     int nspan = 0;
+    int64_t slo = INT64_MAX, shi = INT64_MIN;  // the series' selected blocks over every part (ReduceParams::span)
     bool overlap = false;
     for (uint32_t pi = 0; pi < p.n_parts; ++pi) {
         const DevPartRef &part = p.parts[pi];
@@ -3042,6 +3043,8 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
             if (__ballot_sync(0xffffffffu, mine) != 0xffffffffu) break;
         }
         if (plo <= phi) {
+            slo = plo < slo ? plo : slo;
+            shi = phi > shi ? phi : shi;
             for (int s = 0; s < nspan; ++s)
                 if (!(phi < span_lo[s] || plo > span_hi[s])) overlap = true;
             if (nspan < 4) {
@@ -3070,6 +3073,10 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
         }
     }
     if (lane != 0) return;
+    if (p.span) {
+        p.span[2 * static_cast<size_t>(i)] = slo;
+        p.span[2 * static_cast<size_t>(i) + 1] = shi;
+    }
     if (overlap && !p.dedup_done && atomicCAS(&p.err[0], 0u, static_cast<uint32_t>(kErrOverlap)) == 0u) p.err[1] = i;
     for (uint32_t c = 0; c < p.n_fcols; ++c) p.S[static_cast<size_t>(i) * p.n_fcols + c] = acc[c];
     p.Srows[i] = rows;
@@ -3516,6 +3523,21 @@ __global__ void __launch_bounds__(1024) select_rows_kernel(const __grid_constant
 }
 
 
+// How one word of a partial table combines with the same word of another rank's table.  kind: 0 float sum, 1 float maximum
+// (max, -min), 2 int64 sum (sum, count, rows), 3 int64 maximum (max, ~min, coltype); anything else keeps `a`.
+enum : int { kWordFsum = 0, kWordFmax = 1, kWordIsum = 2, kWordImax = 3 };
+__device__ __forceinline__ uint64_t combine_word(uint64_t a, uint64_t b, int kind) {
+    if (kind == kWordFsum)
+        return static_cast<uint64_t>(__double_as_longlong(__longlong_as_double(static_cast<long long>(a)) + __longlong_as_double(static_cast<long long>(b))));
+    if (kind == kWordFmax) {
+        const double x = __longlong_as_double(static_cast<long long>(a)), y = __longlong_as_double(static_cast<long long>(b));
+        return static_cast<uint64_t>(__double_as_longlong(y > x ? y : x));
+    }
+    if (kind == kWordIsum) return a + b;  // wraps like Go's int64
+    if (kind == kWordImax) return static_cast<uint64_t>(static_cast<int64_t>(b) > static_cast<int64_t>(a) ? b : a);
+    return a;
+}
+
 // Multi-GPU reduce after ONE all-gather of the per-rank partial tables: every word of the table is
 // combined across ranks in rank order (deterministic float sums, unlike a ring all-reduce), which is
 // the liaison's reduceAccumulator.Combine (measure_plan_aggregation.go:96-124) done on the device.
@@ -3523,21 +3545,20 @@ __global__ void combine_tables_kernel(uint64_t *t, uint32_t n, uint64_t words, u
                                       uint64_t si_lo, uint64_t si_hi, uint64_t mi_lo, uint64_t mi_hi) {
     const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= words) return;
+    const int kind = (i >= sf_lo && i < sf_hi) ? kWordFsum : (i >= mf_lo && i < mf_hi) ? kWordFmax : (i >= si_lo && i < si_hi) ? kWordIsum
+                   : (i >= mi_lo && i < mi_hi) ? kWordImax : -1;
     uint64_t a = t[i];
-    for (uint32_t r = 1; r < n; ++r) {
-        const uint64_t b = t[static_cast<uint64_t>(r) * stride + i];
-        if (i >= sf_lo && i < sf_hi) {
-            a = static_cast<uint64_t>(__double_as_longlong(__longlong_as_double(static_cast<long long>(a)) + __longlong_as_double(static_cast<long long>(b))));
-        } else if (i >= mf_lo && i < mf_hi) {
-            const double x = __longlong_as_double(static_cast<long long>(a)), y = __longlong_as_double(static_cast<long long>(b));
-            a = static_cast<uint64_t>(__double_as_longlong(y > x ? y : x));
-        } else if (i >= si_lo && i < si_hi) {
-            a += b;  // wraps like Go's int64
-        } else if (i >= mi_lo && i < mi_hi) {
-            a = static_cast<uint64_t>(static_cast<int64_t>(b) > static_cast<int64_t>(a) ? b : a);
-        }
-    }
+    for (uint32_t r = 1; r < n; ++r) a = combine_word(a, t[static_cast<uint64_t>(r) * stride + i], kind);
     t[i] = a;
+}
+
+// Column type and status of several passes' (or ranks') coltype words (type in bits 0..7, DevErr above): the type any of them
+// saw, a type mix when two disagree, the worst status.
+__device__ __forceinline__ void merge_coltype(int64_t w, int64_t &typ, int64_t &err) {
+    const int64_t wt = w & 0xff, we = w >> 8;
+    if (wt != 0 && typ != 0 && wt != typ) err = err > static_cast<int64_t>(kErrTypeMix) ? err : static_cast<int64_t>(kErrTypeMix);
+    if (typ == 0) typ = wt;
+    err = we > err ? we : err;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3563,16 +3584,21 @@ __device__ __forceinline__ void key_err(const KeyParams &p, uint32_t code, uint3
     if (atomicCAS(&p.err[0], 0u, code) == 0u) p.err[1] = g;
 }
 
+// home slot of a key value: FNV-1a over its key bytes (an int64 key's are its 8 little-endian bytes, see key_slot_i64)
+__device__ __forceinline__ uint32_t key_home(const uint8_t *bytes, uint32_t len) {
+    uint64_t h = 0xcbf29ce484222325ull;
+    for (uint32_t i = 0; i < len; ++i) h = (h ^ __ldg(bytes + i)) * 0x100000001b3ull;
+    return static_cast<uint32_t>(h ^ (h >> 32)) & (kKeySlots - 1);
+}
+
 __device__ void key_insert(const KeyParams &p, const uint8_t *bytes, uint32_t len, uint32_t g) {
     if (len > kMaxLit) {
         key_err(p, kErrKeyLong, g);
         return;
     }
-    uint64_t h = 0xcbf29ce484222325ull;  // FNV-1a
-    for (uint32_t i = 0; i < len; ++i) h = (h ^ __ldg(bytes + i)) * 0x100000001b3ull;
     const unsigned long long mine =
         (1ull << 63) | (static_cast<unsigned long long>(len) << 48) | (len ? (reinterpret_cast<uintptr_t>(bytes) & 0xffffffffffffull) : 0ull);
-    uint32_t s = static_cast<uint32_t>(h ^ (h >> 32)) & (kKeySlots - 1);
+    uint32_t s = key_home(bytes, len);
     for (uint32_t probe = 0; probe < kKeySlots; ++probe) {
         unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.slots[s]);
         if (cur == 0) {
@@ -3935,13 +3961,7 @@ __global__ void permute_table_kernel(TablePtrs dst, TablePtrs src, const int32_t
     if (t < n_fcols) {
         // column type of the query = the type any pass saw; two passes that disagree are a type mix; the worst status wins
         int64_t typ = 0, err = 0;
-        for (uint32_t v = 0; v < n_passes; ++v) {
-            const int64_t w = pass_coltype[static_cast<size_t>(v) * n_fcols + t];
-            const int64_t wt = w & 0xff, we = w >> 8;
-            if (wt != 0 && typ != 0 && wt != typ) err = err > static_cast<int64_t>(kErrTypeMix) ? err : static_cast<int64_t>(kErrTypeMix);
-            if (typ == 0) typ = wt;
-            err = we > err ? we : err;
-        }
+        for (uint32_t v = 0; v < n_passes; ++v) merge_coltype(pass_coltype[static_cast<size_t>(v) * n_fcols + t], typ, err);
         dst.coltype[t] = typ | (err << 8);
     }
     if (t >= n_groups * n_fcols) return;
@@ -3961,6 +3981,181 @@ void launch_permute_table(const TablePtrs &dst, const TablePtrs &src, const int3
                           const int64_t *pass_coltype, uint32_t n_passes, cudaStream_t s) {
     const uint32_t n = n_groups * n_fcols > n_fcols ? n_groups * n_fcols : n_fcols;
     permute_table_kernel<<<(n + 255) / 256, 256, 0, s>>>(dst, src, perm, n_groups, n_fcols, pass_coltype, n_passes);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Keyed collective (bydb_scan_reduce_keyed): every rank ran discovery and its per-value passes into its slot of the root's
+// mailbox (layout: KeyedSlot).  The ranks' value lists differ, so their V_r x G composite tables do not line up slot for slot.
+// The root builds the union of the values, checks that no series lives on two ranks over intersecting time spans, folds the
+// ranks' tables and first appearances into V_u x G union arrays, and then runs the single-context ordering (key_order_kernel,
+// key_perm_kernel, permute_table_kernel) and finalisation on them unchanged.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t slot_values(const KeyedUnionParams &p, uint32_t r) {
+    const uint32_t v = *reinterpret_cast<const uint32_t *>(p.slots + r * p.slot_stride + 8);
+    return v < p.cap ? v : p.cap;
+}
+__device__ __forceinline__ KeyedSlot slot_layout(const KeyedUnionParams &p, uint32_t r) { return KeyedSlot(p.G, p.F, p.NS, slot_values(p, r)); }
+
+// One CTA of kMaxKeyValues threads.  Ranks in rank order, each rank's values in its order: thread v looks value v up in a shared
+// open-addressing table of the values so far (homed by key_home, like key_values_kernel's table; byte equality decides -- the
+// ranks already folded nil into "" or 0), the values not found get the next union indices by a block scan, then enter the table.
+__global__ void __launch_bounds__(kMaxKeyValues) key_union_kernel(const __grid_constant__ KeyedUnionParams p) {
+    __shared__ uint32_t table[kKeySlots];  // union index + 1, 0 = empty
+    __shared__ uint32_t warp_tot[32];
+    const uint32_t t = threadIdx.x, cap = p.cap;
+    for (uint32_t i = t; i < kKeySlots; i += blockDim.x) table[i] = 0;
+    for (uint32_t i = t; i < p.n_ranks * cap; i += blockDim.x) p.inv[i] = -1;
+    __syncthreads();
+    uint32_t n = 0;
+    for (uint32_t r = 0; r < p.n_ranks; ++r) {
+        const uint8_t *slot = p.slots + r * p.slot_stride;
+        const bool mine = t < slot_values(p, r);
+        const KeyedSlot ks = slot_layout(p, r);
+        const uint8_t *b = slot + ks.off_vals + static_cast<size_t>(t) * kMaxLit;
+        uint32_t len = 0, s = 0;
+        int32_t u = -1;
+        if (mine) {
+            len = min(reinterpret_cast<const uint32_t *>(slot + ks.off_lens)[t], static_cast<uint32_t>(kMaxLit));
+            s = key_home(b, len);
+            for (uint32_t e; (e = table[s]) != 0; s = (s + 1) & (kKeySlots - 1)) {
+                const uint8_t *o = p.vals + static_cast<size_t>(e - 1) * kMaxLit;
+                bool eq = p.lens[e - 1] == len;
+                for (uint32_t i = 0; i < len && eq; ++i) eq = o[i] == __ldg(b + i);
+                if (eq) {
+                    u = static_cast<int32_t>(e - 1);
+                    break;
+                }
+            }
+        }
+        uint32_t total = 0;
+        const uint32_t pos = block_excl_scan(mine && u < 0 ? 1u : 0u, warp_tot, total);
+        if (n + total > cap) {  // block-uniform
+            if (t == 0) {
+                p.ctl[1] = kErrKeyCap;
+                p.ctl[0] = n + total;
+            }
+            return;
+        }
+        const bool fresh = mine && u < 0;
+        if (fresh) {
+            u = static_cast<int32_t>(n + pos);
+            for (uint32_t i = 0; i < len; ++i) p.vals[static_cast<size_t>(u) * kMaxLit + i] = __ldg(b + i);
+            p.lens[u] = len;
+        }
+        __syncthreads();  // every thread's lookup of this round is done before the table grows
+        if (mine) p.inv[r * cap + static_cast<uint32_t>(u)] = static_cast<int32_t>(t);
+        if (fresh)
+            while (atomicCAS(&table[s], 0u, static_cast<uint32_t>(u) + 1u) != 0u) s = (s + 1) & (kKeySlots - 1);
+        n += total;
+        __syncthreads();  // the new values' bytes and slots are in place before the next rank looks them up
+    }
+    if (t == 0) p.ctl[0] = n;
+}
+
+// [lo, hi] of series i on rank r, clipped to the query's range; false = the rank selects no block of it
+__device__ __forceinline__ bool rank_span(const KeyedUnionParams &p, uint32_t r, uint32_t i, int64_t &lo, int64_t &hi) {
+    if (slot_values(p, r) == 0) return false;  // no selected block at all: the rank ran no pass, its spans were never written
+    const int64_t *sp = reinterpret_cast<const int64_t *>(p.slots + r * p.slot_stride + slot_layout(p, r).off_span) + 2 * static_cast<size_t>(i);
+    lo = sp[0] > p.tmin ? sp[0] : p.tmin;
+    hi = sp[1] < p.tmax ? sp[1] : p.tmax;
+    return lo <= hi;
+}
+
+// One warp per series: the ranks' spans pairwise (at most 64 ranks, 2016 pairs).  The lowest series index with two intersecting
+// spans goes to ctl[2]: merging first appearances by time (merge_first_kernel) is exact only when the spans are disjoint.
+__global__ void __launch_bounds__(256) rank_span_check_kernel(const __grid_constant__ KeyedUnionParams p) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= p.NS) return;
+    const uint32_t R = p.n_ranks, pairs = R * (R - 1) / 2;
+    bool hit = false;
+    for (uint32_t k = lane; k < pairs && !hit; k += 32) {
+        uint32_t a = 0, rem = k;
+        while (rem >= R - 1 - a) rem -= R - 1 - a++;
+        const uint32_t b = a + 1 + rem;
+        int64_t alo, ahi, blo, bhi;
+        if (rank_span(p, a, i, alo, ahi) && rank_span(p, b, i, blo, bhi)) hit = (alo > blo ? alo : blo) <= (ahi < bhi ? ahi : bhi);
+    }
+    if (__any_sync(0xffffffffu, hit) && lane == 0) {
+        atomicMin(&p.ctl[2], i);
+        atomicCAS(&p.ctl[1], 0u, static_cast<uint32_t>(kErrRankOverlap));
+    }
+}
+
+// One thread per word of the union table (u, g, field) and per union column type (u, field): the ranks in rank order, each
+// through inv, with combine_tables_kernel's per-word rule (deterministic float sums); the column types merge like
+// permute_table_kernel merges passes.  A rank without value u contributes nothing to its rows.
+__global__ void combine_keyed_kernel(const __grid_constant__ KeyedUnionParams p) {
+    const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const uint64_t G = p.G, F = p.F, cap = p.cap, VG = static_cast<uint64_t>(p.n_values) * G, GF = VG * F;
+    const uint64_t words = 7 * GF + VG;  // every region of TableLayout(V_u * G, F) but the coltype words
+    if (i >= words + p.n_values * F) return;
+    if (i >= words) {
+        const uint64_t u = (i - words) / F, c = (i - words) % F;
+        int64_t typ = 0, err = 0;
+        for (uint32_t r = 0; r < p.n_ranks; ++r) {
+            const int32_t v = p.inv[r * cap + u];
+            if (v >= 0) merge_coltype(reinterpret_cast<const int64_t *>(p.slots + r * p.slot_stride + slot_layout(p, r).off_coltype)[v * F + c], typ, err);
+        }
+        p.coltype[i - words] = typ | (err << 8);
+        return;
+    }
+    // region of the word: sum_f64 | max_f64 | negmin_f64 | sum_i64 | cnt | rows | max_i64 | notmin_i64 (TableLayout's order)
+    const int reg = i < 5 * GF ? static_cast<int>(i / GF) : i < 5 * GF + VG ? 5 : static_cast<int>(6 + (i - 5 * GF - VG) / GF);
+    const int kind = reg == 0 ? kWordFsum : reg <= 2 ? kWordFmax : reg <= 5 ? kWordIsum : kWordImax;
+    const uint64_t k = reg < 5 ? i - reg * GF : reg == 5 ? i - 5 * GF : i - 5 * GF - VG - (reg - 6) * GF;
+    const uint64_t j = reg == 5 ? k : k / F, c = reg == 5 ? 0 : k % F;  // union row j = u * G + g
+    const uint64_t u = j / G, g = j % G;
+    uint64_t a = 0;
+    bool first = true;
+    for (uint32_t r = 0; r < p.n_ranks; ++r) {
+        const int32_t v = p.inv[r * cap + u];
+        if (v < 0) continue;
+        const uint64_t VGr = slot_values(p, r) * G, GFr = VGr * F;
+        const uint64_t base = reg <= 5 ? reg * GFr : 5 * GFr + VGr + (reg - 6) * GFr;
+        const uint64_t row = static_cast<uint64_t>(v) * G + g;
+        const uint64_t w = reinterpret_cast<const uint64_t *>(p.slots + r * p.slot_stride + slot_layout(p, r).off_table)[base + (reg == 5 ? row : row * F + c)];
+        a = first ? w : combine_word(a, w, kind);
+        first = false;
+    }
+    p.table[i] = a;
+}
+
+// One thread per (union value u, series i): the first appearance over the ranks -- the least (Kts, Krow), kKeyAbsent skipped.
+// Exact because a series' spans on different ranks are disjoint (rank_span_check_kernel): the earlier span's block comes first.
+__global__ void merge_first_kernel(const __grid_constant__ KeyedUnionParams p) {
+    const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const uint64_t NS = p.NS;
+    if (idx >= p.n_values * NS) return;
+    const uint64_t u = idx / NS, i = idx % NS;
+    int64_t ts = INT64_MAX;
+    uint32_t row = kKeyAbsent;
+    for (uint32_t r = 0; r < p.n_ranks; ++r) {
+        const int32_t v = p.inv[r * p.cap + u];
+        if (v < 0) continue;
+        const uint8_t *slot = p.slots + r * p.slot_stride;
+        const KeyedSlot ks = slot_layout(p, r);
+        const size_t at = static_cast<size_t>(v) * NS + i;
+        const int64_t t = reinterpret_cast<const int64_t *>(slot + ks.off_kts)[at];
+        const uint32_t w = reinterpret_cast<const uint32_t *>(slot + ks.off_krow)[at];
+        if (w != kKeyAbsent && (row == kKeyAbsent || t < ts || (t == ts && w < row))) {
+            ts = t;
+            row = w;
+        }
+    }
+    p.Kts[idx] = ts;
+    p.Krow[idx] = row;
+}
+
+void launch_key_union(const KeyedUnionParams &p, cudaStream_t s) {
+    key_union_kernel<<<1, kMaxKeyValues, 0, s>>>(p);
+    if (p.NS && p.n_ranks > 1) rank_span_check_kernel<<<(p.NS + 7) / 8, 256, 0, s>>>(p);
+}
+void launch_combine_keyed(const KeyedUnionParams &p, cudaStream_t s) {
+    const uint64_t VG = static_cast<uint64_t>(p.n_values) * p.G, n = 7 * VG * p.F + VG + static_cast<uint64_t>(p.n_values) * p.F;
+    if (n) combine_keyed_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(p);
+    const uint64_t m = static_cast<uint64_t>(p.n_values) * p.NS;
+    if (m) merge_first_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(p);
 }
 
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s) {
@@ -4158,6 +4353,10 @@ void preload_kernels() {
     (void)cudaFuncGetAttributes(&ka, key_order_kernel);
     (void)cudaFuncGetAttributes(&ka, key_perm_kernel);
     (void)cudaFuncGetAttributes(&ka, permute_table_kernel);
+    (void)cudaFuncGetAttributes(&ka, key_union_kernel);
+    (void)cudaFuncGetAttributes(&ka, rank_span_check_kernel);
+    (void)cudaFuncGetAttributes(&ka, combine_keyed_kernel);
+    (void)cudaFuncGetAttributes(&ka, merge_first_kernel);
     cudaFuncAttributes a;
     cudaFuncGetAttributes(&a, plan_blocks_kernel);
     cudaFuncGetAttributes(&a, scan_blocks_kernel<true>);

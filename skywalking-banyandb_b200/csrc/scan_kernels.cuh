@@ -54,6 +54,7 @@ enum DevErr : uint32_t {
     kErrPeerTimeout = 11,   // multi-GPU reduce: a peer rank never delivered its partial table / never freed the slot
     kErrKeyCap = 12,        // per-row group key: more distinct values than the caller's max_values
     kErrKeyLong = 13,       // per-row group key: a value longer than kMaxLit bytes
+    kErrRankOverlap = 14,   // keyed collective: one series on two ranks over time spans that intersect
 };
 constexpr int kOpEqOrNil = 7;  // internal predicate operator of the group-key passes: the cell is nil or equals the literal
 constexpr uint32_t kKeyAbsent = 0xffffffffu;  // Krow of a series that never shows the value (a block's first row is below it)
@@ -147,6 +148,8 @@ struct ReduceParams {
     const uint32_t *Pfirst;
     int64_t *Kts;                 // [n_series]
     uint32_t *Krow;               // [n_series]
+    // keyed collective, first pass only (else NULL): [lo, hi] of each series' selected blocks over every part; lo > hi = none
+    int64_t *span;                // [2 * n_series]
     // partial table (see bydb_gpu.h): written by group_reduce
     double *sum_f64, *max_f64, *negmin_f64;
     int64_t *sum_i64, *cnt, *rows, *max_i64, *notmin_i64, *coltype;
@@ -254,6 +257,47 @@ struct TableLayout {
                          reinterpret_cast<int64_t *>(base + off_coltype)};
     }
 };
+// ---- keyed collective (bydb_scan_reduce_keyed): the slot of a rank that found V key values, in the root's mailbox, for G groups,
+// F fields and NS series.  Every region is sized by V, so a rank's need grows with the values it found; the root derives each
+// rank's layout from the V_r in its header.
+//   header    u64 query fingerprint | u32 V_r | u32 pad, then lens[V] u32 and values[V][kMaxLit]
+//   coltype   [V * F] the passes' column types + status
+//   Kts, Krow [V * NS] where each series first shows each value (ReduceParams::Kts / Krow)
+//   span      [NS][2] the series' selected blocks (ReduceParams::span)
+//   table     the composite table TableLayout(V * G, F)
+struct KeyedSlot {
+    size_t off_lens, off_vals, off_coltype, off_kts, off_krow, off_span, off_table, total;
+    __host__ __device__ static size_t up(size_t o) { return (o + 255) / 256 * 256; }
+    __host__ __device__ KeyedSlot(size_t G, size_t F, size_t NS, size_t V) {
+        off_lens = 256;
+        off_vals = up(off_lens + V * 4);
+        off_coltype = up(off_vals + V * kMaxLit);
+        off_kts = up(off_coltype + V * F * 8);
+        off_krow = up(off_kts + V * NS * 8);
+        off_span = up(off_krow + V * NS * 4);
+        off_table = up(off_span + NS * 16);
+        total = off_table + 8 * (V * G * (7 * F + 1) + F);  // TableLayout(V * G, F).total
+    }
+};
+struct KeyedUnionParams {
+    const uint8_t *slots;         // rank r's slot at slots + r * slot_stride (the root's mailbox, this collective's parity)
+    size_t slot_stride;
+    uint32_t G, F, NS, cap;       // groups, fields, series, distinct key values accepted
+    uint32_t n_ranks, n_values;   // n_values: V_u, the union's size (combine / merge_first only)
+    int64_t tmin, tmax;           // the query's range (span check)
+    uint8_t *vals;                // [cap * kMaxLit] union values, in order of first appearance by rank, then by the rank's order
+    uint32_t *lens;               // [cap]
+    int32_t *inv;                 // [n_ranks * cap] inv[r * cap + u]: index of union value u among rank r's values, -1 = absent
+    uint32_t *ctl;                // [0] V_u [1] DevErr [2] first series whose spans on two ranks intersect (preset 0xffffffff)
+    uint64_t *table;              // union composite table TableLayout(V_u * G, F)
+    int64_t *coltype;             // [V_u * F] column types of the union values (permute_table's pass_coltype)
+    int64_t *Kts;                 // [V_u * NS]
+    uint32_t *Krow;               // [V_u * NS]
+};
+// key_union_kernel, then rank_span_check_kernel (both read only the headers and spans; ctl is then read back)
+void launch_key_union(const KeyedUnionParams &p, cudaStream_t s);
+// combine_keyed_kernel and merge_first_kernel into table / coltype / Kts / Krow (p.n_values = V_u > 0)
+void launch_combine_keyed(const KeyedUnionParams &p, cudaStream_t s);
 // dst[j] = src[perm[j]] for every group row of a partial table; coltype = the passes' column types merged
 void launch_permute_table(const TablePtrs &dst, const TablePtrs &src, const int32_t *perm, uint32_t n_groups, uint32_t n_fcols,
                           const int64_t *pass_coltype, uint32_t n_passes, cudaStream_t s);
