@@ -59,6 +59,16 @@ int guarded(F &&f) {
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// the layout of one device scratch allocation: each call carves `bytes` and returns their offset; regions start 256 B aligned
+struct Carve {
+    size_t o = 0;  // bytes carved so far
+    size_t operator()(size_t bytes) {
+        const size_t at = o;
+        o = align_up(o + bytes, 256);
+        return at;
+    }
+};
+
 struct Part {
     uint64_t id = 0;
     PartDir dir;
@@ -146,6 +156,19 @@ struct ExecSlot {
         if (cudaMallocHost(reinterpret_cast<void **>(&zpage), kZeroPageBytes * kMaxBatches) != cudaSuccess) return -1;
         if (cudaEventCreateWithFlags(&busy, cudaEventDisableTiming) != cudaSuccess) return -1;
         return ensure_pinned(kInitialPinned);
+    }
+    ExecSlot() = default;
+    ExecSlot(const ExecSlot &) = delete;
+    ExecSlot &operator=(const ExecSlot &) = delete;
+    // with the slot's device current and none of its work in flight
+    ~ExecSlot() {
+        if (stream) cudaStreamDestroy(stream);
+        for (auto &e : ev)
+            if (e) cudaEventDestroy(e);
+        if (busy) cudaEventDestroy(busy);
+        if (pinned) cudaFreeHost(pinned);
+        for (uint8_t *r : retired) cudaFreeHost(r);
+        if (zpage) cudaFreeHost(zpage);
     }
 };
 
@@ -258,6 +281,19 @@ struct bydb_ctx {
 
 namespace {
 
+// The HBM budget (bydb_cfg.hbm_budget_bytes, 0 = none) is an account of the device memory the context holds for parts and the
+// mailbox: every reservation is given back with hbm_release when that memory goes, or when its allocation fails.
+int hbm_reserve(bydb_ctx *ctx, uint64_t bytes, const char *msg = "HBM budget exceeded") {
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (ctx->hbm_budget && ctx->hbm_used + bytes > ctx->hbm_budget) return fail(BYDB_ENOMEM, msg);
+    ctx->hbm_used += bytes;
+    return 0;
+}
+void hbm_release(bydb_ctx *ctx, uint64_t bytes) {
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    ctx->hbm_used -= bytes;
+}
+
 struct SlotLease {
     bydb_ctx *ctx;
     std::unique_ptr<ExecSlot> slot;
@@ -297,6 +333,7 @@ struct Plan {
     std::vector<std::string> fcols;       // distinct aggregated fields
     std::vector<int> agg_fcol;
     int32_t n_groups = 1;
+    TableLayout tl = TableLayout(1, 1);   // the partial table of n_groups x fcols
     uint32_t total_blocks = 0;
     uint64_t n_series = 0;
 };
@@ -357,18 +394,25 @@ int validate_query(const bydb_query *q, bool need_parts) {
     return 0;
 }
 
-void distinct_fields(const bydb_query *q, std::vector<std::string> &fcols, std::vector<int> &agg_fcol) {
+// The shape of a (validated) query's partial table, into `plan`: its distinct aggregated fields, the field of each
+// aggregation, the series groups and the table layout.  Fills all of them, then refuses more fields than a table holds.
+int query_shape(const bydb_query *q, Plan &plan) {
     for (uint32_t a = 0; a < q->n_aggs; ++a) {
         std::string f = q->aggs[a].field;
         int idx = -1;
-        for (size_t i = 0; i < fcols.size(); ++i)
-            if (fcols[i] == f) idx = static_cast<int>(i);
+        for (size_t i = 0; i < plan.fcols.size(); ++i)
+            if (plan.fcols[i] == f) idx = static_cast<int>(i);
         if (idx < 0) {
-            fcols.push_back(f);
-            idx = static_cast<int>(fcols.size() - 1);
+            plan.fcols.push_back(f);
+            idx = static_cast<int>(plan.fcols.size() - 1);
         }
-        agg_fcol.push_back(idx);
+        plan.agg_fcol.push_back(idx);
     }
+    plan.n_groups = q->series_group ? q->n_groups : 1;
+    plan.n_series = q->n_series;
+    plan.tl = TableLayout(static_cast<size_t>(plan.n_groups), plan.fcols.size());
+    if (plan.fcols.size() > kMaxFcols) return fail(BYDB_EINVAL, "too many distinct aggregated fields (max 8)");
+    return 0;
 }
 
 // the caller's file list of one part, checked
@@ -382,14 +426,22 @@ int file_images(const bydb_part_files *files, std::vector<FileImage> &imgs) {
     return 0;
 }
 
-// zero_copy: the data files stay in (pinned, device-mapped) host memory and the kernels read the
-// pages they need straight over PCIe; only the block directory is uploaded.
 int unpack_fallback_pages(bydb_ctx *ctx, Part &part, size_t n_files, cudaStream_t s);
 int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Part &part, const std::vector<std::string> &families, cudaStream_t s, size_t n_files,
                           size_t *dir_bytes_out);
 
+// how register_part_locked_free admits a part
+struct AdmitOptions {
+    bool zero_copy = false;     // the data files stay in (pinned, device-mapped) host memory and the kernels read the pages they
+                                // need straight over PCIe; only the block directory is uploaded
+    bool transient = false;     // for the length of one call: device memory from the stream-ordered pool
+    bool unpack = false;        // fallback pages are rewritten at admission (unpack_fallback_pages)
+    PartDir *parsed = nullptr;  // the block index as the caller parsed it already
+    bool device_index = false;  // the block index is parsed by kernels (resident parts without `parsed`)
+};
+
 int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_files *files, std::shared_ptr<Part> &out, uint64_t *h2d,
-                              bool zero_copy = false, bool transient = false, bool unpack = false, PartDir *parsed = nullptr, bool device_index = false) {
+                              const AdmitOptions &opt) {
     std::vector<FileImage> imgs;
     if (int rc = file_images(files, imgs)) return rc;
     auto part = std::make_shared<Part>();
@@ -397,7 +449,7 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
     part->device = ctx->device;
     std::string err;
     // resident parts: the block index is inflated and parsed by kernels (index_kernels.cu); the host only decides the file table
-    const bool dev_index = device_index && !parsed && !zero_copy;
+    const bool dev_index = opt.device_index && !opt.parsed && !opt.zero_copy;
     std::vector<std::string> families;
     if (dev_index) {
         for (const auto &f : imgs)
@@ -406,8 +458,8 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
         if (families.size() > 250) return fail(BYDB_EINVAL, "too many tag family files");
         part->dir.files = {"timestamps.bin", "fv.bin"};
         for (const auto &fam : families) part->dir.files.push_back(fam + ".tf");
-    } else if (parsed) {
-        part->dir = std::move(*parsed);  // the caller parsed this slice of the block index already (cold path, in the background)
+    } else if (opt.parsed) {
+        part->dir = std::move(*opt.parsed);  // the caller parsed this slice of the block index already (cold path, in the background)
     } else {
         int rc = build_part_dir(imgs, ctx->names, part->dir, err);
         if (rc) return fail(rc, "part " + std::to_string(part_id) + ": " + err);
@@ -426,7 +478,7 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
         arena = align_up(arena + img->len + 256, 256);
     }
     std::vector<const uint8_t *> mapped(order.size(), nullptr);
-    if (zero_copy) {
+    if (opt.zero_copy) {
         for (size_t i = 0; i < order.size(); ++i) {
             if (order[i]->len == 0) continue;
             cudaPointerAttributes at;
@@ -441,24 +493,22 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
     }
     const size_t nb = part->dir.blocks.size(), nc = part->dir.cols.size(), nf = order.size();
     const size_t dir_bytes = dev_index ? 0 : align_up(nb * sizeof(DevBlock), 256) + align_up(nc * sizeof(DevCol), 256) + align_up((nf + 1) * sizeof(void *), 256);
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        if (ctx->hbm_budget && ctx->hbm_used + arena + dir_bytes > ctx->hbm_budget) return fail(BYDB_ENOMEM, "HBM budget exceeded");
-        ctx->hbm_used += arena + dir_bytes;
-    }
+    if (int rc = hbm_reserve(ctx, arena + dir_bytes)) return rc;
     part->hbm_bytes = arena + dir_bytes;
-    auto undo_budget = [&]() {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        ctx->hbm_used -= part->hbm_bytes;
-    };
+    // every failure from here on gives the part's reservation back; the directory and the unpack arena add to it
+    struct Undo {
+        bydb_ctx *ctx;
+        const Part *part;
+        bool keep = false;
+        ~Undo() {
+            if (!keep) hbm_release(ctx, part->hbm_bytes);
+        }
+    } undo{ctx, part.get()};
     SlotLease lease(ctx);
-    if (lease.init()) {
-        undo_budget();
-        return fail(BYDB_EIO, "cannot create stream");
-    }
+    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
     cudaStream_t s = lease.slot->stream;
     bool alloc_ok;
-    if (transient) {
+    if (opt.transient) {
         part->pool_stream = s;
         alloc_ok = cudaMallocAsync(reinterpret_cast<void **>(&part->d_arena), arena ? arena : 256, s) == cudaSuccess &&
                    (dev_index || cudaMallocAsync(reinterpret_cast<void **>(&part->d_dir), dir_bytes ? dir_bytes : 256, s) == cudaSuccess);
@@ -466,21 +516,15 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
         alloc_ok = cudaMalloc(reinterpret_cast<void **>(&part->d_arena), arena ? arena : 256) == cudaSuccess &&
                    (dev_index || cudaMalloc(reinterpret_cast<void **>(&part->d_dir), dir_bytes ? dir_bytes : 256) == cudaSuccess);
     }
-    if (!alloc_ok) {
-        undo_budget();
-        return fail(BYDB_ENOMEM, "device allocation failed for part " + std::to_string(part_id));
-    }
+    if (!alloc_ok) return fail(BYDB_ENOMEM, "device allocation failed for part " + std::to_string(part_id));
     cudaError_t e = cudaSuccess;
-    if (!zero_copy) {
+    if (!opt.zero_copy) {
         e = cudaMemsetAsync(part->d_arena, 0, arena ? arena : 256, s);
         for (size_t i = 0; i < nf && e == cudaSuccess; ++i)
             if (order[i]->len) e = cudaMemcpyAsync(part->d_arena + offs[i], order[i]->data, order[i]->len, cudaMemcpyHostToDevice, s);
     }
     if (dev_index) {
-        if (e != cudaSuccess) {
-            undo_budget();
-            return fail(BYDB_EIO, std::string("part upload: ") + cudaGetErrorString(e));
-        }
+        if (e != cudaSuccess) return fail(BYDB_EIO, std::string("part upload: ") + cudaGetErrorString(e));
         size_t dbytes = 0;
         int rc = build_part_dir_device(ctx, imgs, *part, families, s, nf, &dbytes);
         std::vector<const uint8_t *> table(nf + 1, nullptr);
@@ -491,61 +535,71 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
         if (!rc && cudaStreamSynchronize(s) != cudaSuccess) rc = fail(BYDB_EIO, "part upload: synchronize");
         if (rc) {
             cudaStreamSynchronize(s);
-            undo_budget();
             return rc;
         }
         if (h2d) {
             for (size_t i = 0; i < nf; ++i) *h2d += order[i]->len;
             *h2d += dbytes;
         }
-        if (unpack) {
+        if (opt.unpack) {
             rc = unpack_fallback_pages(ctx, *part, nf, s);
-            if (rc) {
-                undo_budget();
-                return rc;
-            }
+            if (rc) return rc;
         }
+        undo.keep = true;
         out = part;
         return 0;
     }
     // directory
-    if (lease.slot->ensure_pinned(dir_bytes ? dir_bytes : 256)) {
-        undo_budget();
-        return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    }
+    if (lease.slot->ensure_pinned(dir_bytes ? dir_bytes : 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     uint8_t *hdir = lease.slot->pinned;  // the directory goes up from pinned staging in one copy
     if (nb) memcpy(hdir, part->dir.blocks.data(), nb * sizeof(DevBlock));
     const size_t off_cols = align_up(nb * sizeof(DevBlock), 256);
     if (nc) memcpy(hdir + off_cols, part->dir.cols.data(), nc * sizeof(DevCol));
     const size_t off_files = off_cols + align_up(nc * sizeof(DevCol), 256);
     for (size_t i = 0; i < nf; ++i) {
-        const uint8_t *pfile = zero_copy ? mapped[i] : part->d_arena + offs[i];
+        const uint8_t *pfile = opt.zero_copy ? mapped[i] : part->d_arena + offs[i];
         memcpy(hdir + off_files + i * sizeof(void *), &pfile, sizeof(void *));
     }
     if (e == cudaSuccess && dir_bytes) e = cudaMemcpyAsync(part->d_dir, hdir, dir_bytes, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-        undo_budget();
-        return fail(BYDB_EIO, std::string("part upload: ") + cudaGetErrorString(e));
-    }
+    if (e != cudaSuccess) return fail(BYDB_EIO, std::string("part upload: ") + cudaGetErrorString(e));
     part->d_blocks = reinterpret_cast<const DevBlock *>(part->d_dir);
     part->d_cols = reinterpret_cast<const DevCol *>(part->d_dir + off_cols);
     part->d_files = reinterpret_cast<const uint8_t *const *>(part->d_dir + off_files);
     if (h2d) {
-        if (!zero_copy)
+        if (!opt.zero_copy)
             for (size_t i = 0; i < nf; ++i) *h2d += order[i]->len;
         *h2d += dir_bytes;
     }
-    if (unpack) {
+    if (opt.unpack) {
         const int rc = unpack_fallback_pages(ctx, *part, nf, s);
-        if (rc) {
-            undo_budget();
-            return rc;
-        }
+        if (rc) return rc;
     }
+    undo.keep = true;
     out = part;
     return 0;
 }
+
+// The parts a host-image entry point admits for the length of one call, with ids ~0, ~0 - 1, ...: their budget goes back when
+// this goes away, their memory (stream-ordered) once the last holder lets go.
+struct TransientParts {
+    bydb_ctx *ctx;
+    std::vector<std::shared_ptr<Part>> parts;
+    explicit TransientParts(bydb_ctx *c) : ctx(c) {}
+    TransientParts(const TransientParts &) = delete;
+    TransientParts &operator=(const TransientParts &) = delete;
+    ~TransientParts() {
+        for (auto &p : parts) hbm_release(ctx, p->hbm_bytes);
+    }
+    uint64_t next_id() const { return ~0ull - parts.size(); }
+    int admit(const bydb_part_files *files, uint64_t *h2d, AdmitOptions opt) {
+        opt.transient = true;
+        std::shared_ptr<Part> p;
+        const int rc = register_part_locked_free(ctx, next_id(), files, p, h2d, opt);
+        if (!rc) parts.push_back(std::move(p));
+        return rc;
+    }
+};
 
 
 // ------------------------------------------------------------------------------------------------
@@ -714,11 +768,8 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
     const size_t off_cols = align_up(nb * sizeof(DevBlock), 256);
     const size_t off_files = off_cols + align_up(nc * sizeof(DevCol), 256);
     const size_t dir_bytes = off_files + align_up((n_files + 1) * sizeof(void *), 256);
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        if (ctx->hbm_budget && ctx->hbm_used + dir_bytes > ctx->hbm_budget) return fail(BYDB_ENOMEM, "HBM budget exceeded");
-        ctx->hbm_used += dir_bytes;
-    }
+    rc = hbm_reserve(ctx, dir_bytes);
+    if (rc) return rc;
     part.hbm_bytes += dir_bytes;
     *dir_bytes_out = dir_bytes;
     const cudaError_t ae = part.pool_stream ? cudaMallocAsync(reinterpret_cast<void **>(&part.d_dir), dir_bytes, s) : cudaMalloc(reinterpret_cast<void **>(&part.d_dir), dir_bytes);
@@ -773,11 +824,7 @@ int unpack_fallback_pages(bydb_ctx *ctx, Part &part, size_t n_files, cudaStream_
     part.unpack_skipped = cnt[3];
     if (cnt[0] == 0) return 0;
     const size_t arena = align_up(cnt[1] + 256, 256);
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        if (ctx->hbm_budget && ctx->hbm_used + arena > ctx->hbm_budget) return fail(BYDB_ENOMEM, "HBM budget exceeded while unpacking fallback pages");
-        ctx->hbm_used += arena;
-    }
+    if (int rc = hbm_reserve(ctx, arena, "HBM budget exceeded while unpacking fallback pages")) return rc;
     part.hbm_bytes += arena;
     cudaError_t e = part.pool_stream ? cudaMallocAsync(reinterpret_cast<void **>(&part.d_unpack), arena, s)
                                      : cudaMalloc(reinterpret_cast<void **>(&part.d_unpack), arena);
@@ -832,27 +879,22 @@ struct FinalLayout {
 };
 FinalLayout final_layout(size_t G, size_t A, int32_t top_n) {
     FinalLayout fl;
-    size_t o = 0;
-    auto carve = [&](size_t bytes) {
-        size_t at = o;
-        o = align_up(o + bytes, 256);
-        return at;
-    };
+    Carve carve;
     fl.cap = top_n > 0 ? std::min<size_t>(static_cast<size_t>(top_n), G) : G;
     fl.A = A;
     fl.o_vi = carve(G * A * 8);
     fl.o_vf = carve(G * A * 8);
     fl.o_keys = carve(G * 8);
     fl.o_kst = carve(G);
-    fl.o_out = o;
+    fl.o_out = carve.o;
     fl.o_cnt = carve(16);
     fl.o_isf = carve(A);
     fl.o_sg = carve(fl.cap * 4);
     fl.o_sr = carve(fl.cap * 8);
     fl.o_si = carve(fl.cap * A * 8);
     fl.o_sf = carve(fl.cap * A * 8);
-    fl.out_bytes = o - fl.o_out;
-    fl.total = o;
+    fl.out_bytes = carve.o - fl.o_out;
+    fl.total = carve.o;
     return fl;
 }
 
@@ -923,12 +965,7 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     uint8_t *h = slot.pinned + st.stride * static_cast<size_t>(batch);
     stage_series(q, st, h);
     // ---- device scratch layout
-    size_t o = 0;
-    auto carve = [&](size_t bytes) {
-        size_t at = o;
-        o = align_up(o + bytes, 256);
-        return at;
-    };
+    Carve carve;
     const size_t off_zero = carve(kZeroPageBytes);
     const size_t off_sids = carve(st.bytes);  // the staging as it is: one copy brings sids, order and group_start
     const size_t off_worklist = carve(NB * 4);
@@ -945,7 +982,7 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     const size_t off_first = carve(use_first ? n_first * 4 : 0);
     const size_t off_dd_index = carve(NB * 4), off_dd_rowoff = carve(NB * 8), off_dd_list = carve(NB * 4);
     Scratch sc;
-    CUDA_TRY(sc.alloc(o, stream));
+    CUDA_TRY(sc.alloc(carve.o, stream));
     uint8_t *d = sc.base;
     ZeroPage *z = reinterpret_cast<ZeroPage *>(d + off_zero);
     CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
@@ -1237,14 +1274,11 @@ int make_plan(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::shared_
             plan.parts.push_back(it->second);
         }
     }
-    distinct_fields(q, plan.fcols, plan.agg_fcol);
-    if (plan.fcols.size() > kMaxFcols) return fail(BYDB_EINVAL, "too many distinct aggregated fields (max 8)");
-    plan.n_groups = q->series_group ? q->n_groups : 1;
+    if (int rc = query_shape(q, plan)) return rc;
     uint64_t nb = 0;
     for (auto &p : plan.parts) nb += p->dir.blocks.size();
     if (nb > 0x7fffffffull) return fail(BYDB_EINVAL, "too many blocks");
     plan.total_blocks = static_cast<uint32_t>(nb);
-    plan.n_series = q->n_series;
     return 0;
 }
 
@@ -1256,7 +1290,7 @@ int scan_agg_impl(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::sha
     SlotLease lease(ctx);
     if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
     ExecSlot &slot = *lease.slot;
-    TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
+    const TableLayout &tl = plan.tl;
     Scratch table;
     CUDA_TRY(table.alloc(tl.total, slot.stream));
     memset(&out->stats, 0, sizeof out->stats);
@@ -1335,16 +1369,7 @@ void prepared_destroy(bydb_prepared *p) {
         if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
     if (p->t0) cudaEventDestroy(p->t0);
     if (p->t1) cudaEventDestroy(p->t1);
-    if (p->slot) {
-        if (p->slot->stream) cudaStreamDestroy(p->slot->stream);
-        for (auto &e : p->slot->ev)
-            if (e) cudaEventDestroy(e);
-        if (p->slot->busy) cudaEventDestroy(p->slot->busy);
-        if (p->slot->pinned) cudaFreeHost(p->slot->pinned);
-        for (uint8_t *r : p->slot->retired) cudaFreeHost(r);
-        if (p->slot->zpage) cudaFreeHost(p->slot->zpage);
-    }
-    delete p;
+    delete p;  // and with it the slot
 }
 
 // A graph reads its parts through the device pointers captured with it, so it may only replay while every handle still names
@@ -1366,6 +1391,22 @@ bool check_held_parts(bydb_ctx *ctx, const std::vector<bydb_part_h> &parts, cuda
     return !missing;
 }
 
+// One replay of a captured step on the slot's stream, synchronised: the step's host-side counters as captured, device_ms from
+// the events around the launch, then the counters and the device error of its zero page (batch 0).
+int replay_graph(cudaGraphExec_t exec, ExecSlot &slot, cudaEvent_t t0, cudaEvent_t t1, const bydb_stats &captured, bool express, bydb_stats *stats) {
+    CUDA_TRY(cudaEventRecord(t0, slot.stream));
+    CUDA_TRY(cudaGraphLaunch(exec, slot.stream));
+    CUDA_TRY(cudaEventRecord(t1, slot.stream));
+    CUDA_TRY(cudaStreamSynchronize(slot.stream));
+    CUDA_TRY(cudaGetLastError());
+    *stats = captured;  // the zero-page counters are still 0 there
+    float ms = 0;
+    cudaEventElapsedTime(&ms, t0, t1);
+    stats->device_ms = ms;
+    stats->scan_kernel_ms = 0;  // per-kernel events are not available inside a graph replay
+    return read_zero_page(*slot.page(0), express, stats);
+}
+
 // captures one step into p->exec; returns 0, or a code after leaving the stream out of capture mode
 int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
     Plan plan;
@@ -1377,7 +1418,7 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
         return 0;
     }
     ExecSlot &slot = *p->slot;
-    TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
+    const TableLayout &tl = plan.tl;
     p->host_off = stage_layout(p->q.n_series, tl.G).stride;  // results land behind the staging area, which must survive from replay to replay
     if (slot.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     memset(&p->captured, 0, sizeof p->captured);
@@ -1485,16 +1526,7 @@ int bydb_init(const bydb_cfg *cfg, bydb_ctx **out) {
 void bydb_shutdown(bydb_ctx *ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    cudaDeviceSynchronize();
-    for (auto &s : ctx->free_slots) {
-        if (s->stream) cudaStreamDestroy(s->stream);
-        for (auto &e : s->ev)
-            if (e) cudaEventDestroy(e);
-        if (s->busy) cudaEventDestroy(s->busy);
-        if (s->pinned) cudaFreeHost(s->pinned);
-        for (uint8_t *r : s->retired) cudaFreeHost(r);
-        if (s->zpage) cudaFreeHost(s->zpage);
-    }
+    cudaDeviceSynchronize();  // before any slot goes away: no copy may still read its pinned staging
     ctx->free_slots.clear();
     ctx->parts.clear();
     for (int i = 0; i < StageRing::kBufs; ++i) {
@@ -1522,20 +1554,25 @@ int bydb_part_register(bydb_ctx *ctx, uint64_t part_id, const bydb_part_files *f
     }
     CUDA_TRY(cudaSetDevice(ctx->device));
     std::shared_ptr<Part> part;
-    int rc = register_part_locked_free(ctx, part_id, files, part, nullptr, false, false, true, nullptr, !ctx->host_index);
+    AdmitOptions opt;
+    opt.unpack = true;
+    opt.device_index = !ctx->host_index;
+    int rc = register_part_locked_free(ctx, part_id, files, part, nullptr, opt);
     if (rc) return rc;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    auto again = ctx->by_id.find(part_id);
-    if (again != ctx->by_id.end()) {
-        // another thread registered the same part meanwhile: keep its copy, drop ours (idempotent per part_id)
-        ctx->hbm_used -= part->hbm_bytes;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        auto again = ctx->by_id.find(part_id);
+        if (again == ctx->by_id.end()) {
+            bydb_part_h h = ctx->next_handle++;
+            ctx->parts[h] = part;
+            ctx->by_id[part_id] = h;
+            *out = h;
+            return 0;
+        }
         *out = again->second;
-        return 0;
     }
-    bydb_part_h h = ctx->next_handle++;
-    ctx->parts[h] = part;
-    ctx->by_id[part_id] = h;
-    *out = h;
+    // another thread registered the same part meanwhile: keep its copy, drop ours (idempotent per part_id)
+    hbm_release(ctx, part->hbm_bytes);
     return 0;
     });
 }
@@ -1551,8 +1588,8 @@ int bydb_part_release(bydb_ctx *ctx, bydb_part_h h) {
         victim = it->second;
         ctx->by_id.erase(victim->id);
         ctx->parts.erase(it);
-        ctx->hbm_used -= victim->hbm_bytes;
     }
+    hbm_release(ctx, victim->hbm_bytes);
     cudaSetDevice(ctx->device);
     victim.reset();  // frees HBM once no in-flight query holds the part
     return 0;
@@ -1655,15 +1692,10 @@ int discover_keys(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key,
     const bool int64_key = key->value_type == BYDB_VT_INT64;
     const size_t NS = q->n_series, NB = plan.total_blocks;
     cudaStream_t stream = slot.stream;
-    size_t o = 0;
-    auto carve = [&](size_t bytes) {
-        size_t at = o;
-        o = align_up(o + bytes, 256);
-        return at;
-    };
+    Carve carve;
     const size_t a_sids = carve(NS * 8), a_slots = carve(kKeySlots * 8), a_ctl = carve(16), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
                  a_lens = carve(static_cast<size_t>(cap) * 4);
-    const size_t a_total = o;
+    const size_t a_total = carve.o;
     Scratch ka;
     CUDA_TRY(ka.alloc(a_total, stream));
     const size_t back_bytes = a_total - a_ctl;  // ctl | vals | lens come back in one copy
@@ -1783,16 +1815,11 @@ int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V
     cudaStream_t stream = slot.stream;
     const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
     const StageLayout st = stage_layout(NS, G);
-    size_t o = 0;
-    auto carve = [&](size_t bytes) {
-        size_t at = o;
-        o = align_up(o + bytes, 256);
-        return at;
-    };
+    Carve carve;
     const size_t b_dst = carve(tlc.total), b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16),
                  b_stage = carve(st.bytes);
     Scratch kb;
-    CUDA_TRY(kb.alloc(o, stream));
+    CUDA_TRY(kb.alloc(carve.o, stream));
     CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
     KeyOrderParams ko;
     memset(&ko, 0, sizeof ko);
@@ -1891,15 +1918,10 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     const size_t GP = G * V;
     if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
     TableLayout tlc(GP, F);
-    size_t o = 0;
-    auto carve = [&](size_t bytes) {
-        size_t at = o;
-        o = align_up(o + bytes, 256);
-        return at;
-    };
+    Carve carve;
     const size_t b_src = carve(tlc.total), b_ct = carve(V * F * 8), b_kts = carve(V * NS * 8), b_krow = carve(V * NS * 4);
     Scratch kb;
-    CUDA_TRY(kb.alloc(o, stream));
+    CUDA_TRY(kb.alloc(carve.o, stream));
     CUDA_TRY(cudaMemsetAsync(kb.base + b_ct, 0, V * F * 8, stream));
     if (slot.ensure_pinned(step_pinned_bytes(q, G, GP))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     int64_t *ct = reinterpret_cast<int64_t *>(kb.base + b_ct), *kts = reinterpret_cast<int64_t *>(kb.base + b_kts);
@@ -1966,16 +1988,11 @@ int bydb_encode_pages(bydb_ctx *ctx, const bydb_encode_input *in, bydb_encoded_p
     SlotLease lease(ctx);
     if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
     cudaStream_t stream = lease.slot->stream;
-    size_t o = 0;
-    auto carve = [&](size_t bytes) {
-        size_t at = o;
-        o = align_up(o + bytes, 256);
-        return at;
-    };
+    Carve carve;
     const size_t d_vals = carve(NV * 8), d_boff = carve((NB + 1) * 8), d_soff = carve((NB + 1) * 8), d_scr = carve(is_float ? NV * 8 : 0),
                  d_exp = carve(is_float ? NV * 2 : 0), d_len = carve(NB * 4), d_st = carve(NB), d_ooff = carve((NB + 1) * 8), d_slots = carve(slot_off[NB]);
     Scratch sc;
-    if (sc.alloc(o, stream) != cudaSuccess) {
+    if (sc.alloc(carve.o, stream) != cudaSuccess) {
         cudaGetLastError();
         return fail(BYDB_ENOMEM, "bydb_encode_pages: device allocation failed");
     }
@@ -2182,11 +2199,8 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
     if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
     ExecSlot &slot = *lease.slot;
     Plan base;
-    distinct_fields(q, base.fcols, base.agg_fcol);
-    if (base.fcols.size() > kMaxFcols) return fail(BYDB_EINVAL, "too many distinct aggregated fields (max 8)");
-    base.n_groups = q->series_group ? q->n_groups : 1;
-    base.n_series = q->n_series;
-    TableLayout tl(static_cast<size_t>(base.n_groups), base.fcols.size());
+    if (int rc = query_shape(q, base)) return rc;
+    const TableLayout &tl = base.tl;
     std::vector<FileImage> imgs;
     if (int frc = file_images(files, imgs)) return frc;
     size_t n_primary = 0;
@@ -2224,7 +2238,7 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
         parses.push_back(task->get_future());
         ctx->pool.submit([task] { (*task)(); });
     }
-    std::vector<std::shared_ptr<Part>> keep;
+    TransientParts tmp(ctx);
     std::vector<std::shared_ptr<GatherImage>> gathered;
     int rc = 0, n_slices = 0;
     size_t next = 0;
@@ -2264,26 +2278,19 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
                 continue;
             }
             p = std::make_shared<Part>();
-            p->id = ~0ull - static_cast<uint64_t>(k);
+            p->id = tmp.next_id();
             p->device = ctx->device;
             p->pool_stream = slot.stream;
             p->hbm_bytes = gi->bytes;
-            {
-                std::lock_guard<std::mutex> lk(ctx->mu);
-                if (ctx->hbm_budget && ctx->hbm_used + gi->bytes > ctx->hbm_budget) {
-                    rc = fail(BYDB_ENOMEM, "HBM budget exceeded");
-                    continue;
-                }
-                ctx->hbm_used += gi->bytes;
-            }
+            rc = hbm_reserve(ctx, gi->bytes);
+            if (rc) continue;
             if (cudaMallocAsync(reinterpret_cast<void **>(&p->d_arena), gi->bytes, slot.stream) != cudaSuccess) {
                 p->d_arena = nullptr;
-                std::lock_guard<std::mutex> lk(ctx->mu);
-                ctx->hbm_used -= gi->bytes;
+                hbm_release(ctx, gi->bytes);
                 rc = fail(BYDB_ENOMEM, "device allocation failed for the gathered pages");
                 continue;
             }
-            keep.push_back(p);
+            tmp.parts.push_back(p);
             rc = upload_gather(ctx, *gi, p->d_arena, slot.stream);
             if (rc) continue;
             p->d_blocks = reinterpret_cast<const DevBlock *>(p->d_arena);
@@ -2296,9 +2303,12 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
             h2d = gi->bytes;
             gathered.push_back(gi);                  // the directory vectors feed the staged copies: keep them until the end
         } else {
-            rc = register_part_locked_free(ctx, ~0ull - static_cast<uint64_t>(k), files, p, &h2d, true, true, false, &merged);
+            AdmitOptions opt;
+            opt.zero_copy = true;
+            opt.parsed = &merged;
+            rc = tmp.admit(files, &h2d, opt);
             if (rc) continue;
-            keep.push_back(p);
+            p = tmp.parts.back();
         }
         out->stats.h2d_bytes += h2d;
         Plan plan = base;
@@ -2318,16 +2328,12 @@ static int scan_agg_host_pipelined(bydb_ctx *ctx, const bydb_part_files *files, 
     } else {
         cudaStreamSynchronize(slot.stream);
     }
-    for (int k = 0; k < static_cast<int>(keep.size()); ++k) {
+    for (int k = 0; k < static_cast<int>(tmp.parts.size()); ++k) {
         int rc2 = collect_scan(slot, &out->stats, k);
         if (!rc && rc2) {
             bydb_result_free(ctx, out);
             rc = rc2;
         }
-    }
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        for (auto &p : keep) ctx->hbm_used -= p->hbm_bytes;
     }
     if (!rc && !gather) out->stats.h2d_bytes += out->stats.page_bytes;  // pages were read in place over PCIe
     return rc;
@@ -2353,23 +2359,17 @@ int bydb_scan_agg_host(bydb_ctx *ctx, uint32_t n_parts, const bydb_part_files *p
         if (!wants_unpack(rc)) return rc;
     }
     for (int attempt = rc ? 1 : 0; attempt < 2; ++attempt) {
-        std::vector<std::shared_ptr<Part>> tmp;
+        TransientParts tmp(ctx);
         uint64_t h2d = 0;
         rc = 0;
         g_last_dev_err = 0;
         memset(out, 0, sizeof *out);
-        for (uint32_t i = 0; i < n_parts; ++i) {
-            std::shared_ptr<Part> p;
-            rc = register_part_locked_free(ctx, ~0ull - i, &parts[i], p, &h2d, (q->flags & BYDB_Q_HOST_ZERO_COPY) != 0, true, attempt == 1);
-            if (rc) break;
-            tmp.push_back(p);
-        }
-        if (!rc) rc = scan_agg_impl(ctx, q, &tmp, out, h2d);
-        if (!rc && (q->flags & BYDB_Q_HOST_ZERO_COPY)) out->stats.h2d_bytes += out->stats.page_bytes;  // pages were read in place over PCIe
-        {
-            std::lock_guard<std::mutex> lk(ctx->mu);
-            for (auto &p : tmp) ctx->hbm_used -= p->hbm_bytes;
-        }
+        AdmitOptions opt;
+        opt.zero_copy = (q->flags & BYDB_Q_HOST_ZERO_COPY) != 0;
+        opt.unpack = attempt == 1;
+        for (uint32_t i = 0; i < n_parts && !rc; ++i) rc = tmp.admit(&parts[i], &h2d, opt);
+        if (!rc) rc = scan_agg_impl(ctx, q, &tmp.parts, out, h2d);
+        if (!rc && opt.zero_copy) out->stats.h2d_bytes += out->stats.page_bytes;  // pages were read in place over PCIe
         if (!wants_unpack(rc)) break;
     }
     return rc;
@@ -2387,10 +2387,10 @@ int bydb_partials_layout(const bydb_query *q, bydb_partials_layout_t *out) {
     if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
     int rc = validate_query(q, false);
     if (rc) return rc;
-    std::vector<std::string> fcols;
-    std::vector<int> agg_fcol;
-    distinct_fields(q, fcols, agg_fcol);
-    TableLayout tl(static_cast<size_t>(q->series_group ? q->n_groups : 1), fcols.size());
+    Plan plan;
+    rc = query_shape(q, plan);
+    if (rc) return rc;
+    const TableLayout &tl = plan.tl;
     out->total_bytes = tl.total;
     out->off_sum_f64 = tl.off_sum_f64;
     out->n_sum_f64 = tl.GF;
@@ -2412,7 +2412,7 @@ int bydb_scan_partials(bydb_ctx *ctx, const bydb_query *q, void *d_partials, uin
     Plan plan;
     rc = make_plan(ctx, q, nullptr, plan);
     if (rc) return rc;
-    TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
+    const TableLayout &tl = plan.tl;
     if (bytes < tl.total) return fail(BYDB_EINVAL, "partial table buffer too small");
     CUDA_TRY(cudaSetDevice(ctx->device));
     SlotLease lease(ctx);
@@ -2443,10 +2443,10 @@ int bydb_partials_combine(bydb_ctx *ctx, const bydb_query *q, void *d_tables, ui
     if (!ctx || !d_tables || n_tables == 0) return fail(BYDB_EINVAL, "NULL argument");
     int rc = validate_query(q, false);
     if (rc) return rc;
-    std::vector<std::string> fcols;
-    std::vector<int> agg_fcol;
-    distinct_fields(q, fcols, agg_fcol);
-    TableLayout tl(static_cast<size_t>(q->series_group ? q->n_groups : 1), fcols.size());
+    Plan plan;
+    rc = query_shape(q, plan);
+    if (rc) return rc;
+    const TableLayout &tl = plan.tl;
     if (bytes_each != tl.total) return fail(BYDB_EINVAL, "partial tables must be exactly bydb_partials_layout().total_bytes each");
     CUDA_TRY(cudaSetDevice(ctx->device));
     launch_combine_tables(static_cast<uint8_t *>(d_tables), n_tables, tl, static_cast<cudaStream_t>(stream));
@@ -2462,9 +2462,9 @@ int bydb_reduce_finalize(bydb_ctx *ctx, const bydb_query *q, const void *d_parti
     int rc = validate_query(q, false);
     if (rc) return rc;
     Plan plan;
-    distinct_fields(q, plan.fcols, plan.agg_fcol);
-    plan.n_groups = q->series_group ? q->n_groups : 1;
-    TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
+    rc = query_shape(q, plan);
+    if (rc) return rc;
+    const TableLayout &tl = plan.tl;
     if (bytes < tl.total) return fail(BYDB_EINVAL, "partial table buffer too small");
     CUDA_TRY(cudaSetDevice(ctx->device));
     SlotLease lease(ctx);
@@ -2515,8 +2515,10 @@ int bydb_query_prepare(bydb_ctx *ctx, const bydb_query *q, bydb_prepared **out) 
     bool ok = p->slot->create() == 0;  // with its pinned staging: nothing page-locked is allocated inside an execution
     if (ok) {
         // sized for this query now (see ExecSlot::ensure_pinned: a page-locked allocation inside a collective can stall the peers)
-        const size_t G = q->series_group ? static_cast<size_t>(q->n_groups) : 1;
-        ok = p->slot->ensure_pinned(step_pinned_bytes(q, G, G)) == 0;
+        // a query with too many fields is refused at its first execution, like bydb_scan_agg would
+        Plan shape;
+        (void)query_shape(q, shape);
+        ok = p->slot->ensure_pinned(step_pinned_bytes(q, shape.tl.G, shape.tl.G)) == 0;
     }
     ok = ok && cudaEventCreate(&p->t0) == cudaSuccess && cudaEventCreate(&p->t1) == cudaSuccess;
     if (!ok) {
@@ -2555,20 +2557,9 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
         if (rc) return rc;
         if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
     }
-    ExecSlot &slot = *p->slot;
-    CUDA_TRY(cudaEventRecord(p->t0, slot.stream));
-    CUDA_TRY(cudaGraphLaunch(p->exec, slot.stream));
-    CUDA_TRY(cudaEventRecord(p->t1, slot.stream));
-    CUDA_TRY(cudaStreamSynchronize(slot.stream));
-    CUDA_TRY(cudaGetLastError());
-    out->stats = p->captured;  // host-side counters; the zero-page counters are still 0 there
-    float ms = 0;
-    cudaEventElapsedTime(&ms, p->t0, p->t1);
-    out->stats.device_ms = ms;
-    out->stats.scan_kernel_ms = 0;  // per-kernel events are not available inside a graph replay
-    const int rc = read_zero_page(*slot.page(0), p->express, &out->stats);
+    const int rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, &out->stats);
     if (rc) return rc;
-    return finalize_parse(slot.pinned + p->host_off, p->fl, false, out);
+    return finalize_parse(p->slot->pinned + p->host_off, p->fl, false, out);
     });
 }
 
@@ -2586,11 +2577,12 @@ int bydb_partials_rows(bydb_ctx *ctx, const bydb_query *q, const void *d_partial
     memset(out, 0, sizeof *out);
     int rc = validate_query(q, false);
     if (rc) return rc;
-    std::vector<std::string> fcols;
-    std::vector<int> agg_fcol;
-    distinct_fields(q, fcols, agg_fcol);
-    const size_t G = static_cast<size_t>(q->series_group ? q->n_groups : 1), F = fcols.size(), A = q->n_aggs;
-    TableLayout tl(G, F);
+    Plan plan;
+    rc = query_shape(q, plan);
+    if (rc) return rc;
+    const TableLayout &tl = plan.tl;
+    const std::vector<int> &agg_fcol = plan.agg_fcol;
+    const size_t G = tl.G, F = tl.F, A = q->n_aggs;
     if (bytes < tl.total) return fail(BYDB_EINVAL, "partial table buffer too small");
     CUDA_TRY(cudaSetDevice(ctx->device));
     std::vector<uint8_t> h(tl.total);
@@ -2668,13 +2660,11 @@ int bydb_comm_export(bydb_ctx *ctx, uint64_t max_table_bytes, int32_t max_ranks,
     if (cm.mine) return fail(BYDB_EINVAL, "bydb_comm_export was already called on this context");
     cm.slot_bytes = align_up(max_table_bytes, 256);
     cm.mailbox_bytes = kCommCtl + 2 * static_cast<size_t>(max_ranks) * cm.slot_bytes;
-    {
-        std::lock_guard<std::mutex> lk2(ctx->mu);
-        if (ctx->hbm_budget && ctx->hbm_used + cm.mailbox_bytes > ctx->hbm_budget) return fail(BYDB_ENOMEM, "HBM budget exceeded (mailbox)");
-        ctx->hbm_used += cm.mailbox_bytes;
-    }
+    if (int rc = hbm_reserve(ctx, cm.mailbox_bytes, "HBM budget exceeded (mailbox)")) return rc;
     if (cudaMalloc(reinterpret_cast<void **>(&cm.mine), cm.mailbox_bytes) != cudaSuccess) {
+        cudaGetLastError();  // the failed allocation must not surface in a later call's error check
         cm.mine = nullptr;
+        hbm_release(ctx, cm.mailbox_bytes);
         return fail(BYDB_ENOMEM, "device allocation failed for the mailbox");
     }
     CUDA_TRY(cudaMemset(cm.mine, 0, cm.mailbox_bytes));
@@ -2792,6 +2782,48 @@ static uint32_t comm_wait_host(Comm &cm, const unsigned long long *dev_words, ui
     }
 }
 
+// What one collective of epoch `epoch` uses of the root's mailbox (layout above struct Comm), and this rank's own error word.
+struct MailboxView {
+    uint64_t epoch;
+    size_t parity, slot_bytes;            // slot parity of the epoch, slot size of the root's mailbox
+    uint8_t *slots0, *my_slot;            // rank 0's and this rank's slot of that parity
+    unsigned long long *flags, *status, *done;
+    uint32_t *my_err;
+    uint64_t *last_use;                   // Comm::last_use of this root and parity
+    // Makes this collective the slots' latest use and returns the epoch of the previous one (0 = none): the root must have read
+    // the slots of that one (its `done` word) before they are overwritten.
+    uint64_t claim_slots() {
+        const uint64_t prev = *last_use;
+        *last_use = epoch;
+        return prev;
+    }
+};
+static MailboxView mailbox_view(Comm &cm, int32_t root, uint64_t epoch) {
+    MailboxView v;
+    v.epoch = epoch;
+    v.parity = static_cast<size_t>(epoch & 1u);
+    v.slot_bytes = cm.peer_slot_bytes[static_cast<size_t>(root)];
+    uint8_t *root_mb = cm.peer[static_cast<size_t>(root)];
+    v.slots0 = root_mb + kCommCtl + v.parity * static_cast<size_t>(cm.nranks) * v.slot_bytes;
+    v.my_slot = v.slots0 + static_cast<size_t>(cm.rank) * v.slot_bytes;
+    v.flags = reinterpret_cast<unsigned long long *>(root_mb);
+    v.status = reinterpret_cast<unsigned long long *>(root_mb + kCommStatusOff);
+    v.done = reinterpret_cast<unsigned long long *>(root_mb + kCommDoneOff);
+    v.my_err = reinterpret_cast<uint32_t *>(cm.mine + kCommErrOff);
+    v.last_use = &cm.last_use[2 * static_cast<size_t>(root) + v.parity];
+    return v;
+}
+
+// the first rank whose status word of `epoch` (as read back from the root's mailbox) carries a failure, as that failure
+static int peer_failure(const unsigned long long *status, int nranks, uint64_t epoch, const char *msg) {
+    for (int r = 0; r < nranks; ++r) {
+        const unsigned long long w = status[r];
+        if ((w >> 32) == (epoch & 0xffffffffull) && static_cast<uint32_t>(w) != 0)
+            return fail(-static_cast<int>(static_cast<uint32_t>(w)), "multi-GPU reduce: rank " + std::to_string(r) + msg);
+    }
+    return 0;
+}
+
 // One collective call of the peer-mailbox reduce, shared by bydb_scan_reduce and bydb_scan_reduce_keyed: the epoch and slot
 // parity, the wait for the slots' previous use, this rank's status word and arrival flag, on the root the wait for every rank
 // and the `done` word, and the outcome, most specific first.  What differs between the two forms comes in as hooks:
@@ -2828,67 +2860,50 @@ static int run_collective(bydb_ctx *ctx, int32_t root, int pre_rc, const Collect
     // From here on this rank ALWAYS raises its arrival flag (with a status word in front of it), whatever fails on the
     // host side: the other ranks' calls must neither hang nor fall out of step (every rank counts the same epochs).
     const uint64_t epoch = ++cm.epoch;
-    const size_t parity = static_cast<size_t>(epoch & 1u);
-    const size_t slot = cm.peer_slot_bytes[static_cast<size_t>(root)];
-    uint8_t *root_mb = cm.peer[static_cast<size_t>(root)];
-    uint8_t *slots0 = root_mb + kCommCtl + parity * static_cast<size_t>(cm.nranks) * slot;
-    uint8_t *my_slot = slots0 + static_cast<size_t>(cm.rank) * slot;
-    unsigned long long *flags = reinterpret_cast<unsigned long long *>(root_mb);
-    unsigned long long *status = reinterpret_cast<unsigned long long *>(root_mb + kCommStatusOff);
-    unsigned long long *done = reinterpret_cast<unsigned long long *>(root_mb + kCommDoneOff);
-    uint32_t *my_err = reinterpret_cast<uint32_t *>(cm.mine + kCommErrOff);
-    int rc = pre_rc ? fail(pre_rc, pre_msg) : h.prepare(es, slot);
+    MailboxView mb = mailbox_view(cm, root, epoch);
+    int rc = pre_rc ? fail(pre_rc, pre_msg) : h.prepare(es, mb.slot_bytes);
     // the slots' previous use -- the last collective with THIS root and parity, the same epoch on every rank -- must have been
     // consumed by the root (its `done` word only ever grows) before they are overwritten
-    const uint64_t prev_use = cm.last_use[2 * static_cast<size_t>(root) + parity];
-    cm.last_use[2 * static_cast<size_t>(root) + parity] = epoch;
+    const uint64_t prev_use = mb.claim_slots();
     uint32_t host_perr = 0;  // outcome of the host-polled waits (shared-device mode)
     if (prev_use) {
-        if (cm.shared_device) host_perr = comm_wait_host(cm, done, 1, prev_use);
-        else launch_comm_wait(done, 1, prev_use, my_err, kErrPeerTimeout, s);
+        if (cm.shared_device) host_perr = comm_wait_host(cm, mb.done, 1, prev_use);
+        else launch_comm_wait(mb.done, 1, prev_use, mb.my_err, kErrPeerTimeout, s);
     }
-    if (!rc) rc = h.contribute(es, my_slot);
+    if (!rc) rc = h.contribute(es, mb.my_slot);
     const std::string my_msg = rc ? g_last_error : std::string();
     const unsigned long long st_word = (epoch << 32) | static_cast<unsigned long long>(static_cast<uint32_t>(-rc));
-    cudaMemcpyAsync(status + cm.rank, &st_word, sizeof st_word, cudaMemcpyHostToDevice, s);  // pageable source: staged before the call returns
-    launch_comm_signal(flags + cm.rank, epoch, s);
+    cudaMemcpyAsync(mb.status + cm.rank, &st_word, sizeof st_word, cudaMemcpyHostToDevice, s);  // pageable source: staged before the call returns
+    launch_comm_signal(mb.flags + cm.rank, epoch, s);
     unsigned long long peer_status[kCommMaxRanks] = {0};
-    // the first failure of a rank, from the status words the root holds
-    auto peer_failure = [&]() -> int {
-        for (int r = 0; r < cm.nranks; ++r) {
-            const unsigned long long w = peer_status[r];
-            if ((w >> 32) == (epoch & 0xffffffffull) && static_cast<uint32_t>(w) != 0)
-                return fail(-static_cast<int>(static_cast<uint32_t>(w)), "multi-GPU reduce: rank " + std::to_string(r) + " failed on its side of the collective");
-        }
-        return 0;
-    };
+    const char *peer_msg = " failed on its side of the collective";
     bool finalized = false;
     int frc = 0;
     if (cm.rank == root) {
         // reduce: wait for every rank's share, then the form's own combine and finalisation
         if (cm.shared_device) {
-            const uint32_t e2 = comm_wait_host(cm, flags, static_cast<uint32_t>(cm.nranks), epoch);  // own flag included: own share is complete
+            const uint32_t e2 = comm_wait_host(cm, mb.flags, static_cast<uint32_t>(cm.nranks), epoch);  // own flag included: own share is complete
             host_perr = host_perr ? host_perr : e2;
         } else {
-            launch_comm_wait(flags, static_cast<uint32_t>(cm.nranks), epoch, my_err, kErrPeerTimeout, s);
+            launch_comm_wait(mb.flags, static_cast<uint32_t>(cm.nranks), epoch, mb.my_err, kErrPeerTimeout, s);
         }
         const std::function<int()> settle = [&]() -> int {
             cudaStreamSynchronize(s);
             uint32_t e = 0;
-            if (cudaMemcpy(&e, my_err, sizeof e, cudaMemcpyDeviceToHost) != cudaSuccess || e == 0) e = host_perr;
+            if (cudaMemcpy(&e, mb.my_err, sizeof e, cudaMemcpyDeviceToHost) != cudaSuccess || e == 0) e = host_perr;
             if (e) return fail(dev_err_code(e), dev_err_text(e));
-            cudaMemcpy(peer_status, status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost);
-            return peer_failure();
+            cudaMemcpy(peer_status, mb.status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost);
+            return peer_failure(peer_status, cm.nranks, epoch, peer_msg);
         };
-        if (!rc) frc = h.reduce(es, slots0, slot, settle, finalized);
+        if (!rc) frc = h.reduce(es, mb.slots0, mb.slot_bytes, settle, finalized);
         cudaStreamSynchronize(s);
-        cudaMemcpy(peer_status, status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost);
+        cudaMemcpy(peer_status, mb.status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost);
         // the slots of this parity are free again: nothing reads them any more
-        cudaMemcpyAsync(done, &epoch, sizeof epoch, cudaMemcpyHostToDevice, s);
+        cudaMemcpyAsync(mb.done, &epoch, sizeof epoch, cudaMemcpyHostToDevice, s);
     }
     cudaStreamSynchronize(s);
     uint32_t perr = 0;
-    if (cudaMemcpy(&perr, my_err, sizeof perr, cudaMemcpyDeviceToHost) == cudaSuccess && perr != 0) cudaMemset(my_err, 0, sizeof perr);
+    if (cudaMemcpy(&perr, mb.my_err, sizeof perr, cudaMemcpyDeviceToHost) == cudaSuccess && perr != 0) cudaMemset(mb.my_err, 0, sizeof perr);
     if (!perr) perr = host_perr;
     // ---- outcome, most specific first: this rank's own host-side failure, its device-side errors, a peer's failure
     if (rc) {
@@ -2898,7 +2913,7 @@ static int run_collective(bydb_ctx *ctx, int32_t root, int pre_rc, const Collect
     int crc = h.collect(es);
     if (!crc && perr) crc = fail(dev_err_code(perr), dev_err_text(perr));
     if (!crc && cm.rank == root) {
-        crc = peer_failure();
+        crc = peer_failure(peer_status, cm.nranks, epoch, peer_msg);
         if (!crc) crc = frc;
     }
     if (crc && finalized) h.discard();
@@ -2909,7 +2924,7 @@ static int run_collective(bydb_ctx *ctx, int32_t root, int pre_rc, const Collect
 static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::shared_ptr<Part>> *given, int pre_rc, uint64_t h2d_pre, int32_t root,
                             bydb_result *out) {
     Plan plan;
-    TableLayout tl(1, 1);
+    const TableLayout &tl = plan.tl;
     memset(&out->stats, 0, sizeof out->stats);
     out->stats.h2d_bytes = h2d_pre;
     CollectiveHooks h;
@@ -2917,7 +2932,6 @@ static int scan_reduce_impl(bydb_ctx *ctx, const bydb_query *q, const std::vecto
         int rc = validate_query(q, given == nullptr);
         if (!rc) rc = make_plan(ctx, q, given, plan);
         if (rc) return rc;
-        tl = TableLayout(static_cast<size_t>(plan.n_groups), plan.fcols.size());
         if (tl.total > slot) return fail(BYDB_EINVAL, "partial table larger than the mailbox slots (bydb_comm_export max_table_bytes)");
         if (es.ensure_pinned(step_pinned_bytes(q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
         return 0;
@@ -2983,9 +2997,7 @@ static uint64_t keyed_fingerprint(const bydb_query *q, const bydb_group_key *key
 }
 
 // the slot of a rank of a keyed collective that found V key values
-static KeyedSlot keyed_slot(const bydb_query *q, size_t n_fields, size_t V) {
-    return KeyedSlot(static_cast<size_t>(q->series_group ? q->n_groups : 1), n_fields, q->n_series, V);
-}
+static KeyedSlot keyed_slot(const Plan &plan, size_t V) { return KeyedSlot(plan.tl.G, plan.tl.F, plan.n_series, V); }
 
 int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t *out) {
     return guarded([&]() -> int {
@@ -2994,11 +3006,10 @@ int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key,
     uint32_t cap = 0;
     if (!rc) rc = check_group_key(q, key, cap);
     if (rc) return rc;
-    std::vector<std::string> fcols;
-    std::vector<int> agg_fcol;
-    distinct_fields(q, fcols, agg_fcol);
-    if (fcols.size() > kMaxFcols) return fail(BYDB_EINVAL, "too many distinct aggregated fields (max 8)");
-    *out = keyed_slot(q, fcols.size(), cap).total;
+    Plan plan;
+    rc = query_shape(q, plan);
+    if (rc) return rc;
+    *out = keyed_slot(plan, cap).total;
     return 0;
     });
 }
@@ -3035,7 +3046,7 @@ int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_
         if (rc) return rc;
         const size_t V = values.size(), G = static_cast<size_t>(plan.n_groups), F = plan.fcols.size();
         if (G * cap > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
-        ks = keyed_slot(q, F, V);
+        ks = keyed_slot(plan, V);
         if (ks.total > slot)
             return fail(BYDB_EINVAL, "keyed collective: this rank's " + std::to_string(V) + " key values need " + std::to_string(ks.total) +
                                          " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keyed_reduce_slot_bytes)");
@@ -3079,17 +3090,12 @@ int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_
         }
         // ---- union of the ranks' values, cross-rank span check
         const size_t NS = q->n_series, G = static_cast<size_t>(plan.n_groups), F = plan.fcols.size();
-        size_t o = 0;
-        auto carve = [&](size_t bytes) {
-            size_t at = o;
-            o = align_up(o + bytes, 256);
-            return at;
-        };
+        Carve carve;
         const size_t u_ctl = carve(16), u_vals = carve(static_cast<size_t>(cap) * kMaxLit), u_lens = carve(static_cast<size_t>(cap) * 4),
                      u_inv = carve(static_cast<size_t>(R) * cap * 4);
         const size_t back_bytes = u_inv - u_ctl;  // ctl | vals | lens come back in one copy
         Scratch us;
-        CUDA_TRY(us.alloc(o, s));
+        CUDA_TRY(us.alloc(carve.o, s));
         CUDA_TRY(cudaMemsetAsync(us.base + u_ctl, 0, 8, s));
         CUDA_TRY(cudaMemsetAsync(us.base + u_ctl + 8, 0xff, 4, s));
         KeyedUnionParams up;
@@ -3132,10 +3138,10 @@ int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_
         if (V == 0) return 0;  // no rank selected a block: no rows
         // ---- the ranks' tables, column types and first appearances folded into the union arrays
         const TableLayout tlu(V * G, F);
-        o = 0;
+        carve = Carve();
         const size_t c_table = carve(tlu.total), c_ct = carve(V * F * 8), c_kts = carve(V * NS * 8), c_krow = carve(V * NS * 4);
         Scratch uc;
-        CUDA_TRY(uc.alloc(o, s));
+        CUDA_TRY(uc.alloc(carve.o, s));
         up.n_values = static_cast<uint32_t>(V);
         up.table = reinterpret_cast<uint64_t *>(uc.base + c_table);
         up.coltype = reinterpret_cast<int64_t *>(uc.base + c_ct);
@@ -3179,15 +3185,7 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
     if (run == 0 || !p->reduce_capturable || cm.shared_device) return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
     std::unique_lock<std::mutex> lk(cm.mu);
     const uint64_t epoch = cm.epoch + 1;
-    const size_t parity = static_cast<size_t>(epoch & 1u);
-    const size_t slot_bytes = cm.peer_slot_bytes[static_cast<size_t>(root)];
-    uint8_t *root_mb = cm.peer[static_cast<size_t>(root)];
-    uint8_t *slots0 = root_mb + kCommCtl + parity * static_cast<size_t>(cm.nranks) * slot_bytes;
-    uint8_t *my_slot = slots0 + static_cast<size_t>(cm.rank) * slot_bytes;
-    unsigned long long *flags = reinterpret_cast<unsigned long long *>(root_mb);
-    unsigned long long *status = reinterpret_cast<unsigned long long *>(root_mb + kCommStatusOff);
-    unsigned long long *done = reinterpret_cast<unsigned long long *>(root_mb + kCommDoneOff);
-    uint32_t *my_err = reinterpret_cast<uint32_t *>(cm.mine + kCommErrOff);
+    MailboxView mb = mailbox_view(cm, root, epoch);  // its slots are claimed only when the graph replays
     CommArgs *d_args = reinterpret_cast<CommArgs *>(cm.mine + kCommArgsOff);
     ExecSlot &es = *p->slot;
     // pinned words of this prepared query that the graph's memcpy nodes read / write: the last two zero pages of its slot
@@ -3197,7 +3195,7 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
         lk.unlock();
         return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
     }
-    auto &rg = p->reduce_graphs[root * 2 + static_cast<int>(parity)];
+    auto &rg = p->reduce_graphs[root * 2 + static_cast<int>(mb.parity)];
     // a graph reads its parts through the pointers captured with it (same rule as bydb_scan_agg_prepared)
     if (rg.exec) (void)check_held_parts(ctx, p->parts, rg.exec, rg.held);  // a missing part fails in make_plan below
     if (!rg.exec) {
@@ -3207,10 +3205,10 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
             lk.unlock();
             return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);  // takes part in the collective and reports the failure
         }
-        TableLayout tl(static_cast<size_t>(plan.n_groups), plan.fcols.size());
+        const TableLayout &tl = plan.tl;
         p->host_off = stage_layout(p->q.n_series, tl.G).stride;
         // the version-dedup precheck synchronises: such queries keep the plain path
-        if (parts_overlap(plan.parts, p->q.tmin, p->q.tmax) || tl.total > slot_bytes || es.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) {
+        if (parts_overlap(plan.parts, p->q.tmin, p->q.tmax) || tl.total > mb.slot_bytes || es.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) {
             p->reduce_capturable = false;
             lk.unlock();
             return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
@@ -3230,26 +3228,26 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
                 }
             };
             step("args copy", cudaMemcpyAsync(d_args, h_args, sizeof(CommArgs), cudaMemcpyHostToDevice, s) == cudaSuccess);
-            launch_comm_wait_args(done, 1, d_args, 1, my_err, kErrPeerTimeout, s);
+            launch_comm_wait_args(mb.done, 1, d_args, 1, mb.my_err, kErrPeerTimeout, s);
             step("wait for the slots", true);
-            step("scan", run_scan(ctx, &p->q, plan, es, s, my_slot, tl, &rg.captured) == 0);
+            step("scan", run_scan(ctx, &p->q, plan, es, s, mb.my_slot, tl, &rg.captured) == 0);
             rg.express = es.express[0];
-            launch_comm_signal_args(flags + cm.rank, status + cm.rank, d_args, s);
+            launch_comm_signal_args(mb.flags + cm.rank, mb.status + cm.rank, d_args, s);
             step("signal", true);
             if (cm.rank == root) {
-                launch_comm_wait_args(flags, static_cast<uint32_t>(cm.nranks), d_args, 0, my_err, kErrPeerTimeout, s);
+                launch_comm_wait_args(mb.flags, static_cast<uint32_t>(cm.nranks), d_args, 0, mb.my_err, kErrPeerTimeout, s);
                 step("wait for the ranks", true);
-                launch_combine_tables(slots0, static_cast<uint32_t>(cm.nranks), tl, s, slot_bytes);
+                launch_combine_tables(mb.slots0, static_cast<uint32_t>(cm.nranks), tl, s, mb.slot_bytes);
                 step("combine", true);
                 uint32_t fin_launches = 0;
-                step("finalize", finalize_enqueue(&p->q, plan, es, s, slots0, tl, p->host_off, fin, rg.fl, fin_launches) == 0);
-                launch_comm_done_args(done, d_args, s);
+                step("finalize", finalize_enqueue(&p->q, plan, es, s, mb.slots0, tl, p->host_off, fin, rg.fl, fin_launches) == 0);
+                launch_comm_done_args(mb.done, d_args, s);
                 step("done word", true);
                 step("status read-back",
-                     cudaMemcpyAsync(h_back + 8, status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost, s) == cudaSuccess);
+                     cudaMemcpyAsync(h_back + 8, mb.status, sizeof(unsigned long long) * static_cast<size_t>(cm.nranks), cudaMemcpyDeviceToHost, s) == cudaSuccess);
                 rg.captured.kernel_launches += 3 + fin_launches;
             }
-            step("error read-back", cudaMemcpyAsync(h_back, my_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, s) == cudaSuccess);
+            step("error read-back", cudaMemcpyAsync(h_back, mb.my_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, s) == cudaSuccess);
             rg.captured.kernel_launches += 2;
         }
         cudaGraph_t graph = nullptr;
@@ -3279,35 +3277,18 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
     }
     // ---- replay
     cm.epoch = epoch;
-    const uint64_t prev_use = cm.last_use[2 * static_cast<size_t>(root) + parity];
-    cm.last_use[2 * static_cast<size_t>(root) + parity] = epoch;
     h_args->epoch = epoch;
-    h_args->prev_use = prev_use;
+    h_args->prev_use = mb.claim_slots();
     memset(h_back, 0, kZeroPageBytes);
     memset(es.page(0), 0, kZeroPageBytes);
-    cudaStream_t s = es.stream;
-    CUDA_TRY(cudaEventRecord(p->t0, s));
-    CUDA_TRY(cudaGraphLaunch(rg.exec, s));
-    CUDA_TRY(cudaEventRecord(p->t1, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    CUDA_TRY(cudaGetLastError());
-    out->stats = rg.captured;  // host-side counters; the zero-page counters are still 0 there
-    float ms = 0;
-    cudaEventElapsedTime(&ms, p->t0, p->t1);
-    out->stats.device_ms = ms;
-    out->stats.scan_kernel_ms = 0;  // per-kernel events are not available inside a graph replay
+    const int rc = replay_graph(rg.exec, es, p->t0, p->t1, rg.captured, rg.express, &out->stats);
     const uint32_t perr = *reinterpret_cast<const uint32_t *>(h_back);
-    if (perr != 0) cudaMemset(my_err, 0, sizeof perr);
-    const int rc = read_zero_page(*es.page(0), rg.express, &out->stats);
+    if (perr != 0) cudaMemset(mb.my_err, 0, sizeof perr);
     if (rc) return rc;
     if (perr != 0) return fail(dev_err_code(perr), dev_err_text(perr));
     if (cm.rank != root) return 0;
-    const unsigned long long *peer_status = reinterpret_cast<const unsigned long long *>(h_back + 8);
-    for (int r = 0; r < cm.nranks; ++r) {
-        const unsigned long long w = peer_status[r];
-        if ((w >> 32) == (epoch & 0xffffffffull) && static_cast<uint32_t>(w) != 0)
-            return fail(-static_cast<int>(static_cast<uint32_t>(w)), "multi-GPU reduce: rank " + std::to_string(r) + " failed before its scan");
-    }
+    const int prc = peer_failure(reinterpret_cast<const unsigned long long *>(h_back + 8), cm.nranks, epoch, " failed before its scan");
+    if (prc) return prc;
     return finalize_parse(es.pinned + p->host_off, rg.fl, true, out);
     });
 }
@@ -3321,23 +3302,16 @@ int bydb_scan_reduce_host(bydb_ctx *ctx, uint32_t n_parts, const bydb_part_files
     memset(out, 0, sizeof *out);
     CUDA_TRY(cudaSetDevice(ctx->device));
     g_last_dev_err = 0;
-    std::vector<std::shared_ptr<Part>> tmp;
+    TransientParts tmp(ctx);
     uint64_t h2d = 0;
     int rc = validate_query(q, false);
     if (!rc && (n_parts == 0 || !parts || n_parts > kMaxParts)) rc = fail(BYDB_EINVAL, "need 1..64 host parts");
-    const bool zc = !rc && (q->flags & BYDB_Q_HOST_ZERO_COPY) != 0;
-    for (uint32_t i = 0; i < n_parts && !rc; ++i) {
-        std::shared_ptr<Part> p;
-        // fallback pages are unpacked up front here: a collective cannot be re-run by one rank alone
-        rc = register_part_locked_free(ctx, ~0ull - i, &parts[i], p, &h2d, zc, true, !zc);
-        if (!rc) tmp.push_back(p);
-    }
-    rc = scan_reduce_impl(ctx, q, &tmp, rc, h2d, root, out);
-    if (!rc && zc) out->stats.h2d_bytes += out->stats.page_bytes;  // pages were read in place over PCIe
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        for (auto &p : tmp) ctx->hbm_used -= p->hbm_bytes;
-    }
+    AdmitOptions opt;
+    opt.zero_copy = !rc && (q->flags & BYDB_Q_HOST_ZERO_COPY) != 0;
+    opt.unpack = !opt.zero_copy;  // fallback pages are unpacked up front here: a collective cannot be re-run by one rank alone
+    for (uint32_t i = 0; i < n_parts && !rc; ++i) rc = tmp.admit(&parts[i], &h2d, opt);
+    rc = scan_reduce_impl(ctx, q, &tmp.parts, rc, h2d, root, out);
+    if (!rc && opt.zero_copy) out->stats.h2d_bytes += out->stats.page_bytes;  // pages were read in place over PCIe
     return rc;
     });
 }
