@@ -2427,7 +2427,7 @@ constexpr int kExpressStageBytes = 2 * kSwarChunkBytes;
 constexpr int kExpressStages = BYDB_EXPRESS_STAGES;
 static_assert(kExpressStages >= 2, "the express ring refills a stage while the other is decoded");
 
-// the express lane's per-warp shared memory: its ring only (8 warps x 8 KB + barriers: three CTAs per SM)
+// the express lane's per-warp shared memory: its ring only (8 warps x 8 KB + barriers; its 127 registers hold it to two CTAs per SM)
 struct __align__(128) ExpressSmem {
     uint8_t stage[kExpressStages][kExpressStageBytes];
     uint64_t bar[kExpressStages];
@@ -2516,7 +2516,7 @@ __device__ __forceinline__ ExpressUnit express_unit(const uint8_t *src, uint32_t
     return r;
 }
 
-__global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_express_kernel(const __grid_constant__ ScanParams p) {
+__global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum_express_kernel(const __grid_constant__ ScanParams p) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -2656,6 +2656,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_ex
                         uint8_t *buf = ring_wait(sm, seq0 + s);
                         if (good) {
                             if (j == 0 || (j + 1) * kExpressStageBytes > pe_k) express_zero_edges(buf, j * kExpressStageBytes, ps_k, pe_k, lane);
+#if BYDB_EXPRESS_DECODE
                             const uint8_t *src = buf + lane * kSwarLaneBytes;
                             // the word in front of each window: lane l-1's last word of the same half; for lane 0, the
                             // previous unit's last word (half a) and lane 31's last word of half a (half b)
@@ -2687,6 +2688,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_ex
                                 S += static_cast<int64_t>(Aa) * eu.Ta + static_cast<int64_t>(Ab) * eu.Tb - static_cast<int64_t>(eu.Ra) - static_cast<int64_t>(eu.Rb);
                                 tb += static_cast<int32_t>((tot_n & 0xffffu) + (tot_n >> 16));
                             }
+#endif
                         }
                         if (j == nst_k - 1 && lane == 0) last_byte = buf[(pe_k - 1) % kExpressStageBytes];
                         __syncwarp();
@@ -2705,6 +2707,9 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_FAST_CTAS) scan_sum_ex
                     const int32_t zeros_after = static_cast<int32_t>(nst_k * kExpressStageBytes - pe_k);
                     if (nst_k == 0) good = count_k == 1;  // an empty body: the page holds `first` alone
                     else good = good && tb - zeros_after + 1 == static_cast<int32_t>(count_k) && last_byte < 0x80u;
+#if !BYDB_EXPRESS_DECODE
+                    good = true;  // the fetch-only build keeps every block in the express lane
+#endif
 #pragma unroll
                     for (int m = 16; m >= 1; m >>= 1) S += static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(S), m));
                     acc.add_scaled(first_k, count_k);

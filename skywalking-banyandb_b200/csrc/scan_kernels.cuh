@@ -20,6 +20,12 @@ constexpr int kWarpsPerCta = 8;          // 256 threads; every warp is an indepe
 #ifndef BYDB_EXPRESS_STAGES
 #define BYDB_EXPRESS_STAGES 2            // the express lane's own ring depth (its stages are 4 KB decode units)
 #endif
+#ifndef BYDB_EXPRESS_CTAS
+#define BYDB_EXPRESS_CTAS 2              // resident CTAs per SM the express lane is compiled for: 127 registers, no spills (DESIGN.md 4.2)
+#endif
+#ifndef BYDB_EXPRESS_DECODE
+#define BYDB_EXPRESS_DECODE 1            // 0: the express lane streams its pages and skips the decode (fetch timing only: WRONG sums)
+#endif
 #ifndef BYDB_SPARSE
 #define BYDB_SPARSE 0                    // 1: masked / ranged delta pages take delta_page_sparse (measured slower, see DESIGN.md 4.2; make variant EXTRA="-DBYDB_SPARSE=1 -DBYDB_STAGES=3")
 #endif
