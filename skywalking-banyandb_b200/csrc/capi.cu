@@ -1202,6 +1202,8 @@ int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
     sp.top_is_count = q->aggs[sp.top_agg].func == BYDB_AGG_COUNT;
     sp.rows = fp.rows;
     sp.cnt = fp.cnt;
+    sp.max_i64 = fp.max_i64;
+    sp.max_f64 = fp.max_f64;
     sp.val_i64 = fp.out_i64;
     sp.val_f64 = fp.out_f64;
     sp.is_float = fp.out_is_float;
@@ -2604,13 +2606,20 @@ int bydb_partials_rows(bydb_ctx *ctx, const bydb_query *q, const void *d_partial
             const size_t o = g * F + static_cast<size_t>(agg_fcol[a]);
             const bool isf = owner->is_float[a] != 0;
             const int64_t n = t.cnt[o];
+            const bool met = met_column(isf, n, t.max_i64[o], t.max_f64[o]);  // else MIN / MAX keep the zero value
             int64_t vi = 0, ci = 0;
             double vf = 0.0, cf = 0.0;
             switch (q->aggs[a].func) {
                 case BYDB_AGG_SUM: vi = t.sum_i64[o]; vf = t.sum_f64[o]; break;
                 case BYDB_AGG_COUNT: vi = n; vf = static_cast<double>(n); break;
-                case BYDB_AGG_MAX: vi = n > 0 ? t.max_i64[o] : INT64_MIN; vf = n > 0 ? t.max_f64[o] : -1.7976931348623157e308; break;
-                case BYDB_AGG_MIN: vi = n > 0 ? ~t.notmin_i64[o] : INT64_MAX; vf = n > 0 ? -t.negmin_f64[o] : 1.7976931348623157e308; break;
+                case BYDB_AGG_MAX:
+                    vi = n > 0 ? t.max_i64[o] : met ? INT64_MIN : 0;
+                    vf = n > 0 ? t.max_f64[o] : met ? -1.7976931348623157e308 : 0.0;
+                    break;
+                case BYDB_AGG_MIN:
+                    vi = n > 0 ? ~t.notmin_i64[o] : met ? INT64_MAX : 0;
+                    vf = n > 0 ? -t.negmin_f64[o] : met ? 1.7976931348623157e308 : 0.0;
+                    break;
                 case BYDB_AGG_MEAN: vi = t.sum_i64[o]; vf = t.sum_f64[o]; ci = n; cf = static_cast<double>(n); break;
             }
             owner->val_i64.push_back(isf ? 0 : vi);

@@ -2289,6 +2289,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kFastLane ? BYDB_FAST_CTAS 
                     err = kErrTypeMix;
                 } else {
                     if (!check_col_type(p, c, col.value_type, known_types)) err = kErrTypeMix;  // warp-uniform: every lane keeps the cache
+                    bp.mn.i = 1;  // kept rows met the column (met_column); the values below replace it
                     const uint8_t *page = part.files[col.file_id] + col.off;
                     AggAcc acc;
                     acc.init();
@@ -2938,7 +2939,10 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 2) dedup_kernel(const __gri
 // deterministic reduction of the per-block partials
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void combine(BlockPartial &a, const BlockPartial &b, bool is_float) {
-    if (b.cnt == 0) return;
+    if (b.cnt == 0) {
+        if (a.cnt == 0) a.mn.i |= b.mn.i;  // met_column
+        return;
+    }
     if (a.cnt == 0) {
         a = b;
         return;
@@ -2990,10 +2994,9 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
     // while the series has shown no row (every timestamp, INT64_MAX included, is a valid ts_min)
     int64_t kts = INT64_MAX;
     uint32_t krow = kKeyAbsent;
-    int64_t span_lo[4], span_hi[4];
-    int nspan = 0;
+    // the series' span in part `lane` (a) and part `lane + 32` (b); lo > hi while the part shows no selected block
+    int64_t alo = INT64_MAX, ahi = INT64_MIN, blo = INT64_MAX, bhi = INT64_MIN;
     int64_t slo = INT64_MAX, shi = INT64_MIN;  // the series' selected blocks over every part (ReduceParams::span)
-    bool overlap = false;
     for (uint32_t pi = 0; pi < p.n_parts; ++pi) {
         const DevPartRef &part = p.parts[pi];
         uint32_t lo = 0, hi = part.n_blocks;
@@ -3050,17 +3053,36 @@ __global__ void __launch_bounds__(256) series_reduce_kernel(const __grid_constan
         if (plo <= phi) {
             slo = plo < slo ? plo : slo;
             shi = phi > shi ? phi : shi;
-            for (int s = 0; s < nspan; ++s)
-                if (!(phi < span_lo[s] || plo > span_hi[s])) overlap = true;
-            if (nspan < 4) {
-                span_lo[nspan] = plo;
-                span_hi[nspan] = phi;
-                ++nspan;
-            } else {  // merge into the last span: conservative
-                span_lo[3] = plo < span_lo[3] ? plo : span_lo[3];
-                span_hi[3] = phi > span_hi[3] ? phi : span_hi[3];
+        }
+        if ((pi & 31u) == static_cast<uint32_t>(lane)) {
+            if (pi < 32) {
+                alo = plo;
+                ahi = phi;
+            } else {
+                blo = plo;
+                bhi = phi;
             }
         }
+    }
+    // Exact pairwise test of the part spans (kMaxParts = 64): lane l meets lane l + d for every d below the part count, and its
+    // own two parts.  Two spans overlap when both are non-empty and neither ends before the other begins.
+    bool overlap = false;
+    if (p.n_parts > 1) {
+        const uint32_t reach = p.n_parts < 32 ? p.n_parts : 32;
+        const auto meets = [](int64_t l0, int64_t h0, int64_t l1, int64_t h1) { return l0 <= h0 && l1 <= h1 && l0 <= h1 && l1 <= h0; };
+        overlap = meets(alo, ahi, blo, bhi);
+        for (uint32_t d = 1; d < reach; ++d) {
+            const int src = (lane + static_cast<int>(d)) & 31;
+            const int64_t oal = __shfl_sync(0xffffffffu, static_cast<long long>(alo), src);
+            const int64_t oah = __shfl_sync(0xffffffffu, static_cast<long long>(ahi), src);
+            overlap = overlap || meets(alo, ahi, oal, oah) || meets(blo, bhi, oal, oah);
+            if (p.n_parts > 32) {
+                const int64_t obl = __shfl_sync(0xffffffffu, static_cast<long long>(blo), src);
+                const int64_t obh = __shfl_sync(0xffffffffu, static_cast<long long>(bhi), src);
+                overlap = overlap || meets(alo, ahi, obl, obh) || meets(blo, bhi, obl, obh);
+            }
+        }
+        overlap = __any_sync(0xffffffffu, overlap);
     }
     if (p.Kts) {
 #pragma unroll
@@ -3138,10 +3160,11 @@ __global__ void __launch_bounds__(256) group_reduce_kernel(const __grid_constant
             const bool have = t.cnt > 0;
             p.cnt[o] = t.cnt;
             p.sum_f64[o] = (have && is_float) ? t.sum.f : 0.0;
-            p.max_f64[o] = (have && is_float) ? t.mx.f : -INFINITY;
+            const bool met = !have && t.mn.i != 0;  // met_column: the other type's maximum word carries it
+            p.max_f64[o] = (have && is_float) ? t.mx.f : (met && !is_float) ? 0.0 : -INFINITY;
             p.negmin_f64[o] = (have && is_float) ? -t.mn.f : -INFINITY;
             p.sum_i64[o] = (have && !is_float) ? t.sum.i : 0;
-            p.max_i64[o] = (have && !is_float) ? t.mx.i : INT64_MIN;
+            p.max_i64[o] = (have && !is_float) ? t.mx.i : (met && is_float) ? 0 : INT64_MIN;
             p.notmin_i64[o] = (have && !is_float) ? ~t.mn.i : INT64_MIN;
             // the scan's status rides in the table (bits 8..): an asynchronous bydb_scan_partials has no other way
             // to tell the rank that finalises that one of its blocks failed
@@ -3188,10 +3211,11 @@ __global__ void __launch_bounds__(256) group_reduce_small_kernel(const __grid_co
             const bool have = t.cnt > 0;
             p.cnt[o] = t.cnt;
             p.sum_f64[o] = (have && is_float) ? t.sum.f : 0.0;
-            p.max_f64[o] = (have && is_float) ? t.mx.f : -INFINITY;
+            const bool met = !have && t.mn.i != 0;  // met_column: the other type's maximum word carries it
+            p.max_f64[o] = (have && is_float) ? t.mx.f : (met && !is_float) ? 0.0 : -INFINITY;
             p.negmin_f64[o] = (have && is_float) ? -t.mn.f : -INFINITY;
             p.sum_i64[o] = (have && !is_float) ? t.sum.i : 0;
-            p.max_i64[o] = (have && !is_float) ? t.mx.i : INT64_MIN;
+            p.max_i64[o] = (have && !is_float) ? t.mx.i : (met && is_float) ? 0 : INT64_MIN;
             p.notmin_i64[o] = (have && !is_float) ? ~t.mn.i : INT64_MIN;
             if (g == 0) p.coltype[c] = static_cast<int64_t>(p.col_type[c]) | (static_cast<int64_t>(p.err[0]) << 8);
         }
@@ -3219,7 +3243,8 @@ __device__ __forceinline__ void finalize_group(const FinalizeParams &p, int32_t 
         int64_t vi = 0;
         double vf = 0.0;
         const int fn = p.agg_func[a];
-        if (typ != 0) {
+        // a group that never met the column keeps the zero value for MIN / MAX as well
+        if (typ != 0 && met_column(typ == BYDB_VT_FLOAT64, cnt, p.max_i64[o], p.max_f64[o])) {
             if (fn == BYDB_AGG_COUNT) {
                 vi = cnt;
                 if (p.row_path_types && typ == BYDB_VT_FLOAT64) vf = __ll2double_rn(cnt);  // countFunc[float64], function.go:78-93
@@ -3345,7 +3370,8 @@ __global__ void __launch_bounds__(1024) select_rows_kernel(const __grid_constant
         uint64_t k = 0;
         uint8_t st = 0;  // 0 = no output row, 1 = null aggregate, 2 = competes with key k
         if (p.rows[g] > 0) {
-            const bool null = !p.top_is_count && p.cnt[static_cast<size_t>(g) * p.n_fcols + p.top_fcol] == 0;
+            const size_t oc = static_cast<size_t>(g) * p.n_fcols + p.top_fcol;
+            const bool null = !p.top_is_count && !met_column(isf, p.cnt[oc], p.max_i64[oc], p.max_f64[oc]);
             if (null) {
                 st = 1;
                 ++my_null;

@@ -89,6 +89,15 @@ struct BlockPartial {
 };
 static_assert(sizeof(BlockPartial) == 32, "BlockPartial layout");
 
+// Whether a group met the column.  The reference creates a group's aggregation slot at its first kept row from a block that
+// has the column, null cell or not (aggregation.go:290-312): a group that never met the column keeps the zero value for MIN /
+// MAX, one that met only null cells the empty-fold sentinels.  A BlockPartial without values (cnt == 0) holds that bit in
+// mn.i (1 = met).  In the partial table a group without values holds it in the maximum word of the other type, which its
+// column never uses: 0 = met, the empty maximum (INT64_MIN / -inf) = not met; both combine across tables by maximum.
+__host__ __device__ __forceinline__ bool met_column(bool is_float, int64_t cnt, int64_t max_i64, double max_f64) {
+    return cnt > 0 || (is_float ? max_i64 == 0 : max_f64 == 0.0);
+}
+
 struct ScanParams {
     DevPartRef parts[kMaxParts];
     uint32_t n_parts;
@@ -183,6 +192,8 @@ struct SelectParams {
     uint32_t n_fcols, n_aggs;
     int32_t top_n, top_agg, top_desc, top_fcol, top_is_count;
     const int64_t *rows, *cnt;
+    const int64_t *max_i64;       // the table's maxima: with cnt, whether a group met the column (met_column)
+    const double *max_f64;
     const int64_t *val_i64;       // finalized values [n_groups * n_aggs]
     const double *val_f64;
     const uint8_t *is_float;      // [n_aggs]
