@@ -158,6 +158,10 @@ int ob_builder_append(ob_builder *b, size_t n, const uint64_t *sids, const int64
                       int n_fields, const ob_column *fields, int n_fams, const ob_family *fams);
 /* builds the in-memory part (mustInitFromDataPoints + Flush). */
 ob_part *ob_builder_finish(ob_builder *b);
+/* one part from n builders with their own schemas and disjoint series: each builder's blocks are cut as
+ * ob_builder_finish cuts them, then written in series order, each with its builder's tag families and fields.
+ * NULL (ob_last_error) when two builders share a series. */
+ob_part *ob_builder_finish_many(ob_builder *const *bs, int n_builders);
 
 /* open a part from raw file images (part.go:312-375). names: "meta.bin","primary.bin","timestamps.bin","fv.bin","<fam>.tf","<fam>.tfm" */
 ob_part *ob_part_open(int n_files, const char *const *names, const uint8_t *const *data, const size_t *lens);

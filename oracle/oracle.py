@@ -124,6 +124,8 @@ def lib():
                                     C.POINTER(_Column), C.c_int, C.POINTER(_Family)]
     L.ob_builder_finish.argtypes = [C.c_void_p]
     L.ob_builder_finish.restype = C.c_void_p
+    L.ob_builder_finish_many.argtypes = [C.POINTER(C.c_void_p), C.c_int]
+    L.ob_builder_finish_many.restype = C.c_void_p
     L.ob_part_open.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t)]
     L.ob_part_open.restype = C.c_void_p
     L.ob_part_free.argtypes = [C.c_void_p]
@@ -484,6 +486,27 @@ class PartBuilder:
         if not h:
             raise ValueError("ob_builder_finish: " + _err())
         return Part(h)
+
+
+MeasureRows = Tuple[object, object, object, Sequence[FieldSpec], Sequence[Tuple[str, Sequence[FieldSpec]]]]
+
+
+def build_mixed_part(measures: Sequence[MeasureRows]) -> Part:
+    """One part holding several measures' series, as a part of one group and shard does.
+
+    measures: (sids, ts, versions, fields, families) per measure, each with its own schema; no series may appear in
+    two measures.  Each measure's rows are cut into blocks exactly as PartBuilder.finish cuts them, and the blocks of
+    all measures are written in series order, so consecutive blocks carry different tag families and fields."""
+    builders = []
+    for sids, ts, versions, fields, families in measures:
+        b = PartBuilder()
+        b.append(sids, ts, versions, fields, families)
+        builders.append(b)
+    hs = (C.c_void_p * max(len(builders), 1))(*[b._h for b in builders])
+    h = lib().ob_builder_finish_many(hs, len(builders))
+    if not h:
+        raise ValueError("ob_builder_finish_many: " + _err())
+    return Part(h)
 
 
 # ------------------------------------------------------------------ query

@@ -732,61 +732,114 @@ static void write_block(bwriter *w, const ob_builder *b, uint64_t sid, const siz
     if (w->primary_block.len > OBI_MAX_UNCOMPRESSED_PRIMARY) flush_primary(w);
 }
 
+/* one block of a builder: rows keep[start, start + n) of series sid */
+typedef struct {
+    uint64_t sid;
+    size_t start, n;
+} bcut;
+typedef struct {
+    size_t *keep; /* surviving rows in (sid, ts, -version) order */
+    bcut *cuts;
+    size_t n_cuts;
+} bblocks;
+
+/* part.go:162-205 mustInitFromDataPoints: sort, dedup exactly as part.go:176-190 (note the tsPrev==0 quirk for the very
+ * first row) and cut into blocks; a cut of n == 0 is written as nothing, as write_block skips it */
+static void cut_blocks(const ob_builder *b, bblocks *out) {
+    size_t *perm = (size_t *)malloc(sizeof(size_t) * (b->n ? b->n : 1));
+    for (size_t i = 0; i < b->n; i++) perm[i] = i;
+    g_sort_b = b;
+    qsort(perm, b->n, sizeof(size_t), row_cmp);
+    out->keep = (size_t *)malloc(sizeof(size_t) * (b->n ? b->n : 1));
+    out->cuts = (bcut *)malloc(sizeof(bcut) * (b->n + 1));
+    out->n_cuts = 0;
+    size_t m = 0, index_prev = 0;
+    uint64_t sid_prev = 0, unc = 0;
+    int64_t ts_prev = 0;
+    for (size_t i = 0; i < b->n; i++) {
+        size_t r = perm[i];
+        uint64_t sid = b->sids[r];
+        if (sid_prev == 0) sid_prev = sid;
+        if (sid == sid_prev) {
+            if (ts_prev == b->ts[r]) continue; /* dps.skip(i) */
+            ts_prev = b->ts[r];
+        }
+        /* row survives at position m */
+        if (unc >= OBI_MAX_UNCOMPRESSED_BLOCK || (m - index_prev) > OBI_MAX_BLOCK_LENGTH || sid != sid_prev) {
+            out->cuts[out->n_cuts++] = (bcut){sid_prev, index_prev, m - index_prev};
+            sid_prev = sid;
+            index_prev = m;
+            ts_prev = b->ts[r];
+            unc = 0;
+        }
+        out->keep[m++] = r;
+        unc += row_uncompressed(b, r);
+    }
+    out->cuts[out->n_cuts++] = (bcut){sid_prev, index_prev, m - index_prev};
+    free(perm);
+}
+
 /* part.go:162-205 mustInitFromDataPoints + block_writer.go:264-285 Flush */
-ob_part *ob_builder_finish(ob_builder *b) {
+ob_part *ob_builder_finish(ob_builder *b) { return ob_builder_finish_many(&b, 1); }
+
+/* One part from several builders, each with its own schema: a part holds every series of its group and shard, and each
+ * block carries the tag families and fields of its own series (block.go:88-123 processTagFamilies / processTags).  Each
+ * builder's rows are cut exactly as ob_builder_finish cuts them; the blocks of all builders then go through one block
+ * writer in series order (part.go:192-205, block_writer.go:206-245), so primary blocks mix schemas and the .tf / .tfm
+ * files are shared by family name. */
+ob_part *ob_builder_finish_many(ob_builder *const *bs, int n_builders) {
     ob_part *p = (ob_part *)calloc(1, sizeof *p);
     /* fixed file order for reproducibility */
     obi_part_file(p, "meta.bin", 1);
     obi_part_file(p, "primary.bin", 1);
     obi_part_file(p, "timestamps.bin", 1);
     obi_part_file(p, "fv.bin", 1);
-    if (b->n == 0) {
+    size_t total = 0;
+    for (int k = 0; k < n_builders; k++) total += bs[k]->n;
+    if (total == 0) {
         ob_zstd_compress(&obi_part_file(p, "meta.bin", 0)->data, "", 0, 1);
         return p;
     }
-    size_t *perm = (size_t *)malloc(sizeof(size_t) * b->n);
-    for (size_t i = 0; i < b->n; i++) perm[i] = i;
-    g_sort_b = b;
-    qsort(perm, b->n, sizeof(size_t), row_cmp);
-    /* dedup exactly as part.go:176-190 (note the tsPrev==0 quirk for the very first row) */
-    size_t m = 0;
-    {
-        uint64_t sid_prev = 0;
-        int64_t ts_prev = 0;
-        /* first pass only computes the survivor list; block cutting needs the survivors */
-        size_t *keep = (size_t *)malloc(sizeof(size_t) * b->n);
-        size_t index_prev = 0;
-        uint64_t unc = 0;
-        bwriter w;
-        memset(&w, 0, sizeof w);
-        w.part = p;
-        for (size_t i = 0; i < b->n; i++) {
-            size_t r = perm[i];
-            uint64_t sid = b->sids[r];
-            if (sid_prev == 0) sid_prev = sid;
-            if (sid == sid_prev) {
-                if (ts_prev == b->ts[r]) continue; /* dps.skip(i) */
-                ts_prev = b->ts[r];
-            }
-            /* row survives at position m */
-            if (unc >= OBI_MAX_UNCOMPRESSED_BLOCK || (m - index_prev) > OBI_MAX_BLOCK_LENGTH || sid != sid_prev) {
-                write_block(&w, b, sid_prev, keep + index_prev, m - index_prev);
-                sid_prev = sid;
-                index_prev = m;
-                ts_prev = b->ts[r];
-                unc = 0;
-            }
-            keep[m++] = r;
-            unc += row_uncompressed(b, r);
+    bblocks *bb = (bblocks *)calloc((size_t)n_builders, sizeof(bblocks));
+    size_t *next = (size_t *)calloc((size_t)n_builders, sizeof(size_t));
+    for (int k = 0; k < n_builders; k++)
+        if (bs[k]->n) cut_blocks(bs[k], &bb[k]);
+    bwriter w;
+    memset(&w, 0, sizeof w);
+    w.part = p;
+    int overlap = 0;
+    for (;;) {
+        /* the builder whose next block has the smallest series; series of different builders never meet */
+        int best = -1;
+        for (int k = 0; k < n_builders; k++) {
+            if (next[k] >= bb[k].n_cuts) continue;
+            if (best >= 0 && bb[k].cuts[next[k]].sid == bb[best].cuts[next[best]].sid) overlap = 1;
+            if (best < 0 || bb[k].cuts[next[k]].sid < bb[best].cuts[next[best]].sid) best = k;
         }
-        write_block(&w, b, sid_prev, keep + index_prev, m - index_prev);
-        flush_primary(&w);
-        ob_zstd_compress(&obi_part_file(p, "meta.bin", 0)->data, w.meta_data.p, w.meta_data.len, 1);
+        if (best < 0 || overlap) break;
+        const uint64_t sid = bb[best].cuts[next[best]].sid;
+        while (next[best] < bb[best].n_cuts && bb[best].cuts[next[best]].sid == sid) {
+            const bcut *c = &bb[best].cuts[next[best]++];
+            write_block(&w, bs[best], c->sid, bb[best].keep + c->start, c->n);
+        }
+    }
+    for (int k = 0; k < n_builders; k++) {
+        free(bb[k].keep);
+        free(bb[k].cuts);
+    }
+    free(bb);
+    free(next);
+    if (overlap) {
         ob_buf_free(&w.meta_data);
         ob_buf_free(&w.primary_block);
-        free(keep);
+        ob_part_free(p);
+        ob_set_error("builder: a series appears in more than one builder");
+        return NULL;
     }
-    free(perm);
+    flush_primary(&w);
+    ob_zstd_compress(&obi_part_file(p, "meta.bin", 0)->data, w.meta_data.p, w.meta_data.len, 1);
+    ob_buf_free(&w.meta_data);
+    ob_buf_free(&w.primary_block);
     for (int i = 0; i < p->n_files; i++) p->compressed += p->files[i]->data.len;
     if (part_load_primary_index(p) != 0) {
         ob_part_free(p);

@@ -636,6 +636,50 @@ const char *index_err_text(uint32_t e) {
     return "block index error";
 }
 
+// The part's device directory [DevBlock[nb] | DevCol[nc] | file table], charged to the part: sets d_dir / d_blocks /
+// d_cols / d_files.
+int alloc_part_dir(bydb_ctx *ctx, Part &part, size_t nb, size_t nc, size_t n_files, cudaStream_t s, size_t *dir_bytes_out) {
+    const size_t off_cols = align_up(nb * sizeof(DevBlock), 256);
+    const size_t off_files = off_cols + align_up(nc * sizeof(DevCol), 256);
+    const size_t dir_bytes = off_files + align_up((n_files + 1) * sizeof(void *), 256);
+    if (int rc = hbm_reserve(ctx, dir_bytes)) return rc;
+    part.hbm_bytes += dir_bytes;
+    *dir_bytes_out = dir_bytes;
+    const cudaError_t ae = part.pool_stream ? cudaMallocAsync(reinterpret_cast<void **>(&part.d_dir), dir_bytes, s) : cudaMalloc(reinterpret_cast<void **>(&part.d_dir), dir_bytes);
+    if (ae != cudaSuccess) {
+        part.d_dir = nullptr;
+        return fail(BYDB_ENOMEM, "device allocation failed for the directory of part " + std::to_string(part.id));
+    }
+    part.d_blocks = reinterpret_cast<const DevBlock *>(part.d_dir);
+    part.d_cols = reinterpret_cast<const DevCol *>(part.d_dir + off_cols);
+    part.d_files = reinterpret_cast<const uint8_t *const *>(part.d_dir + off_files);
+    return 0;
+}
+
+// A part whose column names do not fit the device walker's table (more than kIndexMaxNames distinct names, or one longer
+// than kIndexNameMax bytes) is still a valid part: its directory comes from the host parser, with the host's file ids
+// (first use) renumbered onto the file table the caller laid the arena out by (sorted families).
+int build_part_dir_host_for_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Part &part, cudaStream_t s, size_t n_files, size_t *dir_bytes_out) {
+    PartDir dir;
+    std::string err;
+    if (int rc = build_part_dir(imgs, ctx->names, dir, err)) return fail(rc, "part " + std::to_string(part.id) + ": " + err);
+    std::vector<uint8_t> remap(dir.files.size(), 0);
+    for (size_t i = 0; i < dir.files.size(); ++i) {
+        size_t k = 0;
+        while (k < part.dir.files.size() && part.dir.files[k] != dir.files[i]) ++k;
+        if (k == part.dir.files.size()) return fail(BYDB_EINVAL, "part " + std::to_string(part.id) + ": " + dir.files[i] + " is not in the file table");
+        remap[i] = static_cast<uint8_t>(k);
+    }
+    for (DevCol &c : dir.cols) c.file_id = remap[c.file_id];
+    dir.files = std::move(part.dir.files);
+    part.dir = std::move(dir);
+    const size_t nb = part.dir.blocks.size(), nc = part.dir.cols.size();
+    if (int rc = alloc_part_dir(ctx, part, nb, nc, n_files, s, dir_bytes_out)) return rc;
+    if (nb) CUDA_TRY(cudaMemcpyAsync(const_cast<DevBlock *>(part.d_blocks), part.dir.blocks.data(), nb * sizeof(DevBlock), cudaMemcpyHostToDevice, s));
+    if (nc) CUDA_TRY(cudaMemcpyAsync(const_cast<DevCol *>(part.d_cols), part.dir.cols.data(), nc * sizeof(DevCol), cudaMemcpyHostToDevice, s));
+    return 0;
+}
+
 // files: the part's file table (timestamps.bin, fv.bin, <family>.tf ...) is already decided by the caller; d_dir_* are
 // allocated here once the counts are known.
 int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Part &part, const std::vector<std::string> &families, cudaStream_t s,
@@ -711,7 +755,9 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
     auto read_ctl = [&]() -> int {
         CUDA_TRY(cudaMemcpyAsync(&ctl, in.base + off_ctl, sizeof ctl, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(cudaStreamSynchronize(s));
-        if (ctl.err) return fail(BYDB_EINVAL, "part " + std::to_string(part.id) + ": " + index_err_text(ctl.err) + " (#" + std::to_string(ctl.err_where) + ")");
+        // more than 16 families in a block: a valid part this library does not read, as part_dir.cc says too
+        const int code = ctl.err == kIdxTooManyFamilies ? BYDB_ENOTSUP : BYDB_EINVAL;
+        if (ctl.err) return fail(code, "part " + std::to_string(part.id) + ": " + index_err_text(ctl.err) + " (#" + std::to_string(ctl.err_where) + ")");
         return 0;
     };
     // ---- meta.bin: size, then inflate + the primary frames' sizes
@@ -744,6 +790,9 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
     std::vector<IndexName> hnames(kIndexMaxNames);
     if (n_primary) CUDA_TRY(cudaMemcpyAsync(hpb.data(), pbs.base, n_primary * sizeof(IndexPrimary), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(hnames.data(), in.base + off_names, kIndexMaxNames * sizeof(IndexName), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(&ctl, in.base + off_ctl, sizeof ctl, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    if (ctl.err == kIdxNames) return build_part_dir_host_for_device(ctx, imgs, part, s, n_files, dir_bytes_out);
     rc = read_ctl();
     if (rc) return rc;
     uint64_t nb = 0, nc = 0;
@@ -765,20 +814,10 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
     if (n_primary) CUDA_TRY(cudaMemcpyAsync(pbs.base, hpb.data(), n_primary * sizeof(IndexPrimary), cudaMemcpyHostToDevice, s));
     CUDA_TRY(cudaMemcpyAsync(in.base + off_map, map.data(), kIndexMaxNames * sizeof(uint16_t), cudaMemcpyHostToDevice, s));
     // ---- the part's device directory, filled by the second walk
-    const size_t off_cols = align_up(nb * sizeof(DevBlock), 256);
-    const size_t off_files = off_cols + align_up(nc * sizeof(DevCol), 256);
-    const size_t dir_bytes = off_files + align_up((n_files + 1) * sizeof(void *), 256);
-    rc = hbm_reserve(ctx, dir_bytes);
+    rc = alloc_part_dir(ctx, part, nb, nc, n_files, s, dir_bytes_out);
     if (rc) return rc;
-    part.hbm_bytes += dir_bytes;
-    *dir_bytes_out = dir_bytes;
-    const cudaError_t ae = part.pool_stream ? cudaMallocAsync(reinterpret_cast<void **>(&part.d_dir), dir_bytes, s) : cudaMalloc(reinterpret_cast<void **>(&part.d_dir), dir_bytes);
-    if (ae != cudaSuccess) {
-        part.d_dir = nullptr;
-        return fail(BYDB_ENOMEM, "device allocation failed for the directory of part " + std::to_string(part.id));
-    }
-    ip.blocks = reinterpret_cast<DevBlock *>(part.d_dir);
-    ip.cols = reinterpret_cast<DevCol *>(part.d_dir + off_cols);
+    ip.blocks = const_cast<DevBlock *>(part.d_blocks);
+    ip.cols = const_cast<DevCol *>(part.d_cols);
     ip.n_blocks = nb;
     launch_index_walk(ip, true, s);
     launch_index_order(ip, s);
@@ -792,9 +831,6 @@ int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Par
     part.dir.max_block_rows = ctl.max_block_rows;
     part.dir.min_ts = nb ? ctl.min_ts : 0;
     part.dir.max_ts = nb ? ctl.max_ts : 0;
-    part.d_blocks = ip.blocks;
-    part.d_cols = ip.cols;
-    part.d_files = reinterpret_cast<const uint8_t *const *>(part.d_dir + off_files);
     return 0;
 }
 

@@ -107,18 +107,23 @@ __device__ uint32_t intern_name(const IndexParams &p, uint8_t kind, uint32_t fam
     }
 }
 
-struct NameCache {  // consecutive blocks share a schema: position -> (bytes, id), like part_dir.cc's positional cache
+// Consecutive blocks usually share a schema: position -> (family, bytes, id), like part_dir.cc's positional cache.  A part
+// holds the series of several measures, so a neighbouring block may carry the same tag name at the same position in
+// another family: a hit needs the family too.
+struct NameCache {
     const uint8_t *ptr[kIndexCacheSlots];
     uint32_t len[kIndexCacheSlots];
     uint32_t id[kIndexCacheSlots];
+    uint8_t fam[kIndexCacheSlots];  // tags: slot in IndexParams::families (< 251); fields: 0
 };
 __device__ uint32_t resolve_name(const IndexParams &p, NameCache &nc, uint32_t pos, uint8_t kind, uint32_t fam, const uint8_t *name, uint32_t len) {
-    if (pos < kIndexCacheSlots && nc.ptr[pos] && nc.len[pos] == len && bytes_equal(nc.ptr[pos], name, len)) return nc.id[pos];
+    if (pos < kIndexCacheSlots && nc.ptr[pos] && nc.fam[pos] == fam && nc.len[pos] == len && bytes_equal(nc.ptr[pos], name, len)) return nc.id[pos];
     const uint32_t id = intern_name(p, kind, fam, name, len);
     if (pos < kIndexCacheSlots) {
         nc.ptr[pos] = name;
         nc.len[pos] = len;
         nc.id[pos] = id;
+        nc.fam[pos] = static_cast<uint8_t>(fam);
     }
     return id;
 }

@@ -145,11 +145,13 @@ const FileImage *find_file(const std::vector<FileImage> &files, const std::strin
 }  // namespace
 
 // Parses one decompressed primary block (a run of blockMetadata records) into blocks/cols.
-// Column names are resolved through a positional cache first (consecutive blocks share a schema),
-// so the shared NameTable is only touched on a miss.
+// Column names are resolved through a positional cache first (consecutive blocks usually share a schema),
+// so the shared NameTable is only touched on a miss.  A part holds the series of several measures, so
+// neighbouring blocks may carry other families: a tag slot hits only for the same family, position and bytes.
 namespace {
 struct NameSlot {
     std::string raw;
+    size_t fam = SIZE_MAX;  // tags: slot in ParseCtx::fam_cache
     uint16_t id = 0;
 };
 struct ParseCtx {
@@ -168,8 +170,9 @@ struct ParseCtx {
     std::vector<FamSlot> fam_cache;
 };
 
-uint16_t resolve_name(ParseCtx &cx, std::vector<NameSlot> &cache, size_t pos, const char *prefix, const std::string &fam, const uint8_t *p, size_t n) {
-    if (pos < cache.size() && cache[pos].raw.size() == n && memcmp(cache[pos].raw.data(), p, n) == 0) return cache[pos].id;
+uint16_t resolve_name(ParseCtx &cx, std::vector<NameSlot> &cache, size_t pos, const char *prefix, size_t fam_slot, const std::string &fam, const uint8_t *p,
+                      size_t n) {
+    if (pos < cache.size() && cache[pos].fam == fam_slot && cache[pos].raw.size() == n && memcmp(cache[pos].raw.data(), p, n) == 0) return cache[pos].id;
     std::string key(prefix);
     if (!fam.empty()) key += fam + "/";
     key.append(reinterpret_cast<const char *>(p), n);
@@ -180,6 +183,7 @@ uint16_t resolve_name(ParseCtx &cx, std::vector<NameSlot> &cache, size_t pos, co
     }
     if (pos >= cache.size()) cache.resize(pos + 1);
     cache[pos].raw.assign(reinterpret_cast<const char *>(p), n);
+    cache[pos].fam = fam_slot;
     cache[pos].id = id;
     return id;
 }
@@ -275,7 +279,7 @@ int parse_primary_block(ParseCtx &cx, const uint8_t *data, size_t len, std::vect
                 return BYDB_EINVAL;
             }
             col.size = static_cast<uint32_t>(size);
-            col.name_id = resolve_name(cx, cx.field_cache, i, "f:", std::string(), np, nl);
+            col.name_id = resolve_name(cx, cx.field_cache, i, "f:", SIZE_MAX, std::string(), np, nl);
             col.file_id = 1;
             cols.push_back(col);
         }
@@ -309,7 +313,7 @@ int parse_primary_block(ParseCtx &cx, const uint8_t *data, size_t len, std::vect
                     return BYDB_EINVAL;
                 }
                 col.size = static_cast<uint32_t>(size);
-                col.name_id = resolve_name(cx, cx.tag_cache, tag_pos, "t:", fs.name, np, nl);
+                col.name_id = resolve_name(cx, cx.tag_cache, tag_pos, "t:", fams[fi].slot, fs.name, np, nl);
                 col.file_id = static_cast<uint8_t>(fs.file_id);
                 cols.push_back(col);
             }
