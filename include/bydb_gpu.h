@@ -283,7 +283,9 @@ void bydb_query_release(bydb_ctx *ctx, bydb_prepared *pq);
  * so that ONE all-reduce(SUM) over [sum_f64] + [sum_i64,cnt,rows] and one all-reduce(MAX) over the
  * max/negmin halves combine ranks (min is carried as max of the negation; int64 negation of
  * INT64_MIN is handled by carrying ~x instead of -x).  bydb_partials_layout reports the byte
- * offsets so the caller can issue the collectives on sub-ranges. */
+ * offsets so the caller can issue the collectives on sub-ranges.  A caller that merges tables with its own
+ * all-reduce(MAX) over n_max_i64 cannot see a field stored as int64 on one rank and float64 on another;
+ * bydb_partials_combine reports that type mix (BYDB_EINVAL at bydb_reduce_finalize / bydb_partials_rows). */
 typedef struct {
     uint64_t total_bytes;
     uint64_t off_sum_f64, off_max_f64;   /* [sum_f64] , [max_f64 | negmin_f64]                 */

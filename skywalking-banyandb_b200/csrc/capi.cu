@@ -1235,11 +1235,11 @@ int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
     sp.top_agg = q->top_n > 0 ? q->top_agg : 0;
     sp.top_desc = q->top_desc;
     sp.top_fcol = plan.agg_fcol[sp.top_agg];
-    sp.top_is_count = q->aggs[sp.top_agg].func == BYDB_AGG_COUNT;
     sp.rows = fp.rows;
     sp.cnt = fp.cnt;
     sp.max_i64 = fp.max_i64;
     sp.max_f64 = fp.max_f64;
+    sp.coltype = fp.coltype;
     sp.val_i64 = fp.out_i64;
     sp.val_f64 = fp.out_f64;
     sp.is_float = fp.out_is_float;

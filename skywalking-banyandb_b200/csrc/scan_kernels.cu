@@ -3371,7 +3371,10 @@ __global__ void __launch_bounds__(1024) select_rows_kernel(const __grid_constant
         uint8_t st = 0;  // 0 = no output row, 1 = null aggregate, 2 = competes with key k
         if (p.rows[g] > 0) {
             const size_t oc = static_cast<size_t>(g) * p.n_fcols + p.top_fcol;
-            const bool null = !p.top_is_count && !met_column(isf, p.cnt[oc], p.max_i64[oc], p.max_f64[oc]);
+            // a group that never met the column has no aggregate, COUNT included (a COUNT over a float64 field is typed int64,
+            // so the met bit is read by the field's type); one that met only null cells competes with its sentinel / 0
+            const int64_t typ = p.coltype[p.top_fcol] & 0xff;
+            const bool null = typ == 0 || !met_column(typ == BYDB_VT_FLOAT64, p.cnt[oc], p.max_i64[oc], p.max_f64[oc]);
             if (null) {
                 st = 1;
                 ++my_null;
@@ -3554,9 +3557,19 @@ __global__ void __launch_bounds__(1024) select_rows_kernel(const __grid_constant
 }
 
 
+// Column type and status of several passes' (or ranks') coltype words (type in bits 0..7, DevErr above): the type any of them
+// saw, a type mix when two disagree, the worst status.
+__device__ __forceinline__ void merge_coltype(int64_t w, int64_t &typ, int64_t &err) {
+    const int64_t wt = w & 0xff, we = w >> 8;
+    if (wt != 0 && typ != 0 && wt != typ) err = err > static_cast<int64_t>(kErrTypeMix) ? err : static_cast<int64_t>(kErrTypeMix);
+    if (typ == 0) typ = wt;
+    err = we > err ? we : err;
+}
+
 // How one word of a partial table combines with the same word of another rank's table.  kind: 0 float sum, 1 float maximum
-// (max, -min), 2 int64 sum (sum, count, rows), 3 int64 maximum (max, ~min, coltype); anything else keeps `a`.
-enum : int { kWordFsum = 0, kWordFmax = 1, kWordIsum = 2, kWordImax = 3 };
+// (max, -min), 2 int64 sum (sum, count, rows), 3 int64 maximum (max, ~min), 4 column type + status (merge_coltype: a field
+// stored as int64 in one table and float64 in another is a type mix, as inside one scan); anything else keeps `a`.
+enum : int { kWordFsum = 0, kWordFmax = 1, kWordIsum = 2, kWordImax = 3, kWordColtype = 4 };
 __device__ __forceinline__ uint64_t combine_word(uint64_t a, uint64_t b, int kind) {
     if (kind == kWordFsum)
         return static_cast<uint64_t>(__double_as_longlong(__longlong_as_double(static_cast<long long>(a)) + __longlong_as_double(static_cast<long long>(b))));
@@ -3566,30 +3579,29 @@ __device__ __forceinline__ uint64_t combine_word(uint64_t a, uint64_t b, int kin
     }
     if (kind == kWordIsum) return a + b;  // wraps like Go's int64
     if (kind == kWordImax) return static_cast<uint64_t>(static_cast<int64_t>(b) > static_cast<int64_t>(a) ? b : a);
+    if (kind == kWordColtype) {
+        int64_t typ = 0, err = 0;
+        merge_coltype(static_cast<int64_t>(a), typ, err);
+        merge_coltype(static_cast<int64_t>(b), typ, err);
+        return static_cast<uint64_t>(typ | (err << 8));
+    }
     return a;
 }
 
 // Multi-GPU reduce after ONE all-gather of the per-rank partial tables: every word of the table is
 // combined across ranks in rank order (deterministic float sums, unlike a ring all-reduce), which is
 // the liaison's reduceAccumulator.Combine (measure_plan_aggregation.go:96-124) done on the device.
+// The F coltype words [ct_lo, ct_hi) merge like permute_table_kernel merges passes, so a field that is
+// int64 in one table and float64 in another fails the finalisation instead of dropping one type's values.
 __global__ void combine_tables_kernel(uint64_t *t, uint32_t n, uint64_t words, uint64_t stride, uint64_t sf_lo, uint64_t sf_hi, uint64_t mf_lo, uint64_t mf_hi,
-                                      uint64_t si_lo, uint64_t si_hi, uint64_t mi_lo, uint64_t mi_hi) {
+                                      uint64_t si_lo, uint64_t si_hi, uint64_t mi_lo, uint64_t mi_hi, uint64_t ct_lo, uint64_t ct_hi) {
     const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= words) return;
     const int kind = (i >= sf_lo && i < sf_hi) ? kWordFsum : (i >= mf_lo && i < mf_hi) ? kWordFmax : (i >= si_lo && i < si_hi) ? kWordIsum
-                   : (i >= mi_lo && i < mi_hi) ? kWordImax : -1;
+                   : (i >= mi_lo && i < mi_hi) ? kWordImax : (i >= ct_lo && i < ct_hi) ? kWordColtype : -1;
     uint64_t a = t[i];
     for (uint32_t r = 1; r < n; ++r) a = combine_word(a, t[static_cast<uint64_t>(r) * stride + i], kind);
     t[i] = a;
-}
-
-// Column type and status of several passes' (or ranks') coltype words (type in bits 0..7, DevErr above): the type any of them
-// saw, a type mix when two disagree, the worst status.
-__device__ __forceinline__ void merge_coltype(int64_t w, int64_t &typ, int64_t &err) {
-    const int64_t wt = w & 0xff, we = w >> 8;
-    if (wt != 0 && typ != 0 && wt != typ) err = err > static_cast<int64_t>(kErrTypeMix) ? err : static_cast<int64_t>(kErrTypeMix);
-    if (typ == 0) typ = wt;
-    err = we > err ? we : err;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -4256,10 +4268,12 @@ void launch_group_reduce(const ReduceParams &p, cudaStream_t s, bool small_group
 void launch_combine_tables(uint8_t *tables, uint32_t n_tables, const TableLayout &tl, cudaStream_t s, size_t stride_bytes) {
     const uint64_t words = tl.total / 8;
     if (words == 0 || n_tables < 2) return;
-    // word ranges by how they combine: float sums | float maxima (max, -min) | int64 sums (sum, count, rows) | int64 maxima (max, ~min, coltype)
+    // word ranges by how they combine: float sums | float maxima (max, -min) | int64 sums (sum, count, rows) | int64 maxima (max, ~min)
+    // | column types + status (merge_coltype)
     combine_tables_kernel<<<static_cast<unsigned>((words + 255) / 256), 256, 0, s>>>(
         reinterpret_cast<uint64_t *>(tables), n_tables, words, stride_bytes ? stride_bytes / 8 : words, tl.off_sum_f64 / 8, tl.off_max_f64 / 8,
-        tl.off_max_f64 / 8, tl.off_sum_i64 / 8, tl.off_sum_i64 / 8, tl.off_max_i64 / 8, tl.off_max_i64 / 8, words);
+        tl.off_max_f64 / 8, tl.off_sum_i64 / 8, tl.off_sum_i64 / 8, tl.off_max_i64 / 8, tl.off_max_i64 / 8, tl.off_coltype / 8,
+        tl.off_coltype / 8, words);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -190,10 +190,11 @@ constexpr int kMaxDeviceTopN = 2048;
 struct SelectParams {
     int32_t n_groups;
     uint32_t n_fcols, n_aggs;
-    int32_t top_n, top_agg, top_desc, top_fcol, top_is_count;
+    int32_t top_n, top_agg, top_desc, top_fcol;
     const int64_t *rows, *cnt;
     const int64_t *max_i64;       // the table's maxima: with cnt, whether a group met the column (met_column)
     const double *max_f64;
+    const int64_t *coltype;       // the table's column types: met_column reads the word of the FIELD's type, whatever the output type
     const int64_t *val_i64;       // finalized values [n_groups * n_aggs]
     const double *val_f64;
     const uint8_t *is_float;      // [n_aggs]
