@@ -142,7 +142,7 @@ typedef struct {
     uint64_t rows_matched;    /* rows folded into an aggregate                               */
     uint64_t blocks_scanned;
     uint64_t page_bytes;      /* encoded page bytes the scan kernel consumed                 */
-    uint64_t h2d_bytes;       /* host->device bytes moved by this call                       */
+    uint64_t h2d_bytes;       /* host->device bytes moved by this call (a replayed prepared query: 0) */
     uint64_t d2h_bytes;       /* device->host bytes moved by this call                       */
     double scan_kernel_ms;    /* CUDA-event time of the scan kernel on the call's stream     */
     double device_ms;         /* CUDA-event time of all kernels of the call                  */
@@ -264,13 +264,26 @@ int bydb_scan_agg_host(bydb_ctx *ctx, uint32_t n_parts, const bydb_part_files *p
 void bydb_result_free(bydb_ctx *ctx, bydb_result *r);
 
 /* Prepared queries.  A query that is executed many times (dashboard refresh, alert rule) is copied and planned once;
- * from its third execution on, the whole step -- staging copy, block selection, scan, reduce, finalisation, row
+ * from its third execution on, the whole step -- block selection, scan, reduce, finalisation, row
  * selection, read-back -- is replayed as ONE captured CUDA graph: one launch and one synchronisation per call instead of
  * ~20 runtime calls.  Every execution still scans the parts (nothing is cached but the launch sequence).  Results and
  * errors are those of bydb_scan_agg; stats.scan_kernel_ms is 0 on replays (per-kernel events do not exist inside a
  * graph), stats.device_ms is the whole graph.  Queries whose parts overlap in time (version dedup needs a host
  * decision) transparently keep the ordinary path.  One execution at a time per prepared query; different prepared
- * queries run concurrently.  The parts named by the query must stay registered while it exists. */
+ * queries run concurrently.  The parts named by the query must stay registered while it exists.
+ * A replay is nine graph nodes: a reset kernel, block selection, the three scan lanes, the two reduce kernels, finalisation +
+ * row selection, and ONE device-to-host copy that carries the result rows and the step's status and counters.  Its stats say so:
+ * kernel_launches = the plain call's + 1 (the reset kernel), h2d_bytes = 0 (the series list went up when the step was captured),
+ * d2h_bytes = the size of that one copy (the plain call's two copies together).
+ * Device memory a captured query keeps until bydb_query_release, or until one of its handles stops naming the part it was
+ * captured with (then the next execution captures again); it is not charged to hbm_budget_bytes.  With NS series, G groups,
+ * F distinct fields, A aggregations, P parts, NB blocks in those parts and R = min(top_n, G) or G result rows, each term rounded
+ * up to 256 B:
+ *   the partial table (bydb_partials_layout.total_bytes: 56*G*F + 8*G + 8*F)
+ *   + 12*NS + 4*(G+1) + NB*(36 + 32*F) + NS*(32*F + 8) + 4*NS*P (left out above 16 Mi entries)     the scan's lists and partials
+ *   + G*(16*A + 9) + 16 + A + R*(12 + 16*A)                                                        finalisation and result rows
+ *   + 512                                                                                          the zero page and its read-back image.
+ * bench.py's query (NS 10,000, G 1,000, F 1, A 2, P 1, NB 130,000, R 100) keeps 9.5 MB. */
 typedef struct bydb_prepared bydb_prepared;
 int bydb_query_prepare(bydb_ctx *ctx, const bydb_query *q, bydb_prepared **out);
 int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *pq, bydb_result *out);

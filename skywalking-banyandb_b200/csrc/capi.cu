@@ -5,6 +5,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdio>
 #include <chrono>
 #include <condition_variable>
@@ -272,6 +273,7 @@ struct bydb_ctx {
     NameTable names;
     std::unordered_map<bydb_part_h, std::shared_ptr<Part>> parts;
     std::unordered_map<uint64_t, bydb_part_h> by_id;
+    std::atomic<uint64_t> parts_gen{0};  // bumped under mu whenever a handle starts or stops naming a part (see check_held_parts)
     bydb_part_h next_handle = 1;
     std::vector<std::unique_ptr<ExecSlot>> free_slots;
     WorkPool pool;
@@ -608,14 +610,21 @@ struct TransientParts {
 // the handful of interned column names to the context's ids.  Fills part.dir (host copy of the directory) and writes
 // DevBlock[] / DevCol[] straight into the part's device directory.
 // ------------------------------------------------------------------------------------------------
-// device memory from the stream-ordered pool, freed on its stream (behind the work that uses it) when this goes out of scope
+// device memory from the stream-ordered pool, freed on its stream (behind the work that uses it) when this goes out of scope;
+// or, after view(), a region of memory someone else owns (a prepared query's StepState): alloc() then only checks the size
 struct Scratch {
     uint8_t *base = nullptr;
     cudaStream_t stream = nullptr;
+    size_t resident = 0;  // bytes of the viewed region; 0 = memory of the pool
     ~Scratch() {
-        if (base) cudaFreeAsync(base, stream);
+        if (base && !resident) cudaFreeAsync(base, stream);
+    }
+    void view(uint8_t *at, size_t bytes) {
+        base = at;
+        resident = bytes;
     }
     cudaError_t alloc(size_t n, cudaStream_t s) {
+        if (resident) return n <= resident ? cudaSuccess : cudaErrorMemoryAllocation;
         stream = s;
         return cudaMallocAsync(reinterpret_cast<void **>(&base), n ? n : 256, s);
     }
@@ -935,9 +944,10 @@ FinalLayout final_layout(size_t G, size_t A, int32_t top_n) {
 }
 
 // pinned bytes of a step over G series groups whose finalisation sees out_groups groups: run_scan's staging of each batch, then
-// the read-back of the results.  A prepared graph keeps the two apart (its results land at host_off = the staging's stride).
+// the read-back of the results.  A prepared graph keeps the two apart (its results land at host_off = the staging's stride) and
+// reads its zero page back behind the result rows, in the same copy: kZeroPageBytes more.
 size_t step_pinned_bytes(const bydb_query *q, size_t G, size_t out_groups, size_t batches = 1) {
-    return stage_layout(q->n_series, G).stride * batches + final_layout(out_groups, q->n_aggs, q->top_n).out_bytes;
+    return stage_layout(q->n_series, G).stride * batches + final_layout(out_groups, q->n_aggs, q->top_n).out_bytes + kZeroPageBytes;
 }
 
 // the partial-table pointers of ReduceParams / FinalizeParams (the names and order of TablePtrs)
@@ -986,8 +996,41 @@ struct KeyedPass {
     int64_t *span;      // [2 * n_series] see ReduceParams::span, or NULL
 };
 
+// device scratch of run_scan: zero page | staging (sids, order, group_start) | block lists | block and series partials |
+// first_block (n_first = 0: not used) | version-dedup index
+struct ScanLayout {
+    size_t off_zero, off_sids, off_worklist, off_slowlist, off_restlist, off_qsid, off_P, off_Prows, off_Pfirst, off_S, off_Srows, n_first, off_first,
+        off_dd_index, off_dd_rowoff, off_dd_list, total;
+};
+ScanLayout scan_layout(const StageLayout &st, size_t NB, size_t F, size_t n_parts, bool keyed) {
+    ScanLayout sl;
+    Carve carve;
+    sl.off_zero = carve(kZeroPageBytes);
+    sl.off_sids = carve(st.bytes);  // the staging as it is: one copy brings sids, order and group_start
+    sl.off_worklist = carve(NB * 4);
+    sl.off_slowlist = carve(NB * 4);
+    sl.off_restlist = carve(NB * 4);
+    sl.off_qsid = carve(NB * 4);
+    sl.off_P = carve(NB * F * sizeof(BlockPartial));
+    sl.off_Prows = carve(NB * 4);
+    sl.off_Pfirst = carve(keyed ? NB * 4 : 0);
+    sl.off_S = carve(st.NS * F * sizeof(BlockPartial));
+    sl.off_Srows = carve(st.NS * 8);
+    const size_t n_first = st.NS * n_parts;
+    sl.n_first = n_first <= (16u << 20) ? n_first : 0;
+    sl.off_first = carve(sl.n_first * 4);
+    sl.off_dd_index = carve(NB * 4);
+    sl.off_dd_rowoff = carve(NB * 8);
+    sl.off_dd_list = carve(NB * 4);
+    sl.total = carve.o;
+    return sl;
+}
+
+// resident: the scratch is a view into a prepared query's StepState whose staging was uploaded when the state was built, and the
+// step is being captured for replay: one reset kernel instead of the memsets, no staging copy, and the zero page is left for
+// finalize_enqueue to read back with the result rows.
 int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cudaStream_t stream, uint8_t *d_table, const TableLayout &tl,
-             bydb_stats *stats, int batch = 0, const KeyedPass *kp = nullptr) {
+             bydb_stats *stats, int batch = 0, const KeyedPass *kp = nullptr, Scratch *resident = nullptr) {
     cudaEvent_t *ev = slot.ev + 4 * batch;
     ZeroPage *hz = slot.page(batch);
     memset(hz, 0, kZeroPageBytes);  // a failure before the read-back is enqueued must not leave a previous call's status behind
@@ -1000,31 +1043,26 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     if (slot.ensure_pinned(st.stride * static_cast<size_t>(batch + 1))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     uint8_t *h = slot.pinned + st.stride * static_cast<size_t>(batch);
     stage_series(q, st, h);
-    // ---- device scratch layout
-    Carve carve;
-    const size_t off_zero = carve(kZeroPageBytes);
-    const size_t off_sids = carve(st.bytes);  // the staging as it is: one copy brings sids, order and group_start
-    const size_t off_worklist = carve(NB * 4);
-    const size_t off_slowlist = carve(NB * 4);
-    const size_t off_restlist = carve(NB * 4);
-    const size_t off_qsid = carve(NB * 4);
-    const size_t off_P = carve(NB * F * sizeof(BlockPartial));
-    const size_t off_Prows = carve(NB * 4);
-    const size_t off_Pfirst = carve(kp ? NB * 4 : 0);
-    const size_t off_S = carve(NS * F * sizeof(BlockPartial));
-    const size_t off_Srows = carve(NS * 8);
-    const size_t n_first = NS * plan.parts.size();
-    const bool use_first = n_first > 0 && n_first <= (16u << 20);
-    const size_t off_first = carve(use_first ? n_first * 4 : 0);
-    const size_t off_dd_index = carve(NB * 4), off_dd_rowoff = carve(NB * 8), off_dd_list = carve(NB * 4);
-    Scratch sc;
-    CUDA_TRY(sc.alloc(carve.o, stream));
+    // ---- device scratch
+    const ScanLayout sl = scan_layout(st, NB, F, plan.parts.size(), kp != nullptr);
+    const size_t off_sids = sl.off_sids, off_worklist = sl.off_worklist, off_slowlist = sl.off_slowlist, off_restlist = sl.off_restlist, off_qsid = sl.off_qsid,
+                 off_P = sl.off_P, off_Prows = sl.off_Prows, off_Pfirst = sl.off_Pfirst, off_S = sl.off_S, off_Srows = sl.off_Srows, off_first = sl.off_first,
+                 off_dd_index = sl.off_dd_index, off_dd_rowoff = sl.off_dd_rowoff, off_dd_list = sl.off_dd_list;
+    const bool use_first = sl.n_first > 0;
+    Scratch pooled;
+    Scratch &sc = resident ? *resident : pooled;
+    CUDA_TRY(sc.alloc(sl.total, stream));
     uint8_t *d = sc.base;
-    ZeroPage *z = reinterpret_cast<ZeroPage *>(d + off_zero);
-    CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
-    if (use_first) CUDA_TRY(cudaMemsetAsync(d + off_first, 0xff, n_first * 4, stream));
-    CUDA_TRY(cudaMemcpyAsync(d + off_sids, h, st.bytes, cudaMemcpyHostToDevice, stream));
-    if (stats) stats->h2d_bytes += st.bytes;
+    ZeroPage *z = reinterpret_cast<ZeroPage *>(d + sl.off_zero);
+    if (resident) {
+        launch_step_reset(reinterpret_cast<uint32_t *>(z), use_first ? reinterpret_cast<uint32_t *>(d + off_first) : nullptr, sl.n_first, stream);
+        if (stats) stats->kernel_launches += 1;
+    } else {
+        CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
+        if (use_first) CUDA_TRY(cudaMemsetAsync(d + off_first, 0xff, sl.n_first * 4, stream));
+        CUDA_TRY(cudaMemcpyAsync(d + off_sids, h, st.bytes, cudaMemcpyHostToDevice, stream));
+        if (stats) stats->h2d_bytes += st.bytes;
+    }
 
     ScanParams sp;
     memset(&sp, 0, sizeof sp);
@@ -1152,10 +1190,10 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     launch_group_reduce(rp, stream, small_groups);
     CUDA_TRY(cudaEventRecord(ev[3], stream));
     // read back the zero page (errors + counters); the caller synchronises and then calls collect_scan
-    CUDA_TRY(cudaMemcpyAsync(hz, z, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
+    if (!resident) CUDA_TRY(cudaMemcpyAsync(hz, z, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
     if (stats) {
         stats->kernel_launches += (NB ? 1u : 0u) + 2u + (NS ? 1u : 0u) + 1u + extra_launches;
-        stats->d2h_bytes += kZeroPageBytes;
+        if (!resident) stats->d2h_bytes += kZeroPageBytes;
     }
     // the scratch must outlive the kernels: it is freed stream-ordered (after them) when `sc` goes out of scope
     return 0;
@@ -1202,14 +1240,17 @@ int table_status(uint32_t e) {
 }
 
 // finalisation + row selection of the table at d_table, up to and including the read-back copy to slot.pinned + host_off;
-// fl = final_layout() of the query, launches = kernels launched
+// fl = final_layout() of the query, launches = kernels launched, read_back = bytes of that copy.  d_zero: the step's zero page on
+// the device, gathered by the last kernel into kZeroPageBytes behind fl.total and read back in the same copy (it lands at
+// host_off + fl.out_bytes); NULL: the caller reads the zero page back itself.
 int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t stream, const uint8_t *d_table, const TableLayout &tl,
-                     size_t host_off, Scratch &sc, FinalLayout &fl, uint32_t &launches) {
+                     size_t host_off, Scratch &sc, FinalLayout &fl, uint32_t &launches, size_t &read_back, const uint8_t *d_zero = nullptr) {
     const size_t F = plan.fcols.size();
     const int32_t G = plan.n_groups;
     const size_t A = q->n_aggs;
     fl = final_layout(static_cast<size_t>(G), A, q->top_n);
-    CUDA_TRY(sc.alloc(fl.total, stream));
+    read_back = fl.out_bytes + (d_zero ? kZeroPageBytes : 0);
+    CUDA_TRY(sc.alloc(fl.o_out + read_back, stream));
     uint8_t *d = sc.base;
     FinalizeParams fp;
     memset(&fp, 0, sizeof fp);
@@ -1250,9 +1291,13 @@ int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
     sp.sel_rows = reinterpret_cast<int64_t *>(d + fl.o_sr);
     sp.sel_i64 = reinterpret_cast<int64_t *>(d + fl.o_si);
     sp.sel_f64 = reinterpret_cast<double *>(d + fl.o_sf);
+    if (d_zero) {
+        sp.zero_src = reinterpret_cast<const uint32_t *>(d_zero);
+        sp.zero_dst = reinterpret_cast<uint32_t *>(d + fl.total);
+    }
     launches = launch_finalize_select(fp, sp, stream);
-    if (slot.ensure_pinned(host_off + fl.out_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned + host_off, d + fl.o_out, fl.out_bytes, cudaMemcpyDeviceToHost, stream));
+    if (slot.ensure_pinned(host_off + read_back)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned + host_off, d + fl.o_out, read_back, cudaMemcpyDeviceToHost, stream));
     return 0;
 }
 
@@ -1293,11 +1338,12 @@ int finalize_to_host(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
     FinalLayout fl;
     uint32_t launches = 0;
     Scratch sc;
-    int rc = finalize_enqueue(q, plan, slot, stream, d_table, tl, 0, sc, fl, launches);
+    size_t read_back = 0;
+    int rc = finalize_enqueue(q, plan, slot, stream, d_table, tl, 0, sc, fl, launches, read_back);
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(stream));
     CUDA_TRY(cudaGetLastError());
-    out->stats.d2h_bytes += fl.out_bytes;
+    out->stats.d2h_bytes += read_back;
     out->stats.kernel_launches += launches;
     return finalize_parse(slot.pinned, fl, carried_status, out);
 }
@@ -1381,6 +1427,13 @@ struct bydb_prepared {
     FinalLayout fl;
     size_t host_off = 0;
     std::vector<std::shared_ptr<Part>> held;  // the parts whose device pointers are baked into the graph stay alive with it
+    uint64_t held_gen = 0;             // bydb_ctx::parts_gen at which `held` was last compared with the handles
+    // StepState: the device memory of the captured step, one allocation that lives as long as the graph.  Carved as
+    // partial table | run_scan's scratch (scan_layout) | finalize_enqueue's (final_layout) | the zero page's read-back image;
+    // the staging (sids | order | group_start) is uploaded into run_scan's region once, before the capture.
+    uint8_t *step_state = nullptr;
+    size_t zero_image_off = 0;         // where in the slot's pinned memory a replay's zero page lands
+    size_t read_back = 0;              // bytes of the replay's one device-to-host copy
     bydb_stats captured{};             // host-side counters of one step (launch counts, byte counts)
     bool express = false;              // the captured step launches the express lane
     uint64_t runs = 0;
@@ -1400,9 +1453,18 @@ struct bydb_prepared {
 
 namespace {
 
+// drops the captured step: the graph first, then the memory it runs in.  The slot's stream is idle (every replay synchronises).
+void drop_step(bydb_prepared *p) {
+    if (p->exec) cudaGraphExecDestroy(p->exec);
+    p->exec = nullptr;
+    if (p->step_state) cudaFree(p->step_state);
+    p->step_state = nullptr;
+    p->held.clear();
+}
+
 void prepared_destroy(bydb_prepared *p) {
     if (!p) return;
-    if (p->exec) cudaGraphExecDestroy(p->exec);
+    drop_step(p);
     for (auto &kv : p->reduce_graphs)
         if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
     if (p->t0) cudaEventDestroy(p->t0);
@@ -1430,8 +1492,10 @@ bool check_held_parts(bydb_ctx *ctx, const std::vector<bydb_part_h> &parts, cuda
 }
 
 // One replay of a captured step on the slot's stream, synchronised: the step's host-side counters as captured, device_ms from
-// the events around the launch, then the counters and the device error of its zero page (batch 0).
-int replay_graph(cudaGraphExec_t exec, ExecSlot &slot, cudaEvent_t t0, cudaEvent_t t1, const bydb_stats &captured, bool express, bydb_stats *stats) {
+// the events around the launch, then the counters and the device error of its zero page, which the graph reads back to `image`
+// (pinned; the caller zeroes it before the call, so a replay that fails to launch cannot report the previous one's status).
+int replay_graph(cudaGraphExec_t exec, ExecSlot &slot, cudaEvent_t t0, cudaEvent_t t1, const bydb_stats &captured, bool express, const ZeroPage &image,
+                 bydb_stats *stats) {
     CUDA_TRY(cudaEventRecord(t0, slot.stream));
     CUDA_TRY(cudaGraphLaunch(exec, slot.stream));
     CUDA_TRY(cudaEventRecord(t1, slot.stream));
@@ -1442,11 +1506,13 @@ int replay_graph(cudaGraphExec_t exec, ExecSlot &slot, cudaEvent_t t0, cudaEvent
     cudaEventElapsedTime(&ms, t0, t1);
     stats->device_ms = ms;
     stats->scan_kernel_ms = 0;  // per-kernel events are not available inside a graph replay
-    return read_zero_page(*slot.page(0), express, stats);
+    return read_zero_page(image, express, stats);
 }
 
-// captures one step into p->exec; returns 0, or a code after leaving the stream out of capture mode
+// captures one step into p->exec, building the StepState it runs in; returns 0, or a code after leaving the stream out of
+// capture mode.  0 with p->exec == NULL: this query keeps the uncaptured path.
 int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up: a later change is seen by the next run
     Plan plan;
     int rc = make_plan(ctx, &p->q, nullptr, plan);
     if (rc) return rc;
@@ -1457,38 +1523,52 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
     }
     ExecSlot &slot = *p->slot;
     const TableLayout &tl = plan.tl;
-    p->host_off = stage_layout(p->q.n_series, tl.G).stride;  // results land behind the staging area, which must survive from replay to replay
+    const StageLayout st = stage_layout(p->q.n_series, tl.G);
+    const ScanLayout sl = scan_layout(st, plan.total_blocks, plan.fcols.size(), plan.parts.size(), false);
+    const FinalLayout fl = final_layout(tl.G, p->q.n_aggs, p->q.top_n);
+    p->host_off = st.stride;  // the read-back lands behind the staging area
     if (slot.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    memset(&p->captured, 0, sizeof p->captured);
-    cudaError_t e = cudaStreamBeginCapture(slot.stream, cudaStreamCaptureModeThreadLocal);
-    if (e != cudaSuccess) return fail(BYDB_EIO, std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(e));
-    uint32_t fin_launches = 0;
-    {
-        Scratch table, fin;
-        rc = table.alloc(tl.total, slot.stream) == cudaSuccess ? 0 : fail(BYDB_ENOMEM, "cudaMallocAsync (capture)");
-        if (!rc) rc = run_scan(ctx, &p->q, plan, slot, slot.stream, table.base, tl, &p->captured);
-        p->express = slot.express[0];
-        if (!rc) rc = finalize_enqueue(&p->q, plan, slot, slot.stream, table.base, tl, p->host_off, fin, p->fl, fin_launches);
-        // table / fin are released here: inside the capture, i.e. as free nodes of the graph
+    Carve carve;
+    const size_t off_table = carve(tl.total), off_scan = carve(sl.total), off_fin = carve(fl.total + kZeroPageBytes);
+    if (cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
+        cudaGetLastError();
+        p->step_state = nullptr;
+        p->capturable = false;
+        return 0;
     }
+    // the staging goes up once: the graph's kernels read it from the step state on every replay
+    stage_series(&p->q, st, slot.pinned);
+    cudaError_t e = cudaMemcpyAsync(p->step_state + off_scan + sl.off_sids, slot.pinned, st.bytes, cudaMemcpyHostToDevice, slot.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(slot.stream);
+    if (e == cudaSuccess) e = cudaStreamBeginCapture(slot.stream, cudaStreamCaptureModeThreadLocal);
+    if (e != cudaSuccess) {
+        drop_step(p);
+        return fail(BYDB_EIO, std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(e));
+    }
+    memset(&p->captured, 0, sizeof p->captured);
+    uint32_t fin_launches = 0;
+    Scratch scan, fin;
+    scan.view(p->step_state + off_scan, sl.total);
+    fin.view(p->step_state + off_fin, fl.total + kZeroPageBytes);
+    rc = run_scan(ctx, &p->q, plan, slot, slot.stream, p->step_state + off_table, tl, &p->captured, 0, nullptr, &scan);
+    p->express = slot.express[0];
+    if (!rc) rc = finalize_enqueue(&p->q, plan, slot, slot.stream, p->step_state + off_table, tl, p->host_off, fin, p->fl, fin_launches, p->read_back,
+                                   scan.base + sl.off_zero);
     cudaGraph_t graph = nullptr;
     e = cudaStreamEndCapture(slot.stream, &graph);
-    if (rc || e != cudaSuccess || !graph) {
-        if (graph) cudaGraphDestroy(graph);
+    if (!rc && e == cudaSuccess && graph) e = cudaGraphInstantiate(&p->exec, graph, 0);
+    if (graph) cudaGraphDestroy(graph);
+    if (rc || e != cudaSuccess || !p->exec) {
         cudaGetLastError();
+        drop_step(p);
         p->capturable = false;  // fall back to the uncaptured path for good
-        return rc ? rc : 0;
-    }
-    e = cudaGraphInstantiate(&p->exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        p->exec = nullptr;
-        p->capturable = false;
+        return rc;
     }
     p->captured.kernel_launches += fin_launches;  // finalize + select_rows (one fused launch for few groups)
-    p->captured.d2h_bytes += p->fl.out_bytes;
+    p->captured.d2h_bytes += p->read_back;
+    p->zero_image_off = p->host_off + p->fl.out_bytes;
     p->held = plan.parts;
+    p->held_gen = gen;
     return 0;
 }
 
@@ -1604,6 +1684,7 @@ int bydb_part_register(bydb_ctx *ctx, uint64_t part_id, const bydb_part_files *f
             bydb_part_h h = ctx->next_handle++;
             ctx->parts[h] = part;
             ctx->by_id[part_id] = h;
+            ctx->parts_gen.fetch_add(1, std::memory_order_release);
             *out = h;
             return 0;
         }
@@ -1626,6 +1707,7 @@ int bydb_part_release(bydb_ctx *ctx, bydb_part_h h) {
         victim = it->second;
         ctx->by_id.erase(victim->id);
         ctx->parts.erase(it);
+        ctx->parts_gen.fetch_add(1, std::memory_order_release);
     }
     hbm_release(ctx, victim->hbm_bytes);
     cudaSetDevice(ctx->device);
@@ -2589,13 +2671,22 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
         if (rc) return rc;
         if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
     }
-    if (!check_held_parts(ctx, p->parts, p->exec, p->held)) return fail(BYDB_ENOENT, "unknown part handle");
-    if (!p->exec) {
-        const int rc = prepared_capture(ctx, p);
-        if (rc) return rc;
-        if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
+    // the handles can only have changed their parts if one was registered or released since `held` was last compared
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
+    if (gen != p->held_gen) {
+        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
+        if (!p->exec) drop_step(p);  // the state is sized for the parts it was captured with
+        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
+        p->held_gen = gen;
+        if (!p->exec) {
+            const int rc = prepared_capture(ctx, p);
+            if (rc) return rc;
+            if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
+        }
     }
-    const int rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, &out->stats);
+    uint8_t *image = p->slot->pinned + p->zero_image_off;
+    memset(image, 0, kZeroPageBytes);
+    const int rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, *reinterpret_cast<const ZeroPage *>(image), &out->stats);
     if (rc) return rc;
     return finalize_parse(p->slot->pinned + p->host_off, p->fl, false, out);
     });
@@ -3285,7 +3376,8 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
                 launch_combine_tables(mb.slots0, static_cast<uint32_t>(cm.nranks), tl, s, mb.slot_bytes);
                 step("combine", true);
                 uint32_t fin_launches = 0;
-                step("finalize", finalize_enqueue(&p->q, plan, es, s, mb.slots0, tl, p->host_off, fin, rg.fl, fin_launches) == 0);
+                size_t read_back = 0;
+                step("finalize", finalize_enqueue(&p->q, plan, es, s, mb.slots0, tl, p->host_off, fin, rg.fl, fin_launches, read_back) == 0);
                 launch_comm_done_args(mb.done, d_args, s);
                 step("done word", true);
                 step("status read-back",
@@ -3326,7 +3418,7 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
     h_args->prev_use = mb.claim_slots();
     memset(h_back, 0, kZeroPageBytes);
     memset(es.page(0), 0, kZeroPageBytes);
-    const int rc = replay_graph(rg.exec, es, p->t0, p->t1, rg.captured, rg.express, &out->stats);
+    const int rc = replay_graph(rg.exec, es, p->t0, p->t1, rg.captured, rg.express, *es.page(0), &out->stats);
     const uint32_t perr = *reinterpret_cast<const uint32_t *>(h_back);
     if (perr != 0) cudaMemset(mb.my_err, 0, sizeof perr);
     if (rc) return rc;

@@ -3327,6 +3327,7 @@ __device__ __forceinline__ uint64_t order_key_f64(double d) {
 // kFused: the finalisation runs in this (single) CTA first -- one launch less on the tail of every query with few groups
 template <bool kFused>
 __global__ void __launch_bounds__(1024) select_rows_kernel(const __grid_constant__ SelectParams p, const __grid_constant__ FinalizeParams fp) {
+    if (p.zero_src && threadIdx.x < 64) p.zero_dst[threadIdx.x] = p.zero_src[threadIdx.x];
     if (kFused) {
         if (threadIdx.x == 0) finalize_header(fp);
         for (int32_t g = threadIdx.x; g < fp.n_groups; g += blockDim.x) finalize_group(fp, g);
@@ -4201,6 +4202,19 @@ void launch_combine_keyed(const KeyedUnionParams &p, cudaStream_t s) {
     if (m) merge_first_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(p);
 }
 
+// what the two memsets at the head of a step do, as one node of a replayed graph
+__global__ void step_reset_kernel(uint32_t *zero_page, uint32_t *first_block, size_t n_first) {
+    const size_t i0 = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i0 < 64) zero_page[i0] = 0;
+    for (size_t i = i0; i < n_first; i += static_cast<size_t>(gridDim.x) * blockDim.x) first_block[i] = 0xffffffffu;
+}
+void launch_step_reset(uint32_t *zero_page, uint32_t *first_block, size_t n_first, cudaStream_t s) {
+    if (!first_block) n_first = 0;
+    const size_t want = (n_first + 255) / 256;  // the zero page alone still takes one CTA
+    const unsigned blocks = want < 1 ? 1u : want > 1024 ? 1024u : static_cast<unsigned>(want);
+    step_reset_kernel<<<blocks, 256, 0, s>>>(zero_page, first_block, n_first);
+}
+
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s) {
     if (p.total_blocks == 0) return;
     const int threads = 256;
@@ -4403,6 +4417,7 @@ void preload_kernels() {
     (void)cudaFuncGetAttributes(&ka, combine_keyed_kernel);
     (void)cudaFuncGetAttributes(&ka, merge_first_kernel);
     cudaFuncAttributes a;
+    cudaFuncGetAttributes(&a, step_reset_kernel);
     cudaFuncGetAttributes(&a, plan_blocks_kernel);
     cudaFuncGetAttributes(&a, scan_blocks_kernel<true>);
     cudaFuncGetAttributes(&a, scan_blocks_kernel<false>);

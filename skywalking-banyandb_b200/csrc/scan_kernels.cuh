@@ -205,6 +205,8 @@ struct SelectParams {
     int64_t *sel_i64;
     double *sel_f64;
     uint32_t *sel_count;
+    const uint32_t *zero_src;     // optional: the step's zero page (64 words), copied to zero_dst so that it travels in the result's
+    uint32_t *zero_dst;           // read-back; the kernel runs behind everything that writes the page.  NULL: no copy
 };
 void launch_select_rows(const SelectParams &p, cudaStream_t s);
 
@@ -382,6 +384,8 @@ void preload_encode_kernels();   // encode_kernels.cu
 size_t scan_smem_bytes();
 size_t express_smem_bytes();
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s);
+// start of a replayed step: zeroes the 64 words of the zero page and writes 0xffffffff over first_block[n_first] (may be NULL / 0)
+void launch_step_reset(uint32_t *zero_page, uint32_t *first_block, size_t n_first, cudaStream_t s);
 // grid_express: the express lane's grid (launched when p.rest_list is set), grid_fast / grid_slow: the regular lanes'
 void launch_scan_blocks(const ScanParams &p, int grid_express, int grid_fast, int grid_slow, cudaStream_t s);
 void launch_series_reduce(const ReduceParams &p, cudaStream_t s);
