@@ -208,8 +208,9 @@ int bydb_scan_agg(bydb_ctx *ctx, const bydb_query *q, bydb_result *out);
  * range), before the time trim and the predicates.  More than max_values of them give BYDB_ENOMEM (the reference's
  * aggregation memory budget).  Device side: one pass collects the distinct values, then ONE SCAN PASS PER VALUE (the key as
  * an extra predicate) fills that value's slice of a composite partial table; stats count every pass.  A group-key query
- * takes at most 7 predicates of its own.  Not available through the prepared / partial-table entry points, and not over
- * parts that overlap in time; its multi-GPU form is bydb_scan_reduce_keyed (below). */
+ * takes at most 7 predicates of its own.  Not available through the prepared entry points, and not over parts that overlap
+ * in time; its map-phase form (the rows a data node answers with) is bydb_scan_partials_keyed, its multi-GPU forms are
+ * bydb_scan_reduce_keyed and bydb_scan_reduce_keyed_partials (below). */
 typedef struct {
     const char *family;    /* tag family of the key tag                                      */
     const char *tag;       /* tag name                                                       */
@@ -342,6 +343,39 @@ typedef struct {
 int bydb_partials_rows(bydb_ctx *ctx, const bydb_query *q, const void *d_partials, uint64_t bytes, void *stream, bydb_partial_rows *out);
 void bydb_partial_rows_free(bydb_ctx *ctx, bydb_partial_rows *r);
 
+/* Map-phase rows of a group-by on a STORED tag: what a data node answers when the liaison pushes a bydb_scan_agg_keyed query
+ * down with agg_return_partial (measure_plan_distributed.go:277; the liaison then drops replicas by (shard, group-by key) and
+ * folds the rows with reduceAccumulator.Combine).
+ *   - Rows: one per composite group (series group, key value) with rows > 0, in the insertion order bydb_scan_agg_keyed gives
+ *     (measure_plan_groupby.go:127-158).  base.group_id[r] is the series group of row r, key_id[r] its key value.
+ *   - Values: per aggregate exactly what bydb_partials_rows gives for a plain group -- SUM the sum, COUNT the count, MEAN the sum
+ *     with Partial.Count (MEAN only), MAX / MIN the extreme, the N-typed sentinel for a group that met only nulls, 0 for one that
+ *     never met the column; everything typed like the field.
+ *   - Keys: as in bydb_keyed_result (a string key's bytes, nil -> ""; an int64 key's 8 little-endian bytes, nil -> 0).
+ *   - Validation, refusals, caps and device errors: those of bydb_scan_agg_keyed, with the same codes.  top_n / top_agg /
+ *     top_desc do not change the rows (as bydb_partials_rows ignores them).
+ *   - Stats: every pass counted, as bydb_scan_agg_keyed.  The composite table never crosses PCIe: with cap = max_values (0 -> 64),
+ *     V key values found, F distinct aggregated fields and A aggregations,
+ *       d2h_bytes = 256 + align256(64 * cap) + align256(4 * cap)   the discovery read-back
+ *                 + 256 * V                                       each pass's status / counter page
+ *                 + 8 + 8 * F                                     the control word (present rows, column types + status)
+ *                 + n_rows * (8 + 16 * A)                         the rows
+ *     (V = 0: the first term only).  The root of bydb_scan_reduce_keyed_partials adds the union's read-back, the same size as the
+ *     discovery's, and takes no pass term for the union. */
+typedef struct {
+    bydb_partial_rows base;    /* rows as bydb_partials_rows: base.group_id[r] = series_group of row r, Partial.Value / .Count  */
+    const int32_t *key_id;     /* [base.n_rows] index into the key table                                                     */
+    int32_t n_keys;            /* as bydb_keyed_result.n_keys                                                                */
+    int32_t reserved;
+    const uint32_t *key_off;   /* [n_keys + 1]                                                                               */
+    const uint8_t *key_bytes;
+    bydb_stats stats;          /* every pass counted, as bydb_scan_agg_keyed                                                 */
+    void *owner;               /* private                                                                                    */
+} bydb_keyed_partial_rows;
+
+int bydb_scan_partials_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out);
+void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r);
+
 /* ---- multi-GPU reduce behind the C ABI: one process (or thread) per GPU, no torch, no NCCL ----
  * Replaces the liaison gather + reduceAccumulator.Combine (pkg/query/logical/measure/measure_plan_aggregation.go:96-124,
  * measure_plan_distributed.go:254-328) inside one node: every rank owns a MAILBOX in its GPU's memory; in a collective
@@ -393,6 +427,13 @@ int bydb_scan_reduce_host(bydb_ctx *ctx, uint32_t n_parts, const bydb_part_files
  * max_values key values; pass it (or the largest over the queries to come) to bydb_comm_export as max_table_bytes. */
 int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t *out);
 int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out);
+/* The same collective with the root emitting partial rows (bydb_scan_partials_keyed's contract) instead of finalising: a node
+ * of several GPUs answers the liaison's partial request once, for all its GPUs.  Same fingerprint, slot layout, union and span
+ * check; bydb_keyed_reduce_slot_bytes sizes it.  The root gets the union's rows in the insertion order of the whole scan;
+ * non-root ranks get n_rows = 0, n_keys = 0 and their own stats.  A rank contributes the same bytes under either keyed form, so
+ * ranks may mix bydb_scan_reduce_keyed and this call in one collective: the root's call decides what it returns.  Keyed,
+ * keyed-partial and plain collectives keep the epochs in step across failures. */
+int bydb_scan_reduce_keyed_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_partial_rows *out);
 
 const char *bydb_last_error(void);
 const char *bydb_version(void);

@@ -93,6 +93,11 @@ class _PartialRows(C.Structure):
                 ("cnt_f64", C.POINTER(C.c_double)), ("owner", C.c_void_p)]
 
 
+class _KeyedPartialRows(C.Structure):
+    _fields_ = [("base", _PartialRows), ("key_id", C.POINTER(C.c_int32)), ("n_keys", C.c_int32), ("reserved", C.c_int32),
+                ("key_off", C.POINTER(C.c_uint32)), ("key_bytes", C.POINTER(C.c_uint8)), ("stats", _Stats), ("owner", C.c_void_p)]
+
+
 class _Layout(C.Structure):
     _fields_ = [("total_bytes", C.c_uint64), ("off_sum_f64", C.c_uint64), ("off_max_f64", C.c_uint64),
                 ("off_sum_i64", C.c_uint64), ("off_max_i64", C.c_uint64), ("n_sum_f64", C.c_uint64),
@@ -105,7 +110,8 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_query_release", "bydb_partials_layout",
            "bydb_scan_partials", "bydb_partials_combine", "bydb_reduce_finalize", "bydb_partials_rows", "bydb_partial_rows_free", "bydb_comm_export", "bydb_comm_connect",
            "bydb_scan_reduce", "bydb_scan_reduce_prepared", "bydb_scan_reduce_host", "bydb_scan_agg_keyed", "bydb_keyed_result_free",
-           "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed",
+           "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed", "bydb_scan_partials_keyed", "bydb_keyed_partial_rows_free",
+           "bydb_scan_reduce_keyed_partials",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -162,6 +168,10 @@ def load_library():
     L.bydb_scan_reduce_host.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(_PartFiles), C.POINTER(_Query), C.c_int32, C.POINTER(_Result)]
     L.bydb_keyed_reduce_slot_bytes.argtypes = [C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(C.c_uint64)]
     L.bydb_scan_reduce_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32, C.POINTER(_KeyedResult)]
+    L.bydb_scan_partials_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(_KeyedPartialRows)]
+    L.bydb_scan_reduce_keyed_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32, C.POINTER(_KeyedPartialRows)]
+    L.bydb_keyed_partial_rows_free.argtypes = [C.c_void_p, C.POINTER(_KeyedPartialRows)]
+    L.bydb_keyed_partial_rows_free.restype = None
     _lib = L
     return L
 
@@ -326,20 +336,35 @@ def _cq(q):
     return _mk_query(q, keep), keep
 
 
+def _arr(ptr, count, dtype):
+    """`count` elements at a library pointer as a writable array"""
+    if count == 0:
+        return np.zeros(0, dtype=dtype)
+    # one memcpy out of the library's buffer, then a writable array of it: 13 us for a result of 100 rows x 2 aggregates, where
+    # slicing the pointer into a Python list took 42 us and np.ctypeslib.as_array 16 us (timeit, host only)
+    return np.frombuffer(C.string_at(ptr, count * np.dtype(dtype).itemsize), dtype=dtype).copy()
+
+
 def _read_result(r: _Result) -> Result:
     n, a = r.n_rows, r.n_aggs
-
-    def arr(ptr, count, dtype):
-        if count == 0:
-            return np.zeros(0, dtype=dtype)
-        # one memcpy out of the library's buffer, then a writable array of it: 13 us for a result of 100 rows x 2 aggregates, where
-        # slicing the pointer into a Python list took 42 us and np.ctypeslib.as_array 16 us (timeit, host only)
-        return np.frombuffer(C.string_at(ptr, count * np.dtype(dtype).itemsize), dtype=dtype).copy()
-
+    arr = _arr
     return Result(group_id=arr(r.group_id, n, np.int32), rows=arr(r.rows, n, np.int64),
                   is_float=arr(r.is_float, a, np.uint8).astype(bool),
                   val_i64=arr(r.val_i64, n * a, np.int64).reshape(n, a),
                   val_f64=arr(r.val_f64, n * a, np.float64).reshape(n, a), stats=Stats.of(r.stats))
+
+
+def _read_partial_rows(r: _PartialRows, n_aggs: Optional[int] = None) -> Dict[str, np.ndarray]:
+    """the arrays of a bydb_partial_rows; n_aggs: the width of an answer without rows (its arrays may be unset)"""
+    n, a = r.n_rows, (r.n_aggs if r.owner or n_aggs is None else n_aggs)
+    if not r.owner:
+        z = lambda dt: np.zeros((0, a), dtype=dt)  # noqa: E731
+        return dict(group_id=np.zeros(0, np.int32), is_float=np.zeros(a, bool), val_i64=z(np.int64), val_f64=z(np.float64),
+                    cnt_i64=z(np.int64), cnt_f64=z(np.float64))
+    f = _arr
+    return dict(group_id=f(r.group_id, n, np.int32), is_float=f(r.is_float, a, np.uint8).astype(bool),
+                val_i64=f(r.val_i64, n * a, np.int64).reshape(n, a), val_f64=f(r.val_f64, n * a, np.float64).reshape(n, a),
+                cnt_i64=f(r.cnt_i64, n * a, np.int64).reshape(n, a), cnt_f64=f(r.cnt_f64, n * a, np.float64).reshape(n, a))
 
 
 class GraphQuery:
@@ -538,13 +563,43 @@ class Context:
         r = _PartialRows()
         _check(self._L.bydb_partials_rows(self._h, C.byref(cq), d_ptr, nbytes, stream or None, C.byref(r)))
         try:
-            n, a = r.n_rows, r.n_aggs
-            f = lambda ptr, cnt, dt: np.array(ptr[:cnt], dtype=dt)  # noqa: E731
-            return dict(group_id=f(r.group_id, n, np.int32), is_float=f(r.is_float, a, np.uint8).astype(bool),
-                        val_i64=f(r.val_i64, n * a, np.int64).reshape(n, a), val_f64=f(r.val_f64, n * a, np.float64).reshape(n, a),
-                        cnt_i64=f(r.cnt_i64, n * a, np.int64).reshape(n, a), cnt_f64=f(r.cnt_f64, n * a, np.float64).reshape(n, a))
+            return _read_partial_rows(r)
         finally:
             self._L.bydb_partial_rows_free(self._h, C.byref(r))
+
+    def scan_partials_keyed(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> Dict[str, object]:
+        """Map-phase rows of a group-by on a stored tag (bydb_scan_partials_keyed): the arrays of partials_rows, one row per
+        present (series group, key value) in insertion order, plus `key` (the key bytes of each row), `n_keys`, `key_table` (the
+        n_keys distinct values in the library's order) and `stats`."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        r = _KeyedPartialRows()
+        _check(self._L.bydb_scan_partials_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
+        return self._read_keyed_partials(q, r)
+
+    def scan_reduce_keyed_partials(self, q: Query, family: str, tag: str, root: int = 0, max_values: int = 0,
+                                   value_type: int = 0) -> Dict[str, object]:
+        """The keyed collective with the root emitting partial rows (bydb_scan_reduce_keyed_partials): the root gets
+        scan_partials_keyed's rows over all ranks' parts; the others no rows, no keys and their own scan statistics."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        r = _KeyedPartialRows()
+        _check(self._L.bydb_scan_reduce_keyed_partials(self._h, C.byref(cq), C.byref(gk), root, C.byref(r)))
+        return self._read_keyed_partials(q, r)
+
+    def _read_keyed_partials(self, q: Query, r: "_KeyedPartialRows") -> Dict[str, object]:
+        try:
+            out = _read_partial_rows(r.base, len(q.aggs))
+            keys = [bytes(r.key_bytes[r.key_off[k]:r.key_off[k + 1]]) for k in range(r.n_keys)]
+            out["key"] = [keys[k] for k in _arr(r.key_id, r.base.n_rows, np.int32).tolist()]
+            out["n_keys"] = r.n_keys
+            out["key_table"] = keys
+            out["stats"] = Stats.of(r.stats)
+            return out
+        finally:
+            self._L.bydb_keyed_partial_rows_free(self._h, C.byref(r))
 
     # ---- multi-GPU reduce behind the C ABI (peer mailboxes over NVLink; no torch / NCCL on the data path)
     def comm_export(self, max_table_bytes: int, max_ranks: int) -> bytes:

@@ -1787,12 +1787,36 @@ int bydb_scan_agg(bydb_ctx *ctx, const bydb_query *q, bydb_result *out) {
 // rewritten into the arena.  The image goes up through the pinned staging ring in 64 MB chunks.
 // ------------------------------------------------------------------------------------------------
 
+extern "C++" {  // the keyed helpers below are templates over the two answer forms
 namespace {
 struct KeyedOwner {
     std::vector<int32_t> key_id;
     std::vector<uint32_t> key_off;
     std::vector<uint8_t> key_bytes;
 };
+
+// the arrays of a bydb_partial_rows
+struct PartialRowsOwner {
+    std::vector<int32_t> group_id;
+    std::vector<uint8_t> is_float;
+    std::vector<int64_t> val_i64, cnt_i64;
+    std::vector<double> val_f64, cnt_f64;
+};
+
+// one aggregate of a row: the Partial words into the arrays of their type, 0 in the others
+void push_partial(PartialRowsOwner &o, const PartialWords &w, bool is_float) {
+    double vf = 0.0, cf = 0.0;
+    memcpy(&vf, &w.val, 8);
+    memcpy(&cf, &w.cnt, 8);
+    o.val_i64.push_back(is_float ? 0 : static_cast<int64_t>(w.val));
+    o.val_f64.push_back(is_float ? vf : 0.0);
+    o.cnt_i64.push_back(is_float ? 0 : static_cast<int64_t>(w.cnt));
+    o.cnt_f64.push_back(is_float ? cf : 0.0);
+}
+
+// the two answers of a keyed call: finalised rows (bydb_keyed_result) or map-phase partial rows (bydb_keyed_partial_rows)
+bydb_stats &keyed_stats(bydb_keyed_result *out) { return out->base.stats; }
+bydb_stats &keyed_stats(bydb_keyed_partial_rows *out) { return out->stats; }
 using KeyValues = std::vector<std::vector<uint8_t>>;
 
 // the checks of a group key that need no device; cap = the distinct values accepted (max_values, 0 = 64)
@@ -1913,8 +1937,9 @@ int run_keyed_passes(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *k
     return 0;
 }
 
-// the key table of a keyed result: value k is `values[k]`
-void set_key_table(bydb_keyed_result *out, KeyedOwner *owner, const KeyValues &values) {
+// the key table of a keyed answer: value k is `values[k]`
+template <class Out>
+void set_key_table(Out *out, KeyedOwner *owner, const KeyValues &values) {
     owner->key_off.assign(1, 0);
     owner->key_bytes.clear();
     for (const auto &v : values) {
@@ -1927,21 +1952,18 @@ void set_key_table(bydb_keyed_result *out, KeyedOwner *owner, const KeyValues &v
     out->key_bytes = owner->key_bytes.data();
 }
 
-// 3. insertion order of the V x G composite groups from where each series first shows each value (kts / krow), the table at
-// `table` reordered, the ordinary finalisation / Top-N on it, and the rows mapped back to (series group, key value).  The
-// caller sized the slot's pinned staging with step_pinned_bytes(q, G, V * G).
-int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
-                 const int64_t *kts, const uint32_t *krow, bydb_keyed_result *out, KeyedOwner *owner) {
+// 3. insertion order of the V x G composite groups from where each series first shows each value (kts / krow): ko.perm lists
+// the composite groups v * G + g in insertion order, the *ko.n_present that appeared first, in scratch `kb` (enqueued, not
+// synchronised; the staging of the series groups in slot.pinned is in flight).
+int keyed_order(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, const int64_t *kts, const uint32_t *krow, Scratch &kb,
+                KeyOrderParams &ko, bydb_stats &stats) {
     cudaStream_t stream = slot.stream;
-    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    const size_t NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
     const StageLayout st = stage_layout(NS, G);
     Carve carve;
-    const size_t b_dst = carve(tlc.total), b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16),
-                 b_stage = carve(st.bytes);
-    Scratch kb;
+    const size_t b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16), b_stage = carve(st.bytes);
     CUDA_TRY(kb.alloc(carve.o, stream));
     CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
-    KeyOrderParams ko;
     memset(&ko, 0, sizeof ko);
     ko.n_groups = static_cast<int32_t>(G);
     ko.n_values = static_cast<uint32_t>(V);
@@ -1958,19 +1980,35 @@ int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V
     ko.perm = reinterpret_cast<int32_t *>(kb.base + b_perm);
     ko.n_present = reinterpret_cast<uint32_t *>(kb.base + b_np);
     launch_key_order(ko, stream);
-    launch_permute_table(tlc.at(kb.base + b_dst), tlc.at(table), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), coltype,
+    stats.kernel_launches += 2;
+    return 0;
+}
+
+// 4a. bydb_scan_agg_keyed / bydb_scan_reduce_keyed: after the order, the table at `table` reordered, the ordinary finalisation /
+// Top-N on it, and the rows mapped back to (series group, key value).  The caller sized the slot's pinned staging with
+// keyed_pinned_bytes.
+int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
+                 const int64_t *kts, const uint32_t *krow, bydb_keyed_result *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    Scratch kb, dst;
+    KeyOrderParams ko;
+    int rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, out->base.stats);
+    if (rc) return rc;
+    CUDA_TRY(dst.alloc(tlc.total, stream));
+    launch_permute_table(tlc.at(dst.base), tlc.at(table), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), coltype,
                          static_cast<uint32_t>(V), stream);
     CUDA_TRY(cudaStreamSynchronize(stream));  // the staging above is reused by the finalisation's read-back
-    out->base.stats.kernel_launches += 3;
+    out->base.stats.kernel_launches += 1;
     Plan planc = plan;
     planc.n_groups = static_cast<int32_t>(GP);
-    int rc = finalize_to_host(q, planc, slot, stream, kb.base + b_dst, tlc, &out->base, true);
+    rc = finalize_to_host(q, planc, slot, stream, dst.base, tlc, &out->base, true);
     if (rc) {
         cudaStreamSynchronize(stream);
         return rc;
     }
     std::vector<int32_t> perm(GP);
-    CUDA_TRY(cudaMemcpyAsync(perm.data(), kb.base + b_perm, GP * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(perm.data(), ko.perm, GP * 4, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     out->base.stats.d2h_bytes += GP * 4;
     // rows carry the position in insertion order: back to (group of the series, key value)
@@ -1985,22 +2023,121 @@ int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V
     return 0;
 }
 
+// 4b. bydb_scan_partials_keyed / bydb_scan_reduce_keyed_partials: after the order, keyed_partial_rows_kernel writes the wire rows
+// of the present composite groups from the unpermuted table into one packed image; the read-back takes the control word, then
+// exactly n_present rows.  The composite table never leaves the device.
+int keyed_rows(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
+               const int64_t *kts, const uint32_t *krow, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), G = static_cast<size_t>(plan.n_groups), GP = G * V, A = q->n_aggs;
+    const size_t ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
+    Scratch kb, img;
+    KeyOrderParams ko;
+    int rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, out->stats);
+    if (rc) return rc;
+    Carve carve;
+    const size_t i_ctl = carve(ctl_bytes), i_rows = carve(GP * row_bytes);
+    CUDA_TRY(img.alloc(carve.o, stream));
+    KeyedRowsParams kp;
+    memset(&kp, 0, sizeof kp);
+    kp.table = tlc.at(table);
+    kp.perm = ko.perm;
+    kp.n_present = ko.n_present;
+    kp.pass_coltype = coltype;
+    kp.n_groups = static_cast<uint32_t>(G);
+    kp.n_fcols = static_cast<uint32_t>(F);
+    kp.n_aggs = static_cast<uint32_t>(A);
+    kp.n_passes = static_cast<uint32_t>(V);
+    for (size_t a = 0; a < A; ++a) {
+        kp.agg_fcol[a] = plan.agg_fcol[a];
+        kp.agg_func[a] = q->aggs[a].func;
+    }
+    kp.ctl = reinterpret_cast<uint32_t *>(img.base + i_ctl);
+    kp.rows = img.base + i_rows;
+    launch_keyed_partial_rows(kp, GP, stream);
+    out->stats.kernel_launches += 1;
+    // 1. the control word (behind the staging copy that reads slot.pinned, on the same stream)
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base + i_ctl, ctl_bytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    out->stats.d2h_bytes += ctl_bytes;
+    const int64_t *ct = reinterpret_cast<const int64_t *>(slot.pinned + 8);
+    uint32_t dev_err = 0;
+    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(ct[c] >> 8));
+    rc = table_status(dev_err);
+    if (rc) return rc;
+    auto ro = std::make_unique<PartialRowsOwner>();
+    ro->is_float.resize(A);
+    for (size_t a = 0; a < A; ++a) ro->is_float[a] = (ct[plan.agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
+    const size_t n = std::min<size_t>(*reinterpret_cast<const uint32_t *>(slot.pinned), GP);
+    // 2. the rows
+    if (n) {
+        CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base + i_rows, n * row_bytes, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        out->stats.d2h_bytes += n * row_bytes;
+    }
+    ro->group_id.resize(n);
+    owner->key_id.resize(n);
+    for (size_t j = 0; j < n; ++j) {
+        const uint8_t *row = slot.pinned + j * row_bytes;
+        memcpy(&ro->group_id[j], row, 4);
+        memcpy(&owner->key_id[j], row + 4, 4);
+        for (size_t a = 0; a < A; ++a) {
+            PartialWords w;
+            memcpy(&w.val, row + 8 + 8 * a, 8);
+            memcpy(&w.cnt, row + 8 + 8 * (A + a), 8);
+            push_partial(*ro, w, ro->is_float[a] != 0);
+        }
+    }
+    bydb_partial_rows &b = out->base;
+    b.n_rows = static_cast<int32_t>(n);
+    b.n_aggs = static_cast<int32_t>(A);
+    b.group_id = ro->group_id.data();
+    b.is_float = ro->is_float.data();
+    b.val_i64 = ro->val_i64.data();
+    b.val_f64 = ro->val_f64.data();
+    b.cnt_i64 = ro->cnt_i64.data();
+    b.cnt_f64 = ro->cnt_f64.data();
+    b.owner = ro.release();
+    out->key_id = owner->key_id.data();
+    return 0;
+}
+
+// the pinned staging of the ordering and the read-back of a keyed answer over GP composite groups
+size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_result *) {
+    return step_pinned_bytes(q, static_cast<size_t>(plan.n_groups), GP);
+}
+size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_partial_rows *) {
+    return std::max(stage_layout(q->n_series, static_cast<size_t>(plan.n_groups)).stride,
+                    std::max(keyed_ctl_bytes(plan.fcols.size()), GP * keyed_row_bytes(q->n_aggs)));
+}
+
+int keyed_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
+               const int64_t *kts, const uint32_t *krow, bydb_keyed_result *out, KeyedOwner *owner) {
+    return keyed_finish(q, plan, slot, V, table, tlc, coltype, kts, krow, out, owner);
+}
+int keyed_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
+               const int64_t *kts, const uint32_t *krow, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    return keyed_rows(q, plan, slot, V, table, tlc, coltype, kts, krow, out, owner);
+}
+
+void keyed_free(bydb_ctx *ctx, bydb_keyed_result *out) { bydb_keyed_result_free(ctx, out); }
+void keyed_free(bydb_ctx *ctx, bydb_keyed_partial_rows *out) { bydb_keyed_partial_rows_free(ctx, out); }
+
 // a failure past the point where the result owns memory must not leave a half-filled result with the caller
+template <class Out>
 struct KeyedUndo {
     bydb_ctx *ctx;
-    bydb_keyed_result *out;
+    Out *out;
     bool done = false;
     ~KeyedUndo() {
-        if (!done) bydb_keyed_result_free(ctx, out);
+        if (!done) keyed_free(ctx, out);
     }
 };
-}  // namespace
 
-void bydb_encoded_pages_free(bydb_ctx *ctx, bydb_encoded_pages *r);
-
-// Group-by on a stored tag (per-row key): see "Group key" in scan_kernels.cu for the device side.
-int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out) {
-    return guarded([&]() -> int {
+// bydb_scan_agg_keyed and bydb_scan_partials_keyed: discovery, the per-value passes, the order, then the form's own answer
+template <class Out>
+int scan_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
     if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
     memset(out, 0, sizeof *out);
     int rc = validate_query(q, true);
@@ -2020,15 +2157,16 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     ExecSlot &slot = *lease.slot;
     cudaStream_t stream = slot.stream;
     const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
-    memset(&out->base.stats, 0, sizeof out->base.stats);
+    bydb_stats &stats = keyed_stats(out);
+    memset(&stats, 0, sizeof stats);
 
     KeyValues values;
-    rc = discover_keys(ctx, q, key, cap, plan, slot, &out->base.stats, values);
+    rc = discover_keys(ctx, q, key, cap, plan, slot, &stats, values);
     if (rc) return rc;
     const size_t V = values.size();
     auto owner = new KeyedOwner();
     out->owner = owner;
-    KeyedUndo undo{ctx, out};
+    KeyedUndo<Out> undo{ctx, out};
     set_key_table(out, owner, values);
     if (V == 0) {  // no block selected: no rows (n_rows = 0)
         undo.done = true;
@@ -2043,15 +2181,35 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
     Scratch kb;
     CUDA_TRY(kb.alloc(carve.o, stream));
     CUDA_TRY(cudaMemsetAsync(kb.base + b_ct, 0, V * F * 8, stream));
-    if (slot.ensure_pinned(step_pinned_bytes(q, G, GP))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    if (slot.ensure_pinned(keyed_pinned_bytes(q, plan, GP, out))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     int64_t *ct = reinterpret_cast<int64_t *>(kb.base + b_ct), *kts = reinterpret_cast<int64_t *>(kb.base + b_kts);
     uint32_t *krow = reinterpret_cast<uint32_t *>(kb.base + b_krow);
-    rc = run_keyed_passes(ctx, q, key, plan, slot, values, tlc, kb.base + b_src, ct, kts, krow, nullptr, &out->base.stats);
-    if (!rc) rc = keyed_finish(q, plan, slot, V, kb.base + b_src, tlc, ct, kts, krow, out, owner);
+    rc = run_keyed_passes(ctx, q, key, plan, slot, values, tlc, kb.base + b_src, ct, kts, krow, nullptr, &stats);
+    if (!rc) rc = keyed_emit(q, plan, slot, V, kb.base + b_src, tlc, ct, kts, krow, out, owner);
     if (rc) return rc;
     undo.done = true;
     return 0;
-    });
+}
+}  // namespace
+}  // extern "C++"
+
+void bydb_encoded_pages_free(bydb_ctx *ctx, bydb_encoded_pages *r);
+
+// Group-by on a stored tag (per-row key): see "Group key" in scan_kernels.cu for the device side.
+int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out) {
+    return guarded([&]() -> int { return scan_keyed_impl(ctx, q, key, out); });
+}
+
+// The map-phase form of the same query: wire rows of the present composite groups (keyed_partial_rows_kernel).
+int bydb_scan_partials_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out) {
+    return guarded([&]() -> int { return scan_keyed_impl(ctx, q, key, out); });
+}
+
+void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r) {
+    if (!r) return;
+    bydb_partial_rows_free(ctx, &r->base);
+    delete static_cast<KeyedOwner *>(r->owner);
+    memset(r, 0, sizeof *r);
 }
 
 void bydb_keyed_result_free(bydb_ctx *ctx, bydb_keyed_result *r) {
@@ -2693,13 +2851,6 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
 }
 
 
-struct PartialRowsOwner {
-    std::vector<int32_t> group_id;
-    std::vector<uint8_t> is_float;
-    std::vector<int64_t> val_i64, cnt_i64;
-    std::vector<double> val_f64, cnt_f64;
-};
-
 int bydb_partials_rows(bydb_ctx *ctx, const bydb_query *q, const void *d_partials, uint64_t bytes, void *stream, bydb_partial_rows *out) {
     return guarded([&]() -> int {
     if (!ctx || !d_partials || !out) return fail(BYDB_EINVAL, "NULL argument");
@@ -2729,31 +2880,9 @@ int bydb_partials_rows(bydb_ctx *ctx, const bydb_query *q, const void *d_partial
     for (size_t g = 0; g < G; ++g) {
         if (t.rows[g] <= 0) continue;  // the group never appeared on this node
         owner->group_id.push_back(static_cast<int32_t>(g));
-        for (size_t a = 0; a < A; ++a) {
-            const size_t o = g * F + static_cast<size_t>(agg_fcol[a]);
-            const bool isf = owner->is_float[a] != 0;
-            const int64_t n = t.cnt[o];
-            const bool met = met_column(isf, n, t.max_i64[o], t.max_f64[o]);  // else MIN / MAX keep the zero value
-            int64_t vi = 0, ci = 0;
-            double vf = 0.0, cf = 0.0;
-            switch (q->aggs[a].func) {
-                case BYDB_AGG_SUM: vi = t.sum_i64[o]; vf = t.sum_f64[o]; break;
-                case BYDB_AGG_COUNT: vi = n; vf = static_cast<double>(n); break;
-                case BYDB_AGG_MAX:
-                    vi = n > 0 ? t.max_i64[o] : met ? INT64_MIN : 0;
-                    vf = n > 0 ? t.max_f64[o] : met ? -1.7976931348623157e308 : 0.0;
-                    break;
-                case BYDB_AGG_MIN:
-                    vi = n > 0 ? ~t.notmin_i64[o] : met ? INT64_MAX : 0;
-                    vf = n > 0 ? -t.negmin_f64[o] : met ? 1.7976931348623157e308 : 0.0;
-                    break;
-                case BYDB_AGG_MEAN: vi = t.sum_i64[o]; vf = t.sum_f64[o]; ci = n; cf = static_cast<double>(n); break;
-            }
-            owner->val_i64.push_back(isf ? 0 : vi);
-            owner->val_f64.push_back(isf ? vf : 0.0);
-            owner->cnt_i64.push_back(isf ? 0 : ci);
-            owner->cnt_f64.push_back(isf ? cf : 0.0);
-        }
+        for (size_t a = 0; a < A; ++a)
+            push_partial(*owner, partial_words(t, g * F + static_cast<size_t>(agg_fcol[a]), q->aggs[a].func, owner->is_float[a] != 0),
+                         owner->is_float[a] != 0);
     }
     out->n_rows = static_cast<int32_t>(owner->group_id.size());
     out->n_aggs = static_cast<int32_t>(A);
@@ -3153,17 +3282,19 @@ int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key,
 // The keyed collective: discovery and the per-value passes of bydb_scan_agg_keyed on every rank, written into its slot of the
 // root's mailbox (layout KeyedSlot); on the root the union of the values, the cross-rank span check, the union table and first
 // appearances (key_union / rank_span_check / combine_keyed / merge_first kernels), then bydb_scan_agg_keyed's ordering and
-// finalisation.
-int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out) {
-    return guarded([&]() -> int {
+// finalisation -- or, for bydb_scan_reduce_keyed_partials, its partial rows.  The root's call decides the form of its answer;
+// every rank contributes the same slot either way, so ranks may mix the two calls in one collective.
+extern "C++" {
+template <class Out>
+static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, Out *out) {
     if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
     memset(out, 0, sizeof *out);
     g_last_dev_err = 0;
     auto owner = new KeyedOwner();
     out->owner = owner;
-    KeyedUndo undo{ctx, out};
+    KeyedUndo<Out> undo{ctx, out};
     set_key_table(out, owner, {});
-    bydb_stats &stats = out->base.stats;
+    bydb_stats &stats = keyed_stats(out);
     Plan plan;
     uint32_t cap = 0;
     KeyValues values;
@@ -3187,7 +3318,7 @@ int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_
             return fail(BYDB_EINVAL, "keyed collective: this rank's " + std::to_string(V) + " key values need " + std::to_string(ks.total) +
                                          " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keyed_reduce_slot_bytes)");
         // sized for the union (at most cap values) now: the root's finalisation may not allocate page-locked memory later
-        if (es.ensure_pinned(step_pinned_bytes(q, G, G * cap))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+        if (es.ensure_pinned(keyed_pinned_bytes(q, plan, G * cap, out))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
         fp = keyed_fingerprint(q, key, cap);
         header.assign(ks.off_vals + V * kMaxLit, 0);
         const uint32_t v32 = static_cast<uint32_t>(V);
@@ -3285,14 +3416,24 @@ int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_
         up.Krow = reinterpret_cast<uint32_t *>(uc.base + c_krow);
         launch_combine_keyed(up, s);
         stats.kernel_launches += NS ? 2 : 1;
-        return keyed_finish(q, plan, es, V, uc.base + c_table, tlu, up.coltype, up.Kts, up.Krow, out, owner);
+        return keyed_emit(q, plan, es, V, uc.base + c_table, tlu, up.coltype, up.Kts, up.Krow, out, owner);
     };
     h.discard = [] {};  // the result of a failed call is freed by `undo`
     const int rc = run_collective(ctx, root, 0, h);
     if (rc) return rc;
     undo.done = true;
     return 0;
-    });
+}
+
+}  // extern "C++"
+
+int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out) {
+    return guarded([&]() -> int { return scan_reduce_keyed_impl(ctx, q, key, root, out); });
+}
+
+// The keyed collective with the root emitting partial rows instead of finalising.
+int bydb_scan_reduce_keyed_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_partial_rows *out) {
+    return guarded([&]() -> int { return scan_reduce_keyed_impl(ctx, q, key, root, out); });
 }
 
 int bydb_scan_reduce(bydb_ctx *ctx, const bydb_query *q, int32_t root, bydb_result *out) {

@@ -4027,6 +4027,47 @@ void launch_permute_table(const TablePtrs &dst, const TablePtrs &src, const int3
     permute_table_kernel<<<(n + 255) / 256, 256, 0, s>>>(dst, src, perm, n_groups, n_fcols, pass_coltype, n_passes);
 }
 
+// Map-phase rows of a keyed query (bydb_scan_partials_keyed): one thread per (row j, aggregate a) reads composite group perm[j]
+// straight from the unpermuted table and writes its Partial words; no permuted copy, no finalisation.  The grid covers every
+// composite group, so the host needs no round trip to size it; threads of rows at or above *n_present leave at once.  The first
+// F threads merge the passes' column types into the control word, as permute_table_kernel does, so the status and a type mix come
+// back with n_present.
+__global__ void __launch_bounds__(256) keyed_partial_rows_kernel(const __grid_constant__ KeyedRowsParams p) {
+    const size_t t = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const uint32_t n_present = *p.n_present;
+    if (t < p.n_fcols) {
+        int64_t typ = 0, err = 0;
+        for (uint32_t v = 0; v < p.n_passes; ++v) merge_coltype(p.pass_coltype[static_cast<size_t>(v) * p.n_fcols + t], typ, err);
+        reinterpret_cast<int64_t *>(p.ctl + 2)[t] = typ | (err << 8);
+    }
+    if (t == 0) {
+        p.ctl[0] = n_present;
+        p.ctl[1] = 0;
+    }
+    const size_t j = t / p.n_aggs;
+    const uint32_t a = static_cast<uint32_t>(t % p.n_aggs);
+    if (j >= n_present) return;
+    const uint32_t comp = static_cast<uint32_t>(p.perm[j]);
+    const uint32_t c = static_cast<uint32_t>(p.agg_fcol[a]);
+    // the field's type: the first pass that saw the column (passes that disagree fail the call through the control word)
+    int64_t typ = 0;
+    for (uint32_t v = 0; v < p.n_passes && typ == 0; ++v) typ = p.pass_coltype[static_cast<size_t>(v) * p.n_fcols + c] & 0xff;
+    const PartialWords w = partial_words(p.table, static_cast<size_t>(comp) * p.n_fcols + c, p.agg_func[a], typ == BYDB_VT_FLOAT64);
+    uint8_t *row = p.rows + j * keyed_row_bytes(p.n_aggs);
+    if (a == 0) {
+        reinterpret_cast<int32_t *>(row)[0] = static_cast<int32_t>(comp % p.n_groups);
+        reinterpret_cast<int32_t *>(row)[1] = static_cast<int32_t>(comp / p.n_groups);
+    }
+    reinterpret_cast<uint64_t *>(row + 8)[a] = w.val;
+    reinterpret_cast<uint64_t *>(row + 8)[p.n_aggs + a] = w.cnt;
+}
+
+void launch_keyed_partial_rows(const KeyedRowsParams &p, size_t max_rows, cudaStream_t s) {
+    const size_t rows = max_rows * p.n_aggs;
+    const size_t n = rows > p.n_fcols ? rows : (p.n_fcols > 0 ? p.n_fcols : 1);
+    keyed_partial_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(p);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Keyed collective (bydb_scan_reduce_keyed): every rank ran discovery and its per-value passes into its slot of the root's
 // mailbox (layout: KeyedSlot).  The ranks' value lists differ, so their V_r x G composite tables do not line up slot for slot.
@@ -4412,6 +4453,7 @@ void preload_kernels() {
     (void)cudaFuncGetAttributes(&ka, key_order_kernel);
     (void)cudaFuncGetAttributes(&ka, key_perm_kernel);
     (void)cudaFuncGetAttributes(&ka, permute_table_kernel);
+    (void)cudaFuncGetAttributes(&ka, keyed_partial_rows_kernel);
     (void)cudaFuncGetAttributes(&ka, key_union_kernel);
     (void)cudaFuncGetAttributes(&ka, rank_span_check_kernel);
     (void)cudaFuncGetAttributes(&ka, combine_keyed_kernel);

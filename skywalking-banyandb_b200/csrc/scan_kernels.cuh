@@ -6,6 +6,7 @@
 
 #include <cstdint>
 
+#include "../../include/bydb_gpu.h"
 #include "part_dir.hpp"
 
 namespace bydb {
@@ -277,6 +278,63 @@ struct TableLayout {
                          reinterpret_cast<int64_t *>(base + off_coltype)};
     }
 };
+
+// The Partial a data node ships for aggregate `func` of one group of a partial table, word o = group * F + field (emitPartial,
+// measure_plan_aggregation.go:67-84; aggregation.PartialToFieldValues): SUM the sum, COUNT the count, MEAN the sum with the count as
+// Partial.Count, MAX / MIN the extreme -- the N-typed sentinel for a group that met only nulls, the zero value for one that never
+// met the column (met_column).  Both words are typed like the field: the bits of a double when is_float.  The one definition of
+// the wire rule: bydb_partials_rows (host) and keyed_partial_rows_kernel (device) both call it.
+struct PartialWords {
+    uint64_t val, cnt;
+};
+__host__ __device__ __forceinline__ uint64_t f64_bits(double x) {
+#ifdef __CUDA_ARCH__
+    return static_cast<uint64_t>(__double_as_longlong(x));
+#else
+    uint64_t u;
+    __builtin_memcpy(&u, &x, 8);
+    return u;
+#endif
+}
+__host__ __device__ __forceinline__ PartialWords partial_words(const TablePtrs &t, size_t o, int func, bool is_float) {
+    const int64_t n = t.cnt[o];
+    const bool met = met_column(is_float, n, t.max_i64[o], t.max_f64[o]);  // else MIN / MAX keep the zero value
+    int64_t vi = 0, ci = 0;
+    double vf = 0.0, cf = 0.0;
+    switch (func) {
+        case BYDB_AGG_SUM: vi = t.sum_i64[o]; vf = t.sum_f64[o]; break;
+        case BYDB_AGG_COUNT: vi = n; vf = static_cast<double>(n); break;
+        case BYDB_AGG_MAX:
+            vi = n > 0 ? t.max_i64[o] : met ? INT64_MIN : 0;
+            vf = n > 0 ? t.max_f64[o] : met ? -1.7976931348623157e308 : 0.0;
+            break;
+        case BYDB_AGG_MIN:
+            vi = n > 0 ? ~t.notmin_i64[o] : met ? INT64_MAX : 0;
+            vf = n > 0 ? -t.negmin_f64[o] : met ? 1.7976931348623157e308 : 0.0;
+            break;
+        case BYDB_AGG_MEAN: vi = t.sum_i64[o]; vf = t.sum_f64[o]; ci = n; cf = static_cast<double>(n); break;
+    }
+    return is_float ? PartialWords{f64_bits(vf), f64_bits(cf)} : PartialWords{static_cast<uint64_t>(vi), static_cast<uint64_t>(ci)};
+}
+
+// ---- map-phase rows of a keyed query (bydb_scan_partials_keyed): row j < *n_present is composite group perm[j] = v * G + g of the
+// UNPERMUTED V x G table, written as [group_id i32 | key_id i32 | val[A] | cnt[A]] (keyed_row_bytes(A) bytes, partial_words).
+// The control word in front of the rows: u32 n_present | u32 0 | i64 coltype[F] (the passes' column types merged + status).
+__host__ __device__ __forceinline__ size_t keyed_row_bytes(size_t A) { return 8 + 16 * A; }
+__host__ __device__ __forceinline__ size_t keyed_ctl_bytes(size_t F) { return 8 + 8 * F; }
+struct KeyedRowsParams {
+    TablePtrs table;              // composite table TableLayout(V * G, F), as the passes (or the union of the ranks) left it
+    const int32_t *perm;          // key_perm_kernel's insertion order
+    const uint32_t *n_present;
+    const int64_t *pass_coltype;  // [n_passes * n_fcols]
+    uint32_t n_groups, n_fcols, n_aggs, n_passes;
+    int32_t agg_fcol[32];
+    int32_t agg_func[32];
+    uint32_t *ctl;                // control word (keyed_ctl_bytes)
+    uint8_t *rows;                // [max_rows * keyed_row_bytes(n_aggs)]
+};
+// grid over max_rows (= V * G) rows; the threads of rows at or above *n_present leave at once
+void launch_keyed_partial_rows(const KeyedRowsParams &p, size_t max_rows, cudaStream_t s);
 // ---- keyed collective (bydb_scan_reduce_keyed): the slot of a rank that found V key values, in the root's mailbox, for G groups,
 // F fields and NS series.  Every region is sized by V, so a rank's need grows with the values it found; the root derives each
 // rank's layout from the V_r in its header.
