@@ -208,7 +208,7 @@ int bydb_scan_agg(bydb_ctx *ctx, const bydb_query *q, bydb_result *out);
  * range), before the time trim and the predicates.  More than max_values of them give BYDB_ENOMEM (the reference's
  * aggregation memory budget).  Device side: one pass collects the distinct values, then ONE SCAN PASS PER VALUE (the key as
  * an extra predicate) fills that value's slice of a composite partial table; stats count every pass.  A group-key query
- * takes at most 7 predicates of its own.  Not available through the prepared entry points, and not over parts that overlap
+ * takes at most 7 predicates of its own.  Its prepared form is bydb_query_prepare_keyed (below); not over parts that overlap
  * in time; its map-phase form (the rows a data node answers with) is bydb_scan_partials_keyed, its multi-GPU forms are
  * bydb_scan_reduce_keyed and bydb_scan_reduce_keyed_partials (below). */
 typedef struct {
@@ -289,6 +289,41 @@ typedef struct bydb_prepared bydb_prepared;
 int bydb_query_prepare(bydb_ctx *ctx, const bydb_query *q, bydb_prepared **out);
 int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *pq, bydb_result *out);
 void bydb_query_release(bydb_ctx *ctx, bydb_prepared *pq);
+
+/* Prepared group-by on a stored tag: bydb_scan_agg_keyed for a query executed many times (a dashboard panel grouped by a stored
+ * tag).  bydb_query_prepare_keyed checks the arguments as bydb_scan_agg_keyed does (same codes) and copies the query and the key.
+ * Every execution returns what bydb_scan_agg_keyed returns for the same arguments at that moment: code and device-error text
+ * (the block a max_values error names is the one whose value went over the cap first, which varies between plain calls too),
+ * key table, rows, values bit for bit, and the counters (rows_scanned, rows_matched, page_bytes, blocks_scanned, blocks_slow_lane,
+ * slow_lane_reasons, blocks_express_lane) summed over the passes.  Free each result with bydb_keyed_result_free.
+ * Schedule: the first execution runs the plain keyed path; the second discovers the key values once and captures the step -- the
+ * V passes, the insertion order, finalisation and the mapping of rows to (series group, key value) -- as ONE CUDA graph; later
+ * executions replay it, with the key table found at the capture.  Discovery is a function of what the handles name, so the graph
+ * is dropped, and discovery and the capture run again, when a handle stops naming the part object it was captured with; a handle
+ * that names no part any more fails with BYDB_ENOENT.  A query whose discovery fails (above max_values, a plain key page, a
+ * 65-byte value, a key of the wrong type), whose parts overlap in time, or whose state cannot be allocated or captured, keeps
+ * the plain keyed path for good.  V = 0 (no block selected) needs no graph: no rows, no keys, zero stats.
+ * Stats of a replay: h2d_bytes = 0; scan_kernel_ms = 0 and device_ms = the whole graph (as bydb_scan_agg_prepared);
+ * kernel_launches = the plain call's (discovery's two kernels give way to the step's reset kernel and the row-mapping kernel);
+ * d2h_bytes = the size of its ONE copy: with A aggregations and R = min(top_n, V*G) or V*G result rows, each term rounded up to
+ * 256 B,
+ *   256 + A + 4*R + 8*R + 8*R*A + 8*R*A      the result rows (the finalisation's read-back over V*G groups)
+ *   + 8*R                                   the (series group, key value) of each row
+ *   + 256*V                                 each pass's zero page (counters and device error).
+ * Device memory a captured keyed query keeps until bydb_query_release_keyed, or until the graph is dropped; it is not charged to
+ * hbm_budget_bytes.  With GP = V*G composite groups, F fields, NS series, P parts and NB blocks in them, each term rounded up to
+ * 256 B:
+ *   2 * (56*GP*F + 8*GP + 8*F)                                                       the composite table and its permuted copy
+ *   + 8*V*F + 8*V*NS + 4*V*NS                                                        the passes' column types, Kts, Krow
+ *   + 4*NS*V + 4*GP + 4*GP + 16                                                      the insertion order (slots, first series, perm)
+ *   + 256 + 12*NS + 4*(G+1) + NB*(40 + 32*F) + NS*(32*F + 8) + 4*NS*P (left out above 16 Mi entries)   one scan scratch, shared by the passes
+ *   + GP*(16*A + 9) + 16 + A + R*(12 + 16*A)                                          finalisation over GP groups and the result rows
+ *   + 8*R + 256*V                                                                    the row mapping and the passes' zero pages.
+ * One execution at a time per handle; different handles, keyed or plain, run concurrently. */
+typedef struct bydb_prepared_keyed bydb_prepared_keyed;
+int bydb_query_prepare_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out);
+int bydb_scan_agg_keyed_prepared(bydb_ctx *ctx, bydb_prepared_keyed *pq, bydb_keyed_result *out);
+void bydb_query_release_keyed(bydb_ctx *ctx, bydb_prepared_keyed *pq);
 
 /* ---- multi-GPU map/reduce: per-rank partial tables, one collective, one finalize ----
  * Layout of a partial table for (n_groups G, n_fields F = distinct aggregated fields):

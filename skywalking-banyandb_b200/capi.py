@@ -107,7 +107,7 @@ class _Layout(C.Structure):
 # every symbol include/bydb_gpu.h declares (tests/test_capi_symbols.py checks the list against the header)
 EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_release", "bydb_part_info", "bydb_part_fallback_pages", "bydb_part_directory",
            "bydb_scan_agg", "bydb_scan_agg_host", "bydb_result_free", "bydb_query_prepare", "bydb_scan_agg_prepared",
-           "bydb_query_release", "bydb_partials_layout",
+           "bydb_query_release", "bydb_query_prepare_keyed", "bydb_scan_agg_keyed_prepared", "bydb_query_release_keyed", "bydb_partials_layout",
            "bydb_scan_partials", "bydb_partials_combine", "bydb_reduce_finalize", "bydb_partials_rows", "bydb_partial_rows_free", "bydb_comm_export", "bydb_comm_connect",
            "bydb_scan_reduce", "bydb_scan_reduce_prepared", "bydb_scan_reduce_host", "bydb_scan_agg_keyed", "bydb_keyed_result_free",
            "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed", "bydb_scan_partials_keyed", "bydb_keyed_partial_rows_free",
@@ -154,6 +154,10 @@ def load_library():
     L.bydb_scan_agg_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_Result)]
     L.bydb_query_release.argtypes = [C.c_void_p, C.c_void_p]
     L.bydb_query_release.restype = None
+    L.bydb_query_prepare_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(C.c_void_p)]
+    L.bydb_scan_agg_keyed_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_KeyedResult)]
+    L.bydb_query_release_keyed.argtypes = [C.c_void_p, C.c_void_p]
+    L.bydb_query_release_keyed.restype = None
     L.bydb_partials_layout.argtypes = [C.POINTER(_Query), C.POINTER(_Layout)]
     L.bydb_scan_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(_Stats)]
     L.bydb_partials_combine.argtypes = [C.c_void_p, C.POINTER(_Query), C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p]
@@ -396,6 +400,24 @@ class GraphQuery:
             self._h = None
 
 
+class KeyedGraphQuery:
+    """A stored-tag group-by held by the library (bydb_query_prepare_keyed): its passes, order and finalisation are replayed as
+    one CUDA graph from its third run on.  run() gives what Context.scan_agg_keyed gives."""
+
+    def __init__(self, ctx: "Context", handle, q: Query):
+        self._ctx, self._h, self._q = ctx, handle, q
+
+    def run(self) -> Result:
+        r = _KeyedResult()
+        _check(self._ctx._L.bydb_scan_agg_keyed_prepared(self._ctx._h, self._h, C.byref(r)))
+        return self._ctx._read_keyed(self._q, r)
+
+    def release(self):
+        if self._h:
+            self._ctx._L.bydb_query_release_keyed(self._ctx._h, self._h)
+            self._h = None
+
+
 def keyed_reduce_slot_bytes(q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> int:
     """bydb_keyed_reduce_slot_bytes (host only): the mailbox slot a rank of a keyed collective needs at max_values key values."""
     keep: list = []
@@ -480,6 +502,16 @@ class Context:
         r = _KeyedResult()
         _check(self._L.bydb_scan_agg_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
         return self._read_keyed(q, r)
+
+    def prepare_keyed(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> "KeyedGraphQuery":
+        """The prepared form of scan_agg_keyed (bydb_query_prepare_keyed): argument errors are raised here, as scan_agg_keyed
+        raises them; the handle's run() answers as scan_agg_keyed does at that moment."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        h = C.c_void_p()
+        _check(self._L.bydb_query_prepare_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(h)))
+        return KeyedGraphQuery(self, h, q)
 
     def _read_keyed(self, q: Query, r: "_KeyedResult") -> Result:
         try:

@@ -994,6 +994,7 @@ struct KeyedPass {
     int64_t *kts;       // [n_series] see ReduceParams::Kts
     uint32_t *krow;     // [n_series]
     int64_t *span;      // [2 * n_series] see ReduceParams::span, or NULL
+    ZeroPage *zero = nullptr;  // a captured keyed step: the pass's own zero page, reset at the head of the step; NULL: the scratch's
 };
 
 // device scratch of run_scan: zero page | staging (sids, order, group_start) | block lists | block and series partials |
@@ -1028,7 +1029,8 @@ ScanLayout scan_layout(const StageLayout &st, size_t NB, size_t F, size_t n_part
 
 // resident: the scratch is a view into a prepared query's StepState whose staging was uploaded when the state was built, and the
 // step is being captured for replay: one reset kernel instead of the memsets, no staging copy, and the zero page is left for
-// finalize_enqueue to read back with the result rows.
+// finalize_enqueue to read back with the result rows.  A pass of a captured keyed step (kp->zero set) launches no reset of its
+// own: its zero page and first_block were reset at the head of that step.
 int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cudaStream_t stream, uint8_t *d_table, const TableLayout &tl,
              bydb_stats *stats, int batch = 0, const KeyedPass *kp = nullptr, Scratch *resident = nullptr) {
     cudaEvent_t *ev = slot.ev + 4 * batch;
@@ -1053,11 +1055,11 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     Scratch &sc = resident ? *resident : pooled;
     CUDA_TRY(sc.alloc(sl.total, stream));
     uint8_t *d = sc.base;
-    ZeroPage *z = reinterpret_cast<ZeroPage *>(d + sl.off_zero);
-    if (resident) {
+    ZeroPage *z = kp && kp->zero ? kp->zero : reinterpret_cast<ZeroPage *>(d + sl.off_zero);
+    if (resident && !(kp && kp->zero)) {  // a keyed step's reset kernel also covers first_block, which plan_blocks writes alike in every pass
         launch_step_reset(reinterpret_cast<uint32_t *>(z), use_first ? reinterpret_cast<uint32_t *>(d + off_first) : nullptr, sl.n_first, stream);
         if (stats) stats->kernel_launches += 1;
-    } else {
+    } else if (!resident) {
         CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
         if (use_first) CUDA_TRY(cudaMemsetAsync(d + off_first, 0xff, sl.n_first * 4, stream));
         CUDA_TRY(cudaMemcpyAsync(d + off_sids, h, st.bytes, cudaMemcpyHostToDevice, stream));
@@ -1243,8 +1245,9 @@ int table_status(uint32_t e) {
 // fl = final_layout() of the query, launches = kernels launched, read_back = bytes of that copy.  d_zero: the step's zero page on
 // the device, gathered by the last kernel into kZeroPageBytes behind fl.total and read back in the same copy (it lands at
 // host_off + fl.out_bytes); NULL: the caller reads the zero page back itself.
-int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t stream, const uint8_t *d_table, const TableLayout &tl,
-                     size_t host_off, Scratch &sc, FinalLayout &fl, uint32_t &launches, size_t &read_back, const uint8_t *d_zero = nullptr) {
+// finalize_launch: the same up to the kernels; the read-back region is sc.base + fl.o_out, read_back bytes, for the caller to copy.
+int finalize_launch(const bydb_query *q, const Plan &plan, cudaStream_t stream, const uint8_t *d_table, const TableLayout &tl, Scratch &sc,
+                    FinalLayout &fl, uint32_t &launches, size_t &read_back, const uint8_t *d_zero = nullptr) {
     const size_t F = plan.fcols.size();
     const int32_t G = plan.n_groups;
     const size_t A = q->n_aggs;
@@ -1296,8 +1299,14 @@ int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
         sp.zero_dst = reinterpret_cast<uint32_t *>(d + fl.total);
     }
     launches = launch_finalize_select(fp, sp, stream);
+    return 0;
+}
+int finalize_enqueue(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t stream, const uint8_t *d_table, const TableLayout &tl,
+                     size_t host_off, Scratch &sc, FinalLayout &fl, uint32_t &launches, size_t &read_back, const uint8_t *d_zero = nullptr) {
+    int rc = finalize_launch(q, plan, stream, d_table, tl, sc, fl, launches, read_back, d_zero);
+    if (rc) return rc;
     if (slot.ensure_pinned(host_off + read_back)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned + host_off, d + fl.o_out, read_back, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned + host_off, sc.base + fl.o_out, read_back, cudaMemcpyDeviceToHost, stream));
     return 0;
 }
 
@@ -1484,7 +1493,7 @@ bool check_held_parts(bydb_ctx *ctx, const std::vector<bydb_part_h> &parts, cuda
         else if (same && it->second != held[i]) same = false;
     }
     if (missing || !same) {
-        cudaGraphExecDestroy(exec);
+        if (exec) cudaGraphExecDestroy(exec);  // a keyed step that found no key value holds parts but no graph
         exec = nullptr;
         held.clear();
     }
@@ -1895,9 +1904,12 @@ int discover_keys(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key,
 
 // 2. one scan pass per value v (the key as an extra predicate) into slice v of the composite table tlc (V x G groups, value-major)
 // at `table`, with the pass's column types at coltype + v * F and where each series first shows v at kts / krow + v * NS; the
-// first pass also writes the series' spans when `span` is set.  Every pass is synchronised and its device errors collected.
+// first pass also writes the series' spans when `span` is set.  Every pass is synchronised and its device errors collected --
+// unless `resident` is given (a keyed step being captured): then the passes share that scan scratch, pass v keeps its counters
+// and device error in zero page v of `zero_pages` (kZeroPageBytes each) for the step's one read-back, and nothing synchronises.
 int run_keyed_passes(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Plan &plan, ExecSlot &slot, const KeyValues &values,
-                     const TableLayout &tlc, uint8_t *table, int64_t *coltype, int64_t *kts, uint32_t *krow, int64_t *span, bydb_stats *stats) {
+                     const TableLayout &tlc, uint8_t *table, int64_t *coltype, int64_t *kts, uint32_t *krow, int64_t *span, bydb_stats *stats,
+                     Scratch *resident = nullptr, uint8_t *zero_pages = nullptr) {
     const bool int64_key = key->value_type == BYDB_VT_INT64;
     const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
     std::vector<bydb_pred> preds(q->preds, q->preds + q->n_preds);
@@ -1928,6 +1940,11 @@ int run_keyed_passes(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *k
         pass.kts = kts + v * NS;
         pass.krow = krow + v * NS;
         pass.span = v == 0 ? span : nullptr;
+        if (resident) {
+            pass.zero = reinterpret_cast<ZeroPage *>(zero_pages + v * kZeroPageBytes);
+            if (int rc = run_scan(ctx, &qv, plan, slot, slot.stream, table, tlc, stats, 0, &pass, resident)) return rc;
+            continue;
+        }
         int rc = run_scan(ctx, &qv, plan, slot, slot.stream, table, tlc, stats, 0, &pass);
         cudaError_t ce = cudaStreamSynchronize(slot.stream);  // also on failure: nothing may be in flight when the slot goes back
         if (!rc && ce != cudaSuccess) rc = fail(BYDB_EIO, cudaGetErrorString(ce));
@@ -1954,34 +1971,51 @@ void set_key_table(Out *out, KeyedOwner *owner, const KeyValues &values) {
 
 // 3. insertion order of the V x G composite groups from where each series first shows each value (kts / krow): ko.perm lists
 // the composite groups v * G + g in insertion order, the *ko.n_present that appeared first, in scratch `kb` (enqueued, not
-// synchronised; the staging of the series groups in slot.pinned is in flight).
+// synchronised; the staging of the series groups in slot.pinned is in flight).  `resident`: a keyed step being captured -- its
+// step state holds the order's arrays (the slots preset by the step's reset kernel) and the staging it uploaded before the capture.
 int keyed_order(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, const int64_t *kts, const uint32_t *krow, Scratch &kb,
-                KeyOrderParams &ko, bydb_stats &stats) {
+                KeyOrderParams &ko, bydb_stats &stats, const KeyOrderParams *resident = nullptr) {
     cudaStream_t stream = slot.stream;
     const size_t NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
-    const StageLayout st = stage_layout(NS, G);
-    Carve carve;
-    const size_t b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16), b_stage = carve(st.bytes);
-    CUDA_TRY(kb.alloc(carve.o, stream));
-    CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
-    memset(&ko, 0, sizeof ko);
+    if (resident) {
+        ko = *resident;
+    } else {
+        const StageLayout st = stage_layout(NS, G);
+        Carve carve;
+        const size_t b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16), b_stage = carve(st.bytes);
+        CUDA_TRY(kb.alloc(carve.o, stream));
+        CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
+        memset(&ko, 0, sizeof ko);
+        // order | group_start of the series groups: staged again (run_scan's copies live in its own scratch)
+        stage_series(q, st, slot.pinned);
+        CUDA_TRY(cudaMemcpyAsync(kb.base + b_stage, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream));
+        ko.order = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_order);
+        ko.group_start = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_gstart);
+        ko.slot = reinterpret_cast<int32_t *>(kb.base + b_slot);
+        ko.first_series = reinterpret_cast<int32_t *>(kb.base + b_first);
+        ko.perm = reinterpret_cast<int32_t *>(kb.base + b_perm);
+        ko.n_present = reinterpret_cast<uint32_t *>(kb.base + b_np);
+    }
     ko.n_groups = static_cast<int32_t>(G);
     ko.n_values = static_cast<uint32_t>(V);
     ko.n_series = static_cast<uint32_t>(NS);
-    // order | group_start of the series groups: staged again (run_scan's copies live in its own scratch)
-    stage_series(q, st, slot.pinned);
-    CUDA_TRY(cudaMemcpyAsync(kb.base + b_stage, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream));
-    ko.order = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_order);
-    ko.group_start = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_gstart);
     ko.Kts = kts;
     ko.Krow = krow;
-    ko.slot = reinterpret_cast<int32_t *>(kb.base + b_slot);
-    ko.first_series = reinterpret_cast<int32_t *>(kb.base + b_first);
-    ko.perm = reinterpret_cast<int32_t *>(kb.base + b_perm);
-    ko.n_present = reinterpret_cast<uint32_t *>(kb.base + b_np);
     launch_key_order(ko, stream);
     stats.kernel_launches += 2;
     return 0;
+}
+
+// the rows of a finalised keyed answer, which come out of the finalisation in composite terms, as (series group, key value):
+// row r takes pairs[2r] / pairs[2r + 1]
+void set_row_keys(bydb_keyed_result *out, KeyedOwner *owner, const int32_t *pairs) {
+    auto *ro = static_cast<ResultOwner *>(out->base.owner);
+    owner->key_id.resize(ro->group_id.size());
+    for (size_t r = 0; r < ro->group_id.size(); ++r) {
+        ro->group_id[r] = pairs[2 * r];
+        owner->key_id[r] = pairs[2 * r + 1];
+    }
+    out->key_id = owner->key_id.data();
 }
 
 // 4a. bydb_scan_agg_keyed / bydb_scan_reduce_keyed: after the order, the table at `table` reordered, the ordinary finalisation /
@@ -2012,14 +2046,14 @@ int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V
     CUDA_TRY(cudaStreamSynchronize(stream));
     out->base.stats.d2h_bytes += GP * 4;
     // rows carry the position in insertion order: back to (group of the series, key value)
-    auto *ro = static_cast<ResultOwner *>(out->base.owner);
-    owner->key_id.resize(ro->group_id.size());
-    for (size_t r = 0; r < ro->group_id.size(); ++r) {
-        const int32_t comp = perm[static_cast<size_t>(ro->group_id[r])];
-        owner->key_id[r] = comp / static_cast<int32_t>(G);
-        ro->group_id[r] = comp % static_cast<int32_t>(G);
+    const std::vector<int32_t> &pos = static_cast<ResultOwner *>(out->base.owner)->group_id;
+    std::vector<int32_t> pairs(2 * pos.size());
+    for (size_t r = 0; r < pos.size(); ++r) {
+        const int32_t comp = perm[static_cast<size_t>(pos[r])];
+        pairs[2 * r] = comp % static_cast<int32_t>(G);
+        pairs[2 * r + 1] = comp / static_cast<int32_t>(G);
     }
-    out->key_id = owner->key_id.data();
+    set_row_keys(out, owner, pairs.data());
     return 0;
 }
 
@@ -2217,6 +2251,242 @@ void bydb_keyed_result_free(bydb_ctx *ctx, bydb_keyed_result *r) {
     bydb_result_free(ctx, &r->base);
     delete static_cast<KeyedOwner *>(r->owner);
     memset(r, 0, sizeof *r);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Prepared group-by on a stored tag: the V passes, the insertion order, the finalisation and the row mapping captured as ONE
+// graph.  Discovery runs once per capture: its inputs (the parts a handle names, series, range, key) are fixed while the handles
+// keep naming the parts the step was captured with, so the key table is a property of the capture, like the block plan.
+// Everything here is additive: bydb_scan_agg_keyed is untouched.
+// ------------------------------------------------------------------------------------------------
+extern "C++" {
+struct bydb_prepared_keyed {
+    bydb_prepared *pq = nullptr;   // the query's deep copy, its slot, events, graph, step state and held parts
+    std::string family, tag;       // the key's strings: key.family / key.tag point here
+    bydb_group_key key{};
+    uint32_t cap = 0;              // distinct values accepted (check_group_key)
+    KeyValues values;              // found when the step was captured: the key table of every replay
+    bool no_values = false;        // discovery found no value (V = 0): the answer is empty and needs no graph
+    size_t pairs_off = 0, zero_off = 0;  // in the replay's read-back image: the rows' (group, key) pairs, the passes' zero pages
+    ~bydb_prepared_keyed() { prepared_destroy(pq); }
+};
+
+namespace {
+// Discovers the key values and captures the keyed step into k->pq->exec, in a step state of its own:
+//   composite table | permuted table | the passes' column types | Kts | Krow | the order's slots, first_series, perm, n_present |
+//   one scan scratch (scan_layout, the passes run one after another) | finalisation over V x G groups, then the rows' (group, key)
+//   pairs and the V zero pages, so that one copy reads back the rows, their pairs and the passes' counters and errors.
+// Leaves neither a graph nor no_values when this execution, or (capturable cleared) every later one, takes the plain path: a part
+// is missing, the parts overlap, discovery fails (its refusal is the plain call's), or the state or the capture cannot be had.
+void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k) {
+    bydb_prepared *p = k->pq;
+    const bydb_query *q = &p->q;
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up
+    Plan plan;
+    if (make_plan(ctx, q, nullptr, plan)) return;
+    ExecSlot &slot = *p->slot;
+    cudaStream_t stream = slot.stream;
+    bydb_stats discovery{};
+    KeyValues values;
+    if (parts_overlap(plan.parts, q->tmin, q->tmax) || discover_keys(ctx, q, &k->key, k->cap, plan, slot, &discovery, values)) {
+        p->capturable = false;
+        return;
+    }
+    const size_t V = values.size(), F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    if (V == 0) {
+        k->values.clear();
+        k->no_values = true;
+        p->held = plan.parts;
+        p->held_gen = gen;
+        return;
+    }
+    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) {
+        p->capturable = false;
+        return;
+    }
+    const TableLayout tlc(GP, F);
+    const StageLayout st = stage_layout(NS, G);
+    const ScanLayout sl = scan_layout(st, plan.total_blocks, F, plan.parts.size(), true);
+    const FinalLayout fl = final_layout(GP, q->n_aggs, q->top_n);
+    const size_t b_pairs = align_up(fl.cap * 8, 256), b_zero = V * kZeroPageBytes;
+    Carve carve;
+    const size_t o_src = carve(tlc.total), o_dst = carve(tlc.total), o_ct = carve(V * F * 8), o_kts = carve(V * NS * 8), o_krow = carve(V * NS * 4),
+                 o_slot = carve(NS * V * 4), o_first = carve(GP * 4), o_perm = carve(GP * 4), o_np = carve(16), o_scan = carve(sl.total),
+                 o_fin = carve(fl.total + b_pairs + b_zero);
+    p->host_off = st.stride;  // the read-back lands behind the staging area, as in the plain prepared step
+    p->read_back = fl.out_bytes + b_pairs + b_zero;
+    if (slot.ensure_pinned(p->host_off + p->read_back) || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
+        cudaGetLastError();
+        p->step_state = nullptr;
+        p->capturable = false;
+        return;
+    }
+    uint8_t *S = p->step_state, *fin_base = S + o_fin, *zero_pages = fin_base + fl.total + b_pairs;
+    // the staging goes up once: the passes and the order read it from the step state on every replay
+    stage_series(q, st, slot.pinned);
+    cudaError_t e = cudaMemcpyAsync(S + o_scan + sl.off_sids, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e == cudaSuccess) e = cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        drop_step(p);
+        p->capturable = false;
+        return;
+    }
+    bydb_stats &cs = p->captured;
+    memset(&cs, 0, sizeof cs);
+    int64_t *ct = reinterpret_cast<int64_t *>(S + o_ct), *kts = reinterpret_cast<int64_t *>(S + o_kts);
+    uint32_t *krow = reinterpret_cast<uint32_t *>(S + o_krow);
+    KeyedResetParams rp;
+    memset(&rp, 0, sizeof rp);
+    rp.zero[0] = reinterpret_cast<uint32_t *>(ct);
+    rp.n_zero[0] = V * F * 2;
+    rp.zero[1] = reinterpret_cast<uint32_t *>(zero_pages);
+    rp.n_zero[1] = b_zero / 4;
+    rp.ones[0] = sl.n_first ? reinterpret_cast<uint32_t *>(S + o_scan + sl.off_first) : nullptr;
+    rp.n_ones[0] = sl.n_first;
+    rp.ones[1] = reinterpret_cast<uint32_t *>(S + o_slot);
+    rp.n_ones[1] = NS * V;
+    launch_keyed_step_reset(rp, stream);
+    cs.kernel_launches += 1;
+    Scratch scan, kb, fin;
+    scan.view(S + o_scan, sl.total);
+    fin.view(fin_base, fl.total + b_pairs + b_zero);
+    int rc = run_keyed_passes(ctx, q, &k->key, plan, slot, values, tlc, S + o_src, ct, kts, krow, nullptr, &cs, &scan, zero_pages);
+    KeyOrderParams res, ko;
+    memset(&res, 0, sizeof res);
+    res.order = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_order);
+    res.group_start = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_gstart);
+    res.slot = reinterpret_cast<int32_t *>(S + o_slot);
+    res.first_series = reinterpret_cast<int32_t *>(S + o_first);
+    res.perm = reinterpret_cast<int32_t *>(S + o_perm);
+    res.n_present = reinterpret_cast<uint32_t *>(S + o_np);
+    if (!rc) rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, cs, &res);
+    FinalLayout flc;
+    uint32_t fin_launches = 0;
+    size_t fin_back = 0;
+    if (!rc) {
+        launch_permute_table(tlc.at(S + o_dst), tlc.at(S + o_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), ct,
+                             static_cast<uint32_t>(V), stream);
+        Plan planc = plan;
+        planc.n_groups = static_cast<int32_t>(GP);
+        rc = finalize_launch(q, planc, stream, S + o_dst, tlc, fin, flc, fin_launches, fin_back);
+    }
+    if (!rc) {
+        launch_keyed_row_map(reinterpret_cast<const int32_t *>(fin_base + fl.o_sg), reinterpret_cast<const uint32_t *>(fin_base + fl.o_cnt), ko.perm,
+                             static_cast<uint32_t>(G), static_cast<uint32_t>(fl.cap), reinterpret_cast<int32_t *>(fin_base + fl.total), stream);
+        if (cudaMemcpyAsync(slot.pinned + p->host_off, fin_base + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+    }
+    cudaGraph_t graph = nullptr;
+    e = cudaStreamEndCapture(stream, &graph);
+    if (!rc && e == cudaSuccess && graph) e = cudaGraphInstantiate(&p->exec, graph, 0);
+    if (graph) cudaGraphDestroy(graph);
+    if (rc || e != cudaSuccess || !p->exec) {
+        cudaGetLastError();
+        drop_step(p);
+        p->capturable = false;
+        return;
+    }
+    cs.kernel_launches += 1 + fin_launches + 1;  // permute_table, finalisation + row selection, the row mapping
+    cs.d2h_bytes = p->read_back;
+    p->fl = fl;
+    p->express = false;  // the key predicate keeps every pass off the express lane
+    k->values = std::move(values);
+    k->no_values = false;
+    k->pairs_off = fl.out_bytes;
+    k->zero_off = fl.out_bytes + b_pairs;
+    p->held = plan.parts;
+    p->held_gen = gen;
+}
+
+// One replay, synchronised and parsed: the passes' counters add up and the first pass with a device error decides, as the plain
+// path's pass-by-pass collection has it; then the table's carried status, the rows and their (group, key) pairs.
+int keyed_replay(bydb_ctx *ctx, bydb_prepared_keyed *k, bydb_keyed_result *out) {
+    bydb_prepared *p = k->pq;
+    uint8_t *image = p->slot->pinned + p->host_off;
+    const size_t V = k->values.size();
+    memset(image + k->zero_off, 0, V * kZeroPageBytes);  // a replay that fails to launch cannot report the previous one's status
+    auto page = [&](size_t v) -> const ZeroPage & { return *reinterpret_cast<const ZeroPage *>(image + k->zero_off + v * kZeroPageBytes); };
+    bydb_stats &stats = out->base.stats;
+    int rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, false, page(0), &stats);
+    for (size_t v = 1; !rc && v < V; ++v) rc = read_zero_page(page(v), false, &stats);
+    if (rc) return rc;
+    auto owner = new KeyedOwner();
+    out->owner = owner;
+    KeyedUndo<bydb_keyed_result> undo{ctx, out};
+    set_key_table(out, owner, k->values);
+    rc = finalize_parse(image, p->fl, true, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, reinterpret_cast<const int32_t *>(image + k->pairs_off));
+    undo.done = true;
+    return 0;
+}
+}  // namespace
+}  // extern "C++"
+
+int bydb_query_prepare_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out) {
+    return guarded([&]() -> int {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    *out = nullptr;
+    // the argument checks of bydb_scan_agg_keyed, in its order
+    int rc = validate_query(q, true);
+    if (rc) return rc;
+    uint32_t cap = 0;
+    rc = check_group_key(q, key, cap);
+    if (rc) return rc;
+    std::unique_ptr<bydb_prepared_keyed> k(new bydb_prepared_keyed());
+    rc = bydb_query_prepare(ctx, q, &k->pq);
+    if (rc) return rc;
+    k->family = key->family;
+    k->tag = key->tag;
+    k->key = *key;
+    k->key.family = k->family.c_str();
+    k->key.tag = k->tag.c_str();
+    k->cap = cap;
+    *out = k.release();
+    return 0;
+    });
+}
+
+void bydb_query_release_keyed(bydb_ctx *ctx, bydb_prepared_keyed *k) {
+    if (ctx) cudaSetDevice(ctx->device);
+    delete k;
+}
+
+int bydb_scan_agg_keyed_prepared(bydb_ctx *ctx, bydb_prepared_keyed *k, bydb_keyed_result *out) {
+    return guarded([&]() -> int {
+    if (!ctx || !k || !out) return fail(BYDB_EINVAL, "NULL argument");
+    memset(out, 0, sizeof *out);
+    bydb_prepared *p = k->pq;
+    std::lock_guard<std::mutex> lk(p->mu);
+    g_last_dev_err = 0;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    auto plain = [&] { return scan_keyed_impl(ctx, &p->q, &k->key, out); };
+    // as bydb_scan_agg_prepared: the first execution runs the plain keyed path, the second one captures, later ones replay
+    if (p->runs++ == 0 || !p->capturable) return plain();
+    // the handles can only have changed their parts if one was registered or released since `held` was last compared
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
+    if ((p->exec || k->no_values) && gen != p->held_gen) {
+        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
+        if (p->held.empty()) {  // a handle stopped naming its captured part: discovery and the capture run again
+            drop_step(p);
+            k->no_values = false;
+        }
+        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
+        p->held_gen = gen;
+    }
+    if (!p->exec && !k->no_values) {
+        keyed_capture(ctx, k);
+        if (!p->exec && !k->no_values) return plain();
+    }
+    if (k->no_values) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
+        auto owner = new KeyedOwner();
+        out->owner = owner;
+        set_key_table(out, owner, KeyValues());
+        return 0;
+    }
+    return keyed_replay(ctx, k, out);
+    });
 }
 
 

@@ -4256,6 +4256,41 @@ void launch_step_reset(uint32_t *zero_page, uint32_t *first_block, size_t n_firs
     step_reset_kernel<<<blocks, 256, 0, s>>>(zero_page, first_block, n_first);
 }
 
+// the head of a replayed keyed step: the memsets of the plain keyed path as one node (see KeyedResetParams)
+__global__ void keyed_step_reset_kernel(const KeyedResetParams p) {
+    const size_t i0 = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x, stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        for (size_t i = i0; i < p.n_zero[r]; i += stride) p.zero[r][i] = 0;
+        for (size_t i = i0; i < p.n_ones[r]; i += stride) p.ones[r][i] = 0xffffffffu;
+    }
+}
+void launch_keyed_step_reset(const KeyedResetParams &p, cudaStream_t s) {
+    KeyedResetParams q = p;
+    size_t n = 0;
+    for (int r = 0; r < 2; ++r) {
+        if (!q.zero[r]) q.n_zero[r] = 0;
+        if (!q.ones[r]) q.n_ones[r] = 0;
+        n = std::max(n, std::max(q.n_zero[r], q.n_ones[r]));
+    }
+    const size_t want = (n + 255) / 256;
+    const unsigned blocks = want < 1 ? 1u : want > 1024 ? 1024u : static_cast<unsigned>(want);
+    keyed_step_reset_kernel<<<blocks, 256, 0, s>>>(q);
+}
+
+__global__ void keyed_row_map_kernel(const int32_t *sel_group, const uint32_t *sel_count, const int32_t *perm, uint32_t n_groups, uint32_t cap,
+                                     int32_t *pairs) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= min(*sel_count, cap)) return;
+    const int32_t c = perm[sel_group[r]], g = static_cast<int32_t>(n_groups);
+    pairs[2 * r] = c % g;
+    pairs[2 * r + 1] = c / g;
+}
+void launch_keyed_row_map(const int32_t *sel_group, const uint32_t *sel_count, const int32_t *perm, uint32_t n_groups, uint32_t cap,
+                          int32_t *pairs, cudaStream_t s) {
+    keyed_row_map_kernel<<<(cap + 255) / 256, 256, 0, s>>>(sel_group, sel_count, perm, n_groups, cap, pairs);
+}
+
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s) {
     if (p.total_blocks == 0) return;
     const int threads = 256;
@@ -4460,6 +4495,8 @@ void preload_kernels() {
     (void)cudaFuncGetAttributes(&ka, merge_first_kernel);
     cudaFuncAttributes a;
     cudaFuncGetAttributes(&a, step_reset_kernel);
+    cudaFuncGetAttributes(&a, keyed_step_reset_kernel);
+    cudaFuncGetAttributes(&a, keyed_row_map_kernel);
     cudaFuncGetAttributes(&a, plan_blocks_kernel);
     cudaFuncGetAttributes(&a, scan_blocks_kernel<true>);
     cudaFuncGetAttributes(&a, scan_blocks_kernel<false>);

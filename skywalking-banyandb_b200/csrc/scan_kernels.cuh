@@ -379,6 +379,22 @@ void launch_combine_keyed(const KeyedUnionParams &p, cudaStream_t s);
 // dst[j] = src[perm[j]] for every group row of a partial table; coltype = the passes' column types merged
 void launch_permute_table(const TablePtrs &dst, const TablePtrs &src, const int32_t *perm, uint32_t n_groups, uint32_t n_fcols,
                           const int64_t *pass_coltype, uint32_t n_passes, cudaStream_t s);
+// ---- a replayed keyed step (bydb_scan_agg_keyed_prepared)
+// Everything the plain keyed path memsets, reset by ONE kernel at the head of the graph: the 32-bit words of zero[i] are set to 0
+// (the passes' column types, their zero pages), those of ones[i] to 0xffffffff (first_block, the key-order slots).  A NULL range
+// or a count of 0 is skipped.
+struct KeyedResetParams {
+    uint32_t *zero[2];
+    size_t n_zero[2];
+    uint32_t *ones[2];
+    size_t n_ones[2];
+};
+void launch_keyed_step_reset(const KeyedResetParams &p, cudaStream_t s);
+// The (series group, key value) of every selected row, in place of the host's read-back of perm: row r < min(*sel_count, cap)
+// is position sel_group[r] of the insertion order, composite group c = perm[sel_group[r]] = key * n_groups + group, and
+// pairs[2r] / pairs[2r + 1] = c % n_groups / c / n_groups.
+void launch_keyed_row_map(const int32_t *sel_group, const uint32_t *sel_count, const int32_t *perm, uint32_t n_groups, uint32_t cap,
+                          int32_t *pairs, cudaStream_t s);
 constexpr int kFusedFinalizeGroups = 8192;  // up to here one CTA finalises and selects in a single launch
 struct FinalizeParams;
 uint32_t launch_finalize_select(const FinalizeParams &fp, const SelectParams &p, cudaStream_t s);  // -> kernels launched
