@@ -411,6 +411,43 @@ typedef struct {
 int bydb_scan_partials_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out);
 void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r);
 
+/* Prepared map-phase answers: what a data node answers, refresh after refresh, for a query the liaison pushes down with
+ * agg_return_partial (a dashboard panel or an alert rule in a cluster).  The handles are those of the finalised forms above.
+ *   - Answers: every execution returns what the unprepared form returns at that moment, for the handle's query.
+ *       bydb_scan_partials_prepared: bydb_scan_partials (with stats) into a table, then bydb_partials_rows over it -- one row per
+ *         group with rows > 0 in group-id order, Partial.Value / .Count typed like the field, is_float per aggregate.  The scan's
+ *         device error comes first, then the status the table carries.  top_n is ignored, as bydb_partials_rows ignores it.
+ *         stats may be NULL; else it gets the counters of bydb_scan_partials, plus the row kernels' launches and read-back.
+ *       bydb_scan_partials_keyed_prepared: bydb_scan_partials_keyed -- rows in insertion order, the key table, counters summed
+ *         over the passes, the same refusals and codes.  Free the answer with bydb_keyed_partial_rows_free.
+ *     A device error's text names the block that met it first (a type mix, the cap), which varies between unprepared calls too.
+ *   - Schedule: the first execution runs the unprepared path, the second captures the step as ONE CUDA graph, later ones replay
+ *     it.  Parts that overlap in time (plain form; the keyed form answers BYDB_ENOTSUP as bydb_scan_partials_keyed does), a
+ *     discovery that fails, state or pinned staging that cannot be had, or a capture that fails keep the unprepared path.  A
+ *     handle that stops naming its captured part drops the step and captures again; one that names no part gives BYDB_ENOENT.
+ *   - One step per handle: a handle may answer in its finalised and its partial form, but keeps one captured step at a time; an
+ *     execution of the other form drops it and captures its own (bydb_scan_reduce_prepared's per-root graphs are apart).
+ *   - The graph ends in a kernel that writes the zero pages, the control word and exactly the present rows into the handle's
+ *     page-locked staging through its device address: the row count is known only on the device, so no copy node could be sized.
+ *   - Stats of a replay: h2d_bytes = 0; scan_kernel_ms = 0 and device_ms = the whole graph; with V key values (V = 1 for the plain
+ *     form), F distinct fields, A aggregations and n_rows rows,
+ *       d2h_bytes = 256*V + (8 + 8*F) + n_rows*(8 + 16*A)     the zero pages, the control word, the rows -- no padding;
+ *       kernel_launches: plain form = bydb_scan_partials' + 4 (the step's reset kernel, and the three kernels of
+ *         bydb_partials_rows: compaction, rows, copy), i.e. its own first execution's + 1; keyed form = bydb_scan_partials_keyed's
+ *         (discovery's two kernels give way to the step's reset kernel and the copy kernel).
+ *   - Device memory a captured step keeps until the handle is released or the step is dropped; it is not charged to
+ *     hbm_budget_bytes.  Each term rounded up to 256 B, with the names of bydb_query_prepare / bydb_query_prepare_keyed:
+ *       plain:  56*G*F + 8*G + 8*F                                                                  the partial table
+ *               + 256 + 12*NS + 4*(G+1) + NB*(36 + 32*F) + NS*(32*F + 8) + 4*NS*P (left out above 16 Mi entries)   the scan
+ *               + 4*G + 16 + (8 + 8*F) + G*(8 + 16*A)                                               compaction and the row image
+ *       keyed:  56*GP*F + 8*GP + 8*F                                                                the composite table
+ *               + 8*V*F + 8*V*NS + 4*V*NS + 4*NS*V + 4*GP + 4*GP + 16                               passes and insertion order
+ *               + 256 + 12*NS + 4*(G+1) + NB*(40 + 32*F) + NS*(32*F + 8) + 4*NS*P (as above)        one scan scratch
+ *               + 256*V + (8 + 8*F) + GP*(8 + 16*A)                                                 the zero pages and the row image
+ *     and the handle's page-locked staging holds the same read-back at its largest (256*V + 8 + 8*F + G*V*(8 + 16*A)). */
+int bydb_scan_partials_prepared(bydb_ctx *ctx, bydb_prepared *pq, bydb_partial_rows *out, bydb_stats *stats);
+int bydb_scan_partials_keyed_prepared(bydb_ctx *ctx, bydb_prepared_keyed *pq, bydb_keyed_partial_rows *out);
+
 /* ---- multi-GPU reduce behind the C ABI: one process (or thread) per GPU, no torch, no NCCL ----
  * Replaces the liaison gather + reduceAccumulator.Combine (pkg/query/logical/measure/measure_plan_aggregation.go:96-124,
  * measure_plan_distributed.go:254-328) inside one node: every rank owns a MAILBOX in its GPU's memory; in a collective

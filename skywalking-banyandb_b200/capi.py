@@ -107,7 +107,8 @@ class _Layout(C.Structure):
 # every symbol include/bydb_gpu.h declares (tests/test_capi_symbols.py checks the list against the header)
 EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_release", "bydb_part_info", "bydb_part_fallback_pages", "bydb_part_directory",
            "bydb_scan_agg", "bydb_scan_agg_host", "bydb_result_free", "bydb_query_prepare", "bydb_scan_agg_prepared",
-           "bydb_query_release", "bydb_query_prepare_keyed", "bydb_scan_agg_keyed_prepared", "bydb_query_release_keyed", "bydb_partials_layout",
+           "bydb_query_release", "bydb_query_prepare_keyed", "bydb_scan_agg_keyed_prepared", "bydb_query_release_keyed", "bydb_scan_partials_prepared",
+           "bydb_scan_partials_keyed_prepared", "bydb_partials_layout",
            "bydb_scan_partials", "bydb_partials_combine", "bydb_reduce_finalize", "bydb_partials_rows", "bydb_partial_rows_free", "bydb_comm_export", "bydb_comm_connect",
            "bydb_scan_reduce", "bydb_scan_reduce_prepared", "bydb_scan_reduce_host", "bydb_scan_agg_keyed", "bydb_keyed_result_free",
            "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed", "bydb_scan_partials_keyed", "bydb_keyed_partial_rows_free",
@@ -157,6 +158,8 @@ def load_library():
     L.bydb_query_prepare_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(C.c_void_p)]
     L.bydb_scan_agg_keyed_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_KeyedResult)]
     L.bydb_query_release_keyed.argtypes = [C.c_void_p, C.c_void_p]
+    L.bydb_scan_partials_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_PartialRows), C.POINTER(_Stats)]
+    L.bydb_scan_partials_keyed_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_KeyedPartialRows)]
     L.bydb_query_release_keyed.restype = None
     L.bydb_partials_layout.argtypes = [C.POINTER(_Query), C.POINTER(_Layout)]
     L.bydb_scan_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(_Stats)]
@@ -385,6 +388,18 @@ class GraphQuery:
         finally:
             self._ctx._L.bydb_result_free(self._ctx._h, C.byref(r))
 
+    def run_partials(self) -> Dict[str, object]:
+        """The map-phase form (bydb_scan_partials_prepared): the arrays of Context.partials_rows over a fresh
+        scan_partials table of this query, plus `stats`; graph replay from the third execution on."""
+        r, st = _PartialRows(), _Stats()
+        _check(self._ctx._L.bydb_scan_partials_prepared(self._ctx._h, self._h, C.byref(r), C.byref(st)))
+        try:
+            out: Dict[str, object] = dict(_read_partial_rows(r))
+            out["stats"] = Stats.of(st)
+            return out
+        finally:
+            self._ctx._L.bydb_partial_rows_free(self._ctx._h, C.byref(r))
+
     def run_reduce(self, root: int = 0) -> Result:
         """The collective form (bydb_scan_reduce_prepared): graph replay from the second execution on."""
         r = _Result()
@@ -411,6 +426,12 @@ class KeyedGraphQuery:
         r = _KeyedResult()
         _check(self._ctx._L.bydb_scan_agg_keyed_prepared(self._ctx._h, self._h, C.byref(r)))
         return self._ctx._read_keyed(self._q, r)
+
+    def run_partials(self) -> Dict[str, object]:
+        """The map-phase form (bydb_scan_partials_keyed_prepared): what Context.scan_partials_keyed gives at that moment."""
+        r = _KeyedPartialRows()
+        _check(self._ctx._L.bydb_scan_partials_keyed_prepared(self._ctx._h, self._h, C.byref(r)))
+        return self._ctx._read_keyed_partials(self._q, r)
 
     def release(self):
         if self._h:

@@ -17,6 +17,7 @@
 #include <future>
 #include <cstring>
 #include <memory>
+#include <type_traits>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -149,6 +150,15 @@ struct ExecSlot {
         pinned = fresh;
         pinned_bytes = want;
         return 0;
+    }
+    // the device address of pinned + off, through which a kernel writes the staging (rows_to_host_kernel); NULL if it has none
+    uint8_t *pinned_dev(size_t off) {
+        void *d = nullptr;
+        if (cudaHostGetDevicePointer(&d, pinned, 0) != cudaSuccess) {
+            cudaGetLastError();
+            return nullptr;
+        }
+        return static_cast<uint8_t *>(d) + off;
     }
     int create() {
         if (cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess) return -1;
@@ -1356,6 +1366,75 @@ int finalize_to_host(const bydb_query *q, const Plan &plan, ExecSlot &slot, cuda
     out->stats.kernel_launches += launches;
     return finalize_parse(slot.pinned, fl, carried_status, out);
 }
+
+// keyed_partial_rows_kernel over a table of V passes (V x G composite groups in `t`, pass column types at coltype): rows perm[j],
+// j < *n_present, into the image at `image` -- the control word, then the rows right behind it
+KeyedRowsParams rows_params(const bydb_query *q, const Plan &plan, size_t V, const TablePtrs &t, const int64_t *coltype, const int32_t *perm,
+                            const uint32_t *n_present, uint8_t *image) {
+    KeyedRowsParams kp;
+    memset(&kp, 0, sizeof kp);
+    kp.table = t;
+    kp.perm = perm;
+    kp.n_present = n_present;
+    kp.pass_coltype = coltype;
+    kp.n_groups = static_cast<uint32_t>(plan.n_groups);
+    kp.n_fcols = static_cast<uint32_t>(plan.fcols.size());
+    kp.n_aggs = q->n_aggs;
+    kp.n_passes = static_cast<uint32_t>(V);
+    for (size_t a = 0; a < q->n_aggs; ++a) {
+        kp.agg_fcol[a] = plan.agg_fcol[a];
+        kp.agg_func[a] = q->aggs[a].func;
+    }
+    kp.ctl = reinterpret_cast<uint32_t *>(image);
+    kp.rows = image + keyed_ctl_bytes(plan.fcols.size());
+    return kp;
+}
+
+// device scratch of emit_plain_rows: the present groups (perm, n_present), then the row image (control word and up to G rows)
+struct RowsLayout {
+    size_t o_perm, o_np, o_img, total;
+};
+RowsLayout rows_layout(const bydb_query *q, const Plan &plan) {
+    const size_t G = plan.tl.G;
+    RowsLayout rl;
+    Carve carve;
+    rl.o_perm = carve(G * 4);
+    rl.o_np = carve(16);
+    rl.o_img = carve(keyed_ctl_bytes(plan.fcols.size()) + G * keyed_row_bytes(q->n_aggs));
+    rl.total = carve.o;
+    return rl;
+}
+
+// pinned bytes of a plain partial answer: the staging of the scan, then (at its stride) the zero page, the control word and G rows
+size_t partial_pinned_bytes(const bydb_query *q, const Plan &plan) {
+    return stage_layout(q->n_series, plan.tl.G).stride + kZeroPageBytes + keyed_ctl_bytes(plan.fcols.size()) + plan.tl.G * keyed_row_bytes(q->n_aggs);
+}
+
+// The one emitter of a plain table's map-phase rows (bydb_partials_rows, and both paths of bydb_scan_partials_prepared): the groups
+// with rows > 0 compacted in group-id order, their wire rows written by keyed_partial_rows_kernel with the table as its one pass,
+// and rows_to_host_kernel bringing `page_bytes` at d_pages (the step's zero page; 0 = none), the control word and exactly the
+// present rows to the staging whose device address is h_dst.  `work`: rows_layout() bytes of device scratch.  Three launches.
+void emit_plain_rows(const bydb_query *q, const Plan &plan, cudaStream_t s, const uint8_t *d_table, uint8_t *work, const uint8_t *d_pages,
+                     size_t page_bytes, uint8_t *h_dst) {
+    const RowsLayout rl = rows_layout(q, plan);
+    const TablePtrs t = plan.tl.at(const_cast<uint8_t *>(d_table));  // read only
+    int32_t *perm = reinterpret_cast<int32_t *>(work + rl.o_perm);
+    uint32_t *n_present = reinterpret_cast<uint32_t *>(work + rl.o_np);
+    launch_present_groups(t.rows, static_cast<uint32_t>(plan.tl.G), perm, n_present, s);
+    launch_keyed_partial_rows(rows_params(q, plan, 1, t, t.coltype, perm, n_present, work + rl.o_img), plan.tl.G, s);
+    RowsCopyParams cp;
+    memset(&cp, 0, sizeof cp);
+    cp.pages = d_pages;
+    cp.image = work + rl.o_img;
+    cp.dst = h_dst;
+    cp.page_bytes = page_bytes;
+    cp.ctl_bytes = keyed_ctl_bytes(plan.fcols.size());
+    cp.row_bytes = keyed_row_bytes(q->n_aggs);
+    cp.max_rows = static_cast<uint32_t>(plan.tl.G);
+    launch_rows_to_host(cp, s);
+}
+constexpr uint32_t kPlainRowsLaunches = 3;
+
 int make_plan(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::shared_ptr<Part>> *given, Plan &plan) {
     if (given) {
         plan.parts = *given;
@@ -1438,13 +1517,15 @@ struct bydb_prepared {
     std::vector<std::shared_ptr<Part>> held;  // the parts whose device pointers are baked into the graph stay alive with it
     uint64_t held_gen = 0;             // bydb_ctx::parts_gen at which `held` was last compared with the handles
     // StepState: the device memory of the captured step, one allocation that lives as long as the graph.  Carved as
-    // partial table | run_scan's scratch (scan_layout) | finalize_enqueue's (final_layout) | the zero page's read-back image;
+    // partial table | run_scan's scratch (scan_layout) | finalize_enqueue's (final_layout) | the zero page's read-back image, or for
+    // a partial step | emit_plain_rows' (rows_layout);
     // the staging (sids | order | group_start) is uploaded into run_scan's region once, before the capture.
     uint8_t *step_state = nullptr;
     size_t zero_image_off = 0;         // where in the slot's pinned memory a replay's zero page lands
     size_t read_back = 0;              // bytes of the replay's one device-to-host copy
     bydb_stats captured{};             // host-side counters of one step (launch counts, byte counts)
     bool express = false;              // the captured step launches the express lane
+    bool partial_step = false;         // the captured step answers with map-phase rows (bydb_scan_partials[_keyed]_prepared)
     uint64_t runs = 0;
     bool capturable = true;
     // the collective form (bydb_scan_reduce_prepared): one captured graph per (root, slot parity)
@@ -1519,8 +1600,9 @@ int replay_graph(cudaGraphExec_t exec, ExecSlot &slot, cudaEvent_t t0, cudaEvent
 }
 
 // captures one step into p->exec, building the StepState it runs in; returns 0, or a code after leaving the stream out of
-// capture mode.  0 with p->exec == NULL: this query keeps the uncaptured path.
-int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
+// capture mode.  0 with p->exec == NULL: this query keeps the uncaptured path.  The tail after group_reduce: finalisation, row
+// selection and one read-back copy, or (partial) emit_plain_rows, whose last kernel writes the zero page and the rows to the staging.
+int prepared_capture(bydb_ctx *ctx, bydb_prepared *p, bool partial) {
     const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up: a later change is seen by the next run
     Plan plan;
     int rc = make_plan(ctx, &p->q, nullptr, plan);
@@ -1535,11 +1617,13 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
     const StageLayout st = stage_layout(p->q.n_series, tl.G);
     const ScanLayout sl = scan_layout(st, plan.total_blocks, plan.fcols.size(), plan.parts.size(), false);
     const FinalLayout fl = final_layout(tl.G, p->q.n_aggs, p->q.top_n);
+    const RowsLayout rl = rows_layout(&p->q, plan);
     p->host_off = st.stride;  // the read-back lands behind the staging area
-    if (slot.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    if (slot.ensure_pinned(partial ? partial_pinned_bytes(&p->q, plan) : step_pinned_bytes(&p->q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    uint8_t *h_dst = partial ? slot.pinned_dev(p->host_off) : nullptr;
     Carve carve;
-    const size_t off_table = carve(tl.total), off_scan = carve(sl.total), off_fin = carve(fl.total + kZeroPageBytes);
-    if (cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
+    const size_t off_table = carve(tl.total), off_scan = carve(sl.total), off_fin = carve(partial ? rl.total : fl.total + kZeroPageBytes);
+    if ((partial && !h_dst) || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
         cudaGetLastError();
         p->step_state = nullptr;
         p->capturable = false;
@@ -1561,8 +1645,14 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
     fin.view(p->step_state + off_fin, fl.total + kZeroPageBytes);
     rc = run_scan(ctx, &p->q, plan, slot, slot.stream, p->step_state + off_table, tl, &p->captured, 0, nullptr, &scan);
     p->express = slot.express[0];
-    if (!rc) rc = finalize_enqueue(&p->q, plan, slot, slot.stream, p->step_state + off_table, tl, p->host_off, fin, p->fl, fin_launches, p->read_back,
-                                   scan.base + sl.off_zero);
+    if (!rc && partial) {
+        emit_plain_rows(&p->q, plan, slot.stream, p->step_state + off_table, p->step_state + off_fin, scan.base + sl.off_zero, kZeroPageBytes, h_dst);
+        fin_launches = kPlainRowsLaunches;
+        p->read_back = 0;  // sized by the rows present: the replay counts it
+    } else if (!rc) {
+        rc = finalize_enqueue(&p->q, plan, slot, slot.stream, p->step_state + off_table, tl, p->host_off, fin, p->fl, fin_launches, p->read_back,
+                              scan.base + sl.off_zero);
+    }
     cudaGraph_t graph = nullptr;
     e = cudaStreamEndCapture(slot.stream, &graph);
     if (!rc && e == cudaSuccess && graph) e = cudaGraphInstantiate(&p->exec, graph, 0);
@@ -1573,11 +1663,30 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p) {
         p->capturable = false;  // fall back to the uncaptured path for good
         return rc;
     }
-    p->captured.kernel_launches += fin_launches;  // finalize + select_rows (one fused launch for few groups)
+    p->captured.kernel_launches += fin_launches;  // finalize + select_rows (one fused launch for few groups), or the three row kernels
     p->captured.d2h_bytes += p->read_back;
-    p->zero_image_off = p->host_off + p->fl.out_bytes;
+    p->zero_image_off = partial ? p->host_off : p->host_off + p->fl.out_bytes;
+    p->partial_step = partial;
     p->held = plan.parts;
     p->held_gen = gen;
+    return 0;
+}
+
+// Makes p->exec the captured step of the form asked for (partial: map-phase rows), ready to replay: a step of the other form gives
+// way (one step per handle), and a step whose handles stopped naming its parts is captured again.  Returns a code (BYDB_ENOENT: a
+// handle names no part), or 0 with p->exec NULL when this execution takes the uncaptured path.
+int prepared_step(bydb_ctx *ctx, bydb_prepared *p, bool partial) {
+    if (p->exec && p->partial_step != partial) drop_step(p);
+    if (!p->exec) return prepared_capture(ctx, p, partial);
+    // the handles can only have changed their parts if one was registered or released since `held` was last compared
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
+    if (gen != p->held_gen) {
+        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
+        if (!p->exec) drop_step(p);  // the state is sized for the parts it was captured with
+        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
+        p->held_gen = gen;
+        if (!p->exec) return prepared_capture(ctx, p, partial);
+    }
     return 0;
 }
 
@@ -1821,6 +1930,73 @@ void push_partial(PartialRowsOwner &o, const PartialWords &w, bool is_float) {
     o.val_f64.push_back(is_float ? vf : 0.0);
     o.cnt_i64.push_back(is_float ? 0 : static_cast<int64_t>(w.cnt));
     o.cnt_f64.push_back(is_float ? cf : 0.0);
+}
+
+// the status the control word of a row image carries: the column types merged over the passes, the worst status with them
+int rows_status(const uint8_t *ctl, size_t F) {
+    const int64_t *ct = reinterpret_cast<const int64_t *>(ctl + 8);
+    uint32_t dev_err = 0;
+    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(ct[c] >> 8));
+    return table_status(dev_err);
+}
+// the rows a row image holds: its n_present, at most max_rows
+size_t rows_in(const uint8_t *ctl, size_t max_rows) { return std::min<size_t>(*reinterpret_cast<const uint32_t *>(ctl), max_rows); }
+
+// a row image read back to the host -- the control word, then the rows right behind it -- into *b, after its status; each row's
+// key value into *key_id when given (a keyed answer)
+int parse_rows(const uint8_t *img, const bydb_query *q, const Plan &plan, size_t max_rows, bydb_partial_rows *b, std::vector<int32_t> *key_id) {
+    const size_t F = plan.fcols.size(), A = q->n_aggs, row_bytes = keyed_row_bytes(A);
+    int rc = rows_status(img, F);
+    if (rc) return rc;
+    const int64_t *ct = reinterpret_cast<const int64_t *>(img + 8);
+    auto ro = std::make_unique<PartialRowsOwner>();
+    ro->is_float.resize(A);
+    for (size_t a = 0; a < A; ++a) ro->is_float[a] = (ct[plan.agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
+    const size_t n = rows_in(img, max_rows);
+    const uint8_t *rows = img + keyed_ctl_bytes(F);
+    ro->group_id.resize(n);
+    if (key_id) key_id->resize(n);
+    for (size_t j = 0; j < n; ++j) {
+        const uint8_t *row = rows + j * row_bytes;
+        memcpy(&ro->group_id[j], row, 4);
+        if (key_id) memcpy(&(*key_id)[j], row + 4, 4);
+        for (size_t a = 0; a < A; ++a) {
+            PartialWords w;
+            memcpy(&w.val, row + 8 + 8 * a, 8);
+            memcpy(&w.cnt, row + 8 + 8 * (A + a), 8);
+            push_partial(*ro, w, ro->is_float[a] != 0);
+        }
+    }
+    b->n_rows = static_cast<int32_t>(n);
+    b->n_aggs = static_cast<int32_t>(A);
+    b->group_id = ro->group_id.data();
+    b->is_float = ro->is_float.data();
+    b->val_i64 = ro->val_i64.data();
+    b->val_f64 = ro->val_f64.data();
+    b->cnt_i64 = ro->cnt_i64.data();
+    b->cnt_f64 = ro->cnt_f64.data();
+    b->owner = ro.release();
+    return 0;
+}
+
+// bydb_partials_rows over the table at d_table, enqueued on `s`: emit_plain_rows into the slot's staging, synchronised and parsed.
+// stats (when given) count its three kernels and the bytes its copy kernel brought back.
+int partial_rows_to_host(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t s, const uint8_t *d_table, bydb_partial_rows *out,
+                         bydb_stats *stats) {
+    const size_t ctl_bytes = keyed_ctl_bytes(plan.fcols.size()), row_bytes = keyed_row_bytes(q->n_aggs);
+    if (slot.ensure_pinned(ctl_bytes + plan.tl.G * row_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    uint8_t *h_dst = slot.pinned_dev(0);
+    if (!h_dst) return fail(BYDB_EIO, "page-locked staging without a device address");
+    Scratch work;
+    CUDA_TRY(work.alloc(rows_layout(q, plan).total, s));
+    emit_plain_rows(q, plan, s, d_table, work.base, nullptr, 0, h_dst);
+    CUDA_TRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaGetLastError());
+    if (stats) {
+        stats->kernel_launches += kPlainRowsLaunches;
+        stats->d2h_bytes += ctl_bytes + rows_in(slot.pinned, plan.tl.G) * row_bytes;
+    }
+    return parse_rows(slot.pinned, q, plan, plan.tl.G, out, nullptr);
 }
 
 // the two answers of a keyed call: finalised rows (bydb_keyed_result) or map-phase partial rows (bydb_keyed_partial_rows)
@@ -2069,70 +2245,25 @@ int keyed_rows(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, 
     KeyOrderParams ko;
     int rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, out->stats);
     if (rc) return rc;
-    Carve carve;
-    const size_t i_ctl = carve(ctl_bytes), i_rows = carve(GP * row_bytes);
-    CUDA_TRY(img.alloc(carve.o, stream));
-    KeyedRowsParams kp;
-    memset(&kp, 0, sizeof kp);
-    kp.table = tlc.at(table);
-    kp.perm = ko.perm;
-    kp.n_present = ko.n_present;
-    kp.pass_coltype = coltype;
-    kp.n_groups = static_cast<uint32_t>(G);
-    kp.n_fcols = static_cast<uint32_t>(F);
-    kp.n_aggs = static_cast<uint32_t>(A);
-    kp.n_passes = static_cast<uint32_t>(V);
-    for (size_t a = 0; a < A; ++a) {
-        kp.agg_fcol[a] = plan.agg_fcol[a];
-        kp.agg_func[a] = q->aggs[a].func;
-    }
-    kp.ctl = reinterpret_cast<uint32_t *>(img.base + i_ctl);
-    kp.rows = img.base + i_rows;
-    launch_keyed_partial_rows(kp, GP, stream);
+    CUDA_TRY(img.alloc(ctl_bytes + GP * row_bytes, stream));
+    launch_keyed_partial_rows(rows_params(q, plan, V, tlc.at(table), coltype, ko.perm, ko.n_present, img.base), GP, stream);
     out->stats.kernel_launches += 1;
     // 1. the control word (behind the staging copy that reads slot.pinned, on the same stream)
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base + i_ctl, ctl_bytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base, ctl_bytes, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     CUDA_TRY(cudaGetLastError());
     out->stats.d2h_bytes += ctl_bytes;
-    const int64_t *ct = reinterpret_cast<const int64_t *>(slot.pinned + 8);
-    uint32_t dev_err = 0;
-    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(ct[c] >> 8));
-    rc = table_status(dev_err);
+    rc = rows_status(slot.pinned, F);
     if (rc) return rc;
-    auto ro = std::make_unique<PartialRowsOwner>();
-    ro->is_float.resize(A);
-    for (size_t a = 0; a < A; ++a) ro->is_float[a] = (ct[plan.agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
-    const size_t n = std::min<size_t>(*reinterpret_cast<const uint32_t *>(slot.pinned), GP);
-    // 2. the rows
+    const size_t n = rows_in(slot.pinned, GP);
+    // 2. the rows, right behind the control word
     if (n) {
-        CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base + i_rows, n * row_bytes, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaMemcpyAsync(slot.pinned + ctl_bytes, img.base + ctl_bytes, n * row_bytes, cudaMemcpyDeviceToHost, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
         out->stats.d2h_bytes += n * row_bytes;
     }
-    ro->group_id.resize(n);
-    owner->key_id.resize(n);
-    for (size_t j = 0; j < n; ++j) {
-        const uint8_t *row = slot.pinned + j * row_bytes;
-        memcpy(&ro->group_id[j], row, 4);
-        memcpy(&owner->key_id[j], row + 4, 4);
-        for (size_t a = 0; a < A; ++a) {
-            PartialWords w;
-            memcpy(&w.val, row + 8 + 8 * a, 8);
-            memcpy(&w.cnt, row + 8 + 8 * (A + a), 8);
-            push_partial(*ro, w, ro->is_float[a] != 0);
-        }
-    }
-    bydb_partial_rows &b = out->base;
-    b.n_rows = static_cast<int32_t>(n);
-    b.n_aggs = static_cast<int32_t>(A);
-    b.group_id = ro->group_id.data();
-    b.is_float = ro->is_float.data();
-    b.val_i64 = ro->val_i64.data();
-    b.val_f64 = ro->val_f64.data();
-    b.cnt_i64 = ro->cnt_i64.data();
-    b.cnt_f64 = ro->cnt_f64.data();
-    b.owner = ro.release();
+    rc = parse_rows(slot.pinned, q, plan, GP, &out->base, &owner->key_id);
+    if (rc) return rc;
     out->key_id = owner->key_id.data();
     return 0;
 }
@@ -2142,8 +2273,7 @@ size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, cons
     return step_pinned_bytes(q, static_cast<size_t>(plan.n_groups), GP);
 }
 size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_partial_rows *) {
-    return std::max(stage_layout(q->n_series, static_cast<size_t>(plan.n_groups)).stride,
-                    std::max(keyed_ctl_bytes(plan.fcols.size()), GP * keyed_row_bytes(q->n_aggs)));
+    return std::max(stage_layout(q->n_series, static_cast<size_t>(plan.n_groups)).stride, keyed_ctl_bytes(plan.fcols.size()) + GP * keyed_row_bytes(q->n_aggs));
 }
 
 int keyed_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
@@ -2276,9 +2406,12 @@ namespace {
 //   composite table | permuted table | the passes' column types | Kts | Krow | the order's slots, first_series, perm, n_present |
 //   one scan scratch (scan_layout, the passes run one after another) | finalisation over V x G groups, then the rows' (group, key)
 //   pairs and the V zero pages, so that one copy reads back the rows, their pairs and the passes' counters and errors.
+// `partial` (bydb_scan_partials_keyed_prepared) selects the other tail: no permuted table and no finalisation; behind the order,
+// keyed_partial_rows_kernel writes the row image (control word, rows) right behind the V zero pages, and rows_to_host_kernel
+// brings the pages, the control word and exactly the present rows to the staging.
 // Leaves neither a graph nor no_values when this execution, or (capturable cleared) every later one, takes the plain path: a part
 // is missing, the parts overlap, discovery fails (its refusal is the plain call's), or the state or the capture cannot be had.
-void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k) {
+void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     bydb_prepared *p = k->pq;
     const bydb_query *q = &p->q;
     const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up
@@ -2309,19 +2442,22 @@ void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k) {
     const ScanLayout sl = scan_layout(st, plan.total_blocks, F, plan.parts.size(), true);
     const FinalLayout fl = final_layout(GP, q->n_aggs, q->top_n);
     const size_t b_pairs = align_up(fl.cap * 8, 256), b_zero = V * kZeroPageBytes;
+    const size_t b_rows = keyed_ctl_bytes(F) + GP * keyed_row_bytes(q->n_aggs);  // partial: the row image
     Carve carve;
-    const size_t o_src = carve(tlc.total), o_dst = carve(tlc.total), o_ct = carve(V * F * 8), o_kts = carve(V * NS * 8), o_krow = carve(V * NS * 4),
-                 o_slot = carve(NS * V * 4), o_first = carve(GP * 4), o_perm = carve(GP * 4), o_np = carve(16), o_scan = carve(sl.total),
-                 o_fin = carve(fl.total + b_pairs + b_zero);
+    const size_t o_src = carve(tlc.total), o_dst = carve(partial ? 0 : tlc.total), o_ct = carve(V * F * 8), o_kts = carve(V * NS * 8),
+                 o_krow = carve(V * NS * 4), o_slot = carve(NS * V * 4), o_first = carve(GP * 4), o_perm = carve(GP * 4), o_np = carve(16),
+                 o_scan = carve(sl.total), o_fin = carve(partial ? b_zero + b_rows : fl.total + b_pairs + b_zero);
     p->host_off = st.stride;  // the read-back lands behind the staging area, as in the plain prepared step
-    p->read_back = fl.out_bytes + b_pairs + b_zero;
-    if (slot.ensure_pinned(p->host_off + p->read_back) || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
+    p->read_back = partial ? b_zero + b_rows : fl.out_bytes + b_pairs + b_zero;  // partial: the most the copy kernel may write
+    // sized before the capture: the graph writes the staging through its device address
+    uint8_t *h_dst = slot.ensure_pinned(p->host_off + p->read_back) ? nullptr : slot.pinned_dev(p->host_off);
+    if (!h_dst || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
         cudaGetLastError();
         p->step_state = nullptr;
         p->capturable = false;
         return;
     }
-    uint8_t *S = p->step_state, *fin_base = S + o_fin, *zero_pages = fin_base + fl.total + b_pairs;
+    uint8_t *S = p->step_state, *fin_base = S + o_fin, *zero_pages = partial ? fin_base : fin_base + fl.total + b_pairs;
     // the staging goes up once: the passes and the order read it from the step state on every replay
     stage_series(q, st, slot.pinned);
     cudaError_t e = cudaMemcpyAsync(S + o_scan + sl.off_sids, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream);
@@ -2365,17 +2501,29 @@ void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k) {
     FinalLayout flc;
     uint32_t fin_launches = 0;
     size_t fin_back = 0;
-    if (!rc) {
+    if (!rc && partial) {
+        launch_keyed_partial_rows(rows_params(q, plan, V, tlc.at(S + o_src), ct, ko.perm, ko.n_present, zero_pages + b_zero), GP, stream);
+        RowsCopyParams cp;
+        memset(&cp, 0, sizeof cp);
+        cp.pages = zero_pages;
+        cp.image = zero_pages + b_zero;
+        cp.dst = h_dst;
+        cp.page_bytes = b_zero;
+        cp.ctl_bytes = keyed_ctl_bytes(F);
+        cp.row_bytes = keyed_row_bytes(q->n_aggs);
+        cp.max_rows = static_cast<uint32_t>(GP);
+        launch_rows_to_host(cp, stream);
+    } else if (!rc) {
         launch_permute_table(tlc.at(S + o_dst), tlc.at(S + o_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), ct,
                              static_cast<uint32_t>(V), stream);
         Plan planc = plan;
         planc.n_groups = static_cast<int32_t>(GP);
         rc = finalize_launch(q, planc, stream, S + o_dst, tlc, fin, flc, fin_launches, fin_back);
-    }
-    if (!rc) {
-        launch_keyed_row_map(reinterpret_cast<const int32_t *>(fin_base + fl.o_sg), reinterpret_cast<const uint32_t *>(fin_base + fl.o_cnt), ko.perm,
-                             static_cast<uint32_t>(G), static_cast<uint32_t>(fl.cap), reinterpret_cast<int32_t *>(fin_base + fl.total), stream);
-        if (cudaMemcpyAsync(slot.pinned + p->host_off, fin_base + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+        if (!rc) {
+            launch_keyed_row_map(reinterpret_cast<const int32_t *>(fin_base + fl.o_sg), reinterpret_cast<const uint32_t *>(fin_base + fl.o_cnt),
+                                 ko.perm, static_cast<uint32_t>(G), static_cast<uint32_t>(fl.cap), reinterpret_cast<int32_t *>(fin_base + fl.total), stream);
+            if (cudaMemcpyAsync(slot.pinned + p->host_off, fin_base + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+        }
     }
     cudaGraph_t graph = nullptr;
     e = cudaStreamEndCapture(stream, &graph);
@@ -2387,39 +2535,102 @@ void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k) {
         p->capturable = false;
         return;
     }
-    cs.kernel_launches += 1 + fin_launches + 1;  // permute_table, finalisation + row selection, the row mapping
-    cs.d2h_bytes = p->read_back;
+    // permute_table, finalisation + row selection, the row mapping; or the row kernel and the copy kernel.  A partial step's read-back
+    // is sized by the rows present: the replay counts it.
+    cs.kernel_launches += partial ? 2 : 1 + fin_launches + 1;
+    cs.d2h_bytes = partial ? 0 : p->read_back;
+    p->partial_step = partial;
     p->fl = fl;
     p->express = false;  // the key predicate keeps every pass off the express lane
     k->values = std::move(values);
     k->no_values = false;
     k->pairs_off = fl.out_bytes;
-    k->zero_off = fl.out_bytes + b_pairs;
+    k->zero_off = partial ? 0 : fl.out_bytes + b_pairs;
     p->held = plan.parts;
     p->held_gen = gen;
 }
 
+// the answer of a replayed keyed step from its read-back `image`, after the passes' zero pages: the finalised rows and their
+// (group, key) pairs, or the row image (table status, rows, their key values) and the bytes the copy kernel brought back
+int keyed_answer(bydb_prepared_keyed *k, const Plan &, const uint8_t *image, bydb_keyed_result *out, KeyedOwner *owner) {
+    const int rc = finalize_parse(image, k->pq->fl, true, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, reinterpret_cast<const int32_t *>(image + k->pairs_off));
+    return 0;
+}
+int keyed_answer(bydb_prepared_keyed *k, const Plan &shape, const uint8_t *image, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    const size_t V = k->values.size(), GP = V * shape.tl.G, A = k->pq->q.n_aggs;
+    const uint8_t *rows = image + V * kZeroPageBytes;
+    out->stats.d2h_bytes += V * kZeroPageBytes + keyed_ctl_bytes(shape.fcols.size()) + rows_in(rows, GP) * keyed_row_bytes(A);
+    const int rc = parse_rows(rows, &k->pq->q, shape, GP, &out->base, &owner->key_id);
+    if (rc) return rc;
+    out->key_id = owner->key_id.data();
+    return 0;
+}
+
 // One replay, synchronised and parsed: the passes' counters add up and the first pass with a device error decides, as the plain
-// path's pass-by-pass collection has it; then the table's carried status, the rows and their (group, key) pairs.
-int keyed_replay(bydb_ctx *ctx, bydb_prepared_keyed *k, bydb_keyed_result *out) {
+// path's pass-by-pass collection has it; then the answer of the step's form (keyed_answer).
+template <class Out>
+int keyed_replay(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
     bydb_prepared *p = k->pq;
+    Plan shape;
+    int rc = query_shape(&p->q, shape);
+    if (rc) return rc;
     uint8_t *image = p->slot->pinned + p->host_off;
     const size_t V = k->values.size();
-    memset(image + k->zero_off, 0, V * kZeroPageBytes);  // a replay that fails to launch cannot report the previous one's status
+    // a replay that fails to launch cannot report the previous one's status (nor, in a partial step, its control word)
+    memset(image + k->zero_off, 0, V * kZeroPageBytes + (p->partial_step ? keyed_ctl_bytes(shape.fcols.size()) : 0));
     auto page = [&](size_t v) -> const ZeroPage & { return *reinterpret_cast<const ZeroPage *>(image + k->zero_off + v * kZeroPageBytes); };
-    bydb_stats &stats = out->base.stats;
-    int rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, false, page(0), &stats);
+    bydb_stats &stats = keyed_stats(out);
+    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, false, page(0), &stats);
     for (size_t v = 1; !rc && v < V; ++v) rc = read_zero_page(page(v), false, &stats);
     if (rc) return rc;
     auto owner = new KeyedOwner();
     out->owner = owner;
-    KeyedUndo<bydb_keyed_result> undo{ctx, out};
+    KeyedUndo<Out> undo{ctx, out};
     set_key_table(out, owner, k->values);
-    rc = finalize_parse(image, p->fl, true, &out->base);
+    rc = keyed_answer(k, shape, image, out, owner);
     if (rc) return rc;
-    set_row_keys(out, owner, reinterpret_cast<const int32_t *>(image + k->pairs_off));
     undo.done = true;
     return 0;
+}
+
+// bydb_scan_agg_keyed_prepared and bydb_scan_partials_keyed_prepared: one captured step per handle, of the form last asked for
+template <class Out>
+int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
+    if (!ctx || !k || !out) return fail(BYDB_EINVAL, "NULL argument");
+    memset(out, 0, sizeof *out);
+    const bool partial = std::is_same<Out, bydb_keyed_partial_rows>::value;
+    bydb_prepared *p = k->pq;
+    std::lock_guard<std::mutex> lk(p->mu);
+    g_last_dev_err = 0;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    auto plain = [&] { return scan_keyed_impl(ctx, &p->q, &k->key, out); };
+    // as bydb_scan_agg_prepared: the first execution runs the plain keyed path, the second one captures, later ones replay
+    if (p->runs++ == 0 || !p->capturable) return plain();
+    // the handles can only have changed their parts if one was registered or released since `held` was last compared
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
+    if ((p->exec || k->no_values) && gen != p->held_gen) {
+        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
+        if (p->held.empty()) {  // a handle stopped naming its captured part: discovery and the capture run again
+            drop_step(p);
+            k->no_values = false;
+        }
+        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
+        p->held_gen = gen;
+    }
+    if (p->exec && p->partial_step != partial) drop_step(p);  // one step per handle: the other form's gives way
+    if (!p->exec && !k->no_values) {
+        keyed_capture(ctx, k, partial);
+        if (!p->exec && !k->no_values) return plain();
+    }
+    if (k->no_values) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
+        auto owner = new KeyedOwner();
+        out->owner = owner;
+        set_key_table(out, owner, KeyValues());
+        return 0;
+    }
+    return keyed_replay(ctx, k, out);
 }
 }  // namespace
 }  // extern "C++"
@@ -2454,39 +2665,11 @@ void bydb_query_release_keyed(bydb_ctx *ctx, bydb_prepared_keyed *k) {
 }
 
 int bydb_scan_agg_keyed_prepared(bydb_ctx *ctx, bydb_prepared_keyed *k, bydb_keyed_result *out) {
-    return guarded([&]() -> int {
-    if (!ctx || !k || !out) return fail(BYDB_EINVAL, "NULL argument");
-    memset(out, 0, sizeof *out);
-    bydb_prepared *p = k->pq;
-    std::lock_guard<std::mutex> lk(p->mu);
-    g_last_dev_err = 0;
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    auto plain = [&] { return scan_keyed_impl(ctx, &p->q, &k->key, out); };
-    // as bydb_scan_agg_prepared: the first execution runs the plain keyed path, the second one captures, later ones replay
-    if (p->runs++ == 0 || !p->capturable) return plain();
-    // the handles can only have changed their parts if one was registered or released since `held` was last compared
-    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
-    if ((p->exec || k->no_values) && gen != p->held_gen) {
-        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
-        if (p->held.empty()) {  // a handle stopped naming its captured part: discovery and the capture run again
-            drop_step(p);
-            k->no_values = false;
-        }
-        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
-        p->held_gen = gen;
-    }
-    if (!p->exec && !k->no_values) {
-        keyed_capture(ctx, k);
-        if (!p->exec && !k->no_values) return plain();
-    }
-    if (k->no_values) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
-        auto owner = new KeyedOwner();
-        out->owner = owner;
-        set_key_table(out, owner, KeyValues());
-        return 0;
-    }
-    return keyed_replay(ctx, k, out);
-    });
+    return guarded([&]() -> int { return keyed_prepared_impl(ctx, k, out); });
+}
+
+int bydb_scan_partials_keyed_prepared(bydb_ctx *ctx, bydb_prepared_keyed *k, bydb_keyed_partial_rows *out) {
+    return guarded([&]() -> int { return keyed_prepared_impl(ctx, k, out); });
 }
 
 
@@ -3066,7 +3249,8 @@ int bydb_query_prepare(bydb_ctx *ctx, const bydb_query *q, bydb_prepared **out) 
         // a query with too many fields is refused at its first execution, like bydb_scan_agg would
         Plan shape;
         (void)query_shape(q, shape);
-        ok = p->slot->ensure_pinned(step_pinned_bytes(q, shape.tl.G, shape.tl.G)) == 0;
+        // and for its partial form (bydb_scan_partials_prepared), so that no capture of either form grows the staging under a graph
+        ok = p->slot->ensure_pinned(std::max(step_pinned_bytes(q, shape.tl.G, shape.tl.G), partial_pinned_bytes(q, shape))) == 0;
     }
     ok = ok && cudaEventCreate(&p->t0) == cudaSuccess && cudaEventCreate(&p->t1) == cudaSuccess;
     if (!ok) {
@@ -3094,29 +3278,71 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
     // captures; from then on the graph is replayed
     const uint64_t run = p->runs++;
     if (run == 0 || !p->capturable) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
-    if (!p->exec) {
-        const int rc = prepared_capture(ctx, p);
-        if (rc) return rc;
-        if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
-    }
-    // the handles can only have changed their parts if one was registered or released since `held` was last compared
-    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
-    if (gen != p->held_gen) {
-        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
-        if (!p->exec) drop_step(p);  // the state is sized for the parts it was captured with
-        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
-        p->held_gen = gen;
-        if (!p->exec) {
-            const int rc = prepared_capture(ctx, p);
-            if (rc) return rc;
-            if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
-        }
-    }
+    int rc = prepared_step(ctx, p, false);
+    if (rc) return rc;
+    if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
     uint8_t *image = p->slot->pinned + p->zero_image_off;
     memset(image, 0, kZeroPageBytes);
-    const int rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, *reinterpret_cast<const ZeroPage *>(image), &out->stats);
+    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, *reinterpret_cast<const ZeroPage *>(image), &out->stats);
     if (rc) return rc;
     return finalize_parse(p->slot->pinned + p->host_off, p->fl, false, out);
+    });
+}
+
+namespace {
+// bydb_scan_partials with stats into a table of its own, then bydb_partials_rows over it, on one slot: the scan's device error
+// first, then the status the table carries
+int scan_partials_rows_impl(bydb_ctx *ctx, const bydb_query *q, bydb_partial_rows *out, bydb_stats *stats) {
+    Plan plan;
+    int rc = make_plan(ctx, q, nullptr, plan);
+    if (rc) return rc;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    SlotLease lease(ctx);
+    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
+    ExecSlot &slot = *lease.slot;
+    Scratch table;
+    CUDA_TRY(table.alloc(plan.tl.total, slot.stream));
+    bydb_stats local;
+    memset(&local, 0, sizeof local);
+    rc = run_scan(ctx, q, plan, slot, slot.stream, table.base, plan.tl, &local);
+    cudaError_t ce = cudaStreamSynchronize(slot.stream);  // also on failure: nothing may be in flight when the slot goes back
+    if (!rc && ce != cudaSuccess) rc = fail(BYDB_EIO, cudaGetErrorString(ce));
+    if (!rc) rc = collect_scan(slot, &local);
+    if (!rc) rc = partial_rows_to_host(q, plan, slot, slot.stream, table.base, out, &local);
+    if (stats) *stats = local;
+    return rc;
+}
+}  // namespace
+
+int bydb_scan_partials_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_partial_rows *out, bydb_stats *stats) {
+    return guarded([&]() -> int {
+    if (!ctx || !p || !out) return fail(BYDB_EINVAL, "NULL argument");
+    memset(out, 0, sizeof *out);
+    if (stats) memset(stats, 0, sizeof *stats);
+    std::lock_guard<std::mutex> lk(p->mu);
+    g_last_dev_err = 0;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    // the schedule of bydb_scan_agg_prepared: the uncaptured path, then the capture, then replays
+    const uint64_t run = p->runs++;
+    if (run == 0 || !p->capturable) return scan_partials_rows_impl(ctx, &p->q, out, stats);
+    int rc = prepared_step(ctx, p, true);
+    if (rc) return rc;
+    if (!p->exec) return scan_partials_rows_impl(ctx, &p->q, out, stats);
+    Plan shape;
+    rc = query_shape(&p->q, shape);
+    if (rc) return rc;
+    const size_t ctl_bytes = keyed_ctl_bytes(shape.fcols.size());
+    uint8_t *image = p->slot->pinned + p->host_off;  // the zero page, then the row image (control word, rows)
+    memset(image, 0, kZeroPageBytes + ctl_bytes);  // a replay that fails to launch cannot report the previous one's status or rows
+    bydb_stats local{};
+    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, *reinterpret_cast<const ZeroPage *>(image), &local);
+    const uint8_t *rows = image + kZeroPageBytes;
+    if (!rc) {
+        local.d2h_bytes += kZeroPageBytes + ctl_bytes + rows_in(rows, shape.tl.G) * keyed_row_bytes(p->q.n_aggs);
+        rc = parse_rows(rows, &p->q, shape, shape.tl.G, out, nullptr);
+    }
+    if (stats) *stats = local;
+    return rc;
     });
 }
 
@@ -3130,40 +3356,12 @@ int bydb_partials_rows(bydb_ctx *ctx, const bydb_query *q, const void *d_partial
     Plan plan;
     rc = query_shape(q, plan);
     if (rc) return rc;
-    const TableLayout &tl = plan.tl;
-    const std::vector<int> &agg_fcol = plan.agg_fcol;
-    const size_t G = tl.G, F = tl.F, A = q->n_aggs;
-    if (bytes < tl.total) return fail(BYDB_EINVAL, "partial table buffer too small");
+    if (bytes < plan.tl.total) return fail(BYDB_EINVAL, "partial table buffer too small");
     CUDA_TRY(cudaSetDevice(ctx->device));
-    std::vector<uint8_t> h(tl.total);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(cudaMemcpyAsync(h.data(), d_partials, tl.total, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    const TablePtrs t = tl.at(h.data());
-    uint32_t dev_err = 0;
-    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(t.coltype[c] >> 8));
-    rc = table_status(dev_err);
-    if (rc) return rc;
-    auto owner = std::make_unique<PartialRowsOwner>();
-    owner->is_float.resize(A);
-    for (size_t a = 0; a < A; ++a) owner->is_float[a] = (t.coltype[agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
-    for (size_t g = 0; g < G; ++g) {
-        if (t.rows[g] <= 0) continue;  // the group never appeared on this node
-        owner->group_id.push_back(static_cast<int32_t>(g));
-        for (size_t a = 0; a < A; ++a)
-            push_partial(*owner, partial_words(t, g * F + static_cast<size_t>(agg_fcol[a]), q->aggs[a].func, owner->is_float[a] != 0),
-                         owner->is_float[a] != 0);
-    }
-    out->n_rows = static_cast<int32_t>(owner->group_id.size());
-    out->n_aggs = static_cast<int32_t>(A);
-    out->group_id = owner->group_id.data();
-    out->is_float = owner->is_float.data();
-    out->val_i64 = owner->val_i64.data();
-    out->val_f64 = owner->val_f64.data();
-    out->cnt_i64 = owner->cnt_i64.data();
-    out->cnt_f64 = owner->cnt_f64.data();
-    out->owner = owner.release();
-    return 0;
+    SlotLease lease(ctx);
+    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
+    // the rows are built on the device: only the present groups' rows cross PCIe, not the table
+    return partial_rows_to_host(q, plan, *lease.slot, static_cast<cudaStream_t>(stream), static_cast<const uint8_t *>(d_partials), out, nullptr);
     });
 }
 

@@ -4068,6 +4068,47 @@ void launch_keyed_partial_rows(const KeyedRowsParams &p, size_t max_rows, cudaSt
     keyed_partial_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(p);
 }
 
+// one CTA: ordered compaction of the groups that appeared (rows > 0), chunk by chunk, so that any G comes out in group-id order
+__global__ void __launch_bounds__(1024) present_groups_kernel(const int64_t *__restrict__ rows, uint32_t n_groups, int32_t *__restrict__ perm,
+                                                              uint32_t *__restrict__ n_present) {
+    __shared__ uint32_t warp_tot[32];
+    uint32_t base = 0;
+    for (uint32_t g0 = 0; g0 < n_groups; g0 += 1024) {
+        const uint32_t g = g0 + threadIdx.x;
+        const uint32_t f = g < n_groups && rows[g] > 0 ? 1u : 0u;
+        uint32_t total = 0;
+        const uint32_t pos = block_excl_scan(f, warp_tot, total);
+        if (f) perm[base + pos] = static_cast<int32_t>(g);
+        base += total;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *n_present = base;
+}
+
+void launch_present_groups(const int64_t *rows, uint32_t n_groups, int32_t *perm, uint32_t *n_present, cudaStream_t s) {
+    present_groups_kernel<<<1, 1024, 0, s>>>(rows, n_groups, perm, n_present);
+}
+
+// the graph's last node: the zero pages, the control word and the present rows into the host staging (see RowsCopyParams)
+__global__ void rows_to_host_kernel(const RowsCopyParams p) {
+    const uint32_t n = min(*reinterpret_cast<const uint32_t *>(p.image), p.max_rows);
+    const size_t rest = p.ctl_bytes + static_cast<size_t>(n) * p.row_bytes;
+    const size_t v_pages = p.page_bytes / 16, v_all = v_pages + rest / 16;
+    const size_t i0 = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x, stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+    uint4 *dst = reinterpret_cast<uint4 *>(p.dst);
+    for (size_t i = i0; i < v_all; i += stride)
+        dst[i] = i < v_pages ? reinterpret_cast<const uint4 *>(p.pages)[i] : reinterpret_cast<const uint4 *>(p.image)[i - v_pages];
+    if (i0 == 0 && (rest & 15))
+        reinterpret_cast<uint2 *>(p.dst + p.page_bytes)[rest / 8 - 1] = reinterpret_cast<const uint2 *>(p.image)[rest / 8 - 1];
+}
+
+void launch_rows_to_host(const RowsCopyParams &p, cudaStream_t s) {
+    const size_t most = (p.page_bytes + p.ctl_bytes + static_cast<size_t>(p.max_rows) * p.row_bytes + 15) / 16;
+    const size_t want = (most + 255) / 256;
+    const unsigned blocks = want < 1 ? 1u : want > 1024 ? 1024u : static_cast<unsigned>(want);
+    rows_to_host_kernel<<<blocks, 256, 0, s>>>(p);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Keyed collective (bydb_scan_reduce_keyed): every rank ran discovery and its per-value passes into its slot of the root's
 // mailbox (layout: KeyedSlot).  The ranks' value lists differ, so their V_r x G composite tables do not line up slot for slot.
@@ -4489,6 +4530,8 @@ void preload_kernels() {
     (void)cudaFuncGetAttributes(&ka, key_perm_kernel);
     (void)cudaFuncGetAttributes(&ka, permute_table_kernel);
     (void)cudaFuncGetAttributes(&ka, keyed_partial_rows_kernel);
+    (void)cudaFuncGetAttributes(&ka, present_groups_kernel);
+    (void)cudaFuncGetAttributes(&ka, rows_to_host_kernel);
     (void)cudaFuncGetAttributes(&ka, key_union_kernel);
     (void)cudaFuncGetAttributes(&ka, rank_span_check_kernel);
     (void)cudaFuncGetAttributes(&ka, combine_keyed_kernel);

@@ -335,6 +335,23 @@ struct KeyedRowsParams {
 };
 // grid over max_rows (= V * G) rows; the threads of rows at or above *n_present leave at once
 void launch_keyed_partial_rows(const KeyedRowsParams &p, size_t max_rows, cudaStream_t s);
+// ---- map-phase rows of a plain table (bydb_partials_rows and the prepared partial forms) run keyed_partial_rows_kernel with one
+// pass over the table itself; in front of it, one CTA compacts the groups with rows[g] > 0 in group-id order (stable): perm[j] is
+// the j-th present group, *n_present their number -- the shape key_perm_kernel gives (the absent groups are not listed).
+void launch_present_groups(const int64_t *rows, uint32_t n_groups, int32_t *perm, uint32_t *n_present, cudaStream_t s);
+// The rows of a map-phase answer to page-locked host memory, from inside a graph (a copy node cannot take its size from the
+// device): `dst` is the DEVICE address of the staging (cudaHostGetDevicePointer), 16-byte aligned, and receives the page_bytes of
+// `pages` (the passes' zero pages, a multiple of 16), then the control word and exactly min(n_present, max_rows) rows of `image`
+// (n_present = its first word).  16-byte loads and stores; the rows end on an 8-byte word when ctl_bytes + n * row_bytes is
+// not a multiple of 16, and that word goes with one 8-byte store.  Nothing beyond those bytes is written.
+struct RowsCopyParams {
+    const uint8_t *pages;         // 256-byte aligned
+    const uint8_t *image;         // 256-byte aligned: control word (keyed_ctl_bytes), then the rows (keyed_row_bytes each)
+    uint8_t *dst;
+    size_t page_bytes, ctl_bytes, row_bytes;
+    uint32_t max_rows, pad;
+};
+void launch_rows_to_host(const RowsCopyParams &p, cudaStream_t s);
 // ---- keyed collective (bydb_scan_reduce_keyed): the slot of a rank that found V key values, in the root's mailbox, for G groups,
 // F fields and NS series.  Every region is sized by V, so a rank's need grows with the values it found; the root derives each
 // rank's layout from the V_r in its header.
