@@ -411,6 +411,41 @@ typedef struct {
 int bydb_scan_partials_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out);
 void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r);
 
+/* Group-by on a stored tag in ONE scan pass, for up to 65,536 key values (bydb_scan_agg_keyed runs one pass per value).
+ *   - Answer: that of bydb_scan_agg_keyed / bydb_scan_partials_keyed, with the same definitions: a composite group is (series
+ *     group, key value); rows are the composite groups with rows > 0 in insertion order (series by series in ascending id, then
+ *     by time; a group is inserted at its first row that survives the time range and the predicates); with Top-N, rank order,
+ *     ties to the group inserted first.  A nil cell and "" are one string key; for an int64 key a nil cell and a block without
+ *     the column are the key 0.  MEAN quirks, output typing, BYDB_Q_ROW_PATH_TYPES, met-column and the empty-fold sentinels as
+ *     there.  The partial form follows partial_words' wire rule and ignores top_n.  n_keys counts the distinct values of the
+ *     selected blocks before the time trim and the predicates; the key table holds all of them, in no promised order.
+ *   - Caps and refusals: max_values 0 means 64, 1..65,536 are accepted, above gives BYDB_EINVAL; more distinct values than
+ *     max_values gives BYDB_ENOMEM.  A string key must be a dictionary page (a plain page, or a value longer than 64 bytes:
+ *     BYDB_ENOTSUP).  An int64 key takes every page kind bydb_scan_agg_keyed takes; a block whose key column holds more than 256
+ *     distinct values gives BYDB_ENOTSUP, the message naming the block.  A key of the wrong type gives BYDB_EINVAL, parts that
+ *     overlap in time BYDB_ENOTSUP.  Up to 8 predicates (the key takes no predicate slot); block size and Top-N as bydb_scan_agg.
+ *   - Numbers: counts, int64 values and min / max bit-exact; float sums within 1e-9 relative of the reference and bit-identical
+ *     from call to call (the records of a group are folded in scan order by a fixed tree), though not necessarily bit-identical
+ *     with bydb_scan_agg_keyed, whose passes fold zero partials for the blocks without the value.
+ *   - Stats (one pass): rows_scanned, blocks_scanned and rows_matched are what bydb_scan_agg reports for the same query without
+ *     the key; page_bytes counts every page read once (the key page included).  With cap = max_values, V key values found,
+ *     R = sum over the selected blocks of the block's distinct key values, C the composite groups with rows > 0, F distinct
+ *     fields, A aggregations, NS series, NB blocks of the parts, pow2(x) the least power of two >= x:
+ *       d2h_bytes = 32 + V * (64 + 4) (string key) or 32 + V * 8 (int64 key)    the discovery read-back (V = 0: 32 only)
+ *                 + 256 + 8                                                     the scan's status / counter page, C
+ *                 + the finalisation read-back of bydb_scan_agg over C groups   (bydb_scan_agg_keyed_wide)
+ *                   or 8 + 8 * F + C * (8 + 16 * A)                             (bydb_scan_partials_keyed_wide: control word, rows)
+ *                 + 8 * C                                                       each composite group's (series group, key value)
+ *     (C = 0: the first two terms only)
+ *     and the device scratch of one call is, up to 256-byte alignment of each region,
+ *       12 * NS + 12 * S + 68 * cap + 8 * NB   with S = pow2(max(2 * cap, 1024))                            discovery
+ *     + 256 + R * (16 + 32 * F) + 12 * pow2(max(2 * R, 1024)) + 8 * R + 12 * pow2(max(R, 2048))              scan and order
+ *     + 8 * (C * (7 * F + 1) + F) + 12 * C                                                                    the composite table
+ *     + the finalisation's scratch over C groups (or the row image, 8 + 8 * F + C * (8 + 16 * A)).
+ *     Nothing of size G * V is allocated. */
+int bydb_scan_agg_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out);
+int bydb_scan_partials_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out);
+
 /* Prepared map-phase answers: what a data node answers, refresh after refresh, for a query the liaison pushes down with
  * agg_return_partial (a dashboard panel or an alert rule in a cluster).  The handles are those of the finalised forms above.
  *   - Answers: every execution returns what the unprepared form returns at that moment, for the handle's query.

@@ -114,7 +114,8 @@ struct ScanSpec {
     int64_t TMin = INT64_MIN, TMax = INT64_MAX;
     std::vector<Pred> Preds;
     bool OrderDesc = false;
-    uint32_t MaxKeyValues = 0;  // distinct values of a stored-tag GroupBy key (bydb_group_key.max_values; 0 = the library's 64)
+    uint32_t MaxKeyValues = 0;  // distinct values of a stored-tag GroupBy key (bydb_group_key.max_values; 0 = the library's 64);
+                                // up to 256 bydb_scan_agg_keyed answers, up to 65,536 bydb_scan_agg_keyed_wide
 };
 
 struct Error {
@@ -346,7 +347,8 @@ class GPUScanAgg final : public PullOperator {
             key.tag = cd.Name.c_str();
             key.max_values = scan_.MaxKeyValues;
             key.value_type = cd.Type == ColumnType::ColumnTypeInt64 ? BYDB_VT_INT64 : 0;
-            rc = bydb_scan_agg_keyed(ctx_, &q, &key, &kres_);
+            // above the per-value passes' 256 values, the one-pass form (which answers the same rows)
+            rc = scan_.MaxKeyValues > 256 ? bydb_scan_agg_keyed_wide(ctx_, &q, &key, &kres_) : bydb_scan_agg_keyed(ctx_, &q, &key, &kres_);
         }
         if (rc != 0) return fail(rc, bydb_last_error() ? bydb_last_error() : "bydb_scan_agg failed");
         have_result_ = true;

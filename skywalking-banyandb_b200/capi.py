@@ -112,7 +112,7 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_scan_partials", "bydb_partials_combine", "bydb_reduce_finalize", "bydb_partials_rows", "bydb_partial_rows_free", "bydb_comm_export", "bydb_comm_connect",
            "bydb_scan_reduce", "bydb_scan_reduce_prepared", "bydb_scan_reduce_host", "bydb_scan_agg_keyed", "bydb_keyed_result_free",
            "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed", "bydb_scan_partials_keyed", "bydb_keyed_partial_rows_free",
-           "bydb_scan_reduce_keyed_partials",
+           "bydb_scan_reduce_keyed_partials", "bydb_scan_agg_keyed_wide", "bydb_scan_partials_keyed_wide",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -177,6 +177,8 @@ def load_library():
     L.bydb_scan_reduce_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32, C.POINTER(_KeyedResult)]
     L.bydb_scan_partials_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(_KeyedPartialRows)]
     L.bydb_scan_reduce_keyed_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32, C.POINTER(_KeyedPartialRows)]
+    L.bydb_scan_agg_keyed_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(_KeyedResult)]
+    L.bydb_scan_partials_keyed_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(_KeyedPartialRows)]
     L.bydb_keyed_partial_rows_free.argtypes = [C.c_void_p, C.POINTER(_KeyedPartialRows)]
     L.bydb_keyed_partial_rows_free.restype = None
     _lib = L
@@ -524,6 +526,15 @@ class Context:
         _check(self._L.bydb_scan_agg_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
         return self._read_keyed(q, r)
 
+    def scan_agg_keyed_wide(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> Result:
+        """scan_agg_keyed's answer in one scan pass, for up to 65,536 key values (bydb_scan_agg_keyed_wide)."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        r = _KeyedResult()
+        _check(self._L.bydb_scan_agg_keyed_wide(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
+        return self._read_keyed(q, r)
+
     def prepare_keyed(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> "KeyedGraphQuery":
         """The prepared form of scan_agg_keyed (bydb_query_prepare_keyed): argument errors are raised here, as scan_agg_keyed
         raises them; the handle's run() answers as scan_agg_keyed does at that moment."""
@@ -629,6 +640,15 @@ class Context:
         gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
         r = _KeyedPartialRows()
         _check(self._L.bydb_scan_partials_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
+        return self._read_keyed_partials(q, r)
+
+    def scan_partials_keyed_wide(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> Dict[str, object]:
+        """scan_partials_keyed's answer in one scan pass, for up to 65,536 key values (bydb_scan_partials_keyed_wide)."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        r = _KeyedPartialRows()
+        _check(self._L.bydb_scan_partials_keyed_wide(self._h, C.byref(cq), C.byref(gk), C.byref(r)))
         return self._read_keyed_partials(q, r)
 
     def scan_reduce_keyed_partials(self, q: Query, family: str, tag: str, root: int = 0, max_values: int = 0,

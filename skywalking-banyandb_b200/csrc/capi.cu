@@ -366,6 +366,7 @@ const char *dev_err_text(uint32_t code) {
         case kErrKeyCap: return "per-row group key: more distinct key values than bydb_group_key.max_values";
         case kErrKeyLong: return "per-row group key: a key value longer than 64 bytes";
         case kErrRankOverlap: return "keyed collective: a series lives on several ranks over time spans that intersect";
+        case kErrKeyBlock: return "wide group key: a block whose int64 key column holds more than 256 distinct values";
     }
     return "unknown device error";
 }
@@ -1037,6 +1038,33 @@ ScanLayout scan_layout(const StageLayout &st, size_t NB, size_t F, size_t n_part
     return sl;
 }
 
+// the query's side of ScanParams: predicates, fields and what each field's aggregations need, the time range
+void scan_query_params(bydb_ctx *ctx, const bydb_query *q, const Plan &plan, ScanParams &sp) {
+    const size_t F = plan.fcols.size();
+    sp.n_preds = q->n_preds;
+    sp.tmin = q->tmin;
+    sp.tmax = q->tmax;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        for (size_t c = 0; c < F; ++c) sp.fcol_name[c] = ctx->names.find("f:" + plan.fcols[c]);
+        for (uint32_t a = 0; a < q->n_aggs; ++a) {
+            const int fn = q->aggs[a].func;
+            uint8_t need = (fn == BYDB_AGG_SUM || fn == BYDB_AGG_MEAN) ? 1 : (fn == BYDB_AGG_MIN || fn == BYDB_AGG_MAX) ? 2 : 0;
+            sp.fcol_need[plan.agg_fcol[a]] |= need;
+        }
+        for (uint32_t i = 0; i < q->n_preds; ++i) {
+            const bydb_pred &p = q->preds[i];
+            DevPred &dp = sp.preds[i];
+            dp.name_id = ctx->names.find(std::string("t:") + p.family + "/" + p.tag);
+            dp.op = static_cast<uint8_t>(p.op);
+            dp.value_type = static_cast<uint8_t>(p.value_type == BYDB_VT_BINARY ? BYDB_VT_STR : p.value_type);
+            dp.lit_i64 = p.lit_i64;
+            dp.lit_len = p.value_type == BYDB_VT_INT64 ? 0 : static_cast<uint32_t>(p.lit_len);
+            if (dp.lit_len) memcpy(dp.lit, p.lit, dp.lit_len);
+        }
+    }
+}
+
 // resident: the scratch is a view into a prepared query's StepState whose staging was uploaded when the state was built, and the
 // step is being captured for replay: one reset kernel instead of the memsets, no staging copy, and the zero page is left for
 // finalize_enqueue to read back with the result rows.  A pass of a captured keyed step (kp->zero set) launches no reset of its
@@ -1087,28 +1115,7 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     sp.q_sids = reinterpret_cast<const uint64_t *>(d + off_sids);
     sp.n_series = static_cast<uint32_t>(NS);
     sp.n_fcols = static_cast<uint32_t>(F);
-    sp.n_preds = q->n_preds;
-    sp.tmin = q->tmin;
-    sp.tmax = q->tmax;
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        for (size_t c = 0; c < F; ++c) sp.fcol_name[c] = ctx->names.find("f:" + plan.fcols[c]);
-        for (uint32_t a = 0; a < q->n_aggs; ++a) {
-            const int fn = q->aggs[a].func;
-            uint8_t need = (fn == BYDB_AGG_SUM || fn == BYDB_AGG_MEAN) ? 1 : (fn == BYDB_AGG_MIN || fn == BYDB_AGG_MAX) ? 2 : 0;
-            sp.fcol_need[plan.agg_fcol[a]] |= need;
-        }
-        for (uint32_t i = 0; i < q->n_preds; ++i) {
-            const bydb_pred &p = q->preds[i];
-            DevPred &dp = sp.preds[i];
-            dp.name_id = ctx->names.find(std::string("t:") + p.family + "/" + p.tag);
-            dp.op = static_cast<uint8_t>(p.op);
-            dp.value_type = static_cast<uint8_t>(p.value_type == BYDB_VT_BINARY ? BYDB_VT_STR : p.value_type);
-            dp.lit_i64 = p.lit_i64;
-            dp.lit_len = p.value_type == BYDB_VT_INT64 ? 0 : static_cast<uint32_t>(p.lit_len);
-            if (dp.lit_len) memcpy(dp.lit, p.lit, dp.lit_len);
-        }
-    }
+    scan_query_params(ctx, q, plan, sp);
     sp.worklist = reinterpret_cast<uint32_t *>(d + off_worklist);
     sp.work_count = &z->work_count;
     sp.work_next = &z->work_next;
@@ -2354,6 +2361,288 @@ int scan_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *ke
     undo.done = true;
     return 0;
 }
+
+// ---- bydb_scan_agg_keyed_wide / bydb_scan_partials_keyed_wide: one scan pass (see "Wide group key" in scan_kernels.cu)
+int check_wide_key(const bydb_group_key *key, uint32_t &cap) {
+    if (!key || !key->family || !key->tag) return fail(BYDB_EINVAL, "group key without family/tag");
+    if (key->value_type != 0 && key->value_type != BYDB_VT_STR && key->value_type != BYDB_VT_BINARY && key->value_type != BYDB_VT_INT64)
+        return fail(BYDB_EINVAL, "bydb_group_key.value_type must be 0, BYDB_VT_STR, BYDB_VT_BINARY or BYDB_VT_INT64");
+    cap = key->max_values ? key->max_values : 64u;
+    if (cap > kMaxWideKeyValues) return fail(BYDB_EINVAL, "bydb_group_key.max_values above 65536");
+    return 0;
+}
+
+size_t pow2_at_least(size_t n) {
+    size_t p = 1;
+    while (p < n) p <<= 1;
+    return p;
+}
+
+// the composite groups' (series group, key value) back onto rows that carry the position in insertion order
+void wide_row_keys(const std::vector<int32_t> &pairs, std::vector<int32_t> &group_id, std::vector<int32_t> &key_id) {
+    key_id.resize(group_id.size());
+    for (size_t r = 0; r < group_id.size(); ++r) {
+        const size_t j = static_cast<size_t>(group_id[r]);
+        group_id[r] = pairs[2 * j];
+        key_id[r] = pairs[2 * j + 1];
+    }
+}
+
+// the answer forms over the present composite table (n_comp groups of layout tl at `table`, pairs at d_pairs)
+int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const int32_t *d_pairs,
+              const int32_t *, const uint32_t *, bydb_keyed_result *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    Plan planc = plan;
+    planc.n_groups = static_cast<int32_t>(n_comp);
+    int rc = finalize_to_host(q, planc, slot, stream, table, tl, &out->base, true);
+    if (rc) return rc;
+    std::vector<int32_t> pairs(2 * n_comp);
+    CUDA_TRY(cudaMemcpyAsync(pairs.data(), d_pairs, pairs.size() * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    out->base.stats.d2h_bytes += pairs.size() * 4;
+    auto *ro = static_cast<ResultOwner *>(out->base.owner);
+    wide_row_keys(pairs, ro->group_id, owner->key_id);
+    out->key_id = owner->key_id.data();
+    return 0;
+}
+int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const int32_t *d_pairs,
+              const int32_t *d_perm, const uint32_t *d_ncomp, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), A = q->n_aggs, ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
+    Plan planc = plan;
+    planc.n_groups = static_cast<int32_t>(n_comp);
+    Scratch img;
+    CUDA_TRY(img.alloc(ctl_bytes + n_comp * row_bytes, stream));
+    const TablePtrs t = tl.at(table);
+    launch_keyed_partial_rows(rows_params(q, planc, 1, t, t.coltype, d_perm, d_ncomp, img.base), n_comp, stream);
+    out->stats.kernel_launches += 1;
+    if (slot.ensure_pinned(ctl_bytes + n_comp * row_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base, ctl_bytes + n_comp * row_bytes, cudaMemcpyDeviceToHost, stream));
+    std::vector<int32_t> pairs(2 * n_comp);
+    CUDA_TRY(cudaMemcpyAsync(pairs.data(), d_pairs, pairs.size() * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    out->stats.d2h_bytes += ctl_bytes + n_comp * row_bytes + pairs.size() * 4;
+    int rc = parse_rows(slot.pinned, q, planc, n_comp, &out->base, nullptr);
+    if (rc) return rc;
+    auto *ro = static_cast<PartialRowsOwner *>(out->base.owner);
+    wide_row_keys(pairs, ro->group_id, owner->key_id);
+    out->key_id = owner->key_id.data();
+    return 0;
+}
+
+template <class Out>
+int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    memset(out, 0, sizeof *out);
+    int rc = validate_query(q, true);
+    if (rc) return rc;
+    uint32_t cap = 0;
+    rc = check_wide_key(key, cap);
+    if (rc) return rc;
+    g_last_dev_err = 0;
+    Plan plan;
+    rc = make_plan(ctx, q, nullptr, plan);
+    if (rc) return rc;
+    if (parts_overlap(plan.parts, q->tmin, q->tmax))
+        return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    SlotLease lease(ctx);
+    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
+    ExecSlot &slot = *lease.slot;
+    cudaStream_t stream = slot.stream;
+    const bool int64_key = key->value_type == BYDB_VT_INT64;
+    const size_t F = plan.fcols.size(), NS = q->n_series, NB = plan.total_blocks, NBp = align_up(std::max<size_t>(NB, 1), 1024);
+    bydb_stats &stats = keyed_stats(out);
+    memset(&stats, 0, sizeof stats);
+    cudaEvent_t *ev = slot.ev;
+    CUDA_TRY(cudaEventRecord(ev[0], stream));
+
+    // 1. discovery: the value table (S slots), each selected block's rank and distinct values, then their exclusive scan
+    const size_t S = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(cap), kKeySlots));
+    Carve carve;
+    const size_t a_sids = carve(NS * 8), a_grp = carve(NS * 4), a_slots = carve(S * 8), a_ctl = carve(32), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
+                 a_lens = carve(static_cast<size_t>(cap) * 4), a_sid = carve(S * 4), a_nbr = carve(NBp * 4), a_rank = carve(NB * 4),
+                 a_tiles = carve(NBp / 1024 * 4);
+    Scratch ka;
+    CUDA_TRY(ka.alloc(carve.o, stream));
+    if (slot.ensure_pinned(std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    memcpy(slot.pinned, q->series_ids, NS * 8);
+    int32_t *hg = reinterpret_cast<int32_t *>(slot.pinned + NS * 8);
+    for (size_t i = 0; i < NS; ++i) hg[i] = q->series_group ? q->series_group[i] : 0;
+    if (NS) {
+        CUDA_TRY(cudaMemcpyAsync(ka.base + a_sids, slot.pinned, NS * 8, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(ka.base + a_grp, slot.pinned + NS * 8, NS * 4, cudaMemcpyHostToDevice, stream));
+    }
+    stats.h2d_bytes += NS * 12;
+    CUDA_TRY(cudaMemsetAsync(ka.base + a_slots, 0, a_vals - a_slots, stream));
+    CUDA_TRY(cudaMemsetAsync(ka.base + a_nbr, 0, NBp * 4, stream));
+    WideKeyParams wk;
+    memset(&wk, 0, sizeof wk);
+    KeyParams &kp = wk.k;
+    part_refs(plan.parts, kp.parts);
+    kp.n_parts = static_cast<uint32_t>(plan.parts.size());
+    kp.total_blocks = static_cast<uint32_t>(NB);
+    kp.q_sids = reinterpret_cast<const uint64_t *>(ka.base + a_sids);
+    kp.n_series = static_cast<uint32_t>(NS);
+    kp.cap = cap;
+    kp.tmin = q->tmin;
+    kp.tmax = q->tmax;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        kp.key_name = ctx->names.find(std::string("t:") + key->family + "/" + key->tag);
+    }
+    uint32_t *d_ctl = reinterpret_cast<uint32_t *>(ka.base + a_ctl);  // [0] values [1] DevErr [2] its block [3] int64 zero [4] R
+    kp.slots = reinterpret_cast<unsigned long long *>(ka.base + a_slots);
+    kp.count = d_ctl;
+    kp.err = d_ctl + 1;
+    kp.zero = d_ctl + 3;
+    kp.vals = ka.base + a_vals;
+    kp.lens = reinterpret_cast<uint32_t *>(ka.base + a_lens);
+    wk.slot_mask = static_cast<uint32_t>(S - 1);
+    wk.int64_key = int64_key ? 1u : 0u;
+    wk.slot_id = reinterpret_cast<uint32_t *>(ka.base + a_sid);
+    wk.n_by_rank = reinterpret_cast<uint32_t *>(ka.base + a_nbr);
+    wk.rank = reinterpret_cast<uint32_t *>(ka.base + a_rank);
+    launch_key_values_wide(wk, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+    launch_excl_scan(wk.n_by_rank, static_cast<uint32_t>(NBp), reinterpret_cast<uint32_t *>(ka.base + a_tiles), d_ctl + 4, stream);
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, d_ctl, 32, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    stats.kernel_launches += (NB ? 1u : 0u) + 1u + 3u;
+    stats.d2h_bytes += 32;
+    uint32_t ctl[8];
+    memcpy(ctl, slot.pinned, 32);
+    if (ctl[1] != 0) {
+        g_last_dev_err = ctl[1];
+        char buf[64];
+        snprintf(buf, sizeof buf, " (block #%u)", ctl[2]);
+        return fail(dev_err_code(ctl[1]), std::string(dev_err_text(ctl[1])) + buf);
+    }
+    const size_t V = std::min<size_t>(ctl[0], cap), R = ctl[4];
+    KeyValues values(V);
+    if (V) {
+        const size_t vb = V * (int64_key ? 8 : kMaxLit);
+        CUDA_TRY(cudaMemcpyAsync(slot.pinned, kp.vals, vb, cudaMemcpyDeviceToHost, stream));
+        if (!int64_key) CUDA_TRY(cudaMemcpyAsync(slot.pinned + vb, kp.lens, V * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        stats.d2h_bytes += vb + (int64_key ? 0 : V * 4);
+        const uint32_t *hl = reinterpret_cast<const uint32_t *>(slot.pinned + vb);
+        for (size_t v = 0; v < V; ++v) {
+            if (int64_key) values[v].assign(slot.pinned + v * 8, slot.pinned + v * 8 + 8);  // the reference's key bytes: little-endian int64
+            else values[v].assign(slot.pinned + v * kMaxLit, slot.pinned + v * kMaxLit + hl[v]);
+        }
+    }
+    auto owner = new KeyedOwner();
+    out->owner = owner;
+    KeyedUndo<Out> undo{ctx, out};
+    set_key_table(out, owner, values);
+    if (V == 0 || R == 0) {  // no block selected: no rows (n_rows = 0)
+        undo.done = true;
+        return 0;
+    }
+    if (R > 0x7fffffffull) return fail(BYDB_ENOMEM, "wide group-key query: too many (block, key value) records");
+
+    // 2. the scan: one record per present (block, key value)
+    const size_t rec_bytes = wide_record_bytes(F);
+    const size_t C = pow2_at_least(std::max<size_t>(2 * R, 1024)), N = pow2_at_least(std::max<size_t>(R, 2048));
+    Carve cb;
+    const size_t b_zero = cb(kZeroPageBytes), b_rec = cb(R * rec_bytes), b_comp = cb(C * 8), b_cmin = cb(C * 4), b_rslot = cb(R * 4), b_keys = cb(N * 8),
+                 b_heads = cb(N * 4), b_tiles = cb(N / 1024 * 4), b_ctl = cb(8), b_seg = cb(R * 4);
+    Scratch sb;
+    CUDA_TRY(sb.alloc(cb.o, stream));
+    ZeroPage *z = reinterpret_cast<ZeroPage *>(sb.base + b_zero);
+    CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + b_comp, 0, C * 8, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + b_cmin, 0xff, C * 4, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + b_ctl, 0, 8, stream));
+    ScanParams sp;
+    memset(&sp, 0, sizeof sp);
+    part_refs(plan.parts, sp.parts);
+    sp.n_parts = static_cast<uint32_t>(plan.parts.size());
+    sp.total_blocks = static_cast<uint32_t>(NB);
+    sp.q_sids = kp.q_sids;
+    sp.n_series = static_cast<uint32_t>(NS);
+    sp.n_fcols = static_cast<uint32_t>(F);
+    scan_query_params(ctx, q, plan, sp);
+    sp.err = z->err;
+    sp.stats = z->stats;
+    sp.col_type = z->col_type;
+    WideScanParams ws;
+    memset(&ws, 0, sizeof ws);
+    ws.slots = kp.slots;
+    ws.slot_id = wk.slot_id;
+    ws.zero = kp.zero;
+    ws.slot_mask = wk.slot_mask;
+    ws.int64_key = wk.int64_key;
+    ws.key_name = kp.key_name;
+    ws.rank = wk.rank;
+    ws.rec_off = wk.n_by_rank;
+    ws.series_group = reinterpret_cast<const int32_t *>(ka.base + a_grp);
+    ws.records = sb.base + b_rec;
+    CUDA_TRY(cudaEventRecord(ev[1], stream));
+    launch_scan_keyed_wide(sp, ws, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+    CUDA_TRY(cudaEventRecord(ev[2], stream));
+
+    // 3. the composite groups in insertion order
+    WideReduceParams rp;
+    memset(&rp, 0, sizeof rp);
+    rp.records = ws.records;
+    rp.n_records = static_cast<uint32_t>(R);
+    rp.n_fcols = static_cast<uint32_t>(F);
+    rp.comp = reinterpret_cast<unsigned long long *>(sb.base + b_comp);
+    rp.comp_min = reinterpret_cast<uint32_t *>(sb.base + b_cmin);
+    rp.rec_slot = reinterpret_cast<uint32_t *>(sb.base + b_rslot);
+    rp.comp_mask = static_cast<uint32_t>(C - 1);
+    rp.n_sort = static_cast<uint32_t>(N);
+    rp.keys = reinterpret_cast<unsigned long long *>(sb.base + b_keys);
+    rp.heads = reinterpret_cast<uint32_t *>(sb.base + b_heads);
+    rp.tile_sums = reinterpret_cast<uint32_t *>(sb.base + b_tiles);
+    rp.ctl = reinterpret_cast<uint32_t *>(sb.base + b_ctl);
+    rp.seg_start = reinterpret_cast<uint32_t *>(sb.base + b_seg);
+    rp.col_type = z->col_type;
+    rp.scan_err = z->err;
+    launch_wide_order(rp, stream);
+    ZeroPage *hz = slot.page(0);
+    CUDA_TRY(cudaMemcpyAsync(hz, z, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, rp.ctl, 8, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    uint32_t sort_launches = 0;
+    for (size_t size = 4096; size <= N; size <<= 1) sort_launches += 1 + static_cast<uint32_t>(__builtin_ctzll(size) - 11);
+    stats.kernel_launches += (NB ? 1u : 0u) + 2u + 1u + sort_launches + 1u + 3u + 1u;
+    stats.d2h_bytes += kZeroPageBytes + 8;
+    {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, ev[1], ev[2]);
+        stats.scan_kernel_ms += ms;
+    }
+    rc = read_zero_page(*hz, false, &stats);
+    if (rc) return rc;
+    const size_t n_comp = reinterpret_cast<const uint32_t *>(slot.pinned)[1];
+
+    // 4. the fold into a table of the present composite groups, then the form's own answer
+    const TableLayout tl(std::max<size_t>(n_comp, 1), F);
+    Carve cf;
+    const size_t f_table = cf(tl.total), f_pairs = cf(n_comp * 8), f_perm = cf(n_comp * 4);
+    Scratch fb;
+    CUDA_TRY(fb.alloc(cf.o, stream));
+    rp.table = tl.at(fb.base + f_table);
+    rp.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
+    rp.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
+    launch_wide_fold(rp, static_cast<uint32_t>(n_comp), stream);
+    CUDA_TRY(cudaEventRecord(ev[3], stream));
+    stats.kernel_launches += 1;
+    if (n_comp > 0) rc = wide_emit(q, plan, slot, fb.base + f_table, tl, n_comp, rp.pairs, rp.perm, &rp.ctl[1], out, owner);
+    if (rc) return rc;
+    {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, ev[0], ev[3]);
+        stats.device_ms += ms;
+    }
+    undo.done = true;
+    return 0;
+}
 }  // namespace
 }  // extern "C++"
 
@@ -2367,6 +2656,15 @@ int bydb_scan_agg_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key
 // The map-phase form of the same query: wire rows of the present composite groups (keyed_partial_rows_kernel).
 int bydb_scan_partials_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out) {
     return guarded([&]() -> int { return scan_keyed_impl(ctx, q, key, out); });
+}
+
+// Group-by on a stored tag in one scan pass, up to 65,536 values: see "Wide group key" in scan_kernels.cu.
+int bydb_scan_agg_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out) {
+    return guarded([&]() -> int { return scan_keyed_wide_impl(ctx, q, key, out); });
+}
+
+int bydb_scan_partials_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out) {
+    return guarded([&]() -> int { return scan_keyed_wide_impl(ctx, q, key, out); });
 }
 
 void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r) {

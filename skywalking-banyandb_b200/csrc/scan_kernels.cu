@@ -2081,6 +2081,8 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kFastLane ? BYDB_FAST_CTAS 
         uint32_t page_bytes = 0;
         uint32_t err = kErrNone;
 
+        // Steps 1 and 2 of the general lane (kFastLane = false) are copied into scan_keyed_wide_kernel: a change to the time-range or
+        // predicate semantics here must land there too (sharing the code moved this kernel's register allocation, DESIGN.md 4.6).
         // ---- 1. time range -> rows [r0,r1] (block.go:825-829, range.go:143-169)
         uint32_t r0 = 0, r1 = count - 1;
         bool empty = false;
@@ -3629,21 +3631,22 @@ __device__ __forceinline__ void key_err(const KeyParams &p, uint32_t code, uint3
 }
 
 // home slot of a key value: FNV-1a over its key bytes (an int64 key's are its 8 little-endian bytes, see key_slot_i64)
-__device__ __forceinline__ uint32_t key_home(const uint8_t *bytes, uint32_t len) {
+// mask: slots - 1 of the table (the wide key's table is sized from its cap)
+__device__ __forceinline__ uint32_t key_home(const uint8_t *bytes, uint32_t len, uint32_t mask = kKeySlots - 1) {
     uint64_t h = 0xcbf29ce484222325ull;
     for (uint32_t i = 0; i < len; ++i) h = (h ^ __ldg(bytes + i)) * 0x100000001b3ull;
-    return static_cast<uint32_t>(h ^ (h >> 32)) & (kKeySlots - 1);
+    return static_cast<uint32_t>(h ^ (h >> 32)) & mask;
 }
 
-__device__ void key_insert(const KeyParams &p, const uint8_t *bytes, uint32_t len, uint32_t g) {
+__device__ void key_insert(const KeyParams &p, const uint8_t *bytes, uint32_t len, uint32_t g, uint32_t mask = kKeySlots - 1) {
     if (len > kMaxLit) {
         key_err(p, kErrKeyLong, g);
         return;
     }
     const unsigned long long mine =
         (1ull << 63) | (static_cast<unsigned long long>(len) << 48) | (len ? (reinterpret_cast<uintptr_t>(bytes) & 0xffffffffffffull) : 0ull);
-    uint32_t s = key_home(bytes, len);
-    for (uint32_t probe = 0; probe < kKeySlots; ++probe) {
+    uint32_t s = key_home(bytes, len, mask);
+    for (uint32_t probe = 0; probe <= mask; ++probe) {
         unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.slots[s]);
         if (cur == 0) {
             cur = atomicCAS(&p.slots[s], 0ull, mine);
@@ -3658,7 +3661,7 @@ __device__ void key_insert(const KeyParams &p, const uint8_t *bytes, uint32_t le
             for (uint32_t i = 0; i < len && eq; ++i) eq = __ldg(o + i) == __ldg(bytes + i);
             if (eq) return;
         }
-        s = (s + 1) & (kKeySlots - 1);
+        s = (s + 1) & mask;
     }
     key_err(p, kErrKeyCap, g);
 }
@@ -3749,21 +3752,21 @@ __global__ void key_pack_kernel(const __grid_constant__ KeyParams p) {
 // column's zero value (typed_column.go:49-53), so nil and 0 are one key.  The values have no address in the part, so a slot
 // holds the value itself: 0 marks an empty slot and the value 0 is recorded in a flag word of its own (p.zero).  The home
 // slot is key_insert's, FNV-1a over the 8 key bytes.
-__device__ __forceinline__ uint32_t key_slot_i64(unsigned long long u) {
+__device__ __forceinline__ uint32_t key_slot_i64(unsigned long long u, uint32_t mask = kKeySlots - 1) {
     uint64_t h = 0xcbf29ce484222325ull;
 #pragma unroll
     for (int i = 0; i < 8; ++i) h = (h ^ ((u >> (8 * i)) & 0xffu)) * 0x100000001b3ull;
-    return static_cast<uint32_t>(h ^ (h >> 32)) & (kKeySlots - 1);
+    return static_cast<uint32_t>(h ^ (h >> 32)) & mask;
 }
 // u enters the table from its home slot s; false = an error was raised (the caller stops inserting)
-__device__ __noinline__ bool key_insert_i64(const KeyParams &p, unsigned long long u, uint32_t s, uint32_t g) {
+__device__ __forceinline__ bool key_insert_i64_at(const KeyParams &p, unsigned long long u, uint32_t s, uint32_t g, uint32_t mask) {
     if (u == 0ull) {
         if (*reinterpret_cast<volatile uint32_t *>(p.zero) != 0u || atomicExch(p.zero, 1u) != 0u) return true;
         if (atomicAdd(p.count, 1u) < p.cap) return true;
         key_err(p, kErrKeyCap, g);
         return false;
     }
-    for (uint32_t probe = 0; probe < kKeySlots; ++probe) {
+    for (uint32_t probe = 0; probe <= mask; ++probe) {
         unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.slots[s]);
         if (cur == 0ull) {
             cur = atomicCAS(&p.slots[s], 0ull, u);
@@ -3774,10 +3777,14 @@ __device__ __noinline__ bool key_insert_i64(const KeyParams &p, unsigned long lo
             }
         }
         if (cur == u) return true;
-        s = (s + 1) & (kKeySlots - 1);
+        s = (s + 1) & mask;
     }
     key_err(p, kErrKeyCap, g);
     return false;
+}
+
+__device__ __noinline__ bool key_insert_i64(const KeyParams &p, unsigned long long u, uint32_t s, uint32_t g) {
+    return key_insert_i64_at(p, u, s, g, kKeySlots - 1);
 }
 
 // Per-warp cache in shared memory of values already in the table, direct-mapped by the home slot: a value that changes
@@ -4330,6 +4337,980 @@ __global__ void keyed_row_map_kernel(const int32_t *sel_group, const uint32_t *s
 void launch_keyed_row_map(const int32_t *sel_group, const uint32_t *sel_count, const int32_t *perm, uint32_t n_groups, uint32_t cap,
                           int32_t *pairs, cudaStream_t s) {
     keyed_row_map_kernel<<<(cap + 255) / 256, 256, 0, s>>>(sel_group, sel_count, perm, n_groups, cap, pairs);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Wide group key (bydb_scan_agg_keyed_wide): the answer of the per-value passes above in ONE scan pass, for up to
+// kMaxWideKeyValues values.
+//   1. key_values_wide_kernel: one warp per selected block enters the block's distinct key values into a table sized from the
+//      cap (key_insert / key_insert_i64_at), and records the block's scan-order rank and its distinct values D_b (more than
+//      kMaxBlockKeys: kErrKeyBlock).  key_pack_wide_kernel numbers the values in slot order.  The host's exclusive scan of D_b in
+//      rank order then places every block's records, so that the records lie in scan order.
+//   2. scan_keyed_wide_kernel: one warp per selected block: the time range and the predicates -> row mask (the general lane's
+//      steps 1 and 2), the key column -> a block-local index per row, every field page decoded once, each surviving row folded
+//      into one of <= 256 block-local accumulators in shared memory.  Those hold integers only (decimal pages sum in the exact
+//      integer domain, min / max compare integers), so the order of the shared-memory atomics does not matter; raw float cells
+//      are folded by one lane in row order.  A present (block, key) writes one record, a block's records ordered by first row.
+//   3. the composite group of a record is (series group, value id); its lowest record is its first row in scan order.  Sorting
+//      (lowest record of the composite, record) puts the composite groups in insertion order and each one's records in scan
+//      order; wide_fold_kernel folds them in that order with a fixed tree into row j of a partial table that holds only the
+//      present composite groups.  The ordinary finalisation / Top-N, or keyed_partial_rows_kernel, run on it unchanged.
+// ------------------------------------------------------------------------------------------------
+constexpr int kWideWarps = 2;             // 2 x (WarpSmem + WideSmem) per CTA: three CTAs per SM
+constexpr uint32_t kLocalSlots = 2 * kMaxBlockKeys;
+
+struct __align__(16) WideSmem {
+    uint8_t kidx[kMaskWords * 32];        // block-local key index of each row
+    union {
+        struct {                          // int64 key: the block's values (0 = empty; the value 0 has its own flag)
+            unsigned long long val[kLocalSlots];
+            uint8_t idx[kLocalSlots];
+        } t;
+        struct {                          // the field being folded: 128-bit sum (or raw float sum bits in lo)
+            unsigned long long lo[kMaxBlockKeys];
+            long long hi[kMaxBlockKeys];
+        } s;
+    } u;
+    long long mn[kMaxBlockKeys], mx[kMaxBlockKeys];
+    uint32_t cnt[kMaxBlockKeys];
+    unsigned long long dense[kMaxBlockKeys];  // local key k: its slot word (string: bit63 | len << 48 | address; int64: the value)
+    uint32_t gid[kMaxBlockKeys];          // value id of local key k
+    uint32_t krows[kMaxBlockKeys], kfirst[kMaxBlockKeys];
+    uint32_t rank[kMaxBlockKeys];         // position of local key k among the block's records
+    uint32_t n_ins, zero, over, n_local;
+};
+size_t wide_smem_bytes() { return (sizeof(WarpSmem) + sizeof(WideSmem)) * kWideWarps; }
+
+__device__ __forceinline__ uint32_t lower_sid(const DevPartRef &part, uint64_t sid) {
+    uint32_t lo = 0, hi = part.n_blocks;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (part.blocks[mid].sid < sid) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+__device__ __forceinline__ uint32_t upper_sid(const DevPartRef &part, uint64_t sid) {
+    uint32_t lo = 0, hi = part.n_blocks;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (part.blocks[mid].sid <= sid) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// Rank of block b of part pi in scan order over every block of every part: by series, then by time (a part's blocks are sorted by
+// (series, time); the parts of a wide query do not overlap in time, so a series' blocks in another part come before or after all
+// of these, as that part's first block of the series starts earlier or later).  Lanes take the parts.
+__device__ uint32_t scan_rank(const DevPartRef *parts, uint32_t n_parts, uint32_t pi, uint32_t b, int lane) {
+    const uint64_t sid = parts[pi].blocks[b].sid;
+    const uint32_t own_lo = lower_sid(parts[pi], sid);
+    const int64_t own_ts = parts[pi].blocks[own_lo].ts_min;
+    uint32_t r = 0;
+    for (uint32_t q = lane; q < n_parts; q += 32) {
+        if (q == pi) continue;
+        const uint32_t lo = lower_sid(parts[q], sid), hi = upper_sid(parts[q], sid);
+        r += lo;
+        if (hi > lo) {
+            const int64_t ts = parts[q].blocks[lo].ts_min;
+            if (ts < own_ts || (ts == own_ts && q < pi)) r += hi - lo;
+        }
+    }
+    r = __reduce_add_sync(0xffffffffu, r);
+    return r + b;
+}
+
+// ---- the block's key column -> its distinct values in ws->dense[0, n_local) and, with kRows, the local index of every row in
+// ws->kidx.  String key: a dictionary page, local index = dictionary index (a nil entry is the value "").  int64 key: every value
+// of the page enters a local table (pass 1), is numbered in slot order, and with kRows the page is decoded again to look each
+// row's value up (pass 2).  A column absent from the block is one value, "" or 0, on every row.  Returns a DevErr.
+struct LocalInsCons {
+    WideSmem *ws;
+    __device__ __forceinline__ void operator()(uint32_t, int64_t v) {
+        const unsigned long long u = static_cast<unsigned long long>(v);
+        if (u == 0ull) {
+            ws->zero = 1u;
+            return;
+        }
+        uint32_t s = key_slot_i64(u, kLocalSlots - 1);
+        for (uint32_t probe = 0; probe < kLocalSlots; ++probe) {
+            unsigned long long cur = reinterpret_cast<volatile unsigned long long *>(ws->u.t.val)[s];
+            if (cur == 0ull) {
+                cur = atomicCAS(&ws->u.t.val[s], 0ull, u);
+                if (cur == 0ull) {
+                    atomicAdd(&ws->n_ins, 1u);
+                    return;
+                }
+            }
+            if (cur == u) return;
+            s = (s + 1) & (kLocalSlots - 1);
+        }
+        ws->over = 1u;
+    }
+};
+struct LocalIdxCons {
+    WideSmem *ws;
+    __device__ __forceinline__ void operator()(uint32_t row, int64_t v) {
+        const unsigned long long u = static_cast<unsigned long long>(v);
+        uint32_t k = 0;
+        if (u != 0ull) {
+            uint32_t s = key_slot_i64(u, kLocalSlots - 1);
+            for (uint32_t probe = 0; probe < kLocalSlots && ws->u.t.val[s] != u; ++probe) s = (s + 1) & (kLocalSlots - 1);
+            k = ws->u.t.idx[s];
+        }
+        if (row < kMaskWords * 32) ws->kidx[row] = static_cast<uint8_t>(k);
+    }
+};
+
+// every row's value of an int64 key page, to c(row, v); a nil raw cell is 0 (typed_column.go:49-53)
+template <class C>
+__device__ uint32_t key_i64_rows(WarpSmem *sm, const uint8_t *page, uint32_t size, uint32_t count, C &c, int lane) {
+    const uint32_t enc = size >= 1 ? __ldg(page) : 0u;
+    if (size < 1) return kErrCorrupt;
+    if (enc == kEncRawCells) {
+        if (size < 8 + 9ull * count || (reinterpret_cast<uintptr_t>(page) & 7)) return kErrCorrupt;
+        const bool nulls = __ldg(page + 1) != 0;
+        const long long *vals = reinterpret_cast<const long long *>(page + 8);
+        const uint8_t *valid = page + 8 + 8ull * count;
+        for (uint32_t row = lane; row < count; row += 32) c(row, !nulls || __ldg(valid + row) != 0 ? __ldg(vals + row) : 0);
+        return kErrNone;
+    }
+    if (enc == 9) return kErrPlainPage;
+    if (size < 9) return kErrCorrupt;
+    const int64_t first = conv_bytes_to_int64(page + 1);
+    const uint8_t *body = page + 9;
+    const uint32_t blen = size - 9;
+    if (enc == 1 || enc == 2) {
+        int64_t d = 0;
+        uint32_t used = 0;
+        if (enc == 1 && blen != 0) return kErrCorrupt;
+        if (enc == 2 && (!read_varint_seq(body, blen, d, used) || used != blen)) return kErrCorrupt;
+        for (uint32_t row = lane; row < count; row += 32) c(row, static_cast<int64_t>(static_cast<uint64_t>(first) + static_cast<uint64_t>(d) * row));
+        return kErrNone;
+    }
+    if (enc != 3 && enc != 4) return kErrBadEnc;
+    bool ok;
+    if (enc == 3) ok = decode_varint_page<false>(sm, body, blen, count, first, c, lane);
+    else ok = decode_varint_page<true>(sm, body, blen, count, first, c, lane);
+    if (!__all_sync(0xffffffffu, ok)) return kErrCorrupt;
+    return sm->fault ? kErrTmaTimeout : kErrNone;
+}
+
+template <bool kRows>
+__device__ uint32_t wide_block_keys(WarpSmem *sm, WideSmem *ws, const DevPartRef &part, const DevBlock &blk, uint16_t key_name, bool int64_key,
+                                    int lane) {
+    const uint32_t count = blk.count;
+    DevCol col;
+    if (!find_col(part, blk, key_name, col, lane)) {
+        if (kRows)
+            for (uint32_t r = lane; r < count && r < kMaskWords * 32; r += 32) ws->kidx[r] = 0;
+        if (lane == 0) {
+            ws->dense[0] = int64_key ? 0ull : (1ull << 63);
+            ws->n_local = 1;
+        }
+        __syncwarp();
+        return kErrNone;
+    }
+    const uint8_t *page = part.files[col.file_id] + col.off;
+    if (int64_key) {
+        if (col.value_type != BYDB_VT_INT64) return kErrPredType;
+        for (uint32_t s = lane; s < kLocalSlots; s += 32) ws->u.t.val[s] = 0ull;
+        if (lane == 0) ws->n_ins = ws->zero = ws->over = 0;
+        __syncwarp();
+        LocalInsCons ins{ws};
+        uint32_t err = key_i64_rows(sm, page, col.size, count, ins, lane);
+        __syncwarp();
+        if (err != kErrNone) return err;
+        const uint32_t z = ws->zero, n = z + ws->n_ins;
+        if (ws->over || n > kMaxBlockKeys) return kErrKeyBlock;
+        // number the values: 0 first when it occurs, then the slots in order
+        uint32_t base = z;
+        if (lane == 0 && z) ws->dense[0] = 0ull;
+        for (uint32_t s0 = 0; s0 < kLocalSlots; s0 += 32) {
+            const unsigned long long v = ws->u.t.val[s0 + lane];
+            const uint32_t bal = __ballot_sync(0xffffffffu, v != 0ull);
+            if (v != 0ull) {
+                const uint32_t k = base + __popc(bal & ((1u << lane) - 1u));
+                ws->u.t.idx[s0 + lane] = static_cast<uint8_t>(k);
+                ws->dense[k] = v;
+            }
+            base += __popc(bal);
+        }
+        if (lane == 0) ws->n_local = n;
+        __syncwarp();
+        if (kRows) {
+            LocalIdxCons idx{ws};
+            err = key_i64_rows(sm, page, col.size, count, idx, lane);
+            __syncwarp();
+        }
+        return err;
+    }
+    // string key: a dictionary page (pkg/encoding/dictionary.go:52-114); a plain page holds more than 256 values
+    if (col.value_type != BYDB_VT_STR && col.value_type != BYDB_VT_BINARY) return kErrPredType;
+    if (col.size < 2) return kErrCorrupt;
+    if (__ldg(page) == 9) return kErrTagPlain;
+    if (__ldg(page) != 10) return kErrBadEnc;
+    const uint8_t *q = page + 1, *end = page + col.size;
+    uint64_t nvals = 0;
+    uint32_t llen = 0, dlen = 0;
+    if (!read_varuint_seq(q, end, nvals) || nvals == 0 || nvals > kMaxBlockKeys) return kErrCorrupt;
+    uint32_t err = read_cblock_header(q, end, llen, kErrZstdDict);
+    if (err != kErrNone) return err;
+    const uint8_t wt = llen >= 1 ? __ldg(q) : 4;
+    const uint32_t width = 1u << (wt & 3);
+    if (wt > 3 || llen != 1 + nvals * width) return kErrCorrupt;
+    const uint8_t *lens = q + 1;
+    q += llen;
+    err = read_cblock_header(q, end, dlen, kErrZstdDict);
+    if (err != kErrNone) return err;
+    const uint8_t *data = q;
+    q += dlen;
+    uint32_t off_carry = 0;
+    bool bad = false, long_val = false;
+    for (uint32_t base = 0; base < nvals; base += 32) {
+        const uint32_t k = base + lane;
+        uint32_t L = 0;
+        if (k < nvals)
+            for (uint32_t i = 0; i < width; ++i) L = (L << 8) | __ldg(lens + k * width + i);
+        const uint32_t vlen = L > 0 ? L - 1 : 0;
+        uint32_t incl = vlen;
+#pragma unroll
+        for (int sft = 1; sft < 32; sft <<= 1) {
+            const uint32_t o = __shfl_up_sync(0xffffffffu, incl, sft);
+            if (lane >= sft) incl += o;
+        }
+        const uint32_t off = off_carry + incl - vlen;
+        off_carry += __shfl_sync(0xffffffffu, incl, 31);
+        if (k < nvals) {
+            if (off + vlen > dlen) bad = true;
+            else if (vlen > static_cast<uint32_t>(kMaxLit)) long_val = true;
+            else ws->dense[k] = (1ull << 63) | (static_cast<unsigned long long>(vlen) << 48) |
+                                (vlen ? (reinterpret_cast<uintptr_t>(data + off) & 0xffffffffffffull) : 0ull);
+        }
+    }
+    if (__any_sync(0xffffffffu, bad)) return kErrCorrupt;
+    if (__any_sync(0xffffffffu, long_val)) return kErrKeyLong;
+    if (lane == 0) ws->n_local = static_cast<uint32_t>(nvals);
+    __syncwarp();
+    if (!kRows) return kErrNone;
+    // bit-packed RLE pairs [u32 BE n][u8 width][n x width bits] of dictionary indices (as apply_dict_pred reads them)
+    if (end - q < 5) return kErrCorrupt;
+    const uint32_t nrle = static_cast<uint32_t>(load_be64_unaligned(q) >> 32);
+    q += 4;
+    if (nrle == 0) return count == 0 ? kErrNone : kErrCorrupt;
+    if (nrle & 1u) return kErrCorrupt;
+    const uint32_t wbits = __ldg(q++);
+    if (wbits == 0 || wbits > 32) return kErrCorrupt;
+    if (static_cast<uint64_t>(end - q) * 8 < static_cast<uint64_t>(nrle) * wbits) return kErrCorrupt;
+    const uint32_t nruns = nrle >> 1;
+    const uint64_t vmask = (wbits == 32) ? 0xffffffffull : ((1ull << wbits) - 1ull);
+    uint32_t row_carry = 0;
+    for (uint32_t base = 0; base < nruns; base += 32) {
+        const uint32_t ri = base + lane;
+        uint32_t value = 0, cnt = 0;
+        if (ri < nruns) {
+            const uint64_t bo = static_cast<uint64_t>(2 * ri) * wbits;
+            value = read_bits_be(q, bo, wbits, vmask);
+            cnt = read_bits_be(q, bo + wbits, wbits, vmask);
+        }
+        uint32_t incl = cnt;
+#pragma unroll
+        for (int sft = 1; sft < 32; sft <<= 1) {
+            const uint32_t o = __shfl_up_sync(0xffffffffu, incl, sft);
+            if (lane >= sft) incl += o;
+        }
+        uint32_t start = row_carry + incl - cnt, stop = start + cnt;
+        row_carry += __shfl_sync(0xffffffffu, incl, 31);
+        if (ri < nruns && value >= nvals) bad = true;
+        stop = min(stop, min(count, static_cast<uint32_t>(kMaskWords * 32)));
+        start = min(start, stop);
+        if (ri < nruns && !bad) {
+            if (stop - start <= 64) {
+                for (uint32_t r = start; r < stop; ++r) ws->kidx[r] = static_cast<uint8_t>(value);
+            }
+        }
+        // long runs: the whole warp fills them
+        uint32_t lm = __ballot_sync(0xffffffffu, ri < nruns && !bad && stop - start > 64);
+        while (lm) {
+            const int src = __ffs(lm) - 1;
+            lm &= lm - 1;
+            const uint32_t a = __shfl_sync(0xffffffffu, start, src), b = __shfl_sync(0xffffffffu, stop, src);
+            const uint8_t v = static_cast<uint8_t>(__shfl_sync(0xffffffffu, value, src));
+            for (uint32_t r = a + lane; r < b; r += 32) ws->kidx[r] = v;
+        }
+    }
+    __syncwarp();
+    if (__any_sync(0xffffffffu, bad) || row_carry != count) return kErrCorrupt;
+    return kErrNone;
+}
+
+__global__ void __launch_bounds__(kWideWarps * 32) key_values_wide_kernel(const __grid_constant__ WideKeyParams w) {
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    const KeyParams &p = w.k;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    WarpSmem *sm = reinterpret_cast<WarpSmem *>(smem_raw) + warp;
+    WideSmem *ws = reinterpret_cast<WideSmem *>(smem_raw + sizeof(WarpSmem) * kWideWarps) + warp;
+    if (lane == 0) {
+        sm->fault = 0;
+        sm->seq = 0;
+        for (int s = 0; s < kStages; ++s) mbar_init(&sm->bar[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const uint32_t n_warps = gridDim.x * kWideWarps;
+    for (uint32_t g = blockIdx.x * kWideWarps + warp; g < p.total_blocks; g += n_warps) {
+        uint32_t stop = lane == 0 ? *reinterpret_cast<volatile uint32_t *>(&p.err[0]) : 0u;
+        stop = __shfl_sync(0xffffffffu, stop, 0);
+        if (stop != 0u) return;  // warp-uniform
+        uint32_t pi = 0;
+        while (pi + 1 < p.n_parts && g >= p.parts[pi + 1].block_base) ++pi;
+        const DevPartRef &part = p.parts[pi];
+        const DevBlock blk = part.blocks[g - part.block_base];
+        int32_t qi;
+        if (!select_block(p.q_sids, p.n_series, p.tmin, p.tmax, blk, qi)) continue;
+        uint32_t err = wide_block_keys<false>(sm, ws, part, blk, p.key_name, w.int64_key != 0, lane);
+        const uint32_t n = ws->n_local;
+        if (err == kErrNone) {
+            for (uint32_t k = lane; k < n; k += 32) {
+                const unsigned long long v = ws->dense[k];
+                if (w.int64_key) {
+                    key_insert_i64_at(p, v, v == 0ull ? 0u : key_slot_i64(v, w.slot_mask), g, w.slot_mask);
+                } else {
+                    const uint32_t len = static_cast<uint32_t>((v >> 48) & 0x7fffu);
+                    key_insert(p, reinterpret_cast<const uint8_t *>(static_cast<uintptr_t>(v & 0xffffffffffffull)), len, g, w.slot_mask);
+                }
+            }
+            const uint32_t r = scan_rank(p.parts, p.n_parts, pi, g - part.block_base, lane);
+            if (lane == 0) {
+                w.rank[g] = r;
+                w.n_by_rank[r] = n;
+            }
+        } else if (lane == 0) {
+            key_err(p, err, g);
+        }
+        __syncwarp();
+    }
+}
+
+// one CTA: the occupied slots numbered in slot order (int64 key: the value 0 first when it occurs), packed into vals / lens
+__global__ void __launch_bounds__(1024) key_pack_wide_kernel(const __grid_constant__ WideKeyParams w) {
+    __shared__ uint32_t warp_tot[32];
+    const KeyParams &p = w.k;
+    const uint32_t n_slots = w.slot_mask + 1;
+    uint32_t n = w.int64_key && *p.zero != 0u ? 1u : 0u;
+    if (threadIdx.x == 0 && n) reinterpret_cast<unsigned long long *>(p.vals)[0] = 0ull;
+    for (uint32_t s0 = 0; s0 < n_slots; s0 += blockDim.x) {
+        const uint32_t s = s0 + threadIdx.x;
+        const unsigned long long cur = s < n_slots ? p.slots[s] : 0ull;
+        uint32_t total = 0;
+        const uint32_t at = n + block_excl_scan(cur != 0ull ? 1u : 0u, warp_tot, total);
+        if (cur != 0ull) {
+            w.slot_id[s] = at;
+            if (at < p.cap) {
+                if (w.int64_key) {
+                    reinterpret_cast<unsigned long long *>(p.vals)[at] = cur;
+                } else {
+                    const uint32_t len = static_cast<uint32_t>((cur >> 48) & 0x7fffu);
+                    const uint8_t *o = reinterpret_cast<const uint8_t *>(static_cast<uintptr_t>(cur & 0xffffffffffffull));
+                    for (uint32_t i = 0; i < len; ++i) p.vals[static_cast<size_t>(at) * kMaxLit + i] = __ldg(o + i);
+                    p.lens[at] = len;
+                }
+            }
+        }
+        n += total;
+    }
+}
+
+void launch_key_values_wide(const WideKeyParams &p, int grid, cudaStream_t s) {
+    const size_t smem = wide_smem_bytes();
+    cudaFuncSetAttribute(key_values_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (p.k.total_blocks) key_values_wide_kernel<<<grid, kWideWarps * 32, smem, s>>>(p);
+    key_pack_wide_kernel<<<1, 1024, 0, s>>>(p);
+}
+
+// the id of a value the discovery entered (string: by its bytes, int64: by the value)
+__device__ __forceinline__ uint32_t wide_key_id(const WideScanParams &w, unsigned long long v) {
+    if (w.int64_key) {
+        if (v == 0ull) return 0u;
+        uint32_t s = key_slot_i64(v, w.slot_mask);
+        for (uint32_t probe = 0; probe <= w.slot_mask && w.slots[s] != v; ++probe) s = (s + 1) & w.slot_mask;
+        return w.slot_id[s];
+    }
+    const uint32_t len = static_cast<uint32_t>((v >> 48) & 0x7fffu);
+    const uint8_t *b = reinterpret_cast<const uint8_t *>(static_cast<uintptr_t>(v & 0xffffffffffffull));
+    uint32_t s = key_home(b, len, w.slot_mask);
+    for (uint32_t probe = 0; probe <= w.slot_mask; ++probe) {
+        const unsigned long long cur = w.slots[s];
+        if (((cur >> 48) & 0x7fffu) == len) {
+            const uint8_t *o = reinterpret_cast<const uint8_t *>(static_cast<uintptr_t>(cur & 0xffffffffffffull));
+            bool eq = true;
+            for (uint32_t i = 0; i < len && eq; ++i) eq = __ldg(o + i) == __ldg(b + i);
+            if (eq) break;
+        }
+        s = (s + 1) & w.slot_mask;
+    }
+    return w.slot_id[s];
+}
+
+// one surviving row's value into its key's accumulator: 128-bit sum by limbs (each add carries against the value it replaced,
+// so the total is exact in any order), integer min / max, count
+__device__ __forceinline__ void wide_add(WideSmem *ws, uint32_t k, int64_t v, uint32_t need) {
+    if (need & 1u) {
+        const unsigned long long uv = static_cast<unsigned long long>(v);
+        const unsigned long long old = atomicAdd(&ws->u.s.lo[k], uv);
+        const long long hinc = (v >> 63) + (old + uv < old ? 1 : 0);
+        if (hinc) atomicAdd(reinterpret_cast<unsigned long long *>(&ws->u.s.hi[k]), static_cast<unsigned long long>(hinc));
+    }
+    if (need & 2u) {
+        atomicMin(&ws->mn[k], static_cast<long long>(v));
+        atomicMax(&ws->mx[k], static_cast<long long>(v));
+    }
+    atomicAdd(&ws->cnt[k], 1u);
+}
+struct WideAggCons {
+    WideSmem *ws;
+    const uint32_t *mask;
+    uint32_t need;
+    __device__ __forceinline__ void operator()(uint32_t row, int64_t v) {
+        if (row < kMaskWords * 32 && ((mask[row >> 5] >> (row & 31)) & 1u)) wide_add(ws, ws->kidx[row], v, need);
+    }
+};
+
+__global__ void __launch_bounds__(kWideWarps * 32) scan_keyed_wide_kernel(const __grid_constant__ ScanParams p, const __grid_constant__ WideScanParams w) {
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    WarpSmem *sm = reinterpret_cast<WarpSmem *>(smem_raw) + warp;
+    WideSmem *ws = reinterpret_cast<WideSmem *>(smem_raw + sizeof(WarpSmem) * kWideWarps) + warp;
+    if (lane == 0) {
+        sm->fault = 0;
+        sm->seq = 0;
+        sm->st_rows = sm->st_matched = sm->st_bytes = 0;
+        sm->st_blocks = 0;
+        for (int s = 0; s < kStages; ++s) mbar_init(&sm->bar[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    uint32_t known_types = 0;
+    const size_t rec_bytes = wide_record_bytes(p.n_fcols);
+    const uint32_t n_warps = gridDim.x * kWideWarps;
+    for (uint32_t g = blockIdx.x * kWideWarps + warp; g < p.total_blocks; g += n_warps) {
+        uint32_t pi = 0;
+        while (pi + 1 < p.n_parts && g >= p.parts[pi + 1].block_base) ++pi;
+        const DevPartRef &part = p.parts[pi];
+        const DevBlock blk = part.blocks[g - part.block_base];
+        int32_t qi;
+        if (!select_block(p.q_sids, p.n_series, p.tmin, p.tmax, blk, qi)) continue;
+        const uint32_t count = blk.count;
+        uint32_t page_bytes = 0;
+        uint32_t err = count > kMaskWords * 32 ? static_cast<uint32_t>(kErrBigBlock) : static_cast<uint32_t>(kErrNone);
+
+        // ---- 1. time range -> rows [r0,r1]: scan_blocks_kernel's general-lane step 1, kept in step with it
+        uint32_t r0 = 0, r1 = count - 1;
+        bool empty = false;
+        if (err == kErrNone && (p.tmin > blk.ts_min || p.tmax < blk.ts_max)) {
+            const uint8_t *tsp = part.files[0] + blk.ts_off;
+            if (blk.ts_enc == 2) {
+                int64_t d = 0;
+                uint32_t used = 0;
+                if (!read_varint_seq(tsp, blk.ver_off, d, used) || used != blk.ver_off || d <= 0) {
+                    err = kErrCorrupt;
+                } else {
+                    const uint64_t ud = static_cast<uint64_t>(d);
+                    if (p.tmin > blk.ts_min) {
+                        const uint64_t q = (static_cast<uint64_t>(p.tmin) - static_cast<uint64_t>(blk.ts_min) + ud - 1) / ud;
+                        r0 = q > count ? count : static_cast<uint32_t>(q);
+                    }
+                    if (p.tmax < blk.ts_max) {
+                        const uint64_t q = (static_cast<uint64_t>(p.tmax) - static_cast<uint64_t>(blk.ts_min)) / ud;
+                        r1 = q >= count ? count - 1 : static_cast<uint32_t>(q);
+                    }
+                    empty = r0 > r1;
+                }
+                page_bytes += blk.ver_off;
+            } else if (blk.ts_enc != 1) {
+                TsCons tc;
+                tc.tmin = p.tmin;
+                tc.tmax = p.tmax;
+                tc.lt = 0;
+                tc.le = 0;
+                bool ok;
+                if (blk.ts_enc == 3) ok = decode_varint_page<false>(sm, tsp, blk.ver_off, count, blk.ts_min, tc, lane);
+                else ok = decode_varint_page<true>(sm, tsp, blk.ver_off, count, blk.ts_min, tc, lane);
+                if (!__all_sync(0xffffffffu, ok)) err = kErrCorrupt;
+                uint32_t lt = __reduce_add_sync(0xffffffffu, tc.lt), le = __reduce_add_sync(0xffffffffu, tc.le);
+                r0 = lt;
+                if (le == 0 || lt >= le) empty = true;
+                else r1 = le - 1;
+                page_bytes += blk.ver_off;
+            }
+        }
+
+        // ---- 2. tag predicates -> row mask: scan_blocks_kernel's general-lane step 2 (no defer, no dedup), the range folded in
+        const uint32_t nwords = (count + 31) >> 5;
+        if (err == kErrNone) {
+            for (uint32_t wd = lane; wd < kMaskWords; wd += 32) {
+                uint32_t v = 0;
+                if (wd < nwords && !empty) v = (wd == nwords - 1 && (count & 31)) ? ((1u << (count & 31)) - 1u) : 0xffffffffu;
+                sm->mask[wd] = v;
+            }
+            __syncwarp();
+        }
+        for (uint32_t pi2 = 0; pi2 < p.n_preds && err == kErrNone && !empty; ++pi2) {
+            const DevPred &pr = p.preds[pi2];
+            DevCol col;
+            if (!find_col(part, blk, pr.name_id, col, lane)) {
+                if (!cmp_op(pr.op, false, 0)) warp_clear_range(sm->mask, 0, count, lane);
+                __syncwarp();
+                continue;
+            }
+            const uint8_t *page = part.files[col.file_id] + col.off;
+            page_bytes += col.size;
+            if (col.size < 1) {
+                err = kErrCorrupt;
+                break;
+            }
+            const uint32_t enc = __ldg(page);
+            if (pr.value_type == BYDB_VT_INT64) {
+                if (col.value_type != BYDB_VT_INT64) {
+                    err = kErrPredType;
+                } else if (enc == kEncRawCells) {
+                    // a nil raw cell compares as absent
+                    if (col.size < 8 + 9ull * count || (reinterpret_cast<uintptr_t>(page) & 7)) {
+                        err = kErrCorrupt;
+                    } else {
+                        const bool nulls = __ldg(page + 1) != 0;
+                        const long long *vals = reinterpret_cast<const long long *>(page + 8);
+                        const uint8_t *valid = page + 8 + 8ull * count;
+                        for (uint32_t row = lane; row < count; row += 32) {
+                            const bool hv = !nulls || __ldg(valid + row) != 0;
+                            const int64_t v = __ldg(vals + row);
+                            const int c = v < pr.lit_i64 ? -1 : (v > pr.lit_i64 ? 1 : 0);
+                            if (!cmp_op(pr.op, hv, c)) atomicAnd(&sm->mask[row >> 5], ~(1u << (row & 31)));
+                        }
+                    }
+                } else {
+                    CmpCons cc;
+                    cc.lit = pr.lit_i64;
+                    cc.op = pr.op;
+                    cc.mask = sm->mask;
+                    cc.limit = count;
+                    err = key_i64_rows(sm, page, col.size, count, cc, lane);
+                }
+            } else {
+                if (col.value_type != BYDB_VT_STR && col.value_type != BYDB_VT_BINARY) err = kErrPredType;
+                else if (enc == 9) err = apply_plain_pred(sm, pr, page + 1, col.size - 1, count, lane);
+                else if (enc != 10) err = kErrBadEnc;
+                else err = apply_dict_pred(sm, pr, page + 1, col.size - 1, count, lane);
+                err = __reduce_max_sync(0xffffffffu, err);
+            }
+            __syncwarp();
+        }
+        uint32_t rows = 0;
+        if (err == kErrNone) {
+            if (!empty) {
+                warp_clear_range(sm->mask, 0, r0, lane);
+                warp_clear_range(sm->mask, r1 + 1, count, lane);
+            }
+            __syncwarp();
+            uint32_t c = 0;
+            for (uint32_t wd = lane; wd < nwords; wd += 32) c += __popc(sm->mask[wd]);
+            rows = __reduce_add_sync(0xffffffffu, c);
+        }
+
+        // ---- 3. the key column -> block-local index per row, then rows and first row per local key
+        if (err == kErrNone) {
+            DevCol kcol;
+            if (find_col(part, blk, w.key_name, kcol, lane)) page_bytes += kcol.size;
+            err = wide_block_keys<true>(sm, ws, part, blk, w.key_name, w.int64_key != 0, lane);
+        }
+        const uint32_t n_local = err == kErrNone ? ws->n_local : 0u;
+        for (uint32_t k = lane; k < n_local; k += 32) {
+            ws->gid[k] = wide_key_id(w, ws->dense[k]);
+            ws->krows[k] = 0;
+            ws->kfirst[k] = 0xffffffffu;
+        }
+        __syncwarp();
+        if (rows > 0 && n_local > 0) {
+            for (uint32_t wd = lane; wd < nwords; wd += 32) {
+                uint32_t m = sm->mask[wd];
+                while (m) {
+                    const uint32_t row = wd * 32 + __ffs(m) - 1;
+                    m &= m - 1;
+                    const uint32_t k = ws->kidx[row];
+                    atomicAdd(&ws->krows[k], 1u);
+                    atomicMin(&ws->kfirst[k], row);
+                }
+            }
+        }
+        __syncwarp();
+        // a present key's record position: its rank by first row among the block's present keys
+        uint32_t n_present = 0;
+        for (uint32_t k = lane; k < n_local; k += 32) {
+            const uint32_t f = ws->kfirst[k];
+            uint32_t r = 0;
+            if (ws->krows[k] > 0)
+                for (uint32_t k2 = 0; k2 < n_local; ++k2) r += ws->krows[k2] > 0 && ws->kfirst[k2] < f ? 1u : 0u;
+            ws->rank[k] = r;
+            n_present += ws->krows[k] > 0 ? 1u : 0u;
+        }
+        n_present = __reduce_add_sync(0xffffffffu, n_present);
+        __syncwarp();
+        uint8_t *rec0 = w.records + static_cast<size_t>(w.rec_off[w.rank[g]]) * rec_bytes;
+
+        // ---- 4. field pages -> per (block, local key) partial aggregates
+        for (uint32_t c = 0; c < p.n_fcols && n_present > 0; ++c) {
+            DevCol col;
+            const bool have = err == kErrNone && find_col(part, blk, p.fcol_name[c], col, lane);
+            bool is_float = false, raw = false;
+            int exp = 0;
+            if (have) {
+                is_float = col.value_type == BYDB_VT_FLOAT64;
+                if (!is_float && col.value_type != BYDB_VT_INT64) err = kErrTypeMix;
+                else if (!check_col_type(p, c, col.value_type, known_types)) err = kErrTypeMix;
+            }
+            if (have && err == kErrNone) {
+                for (uint32_t k = lane; k < n_local; k += 32) {
+                    ws->u.s.lo[k] = 0;
+                    ws->u.s.hi[k] = 0;
+                    ws->mn[k] = INT64_MAX;  // integer extremes: decimal mantissas use the whole int64 range
+                    ws->mx[k] = INT64_MIN;
+                    ws->cnt[k] = 0;
+                }
+                __syncwarp();
+                const uint8_t *page = part.files[col.file_id] + col.off;
+                const uint32_t need = p.fcol_need[c];
+                const uint32_t enc = col.size >= 1 ? __ldg(page) : 0u;
+                if (col.size < 2) {
+                    err = kErrCorrupt;
+                } else if (enc == 9) {
+                    err = kErrPlainPage;
+                } else if (need == 0 && enc != kEncRawCells) {
+                    // COUNT only: numeric pages hold no nulls, so the count is the key's surviving rows
+                    page_bytes += 1;
+                    for (uint32_t k = lane; k < n_local; k += 32) ws->cnt[k] = ws->krows[k];
+                } else if (enc == kEncRawCells) {
+                    // fallback page: one lane in row order (a fixed float summation order)
+                    page_bytes += col.size;
+                    raw = true;
+                    if (col.size < 8 + 9ull * count || (reinterpret_cast<uintptr_t>(page) & 7)) {
+                        err = kErrCorrupt;
+                    } else if (lane == 0) {
+                        if (is_float)  // raw float cells keep double bits in mn / mx: start from the DBL_MAX sentinels
+                            for (uint32_t k = 0; k < n_local; ++k) {
+                                ws->mn[k] = 0x7fefffffffffffffll;
+                                ws->mx[k] = static_cast<long long>(0xffefffffffffffffull);
+                            }
+                        const bool nulls = __ldg(page + 1) != 0;
+                        const long long *vals = reinterpret_cast<const long long *>(page + 8);
+                        const uint8_t *valid = page + 8 + 8ull * count;
+                        for (uint32_t row = 0; row < count; ++row) {
+                            if (!((sm->mask[row >> 5] >> (row & 31)) & 1u) || (nulls && __ldg(valid + row) == 0)) continue;
+                            const uint32_t k = ws->kidx[row];
+                            const long long v = __ldg(vals + row);
+                            if (is_float) {
+                                const double x = __longlong_as_double(v);
+                                ws->u.s.lo[k] = static_cast<unsigned long long>(__double_as_longlong(__longlong_as_double(static_cast<long long>(ws->u.s.lo[k])) + x));
+                                if (x < __longlong_as_double(ws->mn[k])) ws->mn[k] = v;
+                                if (x > __longlong_as_double(ws->mx[k])) ws->mx[k] = v;
+                                ws->cnt[k] += 1;
+                            } else {
+                                wide_add(ws, k, v, 3u);
+                            }
+                        }
+                    }
+                } else {
+                    page_bytes += col.size;
+                    const uint32_t hdr = is_float ? 11u : 9u;
+                    if (col.size < hdr) {
+                        err = kErrCorrupt;
+                    } else {
+                        if (is_float) exp = static_cast<int16_t>((static_cast<uint32_t>(__ldg(page + 1)) << 8) | __ldg(page + 2));
+                        const int64_t first = conv_bytes_to_int64(page + hdr - 8);
+                        const uint8_t *body = page + hdr;
+                        const uint32_t blen = col.size - hdr;
+                        WideAggCons cons{ws, sm->mask, need};
+                        if (enc == 1 || enc == 2) {
+                            int64_t d = 0;
+                            uint32_t used = 0;
+                            if (enc == 1 && blen != 0) err = kErrCorrupt;
+                            if (enc == 2 && (!read_varint_seq(body, blen, d, used) || used != blen)) err = kErrCorrupt;
+                            if (err == kErrNone)
+                                for (uint32_t row = lane; row < count; row += 32)
+                                    cons(row, static_cast<int64_t>(static_cast<uint64_t>(first) + static_cast<uint64_t>(d) * row));
+                        } else if (enc == 3 || enc == 4) {
+                            bool ok;
+                            if (enc == 3) ok = decode_varint_page<false>(sm, body, blen, count, first, cons, lane);
+                            else ok = decode_varint_page<true>(sm, body, blen, count, first, cons, lane);
+                            if (!__all_sync(0xffffffffu, ok)) err = kErrCorrupt;
+                            else if (sm->fault) err = kErrTmaTimeout;
+                        } else {
+                            err = kErrBadEnc;
+                        }
+                    }
+                }
+            }
+            err = __reduce_max_sync(0xffffffffu, err);
+            __syncwarp();
+            // the records' partials of field c (a present key that met the column: mn.i = 1 until values replace it)
+            for (uint32_t k = lane; k < n_local; k += 32) {
+                if (ws->krows[k] == 0) continue;
+                BlockPartial bp;
+                bp.sum.i = 0;
+                bp.mn.i = have ? 1 : 0;
+                bp.mx.i = 0;
+                bp.cnt = 0;
+                const uint32_t n = ws->cnt[k];
+                if (have && err == kErrNone && n > 0) {
+                    bp.cnt = n;
+                    const unsigned long long lo = ws->u.s.lo[k];
+                    const long long hi = ws->u.s.hi[k];
+                    if (is_float && raw) {
+                        bp.sum.f = __longlong_as_double(static_cast<long long>(lo));
+                        bp.mn.f = __longlong_as_double(ws->mn[k]);
+                        bp.mx.f = __longlong_as_double(ws->mx[k]);
+                    } else if (is_float) {
+                        double s;
+                        if (hi == (static_cast<long long>(lo) >> 63)) s = __ll2double_rn(static_cast<long long>(lo));
+                        else s = __ll2double_rn(hi) * 18446744073709551616.0 + __ull2double_rn(lo);
+                        bp.sum.f = scale_decimal(s, exp);
+                        bp.mn.f = scale_decimal(__ll2double_rn(ws->mn[k]), exp);
+                        bp.mx.f = scale_decimal(__ll2double_rn(ws->mx[k]), exp);
+                    } else {
+                        bp.sum.i = static_cast<int64_t>(lo);
+                        bp.mn.i = ws->mn[k];
+                        bp.mx.i = ws->mx[k];
+                    }
+                }
+                reinterpret_cast<BlockPartial *>(rec0 + static_cast<size_t>(ws->rank[k]) * rec_bytes + 16)[c] = bp;
+            }
+            __syncwarp();
+        }
+        if (sm->fault) err = kErrTmaTimeout;
+        if (err != kErrNone) {
+            set_err(p, err, g, lane);
+            rows = 0;
+        }
+        // record headers: the present keys at their rank, the block's remaining records empty
+        for (uint32_t k = lane; k < n_local; k += 32) {
+            uint32_t *h = reinterpret_cast<uint32_t *>(rec0 + static_cast<size_t>(k) * rec_bytes);
+            if (k >= n_present || err != kErrNone) h[2] = 0;
+            if (ws->krows[k] > 0 && err == kErrNone) {
+                uint32_t *hk = reinterpret_cast<uint32_t *>(rec0 + static_cast<size_t>(ws->rank[k]) * rec_bytes);
+                hk[0] = ws->gid[k];
+                hk[1] = ws->kfirst[k];
+                hk[2] = ws->krows[k];
+                hk[3] = static_cast<uint32_t>(w.series_group[qi]);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) {
+            sm->st_rows += count;
+            sm->st_matched += rows;
+            sm->st_bytes += page_bytes;
+            sm->st_blocks += 1;
+        }
+    }
+    if (lane == 0 && sm->st_blocks) {
+        atomicAdd(&p.stats[0], sm->st_rows);
+        atomicAdd(&p.stats[1], sm->st_matched);
+        atomicAdd(&p.stats[2], sm->st_bytes);
+        atomicAdd(&p.stats[3], static_cast<unsigned long long>(sm->st_blocks));
+    }
+}
+
+void launch_scan_keyed_wide(const ScanParams &p, const WideScanParams &w, int grid, cudaStream_t s) {
+    const size_t smem = wide_smem_bytes();
+    cudaFuncSetAttribute(scan_keyed_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (p.total_blocks) scan_keyed_wide_kernel<<<grid, kWideWarps * 32, smem, s>>>(p, w);
+}
+int scan_keyed_wide_ctas_per_sm() {
+    const size_t smem = wide_smem_bytes();
+    cudaFuncSetAttribute(scan_keyed_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, scan_keyed_wide_kernel, kWideWarps * 32, smem) != cudaSuccess || n < 1) n = 1;
+    return n;
+}
+
+// ---- 3. composite groups
+__device__ __forceinline__ const uint32_t *wide_header(const WideReduceParams &p, uint32_t r) {
+    return reinterpret_cast<const uint32_t *>(p.records + static_cast<size_t>(r) * wide_record_bytes(p.n_fcols));
+}
+__global__ void wide_comp_kernel(const __grid_constant__ WideReduceParams p) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= p.n_records) return;
+    const uint32_t *h = wide_header(p, r);
+    if (h[2] == 0) {
+        p.rec_slot[r] = 0xffffffffu;
+        return;
+    }
+    const unsigned long long key = ((static_cast<unsigned long long>(h[3]) << 32) | h[0]) + 1ull;
+    uint32_t s = key_slot_i64(key, p.comp_mask);
+    for (;;) {
+        unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.comp[s]);
+        if (cur == 0ull) cur = atomicCAS(&p.comp[s], 0ull, key);
+        if (cur == 0ull || cur == key) break;
+        s = (s + 1) & p.comp_mask;  // the table has twice the records' slots: a free one is always ahead
+    }
+    atomicMin(&p.comp_min[s], r);
+    p.rec_slot[r] = s;
+    atomicAdd(&p.ctl[0], 1u);
+}
+__global__ void wide_keys_kernel(const __grid_constant__ WideReduceParams p) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.n_sort) return;
+    const uint32_t s = i < p.n_records ? p.rec_slot[i] : 0xffffffffu;
+    p.keys[i] = s == 0xffffffffu ? ~0ull : (static_cast<unsigned long long>(p.comp_min[s]) << 32) | i;
+}
+// bitonic sort of n_sort keys: 2048-key tiles in shared memory for the strides below 2048, a global step for the others
+__global__ void __launch_bounds__(1024) bitonic_tile_kernel(unsigned long long *keys, uint32_t size_lo, uint32_t size_hi) {
+    __shared__ unsigned long long s[2048];
+    const uint32_t base = blockIdx.x * 2048u, t = threadIdx.x;
+    s[t] = keys[base + t];
+    s[t + 1024] = keys[base + t + 1024];
+    __syncthreads();
+    for (uint32_t size = size_lo; size <= size_hi; size <<= 1) {
+        for (uint32_t j = min(size >> 1, 1024u); j > 0; j >>= 1) {
+            const uint32_t i = 2 * t - (t & (j - 1)), ixj = i + j;
+            const bool asc = ((base + i) & size) == 0;
+            const unsigned long long a = s[i], b = s[ixj];
+            if ((a > b) == asc) {
+                s[i] = b;
+                s[ixj] = a;
+            }
+            __syncthreads();
+        }
+    }
+    keys[base + t] = s[t];
+    keys[base + t + 1024] = s[t + 1024];
+}
+__global__ void bitonic_step_kernel(unsigned long long *keys, uint32_t j, uint32_t size, uint32_t n_half) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_half) return;
+    const uint32_t i = 2 * t - (t & (j - 1)), ixj = i + j;
+    const bool asc = (i & size) == 0;
+    const unsigned long long a = keys[i], b = keys[ixj];
+    if ((a > b) == asc) {
+        keys[i] = b;
+        keys[ixj] = a;
+    }
+}
+__global__ void wide_heads_kernel(const __grid_constant__ WideReduceParams p) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.n_sort) return;
+    const unsigned long long k = p.keys[i];
+    p.heads[i] = k != ~0ull && (i == 0 || (p.keys[i - 1] >> 32) != (k >> 32)) ? 1u : 0u;
+}
+// exclusive scan of heads in place, tile by tile: ctl[1] = the total
+__global__ void __launch_bounds__(1024) scan_tiles_kernel(uint32_t *v, uint32_t *tile_sums) {
+    __shared__ uint32_t warp_tot[32];
+    const uint32_t i = blockIdx.x * 1024u + threadIdx.x;
+    uint32_t total = 0;
+    const uint32_t x = block_excl_scan(v[i], warp_tot, total);
+    v[i] = x;
+    if (threadIdx.x == 0) tile_sums[blockIdx.x] = total;
+}
+__global__ void __launch_bounds__(1024) scan_sums_kernel(uint32_t *tile_sums, uint32_t n, uint32_t *total_out) {
+    __shared__ uint32_t warp_tot[32];
+    uint32_t carry = 0;
+    for (uint32_t b = 0; b < n; b += 1024) {
+        const uint32_t i = b + threadIdx.x;
+        uint32_t total = 0;
+        const uint32_t x = block_excl_scan(i < n ? tile_sums[i] : 0u, warp_tot, total);
+        if (i < n) tile_sums[i] = carry + x;
+        carry += total;
+    }
+    if (threadIdx.x == 0) *total_out = carry;
+}
+__global__ void scan_add_kernel(uint32_t *v, const uint32_t *tile_sums) { v[blockIdx.x * 1024u + threadIdx.x] += tile_sums[blockIdx.x]; }
+__global__ void wide_seg_kernel(const __grid_constant__ WideReduceParams p) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.n_sort) return;
+    const unsigned long long k = p.keys[i];
+    if (k != ~0ull && (i == 0 || (p.keys[i - 1] >> 32) != (k >> 32))) p.seg_start[p.heads[i]] = i;
+}
+
+void launch_excl_scan(uint32_t *v, uint32_t n, uint32_t *tile_sums, uint32_t *total, cudaStream_t s) {
+    if (n == 0) return;
+    scan_tiles_kernel<<<n / 1024, 1024, 0, s>>>(v, tile_sums);
+    scan_sums_kernel<<<1, 1024, 0, s>>>(tile_sums, n / 1024, total);
+    scan_add_kernel<<<n / 1024, 1024, 0, s>>>(v, tile_sums);
+}
+
+void launch_wide_order(const WideReduceParams &p, cudaStream_t s) {
+    const uint32_t R = p.n_records, N = p.n_sort;
+    if (R) wide_comp_kernel<<<(R + 255) / 256, 256, 0, s>>>(p);
+    wide_keys_kernel<<<N / 256, 256, 0, s>>>(p);
+    bitonic_tile_kernel<<<N / 2048, 1024, 0, s>>>(p.keys, 2, 2048);
+    for (uint32_t size = 4096; size <= N; size <<= 1) {
+        for (uint32_t j = size >> 1; j >= 2048; j >>= 1) bitonic_step_kernel<<<N / 2 / 256, 256, 0, s>>>(p.keys, j, size, N / 2);
+        bitonic_tile_kernel<<<N / 2048, 1024, 0, s>>>(p.keys, size, size);
+    }
+    wide_heads_kernel<<<N / 256, 256, 0, s>>>(p);
+    launch_excl_scan(p.heads, N, p.tile_sums, &p.ctl[1], s);
+    wide_seg_kernel<<<N / 256, 256, 0, s>>>(p);
+}
+
+// one warp per composite group j: its records in scan order, lane-strided, then a fixed xor tree (group_reduce_small's), into
+// row j of the table
+__global__ void __launch_bounds__(256) wide_fold_kernel(const __grid_constant__ WideReduceParams p, uint32_t n_comp) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (blockIdx.x == 0 && threadIdx.x < p.n_fcols)
+        p.table.coltype[threadIdx.x] = static_cast<int64_t>(p.col_type[threadIdx.x]) | (static_cast<int64_t>(*p.scan_err) << 8);
+    if (j >= n_comp) return;
+    const uint32_t lo = p.seg_start[j], hi = j + 1 < n_comp ? p.seg_start[j + 1] : p.ctl[0];
+    const size_t rec_bytes = wide_record_bytes(p.n_fcols);
+    if (lane == 0) {
+        const uint32_t *h = wide_header(p, static_cast<uint32_t>(p.keys[lo]));
+        p.pairs[2 * static_cast<size_t>(j)] = static_cast<int32_t>(h[3]);
+        p.pairs[2 * static_cast<size_t>(j) + 1] = static_cast<int32_t>(h[0]);
+        p.perm[j] = static_cast<int32_t>(j);
+    }
+    int64_t rows = 0;
+    for (uint32_t i = lo + lane; i < hi; i += 32) rows += wide_header(p, static_cast<uint32_t>(p.keys[i]))[2];
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) rows += static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(rows), m));
+    if (lane == 0) p.table.rows[j] = rows;
+    for (uint32_t c = 0; c < p.n_fcols; ++c) {
+        const bool is_float = p.col_type[c] == BYDB_VT_FLOAT64;
+        BlockPartial acc;
+        acc.sum.i = 0;
+        acc.mn.i = 0;
+        acc.mx.i = 0;
+        acc.cnt = 0;
+        for (uint32_t i = lo + lane; i < hi; i += 32)
+            combine(acc, reinterpret_cast<const BlockPartial *>(p.records + static_cast<size_t>(static_cast<uint32_t>(p.keys[i])) * rec_bytes + 16)[c], is_float);
+#pragma unroll
+        for (int m = 16; m >= 1; m >>= 1) {
+            BlockPartial o;
+            o.sum.i = static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(acc.sum.i), m));
+            o.mn.i = static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(acc.mn.i), m));
+            o.mx.i = static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(acc.mx.i), m));
+            o.cnt = static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(acc.cnt), m));
+            BlockPartial a = (lane & m) ? o : acc, b = (lane & m) ? acc : o;
+            combine(a, b, is_float);
+            acc = a;
+        }
+        if (lane == 0) {
+            const BlockPartial &t = acc;
+            const size_t o = static_cast<size_t>(j) * p.n_fcols + c;
+            const bool have = t.cnt > 0;
+            const bool met = !have && t.mn.i != 0;  // met_column: the other type's maximum word carries it
+            p.table.cnt[o] = t.cnt;
+            p.table.sum_f64[o] = (have && is_float) ? t.sum.f : 0.0;
+            p.table.max_f64[o] = (have && is_float) ? t.mx.f : (met && !is_float) ? 0.0 : -INFINITY;
+            p.table.negmin_f64[o] = (have && is_float) ? -t.mn.f : -INFINITY;
+            p.table.sum_i64[o] = (have && !is_float) ? t.sum.i : 0;
+            p.table.max_i64[o] = (have && !is_float) ? t.mx.i : (met && is_float) ? 0 : INT64_MIN;
+            p.table.notmin_i64[o] = (have && !is_float) ? ~t.mn.i : INT64_MIN;
+        }
+    }
+}
+
+void launch_wide_fold(const WideReduceParams &p, uint32_t n_comp, cudaStream_t s) {
+    const uint32_t warps = n_comp > 0 ? n_comp : 1u;
+    wide_fold_kernel<<<(warps + 7) / 8, 256, 0, s>>>(p, n_comp);
 }
 
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s) {

@@ -62,6 +62,7 @@ enum DevErr : uint32_t {
     kErrKeyCap = 12,        // per-row group key: more distinct values than the caller's max_values
     kErrKeyLong = 13,       // per-row group key: a value longer than kMaxLit bytes
     kErrRankOverlap = 14,   // keyed collective: one series on two ranks over time spans that intersect
+    kErrKeyBlock = 15,      // wide group key: a block whose key column holds more than kMaxBlockKeys distinct values
 };
 constexpr int kOpEqOrNil = 7;  // internal predicate operator of the group-key passes: the cell is nil or equals the literal
 constexpr uint32_t kKeyAbsent = 0xffffffffu;  // Krow of a series that never shows the value (a block's first row is below it)
@@ -233,6 +234,7 @@ struct KeyParams {
 };
 // int64_key: the key tag is an int64 column (key_values_i64_kernel), else a dictionary string tag (key_values_kernel)
 void launch_key_values(const KeyParams &p, bool int64_key, int grid, cudaStream_t s);
+
 struct KeyOrderParams {
     int32_t n_groups;             // G: groups of series
     uint32_t n_values;            // V
@@ -278,6 +280,66 @@ struct TableLayout {
                          reinterpret_cast<int64_t *>(base + off_coltype)};
     }
 };
+
+// ---- one-pass group key (bydb_scan_agg_keyed_wide): see "Wide group key" in scan_kernels.cu
+constexpr uint32_t kMaxWideKeyValues = 65536;
+constexpr uint32_t kMaxBlockKeys = 256;  // distinct key values of one block (a block-local index is one byte)
+// the value table of a wide key: slots as KeyParams::slots, slot_mask + 1 of them (a power of two, at least twice the cap)
+struct WideKeyParams {
+    KeyParams k;                  // k.vals / k.lens: [cap] packed by key_pack_wide_kernel in id order
+    uint32_t slot_mask;
+    uint32_t int64_key;
+    uint32_t *slot_id;            // [slot_mask + 1] id of the value in an occupied slot (int64 key: the value 0, if it occurs, is id 0)
+    uint32_t *n_by_rank;          // [total_blocks] distinct values of the selected block of that scan-order rank, else 0
+    uint32_t *rank;               // [total_blocks] scan-order rank of a selected block: (series, time) over every part
+};
+// discovery (one warp per selected block) and the numbering of the values; *k.count = distinct values
+void launch_key_values_wide(const WideKeyParams &p, int grid, cudaStream_t s);
+// exclusive prefix sum of v[0, n) in place (n a multiple of 1024), tile_sums [n / 1024], *total = the sum
+void launch_excl_scan(uint32_t *v, uint32_t n, uint32_t *tile_sums, uint32_t *total, cudaStream_t s);
+// A record per (selected block, block-local key value that a surviving row shows), in scan order: the blocks by rank, a block's
+// records by their first surviving row.  [u32 value id | u32 first row | u32 rows | i32 series group] then F BlockPartial.
+__host__ __device__ __forceinline__ size_t wide_record_bytes(size_t F) { return 16 + sizeof(BlockPartial) * F; }
+struct WideScanParams {
+    const unsigned long long *slots;
+    const uint32_t *slot_id;
+    const uint32_t *zero;         // int64 key: the value 0 occurs (id 0)
+    uint32_t slot_mask, int64_key;
+    uint16_t key_name;
+    uint16_t pad[3];
+    const uint32_t *rank;         // WideKeyParams::rank
+    const uint32_t *rec_off;      // [total_blocks] first record of the block of that rank (exclusive scan of n_by_rank)
+    const int32_t *series_group;  // [n_series]
+    uint8_t *records;             // [R * wide_record_bytes(F)]
+};
+// ScanParams supplies the parts, the selection, the predicates, the fields, the column types, err and stats (the plain scan's
+// counters: rows_scanned, rows_matched, page_bytes, blocks)
+void launch_scan_keyed_wide(const ScanParams &p, const WideScanParams &w, int grid, cudaStream_t s);
+int scan_keyed_wide_ctas_per_sm();
+// the records folded into a partial table of the present composite groups (series group, value id) in insertion order
+struct WideReduceParams {
+    const uint8_t *records;
+    uint32_t n_records, n_fcols;  // R, F
+    unsigned long long *comp;     // [comp_mask + 1] composite (series group << 32 | value id) + 1, 0 = empty
+    uint32_t *comp_min;           // [comp_mask + 1] lowest record of the composite, preset 0xffffffff
+    uint32_t *rec_slot;           // [R] composite slot of a record with rows > 0, else 0xffffffff
+    uint32_t comp_mask;
+    uint32_t n_sort;              // power of two >= max(R, 2048)
+    unsigned long long *keys;     // [n_sort] min record of the composite << 32 | record; ~0 = no rows
+    uint32_t *heads;              // [n_sort] 1 = first record of a composite, then (exclusive scan) the composite's index
+    uint32_t *tile_sums;          // [n_sort / 1024 + 1]
+    uint32_t *ctl;                // [0] records with rows [1] composite groups N_c
+    uint32_t *seg_start;          // [R] first sorted record of composite j
+    const int32_t *col_type;      // [F] the scan's column types
+    const uint32_t *scan_err;     // the scan's DevErr (carried in the table's coltype words)
+    TablePtrs table;              // TableLayout(N_c, F)
+    int32_t *pairs;               // [2 N_c] series group, value id of composite j
+    int32_t *perm;                // [N_c] j (the identity order keyed_partial_rows_kernel reads)
+};
+// composite slots, sort keys, the sort, the heads and their scan: ctl[1] = N_c afterwards
+void launch_wide_order(const WideReduceParams &p, cudaStream_t s);
+// the fold into p.table / pairs / perm (p.table sized for ctl[1] groups)
+void launch_wide_fold(const WideReduceParams &p, uint32_t n_comp, cudaStream_t s);
 
 // The Partial a data node ships for aggregate `func` of one group of a partial table, word o = group * F + field (emitPartial,
 // measure_plan_aggregation.go:67-84; aggregation.PartialToFieldValues): SUM the sum, COUNT the count, MEAN the sum with the count as

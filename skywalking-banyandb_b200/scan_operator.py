@@ -117,7 +117,8 @@ class ScanSpec:
     # ^ orderBy sort of the request: the scan visits the series list backwards, so groups are numbered (and non-key
     #   projected tags take their first-seen value) from the far end -- aggregation.go:211-213 on a reversed stream
     max_key_values: int = 0
-    # ^ distinct values a stored-tag GroupBy key may take over the query (bydb_group_key.max_values; 0 = the library's 64)
+    # ^ distinct values a stored-tag GroupBy key may take over the query (bydb_group_key.max_values; 0 = the library's 64):
+    #   up to 256 the per-value passes of scan_agg_keyed answer, up to 65,536 the one pass of scan_agg_keyed_wide
 
 
 def _key_cell(t: ColumnType, k: bytes):
@@ -249,7 +250,9 @@ class GPUScanAgg:
         else:
             cdef = self._in.Columns[self._stored_key]
             vt = capi.VT_INT64 if cdef.Type == ColumnType.ColumnTypeInt64 else 0
-            self._result = self._ctx.scan_agg_keyed(q, cdef.TagFamily, cdef.Name, sc.max_key_values, vt)
+            # above the per-value passes' 256 values, the one-pass form (which answers the same rows)
+            keyed = self._ctx.scan_agg_keyed_wide if sc.max_key_values > 256 else self._ctx.scan_agg_keyed
+            self._result = keyed(q, cdef.TagFamily, cdef.Name, sc.max_key_values, vt)
         self.stats = self._result.stats
         # offset / limit window over the (Top-ordered) output rows, limit.go:56-73
         n = len(self._result.group_id)
