@@ -19,6 +19,7 @@
 #include <memory>
 #include <type_traits>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -1038,9 +1039,17 @@ ScanLayout scan_layout(const StageLayout &st, size_t NB, size_t F, size_t n_part
     return sl;
 }
 
-// the query's side of ScanParams: predicates, fields and what each field's aggregations need, the time range
-void scan_query_params(bydb_ctx *ctx, const bydb_query *q, const Plan &plan, ScanParams &sp) {
+// the head of a scan's ScanParams, the rest zeroed: the plan's parts and blocks, the series (their ids at q_sids on the device), and
+// the query's side -- predicates, fields and what each field's aggregations need, the time range
+void scan_params_head(bydb_ctx *ctx, const bydb_query *q, const Plan &plan, const uint64_t *q_sids, ScanParams &sp) {
     const size_t F = plan.fcols.size();
+    memset(&sp, 0, sizeof sp);
+    part_refs(plan.parts, sp.parts);
+    sp.n_parts = static_cast<uint32_t>(plan.parts.size());
+    sp.total_blocks = static_cast<uint32_t>(plan.total_blocks);
+    sp.q_sids = q_sids;
+    sp.n_series = static_cast<uint32_t>(q->n_series);
+    sp.n_fcols = static_cast<uint32_t>(F);
     sp.n_preds = q->n_preds;
     sp.tmin = q->tmin;
     sp.tmax = q->tmax;
@@ -1105,17 +1114,11 @@ int run_scan(bydb_ctx *ctx, const bydb_query *q, Plan &plan, ExecSlot &slot, cud
     }
 
     ScanParams sp;
-    memset(&sp, 0, sizeof sp);
+    scan_params_head(ctx, q, plan, reinterpret_cast<const uint64_t *>(d + off_sids), sp);
     ReduceParams rp;
     memset(&rp, 0, sizeof rp);
-    part_refs(plan.parts, sp.parts);
     std::copy(sp.parts, sp.parts + plan.parts.size(), rp.parts);
-    sp.n_parts = rp.n_parts = static_cast<uint32_t>(plan.parts.size());
-    sp.total_blocks = static_cast<uint32_t>(NB);
-    sp.q_sids = reinterpret_cast<const uint64_t *>(d + off_sids);
-    sp.n_series = static_cast<uint32_t>(NS);
-    sp.n_fcols = static_cast<uint32_t>(F);
-    scan_query_params(ctx, q, plan, sp);
+    rp.n_parts = sp.n_parts;
     sp.worklist = reinterpret_cast<uint32_t *>(d + off_worklist);
     sp.work_count = &z->work_count;
     sp.work_next = &z->work_next;
@@ -1533,6 +1536,7 @@ struct bydb_prepared {
     bydb_stats captured{};             // host-side counters of one step (launch counts, byte counts)
     bool express = false;              // the captured step launches the express lane
     bool partial_step = false;         // the captured step answers with map-phase rows (bydb_scan_partials[_keyed]_prepared)
+    bool empty_step = false;           // a keyed step whose discovery found no value: it holds its parts, needs no graph, answers empty
     uint64_t runs = 0;
     bool capturable = true;
     // the collective form (bydb_scan_reduce_prepared): one captured graph per (root, slot parity)
@@ -1557,6 +1561,7 @@ void drop_step(bydb_prepared *p) {
     if (p->step_state) cudaFree(p->step_state);
     p->step_state = nullptr;
     p->held.clear();
+    p->empty_step = false;
 }
 
 void prepared_destroy(bydb_prepared *p) {
@@ -1606,6 +1611,48 @@ int replay_graph(cudaGraphExec_t exec, ExecSlot &slot, cudaEvent_t t0, cudaEvent
     return read_zero_page(image, express, stats);
 }
 
+// What capture_graph did: `rc` is the failure code of its enqueue (no graph is instantiated then), `err` the runtime's first error,
+// raised by the call `failed` names.
+struct GraphCapture {
+    int rc = 0;
+    cudaError_t err = cudaSuccess;
+    const char *failed = nullptr;
+};
+constexpr const char *kBeginCapture = "begin capture";
+
+// Captures what enqueue() (returning 0 or a code) puts on stream `s` as one graph, instantiated into *exec.  The file's only capture:
+// the stream always leaves capture mode again.
+template <class Enqueue>
+GraphCapture capture_graph(cudaStream_t s, cudaGraphExec_t *exec, Enqueue &&enqueue) {
+    GraphCapture c;
+    c.err = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
+    if (c.err != cudaSuccess) {
+        c.failed = kBeginCapture;
+        return c;
+    }
+    c.rc = enqueue();
+    cudaGraph_t graph = nullptr;
+    c.err = cudaStreamEndCapture(s, &graph);
+    if (c.err != cudaSuccess) c.failed = "end capture";
+    if (!c.rc && c.err == cudaSuccess && graph) {
+        c.err = cudaGraphInstantiate(exec, graph, 0);
+        if (c.err != cudaSuccess) c.failed = "instantiate";
+    }
+    if (graph) cudaGraphDestroy(graph);
+    return c;
+}
+
+// Allocates the step state p->step_state (`bytes`) and uploads the query's staging (layout st) into it at `sids_off`, synchronised: the
+// captured kernels read the staging from there on every replay.  False when the state cannot be had; else `e` is the upload's error.
+bool make_step_state(bydb_prepared *p, size_t bytes, const StageLayout &st, size_t sids_off, cudaError_t &e) {
+    if (cudaMalloc(reinterpret_cast<void **>(&p->step_state), bytes) != cudaSuccess) return false;
+    ExecSlot &slot = *p->slot;
+    stage_series(&p->q, st, slot.pinned);
+    e = cudaMemcpyAsync(p->step_state + sids_off, slot.pinned, st.bytes, cudaMemcpyHostToDevice, slot.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(slot.stream);
+    return true;
+}
+
 // captures one step into p->exec, building the StepState it runs in; returns 0, or a code after leaving the stream out of
 // capture mode.  0 with p->exec == NULL: this query keeps the uncaptured path.  The tail after group_reduce: finalisation, row
 // selection and one read-back copy, or (partial) emit_plain_rows, whose last kernel writes the zero page and the rows to the staging.
@@ -1630,45 +1677,41 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p, bool partial) {
     uint8_t *h_dst = partial ? slot.pinned_dev(p->host_off) : nullptr;
     Carve carve;
     const size_t off_table = carve(tl.total), off_scan = carve(sl.total), off_fin = carve(partial ? rl.total : fl.total + kZeroPageBytes);
-    if ((partial && !h_dst) || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
+    cudaError_t e = cudaSuccess;
+    if ((partial && !h_dst) || !make_step_state(p, carve.o, st, off_scan + sl.off_sids, e)) {
         cudaGetLastError();
         p->step_state = nullptr;
         p->capturable = false;
         return 0;
     }
-    // the staging goes up once: the graph's kernels read it from the step state on every replay
-    stage_series(&p->q, st, slot.pinned);
-    cudaError_t e = cudaMemcpyAsync(p->step_state + off_scan + sl.off_sids, slot.pinned, st.bytes, cudaMemcpyHostToDevice, slot.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(slot.stream);
-    if (e == cudaSuccess) e = cudaStreamBeginCapture(slot.stream, cudaStreamCaptureModeThreadLocal);
-    if (e != cudaSuccess) {
-        drop_step(p);
-        return fail(BYDB_EIO, std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(e));
-    }
-    memset(&p->captured, 0, sizeof p->captured);
     uint32_t fin_launches = 0;
-    Scratch scan, fin;
-    scan.view(p->step_state + off_scan, sl.total);
-    fin.view(p->step_state + off_fin, fl.total + kZeroPageBytes);
-    rc = run_scan(ctx, &p->q, plan, slot, slot.stream, p->step_state + off_table, tl, &p->captured, 0, nullptr, &scan);
-    p->express = slot.express[0];
-    if (!rc && partial) {
-        emit_plain_rows(&p->q, plan, slot.stream, p->step_state + off_table, p->step_state + off_fin, scan.base + sl.off_zero, kZeroPageBytes, h_dst);
-        fin_launches = kPlainRowsLaunches;
-        p->read_back = 0;  // sized by the rows present: the replay counts it
-    } else if (!rc) {
-        rc = finalize_enqueue(&p->q, plan, slot, slot.stream, p->step_state + off_table, tl, p->host_off, fin, p->fl, fin_launches, p->read_back,
-                              scan.base + sl.off_zero);
+    GraphCapture c;
+    if (e == cudaSuccess) c = capture_graph(slot.stream, &p->exec, [&]() -> int {
+        memset(&p->captured, 0, sizeof p->captured);
+        Scratch scan, fin;
+        scan.view(p->step_state + off_scan, sl.total);
+        fin.view(p->step_state + off_fin, fl.total + kZeroPageBytes);
+        rc = run_scan(ctx, &p->q, plan, slot, slot.stream, p->step_state + off_table, tl, &p->captured, 0, nullptr, &scan);
+        p->express = slot.express[0];
+        if (!rc && partial) {
+            emit_plain_rows(&p->q, plan, slot.stream, p->step_state + off_table, p->step_state + off_fin, scan.base + sl.off_zero, kZeroPageBytes, h_dst);
+            fin_launches = kPlainRowsLaunches;
+            p->read_back = 0;  // sized by the rows present: the replay counts it
+        } else if (!rc) {
+            rc = finalize_enqueue(&p->q, plan, slot, slot.stream, p->step_state + off_table, tl, p->host_off, fin, p->fl, fin_launches, p->read_back,
+                                  scan.base + sl.off_zero);
+        }
+        return rc;
+    });
+    if (e != cudaSuccess || c.failed == kBeginCapture) {
+        drop_step(p);
+        return fail(BYDB_EIO, std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(e != cudaSuccess ? e : c.err));
     }
-    cudaGraph_t graph = nullptr;
-    e = cudaStreamEndCapture(slot.stream, &graph);
-    if (!rc && e == cudaSuccess && graph) e = cudaGraphInstantiate(&p->exec, graph, 0);
-    if (graph) cudaGraphDestroy(graph);
-    if (rc || e != cudaSuccess || !p->exec) {
+    if (c.rc || c.err != cudaSuccess || !p->exec) {
         cudaGetLastError();
         drop_step(p);
         p->capturable = false;  // fall back to the uncaptured path for good
-        return rc;
+        return c.rc;
     }
     p->captured.kernel_launches += fin_launches;  // finalize + select_rows (one fused launch for few groups), or the three row kernels
     p->captured.d2h_bytes += p->read_back;
@@ -1679,24 +1722,933 @@ int prepared_capture(bydb_ctx *ctx, bydb_prepared *p, bool partial) {
     return 0;
 }
 
-// Makes p->exec the captured step of the form asked for (partial: map-phase rows), ready to replay: a step of the other form gives
-// way (one step per handle), and a step whose handles stopped naming its parts is captured again.  Returns a code (BYDB_ENOENT: a
-// handle names no part), or 0 with p->exec NULL when this execution takes the uncaptured path.
-int prepared_step(bydb_ctx *ctx, bydb_prepared *p, bool partial) {
+// The schedule of a prepared query: its first execution runs the uncaptured path (which also performs the one-time kernel attribute
+// setup), the second one captures, later ones replay.  Makes the step of the form asked for (partial: map-phase rows) ready to replay,
+// capturing it with capture() when there is none: a step of the other form gives way (one step per handle), and a step whose handles
+// stopped naming its parts is captured again.  Returns a code (BYDB_ENOENT: a handle names no part), or 0 with neither p->exec nor
+// p->empty_step when this execution takes the uncaptured path.
+template <class Capture>
+int prepared_step(bydb_ctx *ctx, bydb_prepared *p, bool partial, Capture &&capture) {
+    if (p->runs++ == 0 || !p->capturable) return 0;
     if (p->exec && p->partial_step != partial) drop_step(p);
-    if (!p->exec) return prepared_capture(ctx, p, partial);
+    if (!p->exec && !p->empty_step) return capture();
     // the handles can only have changed their parts if one was registered or released since `held` was last compared
     const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
     if (gen != p->held_gen) {
         const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
-        if (!p->exec) drop_step(p);  // the state is sized for the parts it was captured with
+        if (!p->exec && p->held.empty()) drop_step(p);  // the state is sized for the parts it was captured with
         if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
         p->held_gen = gen;
-        if (!p->exec) return prepared_capture(ctx, p, partial);
+        if (!p->exec && !p->empty_step) return capture();
     }
     return 0;
 }
 
+struct KeyedOwner {
+    std::vector<int32_t> key_id;
+    std::vector<uint32_t> key_off;
+    std::vector<uint8_t> key_bytes;
+};
+
+// the arrays of a bydb_partial_rows
+struct PartialRowsOwner {
+    std::vector<int32_t> group_id;
+    std::vector<uint8_t> is_float;
+    std::vector<int64_t> val_i64, cnt_i64;
+    std::vector<double> val_f64, cnt_f64;
+};
+
+// one aggregate of a row: the Partial words into the arrays of their type, 0 in the others
+void push_partial(PartialRowsOwner &o, const PartialWords &w, bool is_float) {
+    double vf = 0.0, cf = 0.0;
+    memcpy(&vf, &w.val, 8);
+    memcpy(&cf, &w.cnt, 8);
+    o.val_i64.push_back(is_float ? 0 : static_cast<int64_t>(w.val));
+    o.val_f64.push_back(is_float ? vf : 0.0);
+    o.cnt_i64.push_back(is_float ? 0 : static_cast<int64_t>(w.cnt));
+    o.cnt_f64.push_back(is_float ? cf : 0.0);
+}
+
+// the status the control word of a row image carries: the column types merged over the passes, the worst status with them
+int rows_status(const uint8_t *ctl, size_t F) {
+    const int64_t *ct = reinterpret_cast<const int64_t *>(ctl + 8);
+    uint32_t dev_err = 0;
+    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(ct[c] >> 8));
+    return table_status(dev_err);
+}
+// the rows a row image holds: its n_present, at most max_rows
+size_t rows_in(const uint8_t *ctl, size_t max_rows) { return std::min<size_t>(*reinterpret_cast<const uint32_t *>(ctl), max_rows); }
+
+// a row image read back to the host -- the control word, then the rows right behind it -- into *b, after its status
+int parse_rows(const uint8_t *img, const bydb_query *q, const Plan &plan, size_t max_rows, bydb_partial_rows *b) {
+    const size_t F = plan.fcols.size(), A = q->n_aggs, row_bytes = keyed_row_bytes(A);
+    int rc = rows_status(img, F);
+    if (rc) return rc;
+    const int64_t *ct = reinterpret_cast<const int64_t *>(img + 8);
+    auto ro = std::make_unique<PartialRowsOwner>();
+    ro->is_float.resize(A);
+    for (size_t a = 0; a < A; ++a) ro->is_float[a] = (ct[plan.agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
+    const size_t n = rows_in(img, max_rows);
+    const uint8_t *rows = img + keyed_ctl_bytes(F);
+    ro->group_id.resize(n);
+    for (size_t j = 0; j < n; ++j) {
+        const uint8_t *row = rows + j * row_bytes;
+        memcpy(&ro->group_id[j], row, 4);
+        for (size_t a = 0; a < A; ++a) {
+            PartialWords w;
+            memcpy(&w.val, row + 8 + 8 * a, 8);
+            memcpy(&w.cnt, row + 8 + 8 * (A + a), 8);
+            push_partial(*ro, w, ro->is_float[a] != 0);
+        }
+    }
+    b->n_rows = static_cast<int32_t>(n);
+    b->n_aggs = static_cast<int32_t>(A);
+    b->group_id = ro->group_id.data();
+    b->is_float = ro->is_float.data();
+    b->val_i64 = ro->val_i64.data();
+    b->val_f64 = ro->val_f64.data();
+    b->cnt_i64 = ro->cnt_i64.data();
+    b->cnt_f64 = ro->cnt_f64.data();
+    b->owner = ro.release();
+    return 0;
+}
+
+// bydb_partials_rows over the table at d_table, enqueued on `s`: emit_plain_rows into the slot's staging, synchronised and parsed.
+// stats (when given) count its three kernels and the bytes its copy kernel brought back.
+int partial_rows_to_host(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t s, const uint8_t *d_table, bydb_partial_rows *out,
+                         bydb_stats *stats) {
+    const size_t ctl_bytes = keyed_ctl_bytes(plan.fcols.size()), row_bytes = keyed_row_bytes(q->n_aggs);
+    if (slot.ensure_pinned(ctl_bytes + plan.tl.G * row_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    uint8_t *h_dst = slot.pinned_dev(0);
+    if (!h_dst) return fail(BYDB_EIO, "page-locked staging without a device address");
+    Scratch work;
+    CUDA_TRY(work.alloc(rows_layout(q, plan).total, s));
+    emit_plain_rows(q, plan, s, d_table, work.base, nullptr, 0, h_dst);
+    CUDA_TRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaGetLastError());
+    if (stats) {
+        stats->kernel_launches += kPlainRowsLaunches;
+        stats->d2h_bytes += ctl_bytes + rows_in(slot.pinned, plan.tl.G) * row_bytes;
+    }
+    return parse_rows(slot.pinned, q, plan, plan.tl.G, out);
+}
+
+// the two answers of a keyed call: finalised rows (bydb_keyed_result) or map-phase partial rows (bydb_keyed_partial_rows)
+bydb_stats &keyed_stats(bydb_keyed_result *out) { return out->base.stats; }
+bydb_stats &keyed_stats(bydb_keyed_partial_rows *out) { return out->stats; }
+using KeyValues = std::vector<std::vector<uint8_t>>;
+
+// the checks of a group key that need no device; cap = the distinct values accepted (max_values, 0 = 64), at most max_cap.  A key
+// that runs as an extra predicate of every pass (pred_slot) leaves the query one predicate fewer.
+int check_group_key(const bydb_query *q, const bydb_group_key *key, uint32_t max_cap, bool pred_slot, uint32_t &cap) {
+    if (!key || !key->family || !key->tag) return fail(BYDB_EINVAL, "group key without family/tag");
+    if (key->value_type != 0 && key->value_type != BYDB_VT_STR && key->value_type != BYDB_VT_BINARY && key->value_type != BYDB_VT_INT64)
+        return fail(BYDB_EINVAL, "bydb_group_key.value_type must be 0, BYDB_VT_STR, BYDB_VT_BINARY or BYDB_VT_INT64");
+    cap = key->max_values ? key->max_values : 64u;
+    if (cap > max_cap) return fail(BYDB_EINVAL, "bydb_group_key.max_values above " + std::to_string(max_cap));
+    if (pred_slot && q->n_preds + 1 > kMaxPreds) return fail(BYDB_ENOTSUP, "a group-key query takes at most 7 predicates");
+    return 0;
+}
+
+// The parameters of a key discovery over the plan's blocks, with its device arrays at `base`: the series ids (staged in `pinned` for
+// the caller's upload), the value table, the control word ([0] values [1] DevErr [2] its block [3] int64 zero) and the packed values.
+KeyParams key_params(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, uint8_t *pinned, uint8_t *base,
+                     size_t a_sids, size_t a_slots, size_t a_ctl, size_t a_vals, size_t a_lens) {
+    const size_t NS = q->n_series;
+    if (NS) memcpy(pinned, q->series_ids, NS * 8);
+    KeyParams kp;
+    memset(&kp, 0, sizeof kp);
+    part_refs(plan.parts, kp.parts);
+    kp.n_parts = static_cast<uint32_t>(plan.parts.size());
+    kp.total_blocks = static_cast<uint32_t>(plan.total_blocks);
+    kp.q_sids = reinterpret_cast<const uint64_t *>(base + a_sids);
+    kp.n_series = static_cast<uint32_t>(NS);
+    kp.cap = cap;
+    kp.tmin = q->tmin;
+    kp.tmax = q->tmax;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        kp.key_name = ctx->names.find(std::string("t:") + key->family + "/" + key->tag);
+    }
+    kp.slots = reinterpret_cast<unsigned long long *>(base + a_slots);
+    kp.count = reinterpret_cast<uint32_t *>(base + a_ctl);
+    kp.err = kp.count + 1;
+    kp.zero = kp.count + 3;
+    kp.vals = base + a_vals;
+    kp.lens = reinterpret_cast<uint32_t *>(base + a_lens);
+    return kp;
+}
+
+// the failure a discovery's control word reports (a device error, with the block that raised it), or 0
+int discovery_status(const uint32_t *ctl) {
+    if (ctl[1] == 0) return 0;
+    g_last_dev_err = ctl[1];
+    char buf[64];
+    snprintf(buf, sizeof buf, " (block #%u)", ctl[2]);
+    return fail(dev_err_code(ctl[1]), std::string(dev_err_text(ctl[1])) + buf);
+}
+
+// V packed key values read back to the host: int64 at an 8-byte stride (the reference's key bytes: little-endian int64), or strings
+// at a kMaxLit stride with their lengths
+KeyValues unpack_values(size_t V, bool int64_key, const uint8_t *vals, const uint32_t *lens) {
+    KeyValues values(V);
+    for (size_t v = 0; v < V; ++v) {
+        if (int64_key) values[v].assign(vals + v * 8, vals + v * 8 + 8);
+        else values[v].assign(vals + v * kMaxLit, vals + v * kMaxLit + std::min<uint32_t>(lens[v], kMaxLit));
+    }
+    return values;
+}
+
+// 1. the distinct key values of the selected blocks, on the slot's stream, synchronised
+int discover_keys(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats *stats,
+                  KeyValues &values) {
+    const bool int64_key = key->value_type == BYDB_VT_INT64;
+    const size_t NS = q->n_series;
+    cudaStream_t stream = slot.stream;
+    Carve carve;
+    const size_t a_sids = carve(NS * 8), a_slots = carve(kKeySlots * 8), a_ctl = carve(16), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
+                 a_lens = carve(static_cast<size_t>(cap) * 4);
+    const size_t a_total = carve.o;
+    Scratch ka;
+    CUDA_TRY(ka.alloc(a_total, stream));
+    const size_t back_bytes = a_total - a_ctl;  // ctl | vals | lens come back in one copy
+    if (slot.ensure_pinned(std::max(back_bytes, NS * 8) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    const KeyParams kpar = key_params(ctx, q, key, cap, plan, slot.pinned, ka.base, a_sids, a_slots, a_ctl, a_vals, a_lens);
+    if (NS) CUDA_TRY(cudaMemcpyAsync(ka.base + a_sids, slot.pinned, NS * 8, cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemsetAsync(ka.base + a_slots, 0, a_total - a_slots, stream));
+    launch_key_values(kpar, int64_key, ctx->sm_count * 4, stream);
+    CUDA_TRY(cudaStreamSynchronize(stream));  // the staging of the series ids must be consumed before the read-back reuses it
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, ka.base + a_ctl, back_bytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    stats->kernel_launches += 2;
+    stats->h2d_bytes += NS * 8;
+    stats->d2h_bytes += back_bytes;
+    const uint32_t *ctl = reinterpret_cast<const uint32_t *>(slot.pinned);
+    if (int rc = discovery_status(ctl)) return rc;
+    values = unpack_values(std::min<size_t>(ctl[0], cap), int64_key, slot.pinned + (a_vals - a_ctl),
+                           reinterpret_cast<const uint32_t *>(slot.pinned + (a_lens - a_ctl)));
+    return 0;
+}
+
+// 2. one scan pass per value v (the key as an extra predicate) into slice v of the composite table tlc (V x G groups, value-major)
+// at `table`, with the pass's column types at coltype + v * F and where each series first shows v at kts / krow + v * NS; the
+// first pass also writes the series' spans when `span` is set.  Every pass is synchronised and its device errors collected --
+// unless `resident` is given (a keyed step being captured): then the passes share that scan scratch, pass v keeps its counters
+// and device error in zero page v of `zero_pages` (kZeroPageBytes each) for the step's one read-back, and nothing synchronises.
+int run_keyed_passes(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Plan &plan, ExecSlot &slot, const KeyValues &values,
+                     const TableLayout &tlc, uint8_t *table, int64_t *coltype, int64_t *kts, uint32_t *krow, int64_t *span, bydb_stats *stats,
+                     Scratch *resident = nullptr, uint8_t *zero_pages = nullptr) {
+    const bool int64_key = key->value_type == BYDB_VT_INT64;
+    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
+    std::vector<bydb_pred> preds(q->preds, q->preds + q->n_preds);
+    preds.emplace_back();
+    bydb_query qv = *q;
+    qv.n_preds = q->n_preds + 1;
+    for (size_t v = 0; v < values.size(); ++v) {
+        bydb_pred &kpred = preds.back();
+        memset(&kpred, 0, sizeof kpred);
+        kpred.family = key->family;
+        kpred.tag = key->tag;
+        if (int64_key) {
+            int64_t lit = 0;
+            memcpy(&lit, values[v].data(), 8);
+            kpred.op = lit == 0 ? kOpEqOrNil : BYDB_OP_EQ;  // a nil cell is the column's zero value (typed_column.go:49-53)
+            kpred.value_type = BYDB_VT_INT64;
+            kpred.lit_i64 = lit;
+        } else {
+            kpred.op = values[v].empty() ? kOpEqOrNil : BYDB_OP_EQ;  // a nil cell and "" are the same key (groupby.go:226-254)
+            kpred.value_type = BYDB_VT_STR;
+            kpred.lit = values[v].data();
+            kpred.lit_len = values[v].size();
+        }
+        qv.preds = preds.data();
+        KeyedPass pass;
+        pass.group_off = v * G;
+        pass.coltype = coltype + v * F;
+        pass.kts = kts + v * NS;
+        pass.krow = krow + v * NS;
+        pass.span = v == 0 ? span : nullptr;
+        if (resident) {
+            pass.zero = reinterpret_cast<ZeroPage *>(zero_pages + v * kZeroPageBytes);
+            if (int rc = run_scan(ctx, &qv, plan, slot, slot.stream, table, tlc, stats, 0, &pass, resident)) return rc;
+            continue;
+        }
+        int rc = run_scan(ctx, &qv, plan, slot, slot.stream, table, tlc, stats, 0, &pass);
+        cudaError_t ce = cudaStreamSynchronize(slot.stream);  // also on failure: nothing may be in flight when the slot goes back
+        if (!rc && ce != cudaSuccess) rc = fail(BYDB_EIO, cudaGetErrorString(ce));
+        if (!rc) rc = collect_scan(slot, stats);
+        if (rc) return rc;
+    }
+    return 0;
+}
+
+// the key table of a keyed answer: value k is `values[k]`
+template <class Out>
+void set_key_table(Out *out, KeyedOwner *owner, const KeyValues &values) {
+    owner->key_off.assign(1, 0);
+    owner->key_bytes.clear();
+    for (const auto &v : values) {
+        owner->key_bytes.insert(owner->key_bytes.end(), v.begin(), v.end());
+        owner->key_off.push_back(static_cast<uint32_t>(owner->key_bytes.size()));
+    }
+    if (owner->key_bytes.empty()) owner->key_bytes.push_back(0);
+    out->n_keys = static_cast<int32_t>(values.size());
+    out->key_off = owner->key_off.data();
+    out->key_bytes = owner->key_bytes.data();
+}
+
+// 3. insertion order of the V x G composite groups from where each series first shows each value (kts / krow): ko.perm lists
+// the composite groups v * G + g in insertion order, the *ko.n_present that appeared first, in scratch `kb` (enqueued, not
+// synchronised; the staging of the series groups in slot.pinned is in flight).  `resident`: a keyed step being captured -- its
+// step state holds the order's arrays (the slots preset by the step's reset kernel) and the staging it uploaded before the capture.
+int keyed_order(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, const int64_t *kts, const uint32_t *krow, Scratch &kb,
+                KeyOrderParams &ko, bydb_stats &stats, const KeyOrderParams *resident = nullptr) {
+    cudaStream_t stream = slot.stream;
+    const size_t NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    if (resident) {
+        ko = *resident;
+    } else {
+        const StageLayout st = stage_layout(NS, G);
+        Carve carve;
+        const size_t b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16), b_stage = carve(st.bytes);
+        CUDA_TRY(kb.alloc(carve.o, stream));
+        CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
+        memset(&ko, 0, sizeof ko);
+        // order | group_start of the series groups: staged again (run_scan's copies live in its own scratch)
+        stage_series(q, st, slot.pinned);
+        CUDA_TRY(cudaMemcpyAsync(kb.base + b_stage, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream));
+        ko.order = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_order);
+        ko.group_start = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_gstart);
+        ko.slot = reinterpret_cast<int32_t *>(kb.base + b_slot);
+        ko.first_series = reinterpret_cast<int32_t *>(kb.base + b_first);
+        ko.perm = reinterpret_cast<int32_t *>(kb.base + b_perm);
+        ko.n_present = reinterpret_cast<uint32_t *>(kb.base + b_np);
+    }
+    ko.n_groups = static_cast<int32_t>(G);
+    ko.n_values = static_cast<uint32_t>(V);
+    ko.n_series = static_cast<uint32_t>(NS);
+    ko.Kts = kts;
+    ko.Krow = krow;
+    launch_key_order(ko, stream);
+    stats.kernel_launches += 2;
+    return 0;
+}
+
+// The rows of a keyed answer as (series group, key value): the group into group_id (the answer's), the key value into the owner's
+// key_id, which out->key_id then names.  Row r takes the pair of int32 at pairs + j * stride, with j = r, or with j = group_id[r]
+// (by_position: the rows carry their composite group's position).
+template <class Out>
+void set_row_keys(Out *out, KeyedOwner *owner, std::vector<int32_t> &group_id, const void *pairs, size_t stride, bool by_position) {
+    owner->key_id.resize(group_id.size());
+    for (size_t r = 0; r < group_id.size(); ++r) {
+        const uint8_t *pair = static_cast<const uint8_t *>(pairs) + (by_position ? static_cast<size_t>(group_id[r]) : r) * stride;
+        memcpy(&group_id[r], pair, 4);
+        memcpy(&owner->key_id[r], pair + 4, 4);
+    }
+    out->key_id = owner->key_id.data();
+}
+
+// 4a. bydb_scan_agg_keyed / bydb_scan_reduce_keyed: after the order, the table at `table` reordered, the ordinary finalisation /
+// Top-N on it, and the rows mapped back to (series group, key value).  The caller sized the slot's pinned staging with
+// keyed_pinned_bytes.
+int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
+                 const int64_t *kts, const uint32_t *krow, bydb_keyed_result *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    Scratch kb, dst;
+    KeyOrderParams ko;
+    int rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, out->base.stats);
+    if (rc) return rc;
+    CUDA_TRY(dst.alloc(tlc.total, stream));
+    launch_permute_table(tlc.at(dst.base), tlc.at(table), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), coltype,
+                         static_cast<uint32_t>(V), stream);
+    CUDA_TRY(cudaStreamSynchronize(stream));  // the staging above is reused by the finalisation's read-back
+    out->base.stats.kernel_launches += 1;
+    Plan planc = plan;
+    planc.n_groups = static_cast<int32_t>(GP);
+    rc = finalize_to_host(q, planc, slot, stream, dst.base, tlc, &out->base, true);
+    if (rc) {
+        cudaStreamSynchronize(stream);
+        return rc;
+    }
+    std::vector<int32_t> perm(GP);
+    CUDA_TRY(cudaMemcpyAsync(perm.data(), ko.perm, GP * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    out->base.stats.d2h_bytes += GP * 4;
+    // rows carry the position in insertion order: back to (group of the series, key value)
+    std::vector<int32_t> &pos = static_cast<ResultOwner *>(out->base.owner)->group_id;
+    std::vector<int32_t> pairs(2 * pos.size());
+    for (size_t r = 0; r < pos.size(); ++r) {
+        const int32_t comp = perm[static_cast<size_t>(pos[r])];
+        pairs[2 * r] = comp % static_cast<int32_t>(G);
+        pairs[2 * r + 1] = comp / static_cast<int32_t>(G);
+    }
+    set_row_keys(out, owner, pos, pairs.data(), 8, false);
+    return 0;
+}
+
+// 4b. bydb_scan_partials_keyed / bydb_scan_reduce_keyed_partials: after the order, keyed_partial_rows_kernel writes the wire rows
+// of the present composite groups from the unpermuted table into one packed image; the read-back takes the control word, then
+// exactly n_present rows.  The composite table never leaves the device.
+int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
+                 const int64_t *kts, const uint32_t *krow, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), G = static_cast<size_t>(plan.n_groups), GP = G * V, A = q->n_aggs;
+    const size_t ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
+    Scratch kb, img;
+    KeyOrderParams ko;
+    int rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, out->stats);
+    if (rc) return rc;
+    CUDA_TRY(img.alloc(ctl_bytes + GP * row_bytes, stream));
+    launch_keyed_partial_rows(rows_params(q, plan, V, tlc.at(table), coltype, ko.perm, ko.n_present, img.base), GP, stream);
+    out->stats.kernel_launches += 1;
+    // 1. the control word (behind the staging copy that reads slot.pinned, on the same stream)
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base, ctl_bytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    out->stats.d2h_bytes += ctl_bytes;
+    rc = rows_status(slot.pinned, F);
+    if (rc) return rc;
+    const size_t n = rows_in(slot.pinned, GP);
+    // 2. the rows, right behind the control word
+    if (n) {
+        CUDA_TRY(cudaMemcpyAsync(slot.pinned + ctl_bytes, img.base + ctl_bytes, n * row_bytes, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        out->stats.d2h_bytes += n * row_bytes;
+    }
+    rc = parse_rows(slot.pinned, q, plan, GP, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, static_cast<PartialRowsOwner *>(out->base.owner)->group_id, slot.pinned + ctl_bytes, row_bytes, false);
+    return 0;
+}
+
+// the pinned staging of the ordering and the read-back of a keyed answer over GP composite groups
+size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_result *) {
+    return step_pinned_bytes(q, static_cast<size_t>(plan.n_groups), GP);
+}
+size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_partial_rows *) {
+    return std::max(stage_layout(q->n_series, static_cast<size_t>(plan.n_groups)).stride, keyed_ctl_bytes(plan.fcols.size()) + GP * keyed_row_bytes(q->n_aggs));
+}
+
+void keyed_free(bydb_ctx *ctx, bydb_keyed_result *out) { bydb_keyed_result_free(ctx, out); }
+void keyed_free(bydb_ctx *ctx, bydb_keyed_partial_rows *out) { bydb_keyed_partial_rows_free(ctx, out); }
+
+// a keyed answer being filled: its owner and key table (value k is values[k]) are set up on construction, and a failure past that
+// point must not leave a half-filled result with the caller, so the answer is freed again unless `done` is set
+template <class Out>
+struct KeyedAnswer {
+    bydb_ctx *ctx;
+    Out *out;
+    KeyedOwner *owner;
+    bool done = false;
+    KeyedAnswer(bydb_ctx *c, Out *o, const KeyValues &values) : ctx(c), out(o), owner(new KeyedOwner()) {
+        out->owner = owner;
+        set_key_table(out, owner, values);
+    }
+    ~KeyedAnswer() {
+        if (!done) keyed_free(ctx, out);
+    }
+};
+
+// The preamble of an unprepared keyed call: the arguments and the key (cap at most max_cap; pred_slot: see check_group_key), the
+// plan, the refusal of parts that overlap in time, the device, the slot and the answer's zeroed stats
+template <class Out>
+int keyed_call(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t max_cap, bool pred_slot, Out *out, uint32_t &cap, Plan &plan,
+               std::optional<SlotLease> &lease) {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    memset(out, 0, sizeof *out);
+    int rc = validate_query(q, true);
+    if (rc) return rc;
+    rc = check_group_key(q, key, max_cap, pred_slot, cap);
+    if (rc) return rc;
+    g_last_dev_err = 0;
+    rc = make_plan(ctx, q, nullptr, plan);
+    if (rc) return rc;
+    if (parts_overlap(plan.parts, q->tmin, q->tmax))
+        return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    lease.emplace(ctx);
+    if (lease->init()) return fail(BYDB_EIO, "cannot create stream");
+    bydb_stats &stats = keyed_stats(out);
+    memset(&stats, 0, sizeof stats);
+    return 0;
+}
+
+// bydb_scan_agg_keyed and bydb_scan_partials_keyed: discovery, the per-value passes, the order, then the form's own answer
+template <class Out>
+int scan_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
+    uint32_t cap = 0;
+    Plan plan;
+    std::optional<SlotLease> lease;
+    int rc = keyed_call(ctx, q, key, kMaxKeyValues, true, out, cap, plan, lease);
+    if (rc) return rc;
+    ExecSlot &slot = *lease->slot;
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
+    bydb_stats &stats = keyed_stats(out);
+
+    KeyValues values;
+    rc = discover_keys(ctx, q, key, cap, plan, slot, &stats, values);
+    if (rc) return rc;
+    const size_t V = values.size();
+    KeyedAnswer<Out> answer(ctx, out, values);
+    if (V == 0) {  // no block selected: no rows (n_rows = 0)
+        answer.done = true;
+        return 0;
+    }
+
+    const size_t GP = G * V;
+    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
+    TableLayout tlc(GP, F);
+    Carve carve;
+    const size_t b_src = carve(tlc.total), b_ct = carve(V * F * 8), b_kts = carve(V * NS * 8), b_krow = carve(V * NS * 4);
+    Scratch kb;
+    CUDA_TRY(kb.alloc(carve.o, stream));
+    CUDA_TRY(cudaMemsetAsync(kb.base + b_ct, 0, V * F * 8, stream));
+    if (slot.ensure_pinned(keyed_pinned_bytes(q, plan, GP, out))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    int64_t *ct = reinterpret_cast<int64_t *>(kb.base + b_ct), *kts = reinterpret_cast<int64_t *>(kb.base + b_kts);
+    uint32_t *krow = reinterpret_cast<uint32_t *>(kb.base + b_krow);
+    rc = run_keyed_passes(ctx, q, key, plan, slot, values, tlc, kb.base + b_src, ct, kts, krow, nullptr, &stats);
+    if (!rc) rc = keyed_finish(q, plan, slot, V, kb.base + b_src, tlc, ct, kts, krow, out, answer.owner);
+    if (rc) return rc;
+    answer.done = true;
+    return 0;
+}
+
+// ---- bydb_scan_agg_keyed_wide / bydb_scan_partials_keyed_wide: one scan pass (see "Wide group key" in scan_kernels.cu)
+size_t pow2_at_least(size_t n) {
+    size_t p = 1;
+    while (p < n) p <<= 1;
+    return p;
+}
+
+// the answer forms over the table of the present composite groups (n_comp groups of layout tl at `table`) that the fold `rp` wrote
+int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const WideReduceParams &rp,
+              bydb_keyed_result *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    Plan planc = plan;
+    planc.n_groups = static_cast<int32_t>(n_comp);
+    int rc = finalize_to_host(q, planc, slot, stream, table, tl, &out->base, true);
+    if (rc) return rc;
+    std::vector<int32_t> pairs(2 * n_comp);
+    CUDA_TRY(cudaMemcpyAsync(pairs.data(), rp.pairs, pairs.size() * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    out->base.stats.d2h_bytes += pairs.size() * 4;
+    set_row_keys(out, owner, static_cast<ResultOwner *>(out->base.owner)->group_id, pairs.data(), 8, true);
+    return 0;
+}
+int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const WideReduceParams &rp,
+              bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size(), A = q->n_aggs, ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
+    Plan planc = plan;
+    planc.n_groups = static_cast<int32_t>(n_comp);
+    Scratch img;
+    CUDA_TRY(img.alloc(ctl_bytes + n_comp * row_bytes, stream));
+    const TablePtrs t = tl.at(table);
+    launch_keyed_partial_rows(rows_params(q, planc, 1, t, t.coltype, rp.perm, &rp.ctl[1], img.base), n_comp, stream);
+    out->stats.kernel_launches += 1;
+    if (slot.ensure_pinned(ctl_bytes + n_comp * row_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base, ctl_bytes + n_comp * row_bytes, cudaMemcpyDeviceToHost, stream));
+    std::vector<int32_t> pairs(2 * n_comp);
+    CUDA_TRY(cudaMemcpyAsync(pairs.data(), rp.pairs, pairs.size() * 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    out->stats.d2h_bytes += ctl_bytes + n_comp * row_bytes + pairs.size() * 4;
+    int rc = parse_rows(slot.pinned, q, planc, n_comp, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, static_cast<PartialRowsOwner *>(out->base.owner)->group_id, pairs.data(), 8, true);
+    return 0;
+}
+
+template <class Out>
+int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
+    uint32_t cap = 0;
+    Plan plan;
+    std::optional<SlotLease> lease;
+    int rc = keyed_call(ctx, q, key, kMaxWideKeyValues, false, out, cap, plan, lease);
+    if (rc) return rc;
+    ExecSlot &slot = *lease->slot;
+    cudaStream_t stream = slot.stream;
+    const bool int64_key = key->value_type == BYDB_VT_INT64;
+    const size_t F = plan.fcols.size(), NS = q->n_series, NB = plan.total_blocks, NBp = align_up(std::max<size_t>(NB, 1), 1024);
+    bydb_stats &stats = keyed_stats(out);
+    cudaEvent_t *ev = slot.ev;
+    CUDA_TRY(cudaEventRecord(ev[0], stream));
+
+    // 1. discovery: the value table (S slots), each selected block's rank and distinct values, then their exclusive scan
+    const size_t S = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(cap), kKeySlots));
+    Carve carve;
+    const size_t a_sids = carve(NS * 8), a_grp = carve(NS * 4), a_slots = carve(S * 8), a_ctl = carve(32), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
+                 a_lens = carve(static_cast<size_t>(cap) * 4), a_sid = carve(S * 4), a_nbr = carve(NBp * 4), a_rank = carve(NB * 4),
+                 a_tiles = carve(NBp / 1024 * 4);
+    Scratch ka;
+    CUDA_TRY(ka.alloc(carve.o, stream));
+    if (slot.ensure_pinned(std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    WideKeyParams wk;
+    memset(&wk, 0, sizeof wk);
+    KeyParams &kp = wk.k;
+    kp = key_params(ctx, q, key, cap, plan, slot.pinned, ka.base, a_sids, a_slots, a_ctl, a_vals, a_lens);
+    int32_t *hg = reinterpret_cast<int32_t *>(slot.pinned + NS * 8);
+    for (size_t i = 0; i < NS; ++i) hg[i] = q->series_group ? q->series_group[i] : 0;
+    if (NS) {
+        CUDA_TRY(cudaMemcpyAsync(ka.base + a_sids, slot.pinned, NS * 8, cudaMemcpyHostToDevice, stream));
+        CUDA_TRY(cudaMemcpyAsync(ka.base + a_grp, slot.pinned + NS * 8, NS * 4, cudaMemcpyHostToDevice, stream));
+    }
+    stats.h2d_bytes += NS * 12;
+    CUDA_TRY(cudaMemsetAsync(ka.base + a_slots, 0, a_vals - a_slots, stream));
+    CUDA_TRY(cudaMemsetAsync(ka.base + a_nbr, 0, NBp * 4, stream));
+    uint32_t *d_ctl = kp.count;  // as discovery's, and [4] R
+    wk.slot_mask = static_cast<uint32_t>(S - 1);
+    wk.int64_key = int64_key ? 1u : 0u;
+    wk.slot_id = reinterpret_cast<uint32_t *>(ka.base + a_sid);
+    wk.n_by_rank = reinterpret_cast<uint32_t *>(ka.base + a_nbr);
+    wk.rank = reinterpret_cast<uint32_t *>(ka.base + a_rank);
+    launch_key_values_wide(wk, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+    launch_excl_scan(wk.n_by_rank, static_cast<uint32_t>(NBp), reinterpret_cast<uint32_t *>(ka.base + a_tiles), d_ctl + 4, stream);
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, d_ctl, 32, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    stats.kernel_launches += (NB ? 1u : 0u) + 1u + 3u;
+    stats.d2h_bytes += 32;
+    uint32_t ctl[8];
+    memcpy(ctl, slot.pinned, 32);
+    rc = discovery_status(ctl);
+    if (rc) return rc;
+    const size_t V = std::min<size_t>(ctl[0], cap), R = ctl[4];
+    KeyValues values;
+    if (V) {
+        const size_t vb = V * (int64_key ? 8 : kMaxLit);
+        CUDA_TRY(cudaMemcpyAsync(slot.pinned, kp.vals, vb, cudaMemcpyDeviceToHost, stream));
+        if (!int64_key) CUDA_TRY(cudaMemcpyAsync(slot.pinned + vb, kp.lens, V * 4, cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaStreamSynchronize(stream));
+        stats.d2h_bytes += vb + (int64_key ? 0 : V * 4);
+        values = unpack_values(V, int64_key, slot.pinned, reinterpret_cast<const uint32_t *>(slot.pinned + vb));
+    }
+    KeyedAnswer<Out> answer(ctx, out, values);
+    if (V == 0 || R == 0) {  // no block selected: no rows (n_rows = 0)
+        answer.done = true;
+        return 0;
+    }
+    if (R > 0x7fffffffull) return fail(BYDB_ENOMEM, "wide group-key query: too many (block, key value) records");
+
+    // 2. the scan: one record per present (block, key value)
+    const size_t rec_bytes = wide_record_bytes(F);
+    const size_t C = pow2_at_least(std::max<size_t>(2 * R, 1024)), N = pow2_at_least(std::max<size_t>(R, 2048));
+    Carve cb;
+    const size_t b_zero = cb(kZeroPageBytes), b_rec = cb(R * rec_bytes), b_comp = cb(C * 8), b_cmin = cb(C * 4), b_rslot = cb(R * 4), b_keys = cb(N * 8),
+                 b_heads = cb(N * 4), b_tiles = cb(N / 1024 * 4), b_ctl = cb(8), b_seg = cb(R * 4);
+    Scratch sb;
+    CUDA_TRY(sb.alloc(cb.o, stream));
+    ZeroPage *z = reinterpret_cast<ZeroPage *>(sb.base + b_zero);
+    CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + b_comp, 0, C * 8, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + b_cmin, 0xff, C * 4, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + b_ctl, 0, 8, stream));
+    ScanParams sp;
+    scan_params_head(ctx, q, plan, kp.q_sids, sp);
+    sp.err = z->err;
+    sp.stats = z->stats;
+    sp.col_type = z->col_type;
+    WideScanParams ws;
+    memset(&ws, 0, sizeof ws);
+    ws.slots = kp.slots;
+    ws.slot_id = wk.slot_id;
+    ws.zero = kp.zero;
+    ws.slot_mask = wk.slot_mask;
+    ws.int64_key = wk.int64_key;
+    ws.key_name = kp.key_name;
+    ws.rank = wk.rank;
+    ws.rec_off = wk.n_by_rank;
+    ws.series_group = reinterpret_cast<const int32_t *>(ka.base + a_grp);
+    ws.records = sb.base + b_rec;
+    CUDA_TRY(cudaEventRecord(ev[1], stream));
+    launch_scan_keyed_wide(sp, ws, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+    CUDA_TRY(cudaEventRecord(ev[2], stream));
+
+    // 3. the composite groups in insertion order
+    WideReduceParams rp;
+    memset(&rp, 0, sizeof rp);
+    rp.records = ws.records;
+    rp.n_records = static_cast<uint32_t>(R);
+    rp.n_fcols = static_cast<uint32_t>(F);
+    rp.comp = reinterpret_cast<unsigned long long *>(sb.base + b_comp);
+    rp.comp_min = reinterpret_cast<uint32_t *>(sb.base + b_cmin);
+    rp.rec_slot = reinterpret_cast<uint32_t *>(sb.base + b_rslot);
+    rp.comp_mask = static_cast<uint32_t>(C - 1);
+    rp.n_sort = static_cast<uint32_t>(N);
+    rp.keys = reinterpret_cast<unsigned long long *>(sb.base + b_keys);
+    rp.heads = reinterpret_cast<uint32_t *>(sb.base + b_heads);
+    rp.tile_sums = reinterpret_cast<uint32_t *>(sb.base + b_tiles);
+    rp.ctl = reinterpret_cast<uint32_t *>(sb.base + b_ctl);
+    rp.seg_start = reinterpret_cast<uint32_t *>(sb.base + b_seg);
+    rp.col_type = z->col_type;
+    rp.scan_err = z->err;
+    launch_wide_order(rp, stream);
+    ZeroPage *hz = slot.page(0);
+    CUDA_TRY(cudaMemcpyAsync(hz, z, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, rp.ctl, 8, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    CUDA_TRY(cudaGetLastError());
+    uint32_t sort_launches = 0;
+    for (size_t size = 4096; size <= N; size <<= 1) sort_launches += 1 + static_cast<uint32_t>(__builtin_ctzll(size) - 11);
+    stats.kernel_launches += (NB ? 1u : 0u) + 2u + 1u + sort_launches + 1u + 3u + 1u;
+    stats.d2h_bytes += kZeroPageBytes + 8;
+    {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, ev[1], ev[2]);
+        stats.scan_kernel_ms += ms;
+    }
+    rc = read_zero_page(*hz, false, &stats);
+    if (rc) return rc;
+    const size_t n_comp = reinterpret_cast<const uint32_t *>(slot.pinned)[1];
+
+    // 4. the fold into a table of the present composite groups, then the form's own answer
+    const TableLayout tl(std::max<size_t>(n_comp, 1), F);
+    Carve cf;
+    const size_t f_table = cf(tl.total), f_pairs = cf(n_comp * 8), f_perm = cf(n_comp * 4);
+    Scratch fb;
+    CUDA_TRY(fb.alloc(cf.o, stream));
+    rp.table = tl.at(fb.base + f_table);
+    rp.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
+    rp.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
+    launch_wide_fold(rp, static_cast<uint32_t>(n_comp), stream);
+    CUDA_TRY(cudaEventRecord(ev[3], stream));
+    stats.kernel_launches += 1;
+    if (n_comp > 0) rc = wide_emit(q, plan, slot, fb.base + f_table, tl, n_comp, rp, out, answer.owner);
+    if (rc) return rc;
+    {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, ev[0], ev[3]);
+        stats.device_ms += ms;
+    }
+    answer.done = true;
+    return 0;
+}
+
+}  // namespace
+
+// ------------------------------------------------------------------------------------------------
+// Prepared group-by on a stored tag: the V passes, the insertion order, the finalisation and the row mapping captured as ONE
+// graph.  Discovery runs once per capture: its inputs (the parts a handle names, series, range, key) are fixed while the handles
+// keep naming the parts the step was captured with, so the key table is a property of the capture, like the block plan.
+// Everything here is additive: bydb_scan_agg_keyed is untouched.
+// ------------------------------------------------------------------------------------------------
+struct bydb_prepared_keyed {
+    bydb_prepared *pq = nullptr;   // the query's deep copy, its slot, events, graph, step state and held parts
+    std::string family, tag;       // the key's strings: key.family / key.tag point here
+    bydb_group_key key{};
+    uint32_t cap = 0;              // distinct values accepted (check_group_key)
+    KeyValues values;              // found when the step was captured: the key table of every replay
+    size_t pairs_off = 0, zero_off = 0;  // in the replay's read-back image: the rows' (group, key) pairs, the passes' zero pages
+    ~bydb_prepared_keyed() { prepared_destroy(pq); }
+};
+
+namespace {
+// Discovers the key values and captures the keyed step into k->pq->exec, in a step state of its own:
+//   composite table | permuted table | the passes' column types | Kts | Krow | the order's slots, first_series, perm, n_present |
+//   one scan scratch (scan_layout, the passes run one after another) | finalisation over V x G groups, then the rows' (group, key)
+//   pairs and the V zero pages, so that one copy reads back the rows, their pairs and the passes' counters and errors.
+// `partial` (bydb_scan_partials_keyed_prepared) selects the other tail: no permuted table and no finalisation; behind the order,
+// keyed_partial_rows_kernel writes the row image (control word, rows) right behind the V zero pages, and rows_to_host_kernel
+// brings the pages, the control word and exactly the present rows to the staging.
+// Leaves neither a graph nor p->empty_step when this execution, or (capturable cleared) every later one, takes the plain path: a part
+// is missing, the parts overlap, discovery fails (its refusal is the plain call's), or the state or the capture cannot be had.
+void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
+    bydb_prepared *p = k->pq;
+    const bydb_query *q = &p->q;
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up
+    Plan plan;
+    if (make_plan(ctx, q, nullptr, plan)) return;
+    ExecSlot &slot = *p->slot;
+    cudaStream_t stream = slot.stream;
+    bydb_stats discovery{};
+    KeyValues values;
+    if (parts_overlap(plan.parts, q->tmin, q->tmax) || discover_keys(ctx, q, &k->key, k->cap, plan, slot, &discovery, values)) {
+        p->capturable = false;
+        return;
+    }
+    const size_t V = values.size(), F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    if (V == 0) {
+        k->values.clear();
+        p->empty_step = true;
+        p->held = plan.parts;
+        p->held_gen = gen;
+        return;
+    }
+    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) {
+        p->capturable = false;
+        return;
+    }
+    const TableLayout tlc(GP, F);
+    const StageLayout st = stage_layout(NS, G);
+    const ScanLayout sl = scan_layout(st, plan.total_blocks, F, plan.parts.size(), true);
+    const FinalLayout fl = final_layout(GP, q->n_aggs, q->top_n);
+    const size_t b_pairs = align_up(fl.cap * 8, 256), b_zero = V * kZeroPageBytes;
+    const size_t b_rows = keyed_ctl_bytes(F) + GP * keyed_row_bytes(q->n_aggs);  // partial: the row image
+    Carve carve;
+    const size_t o_src = carve(tlc.total), o_dst = carve(partial ? 0 : tlc.total), o_ct = carve(V * F * 8), o_kts = carve(V * NS * 8),
+                 o_krow = carve(V * NS * 4), o_slot = carve(NS * V * 4), o_first = carve(GP * 4), o_perm = carve(GP * 4), o_np = carve(16),
+                 o_scan = carve(sl.total), o_fin = carve(partial ? b_zero + b_rows : fl.total + b_pairs + b_zero);
+    p->host_off = st.stride;  // the read-back lands behind the staging area, as in the plain prepared step
+    p->read_back = partial ? b_zero + b_rows : fl.out_bytes + b_pairs + b_zero;  // partial: the most the copy kernel may write
+    // sized before the capture: the graph writes the staging through its device address
+    uint8_t *h_dst = slot.ensure_pinned(p->host_off + p->read_back) ? nullptr : slot.pinned_dev(p->host_off);
+    cudaError_t e = cudaSuccess;
+    if (!h_dst || !make_step_state(p, carve.o, st, o_scan + sl.off_sids, e)) {
+        cudaGetLastError();
+        p->step_state = nullptr;
+        p->capturable = false;
+        return;
+    }
+    uint8_t *S = p->step_state, *fin_base = S + o_fin, *zero_pages = partial ? fin_base : fin_base + fl.total + b_pairs;
+    bydb_stats &cs = p->captured;
+    uint32_t fin_launches = 0;
+    GraphCapture c;
+    if (e == cudaSuccess) c = capture_graph(stream, &p->exec, [&]() -> int {
+        memset(&cs, 0, sizeof cs);
+        int64_t *ct = reinterpret_cast<int64_t *>(S + o_ct), *kts = reinterpret_cast<int64_t *>(S + o_kts);
+        uint32_t *krow = reinterpret_cast<uint32_t *>(S + o_krow);
+        KeyedResetParams rp;
+        memset(&rp, 0, sizeof rp);
+        rp.zero[0] = reinterpret_cast<uint32_t *>(ct);
+        rp.n_zero[0] = V * F * 2;
+        rp.zero[1] = reinterpret_cast<uint32_t *>(zero_pages);
+        rp.n_zero[1] = b_zero / 4;
+        rp.ones[0] = sl.n_first ? reinterpret_cast<uint32_t *>(S + o_scan + sl.off_first) : nullptr;
+        rp.n_ones[0] = sl.n_first;
+        rp.ones[1] = reinterpret_cast<uint32_t *>(S + o_slot);
+        rp.n_ones[1] = NS * V;
+        launch_keyed_step_reset(rp, stream);
+        cs.kernel_launches += 1;
+        Scratch scan, kb, fin;
+        scan.view(S + o_scan, sl.total);
+        fin.view(fin_base, fl.total + b_pairs + b_zero);
+        int rc = run_keyed_passes(ctx, q, &k->key, plan, slot, values, tlc, S + o_src, ct, kts, krow, nullptr, &cs, &scan, zero_pages);
+        KeyOrderParams res, ko;
+        memset(&res, 0, sizeof res);
+        res.order = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_order);
+        res.group_start = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_gstart);
+        res.slot = reinterpret_cast<int32_t *>(S + o_slot);
+        res.first_series = reinterpret_cast<int32_t *>(S + o_first);
+        res.perm = reinterpret_cast<int32_t *>(S + o_perm);
+        res.n_present = reinterpret_cast<uint32_t *>(S + o_np);
+        if (!rc) rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, cs, &res);
+        FinalLayout flc;
+        size_t fin_back = 0;
+        if (!rc && partial) {
+            launch_keyed_partial_rows(rows_params(q, plan, V, tlc.at(S + o_src), ct, ko.perm, ko.n_present, zero_pages + b_zero), GP, stream);
+            RowsCopyParams cp;
+            memset(&cp, 0, sizeof cp);
+            cp.pages = zero_pages;
+            cp.image = zero_pages + b_zero;
+            cp.dst = h_dst;
+            cp.page_bytes = b_zero;
+            cp.ctl_bytes = keyed_ctl_bytes(F);
+            cp.row_bytes = keyed_row_bytes(q->n_aggs);
+            cp.max_rows = static_cast<uint32_t>(GP);
+            launch_rows_to_host(cp, stream);
+        } else if (!rc) {
+            launch_permute_table(tlc.at(S + o_dst), tlc.at(S + o_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), ct,
+                                 static_cast<uint32_t>(V), stream);
+            Plan planc = plan;
+            planc.n_groups = static_cast<int32_t>(GP);
+            rc = finalize_launch(q, planc, stream, S + o_dst, tlc, fin, flc, fin_launches, fin_back);
+            if (!rc) {
+                launch_keyed_row_map(reinterpret_cast<const int32_t *>(fin_base + fl.o_sg), reinterpret_cast<const uint32_t *>(fin_base + fl.o_cnt),
+                                     ko.perm, static_cast<uint32_t>(G), static_cast<uint32_t>(fl.cap), reinterpret_cast<int32_t *>(fin_base + fl.total), stream);
+                if (cudaMemcpyAsync(slot.pinned + p->host_off, fin_base + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+            }
+        }
+        return rc;
+    });
+    if (e != cudaSuccess || c.rc || c.err != cudaSuccess || !p->exec) {
+        cudaGetLastError();
+        drop_step(p);
+        p->capturable = false;
+        return;
+    }
+    // permute_table, finalisation + row selection, the row mapping; or the row kernel and the copy kernel.  A partial step's read-back
+    // is sized by the rows present: the replay counts it.
+    cs.kernel_launches += partial ? 2 : 1 + fin_launches + 1;
+    cs.d2h_bytes = partial ? 0 : p->read_back;
+    p->partial_step = partial;
+    p->fl = fl;
+    p->express = false;  // the key predicate keeps every pass off the express lane
+    k->values = std::move(values);
+    k->pairs_off = fl.out_bytes;
+    k->zero_off = partial ? 0 : fl.out_bytes + b_pairs;
+    p->held = plan.parts;
+    p->held_gen = gen;
+}
+
+// the answer of a replayed keyed step from its read-back `image`, after the passes' zero pages: the finalised rows and their
+// (group, key) pairs, or the row image (table status, rows, their key values) and the bytes the copy kernel brought back
+int keyed_answer(bydb_prepared_keyed *k, const Plan &, const uint8_t *image, bydb_keyed_result *out, KeyedOwner *owner) {
+    const int rc = finalize_parse(image, k->pq->fl, true, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, static_cast<ResultOwner *>(out->base.owner)->group_id, image + k->pairs_off, 8, false);
+    return 0;
+}
+int keyed_answer(bydb_prepared_keyed *k, const Plan &shape, const uint8_t *image, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    const size_t V = k->values.size(), GP = V * shape.tl.G, A = k->pq->q.n_aggs;
+    const uint8_t *rows = image + V * kZeroPageBytes;
+    const size_t ctl_bytes = keyed_ctl_bytes(shape.fcols.size()), row_bytes = keyed_row_bytes(A);
+    out->stats.d2h_bytes += V * kZeroPageBytes + ctl_bytes + rows_in(rows, GP) * row_bytes;
+    const int rc = parse_rows(rows, &k->pq->q, shape, GP, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, static_cast<PartialRowsOwner *>(out->base.owner)->group_id, rows + ctl_bytes, row_bytes, false);
+    return 0;
+}
+
+// One replay, synchronised and parsed: the passes' counters add up and the first pass with a device error decides, as the plain
+// path's pass-by-pass collection has it; then the answer of the step's form (keyed_answer).
+template <class Out>
+int keyed_replay(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
+    bydb_prepared *p = k->pq;
+    Plan shape;
+    int rc = query_shape(&p->q, shape);
+    if (rc) return rc;
+    uint8_t *image = p->slot->pinned + p->host_off;
+    const size_t V = k->values.size();
+    // a replay that fails to launch cannot report the previous one's status (nor, in a partial step, its control word)
+    memset(image + k->zero_off, 0, V * kZeroPageBytes + (p->partial_step ? keyed_ctl_bytes(shape.fcols.size()) : 0));
+    auto page = [&](size_t v) -> const ZeroPage & { return *reinterpret_cast<const ZeroPage *>(image + k->zero_off + v * kZeroPageBytes); };
+    bydb_stats &stats = keyed_stats(out);
+    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, false, page(0), &stats);
+    for (size_t v = 1; !rc && v < V; ++v) rc = read_zero_page(page(v), false, &stats);
+    if (rc) return rc;
+    KeyedAnswer<Out> answer(ctx, out, k->values);
+    rc = keyed_answer(k, shape, image, out, answer.owner);
+    if (rc) return rc;
+    answer.done = true;
+    return 0;
+}
+
+// bydb_scan_agg_keyed_prepared and bydb_scan_partials_keyed_prepared: one captured step per handle, of the form last asked for
+template <class Out>
+int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
+    if (!ctx || !k || !out) return fail(BYDB_EINVAL, "NULL argument");
+    memset(out, 0, sizeof *out);
+    const bool partial = std::is_same<Out, bydb_keyed_partial_rows>::value;
+    bydb_prepared *p = k->pq;
+    std::lock_guard<std::mutex> lk(p->mu);
+    g_last_dev_err = 0;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    const int rc = prepared_step(ctx, p, partial, [&] {
+        keyed_capture(ctx, k, partial);
+        return 0;
+    });
+    if (rc) return rc;
+    if (!p->exec && !p->empty_step) return scan_keyed_impl(ctx, &p->q, &k->key, out);
+    if (p->empty_step) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
+        KeyedAnswer<Out> answer(ctx, out, KeyValues());
+        answer.done = true;
+        return 0;
+    }
+    return keyed_replay(ctx, k, out);
+}
 }  // namespace
 
 // ================================================================================================
@@ -1912,739 +2864,6 @@ int bydb_scan_agg(bydb_ctx *ctx, const bydb_query *q, bydb_result *out) {
 // rewritten into the arena.  The image goes up through the pinned staging ring in 64 MB chunks.
 // ------------------------------------------------------------------------------------------------
 
-extern "C++" {  // the keyed helpers below are templates over the two answer forms
-namespace {
-struct KeyedOwner {
-    std::vector<int32_t> key_id;
-    std::vector<uint32_t> key_off;
-    std::vector<uint8_t> key_bytes;
-};
-
-// the arrays of a bydb_partial_rows
-struct PartialRowsOwner {
-    std::vector<int32_t> group_id;
-    std::vector<uint8_t> is_float;
-    std::vector<int64_t> val_i64, cnt_i64;
-    std::vector<double> val_f64, cnt_f64;
-};
-
-// one aggregate of a row: the Partial words into the arrays of their type, 0 in the others
-void push_partial(PartialRowsOwner &o, const PartialWords &w, bool is_float) {
-    double vf = 0.0, cf = 0.0;
-    memcpy(&vf, &w.val, 8);
-    memcpy(&cf, &w.cnt, 8);
-    o.val_i64.push_back(is_float ? 0 : static_cast<int64_t>(w.val));
-    o.val_f64.push_back(is_float ? vf : 0.0);
-    o.cnt_i64.push_back(is_float ? 0 : static_cast<int64_t>(w.cnt));
-    o.cnt_f64.push_back(is_float ? cf : 0.0);
-}
-
-// the status the control word of a row image carries: the column types merged over the passes, the worst status with them
-int rows_status(const uint8_t *ctl, size_t F) {
-    const int64_t *ct = reinterpret_cast<const int64_t *>(ctl + 8);
-    uint32_t dev_err = 0;
-    for (size_t c = 0; c < F; ++c) dev_err = std::max(dev_err, static_cast<uint32_t>(ct[c] >> 8));
-    return table_status(dev_err);
-}
-// the rows a row image holds: its n_present, at most max_rows
-size_t rows_in(const uint8_t *ctl, size_t max_rows) { return std::min<size_t>(*reinterpret_cast<const uint32_t *>(ctl), max_rows); }
-
-// a row image read back to the host -- the control word, then the rows right behind it -- into *b, after its status; each row's
-// key value into *key_id when given (a keyed answer)
-int parse_rows(const uint8_t *img, const bydb_query *q, const Plan &plan, size_t max_rows, bydb_partial_rows *b, std::vector<int32_t> *key_id) {
-    const size_t F = plan.fcols.size(), A = q->n_aggs, row_bytes = keyed_row_bytes(A);
-    int rc = rows_status(img, F);
-    if (rc) return rc;
-    const int64_t *ct = reinterpret_cast<const int64_t *>(img + 8);
-    auto ro = std::make_unique<PartialRowsOwner>();
-    ro->is_float.resize(A);
-    for (size_t a = 0; a < A; ++a) ro->is_float[a] = (ct[plan.agg_fcol[a]] & 0xff) == BYDB_VT_FLOAT64 ? 1 : 0;
-    const size_t n = rows_in(img, max_rows);
-    const uint8_t *rows = img + keyed_ctl_bytes(F);
-    ro->group_id.resize(n);
-    if (key_id) key_id->resize(n);
-    for (size_t j = 0; j < n; ++j) {
-        const uint8_t *row = rows + j * row_bytes;
-        memcpy(&ro->group_id[j], row, 4);
-        if (key_id) memcpy(&(*key_id)[j], row + 4, 4);
-        for (size_t a = 0; a < A; ++a) {
-            PartialWords w;
-            memcpy(&w.val, row + 8 + 8 * a, 8);
-            memcpy(&w.cnt, row + 8 + 8 * (A + a), 8);
-            push_partial(*ro, w, ro->is_float[a] != 0);
-        }
-    }
-    b->n_rows = static_cast<int32_t>(n);
-    b->n_aggs = static_cast<int32_t>(A);
-    b->group_id = ro->group_id.data();
-    b->is_float = ro->is_float.data();
-    b->val_i64 = ro->val_i64.data();
-    b->val_f64 = ro->val_f64.data();
-    b->cnt_i64 = ro->cnt_i64.data();
-    b->cnt_f64 = ro->cnt_f64.data();
-    b->owner = ro.release();
-    return 0;
-}
-
-// bydb_partials_rows over the table at d_table, enqueued on `s`: emit_plain_rows into the slot's staging, synchronised and parsed.
-// stats (when given) count its three kernels and the bytes its copy kernel brought back.
-int partial_rows_to_host(const bydb_query *q, const Plan &plan, ExecSlot &slot, cudaStream_t s, const uint8_t *d_table, bydb_partial_rows *out,
-                         bydb_stats *stats) {
-    const size_t ctl_bytes = keyed_ctl_bytes(plan.fcols.size()), row_bytes = keyed_row_bytes(q->n_aggs);
-    if (slot.ensure_pinned(ctl_bytes + plan.tl.G * row_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    uint8_t *h_dst = slot.pinned_dev(0);
-    if (!h_dst) return fail(BYDB_EIO, "page-locked staging without a device address");
-    Scratch work;
-    CUDA_TRY(work.alloc(rows_layout(q, plan).total, s));
-    emit_plain_rows(q, plan, s, d_table, work.base, nullptr, 0, h_dst);
-    CUDA_TRY(cudaStreamSynchronize(s));
-    CUDA_TRY(cudaGetLastError());
-    if (stats) {
-        stats->kernel_launches += kPlainRowsLaunches;
-        stats->d2h_bytes += ctl_bytes + rows_in(slot.pinned, plan.tl.G) * row_bytes;
-    }
-    return parse_rows(slot.pinned, q, plan, plan.tl.G, out, nullptr);
-}
-
-// the two answers of a keyed call: finalised rows (bydb_keyed_result) or map-phase partial rows (bydb_keyed_partial_rows)
-bydb_stats &keyed_stats(bydb_keyed_result *out) { return out->base.stats; }
-bydb_stats &keyed_stats(bydb_keyed_partial_rows *out) { return out->stats; }
-using KeyValues = std::vector<std::vector<uint8_t>>;
-
-// the checks of a group key that need no device; cap = the distinct values accepted (max_values, 0 = 64)
-int check_group_key(const bydb_query *q, const bydb_group_key *key, uint32_t &cap) {
-    if (!key || !key->family || !key->tag) return fail(BYDB_EINVAL, "group key without family/tag");
-    if (key->value_type != 0 && key->value_type != BYDB_VT_STR && key->value_type != BYDB_VT_BINARY && key->value_type != BYDB_VT_INT64)
-        return fail(BYDB_EINVAL, "bydb_group_key.value_type must be 0, BYDB_VT_STR, BYDB_VT_BINARY or BYDB_VT_INT64");
-    cap = key->max_values ? key->max_values : 64u;
-    if (cap > kMaxKeyValues) return fail(BYDB_EINVAL, "bydb_group_key.max_values above 256");
-    if (q->n_preds + 1 > kMaxPreds) return fail(BYDB_ENOTSUP, "a group-key query takes at most 7 predicates");
-    return 0;
-}
-
-// 1. the distinct key values of the selected blocks, on the slot's stream, synchronised
-int discover_keys(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats *stats,
-                  KeyValues &values) {
-    const bool int64_key = key->value_type == BYDB_VT_INT64;
-    const size_t NS = q->n_series, NB = plan.total_blocks;
-    cudaStream_t stream = slot.stream;
-    Carve carve;
-    const size_t a_sids = carve(NS * 8), a_slots = carve(kKeySlots * 8), a_ctl = carve(16), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
-                 a_lens = carve(static_cast<size_t>(cap) * 4);
-    const size_t a_total = carve.o;
-    Scratch ka;
-    CUDA_TRY(ka.alloc(a_total, stream));
-    const size_t back_bytes = a_total - a_ctl;  // ctl | vals | lens come back in one copy
-    if (slot.ensure_pinned(std::max(back_bytes, NS * 8) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    if (NS) memcpy(slot.pinned, q->series_ids, NS * 8);
-    if (NS) CUDA_TRY(cudaMemcpyAsync(ka.base + a_sids, slot.pinned, NS * 8, cudaMemcpyHostToDevice, stream));
-    CUDA_TRY(cudaMemsetAsync(ka.base + a_slots, 0, a_total - a_slots, stream));
-    KeyParams kpar;
-    memset(&kpar, 0, sizeof kpar);
-    part_refs(plan.parts, kpar.parts);
-    kpar.n_parts = static_cast<uint32_t>(plan.parts.size());
-    kpar.total_blocks = static_cast<uint32_t>(NB);
-    kpar.q_sids = reinterpret_cast<const uint64_t *>(ka.base + a_sids);
-    kpar.n_series = static_cast<uint32_t>(NS);
-    kpar.cap = cap;
-    kpar.tmin = q->tmin;
-    kpar.tmax = q->tmax;
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        kpar.key_name = ctx->names.find(std::string("t:") + key->family + "/" + key->tag);
-    }
-    kpar.slots = reinterpret_cast<unsigned long long *>(ka.base + a_slots);
-    kpar.count = reinterpret_cast<uint32_t *>(ka.base + a_ctl);
-    kpar.err = reinterpret_cast<uint32_t *>(ka.base + a_ctl) + 1;
-    kpar.zero = reinterpret_cast<uint32_t *>(ka.base + a_ctl) + 3;
-    kpar.vals = ka.base + a_vals;
-    kpar.lens = reinterpret_cast<uint32_t *>(ka.base + a_lens);
-    launch_key_values(kpar, int64_key, ctx->sm_count * 4, stream);
-    CUDA_TRY(cudaStreamSynchronize(stream));  // the staging of the series ids must be consumed before the read-back reuses it
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, ka.base + a_ctl, back_bytes, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    CUDA_TRY(cudaGetLastError());
-    stats->kernel_launches += 2;
-    stats->h2d_bytes += NS * 8;
-    stats->d2h_bytes += back_bytes;
-    const uint32_t *ctl = reinterpret_cast<const uint32_t *>(slot.pinned);
-    if (ctl[1] != 0) {
-        g_last_dev_err = ctl[1];
-        char buf[64];
-        snprintf(buf, sizeof buf, " (block #%u)", ctl[2]);
-        return fail(dev_err_code(ctl[1]), std::string(dev_err_text(ctl[1])) + buf);
-    }
-    const size_t V = std::min<size_t>(ctl[0], cap);
-    values.assign(V, {});
-    const uint8_t *hv = slot.pinned + (a_vals - a_ctl);
-    const uint32_t *hl = reinterpret_cast<const uint32_t *>(slot.pinned + (a_lens - a_ctl));
-    for (size_t v = 0; v < V; ++v) {
-        if (int64_key) values[v].assign(hv + v * 8, hv + v * 8 + 8);  // the reference's key bytes: little-endian int64
-        else values[v].assign(hv + v * kMaxLit, hv + v * kMaxLit + hl[v]);
-    }
-    return 0;
-}
-
-// 2. one scan pass per value v (the key as an extra predicate) into slice v of the composite table tlc (V x G groups, value-major)
-// at `table`, with the pass's column types at coltype + v * F and where each series first shows v at kts / krow + v * NS; the
-// first pass also writes the series' spans when `span` is set.  Every pass is synchronised and its device errors collected --
-// unless `resident` is given (a keyed step being captured): then the passes share that scan scratch, pass v keeps its counters
-// and device error in zero page v of `zero_pages` (kZeroPageBytes each) for the step's one read-back, and nothing synchronises.
-int run_keyed_passes(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Plan &plan, ExecSlot &slot, const KeyValues &values,
-                     const TableLayout &tlc, uint8_t *table, int64_t *coltype, int64_t *kts, uint32_t *krow, int64_t *span, bydb_stats *stats,
-                     Scratch *resident = nullptr, uint8_t *zero_pages = nullptr) {
-    const bool int64_key = key->value_type == BYDB_VT_INT64;
-    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
-    std::vector<bydb_pred> preds(q->preds, q->preds + q->n_preds);
-    preds.emplace_back();
-    bydb_query qv = *q;
-    qv.n_preds = q->n_preds + 1;
-    for (size_t v = 0; v < values.size(); ++v) {
-        bydb_pred &kpred = preds.back();
-        memset(&kpred, 0, sizeof kpred);
-        kpred.family = key->family;
-        kpred.tag = key->tag;
-        if (int64_key) {
-            int64_t lit = 0;
-            memcpy(&lit, values[v].data(), 8);
-            kpred.op = lit == 0 ? kOpEqOrNil : BYDB_OP_EQ;  // a nil cell is the column's zero value (typed_column.go:49-53)
-            kpred.value_type = BYDB_VT_INT64;
-            kpred.lit_i64 = lit;
-        } else {
-            kpred.op = values[v].empty() ? kOpEqOrNil : BYDB_OP_EQ;  // a nil cell and "" are the same key (groupby.go:226-254)
-            kpred.value_type = BYDB_VT_STR;
-            kpred.lit = values[v].data();
-            kpred.lit_len = values[v].size();
-        }
-        qv.preds = preds.data();
-        KeyedPass pass;
-        pass.group_off = v * G;
-        pass.coltype = coltype + v * F;
-        pass.kts = kts + v * NS;
-        pass.krow = krow + v * NS;
-        pass.span = v == 0 ? span : nullptr;
-        if (resident) {
-            pass.zero = reinterpret_cast<ZeroPage *>(zero_pages + v * kZeroPageBytes);
-            if (int rc = run_scan(ctx, &qv, plan, slot, slot.stream, table, tlc, stats, 0, &pass, resident)) return rc;
-            continue;
-        }
-        int rc = run_scan(ctx, &qv, plan, slot, slot.stream, table, tlc, stats, 0, &pass);
-        cudaError_t ce = cudaStreamSynchronize(slot.stream);  // also on failure: nothing may be in flight when the slot goes back
-        if (!rc && ce != cudaSuccess) rc = fail(BYDB_EIO, cudaGetErrorString(ce));
-        if (!rc) rc = collect_scan(slot, stats);
-        if (rc) return rc;
-    }
-    return 0;
-}
-
-// the key table of a keyed answer: value k is `values[k]`
-template <class Out>
-void set_key_table(Out *out, KeyedOwner *owner, const KeyValues &values) {
-    owner->key_off.assign(1, 0);
-    owner->key_bytes.clear();
-    for (const auto &v : values) {
-        owner->key_bytes.insert(owner->key_bytes.end(), v.begin(), v.end());
-        owner->key_off.push_back(static_cast<uint32_t>(owner->key_bytes.size()));
-    }
-    if (owner->key_bytes.empty()) owner->key_bytes.push_back(0);
-    out->n_keys = static_cast<int32_t>(values.size());
-    out->key_off = owner->key_off.data();
-    out->key_bytes = owner->key_bytes.data();
-}
-
-// 3. insertion order of the V x G composite groups from where each series first shows each value (kts / krow): ko.perm lists
-// the composite groups v * G + g in insertion order, the *ko.n_present that appeared first, in scratch `kb` (enqueued, not
-// synchronised; the staging of the series groups in slot.pinned is in flight).  `resident`: a keyed step being captured -- its
-// step state holds the order's arrays (the slots preset by the step's reset kernel) and the staging it uploaded before the capture.
-int keyed_order(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, const int64_t *kts, const uint32_t *krow, Scratch &kb,
-                KeyOrderParams &ko, bydb_stats &stats, const KeyOrderParams *resident = nullptr) {
-    cudaStream_t stream = slot.stream;
-    const size_t NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
-    if (resident) {
-        ko = *resident;
-    } else {
-        const StageLayout st = stage_layout(NS, G);
-        Carve carve;
-        const size_t b_slot = carve(NS * V * 4), b_first = carve(GP * 4), b_perm = carve(GP * 4), b_np = carve(16), b_stage = carve(st.bytes);
-        CUDA_TRY(kb.alloc(carve.o, stream));
-        CUDA_TRY(cudaMemsetAsync(kb.base + b_slot, 0xff, NS * V * 4, stream));
-        memset(&ko, 0, sizeof ko);
-        // order | group_start of the series groups: staged again (run_scan's copies live in its own scratch)
-        stage_series(q, st, slot.pinned);
-        CUDA_TRY(cudaMemcpyAsync(kb.base + b_stage, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream));
-        ko.order = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_order);
-        ko.group_start = reinterpret_cast<const int32_t *>(kb.base + b_stage + st.off_gstart);
-        ko.slot = reinterpret_cast<int32_t *>(kb.base + b_slot);
-        ko.first_series = reinterpret_cast<int32_t *>(kb.base + b_first);
-        ko.perm = reinterpret_cast<int32_t *>(kb.base + b_perm);
-        ko.n_present = reinterpret_cast<uint32_t *>(kb.base + b_np);
-    }
-    ko.n_groups = static_cast<int32_t>(G);
-    ko.n_values = static_cast<uint32_t>(V);
-    ko.n_series = static_cast<uint32_t>(NS);
-    ko.Kts = kts;
-    ko.Krow = krow;
-    launch_key_order(ko, stream);
-    stats.kernel_launches += 2;
-    return 0;
-}
-
-// the rows of a finalised keyed answer, which come out of the finalisation in composite terms, as (series group, key value):
-// row r takes pairs[2r] / pairs[2r + 1]
-void set_row_keys(bydb_keyed_result *out, KeyedOwner *owner, const int32_t *pairs) {
-    auto *ro = static_cast<ResultOwner *>(out->base.owner);
-    owner->key_id.resize(ro->group_id.size());
-    for (size_t r = 0; r < ro->group_id.size(); ++r) {
-        ro->group_id[r] = pairs[2 * r];
-        owner->key_id[r] = pairs[2 * r + 1];
-    }
-    out->key_id = owner->key_id.data();
-}
-
-// 4a. bydb_scan_agg_keyed / bydb_scan_reduce_keyed: after the order, the table at `table` reordered, the ordinary finalisation /
-// Top-N on it, and the rows mapped back to (series group, key value).  The caller sized the slot's pinned staging with
-// keyed_pinned_bytes.
-int keyed_finish(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
-                 const int64_t *kts, const uint32_t *krow, bydb_keyed_result *out, KeyedOwner *owner) {
-    cudaStream_t stream = slot.stream;
-    const size_t F = plan.fcols.size(), G = static_cast<size_t>(plan.n_groups), GP = G * V;
-    Scratch kb, dst;
-    KeyOrderParams ko;
-    int rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, out->base.stats);
-    if (rc) return rc;
-    CUDA_TRY(dst.alloc(tlc.total, stream));
-    launch_permute_table(tlc.at(dst.base), tlc.at(table), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), coltype,
-                         static_cast<uint32_t>(V), stream);
-    CUDA_TRY(cudaStreamSynchronize(stream));  // the staging above is reused by the finalisation's read-back
-    out->base.stats.kernel_launches += 1;
-    Plan planc = plan;
-    planc.n_groups = static_cast<int32_t>(GP);
-    rc = finalize_to_host(q, planc, slot, stream, dst.base, tlc, &out->base, true);
-    if (rc) {
-        cudaStreamSynchronize(stream);
-        return rc;
-    }
-    std::vector<int32_t> perm(GP);
-    CUDA_TRY(cudaMemcpyAsync(perm.data(), ko.perm, GP * 4, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    out->base.stats.d2h_bytes += GP * 4;
-    // rows carry the position in insertion order: back to (group of the series, key value)
-    const std::vector<int32_t> &pos = static_cast<ResultOwner *>(out->base.owner)->group_id;
-    std::vector<int32_t> pairs(2 * pos.size());
-    for (size_t r = 0; r < pos.size(); ++r) {
-        const int32_t comp = perm[static_cast<size_t>(pos[r])];
-        pairs[2 * r] = comp % static_cast<int32_t>(G);
-        pairs[2 * r + 1] = comp / static_cast<int32_t>(G);
-    }
-    set_row_keys(out, owner, pairs.data());
-    return 0;
-}
-
-// 4b. bydb_scan_partials_keyed / bydb_scan_reduce_keyed_partials: after the order, keyed_partial_rows_kernel writes the wire rows
-// of the present composite groups from the unpermuted table into one packed image; the read-back takes the control word, then
-// exactly n_present rows.  The composite table never leaves the device.
-int keyed_rows(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
-               const int64_t *kts, const uint32_t *krow, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
-    cudaStream_t stream = slot.stream;
-    const size_t F = plan.fcols.size(), G = static_cast<size_t>(plan.n_groups), GP = G * V, A = q->n_aggs;
-    const size_t ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
-    Scratch kb, img;
-    KeyOrderParams ko;
-    int rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, out->stats);
-    if (rc) return rc;
-    CUDA_TRY(img.alloc(ctl_bytes + GP * row_bytes, stream));
-    launch_keyed_partial_rows(rows_params(q, plan, V, tlc.at(table), coltype, ko.perm, ko.n_present, img.base), GP, stream);
-    out->stats.kernel_launches += 1;
-    // 1. the control word (behind the staging copy that reads slot.pinned, on the same stream)
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base, ctl_bytes, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    CUDA_TRY(cudaGetLastError());
-    out->stats.d2h_bytes += ctl_bytes;
-    rc = rows_status(slot.pinned, F);
-    if (rc) return rc;
-    const size_t n = rows_in(slot.pinned, GP);
-    // 2. the rows, right behind the control word
-    if (n) {
-        CUDA_TRY(cudaMemcpyAsync(slot.pinned + ctl_bytes, img.base + ctl_bytes, n * row_bytes, cudaMemcpyDeviceToHost, stream));
-        CUDA_TRY(cudaStreamSynchronize(stream));
-        out->stats.d2h_bytes += n * row_bytes;
-    }
-    rc = parse_rows(slot.pinned, q, plan, GP, &out->base, &owner->key_id);
-    if (rc) return rc;
-    out->key_id = owner->key_id.data();
-    return 0;
-}
-
-// the pinned staging of the ordering and the read-back of a keyed answer over GP composite groups
-size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_result *) {
-    return step_pinned_bytes(q, static_cast<size_t>(plan.n_groups), GP);
-}
-size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_partial_rows *) {
-    return std::max(stage_layout(q->n_series, static_cast<size_t>(plan.n_groups)).stride, keyed_ctl_bytes(plan.fcols.size()) + GP * keyed_row_bytes(q->n_aggs));
-}
-
-int keyed_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
-               const int64_t *kts, const uint32_t *krow, bydb_keyed_result *out, KeyedOwner *owner) {
-    return keyed_finish(q, plan, slot, V, table, tlc, coltype, kts, krow, out, owner);
-}
-int keyed_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, size_t V, uint8_t *table, const TableLayout &tlc, const int64_t *coltype,
-               const int64_t *kts, const uint32_t *krow, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
-    return keyed_rows(q, plan, slot, V, table, tlc, coltype, kts, krow, out, owner);
-}
-
-void keyed_free(bydb_ctx *ctx, bydb_keyed_result *out) { bydb_keyed_result_free(ctx, out); }
-void keyed_free(bydb_ctx *ctx, bydb_keyed_partial_rows *out) { bydb_keyed_partial_rows_free(ctx, out); }
-
-// a failure past the point where the result owns memory must not leave a half-filled result with the caller
-template <class Out>
-struct KeyedUndo {
-    bydb_ctx *ctx;
-    Out *out;
-    bool done = false;
-    ~KeyedUndo() {
-        if (!done) keyed_free(ctx, out);
-    }
-};
-
-// bydb_scan_agg_keyed and bydb_scan_partials_keyed: discovery, the per-value passes, the order, then the form's own answer
-template <class Out>
-int scan_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
-    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
-    memset(out, 0, sizeof *out);
-    int rc = validate_query(q, true);
-    if (rc) return rc;
-    uint32_t cap = 0;
-    rc = check_group_key(q, key, cap);
-    if (rc) return rc;
-    g_last_dev_err = 0;
-    Plan plan;
-    rc = make_plan(ctx, q, nullptr, plan);
-    if (rc) return rc;
-    if (parts_overlap(plan.parts, q->tmin, q->tmax))
-        return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    SlotLease lease(ctx);
-    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
-    ExecSlot &slot = *lease.slot;
-    cudaStream_t stream = slot.stream;
-    const size_t F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups);
-    bydb_stats &stats = keyed_stats(out);
-    memset(&stats, 0, sizeof stats);
-
-    KeyValues values;
-    rc = discover_keys(ctx, q, key, cap, plan, slot, &stats, values);
-    if (rc) return rc;
-    const size_t V = values.size();
-    auto owner = new KeyedOwner();
-    out->owner = owner;
-    KeyedUndo<Out> undo{ctx, out};
-    set_key_table(out, owner, values);
-    if (V == 0) {  // no block selected: no rows (n_rows = 0)
-        undo.done = true;
-        return 0;
-    }
-
-    const size_t GP = G * V;
-    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
-    TableLayout tlc(GP, F);
-    Carve carve;
-    const size_t b_src = carve(tlc.total), b_ct = carve(V * F * 8), b_kts = carve(V * NS * 8), b_krow = carve(V * NS * 4);
-    Scratch kb;
-    CUDA_TRY(kb.alloc(carve.o, stream));
-    CUDA_TRY(cudaMemsetAsync(kb.base + b_ct, 0, V * F * 8, stream));
-    if (slot.ensure_pinned(keyed_pinned_bytes(q, plan, GP, out))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    int64_t *ct = reinterpret_cast<int64_t *>(kb.base + b_ct), *kts = reinterpret_cast<int64_t *>(kb.base + b_kts);
-    uint32_t *krow = reinterpret_cast<uint32_t *>(kb.base + b_krow);
-    rc = run_keyed_passes(ctx, q, key, plan, slot, values, tlc, kb.base + b_src, ct, kts, krow, nullptr, &stats);
-    if (!rc) rc = keyed_emit(q, plan, slot, V, kb.base + b_src, tlc, ct, kts, krow, out, owner);
-    if (rc) return rc;
-    undo.done = true;
-    return 0;
-}
-
-// ---- bydb_scan_agg_keyed_wide / bydb_scan_partials_keyed_wide: one scan pass (see "Wide group key" in scan_kernels.cu)
-int check_wide_key(const bydb_group_key *key, uint32_t &cap) {
-    if (!key || !key->family || !key->tag) return fail(BYDB_EINVAL, "group key without family/tag");
-    if (key->value_type != 0 && key->value_type != BYDB_VT_STR && key->value_type != BYDB_VT_BINARY && key->value_type != BYDB_VT_INT64)
-        return fail(BYDB_EINVAL, "bydb_group_key.value_type must be 0, BYDB_VT_STR, BYDB_VT_BINARY or BYDB_VT_INT64");
-    cap = key->max_values ? key->max_values : 64u;
-    if (cap > kMaxWideKeyValues) return fail(BYDB_EINVAL, "bydb_group_key.max_values above 65536");
-    return 0;
-}
-
-size_t pow2_at_least(size_t n) {
-    size_t p = 1;
-    while (p < n) p <<= 1;
-    return p;
-}
-
-// the composite groups' (series group, key value) back onto rows that carry the position in insertion order
-void wide_row_keys(const std::vector<int32_t> &pairs, std::vector<int32_t> &group_id, std::vector<int32_t> &key_id) {
-    key_id.resize(group_id.size());
-    for (size_t r = 0; r < group_id.size(); ++r) {
-        const size_t j = static_cast<size_t>(group_id[r]);
-        group_id[r] = pairs[2 * j];
-        key_id[r] = pairs[2 * j + 1];
-    }
-}
-
-// the answer forms over the present composite table (n_comp groups of layout tl at `table`, pairs at d_pairs)
-int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const int32_t *d_pairs,
-              const int32_t *, const uint32_t *, bydb_keyed_result *out, KeyedOwner *owner) {
-    cudaStream_t stream = slot.stream;
-    Plan planc = plan;
-    planc.n_groups = static_cast<int32_t>(n_comp);
-    int rc = finalize_to_host(q, planc, slot, stream, table, tl, &out->base, true);
-    if (rc) return rc;
-    std::vector<int32_t> pairs(2 * n_comp);
-    CUDA_TRY(cudaMemcpyAsync(pairs.data(), d_pairs, pairs.size() * 4, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    out->base.stats.d2h_bytes += pairs.size() * 4;
-    auto *ro = static_cast<ResultOwner *>(out->base.owner);
-    wide_row_keys(pairs, ro->group_id, owner->key_id);
-    out->key_id = owner->key_id.data();
-    return 0;
-}
-int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const int32_t *d_pairs,
-              const int32_t *d_perm, const uint32_t *d_ncomp, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
-    cudaStream_t stream = slot.stream;
-    const size_t F = plan.fcols.size(), A = q->n_aggs, ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
-    Plan planc = plan;
-    planc.n_groups = static_cast<int32_t>(n_comp);
-    Scratch img;
-    CUDA_TRY(img.alloc(ctl_bytes + n_comp * row_bytes, stream));
-    const TablePtrs t = tl.at(table);
-    launch_keyed_partial_rows(rows_params(q, planc, 1, t, t.coltype, d_perm, d_ncomp, img.base), n_comp, stream);
-    out->stats.kernel_launches += 1;
-    if (slot.ensure_pinned(ctl_bytes + n_comp * row_bytes)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, img.base, ctl_bytes + n_comp * row_bytes, cudaMemcpyDeviceToHost, stream));
-    std::vector<int32_t> pairs(2 * n_comp);
-    CUDA_TRY(cudaMemcpyAsync(pairs.data(), d_pairs, pairs.size() * 4, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    CUDA_TRY(cudaGetLastError());
-    out->stats.d2h_bytes += ctl_bytes + n_comp * row_bytes + pairs.size() * 4;
-    int rc = parse_rows(slot.pinned, q, planc, n_comp, &out->base, nullptr);
-    if (rc) return rc;
-    auto *ro = static_cast<PartialRowsOwner *>(out->base.owner);
-    wide_row_keys(pairs, ro->group_id, owner->key_id);
-    out->key_id = owner->key_id.data();
-    return 0;
-}
-
-template <class Out>
-int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
-    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
-    memset(out, 0, sizeof *out);
-    int rc = validate_query(q, true);
-    if (rc) return rc;
-    uint32_t cap = 0;
-    rc = check_wide_key(key, cap);
-    if (rc) return rc;
-    g_last_dev_err = 0;
-    Plan plan;
-    rc = make_plan(ctx, q, nullptr, plan);
-    if (rc) return rc;
-    if (parts_overlap(plan.parts, q->tmin, q->tmax))
-        return fail(BYDB_ENOTSUP, "group-key query over parts that overlap in time (version dedup) is not supported on the device path");
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    SlotLease lease(ctx);
-    if (lease.init()) return fail(BYDB_EIO, "cannot create stream");
-    ExecSlot &slot = *lease.slot;
-    cudaStream_t stream = slot.stream;
-    const bool int64_key = key->value_type == BYDB_VT_INT64;
-    const size_t F = plan.fcols.size(), NS = q->n_series, NB = plan.total_blocks, NBp = align_up(std::max<size_t>(NB, 1), 1024);
-    bydb_stats &stats = keyed_stats(out);
-    memset(&stats, 0, sizeof stats);
-    cudaEvent_t *ev = slot.ev;
-    CUDA_TRY(cudaEventRecord(ev[0], stream));
-
-    // 1. discovery: the value table (S slots), each selected block's rank and distinct values, then their exclusive scan
-    const size_t S = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(cap), kKeySlots));
-    Carve carve;
-    const size_t a_sids = carve(NS * 8), a_grp = carve(NS * 4), a_slots = carve(S * 8), a_ctl = carve(32), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
-                 a_lens = carve(static_cast<size_t>(cap) * 4), a_sid = carve(S * 4), a_nbr = carve(NBp * 4), a_rank = carve(NB * 4),
-                 a_tiles = carve(NBp / 1024 * 4);
-    Scratch ka;
-    CUDA_TRY(ka.alloc(carve.o, stream));
-    if (slot.ensure_pinned(std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    memcpy(slot.pinned, q->series_ids, NS * 8);
-    int32_t *hg = reinterpret_cast<int32_t *>(slot.pinned + NS * 8);
-    for (size_t i = 0; i < NS; ++i) hg[i] = q->series_group ? q->series_group[i] : 0;
-    if (NS) {
-        CUDA_TRY(cudaMemcpyAsync(ka.base + a_sids, slot.pinned, NS * 8, cudaMemcpyHostToDevice, stream));
-        CUDA_TRY(cudaMemcpyAsync(ka.base + a_grp, slot.pinned + NS * 8, NS * 4, cudaMemcpyHostToDevice, stream));
-    }
-    stats.h2d_bytes += NS * 12;
-    CUDA_TRY(cudaMemsetAsync(ka.base + a_slots, 0, a_vals - a_slots, stream));
-    CUDA_TRY(cudaMemsetAsync(ka.base + a_nbr, 0, NBp * 4, stream));
-    WideKeyParams wk;
-    memset(&wk, 0, sizeof wk);
-    KeyParams &kp = wk.k;
-    part_refs(plan.parts, kp.parts);
-    kp.n_parts = static_cast<uint32_t>(plan.parts.size());
-    kp.total_blocks = static_cast<uint32_t>(NB);
-    kp.q_sids = reinterpret_cast<const uint64_t *>(ka.base + a_sids);
-    kp.n_series = static_cast<uint32_t>(NS);
-    kp.cap = cap;
-    kp.tmin = q->tmin;
-    kp.tmax = q->tmax;
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        kp.key_name = ctx->names.find(std::string("t:") + key->family + "/" + key->tag);
-    }
-    uint32_t *d_ctl = reinterpret_cast<uint32_t *>(ka.base + a_ctl);  // [0] values [1] DevErr [2] its block [3] int64 zero [4] R
-    kp.slots = reinterpret_cast<unsigned long long *>(ka.base + a_slots);
-    kp.count = d_ctl;
-    kp.err = d_ctl + 1;
-    kp.zero = d_ctl + 3;
-    kp.vals = ka.base + a_vals;
-    kp.lens = reinterpret_cast<uint32_t *>(ka.base + a_lens);
-    wk.slot_mask = static_cast<uint32_t>(S - 1);
-    wk.int64_key = int64_key ? 1u : 0u;
-    wk.slot_id = reinterpret_cast<uint32_t *>(ka.base + a_sid);
-    wk.n_by_rank = reinterpret_cast<uint32_t *>(ka.base + a_nbr);
-    wk.rank = reinterpret_cast<uint32_t *>(ka.base + a_rank);
-    launch_key_values_wide(wk, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
-    launch_excl_scan(wk.n_by_rank, static_cast<uint32_t>(NBp), reinterpret_cast<uint32_t *>(ka.base + a_tiles), d_ctl + 4, stream);
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, d_ctl, 32, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    CUDA_TRY(cudaGetLastError());
-    stats.kernel_launches += (NB ? 1u : 0u) + 1u + 3u;
-    stats.d2h_bytes += 32;
-    uint32_t ctl[8];
-    memcpy(ctl, slot.pinned, 32);
-    if (ctl[1] != 0) {
-        g_last_dev_err = ctl[1];
-        char buf[64];
-        snprintf(buf, sizeof buf, " (block #%u)", ctl[2]);
-        return fail(dev_err_code(ctl[1]), std::string(dev_err_text(ctl[1])) + buf);
-    }
-    const size_t V = std::min<size_t>(ctl[0], cap), R = ctl[4];
-    KeyValues values(V);
-    if (V) {
-        const size_t vb = V * (int64_key ? 8 : kMaxLit);
-        CUDA_TRY(cudaMemcpyAsync(slot.pinned, kp.vals, vb, cudaMemcpyDeviceToHost, stream));
-        if (!int64_key) CUDA_TRY(cudaMemcpyAsync(slot.pinned + vb, kp.lens, V * 4, cudaMemcpyDeviceToHost, stream));
-        CUDA_TRY(cudaStreamSynchronize(stream));
-        stats.d2h_bytes += vb + (int64_key ? 0 : V * 4);
-        const uint32_t *hl = reinterpret_cast<const uint32_t *>(slot.pinned + vb);
-        for (size_t v = 0; v < V; ++v) {
-            if (int64_key) values[v].assign(slot.pinned + v * 8, slot.pinned + v * 8 + 8);  // the reference's key bytes: little-endian int64
-            else values[v].assign(slot.pinned + v * kMaxLit, slot.pinned + v * kMaxLit + hl[v]);
-        }
-    }
-    auto owner = new KeyedOwner();
-    out->owner = owner;
-    KeyedUndo<Out> undo{ctx, out};
-    set_key_table(out, owner, values);
-    if (V == 0 || R == 0) {  // no block selected: no rows (n_rows = 0)
-        undo.done = true;
-        return 0;
-    }
-    if (R > 0x7fffffffull) return fail(BYDB_ENOMEM, "wide group-key query: too many (block, key value) records");
-
-    // 2. the scan: one record per present (block, key value)
-    const size_t rec_bytes = wide_record_bytes(F);
-    const size_t C = pow2_at_least(std::max<size_t>(2 * R, 1024)), N = pow2_at_least(std::max<size_t>(R, 2048));
-    Carve cb;
-    const size_t b_zero = cb(kZeroPageBytes), b_rec = cb(R * rec_bytes), b_comp = cb(C * 8), b_cmin = cb(C * 4), b_rslot = cb(R * 4), b_keys = cb(N * 8),
-                 b_heads = cb(N * 4), b_tiles = cb(N / 1024 * 4), b_ctl = cb(8), b_seg = cb(R * 4);
-    Scratch sb;
-    CUDA_TRY(sb.alloc(cb.o, stream));
-    ZeroPage *z = reinterpret_cast<ZeroPage *>(sb.base + b_zero);
-    CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
-    CUDA_TRY(cudaMemsetAsync(sb.base + b_comp, 0, C * 8, stream));
-    CUDA_TRY(cudaMemsetAsync(sb.base + b_cmin, 0xff, C * 4, stream));
-    CUDA_TRY(cudaMemsetAsync(sb.base + b_ctl, 0, 8, stream));
-    ScanParams sp;
-    memset(&sp, 0, sizeof sp);
-    part_refs(plan.parts, sp.parts);
-    sp.n_parts = static_cast<uint32_t>(plan.parts.size());
-    sp.total_blocks = static_cast<uint32_t>(NB);
-    sp.q_sids = kp.q_sids;
-    sp.n_series = static_cast<uint32_t>(NS);
-    sp.n_fcols = static_cast<uint32_t>(F);
-    scan_query_params(ctx, q, plan, sp);
-    sp.err = z->err;
-    sp.stats = z->stats;
-    sp.col_type = z->col_type;
-    WideScanParams ws;
-    memset(&ws, 0, sizeof ws);
-    ws.slots = kp.slots;
-    ws.slot_id = wk.slot_id;
-    ws.zero = kp.zero;
-    ws.slot_mask = wk.slot_mask;
-    ws.int64_key = wk.int64_key;
-    ws.key_name = kp.key_name;
-    ws.rank = wk.rank;
-    ws.rec_off = wk.n_by_rank;
-    ws.series_group = reinterpret_cast<const int32_t *>(ka.base + a_grp);
-    ws.records = sb.base + b_rec;
-    CUDA_TRY(cudaEventRecord(ev[1], stream));
-    launch_scan_keyed_wide(sp, ws, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
-    CUDA_TRY(cudaEventRecord(ev[2], stream));
-
-    // 3. the composite groups in insertion order
-    WideReduceParams rp;
-    memset(&rp, 0, sizeof rp);
-    rp.records = ws.records;
-    rp.n_records = static_cast<uint32_t>(R);
-    rp.n_fcols = static_cast<uint32_t>(F);
-    rp.comp = reinterpret_cast<unsigned long long *>(sb.base + b_comp);
-    rp.comp_min = reinterpret_cast<uint32_t *>(sb.base + b_cmin);
-    rp.rec_slot = reinterpret_cast<uint32_t *>(sb.base + b_rslot);
-    rp.comp_mask = static_cast<uint32_t>(C - 1);
-    rp.n_sort = static_cast<uint32_t>(N);
-    rp.keys = reinterpret_cast<unsigned long long *>(sb.base + b_keys);
-    rp.heads = reinterpret_cast<uint32_t *>(sb.base + b_heads);
-    rp.tile_sums = reinterpret_cast<uint32_t *>(sb.base + b_tiles);
-    rp.ctl = reinterpret_cast<uint32_t *>(sb.base + b_ctl);
-    rp.seg_start = reinterpret_cast<uint32_t *>(sb.base + b_seg);
-    rp.col_type = z->col_type;
-    rp.scan_err = z->err;
-    launch_wide_order(rp, stream);
-    ZeroPage *hz = slot.page(0);
-    CUDA_TRY(cudaMemcpyAsync(hz, z, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, rp.ctl, 8, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    CUDA_TRY(cudaGetLastError());
-    uint32_t sort_launches = 0;
-    for (size_t size = 4096; size <= N; size <<= 1) sort_launches += 1 + static_cast<uint32_t>(__builtin_ctzll(size) - 11);
-    stats.kernel_launches += (NB ? 1u : 0u) + 2u + 1u + sort_launches + 1u + 3u + 1u;
-    stats.d2h_bytes += kZeroPageBytes + 8;
-    {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, ev[1], ev[2]);
-        stats.scan_kernel_ms += ms;
-    }
-    rc = read_zero_page(*hz, false, &stats);
-    if (rc) return rc;
-    const size_t n_comp = reinterpret_cast<const uint32_t *>(slot.pinned)[1];
-
-    // 4. the fold into a table of the present composite groups, then the form's own answer
-    const TableLayout tl(std::max<size_t>(n_comp, 1), F);
-    Carve cf;
-    const size_t f_table = cf(tl.total), f_pairs = cf(n_comp * 8), f_perm = cf(n_comp * 4);
-    Scratch fb;
-    CUDA_TRY(fb.alloc(cf.o, stream));
-    rp.table = tl.at(fb.base + f_table);
-    rp.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
-    rp.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
-    launch_wide_fold(rp, static_cast<uint32_t>(n_comp), stream);
-    CUDA_TRY(cudaEventRecord(ev[3], stream));
-    stats.kernel_launches += 1;
-    if (n_comp > 0) rc = wide_emit(q, plan, slot, fb.base + f_table, tl, n_comp, rp.pairs, rp.perm, &rp.ctl[1], out, owner);
-    if (rc) return rc;
-    {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, ev[0], ev[3]);
-        stats.device_ms += ms;
-    }
-    undo.done = true;
-    return 0;
-}
-}  // namespace
-}  // extern "C++"
 
 void bydb_encoded_pages_free(bydb_ctx *ctx, bydb_encoded_pages *r);
 
@@ -2681,257 +2900,6 @@ void bydb_keyed_result_free(bydb_ctx *ctx, bydb_keyed_result *r) {
     memset(r, 0, sizeof *r);
 }
 
-// ------------------------------------------------------------------------------------------------
-// Prepared group-by on a stored tag: the V passes, the insertion order, the finalisation and the row mapping captured as ONE
-// graph.  Discovery runs once per capture: its inputs (the parts a handle names, series, range, key) are fixed while the handles
-// keep naming the parts the step was captured with, so the key table is a property of the capture, like the block plan.
-// Everything here is additive: bydb_scan_agg_keyed is untouched.
-// ------------------------------------------------------------------------------------------------
-extern "C++" {
-struct bydb_prepared_keyed {
-    bydb_prepared *pq = nullptr;   // the query's deep copy, its slot, events, graph, step state and held parts
-    std::string family, tag;       // the key's strings: key.family / key.tag point here
-    bydb_group_key key{};
-    uint32_t cap = 0;              // distinct values accepted (check_group_key)
-    KeyValues values;              // found when the step was captured: the key table of every replay
-    bool no_values = false;        // discovery found no value (V = 0): the answer is empty and needs no graph
-    size_t pairs_off = 0, zero_off = 0;  // in the replay's read-back image: the rows' (group, key) pairs, the passes' zero pages
-    ~bydb_prepared_keyed() { prepared_destroy(pq); }
-};
-
-namespace {
-// Discovers the key values and captures the keyed step into k->pq->exec, in a step state of its own:
-//   composite table | permuted table | the passes' column types | Kts | Krow | the order's slots, first_series, perm, n_present |
-//   one scan scratch (scan_layout, the passes run one after another) | finalisation over V x G groups, then the rows' (group, key)
-//   pairs and the V zero pages, so that one copy reads back the rows, their pairs and the passes' counters and errors.
-// `partial` (bydb_scan_partials_keyed_prepared) selects the other tail: no permuted table and no finalisation; behind the order,
-// keyed_partial_rows_kernel writes the row image (control word, rows) right behind the V zero pages, and rows_to_host_kernel
-// brings the pages, the control word and exactly the present rows to the staging.
-// Leaves neither a graph nor no_values when this execution, or (capturable cleared) every later one, takes the plain path: a part
-// is missing, the parts overlap, discovery fails (its refusal is the plain call's), or the state or the capture cannot be had.
-void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
-    bydb_prepared *p = k->pq;
-    const bydb_query *q = &p->q;
-    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up
-    Plan plan;
-    if (make_plan(ctx, q, nullptr, plan)) return;
-    ExecSlot &slot = *p->slot;
-    cudaStream_t stream = slot.stream;
-    bydb_stats discovery{};
-    KeyValues values;
-    if (parts_overlap(plan.parts, q->tmin, q->tmax) || discover_keys(ctx, q, &k->key, k->cap, plan, slot, &discovery, values)) {
-        p->capturable = false;
-        return;
-    }
-    const size_t V = values.size(), F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
-    if (V == 0) {
-        k->values.clear();
-        k->no_values = true;
-        p->held = plan.parts;
-        p->held_gen = gen;
-        return;
-    }
-    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) {
-        p->capturable = false;
-        return;
-    }
-    const TableLayout tlc(GP, F);
-    const StageLayout st = stage_layout(NS, G);
-    const ScanLayout sl = scan_layout(st, plan.total_blocks, F, plan.parts.size(), true);
-    const FinalLayout fl = final_layout(GP, q->n_aggs, q->top_n);
-    const size_t b_pairs = align_up(fl.cap * 8, 256), b_zero = V * kZeroPageBytes;
-    const size_t b_rows = keyed_ctl_bytes(F) + GP * keyed_row_bytes(q->n_aggs);  // partial: the row image
-    Carve carve;
-    const size_t o_src = carve(tlc.total), o_dst = carve(partial ? 0 : tlc.total), o_ct = carve(V * F * 8), o_kts = carve(V * NS * 8),
-                 o_krow = carve(V * NS * 4), o_slot = carve(NS * V * 4), o_first = carve(GP * 4), o_perm = carve(GP * 4), o_np = carve(16),
-                 o_scan = carve(sl.total), o_fin = carve(partial ? b_zero + b_rows : fl.total + b_pairs + b_zero);
-    p->host_off = st.stride;  // the read-back lands behind the staging area, as in the plain prepared step
-    p->read_back = partial ? b_zero + b_rows : fl.out_bytes + b_pairs + b_zero;  // partial: the most the copy kernel may write
-    // sized before the capture: the graph writes the staging through its device address
-    uint8_t *h_dst = slot.ensure_pinned(p->host_off + p->read_back) ? nullptr : slot.pinned_dev(p->host_off);
-    if (!h_dst || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
-        cudaGetLastError();
-        p->step_state = nullptr;
-        p->capturable = false;
-        return;
-    }
-    uint8_t *S = p->step_state, *fin_base = S + o_fin, *zero_pages = partial ? fin_base : fin_base + fl.total + b_pairs;
-    // the staging goes up once: the passes and the order read it from the step state on every replay
-    stage_series(q, st, slot.pinned);
-    cudaError_t e = cudaMemcpyAsync(S + o_scan + sl.off_sids, slot.pinned, st.bytes, cudaMemcpyHostToDevice, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    if (e == cudaSuccess) e = cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        drop_step(p);
-        p->capturable = false;
-        return;
-    }
-    bydb_stats &cs = p->captured;
-    memset(&cs, 0, sizeof cs);
-    int64_t *ct = reinterpret_cast<int64_t *>(S + o_ct), *kts = reinterpret_cast<int64_t *>(S + o_kts);
-    uint32_t *krow = reinterpret_cast<uint32_t *>(S + o_krow);
-    KeyedResetParams rp;
-    memset(&rp, 0, sizeof rp);
-    rp.zero[0] = reinterpret_cast<uint32_t *>(ct);
-    rp.n_zero[0] = V * F * 2;
-    rp.zero[1] = reinterpret_cast<uint32_t *>(zero_pages);
-    rp.n_zero[1] = b_zero / 4;
-    rp.ones[0] = sl.n_first ? reinterpret_cast<uint32_t *>(S + o_scan + sl.off_first) : nullptr;
-    rp.n_ones[0] = sl.n_first;
-    rp.ones[1] = reinterpret_cast<uint32_t *>(S + o_slot);
-    rp.n_ones[1] = NS * V;
-    launch_keyed_step_reset(rp, stream);
-    cs.kernel_launches += 1;
-    Scratch scan, kb, fin;
-    scan.view(S + o_scan, sl.total);
-    fin.view(fin_base, fl.total + b_pairs + b_zero);
-    int rc = run_keyed_passes(ctx, q, &k->key, plan, slot, values, tlc, S + o_src, ct, kts, krow, nullptr, &cs, &scan, zero_pages);
-    KeyOrderParams res, ko;
-    memset(&res, 0, sizeof res);
-    res.order = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_order);
-    res.group_start = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_gstart);
-    res.slot = reinterpret_cast<int32_t *>(S + o_slot);
-    res.first_series = reinterpret_cast<int32_t *>(S + o_first);
-    res.perm = reinterpret_cast<int32_t *>(S + o_perm);
-    res.n_present = reinterpret_cast<uint32_t *>(S + o_np);
-    if (!rc) rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, cs, &res);
-    FinalLayout flc;
-    uint32_t fin_launches = 0;
-    size_t fin_back = 0;
-    if (!rc && partial) {
-        launch_keyed_partial_rows(rows_params(q, plan, V, tlc.at(S + o_src), ct, ko.perm, ko.n_present, zero_pages + b_zero), GP, stream);
-        RowsCopyParams cp;
-        memset(&cp, 0, sizeof cp);
-        cp.pages = zero_pages;
-        cp.image = zero_pages + b_zero;
-        cp.dst = h_dst;
-        cp.page_bytes = b_zero;
-        cp.ctl_bytes = keyed_ctl_bytes(F);
-        cp.row_bytes = keyed_row_bytes(q->n_aggs);
-        cp.max_rows = static_cast<uint32_t>(GP);
-        launch_rows_to_host(cp, stream);
-    } else if (!rc) {
-        launch_permute_table(tlc.at(S + o_dst), tlc.at(S + o_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), ct,
-                             static_cast<uint32_t>(V), stream);
-        Plan planc = plan;
-        planc.n_groups = static_cast<int32_t>(GP);
-        rc = finalize_launch(q, planc, stream, S + o_dst, tlc, fin, flc, fin_launches, fin_back);
-        if (!rc) {
-            launch_keyed_row_map(reinterpret_cast<const int32_t *>(fin_base + fl.o_sg), reinterpret_cast<const uint32_t *>(fin_base + fl.o_cnt),
-                                 ko.perm, static_cast<uint32_t>(G), static_cast<uint32_t>(fl.cap), reinterpret_cast<int32_t *>(fin_base + fl.total), stream);
-            if (cudaMemcpyAsync(slot.pinned + p->host_off, fin_base + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
-        }
-    }
-    cudaGraph_t graph = nullptr;
-    e = cudaStreamEndCapture(stream, &graph);
-    if (!rc && e == cudaSuccess && graph) e = cudaGraphInstantiate(&p->exec, graph, 0);
-    if (graph) cudaGraphDestroy(graph);
-    if (rc || e != cudaSuccess || !p->exec) {
-        cudaGetLastError();
-        drop_step(p);
-        p->capturable = false;
-        return;
-    }
-    // permute_table, finalisation + row selection, the row mapping; or the row kernel and the copy kernel.  A partial step's read-back
-    // is sized by the rows present: the replay counts it.
-    cs.kernel_launches += partial ? 2 : 1 + fin_launches + 1;
-    cs.d2h_bytes = partial ? 0 : p->read_back;
-    p->partial_step = partial;
-    p->fl = fl;
-    p->express = false;  // the key predicate keeps every pass off the express lane
-    k->values = std::move(values);
-    k->no_values = false;
-    k->pairs_off = fl.out_bytes;
-    k->zero_off = partial ? 0 : fl.out_bytes + b_pairs;
-    p->held = plan.parts;
-    p->held_gen = gen;
-}
-
-// the answer of a replayed keyed step from its read-back `image`, after the passes' zero pages: the finalised rows and their
-// (group, key) pairs, or the row image (table status, rows, their key values) and the bytes the copy kernel brought back
-int keyed_answer(bydb_prepared_keyed *k, const Plan &, const uint8_t *image, bydb_keyed_result *out, KeyedOwner *owner) {
-    const int rc = finalize_parse(image, k->pq->fl, true, &out->base);
-    if (rc) return rc;
-    set_row_keys(out, owner, reinterpret_cast<const int32_t *>(image + k->pairs_off));
-    return 0;
-}
-int keyed_answer(bydb_prepared_keyed *k, const Plan &shape, const uint8_t *image, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
-    const size_t V = k->values.size(), GP = V * shape.tl.G, A = k->pq->q.n_aggs;
-    const uint8_t *rows = image + V * kZeroPageBytes;
-    out->stats.d2h_bytes += V * kZeroPageBytes + keyed_ctl_bytes(shape.fcols.size()) + rows_in(rows, GP) * keyed_row_bytes(A);
-    const int rc = parse_rows(rows, &k->pq->q, shape, GP, &out->base, &owner->key_id);
-    if (rc) return rc;
-    out->key_id = owner->key_id.data();
-    return 0;
-}
-
-// One replay, synchronised and parsed: the passes' counters add up and the first pass with a device error decides, as the plain
-// path's pass-by-pass collection has it; then the answer of the step's form (keyed_answer).
-template <class Out>
-int keyed_replay(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
-    bydb_prepared *p = k->pq;
-    Plan shape;
-    int rc = query_shape(&p->q, shape);
-    if (rc) return rc;
-    uint8_t *image = p->slot->pinned + p->host_off;
-    const size_t V = k->values.size();
-    // a replay that fails to launch cannot report the previous one's status (nor, in a partial step, its control word)
-    memset(image + k->zero_off, 0, V * kZeroPageBytes + (p->partial_step ? keyed_ctl_bytes(shape.fcols.size()) : 0));
-    auto page = [&](size_t v) -> const ZeroPage & { return *reinterpret_cast<const ZeroPage *>(image + k->zero_off + v * kZeroPageBytes); };
-    bydb_stats &stats = keyed_stats(out);
-    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, false, page(0), &stats);
-    for (size_t v = 1; !rc && v < V; ++v) rc = read_zero_page(page(v), false, &stats);
-    if (rc) return rc;
-    auto owner = new KeyedOwner();
-    out->owner = owner;
-    KeyedUndo<Out> undo{ctx, out};
-    set_key_table(out, owner, k->values);
-    rc = keyed_answer(k, shape, image, out, owner);
-    if (rc) return rc;
-    undo.done = true;
-    return 0;
-}
-
-// bydb_scan_agg_keyed_prepared and bydb_scan_partials_keyed_prepared: one captured step per handle, of the form last asked for
-template <class Out>
-int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
-    if (!ctx || !k || !out) return fail(BYDB_EINVAL, "NULL argument");
-    memset(out, 0, sizeof *out);
-    const bool partial = std::is_same<Out, bydb_keyed_partial_rows>::value;
-    bydb_prepared *p = k->pq;
-    std::lock_guard<std::mutex> lk(p->mu);
-    g_last_dev_err = 0;
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    auto plain = [&] { return scan_keyed_impl(ctx, &p->q, &k->key, out); };
-    // as bydb_scan_agg_prepared: the first execution runs the plain keyed path, the second one captures, later ones replay
-    if (p->runs++ == 0 || !p->capturable) return plain();
-    // the handles can only have changed their parts if one was registered or released since `held` was last compared
-    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
-    if ((p->exec || k->no_values) && gen != p->held_gen) {
-        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
-        if (p->held.empty()) {  // a handle stopped naming its captured part: discovery and the capture run again
-            drop_step(p);
-            k->no_values = false;
-        }
-        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
-        p->held_gen = gen;
-    }
-    if (p->exec && p->partial_step != partial) drop_step(p);  // one step per handle: the other form's gives way
-    if (!p->exec && !k->no_values) {
-        keyed_capture(ctx, k, partial);
-        if (!p->exec && !k->no_values) return plain();
-    }
-    if (k->no_values) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
-        auto owner = new KeyedOwner();
-        out->owner = owner;
-        set_key_table(out, owner, KeyValues());
-        return 0;
-    }
-    return keyed_replay(ctx, k, out);
-}
-}  // namespace
-}  // extern "C++"
 
 int bydb_query_prepare_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out) {
     return guarded([&]() -> int {
@@ -2941,7 +2909,7 @@ int bydb_query_prepare_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_grou
     int rc = validate_query(q, true);
     if (rc) return rc;
     uint32_t cap = 0;
-    rc = check_group_key(q, key, cap);
+    rc = check_group_key(q, key, kMaxKeyValues, true, cap);
     if (rc) return rc;
     std::unique_ptr<bydb_prepared_keyed> k(new bydb_prepared_keyed());
     rc = bydb_query_prepare(ctx, q, &k->pq);
@@ -3572,11 +3540,7 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
     std::lock_guard<std::mutex> lk(p->mu);
     g_last_dev_err = 0;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    // the first execution runs the ordinary path (it also performs the one-time kernel attribute setup); the second one
-    // captures; from then on the graph is replayed
-    const uint64_t run = p->runs++;
-    if (run == 0 || !p->capturable) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
-    int rc = prepared_step(ctx, p, false);
+    int rc = prepared_step(ctx, p, false, [&] { return prepared_capture(ctx, p, false); });
     if (rc) return rc;
     if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
     uint8_t *image = p->slot->pinned + p->zero_image_off;
@@ -3620,10 +3584,7 @@ int bydb_scan_partials_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_partial_ro
     std::lock_guard<std::mutex> lk(p->mu);
     g_last_dev_err = 0;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    // the schedule of bydb_scan_agg_prepared: the uncaptured path, then the capture, then replays
-    const uint64_t run = p->runs++;
-    if (run == 0 || !p->capturable) return scan_partials_rows_impl(ctx, &p->q, out, stats);
-    int rc = prepared_step(ctx, p, true);
+    int rc = prepared_step(ctx, p, true, [&] { return prepared_capture(ctx, p, true); });
     if (rc) return rc;
     if (!p->exec) return scan_partials_rows_impl(ctx, &p->q, out, stats);
     Plan shape;
@@ -3637,7 +3598,7 @@ int bydb_scan_partials_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_partial_ro
     const uint8_t *rows = image + kZeroPageBytes;
     if (!rc) {
         local.d2h_bytes += kZeroPageBytes + ctl_bytes + rows_in(rows, shape.tl.G) * keyed_row_bytes(p->q.n_aggs);
-        rc = parse_rows(rows, &p->q, shape, shape.tl.G, out, nullptr);
+        rc = parse_rows(rows, &p->q, shape, shape.tl.G, out);
     }
     if (stats) *stats = local;
     return rc;
@@ -4035,7 +3996,7 @@ int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key,
     if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
     int rc = validate_query(q, false);
     uint32_t cap = 0;
-    if (!rc) rc = check_group_key(q, key, cap);
+    if (!rc) rc = check_group_key(q, key, kMaxKeyValues, true, cap);
     if (rc) return rc;
     Plan plan;
     rc = query_shape(q, plan);
@@ -4050,16 +4011,14 @@ int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key,
 // appearances (key_union / rank_span_check / combine_keyed / merge_first kernels), then bydb_scan_agg_keyed's ordering and
 // finalisation -- or, for bydb_scan_reduce_keyed_partials, its partial rows.  The root's call decides the form of its answer;
 // every rank contributes the same slot either way, so ranks may mix the two calls in one collective.
-extern "C++" {
+}  // extern "C"
+
 template <class Out>
 static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, Out *out) {
     if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
     memset(out, 0, sizeof *out);
     g_last_dev_err = 0;
-    auto owner = new KeyedOwner();
-    out->owner = owner;
-    KeyedUndo<Out> undo{ctx, out};
-    set_key_table(out, owner, {});
+    KeyedAnswer<Out> answer(ctx, out, {});
     bydb_stats &stats = keyed_stats(out);
     Plan plan;
     uint32_t cap = 0;
@@ -4070,7 +4029,7 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
     CollectiveHooks h;
     h.prepare = [&](ExecSlot &es, size_t slot) -> int {
         int rc = validate_query(q, true);
-        if (!rc) rc = check_group_key(q, key, cap);
+        if (!rc) rc = check_group_key(q, key, kMaxKeyValues, true, cap);
         if (!rc) rc = make_plan(ctx, q, nullptr, plan);
         if (rc) return rc;
         if (parts_overlap(plan.parts, q->tmin, q->tmax))
@@ -4161,13 +4120,7 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
                                           ") lives on several ranks over time spans that intersect");
         }
         const size_t V = std::min<size_t>(ctl[0], cap);
-        KeyValues uvals(V);
-        const uint32_t *hl = reinterpret_cast<const uint32_t *>(es.pinned + (u_lens - u_ctl));
-        for (size_t u = 0; u < V; ++u) {
-            const uint8_t *b = es.pinned + (u_vals - u_ctl) + u * kMaxLit;
-            uvals[u].assign(b, b + std::min<uint32_t>(hl[u], kMaxLit));
-        }
-        set_key_table(out, owner, uvals);
+        set_key_table(out, answer.owner, unpack_values(V, false, es.pinned + (u_vals - u_ctl), reinterpret_cast<const uint32_t *>(es.pinned + (u_lens - u_ctl))));
         if (V == 0) return 0;  // no rank selected a block: no rows
         // ---- the ranks' tables, column types and first appearances folded into the union arrays
         const TableLayout tlu(V * G, F);
@@ -4182,16 +4135,16 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
         up.Krow = reinterpret_cast<uint32_t *>(uc.base + c_krow);
         launch_combine_keyed(up, s);
         stats.kernel_launches += NS ? 2 : 1;
-        return keyed_emit(q, plan, es, V, uc.base + c_table, tlu, up.coltype, up.Kts, up.Krow, out, owner);
+        return keyed_finish(q, plan, es, V, uc.base + c_table, tlu, up.coltype, up.Kts, up.Krow, out, answer.owner);
     };
-    h.discard = [] {};  // the result of a failed call is freed by `undo`
+    h.discard = [] {};  // the result of a failed call is freed by `answer`
     const int rc = run_collective(ctx, root, 0, h);
     if (rc) return rc;
-    undo.done = true;
+    answer.done = true;
     return 0;
 }
 
-}  // extern "C++"
+extern "C" {
 
 int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out) {
     return guarded([&]() -> int { return scan_reduce_keyed_impl(ctx, q, key, root, out); });
@@ -4259,9 +4212,9 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
         memset(&rg.captured, 0, sizeof rg.captured);
         cudaStream_t s = es.stream;
         cudaGetLastError();  // a stale error of an earlier call must not be blamed on the capture
-        cudaError_t e = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
         const char *bad_step = nullptr;  // first step of the capture the runtime objected to (BYDB_TRACE prints it)
-        if (e == cudaSuccess) {
+        cudaError_t e = cudaSuccess;
+        const GraphCapture c = capture_graph(s, &rg.exec, [&]() -> int {
             Scratch fin;
             auto step = [&](const char *name, bool good) {
                 const cudaError_t le = cudaGetLastError();
@@ -4293,20 +4246,12 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
             }
             step("error read-back", cudaMemcpyAsync(h_back, mb.my_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, s) == cudaSuccess);
             rg.captured.kernel_launches += 2;
+            return bad_step ? 1 : 0;
+        });
+        if (!bad_step) {
+            bad_step = c.failed;
+            e = c.err;
         }
-        cudaGraph_t graph = nullptr;
-        if (e == cudaSuccess || bad_step) {
-            const cudaError_t ee = cudaStreamEndCapture(s, &graph);  // always leave capture mode
-            if (!bad_step && ee != cudaSuccess) {
-                bad_step = "end capture";
-                e = ee;
-            }
-        }
-        if (!bad_step && graph) {
-            e = cudaGraphInstantiate(&rg.exec, graph, 0);
-            if (e != cudaSuccess) bad_step = "instantiate";
-        }
-        if (graph) cudaGraphDestroy(graph);
         if (bad_step || !rg.exec) {
             static const bool trace = getenv("BYDB_TRACE") != nullptr;
             if (trace) fprintf(stderr, "[bydb] prepared collective: capture failed at '%s' (%s); keeping the plain path\n", bad_step ? bad_step : "?", cudaGetErrorString(e));
