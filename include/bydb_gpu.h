@@ -73,6 +73,10 @@ typedef struct {
 #define BYDB_CFG_HOST_INDEX 1u /* bydb_part_register: parse the block index (meta.bin / primary.bin / *.tfm) on the host instead of
                                   with the device kernels (the default; both build the same directory -- the host parser is what
                                   the cold host-buffer paths use, where one frame's latency matters more than throughput) */
+#define BYDB_CFG_NO_DENSE_PAGES 2u /* bydb_part_register: keep every page as the part stores it.  By default the narrow delta field
+                                     pages that the all-rows SUM / COUNT / MEAN scan reads (varints of <= 3 bytes, values spanning
+                                     <= 32 bits) also get a bit-plane form in HBM when that form is smaller; results are the same
+                                     bit for bit, the scan reads fewer bytes, the part holds more (bydb_part_dense_pages) */
 
 /* One file image of a part (banyand/measure/part.go:40-55).  name is one of "meta.bin",
  * "primary.bin", "timestamps.bin", "fv.bin", "<family>.tf", "<family>.tfm". */
@@ -171,7 +175,9 @@ typedef struct {
 int bydb_init(const bydb_cfg *cfg, bydb_ctx **out);
 void bydb_shutdown(bydb_ctx *ctx);
 
-/* Upload an immutable part into HBM and build its block directory.  Idempotent per part_id. */
+/* Upload an immutable part into HBM and build its block directory.  Idempotent per part_id.  Unless the context was made with
+ * BYDB_CFG_NO_DENSE_PAGES, the part also holds the dense form of its narrow delta field pages: about 2.8 GB more for bench.py's
+ * 1e9-datapoint part (21.8 GB of reference pages and directory), charged to the part like everything else it holds. */
 int bydb_part_register(bydb_ctx *ctx, uint64_t part_id, const bydb_part_files *files, bydb_part_h *out);
 int bydb_part_release(bydb_ctx *ctx, bydb_part_h part);
 /* resident bytes / block / row counts of a registered part */
@@ -181,6 +187,9 @@ int bydb_part_info(bydb_ctx *ctx, bydb_part_h part, uint64_t *hbm_bytes, uint64_
  * 291-304): `unpacked` were rewritten into scan-friendly pages in HBM when the part was registered, `left` could
  * not be (a query that touches one of those returns BYDB_ENOTSUP). */
 int bydb_part_fallback_pages(bydb_ctx *ctx, bydb_part_h part, uint64_t *unpacked, uint64_t *left);
+/* Dense pages of a registered part (BYDB_CFG_NO_DENSE_PAGES): `pages` field pages got a bit-plane form at registration, held in
+ * `bytes` of HBM beside the part's own pages (included in bydb_part_info's hbm_bytes). */
+int bydb_part_dense_pages(bydb_ctx *ctx, bydb_part_h part, uint64_t *pages, uint64_t *bytes);
 /* Diagnostics: copies the part's DEVICE block directory (the DevBlock[64 B] / DevCol[16 B] records the scan kernels read,
  * csrc/part_dir.hpp) into caller buffers; either pointer may be NULL to only query the counts.  Tests compare the directory the
  * device index kernels build with the host parser's. */

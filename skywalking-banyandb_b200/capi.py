@@ -105,7 +105,7 @@ class _Layout(C.Structure):
 
 
 # every symbol include/bydb_gpu.h declares (tests/test_capi_symbols.py checks the list against the header)
-EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_release", "bydb_part_info", "bydb_part_fallback_pages", "bydb_part_directory",
+EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_release", "bydb_part_info", "bydb_part_fallback_pages", "bydb_part_dense_pages", "bydb_part_directory",
            "bydb_scan_agg", "bydb_scan_agg_host", "bydb_result_free", "bydb_query_prepare", "bydb_scan_agg_prepared",
            "bydb_query_release", "bydb_query_prepare_keyed", "bydb_scan_agg_keyed_prepared", "bydb_query_release_keyed", "bydb_scan_partials_prepared",
            "bydb_scan_partials_keyed_prepared", "bydb_partials_layout",
@@ -141,6 +141,7 @@ def load_library():
     L.bydb_part_release.argtypes = [C.c_void_p, C.c_uint64]
     L.bydb_part_info.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.bydb_part_fallback_pages.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    L.bydb_part_dense_pages.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.bydb_part_directory.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.bydb_scan_agg.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_Result)]
     L.bydb_scan_agg_host.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(_PartFiles), C.POINTER(_Query), C.POINTER(_Result)]
@@ -454,9 +455,10 @@ def keyed_reduce_slot_bytes(q: Query, family: str, tag: str, max_values: int = 0
 class Context:
     """bydb_ctx: one device, its streams and the HBM part cache."""
 
-    def __init__(self, device: int = 0, warps_per_sm: int = 0, hbm_budget_bytes: int = 0, host_index: bool = False):
+    def __init__(self, device: int = 0, warps_per_sm: int = 0, hbm_budget_bytes: int = 0, host_index: bool = False, dense_pages: bool = True):
+        """dense_pages=False: registered parts keep every page as stored (BYDB_CFG_NO_DENSE_PAGES)."""
         self._L = load_library()
-        cfg = _Cfg(device, warps_per_sm, hbm_budget_bytes, 1 if host_index else 0, 0)
+        cfg = _Cfg(device, warps_per_sm, hbm_budget_bytes, (1 if host_index else 0) | (0 if dense_pages else 2), 0)
         h = C.c_void_p()
         _check(self._L.bydb_init(C.byref(cfg), C.byref(h)))
         self._h = h
@@ -491,7 +493,10 @@ class Context:
         _check(self._L.bydb_part_info(self._h, handle, C.byref(a), C.byref(b), C.byref(c)))
         u, l = C.c_uint64(), C.c_uint64()
         _check(self._L.bydb_part_fallback_pages(self._h, handle, C.byref(u), C.byref(l)))
-        return dict(hbm_bytes=a.value, n_blocks=b.value, n_rows=c.value, fallback_unpacked=u.value, fallback_left=l.value)
+        dp, db = C.c_uint64(), C.c_uint64()
+        _check(self._L.bydb_part_dense_pages(self._h, handle, C.byref(dp), C.byref(db)))
+        return dict(hbm_bytes=a.value, n_blocks=b.value, n_rows=c.value, fallback_unpacked=u.value, fallback_left=l.value,
+                    dense_pages=dp.value, dense_bytes=db.value)
 
     def part_directory(self, handle: int):
         """-> (blocks [n, 64] uint8, cols [n, 16] uint8): the part's device block directory, byte for byte (diagnostics)."""

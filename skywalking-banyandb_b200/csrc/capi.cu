@@ -79,6 +79,8 @@ struct Part {
     uint8_t *d_dir = nullptr;         // DevBlock[] | DevCol[] | file pointer table
     uint8_t *d_unpack = nullptr;      // fallback pages rewritten at admission (unpack_kernels.cu); file slot `n_files`
     uint64_t unpacked_pages = 0, unpack_skipped = 0;
+    uint8_t *d_dense = nullptr;       // DevDense[n_cols] | the plane streams (build_dense_pages); resident parts only
+    uint64_t dense_pages = 0, dense_bytes = 0;
     const DevBlock *d_blocks = nullptr;
     const DevCol *d_cols = nullptr;
     const uint8_t *const *d_files = nullptr;
@@ -90,10 +92,12 @@ struct Part {
             if (d_arena) cudaFreeAsync(d_arena, pool_stream);
             if (d_dir) cudaFreeAsync(d_dir, pool_stream);
             if (d_unpack) cudaFreeAsync(d_unpack, pool_stream);
+            if (d_dense) cudaFreeAsync(d_dense, pool_stream);
         } else {
             if (d_arena) cudaFree(d_arena);
             if (d_dir) cudaFree(d_dir);
             if (d_unpack) cudaFree(d_unpack);
+            if (d_dense) cudaFree(d_dense);
         }
     }
 };
@@ -280,6 +284,7 @@ struct bydb_ctx {
     uint64_t hbm_budget = 0;
     uint64_t hbm_used = 0;
     bool host_index = false;   // BYDB_CFG_HOST_INDEX: parse the block index of resident parts on the host (part_dir.cc)
+    bool dense_pages = true;   // resident parts get the dense form of their narrow field pages (BYDB_CFG_NO_DENSE_PAGES clears it)
     std::mutex mu;
     NameTable names;
     std::unordered_map<bydb_part_h, std::shared_ptr<Part>> parts;
@@ -441,6 +446,7 @@ int file_images(const bydb_part_files *files, std::vector<FileImage> &imgs) {
 }
 
 int unpack_fallback_pages(bydb_ctx *ctx, Part &part, size_t n_files, cudaStream_t s);
+int build_dense_pages(bydb_ctx *ctx, Part &part, cudaStream_t s);
 int build_part_dir_device(bydb_ctx *ctx, const std::vector<FileImage> &imgs, Part &part, const std::vector<std::string> &families, cudaStream_t s, size_t n_files,
                           size_t *dir_bytes_out);
 
@@ -450,6 +456,7 @@ struct AdmitOptions {
                                 // need straight over PCIe; only the block directory is uploaded
     bool transient = false;     // for the length of one call: device memory from the stream-ordered pool
     bool unpack = false;        // fallback pages are rewritten at admission (unpack_fallback_pages)
+    bool dense = false;         // narrow field pages get their dense form (build_dense_pages)
     PartDir *parsed = nullptr;  // the block index as the caller parsed it already
     bool device_index = false;  // the block index is parsed by kernels (resident parts without `parsed`)
 };
@@ -559,6 +566,10 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
             rc = unpack_fallback_pages(ctx, *part, nf, s);
             if (rc) return rc;
         }
+        if (opt.dense) {
+            rc = build_dense_pages(ctx, *part, s);
+            if (rc) return rc;
+        }
         undo.keep = true;
         out = part;
         return 0;
@@ -587,6 +598,10 @@ int register_part_locked_free(bydb_ctx *ctx, uint64_t part_id, const bydb_part_f
     }
     if (opt.unpack) {
         const int rc = unpack_fallback_pages(ctx, *part, nf, s);
+        if (rc) return rc;
+    }
+    if (opt.dense) {
+        const int rc = build_dense_pages(ctx, *part, s);
         if (rc) return rc;
     }
     undo.keep = true;
@@ -904,6 +919,56 @@ int unpack_fallback_pages(bydb_ctx *ctx, Part &part, size_t n_files, cudaStream_
     return 0;
 }
 
+// Gives the narrow delta field pages of a resident part their dense form (DESIGN.md 3.3; dense_page.cuh): classify fills the
+// descriptors in a scratch table and sizes the plane streams, then ONE allocation [DevDense[n_cols] | planes] is charged to the
+// part and the write pass lays the planes out in it.  The reference pages stay where they are: every other lane reads them.
+int build_dense_pages(bydb_ctx *ctx, Part &part, cudaStream_t s) {
+    const size_t nb = part.dir.blocks.size(), nc = part.dir.cols.size();
+    if (nb == 0 || nc == 0 || part.dir.files.size() < 2 || part.dir.files[1] != "fv.bin") return 0;
+    const size_t table = align_up(nc * sizeof(DevDense), 256);
+    Scratch scratch;
+    CUDA_TRY(scratch.alloc(256 + table, s));
+    CUDA_TRY(cudaMemsetAsync(scratch.base, 0, 256 + table, s));
+    DenseParams dp{};
+    dp.blocks = part.d_blocks;
+    dp.cols = part.d_cols;
+    dp.files = part.d_files;
+    dp.dense = reinterpret_cast<DevDense *>(scratch.base + 256);
+    dp.n_blocks = static_cast<uint32_t>(nb);
+    dp.fv_file_id = 1;
+    dp.counters = reinterpret_cast<unsigned long long *>(scratch.base);
+    const int grid = static_cast<int>(std::min<size_t>((nb + kWarpsPerCta - 1) / kWarpsPerCta, 2 * static_cast<size_t>(ctx->sm_count)));
+    launch_dense_classify(dp, grid, s);
+    CUDA_TRY(cudaGetLastError());
+    unsigned long long cnt[4] = {0, 0, 0, 0};
+    CUDA_TRY(cudaMemcpyAsync(cnt, scratch.base, sizeof cnt, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    if (cnt[0] == 0) return 0;
+    const size_t bytes = table + align_up(cnt[1], 256);
+    if (int rc = hbm_reserve(ctx, bytes, "HBM budget exceeded while building dense pages")) return rc;
+    part.hbm_bytes += bytes;
+    cudaError_t e = part.pool_stream ? cudaMallocAsync(reinterpret_cast<void **>(&part.d_dense), bytes, s)
+                                     : cudaMalloc(reinterpret_cast<void **>(&part.d_dense), bytes);
+    if (e != cudaSuccess) {
+        part.d_dense = nullptr;
+        return fail(BYDB_ENOMEM, "device allocation failed for the dense pages");
+    }
+    Scratch rows;
+    CUDA_TRY(rows.alloc(static_cast<size_t>(grid) * kWarpsPerCta * cnt[2] * 4, s));
+    CUDA_TRY(cudaMemcpyAsync(part.d_dense, dp.dense, nc * sizeof(DevDense), cudaMemcpyDeviceToDevice, s));
+    dp.dense = reinterpret_cast<DevDense *>(part.d_dense);
+    dp.arena = part.d_dense + table;
+    dp.scratch = reinterpret_cast<uint32_t *>(rows.base);
+    dp.scratch_rows = static_cast<uint32_t>(cnt[2]);
+    launch_dense_write(dp, grid, s);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(cnt, scratch.base, sizeof cnt, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    part.dense_pages = cnt[3];
+    part.dense_bytes = bytes;
+    return 0;
+}
+
 // staging of one step, in pinned memory and on the device alike: series ids | order (query-series indices sorted by
 // (group, series)) | group_start (where each group begins in order), back to back so that one copy takes all three
 struct StageLayout {
@@ -981,7 +1046,7 @@ void part_refs(const std::vector<std::shared_ptr<Part>> &parts, DevPartRef *out)
     uint32_t base = 0;
     for (size_t i = 0; i < parts.size(); ++i) {
         const Part &p = *parts[i];
-        out[i] = DevPartRef{p.d_blocks, p.d_cols, p.d_files, static_cast<uint32_t>(p.dir.blocks.size()), base};
+        out[i] = DevPartRef{p.d_blocks, p.d_cols, p.d_files, reinterpret_cast<const DevDense *>(p.d_dense), static_cast<uint32_t>(p.dir.blocks.size()), base};
         base += out[i].n_blocks;
     }
 }
@@ -2676,6 +2741,7 @@ int bydb_init(const bydb_cfg *cfg, bydb_ctx **out) {
     ctx->sm_count = prop.multiProcessorCount;
     ctx->hbm_budget = cfg ? cfg->hbm_budget_bytes : 0;
     ctx->host_index = cfg && (cfg->flags & BYDB_CFG_HOST_INDEX) != 0;
+    ctx->dense_pages = !(cfg && (cfg->flags & BYDB_CFG_NO_DENSE_PAGES) != 0);
     if (upload_pow10_table()) {
         delete ctx;
         return fail(BYDB_EIO, "cannot upload constant tables (is the library built for this GPU?)");
@@ -2751,6 +2817,7 @@ int bydb_part_register(bydb_ctx *ctx, uint64_t part_id, const bydb_part_files *f
     std::shared_ptr<Part> part;
     AdmitOptions opt;
     opt.unpack = true;
+    opt.dense = ctx->dense_pages;
     opt.device_index = !ctx->host_index;
     int rc = register_part_locked_free(ctx, part_id, files, part, nullptr, opt);
     if (rc) return rc;
@@ -2814,6 +2881,18 @@ int bydb_part_fallback_pages(bydb_ctx *ctx, bydb_part_h h, uint64_t *unpacked, u
     if (it == ctx->parts.end()) return fail(BYDB_ENOENT, "unknown part handle");
     if (unpacked) *unpacked = it->second->unpacked_pages;
     if (left) *left = it->second->unpack_skipped;
+    return 0;
+    });
+}
+
+int bydb_part_dense_pages(bydb_ctx *ctx, bydb_part_h h, uint64_t *pages, uint64_t *bytes) {
+    return guarded([&]() -> int {
+    if (!ctx) return fail(BYDB_EINVAL, "ctx is NULL");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    auto it = ctx->parts.find(h);
+    if (it == ctx->parts.end()) return fail(BYDB_ENOENT, "unknown part handle");
+    if (pages) *pages = it->second->dense_pages;
+    if (bytes) *bytes = it->second->dense_bytes;
     return 0;
     });
 }

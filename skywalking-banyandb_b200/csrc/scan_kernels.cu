@@ -2555,19 +2555,21 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum
         for (uint32_t c = 0; c < p.n_fcols; ++c) {
             // ---- this lane's page of field c
             const uint8_t *abase = nullptr;
-            uint32_t pstart = 0, pend = 0, total = 0, nst = 0;
+            uint32_t pstart = 0, pend = 0, total = 0, nst = 0, dense_b = 0;
             int64_t first = 0;
             int exp = 0;
-            bool has_page = false, is_float = false, count_only = false;
+            bool has_page = false, is_float = false, count_only = false, dense = false;
             if (ok) {
                 const DevCol *cols = p.parts[pi].cols + col_begin;
                 DevCol col{};
                 bool found = false;
+                uint32_t ci = 0;
                 for (uint32_t i = 0; i < n_cols && !found; ++i) {
                     const DevCol cc = cols[i];
                     if (cc.name_id == p.fcol_name[c]) {
                         col = cc;
                         found = true;
+                        ci = i;
                     }
                 }
                 if (found) {
@@ -2584,6 +2586,18 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum
                         if (col.size < 2 || __ldg(page) == 9 || (__ldg(page) == kEncRawCells && __ldg(page + 1))) ok = false;
                         count_only = ok;
                         page_bytes += 1;
+                    } else if (ok && p.parts[pi].dense && p.parts[pi].dense[col_begin + ci].n == count) {
+                        // the page's bit planes (dense_page.cuh): the descriptor stands in for the page header
+                        const DevDense dd = p.parts[pi].dense[col_begin + ci];
+                        exp = dd.exp;
+                        first = dd.min;
+                        dense_b = dd.b;
+                        abase = dd.planes;
+                        pend = total = dd.plane_bytes;
+                        nst = (total + kExpressStageBytes - 1) / kExpressStageBytes;
+                        has_page = true;
+                        dense = true;
+                        page_bytes += col.size;  // the counter stays the query's encoded page bytes, whichever form was read
                     } else if (ok) {
                         if (col.size < hdr || __ldg(page) != 3) {
                             ok = false;  // not a plain EncodeTypeDelta page
@@ -2640,6 +2654,11 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum
                     const uint32_t tot_k = __shfl_sync(0xffffffffu, total, k);
                     const int64_t first_k = static_cast<int64_t>(shfl_u64(static_cast<uint64_t>(first), k));
                     const uint8_t *ab_k = reinterpret_cast<const uint8_t *>(shfl_u64(reinterpret_cast<uint64_t>(abase), k));
+                    const bool dense_k = __shfl_sync(0xffffffffu, dense, k);
+                    const uint32_t b_k = __shfl_sync(0xffffffffu, dense_b, k);
+                    uint32_t plane_end[kDensePlanes];
+                    dense_plane_ends(count_k, b_k, plane_end);
+                    uint64_t U = 0;  // dense page: this lane's share of sum (v - first)
                     int64_t S = 0;
                     // terminators before the unit.  Every byte of every unit is decoded, and the zeros that stand in for the
                     // bytes outside the body are one-byte varints of delta 0: they add nothing to T or R' and one terminator
@@ -2657,7 +2676,17 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum
                     for (uint32_t j = 0; j < nst_k; ++j) {
                         const uint32_t s = sb_k + j;
                         uint8_t *buf = ring_wait(sm, seq0 + s);
-                        if (good) {
+                        if (dense_k) {
+#if BYDB_EXPRESS_DECODE
+                            // lane l sums the 16-byte pieces l, l + 32, ... of the unit; pieces past the stream hold stale bytes
+#pragma unroll
+                            for (int q = 0; q < kExpressStageBytes / 512; ++q) {
+                                const uint32_t pc = static_cast<uint32_t>(lane) + 32u * q;
+                                const uint4 v = *reinterpret_cast<const uint4 *>(buf + 16 * pc);
+                                U += dense_piece_sum(v, j * kExpressStageBytes + 16 * pc, plane_end, b_k);
+                            }
+#endif
+                        } else if (good) {
                             if (j == 0 || (j + 1) * kExpressStageBytes > pe_k) express_zero_edges(buf, j * kExpressStageBytes, ps_k, pe_k, lane);
 #if BYDB_EXPRESS_DECODE
                             const uint8_t *src = buf + lane * kSwarLaneBytes;
@@ -2693,7 +2722,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum
                             }
 #endif
                         }
-                        if (j == nst_k - 1 && lane == 0) last_byte = buf[(pe_k - 1) % kExpressStageBytes];
+                        if (!dense_k && j == nst_k - 1 && lane == 0) last_byte = buf[(pe_k - 1) % kExpressStageBytes];
                         __syncwarp();
                         const uint32_t nx = s + kExpressStages;
                         if (nx < ts) {
@@ -2708,17 +2737,20 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum
                     }
                     last_byte = __shfl_sync(0xffffffffu, last_byte, 0);
                     const int32_t zeros_after = static_cast<int32_t>(nst_k * kExpressStageBytes - pe_k);
-                    if (nst_k == 0) good = count_k == 1;  // an empty body: the page holds `first` alone
+                    if (dense_k) good = true;  // checked when the planes were written (a b = 0 page has no stages)
+                    else if (nst_k == 0) good = count_k == 1;  // an empty body: the page holds `first` alone
                     else good = good && tb - zeros_after + 1 == static_cast<int32_t>(count_k) && last_byte < 0x80u;
 #if !BYDB_EXPRESS_DECODE
                     good = true;  // the fetch-only build keeps every block in the express lane
 #endif
+                    // sum v = count * first + S (varint: S may be negative) or + U (dense: first = m, every u >= 0, U < 2^58); one
+                    // of the two is zero, so the warp reduces them as one 64-bit word
+                    uint64_t us = U + static_cast<uint64_t>(S);
 #pragma unroll
-                    for (int m = 16; m >= 1; m >>= 1) S += static_cast<int64_t>(shfl_xor_u64(static_cast<uint64_t>(S), m));
+                    for (int m = 16; m >= 1; m >>= 1) us += shfl_xor_u64(us, m);
                     acc.add_scaled(first_k, count_k);
-                    const uint64_t us = static_cast<uint64_t>(S);
                     acc.lo += us;
-                    acc.hi += (S >> 63) + (acc.lo < us ? 1 : 0);
+                    acc.hi += (dense_k ? 0 : (static_cast<int64_t>(us) >> 63)) + (acc.lo < us ? 1 : 0);
                     acc.cnt = count_k;
                 } else if (cok) {
                     acc.cnt = count_k;
@@ -2772,6 +2804,135 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, BYDB_EXPRESS_CTAS) scan_sum
     if (sm->fault && lane == 0) atomicCAS(&p.err[0], 0u, static_cast<uint32_t>(kErrTmaTimeout));
 }
 
+
+// ------------------------------------------------------------------------------------------------
+// Dense pages (DESIGN.md 3.3): when a resident part is admitted, each field page the express lane would sum is rewritten as bit
+// planes (dense_page.cuh) if that form is smaller; the express lane then streams the planes instead of the varints.  Two passes,
+// a warp per block, the host sizing the arena between them:
+//   classify  decodes the page with the fast lane's decoder (delta_page_fast: min / max, and the lane's acceptance -- no varint
+//             of 4+ bytes, `count` terminators, the last byte a terminator), fills the page's descriptor and reserves its planes
+//   write     decodes the converted pages again with the general decoder into per-warp scratch and lays out their planes
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ WarpSmem *dense_warp_init(int lane) {
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    WarpSmem *sm = reinterpret_cast<WarpSmem *>(smem_raw) + (threadIdx.x >> 5);
+    if (lane == 0) {
+        sm->fault = 0;
+        sm->seq = 0;
+        for (int s = 0; s < kStages; ++s) mbar_init(&sm->bar[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    return sm;
+}
+// the page header of a field page that may have a dense form: 0 = it has none
+__device__ __forceinline__ uint32_t dense_page_hdr(const DenseParams &p, const DevCol &col, const uint8_t *&page) {
+    if (col.file_id != p.fv_file_id || (col.value_type != BYDB_VT_INT64 && col.value_type != BYDB_VT_FLOAT64)) return 0;
+    const uint32_t hdr = col.value_type == BYDB_VT_FLOAT64 ? 11u : 9u;
+    page = p.files[col.file_id] + col.off;
+    return col.size >= hdr && __ldg(page) == 3 ? hdr : 0;
+}
+
+__global__ void __launch_bounds__(kWarpsPerCta * 32) dense_classify_kernel(const __grid_constant__ DenseParams p) {
+    const int lane = threadIdx.x & 31;
+    WarpSmem *sm = dense_warp_init(lane);
+    for (uint32_t bi = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); bi < p.n_blocks; bi += gridDim.x * kWarpsPerCta) {
+        const DevBlock blk = p.blocks[bi];
+        if (blk.count == 0 || blk.count > kDenseMaxRows) continue;
+        for (uint32_t c = 0; c < blk.n_cols; ++c) {
+            const uint32_t ci = blk.col_begin + c;
+            const DevCol col = p.cols[ci];
+            const uint8_t *page = nullptr;
+            const uint32_t hdr = dense_page_hdr(p, col, page);
+            if (hdr == 0) continue;
+            const int64_t first = conv_bytes_to_int64(page + hdr - 8);
+            // every prefix stays inside int64: a varint of <= 3 bytes moves the value by less than 2^20
+            const int64_t reach = static_cast<int64_t>(blk.count) << 20;
+            if (first < INT64_MIN + reach || first > INT64_MAX - reach) continue;
+            __syncwarp();  // every lane is done with the previous page's result slot
+            if (lane == 0) {
+                sm->a_body = page + hdr;
+                sm->a_len = col.size - hdr;
+                sm->a_count = blk.count;
+                sm->a_first = first;
+                sm->a_r0 = 0;
+                sm->a_r1 = blk.count - 1;
+            }
+            __syncwarp();
+            if (delta_page_fast<kRowsAll, kNeedMinMax>(sm, lane) != 0 || sm->fault) continue;
+            const int64_t mn = sm->res_mn, mx = sm->res_mx;
+            const uint64_t span = static_cast<uint64_t>(mx) - static_cast<uint64_t>(mn);
+            if (span > 0xffffffffull) continue;
+            const uint32_t b = span ? 64u - static_cast<uint32_t>(__clzll(static_cast<long long>(span))) : 0u;
+            const uint32_t bytes = dense_stream_bytes(blk.count, b);
+            if (sizeof(DevDense) + bytes >= col.size) continue;  // only a smaller form is kept
+            if (lane == 0) {
+                DevDense d{};
+                d.planes = reinterpret_cast<const uint8_t *>(static_cast<uintptr_t>(atomicAdd(&p.counters[1], static_cast<unsigned long long>(bytes))));
+                d.min = mn;
+                d.n = blk.count;
+                d.plane_bytes = bytes;
+                d.exp = hdr == 11 ? static_cast<int16_t>((static_cast<uint32_t>(__ldg(page + 1)) << 8) | __ldg(page + 2)) : 0;
+                d.b = static_cast<uint8_t>(b);
+                p.dense[ci] = d;
+                atomicAdd(&p.counters[0], 1ull);
+                atomicMax(&p.counters[2], static_cast<unsigned long long>(blk.count));
+            }
+        }
+    }
+}
+
+// general-decoder consumer of the write pass: u = v - m of every row
+struct DenseCons {
+    uint32_t *u;
+    int64_t m;
+    uint32_t n;
+    __device__ __forceinline__ void operator()(uint32_t row, int64_t v) {
+        if (row < n) u[row] = static_cast<uint32_t>(v - m);
+    }
+};
+
+__global__ void __launch_bounds__(kWarpsPerCta * 32) dense_write_kernel(const __grid_constant__ DenseParams p) {
+    const int lane = threadIdx.x & 31;
+    WarpSmem *sm = dense_warp_init(lane);
+    const uint32_t gw = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
+    uint32_t *u = p.scratch + static_cast<size_t>(gw) * p.scratch_rows;
+    for (uint32_t bi = gw; bi < p.n_blocks; bi += gridDim.x * kWarpsPerCta) {
+        const DevBlock blk = p.blocks[bi];
+        for (uint32_t c = 0; c < blk.n_cols; ++c) {
+            const uint32_t ci = blk.col_begin + c;
+            const DevDense d = p.dense[ci];
+            if (d.n == 0) continue;
+            const DevCol col = p.cols[ci];
+            const uint8_t *page = nullptr;
+            const uint32_t hdr = dense_page_hdr(p, col, page);
+            DenseCons cons{u, d.min, d.n};
+            bool ok = hdr != 0 && d.n <= p.scratch_rows &&
+                      decode_varint_page<false>(sm, page + hdr, col.size - hdr, d.n, conv_bytes_to_int64(page + hdr - 8), cons, lane);
+            ok = ok && !sm->fault;
+            __syncwarp();  // the rows' u are visible to the warp
+            uint8_t *out = p.arena + reinterpret_cast<uintptr_t>(d.planes);
+            if (ok) {
+                uint32_t at = 0;
+                for (int k = 0; k < kDensePlanes; ++k) {
+                    const uint32_t w = dense_width(k);
+                    if (!(d.b & w)) continue;
+                    const uint32_t words = dense_plane_bytes(d.n, w) / 4;
+                    uint32_t *plane = reinterpret_cast<uint32_t *>(out + at);
+                    for (uint32_t q = lane; q < words; q += 32) plane[q] = dense_encode_word(u, d.n, d.b, w, q);
+                    at += words * 4;
+                }
+            }
+            if (lane == 0) {
+                // a page the second decode disagrees with keeps its varints (it cannot happen for a page classify accepted)
+                if (ok) p.dense[ci].planes = out;
+                else p.dense[ci].n = 0;
+                if (ok) atomicAdd(&p.counters[3], 1ull);
+            }
+            __syncwarp();  // before the next page overwrites u
+        }
+    }
+}
 
 // ------------------------------------------------------------------------------------------------
 // version dedup across parts (banyand/measure/query.go:912-942,995-1004; query_batch.go:151-161):
@@ -5344,6 +5505,15 @@ void launch_scan_blocks(const ScanParams &p, int grid_express, int grid_fast, in
     scan_blocks_kernel<false><<<grid_slow, kWarpsPerCta * 32, smem, s>>>(p);
 }
 
+void launch_dense_classify(const DenseParams &p, int grid, cudaStream_t s) {
+    cudaFuncSetAttribute(dense_classify_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(scan_smem_bytes()));
+    dense_classify_kernel<<<grid, kWarpsPerCta * 32, scan_smem_bytes(), s>>>(p);
+}
+void launch_dense_write(const DenseParams &p, int grid, cudaStream_t s) {
+    cudaFuncSetAttribute(dense_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(scan_smem_bytes()));
+    dense_write_kernel<<<grid, kWarpsPerCta * 32, scan_smem_bytes(), s>>>(p);
+}
+
 void scan_max_ctas_per_sm(int *express, int *fast, int *slow) {
     scan_set_attrs();
     int e = 1, a = 1, b = 1;
@@ -5525,6 +5695,8 @@ void preload_kernels() {
     cudaFuncGetAttributes(&a, scan_blocks_kernel<true>);
     cudaFuncGetAttributes(&a, scan_blocks_kernel<false>);
     cudaFuncGetAttributes(&a, scan_sum_express_kernel);
+    cudaFuncGetAttributes(&a, dense_classify_kernel);
+    cudaFuncGetAttributes(&a, dense_write_kernel);
     cudaFuncGetAttributes(&a, detect_overlap_kernel);
     cudaFuncGetAttributes(&a, dedup_kernel);
     cudaFuncGetAttributes(&a, series_reduce_kernel);

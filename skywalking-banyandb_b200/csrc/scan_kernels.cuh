@@ -7,6 +7,7 @@
 #include <cstdint>
 
 #include "../../include/bydb_gpu.h"
+#include "dense_page.cuh"
 #include "part_dir.hpp"
 
 namespace bydb {
@@ -71,6 +72,7 @@ struct DevPartRef {
     const DevBlock *blocks;
     const DevCol *cols;
     const uint8_t *const *files;  // device array of file base pointers (indexed by DevCol::file_id)
+    const DevDense *dense;        // dense forms of the pages, parallel to cols (NULL: the part has none)
     uint32_t n_blocks;
     uint32_t block_base;          // global index of blocks[0] in this query
 };
@@ -101,7 +103,7 @@ __host__ __device__ __forceinline__ bool met_column(bool is_float, int64_t cnt, 
 }
 
 struct ScanParams {
-    DevPartRef parts[kMaxParts];
+    DevPartRef parts[kMaxParts];  // kernel parameters stay within 4 KB: see the static_asserts below
     uint32_t n_parts;
     uint32_t total_blocks;
     const uint64_t *q_sids;       // ascending
@@ -140,6 +142,8 @@ struct ScanParams {
     uint32_t n_dd_blocks;
     uint32_t pad1;
 };
+
+static_assert(sizeof(ScanParams) + 256 <= 4096, "ScanParams (with WideScanParams beside it) must fit the 4 KB kernel-parameter space");
 
 struct ReduceParams {
     DevPartRef parts[kMaxParts];
@@ -232,6 +236,7 @@ struct KeyParams {
     uint8_t *vals;                // [cap * kMaxLit] packed by key_pack (int64 key: [cap] values, 8 little-endian bytes each)
     uint32_t *lens;               // [cap]
 };
+static_assert(sizeof(ReduceParams) <= 4096 && sizeof(KeyParams) + 64 <= 4096, "kernel-parameter space");
 // int64_key: the key tag is an int64 column (key_values_i64_kernel), else a dictionary string tag (key_values_kernel)
 void launch_key_values(const KeyParams &p, bool int64_key, int grid, cudaStream_t s);
 
@@ -516,6 +521,25 @@ struct UnpackParams {
 size_t unpack_scratch_stride();
 void launch_classify_pages(const UnpackParams &p, cudaStream_t s);
 void launch_unpack_pages(const UnpackParams &p, int n_warps, cudaStream_t s);
+
+// ---- dense pages at part admission (scan_kernels.cu, "Dense pages"; the form: dense_page.cuh)
+struct DenseParams {
+    const DevBlock *blocks;
+    const DevCol *cols;
+    const uint8_t *const *files;
+    DevDense *dense;                // [n_cols] the part's descriptor table, zeroed
+    uint32_t n_blocks;
+    uint32_t fv_file_id;            // the field pages' file (fv.bin)
+    unsigned long long *counters;   // [0] pages classify converted [1] plane bytes [2] most rows of such a page [3] pages written
+    uint8_t *arena;                 // write pass: the plane streams (classify left each page's offset in DevDense::planes)
+    uint32_t *scratch;              // write pass: scratch_rows words per warp of the grid
+    uint32_t scratch_rows;
+    uint32_t pad;
+};
+// classify: a warp per block decodes each narrow field page with the fast lane's decoder and fills its descriptor (planes =
+// offset into the arena); write: a warp per block decodes the converted pages again and lays out their planes
+void launch_dense_classify(const DenseParams &p, int grid, cudaStream_t s);
+void launch_dense_write(const DenseParams &p, int grid, cudaStream_t s);
 
 // ---- write side: numeric field pages encoded on the device (encode_kernels.cu)
 struct EncodeParams {
