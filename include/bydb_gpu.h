@@ -551,6 +551,58 @@ int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_
  * keyed-partial and plain collectives keep the epochs in step across failures. */
 int bydb_scan_reduce_keyed_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_partial_rows *out);
 
+/* The collective form of bydb_scan_agg_keyed_wide / bydb_scan_partials_keyed_wide: group-by on a stored tag with up to 65,536 key
+ * values across the ranks of the peer mailboxes.  Every rank runs the wide path's discovery, scan and order over ITS parts and
+ * writes its present composite groups (series group, key value) -- their table in its insertion order, their first series, its
+ * values and the series' spans -- straight into its slot of the root's mailbox.  The root takes the union of the ranks' values,
+ * rebuilds the insertion order of the whole scan, folds each composite group's rows in rank order (deterministic float sums) and
+ * answers once.
+ *   - Every rank passes the SAME series_ids, series_group, n_groups, tmin / tmax, predicates, aggregations, Top-N, flags and
+ *     *key (max_values included); only `parts` differ.  The fingerprint also names the form: a rank calling bydb_scan_reduce_keyed
+ *     (or its partial form) in the same collective, or passing other arguments, makes the root fail with BYDB_EINVAL.  The two
+ *     calls below may be mixed: every rank contributes the same bytes, the root's call decides its answer's form.
+ *   - The root's answer is what bydb_scan_agg_keyed_wide (bydb_scan_partials_keyed_wide) answers over all ranks' parts: rows in
+ *     the insertion order of the whole scan, or Top-N order with ties to the group inserted first; n_keys = the distinct values
+ *     over all ranks' selected blocks; key bytes, nil rules, typing, BYDB_Q_ROW_PATH_TYPES and the sentinels as there.  Counts,
+ *     int64 values and min / max are exact, float sums within 1e-9 relative and bit-identical from call to call.  The order of
+ *     the key table is not part of the contract.  Non-root ranks get n_rows = 0, n_keys = 0 and their own stats.
+ *   - Caps and refusals: max_values 0 means 64, 1..65,536 are accepted, above gives BYDB_EINVAL.  More distinct values over all
+ *     ranks than max_values gives BYDB_ENOMEM at the root, even when every rank alone is under the cap.  A block with more than
+ *     256 values gives BYDB_ENOTSUP naming the block, parts of one rank that overlap in time BYDB_ENOTSUP, and a series whose
+ *     clipped spans on two ranks intersect BYDB_ENOTSUP at the root naming the series (the rule of bydb_scan_reduce_keyed).
+ *     Up to 8 predicates (the key takes no predicate slot).
+ *   - Insertion order: the root sorts each union composite group by its least (series index of its first row, order of that
+ *     rank's span within the series, position in that rank's list).  The fields hold series indexes below 2^31, 64 ranks and
+ *     lists below 2^27 groups -- a mailbox slot (at most 4 GiB) holds fewer -- and a rank whose list would not fit is refused
+ *     with BYDB_EINVAL, as a rank whose slot is too small is.
+ *   - Slots: bydb_keyed_wide_reduce_slot_bytes (host only, like bydb_keyed_reduce_slot_bytes) gives the slot a rank needs at
+ *     V = max_values key values and max_present present composite groups; pass it (or the largest over the queries to come) to
+ *     bydb_comm_export as max_table_bytes.  A rank whose V_r values and C_r present groups do not fit the exported slot fails with
+ *     BYDB_EINVAL (and so does the root); every failure keeps the ranks' epochs in step, with any roots and any collectives.
+ *   - Stats of every rank, with V_r, R_r, C_r the V, R, C of bydb_scan_agg_keyed_wide over the rank's parts, NB its parts' blocks and
+ *     sort(N) = the sum over the powers of two s from 4,096 to N of log2(s) - 10: rows_scanned, rows_matched, blocks_scanned and
+ *     page_bytes are those of its one wide pass;
+ *       d2h_bytes = 32 + V_r * (64 + 4) (string key) or 32 + V_r * 8 (int64 key), + 256 + 8 when V_r > 0
+ *       kernel_launches = (NB > 0) + 4, and when V_r > 0: + (NB > 0) + 10 + sort(pow2(max(R_r, 2048))) + (C_r > 0)
+ *     A rank's values, spans and table travel to the root's mailbox device to device (the header and values from the host) and
+ *     are not counted.  The root adds, with V_u, C_u the union's values and composite groups, R ranks, sum V and sum C over the ranks:
+ *       d2h_bytes += 16 * R, and when sum V > 0: + 16 + V_u * (64 + 4), and when C_u > 0: + the finalisation read-back of
+ *                    bydb_scan_agg over C_u groups (or 8 + 8 * F + C_u * (8 + 16 * A) for the partial form) + 8 * C_u
+ *       kernel_launches += when sum V > 0: 6 + (NS > 0 and R > 1) + (sum C > 0), and when C_u > 0: + 8 +
+ *                    sort(pow2(max(sum C, 2048))) + the finalisation's kernels (or 1 for the partial form)
+ *       h2d_bytes += 8 * (R + 1) when sum V > 0
+ *     The root's merge takes, up to 256-byte alignment of each region, with pow2(x) the least power of two >= x,
+ *       32 + 8 * (R + 1) + 8 * pow2(max(2 * sum V, 1024)) + 8 * sum V + 68 * cap + 28 * pow2(max(2 * sum C, 1024)) + 20 * sum C
+ *       + 8 * pow2(max(sum C, 2048)) (+ the exclusive scans' tile sums)                                  the union and the order
+ *       + 8 * (C_u * (7 * F + 1) + F) + 12 * C_u                                                         the folded table
+ *       + the finalisation's scratch over C_u groups (or the row image, 8 + 8 * F + C_u * (8 + 16 * A))
+ *     of device scratch, and a rank 4 * (NB + C_r) beside its wide pass.  The root's page-locked staging is sized before the
+ *     collective for the most composite groups the slots can carry. */
+int bydb_keyed_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t max_present, uint64_t *out);
+int bydb_scan_reduce_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out);
+int bydb_scan_reduce_keyed_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root,
+                                         bydb_keyed_partial_rows *out);
+
 const char *bydb_last_error(void);
 const char *bydb_version(void);
 

@@ -113,6 +113,7 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_scan_reduce", "bydb_scan_reduce_prepared", "bydb_scan_reduce_host", "bydb_scan_agg_keyed", "bydb_keyed_result_free",
            "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed", "bydb_scan_partials_keyed", "bydb_keyed_partial_rows_free",
            "bydb_scan_reduce_keyed_partials", "bydb_scan_agg_keyed_wide", "bydb_scan_partials_keyed_wide",
+           "bydb_keyed_wide_reduce_slot_bytes", "bydb_scan_reduce_keyed_wide", "bydb_scan_reduce_keyed_wide_partials",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -180,6 +181,10 @@ def load_library():
     L.bydb_scan_reduce_keyed_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32, C.POINTER(_KeyedPartialRows)]
     L.bydb_scan_agg_keyed_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(_KeyedResult)]
     L.bydb_scan_partials_keyed_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(_KeyedPartialRows)]
+    L.bydb_keyed_wide_reduce_slot_bytes.argtypes = [C.POINTER(_Query), C.POINTER(_GroupKey), C.c_uint64, C.POINTER(C.c_uint64)]
+    L.bydb_scan_reduce_keyed_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32, C.POINTER(_KeyedResult)]
+    L.bydb_scan_reduce_keyed_wide_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.c_int32,
+                                                       C.POINTER(_KeyedPartialRows)]
     L.bydb_keyed_partial_rows_free.argtypes = [C.c_void_p, C.POINTER(_KeyedPartialRows)]
     L.bydb_keyed_partial_rows_free.restype = None
     _lib = L
@@ -449,6 +454,17 @@ def keyed_reduce_slot_bytes(q: Query, family: str, tag: str, max_values: int = 0
     gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
     out = C.c_uint64()
     _check(load_library().bydb_keyed_reduce_slot_bytes(C.byref(cq), C.byref(gk), C.byref(out)))
+    return out.value
+
+
+def keyed_wide_reduce_slot_bytes(q: Query, family: str, tag: str, max_values: int = 0, max_present: int = 0, value_type: int = 0) -> int:
+    """bydb_keyed_wide_reduce_slot_bytes (host only): the mailbox slot a rank of the wide keyed collective needs at max_values key
+    values and max_present present composite groups."""
+    keep: list = []
+    cq = _mk_query(q, keep)
+    gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+    out = C.c_uint64()
+    _check(load_library().bydb_keyed_wide_reduce_slot_bytes(C.byref(cq), C.byref(gk), max_present, C.byref(out)))
     return out.value
 
 
@@ -728,6 +744,33 @@ class Context:
         r = _KeyedResult()
         _check(self._L.bydb_scan_reduce_keyed(self._h, C.byref(cq), C.byref(gk), root, C.byref(r)))
         return self._read_keyed(q, r)
+
+    def keyed_wide_reduce_slot_bytes(self, q: Query, family: str, tag: str, max_values: int = 0, max_present: int = 0,
+                                     value_type: int = 0) -> int:
+        """Mailbox slot bytes the wide keyed collective needs (bydb_keyed_wide_reduce_slot_bytes): pass it to comm_export."""
+        return keyed_wide_reduce_slot_bytes(q, family, tag, max_values, max_present, value_type)
+
+    def scan_reduce_keyed_wide(self, q: Query, family: str, tag: str, root: int = 0, max_values: int = 0, value_type: int = 0) -> Result:
+        """Collective group-by on a stored tag with up to 65,536 values (bydb_scan_reduce_keyed_wide): every rank passes the same
+        query but its parts.  The root gets scan_agg_keyed_wide's answer over all ranks' parts; the others an empty result with
+        their own scan statistics."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        r = _KeyedResult()
+        _check(self._L.bydb_scan_reduce_keyed_wide(self._h, C.byref(cq), C.byref(gk), root, C.byref(r)))
+        return self._read_keyed(q, r)
+
+    def scan_reduce_keyed_wide_partials(self, q: Query, family: str, tag: str, root: int = 0, max_values: int = 0,
+                                        value_type: int = 0) -> Dict[str, object]:
+        """The wide keyed collective with the root emitting partial rows (bydb_scan_reduce_keyed_wide_partials): the root gets
+        scan_partials_keyed_wide's rows over all ranks' parts; the others no rows, no keys and their own scan statistics."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        r = _KeyedPartialRows()
+        _check(self._L.bydb_scan_reduce_keyed_wide_partials(self._h, C.byref(cq), C.byref(gk), root, C.byref(r)))
+        return self._read_keyed_partials(q, r)
 
     def partials_combine(self, q, d_ptr: int, n_tables: int, bytes_each: int, stream: int = 0) -> None:
         cq, keep = _cq(q)

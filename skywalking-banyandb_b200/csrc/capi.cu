@@ -2327,18 +2327,21 @@ int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *ta
     return 0;
 }
 
-template <class Out>
-int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
-    uint32_t cap = 0;
-    Plan plan;
-    std::optional<SlotLease> lease;
-    int rc = keyed_call(ctx, q, key, kMaxWideKeyValues, false, out, cap, plan, lease);
-    if (rc) return rc;
-    ExecSlot &slot = *lease->slot;
+// Steps 1-3 of the wide path, on the slot's stream, synchronised: discovery (w.values), the scan and the order (w.n_comp composite
+// groups).  w.rp then holds everything launch_wide_fold reads but its outputs (table, pairs, perm), and the scratch behind it stays
+// alive in `w`.  No value or no record: w.R = 0 and nothing past discovery ran.
+struct WidePass {
+    KeyValues values;
+    size_t R = 0, n_comp = 0;
+    Scratch ka, sb;           // discovery | scan and order
+    WideKeyParams wk;
+    WideReduceParams rp;
+};
+int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats &stats,
+              WidePass &w) {
     cudaStream_t stream = slot.stream;
     const bool int64_key = key->value_type == BYDB_VT_INT64;
     const size_t F = plan.fcols.size(), NS = q->n_series, NB = plan.total_blocks, NBp = align_up(std::max<size_t>(NB, 1), 1024);
-    bydb_stats &stats = keyed_stats(out);
     cudaEvent_t *ev = slot.ev;
     CUDA_TRY(cudaEventRecord(ev[0], stream));
 
@@ -2348,10 +2351,10 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     const size_t a_sids = carve(NS * 8), a_grp = carve(NS * 4), a_slots = carve(S * 8), a_ctl = carve(32), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
                  a_lens = carve(static_cast<size_t>(cap) * 4), a_sid = carve(S * 4), a_nbr = carve(NBp * 4), a_rank = carve(NB * 4),
                  a_tiles = carve(NBp / 1024 * 4);
-    Scratch ka;
+    Scratch &ka = w.ka;
     CUDA_TRY(ka.alloc(carve.o, stream));
     if (slot.ensure_pinned(std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    WideKeyParams wk;
+    WideKeyParams &wk = w.wk;
     memset(&wk, 0, sizeof wk);
     KeyParams &kp = wk.k;
     kp = key_params(ctx, q, key, cap, plan, slot.pinned, ka.base, a_sids, a_slots, a_ctl, a_vals, a_lens);
@@ -2379,24 +2382,20 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     stats.d2h_bytes += 32;
     uint32_t ctl[8];
     memcpy(ctl, slot.pinned, 32);
-    rc = discovery_status(ctl);
+    int rc = discovery_status(ctl);
     if (rc) return rc;
     const size_t V = std::min<size_t>(ctl[0], cap), R = ctl[4];
-    KeyValues values;
     if (V) {
         const size_t vb = V * (int64_key ? 8 : kMaxLit);
         CUDA_TRY(cudaMemcpyAsync(slot.pinned, kp.vals, vb, cudaMemcpyDeviceToHost, stream));
         if (!int64_key) CUDA_TRY(cudaMemcpyAsync(slot.pinned + vb, kp.lens, V * 4, cudaMemcpyDeviceToHost, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
         stats.d2h_bytes += vb + (int64_key ? 0 : V * 4);
-        values = unpack_values(V, int64_key, slot.pinned, reinterpret_cast<const uint32_t *>(slot.pinned + vb));
+        w.values = unpack_values(V, int64_key, slot.pinned, reinterpret_cast<const uint32_t *>(slot.pinned + vb));
     }
-    KeyedAnswer<Out> answer(ctx, out, values);
-    if (V == 0 || R == 0) {  // no block selected: no rows (n_rows = 0)
-        answer.done = true;
-        return 0;
-    }
+    if (V == 0 || R == 0) return 0;  // no block selected: no rows (n_rows = 0)
     if (R > 0x7fffffffull) return fail(BYDB_ENOMEM, "wide group-key query: too many (block, key value) records");
+    w.R = R;
 
     // 2. the scan: one record per present (block, key value)
     const size_t rec_bytes = wide_record_bytes(F);
@@ -2404,7 +2403,7 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     Carve cb;
     const size_t b_zero = cb(kZeroPageBytes), b_rec = cb(R * rec_bytes), b_comp = cb(C * 8), b_cmin = cb(C * 4), b_rslot = cb(R * 4), b_keys = cb(N * 8),
                  b_heads = cb(N * 4), b_tiles = cb(N / 1024 * 4), b_ctl = cb(8), b_seg = cb(R * 4);
-    Scratch sb;
+    Scratch &sb = w.sb;
     CUDA_TRY(sb.alloc(cb.o, stream));
     ZeroPage *z = reinterpret_cast<ZeroPage *>(sb.base + b_zero);
     CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
@@ -2433,7 +2432,7 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     CUDA_TRY(cudaEventRecord(ev[2], stream));
 
     // 3. the composite groups in insertion order
-    WideReduceParams rp;
+    WideReduceParams &rp = w.rp;
     memset(&rp, 0, sizeof rp);
     rp.records = ws.records;
     rp.n_records = static_cast<uint32_t>(R);
@@ -2467,9 +2466,33 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     }
     rc = read_zero_page(*hz, false, &stats);
     if (rc) return rc;
-    const size_t n_comp = reinterpret_cast<const uint32_t *>(slot.pinned)[1];
+    w.n_comp = reinterpret_cast<const uint32_t *>(slot.pinned)[1];
+    return 0;
+}
+
+template <class Out>
+int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
+    uint32_t cap = 0;
+    Plan plan;
+    std::optional<SlotLease> lease;
+    int rc = keyed_call(ctx, q, key, kMaxWideKeyValues, false, out, cap, plan, lease);
+    if (rc) return rc;
+    ExecSlot &slot = *lease->slot;
+    cudaStream_t stream = slot.stream;
+    const size_t F = plan.fcols.size();
+    bydb_stats &stats = keyed_stats(out);
+    WidePass w;
+    rc = wide_pass(ctx, q, key, cap, plan, slot, stats, w);
+    if (rc) return rc;
+    KeyedAnswer<Out> answer(ctx, out, w.values);
+    if (w.R == 0) {  // no block selected: no rows (n_rows = 0)
+        answer.done = true;
+        return 0;
+    }
 
     // 4. the fold into a table of the present composite groups, then the form's own answer
+    const size_t n_comp = w.n_comp;
+    WideReduceParams &rp = w.rp;
     const TableLayout tl(std::max<size_t>(n_comp, 1), F);
     Carve cf;
     const size_t f_table = cf(tl.total), f_pairs = cf(n_comp * 8), f_perm = cf(n_comp * 4);
@@ -2479,13 +2502,13 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     rp.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
     rp.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
     launch_wide_fold(rp, static_cast<uint32_t>(n_comp), stream);
-    CUDA_TRY(cudaEventRecord(ev[3], stream));
+    CUDA_TRY(cudaEventRecord(slot.ev[3], stream));
     stats.kernel_launches += 1;
     if (n_comp > 0) rc = wide_emit(q, plan, slot, fb.base + f_table, tl, n_comp, rp, out, answer.owner);
     if (rc) return rc;
     {
         float ms = 0;
-        cudaEventElapsedTime(&ms, ev[0], ev[3]);
+        cudaEventElapsedTime(&ms, slot.ev[0], slot.ev[3]);
         stats.device_ms += ms;
     }
     answer.done = true;
@@ -4232,6 +4255,255 @@ int bydb_scan_reduce_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_
 // The keyed collective with the root emitting partial rows instead of finalising.
 int bydb_scan_reduce_keyed_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_partial_rows *out) {
     return guarded([&]() -> int { return scan_reduce_keyed_impl(ctx, q, key, root, out); });
+}
+
+int bydb_keyed_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t max_present, uint64_t *out) {
+    return guarded([&]() -> int {
+    if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
+    int rc = validate_query(q, false);
+    uint32_t cap = 0;
+    if (!rc) rc = check_group_key(q, key, kMaxWideKeyValues, false, cap);
+    if (rc) return rc;
+    Plan plan;
+    rc = query_shape(q, plan);
+    if (rc) return rc;
+    *out = WideSlot(plan.fcols.size(), q->n_series, cap, max_present).total;
+    return 0;
+    });
+}
+}  // extern "C"
+
+// the keyed fingerprint of the wide form: a rank of the per-value collective in the same round does not match it
+static uint64_t keyed_wide_fingerprint(const bydb_query *q, const bydb_group_key *key, uint32_t cap) {
+    uint64_t h = keyed_fingerprint(q, key, cap);
+    for (const char *s = "wide"; *s; ++s) h = (h ^ static_cast<uint8_t>(*s)) * 0x100000001b3ull;
+    return h;
+}
+
+// The wide keyed collective: on every rank the wide path's discovery, scan and order (wide_pass), then wide_fold_kernel writes the
+// rank's present composite groups straight into its slot of the root's mailbox (layout WideSlot), wide_series_kernel the series'
+// spans and wide_first_kernel each composite's first series; on the root the union of the values, the span check, the union
+// composites in insertion order and their fold in rank order (launch_wide_union / launch_wide_merge), then wide_emit as in
+// bydb_scan_agg_keyed_wide.  The root's call decides the answer's form; ranks may mix the two calls in one collective.
+template <class Out>
+static int scan_reduce_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, Out *out) {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    memset(out, 0, sizeof *out);
+    g_last_dev_err = 0;
+    KeyedAnswer<Out> answer(ctx, out, {});
+    bydb_stats &stats = keyed_stats(out);
+    Plan plan;
+    uint32_t cap = 0;
+    uint64_t fp = 0;
+    size_t slot_bytes = 0;
+    WidePass w;
+    CollectiveHooks h;
+    h.prepare = [&](ExecSlot &es, size_t slot) -> int {
+        slot_bytes = slot;
+        int rc = validate_query(q, true);
+        if (!rc) rc = check_group_key(q, key, kMaxWideKeyValues, false, cap);
+        if (!rc) rc = make_plan(ctx, q, nullptr, plan);
+        if (rc) return rc;
+        if (parts_overlap(plan.parts, q->tmin, q->tmax))
+            return fail(BYDB_ENOTSUP, "group-key query over parts of one rank that overlap in time (version dedup) is not supported on the device path");
+        fp = keyed_wide_fingerprint(q, key, cap);
+        const size_t F = plan.fcols.size(), NS = q->n_series;
+        // the staging of this rank's pass; on the root also the union's read-back and the answer over the most composite groups the
+        // slots can carry (no page-locked allocation may follow inside the collective)
+        size_t pinned = std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256;
+        if (ctx->comm.rank == root) {
+            const size_t per_comp = 8 * (7 * F + 1) + 12, fixed = WideSlot(F, NS, 0, 0).total;
+            const size_t fit = slot > fixed ? (slot - fixed) / per_comp : 0;
+            const size_t most = std::min<size_t>(static_cast<size_t>(ctx->comm.nranks) * fit, static_cast<size_t>(plan.n_groups) * cap);
+            pinned = std::max({pinned, 32 + static_cast<size_t>(cap) * (kMaxLit + 4), keyed_pinned_bytes(q, plan, std::max<size_t>(most, 1), out)});
+        }
+        if (es.ensure_pinned(pinned)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+        return 0;
+    };
+    h.contribute = [&](ExecSlot &es, uint8_t *my_slot) -> int {
+        cudaStream_t s = es.stream;
+        const size_t F = plan.fcols.size(), NS = q->n_series;
+        int rc = wide_pass(ctx, q, key, cap, plan, es, stats, w);
+        if (rc) return rc;
+        const size_t V = w.values.size(), C = w.n_comp;
+        const WideSlot ws(F, NS, V, C);
+        if (ws.total > slot_bytes || C >= kWideMaxRankComposites)
+            return fail(BYDB_EINVAL, "wide keyed collective: this rank's " + std::to_string(V) + " key values and " + std::to_string(C) +
+                                         " composite groups need " + std::to_string(ws.total) +
+                                         " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keyed_wide_reduce_slot_bytes)");
+        if (w.R) {
+            WideReduceParams &rp = w.rp;
+            rp.table = TableLayout(C, F).at(my_slot + ws.off_table);
+            rp.pairs = reinterpret_cast<int32_t *>(my_slot + ws.off_pairs);
+            Scratch pb;
+            CUDA_TRY(pb.alloc(C * 4, s));
+            rp.perm = reinterpret_cast<int32_t *>(pb.base);
+            launch_wide_fold(rp, static_cast<uint32_t>(C), s);
+            Scratch rs;
+            CUDA_TRY(rs.alloc(std::max<size_t>(plan.total_blocks, 1) * 4, s));
+            WideFirstParams fp1;
+            memset(&fp1, 0, sizeof fp1);
+            fp1.rank = w.wk.rank;
+            fp1.rank_series = reinterpret_cast<uint32_t *>(rs.base);
+            fp1.span = reinterpret_cast<int64_t *>(my_slot + ws.off_span);
+            fp1.keys = rp.keys;
+            fp1.seg_start = rp.seg_start;
+            fp1.rec_off = w.wk.n_by_rank;
+            fp1.n_blocks = static_cast<uint32_t>(plan.total_blocks);
+            fp1.n_comp = static_cast<uint32_t>(C);
+            fp1.first = reinterpret_cast<uint32_t *>(my_slot + ws.off_first);
+            launch_wide_series(w.wk.k, fp1, s);
+            launch_wide_first(fp1, s);
+            stats.kernel_launches += 1 + 1 + (C ? 1 : 0);
+        } else {
+            CUDA_TRY(cudaMemsetAsync(my_slot + ws.off_table, 0, F * 8, s));  // no table: the column types of nothing
+        }
+        // the header, the value lengths and the values (pageable: staged before the call returns)
+        std::vector<uint8_t> head(ws.off_span, 0);
+        const uint32_t v32 = static_cast<uint32_t>(V), c32 = static_cast<uint32_t>(C);
+        memcpy(head.data(), &fp, 8);
+        memcpy(head.data() + 8, &v32, 4);
+        memcpy(head.data() + 12, &c32, 4);
+        for (size_t v = 0; v < V; ++v) {
+            const uint32_t len = static_cast<uint32_t>(w.values[v].size());
+            memcpy(head.data() + ws.off_lens + 4 * v, &len, 4);
+            if (len) memcpy(head.data() + ws.off_vals + v * kMaxLit, w.values[v].data(), len);
+        }
+        CUDA_TRY(cudaMemcpyAsync(my_slot, head.data(), head.size(), cudaMemcpyHostToDevice, s));
+        return 0;
+    };
+    h.collect = [&](ExecSlot &) { return 0; };  // the pass was collected as it ran
+    h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &settle, bool &) -> int {
+        int rc = settle();  // a failed rank's slot holds nothing to read
+        if (rc) return rc;
+        cudaStream_t s = es.stream;
+        const uint32_t R = static_cast<uint32_t>(ctx->comm.nranks);
+        const size_t F = plan.fcols.size(), NS = q->n_series;
+        std::vector<uint32_t> v_off(R + 1, 0), row_off(R + 1, 0);
+        for (uint32_t r = 0; r < R; ++r) {
+            uint32_t hd[4] = {0, 0, 0, 0};
+            CUDA_TRY(cudaMemcpy(hd, slots0 + r * slot, 16, cudaMemcpyDeviceToHost));
+            uint64_t theirs = 0;
+            memcpy(&theirs, hd, 8);
+            if (theirs != fp)
+                return fail(BYDB_EINVAL, "wide keyed collective: rank " + std::to_string(r) +
+                                             " passed another query or group key, or called the per-value keyed collective (only the parts may differ between ranks)");
+            v_off[r + 1] = v_off[r] + std::min(hd[2], cap);
+            row_off[r + 1] = row_off[r] + hd[3];
+        }
+        stats.d2h_bytes += 16ull * R;
+        const uint32_t n_vals = v_off[R], n_rows = row_off[R];
+        if (n_vals == 0) return 0;  // no rank selected a block: no rows, no keys
+        // ---- the union of the values, the span check, the union composites
+        const size_t nv = align_up(n_vals, 1024), nr = align_up(std::max<uint32_t>(n_rows, 1), 1024);
+        const size_t VS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_vals), 1024)), CS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_rows), 1024));
+        const size_t N = pow2_at_least(std::max<size_t>(n_rows, 2048));
+        Carve carve;
+        const size_t u_ctl = carve(32), u_off = carve(8 * (R + 1)), u_vslot = carve(VS * 8), u_vid = carve(n_vals * 4), u_vhead = carve(nv * 4),
+                     u_tiles = carve(std::max(nv, nr) / 1024 * 4), u_vals = carve(static_cast<size_t>(cap) * kMaxLit), u_lens = carve(static_cast<size_t>(cap) * 4),
+                     u_comp = carve(CS * 8), u_cranks = carve(CS * 8), u_cfirst = carve(CS * 8), u_cidx = carve(CS * 4), u_rslot = carve(n_rows * 4),
+                     u_rkey = carve(n_rows * 8), u_keys = carve(N * 8), u_seg = carve(nr * 4), u_order = carve(n_rows * 4);
+        Scratch us;
+        CUDA_TRY(us.alloc(carve.o, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl, 0, 32, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl + 12, 0xff, 4, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_vslot, 0, VS * 8, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_comp, 0, CS * 16, s));  // comp, cranks
+        CUDA_TRY(cudaMemsetAsync(us.base + u_cfirst, 0xff, u_rslot - u_cfirst, s));  // cfirst, cidx
+        CUDA_TRY(cudaMemsetAsync(us.base + u_seg, 0, nr * 4, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_order, 0xff, n_rows * 4, s));
+        std::vector<uint32_t> offs(v_off);
+        offs.insert(offs.end(), row_off.begin(), row_off.end());
+        CUDA_TRY(cudaMemcpyAsync(us.base + u_off, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
+        stats.h2d_bytes += offs.size() * 4;
+        WideUnionParams up;
+        memset(&up, 0, sizeof up);
+        up.slots = slots0;
+        up.slot_stride = slot;
+        up.F = static_cast<uint32_t>(F);
+        up.NS = static_cast<uint32_t>(NS);
+        up.cap = cap;
+        up.n_ranks = R;
+        up.tmin = q->tmin;
+        up.tmax = q->tmax;
+        up.v_off = reinterpret_cast<const uint32_t *>(us.base + u_off);
+        up.row_off = up.v_off + (R + 1);
+        up.n_vals = n_vals;
+        up.n_rows = n_rows;
+        up.vmask = static_cast<uint32_t>(VS - 1);
+        up.cmask = static_cast<uint32_t>(CS - 1);
+        up.vslot = reinterpret_cast<unsigned long long *>(us.base + u_vslot);
+        up.vid = reinterpret_cast<uint32_t *>(us.base + u_vid);
+        up.vhead = reinterpret_cast<uint32_t *>(us.base + u_vhead);
+        up.tiles = reinterpret_cast<uint32_t *>(us.base + u_tiles);
+        up.vals = us.base + u_vals;
+        up.lens = reinterpret_cast<uint32_t *>(us.base + u_lens);
+        up.comp = reinterpret_cast<unsigned long long *>(us.base + u_comp);
+        up.cranks = reinterpret_cast<unsigned long long *>(us.base + u_cranks);
+        up.cfirst = reinterpret_cast<unsigned long long *>(us.base + u_cfirst);
+        up.cidx = reinterpret_cast<uint32_t *>(us.base + u_cidx);
+        up.row_slot = reinterpret_cast<uint32_t *>(us.base + u_rslot);
+        up.row_key = reinterpret_cast<unsigned long long *>(us.base + u_rkey);
+        up.n_sort = static_cast<uint32_t>(N);
+        up.keys = reinterpret_cast<unsigned long long *>(us.base + u_keys);
+        up.seg = reinterpret_cast<uint32_t *>(us.base + u_seg);
+        up.order = reinterpret_cast<uint32_t *>(us.base + u_order);
+        up.ctl = reinterpret_cast<uint32_t *>(us.base + u_ctl);
+        stats.kernel_launches += launch_wide_union(up, s);
+        CUDA_TRY(cudaMemcpyAsync(es.pinned, up.ctl, 16, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaGetLastError());
+        stats.d2h_bytes += 16;
+        uint32_t ctl[4];
+        memcpy(ctl, es.pinned, 16);
+        if (ctl[0] > cap)
+            return fail(BYDB_ENOMEM, "wide keyed collective: more distinct key values over all ranks than bydb_group_key.max_values (" + std::to_string(cap) + ")");
+        if (ctl[2] == kErrRankOverlap) {
+            const uint32_t i = ctl[3];
+            return fail(BYDB_ENOTSUP, "wide keyed collective: series #" + std::to_string(i) + " (id " + std::to_string(i < NS ? q->series_ids[i] : 0) +
+                                          ") lives on several ranks over time spans that intersect");
+        }
+        const size_t V = ctl[0], C = ctl[1];
+        // ---- the union composites in insertion order, folded over their ranks into a table of C_u groups
+        const TableLayout tl(std::max<size_t>(C, 1), F);
+        Carve cf;
+        const size_t f_table = cf(tl.total), f_pairs = cf(C * 8), f_perm = cf(C * 4);
+        Scratch fb;
+        CUDA_TRY(fb.alloc(cf.o, s));
+        up.table = tl.at(fb.base + f_table);
+        up.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
+        up.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
+        if (C) stats.kernel_launches += launch_wide_merge(up, static_cast<uint32_t>(C), s);
+        CUDA_TRY(cudaMemcpyAsync(es.pinned, up.vals, V * kMaxLit, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(es.pinned + V * kMaxLit, up.lens, V * 4, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaGetLastError());
+        stats.d2h_bytes += V * (kMaxLit + 4);
+        set_key_table(out, answer.owner, unpack_values(V, false, es.pinned, reinterpret_cast<const uint32_t *>(es.pinned + V * kMaxLit)));
+        if (C == 0) return 0;
+        WideReduceParams rp;
+        memset(&rp, 0, sizeof rp);
+        rp.pairs = up.pairs;
+        rp.perm = up.perm;
+        rp.ctl = up.ctl;  // ctl[1] = C_u, the present rows keyed_partial_rows_kernel reads
+        return wide_emit(q, plan, es, fb.base + f_table, tl, C, rp, out, answer.owner);
+    };
+    h.discard = [] {};  // the result of a failed call is freed by `answer`
+    const int rc = run_collective(ctx, root, 0, h);
+    if (rc) return rc;
+    answer.done = true;
+    return 0;
+}
+
+extern "C" {
+
+int bydb_scan_reduce_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out) {
+    return guarded([&]() -> int { return scan_reduce_keyed_wide_impl(ctx, q, key, root, out); });
+}
+
+int bydb_scan_reduce_keyed_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root,
+                                         bydb_keyed_partial_rows *out) {
+    return guarded([&]() -> int { return scan_reduce_keyed_wide_impl(ctx, q, key, root, out); });
 }
 
 int bydb_scan_reduce(bydb_ctx *ctx, const bydb_query *q, int32_t root, bydb_result *out) {

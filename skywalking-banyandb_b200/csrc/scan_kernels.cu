@@ -5474,6 +5474,302 @@ void launch_wide_fold(const WideReduceParams &p, uint32_t n_comp, cudaStream_t s
     wide_fold_kernel<<<(warps + 7) / 8, 256, 0, s>>>(p, n_comp);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Wide keyed collective (bydb_scan_reduce_keyed_wide): every rank ran the wide path's discovery, scan and order, and folded its
+// present composite groups straight into its slot of the root's mailbox (layout: WideSlot), with each one's first series and the
+// series' spans.  The root merges the ranks' lists: the union of the values, the span check, the union composites in the
+// insertion order of the whole scan, each folded over its ranks in rank order (see WideUnionParams).
+// ------------------------------------------------------------------------------------------------
+__global__ void wide_series_kernel(const __grid_constant__ KeyParams k, const WideFirstParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < k.n_series) {
+        const uint64_t sid = k.q_sids[t];
+        int64_t lo = INT64_MAX, hi = INT64_MIN;
+        for (uint32_t pi = 0; pi < k.n_parts; ++pi) {
+            const DevPartRef &part = k.parts[pi];
+            for (uint32_t b = lower_sid(part, sid), e = upper_sid(part, sid); b < e; ++b) {
+                const DevBlock &blk = part.blocks[b];
+                int32_t qi;
+                if (!select_block(k.q_sids, k.n_series, k.tmin, k.tmax, blk, qi)) continue;
+                lo = blk.ts_min < lo ? blk.ts_min : lo;
+                hi = blk.ts_max > hi ? blk.ts_max : hi;
+            }
+        }
+        p.span[2 * static_cast<size_t>(t)] = lo;
+        p.span[2 * static_cast<size_t>(t) + 1] = hi;
+    }
+    if (t < k.total_blocks) {
+        uint32_t pi = 0;
+        while (pi + 1 < k.n_parts && t >= k.parts[pi + 1].block_base) ++pi;
+        int32_t qi;
+        if (select_block(k.q_sids, k.n_series, k.tmin, k.tmax, k.parts[pi].blocks[t - k.parts[pi].block_base], qi)) p.rank_series[p.rank[t]] = static_cast<uint32_t>(qi);
+    }
+}
+__global__ void wide_first_kernel(const WideFirstParams p) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= p.n_comp) return;
+    const uint32_t rec = static_cast<uint32_t>(p.keys[p.seg_start[j]]);
+    uint32_t lo = 0, hi = p.n_blocks;  // the first rank whose records start above rec
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (p.rec_off[mid] <= rec) lo = mid + 1;
+        else hi = mid;
+    }
+    p.first[j] = p.rank_series[lo - 1];
+}
+void launch_wide_series(const KeyParams &k, const WideFirstParams &p, cudaStream_t s) {
+    const uint32_t n = k.n_series > k.total_blocks ? k.n_series : k.total_blocks;
+    if (n) wide_series_kernel<<<(n + 255) / 256, 256, 0, s>>>(k, p);
+}
+void launch_wide_first(const WideFirstParams &p, cudaStream_t s) {
+    if (p.n_comp) wide_first_kernel<<<(p.n_comp + 255) / 256, 256, 0, s>>>(p);
+}
+
+// rank r's header words, its value count clamped to the cap, and its slot layout
+__device__ __forceinline__ const uint8_t *wide_slot_at(const WideUnionParams &p, uint32_t r) { return p.slots + r * p.slot_stride; }
+__device__ __forceinline__ WideSlot wide_slot_layout(const WideUnionParams &p, uint32_t r) {
+    const uint32_t *h = reinterpret_cast<const uint32_t *>(wide_slot_at(p, r));
+    return WideSlot(p.F, p.NS, h[2] < p.cap ? h[2] : p.cap, h[3]);
+}
+// the rank of flat index t of an exclusive scan over the ranks
+__device__ __forceinline__ uint32_t wide_rank_of(const uint32_t *off, uint32_t n_ranks, uint32_t t) {
+    uint32_t r = 0;
+    while (r + 1 < n_ranks && off[r + 1] <= t) ++r;
+    return r;
+}
+// value v of rank r: its bytes and length
+__device__ __forceinline__ const uint8_t *wide_value(const WideUnionParams &p, uint32_t r, uint32_t v, uint32_t &len) {
+    const uint8_t *slot = wide_slot_at(p, r);
+    const WideSlot ws = wide_slot_layout(p, r);
+    len = min(reinterpret_cast<const uint32_t *>(slot + ws.off_lens)[v], static_cast<uint32_t>(kMaxLit));
+    return slot + ws.off_vals + static_cast<size_t>(v) * kMaxLit;
+}
+
+__global__ void wide_union_insert_kernel(const __grid_constant__ WideUnionParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= p.n_vals) return;
+    const uint32_t r = wide_rank_of(p.v_off, p.n_ranks, t), v = t - p.v_off[r];
+    uint32_t len;
+    const uint8_t *b = wide_value(p, r, v, len);
+    const unsigned long long mine = ((static_cast<unsigned long long>(r) << 32) | v) + 1ull;
+    uint32_t s = key_home(b, len, p.vmask);
+    for (;;) {  // the table has twice the values' slots: a free one is always ahead
+        unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.vslot[s]);
+        if (cur == 0ull) cur = atomicCAS(&p.vslot[s], 0ull, mine);
+        if (cur == 0ull) break;
+        uint32_t olen;
+        const uint8_t *o = wide_value(p, static_cast<uint32_t>((cur - 1ull) >> 32), static_cast<uint32_t>(cur - 1ull), olen);
+        bool eq = olen == len;
+        for (uint32_t i = 0; i < len && eq; ++i) eq = __ldg(o + i) == __ldg(b + i);
+        if (eq) {
+            atomicMin(&p.vslot[s], mine);
+            break;
+        }
+        s = (s + 1) & p.vmask;
+    }
+    p.vid[t] = s;
+}
+__global__ void wide_union_heads_kernel(const __grid_constant__ WideUnionParams p, uint32_t n) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    uint32_t head = 0;
+    if (t < p.n_vals) {
+        const uint32_t r = wide_rank_of(p.v_off, p.n_ranks, t), v = t - p.v_off[r];
+        head = p.vslot[p.vid[t]] - 1ull == ((static_cast<unsigned long long>(r) << 32) | v) ? 1u : 0u;
+    }
+    p.vhead[t] = head;
+}
+__global__ void wide_union_ids_kernel(const __grid_constant__ WideUnionParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= p.n_vals) return;
+    const unsigned long long w = p.vslot[p.vid[t]] - 1ull;
+    const uint32_t ro = static_cast<uint32_t>(w >> 32), vo = static_cast<uint32_t>(w);
+    const uint32_t owner = p.v_off[ro] + vo, u = p.vhead[owner];
+    if (owner == t && u < p.cap) {
+        uint32_t len;
+        const uint8_t *b = wide_value(p, ro, vo, len);
+        for (uint32_t i = 0; i < len; ++i) p.vals[static_cast<size_t>(u) * kMaxLit + i] = __ldg(b + i);
+        p.lens[u] = len;
+    }
+    p.vid[t] = u;
+}
+
+// [lo, hi] of series i on rank r, clipped to the query's range; false = the rank selects no block of it (rank_span's rule)
+__device__ __forceinline__ bool wide_rank_span(const WideUnionParams &p, uint32_t r, uint32_t i, int64_t &lo, int64_t &hi) {
+    if (reinterpret_cast<const uint32_t *>(wide_slot_at(p, r))[2] == 0) return false;  // no selected block: no spans were written
+    const int64_t *sp = reinterpret_cast<const int64_t *>(wide_slot_at(p, r) + wide_slot_layout(p, r).off_span) + 2 * static_cast<size_t>(i);
+    lo = sp[0] > p.tmin ? sp[0] : p.tmin;
+    hi = sp[1] < p.tmax ? sp[1] : p.tmax;
+    return lo <= hi;
+}
+// rank_span_check_kernel over the wide slots: one warp per series, the ranks' spans pairwise
+__global__ void __launch_bounds__(256) wide_span_check_kernel(const __grid_constant__ WideUnionParams p) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= p.NS) return;
+    const uint32_t R = p.n_ranks, pairs = R * (R - 1) / 2;
+    bool hit = false;
+    for (uint32_t k = lane; k < pairs && !hit; k += 32) {
+        uint32_t a = 0, rem = k;
+        while (rem >= R - 1 - a) rem -= R - 1 - a++;
+        const uint32_t b = a + 1 + rem;
+        int64_t alo, ahi, blo, bhi;
+        if (wide_rank_span(p, a, i, alo, ahi) && wide_rank_span(p, b, i, blo, bhi)) hit = (alo > blo ? alo : blo) <= (ahi < bhi ? ahi : bhi);
+    }
+    if (__any_sync(0xffffffffu, hit) && lane == 0) {
+        atomicMin(&p.ctl[3], i);
+        atomicCAS(&p.ctl[2], 0u, static_cast<uint32_t>(kErrRankOverlap));
+    }
+}
+// the order of rank r's span among the ranks' spans of series i (by start; a tie, which the span check refuses, by rank)
+__device__ uint32_t wide_span_order(const WideUnionParams &p, uint32_t r, uint32_t i) {
+    int64_t lo, hi, olo, ohi;
+    if (!wide_rank_span(p, r, i, lo, hi)) return 0;
+    uint32_t o = 0;
+    for (uint32_t q = 0; q < p.n_ranks; ++q)
+        if (q != r && wide_rank_span(p, q, i, olo, ohi) && (olo < lo || (olo == lo && q < r))) ++o;
+    return o;
+}
+__device__ __forceinline__ unsigned long long wide_order_key(uint32_t series, uint32_t span_order, uint32_t j) {
+    return (static_cast<unsigned long long>(series) << 33) | (static_cast<unsigned long long>(span_order & 63u) << 27) | (j & (kWideMaxRankComposites - 1));
+}
+__global__ void wide_comp_union_kernel(const __grid_constant__ WideUnionParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= p.n_rows) return;
+    const uint32_t r = wide_rank_of(p.row_off, p.n_ranks, t), j = t - p.row_off[r];
+    const uint8_t *slot = wide_slot_at(p, r);
+    const WideSlot ws = wide_slot_layout(p, r);
+    const int32_t *pair = reinterpret_cast<const int32_t *>(slot + ws.off_pairs) + 2 * static_cast<size_t>(j);
+    const uint32_t u = p.vid[p.v_off[r] + static_cast<uint32_t>(pair[1])];
+    const unsigned long long key = ((static_cast<unsigned long long>(static_cast<uint32_t>(pair[0])) << 32) | u) + 1ull;
+    uint32_t s = key_slot_i64(key, p.cmask);
+    for (;;) {  // twice the rows' slots: a free one is always ahead
+        unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.comp[s]);
+        if (cur == 0ull) {
+            cur = atomicCAS(&p.comp[s], 0ull, key);
+            if (cur == 0ull) atomicAdd(&p.ctl[1], 1u);
+        }
+        if (cur == 0ull || cur == key) break;
+        s = (s + 1) & p.cmask;
+    }
+    const uint32_t series = reinterpret_cast<const uint32_t *>(slot + ws.off_first)[j];
+    const unsigned long long k = wide_order_key(series, wide_span_order(p, r, series), j);
+    p.row_slot[t] = s;
+    p.row_key[t] = k;
+    atomicMin(&p.cfirst[s], k);
+    atomicOr(&p.cranks[s], 1ull << r);
+}
+__global__ void wide_comp_keys_kernel(const __grid_constant__ WideUnionParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= p.n_sort) return;
+    p.keys[t] = t < p.n_rows && p.cfirst[p.row_slot[t]] == p.row_key[t] ? p.row_key[t] : ~0ull;
+}
+// composite c < C_u: the row its least key names (the rank whose span of that series has that order) -> its slot
+__global__ void wide_comp_place_kernel(const __grid_constant__ WideUnionParams p, uint32_t n_comp) {
+    const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_comp) return;
+    const unsigned long long k = p.keys[c];
+    const uint32_t series = static_cast<uint32_t>(k >> 33), o = static_cast<uint32_t>(k >> 27) & 63u, j = static_cast<uint32_t>(k) & (kWideMaxRankComposites - 1);
+    for (uint32_t r = 0; r < p.n_ranks; ++r) {
+        int64_t lo, hi;
+        if (j >= p.row_off[r + 1] - p.row_off[r] || !wide_rank_span(p, r, series, lo, hi) || wide_span_order(p, r, series) != o) continue;
+        const uint32_t t = p.row_off[r] + j, s = p.row_slot[t];
+        if (p.row_key[t] != k) continue;
+        const unsigned long long key = p.comp[s] - 1ull;
+        p.cidx[s] = c;
+        p.seg[c] = __popcll(p.cranks[s]);
+        p.pairs[2 * static_cast<size_t>(c)] = static_cast<int32_t>(key >> 32);
+        p.pairs[2 * static_cast<size_t>(c) + 1] = static_cast<int32_t>(static_cast<uint32_t>(key));
+        p.perm[c] = static_cast<int32_t>(c);
+        return;
+    }
+}
+__global__ void wide_comp_order_kernel(const __grid_constant__ WideUnionParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= p.n_rows) return;
+    const uint32_t s = p.row_slot[t], c = p.cidx[s];
+    if (c == 0xffffffffu) return;  // only under a span intersection, which fails the call
+    const uint32_t r = wide_rank_of(p.row_off, p.n_ranks, t);
+    p.order[p.seg[c] + __popcll(p.cranks[s] & ((1ull << r) - 1ull))] = t;
+}
+// One thread per word of the union table (c, field) and per column type: composite c's rows in rank order with
+// combine_tables_kernel's per-word rule (deterministic float sums); the column types of every rank merge (merge_coltype), so a
+// field stored as int64 on one rank and float64 on another fails as it does inside one scan.
+__global__ void wide_comp_fold_kernel(const __grid_constant__ WideUnionParams p, uint32_t n_comp) {
+    const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    const uint64_t F = p.F, CF = static_cast<uint64_t>(n_comp) * F, words = 7 * CF + n_comp;
+    if (i >= words + F) return;
+    if (i >= words) {
+        const uint32_t c = static_cast<uint32_t>(i - words);
+        int64_t typ = 0, err = 0;
+        for (uint32_t r = 0; r < p.n_ranks; ++r) {
+            const WideSlot ws = wide_slot_layout(p, r);
+            const uint64_t Cr = p.row_off[r + 1] - p.row_off[r];
+            merge_coltype(reinterpret_cast<const int64_t *>(wide_slot_at(p, r) + ws.off_table)[7 * Cr * F + Cr + c], typ, err);
+        }
+        p.table.coltype[c] = typ | (err << 8);
+        return;
+    }
+    // region of the word: sum_f64 | max_f64 | negmin_f64 | sum_i64 | cnt | rows | max_i64 | notmin_i64 (TableLayout's order)
+    const int reg = i < 5 * CF ? static_cast<int>(i / CF) : i < 5 * CF + n_comp ? 5 : static_cast<int>(6 + (i - 5 * CF - n_comp) / CF);
+    const int kind = reg == 0 ? kWordFsum : reg <= 2 ? kWordFmax : reg <= 5 ? kWordIsum : kWordImax;
+    const uint64_t k = reg < 5 ? i - reg * CF : reg == 5 ? i - 5 * CF : i - 5 * CF - n_comp - (reg - 6) * CF;
+    const uint64_t c = reg == 5 ? k : k / F, f = reg == 5 ? 0 : k % F;
+    const uint32_t lo = p.seg[c], hi = c + 1 < n_comp ? p.seg[c + 1] : p.n_rows;
+    uint64_t a = 0;
+    bool first = true;
+    for (uint32_t e = lo; e < hi; ++e) {
+        const uint32_t t = p.order[e];
+        if (t >= p.n_rows) continue;  // only under a span intersection, which fails the call
+        const uint32_t r = wide_rank_of(p.row_off, p.n_ranks, t);
+        const uint64_t j = t - p.row_off[r], Cr = p.row_off[r + 1] - p.row_off[r], CFr = Cr * F;
+        const uint64_t base = reg <= 5 ? reg * CFr : 5 * CFr + Cr + (reg - 6) * CFr;
+        const uint64_t w = reinterpret_cast<const uint64_t *>(wide_slot_at(p, r) + wide_slot_layout(p, r).off_table)[base + (reg == 5 ? j : j * F + f)];
+        a = first ? w : combine_word(a, w, kind);
+        first = false;
+    }
+    reinterpret_cast<uint64_t *>(p.table.sum_f64)[i] = a;  // the regions lie back to back from sum_f64 on
+}
+
+uint32_t launch_wide_union(const WideUnionParams &p, cudaStream_t s) {
+    const uint32_t nv = (p.n_vals + 1023u) / 1024u * 1024u;
+    uint32_t n = 0;
+    if (p.n_vals) {
+        wide_union_insert_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
+        wide_union_heads_kernel<<<nv / 256, 256, 0, s>>>(p, nv);
+        launch_excl_scan(p.vhead, nv, p.tiles, &p.ctl[0], s);
+        wide_union_ids_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
+        n += 6;
+    }
+    if (p.NS && p.n_ranks > 1) {
+        wide_span_check_kernel<<<(p.NS + 7) / 8, 256, 0, s>>>(p);
+        n += 1;
+    }
+    if (p.n_rows) {
+        wide_comp_union_kernel<<<(p.n_rows + 255) / 256, 256, 0, s>>>(p);
+        n += 1;
+    }
+    return n;
+}
+uint32_t launch_wide_merge(const WideUnionParams &p, uint32_t n_comp, cudaStream_t s) {
+    const uint32_t N = p.n_sort, nr = (p.n_rows + 1023u) / 1024u * 1024u;
+    uint32_t n = 0;
+    wide_comp_keys_kernel<<<N / 256, 256, 0, s>>>(p);
+    bitonic_tile_kernel<<<N / 2048, 1024, 0, s>>>(p.keys, 2, 2048);
+    n += 2;
+    for (uint32_t size = 4096; size <= N; size <<= 1) {
+        for (uint32_t j = size >> 1; j >= 2048; j >>= 1, ++n) bitonic_step_kernel<<<N / 2 / 256, 256, 0, s>>>(p.keys, j, size, N / 2);
+        bitonic_tile_kernel<<<N / 2048, 1024, 0, s>>>(p.keys, size, size);
+        n += 1;
+    }
+    wide_comp_place_kernel<<<(n_comp + 255) / 256, 256, 0, s>>>(p, n_comp);
+    launch_excl_scan(p.seg, nr, p.tiles, &p.ctl[0] + 4, s);
+    wide_comp_order_kernel<<<(p.n_rows + 255) / 256, 256, 0, s>>>(p);
+    const uint64_t words = (7ull * p.F + 1) * n_comp + p.F;
+    wide_comp_fold_kernel<<<static_cast<unsigned>((words + 255) / 256), 256, 0, s>>>(p, n_comp);
+    return n + 6;
+}
+
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s) {
     if (p.total_blocks == 0) return;
     const int threads = 256;

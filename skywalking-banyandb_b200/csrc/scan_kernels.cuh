@@ -460,6 +460,91 @@ struct KeyedUnionParams {
 void launch_key_union(const KeyedUnionParams &p, cudaStream_t s);
 // combine_keyed_kernel and merge_first_kernel into table / coltype / Kts / Krow (p.n_values = V_u > 0)
 void launch_combine_keyed(const KeyedUnionParams &p, cudaStream_t s);
+// ---- wide keyed collective (bydb_scan_reduce_keyed_wide): the slot of a rank that found V key values and C present composite
+// groups, for F fields and NS series.  Every region starts on a 256-byte boundary; the root derives a rank's layout from the
+// V_r and C_r in its header.
+//   header    u64 query fingerprint | u32 V_r | u32 C_r
+//   lens      [V] u32, values [V][kMaxLit] (an int64 key's 8 little-endian bytes, length 8)
+//   span      [NS][2] i64 the series' selected blocks (as ReduceParams::span)
+//   pairs     [C][2] i32 (series group, value id) of composite j, in the rank's insertion order (wide_fold_kernel)
+//   first     [C] u32 the series index of composite j's first row
+//   table     the rank's composite table TableLayout(C, F) in its insertion order (wide_fold_kernel)
+struct WideSlot {
+    size_t off_lens, off_vals, off_span, off_pairs, off_first, off_table, total;
+    __host__ __device__ WideSlot(size_t F, size_t NS, size_t V, size_t C) {
+        off_lens = 256;
+        off_vals = KeyedSlot::up(off_lens + V * 4);
+        off_span = KeyedSlot::up(off_vals + V * kMaxLit);
+        off_pairs = KeyedSlot::up(off_span + NS * 16);
+        off_first = KeyedSlot::up(off_pairs + C * 8);
+        off_table = KeyedSlot::up(off_first + C * 4);
+        total = off_table + 8 * (C * (7 * F + 1) + F);  // TableLayout(C, F).total
+    }
+};
+// A rank's first appearances: ranks whose records the scan wrote (WideKeyParams::rank, WideScanParams::rec_off) back to series.
+//   wide_series_kernel: thread i < NS writes span[i] (the series' selected blocks over every part); thread g < total_blocks writes
+//     the series index of a selected block at its scan-order rank, rank_series[rank[g]]
+//   wide_first_kernel: composite j < n_comp (its lowest record keys[seg_start[j]]) -> the block holding that record (the last rank
+//     whose rec_off does not exceed it) -> first[j] = that block's series index
+struct WideFirstParams {
+    const uint32_t *rank;             // WideKeyParams::rank
+    uint32_t *rank_series;            // [total_blocks]
+    int64_t *span;                    // [2 * NS]
+    const unsigned long long *keys;   // WideReduceParams::keys, sorted
+    const uint32_t *seg_start;        // WideReduceParams::seg_start
+    const uint32_t *rec_off;          // WideScanParams::rec_off
+    uint32_t n_blocks, n_comp;
+    uint32_t *first;                  // [n_comp]
+};
+static_assert(sizeof(KeyParams) + sizeof(WideFirstParams) <= 4096, "kernel-parameter space");
+void launch_wide_series(const KeyParams &k, const WideFirstParams &p, cudaStream_t s);
+void launch_wide_first(const WideFirstParams &p, cudaStream_t s);
+// The root of the wide collective.  Flat indices: rank r's value v is v_off[r] + v, its composite row j is row_off[r] + j.
+//   1. the union of the values (launch_wide_union): every (r, v) enters a table homed by key_home over its bytes; the slot keeps the
+//      least (r, v) with those bytes; the least ones are numbered by an exclusive scan in (r, v) order -- ranks in rank order, each
+//      rank's values in its order -- and write the union values; vid[r, v] = the union id.  wide_span_check_kernel is
+//      rank_span_check_kernel's rule over the wide slots.  wide_comp_union_kernel enters each row's composite (g, union id) into a
+//      composite table (ctl[1] = C_u) with its order key, the least key of a composite and the set of ranks that hold it.
+//   2. the merge (launch_wide_merge): the composites sorted by their least order key are the insertion order of the whole scan;
+//      each composite's rows are laid out in rank order, and wide_comp_fold_kernel folds them with combine_word into row c of a
+//      TableLayout(C_u, F) table and pairs[c] = (g, u).
+// Order key of a row (wide_order_key): series index of its first row << 33 | the span order of its rank within that series << 27
+// | its position in its rank's list.  Exact because a series' spans on different ranks are disjoint (the span check): its earlier
+// span comes first in the scan.  The fields fit: series indexes are below 2^31, ranks at most 64, a rank's list at most
+// kWideMaxRankComposites long.
+constexpr uint32_t kWideMaxRankComposites = 1u << 27;
+struct WideUnionParams {
+    const uint8_t *slots;             // rank r's slot at slots + r * slot_stride (the root's mailbox, this collective's parity)
+    size_t slot_stride;
+    uint32_t F, NS, cap, n_ranks;
+    int64_t tmin, tmax;               // the query's range (span check)
+    const uint32_t *v_off, *row_off;  // [n_ranks + 1] exclusive scans of V_r and C_r
+    uint32_t n_vals, n_rows;          // sum of V_r, sum of C_r
+    uint32_t vmask, cmask;            // slots - 1 of the value and composite tables (powers of two, at least twice the entries)
+    unsigned long long *vslot;        // [vmask + 1] least (r << 32 | v) + 1 with the slot's bytes, 0 = empty
+    uint32_t *vid;                    // [n_vals] the value's slot, then its union id
+    uint32_t *vhead;                  // [align(n_vals, 1024)] 1 = (r, v) is the least with its bytes, then (exclusive scan) its union id
+    uint32_t *tiles;                  // [align(max(n_vals, n_rows), 1024) / 1024] the exclusive scans' tile sums
+    uint8_t *vals;                    // [cap * kMaxLit] union values
+    uint32_t *lens;                   // [cap]
+    unsigned long long *comp;         // [cmask + 1] composite (g << 32 | u) + 1, 0 = empty
+    unsigned long long *cfirst;       // [cmask + 1] least order key of the composite's rows, preset ~0
+    unsigned long long *cranks;       // [cmask + 1] bit r: rank r holds the composite
+    uint32_t *cidx;                   // [cmask + 1] the composite's position in insertion order, preset 0xffffffff
+    uint32_t *row_slot;               // [n_rows] composite slot of the row
+    unsigned long long *row_key;      // [n_rows] order key of the row
+    uint32_t n_sort;                  // power of two >= max(n_rows, 2048)
+    unsigned long long *keys;         // [n_sort] the composites' least keys, ~0 elsewhere
+    uint32_t *seg;                    // [align(n_rows, 1024)] rows of composite c, then (exclusive scan) its first entry in `order`
+    uint32_t *order;                  // [n_rows] flat rows, composite by composite, each composite's in rank order
+    uint32_t *ctl;                    // [0] V_u [1] C_u [2] DevErr of the span check [3] first series whose spans intersect (preset ~0)
+    TablePtrs table;                  // TableLayout(C_u, F)
+    int32_t *pairs;                   // [2 * C_u]
+    int32_t *perm;                    // [C_u] c (the identity order keyed_partial_rows_kernel reads)
+};
+// -> kernels launched
+uint32_t launch_wide_union(const WideUnionParams &p, cudaStream_t s);
+uint32_t launch_wide_merge(const WideUnionParams &p, uint32_t n_comp, cudaStream_t s);
 // dst[j] = src[perm[j]] for every group row of a partial table; coltype = the passes' column types merged
 void launch_permute_table(const TablePtrs &dst, const TablePtrs &src, const int32_t *perm, uint32_t n_groups, uint32_t n_fcols,
                           const int64_t *pass_coltype, uint32_t n_passes, cudaStream_t s);
