@@ -80,8 +80,10 @@ def _edges():
     return out
 
 
-def _part(rng, n_pad=72_000):
-    blocks = []   # (name, int64 values)
+def _blocks(rng, n_pad=72_000):
+    """-> ((name, int64 values) of every block in series order, number of boundary blocks in front of the padding).  The
+    pages keep their varints (no dense form, tests/test_gpu_dense_boundaries.py), so these blocks pin the SWAR decode."""
+    blocks = []
     for name, lens in _edges():
         blocks.append((name, values_with_lengths(lens, rng)))
         # behind every boundary block: a page of long varints, a narrow page, a 1-row block
@@ -91,6 +93,11 @@ def _part(rng, n_pad=72_000):
     n_lead = len(blocks)
     for _ in range(n_pad):
         blocks.append(("pad", values_with_lengths([1] * 23, rng)))
+    return blocks, n_lead
+
+
+def _part(rng, n_pad=72_000):
+    blocks, n_lead = _blocks(rng, n_pad)
     express = slow = 0
     for name, v in blocks[:n_lead]:
         cls = page_class(v, None, True) if v.size > 1 else "const"

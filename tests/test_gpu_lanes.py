@@ -336,12 +336,8 @@ def test_varint_at_every_boundary(bydb, gpu_ctx, width):
 
 
 # ------------------------------------------------------------------ express batch hand-over
-@gpu
-def test_express_batch_handover(bydb, gpu_ctx):
-    """A warp of the express lane takes up to 8 blocks at a time and streams their pages through one TMA ring; it does so while
-    more than 16 blocks per warp are left, so the part holds ~72k blocks and the mixed pages sit at its front.  The mix: 1-row
-    blocks (no page body), bodies of exactly 2048 and 4096 bytes (a stage / two), 2047 and 2049, narrow 3-byte pages, and one
-    wide page per group of 8, which leaves the ring while its neighbours stay."""
+def handover_blocks():
+    """-> (kinds, rows, int64 values) of the blocks of test_express_batch_handover, in series order."""
     rng = np.random.default_rng(8)
     pattern = [("n", 1), ("b", 2049), ("b", 2048), ("w", 2050), ("b", 4097), ("b", 2050), ("d3", 600), ("b", 4096)]
     lens, kinds = [], []
@@ -349,9 +345,7 @@ def test_express_batch_handover(bydb, gpu_ctx):
         k, n = pattern[i % 8] if i < 4000 else ("b", 24)
         lens.append(n)
         kinds.append(k)
-    sids = np.repeat(np.arange(1, len(lens) + 1, dtype=np.uint64), lens)
-    ts = np.concatenate([T0 + np.arange(n, dtype=np.int64) * STEP for n in lens])
-    vals, expect_express, expect_slow = [], 0, 0
+    vals = []
     for k, n in zip(kinds, lens):
         if k == "n":
             v = np.array([int(rng.integers(0, 100))], np.int64)
@@ -359,10 +353,25 @@ def test_express_batch_handover(bydb, gpu_ctx):
             v = shape_values("d3", n, rng)[0]
         else:
             v = wide_at(n // 2, n, 4) if k == "w" else np.concatenate([[50], 50 + np.cumsum(_signed(rng, 0, 63, n - 1))])
-        cls = page_class(v, None, False) if n > 1 else "const"
+        vals.append(np.asarray(v, np.int64))
+    return kinds, lens, vals
+
+
+@gpu
+def test_express_batch_handover(bydb, gpu_ctx):
+    """A warp of the express lane takes up to 8 blocks at a time and streams their pages through one TMA ring; it does so while
+    more than 16 blocks per warp are left, so the part holds ~72k blocks and the mixed pages sit at its front.  The mix: 1-row
+    blocks (no page body), bodies of exactly 2048 and 4096 bytes (a stage / two), 2047 and 2049, narrow 3-byte pages, and one
+    wide page per group of 8, which leaves the ring while its neighbours stay.  These pages keep their varints (no dense form,
+    tests/test_gpu_dense_boundaries.py), so the test pins the SWAR decode."""
+    kinds, lens, vals = handover_blocks()
+    sids = np.repeat(np.arange(1, len(lens) + 1, dtype=np.uint64), lens)
+    ts = np.concatenate([T0 + np.arange(n, dtype=np.int64) * STEP for n in lens])
+    expect_express = expect_slow = 0
+    for v in vals:
+        cls = page_class(v, None, False) if v.size > 1 else "const"
         expect_express += cls == "delta"
         expect_slow += cls == "wide"
-        vals.append(np.asarray(v, np.int64))
     body = {("b", 2049): 2048, ("b", 2048): 2047, ("b", 2050): 2049, ("b", 4097): 4096, ("b", 4096): 4095}
     for (k, n), want_body in body.items():   # the page bodies the case claims
         i = list(zip(kinds, lens)).index((k, n))
