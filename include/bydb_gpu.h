@@ -455,6 +455,41 @@ void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r);
 int bydb_scan_agg_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out);
 int bydb_scan_partials_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out);
 
+/* Prepared wide group-by on a stored tag: bydb_scan_agg_keyed_wide for a query executed many times (a dashboard panel grouped by
+ * endpoint, instance or status code).  The handle is a bydb_prepared_keyed: bydb_scan_agg_keyed_prepared,
+ * bydb_scan_partials_keyed_prepared and bydb_query_release_keyed take it, and on it answer what bydb_scan_agg_keyed_wide /
+ * bydb_scan_partials_keyed_wide answer at that moment: code and device-error text, rows in the same order, each row's series group
+ * and key bytes, values bit for bit, n_keys, and the counters (rows_scanned, rows_matched, page_bytes, blocks_scanned, ...).
+ *   - Arguments: checked at prepare as the wide call checks them, in its order and with its codes (max_values 0 means 64,
+ *     1..65,536 accepted, above BYDB_EINVAL; up to 8 predicates, the key takes no slot; the key's type).  A refusal that depends
+ *     on the data (above max_values: BYDB_ENOMEM; a block with more than 256 values, a plain string key page or a 65-byte value,
+ *     parts that overlap in time: BYDB_ENOTSUP) comes at every execution as the unprepared call gives it, and the handle keeps the
+ *     unprepared path for good.
+ *   - Schedule: the first execution runs the unprepared wide path; the second runs its discovery, scan and order once to learn
+ *     the key table, R and C (functions of the parts the handles name and of the query), captures the step -- a reset kernel,
+ *     the scan, the order, the fold into C composite groups, the form's tail and its read-back -- as ONE CUDA graph, and answers
+ *     from its first replay; later executions replay it, with the key table found at the capture (the same on every replay).
+ *     Part lifecycle, one step per handle of the form last asked for, one execution at a time per handle: as the keyed prepared
+ *     forms above.  V = 0 (no block selected) needs no graph: no rows, no keys, zero stats.  C = 0 captures and answers no rows.
+ *   - Stats of a replay: h2d_bytes = 0; scan_kernel_ms = 0 and device_ms = the whole graph; with NB blocks in the parts, R
+ *     records, C present composite groups, F fields, A aggregations, N = pow2(max(R, 2048)) and align256(x) = x rounded up to 256,
+ *       kernel_launches = 1 (reset) + (NB > 0) (scan) + 8 + sum over s = 4096..N (s a power of two) of (log2(s) - 10)  (order)
+ *                         + (C > 0) * (1 (fold) + the finalisation's launches over C groups, or 2: rows and copy kernels),
+ *         i.e. the unprepared call's with discovery's five launches given way to the reset kernel (partial form: plus the copy
+ *         kernel; C = 0: less the fold);
+ *       d2h_bytes = finalised: the finalisation's read-back over C groups + 256 + 8*C   (rows, zero page, pairs: ONE copy)
+ *                   partial:   align256(8*C) + 256 + (8 + 8*F) + n_rows*(8 + 16*A)   (pairs, zero page, control word, rows)
+ *                   C = 0:     256                                                   (the zero page).
+ *   - Device memory a captured step keeps until bydb_query_release_keyed, or until the step is dropped; it is not charged to
+ *     hbm_budget_bytes.  With cap = max_values, NS series, S = pow2(max(2*cap, 1024)), M = pow2(max(2*R, 1024)), each term
+ *     rounded up to 256 B:
+ *       12*NS + 12*S + 68*cap + 8*NB + 32 + 4*(NB/1024 + 1)                             discovery's outputs (a copy)
+ *       + 56*C*F + 8*C + 8*F + 4*C                                                      the table of C groups, perm
+ *       + 256 + 12*M + 8 + R*(16 + 32*F) + 8*R + 12*N + 4*N/1024                        scan and order
+ *       + (finalised) the finalisation's scratch over C groups + 256 + 8*C,  or  (partial) 8*C + (8 + 8*F) + C*(8 + 16*A)
+ *     (C = 0: no finalisation or row image).  The handle's page-locked staging holds the read-back. */
+int bydb_query_prepare_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out);
+
 /* Prepared map-phase answers: what a data node answers, refresh after refresh, for a query the liaison pushes down with
  * agg_return_partial (a dashboard panel or an alert rule in a cluster).  The handles are those of the finalised forms above.
  *   - Answers: every execution returns what the unprepared form returns at that moment, for the handle's query.

@@ -114,6 +114,7 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed", "bydb_scan_partials_keyed", "bydb_keyed_partial_rows_free",
            "bydb_scan_reduce_keyed_partials", "bydb_scan_agg_keyed_wide", "bydb_scan_partials_keyed_wide",
            "bydb_keyed_wide_reduce_slot_bytes", "bydb_scan_reduce_keyed_wide", "bydb_scan_reduce_keyed_wide_partials",
+           "bydb_query_prepare_keyed_wide",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -158,6 +159,7 @@ def load_library():
     L.bydb_query_release.argtypes = [C.c_void_p, C.c_void_p]
     L.bydb_query_release.restype = None
     L.bydb_query_prepare_keyed.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(C.c_void_p)]
+    L.bydb_query_prepare_keyed_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKey), C.POINTER(C.c_void_p)]
     L.bydb_scan_agg_keyed_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_KeyedResult)]
     L.bydb_query_release_keyed.argtypes = [C.c_void_p, C.c_void_p]
     L.bydb_scan_partials_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_PartialRows), C.POINTER(_Stats)]
@@ -564,6 +566,17 @@ class Context:
         gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
         h = C.c_void_p()
         _check(self._L.bydb_query_prepare_keyed(self._h, C.byref(cq), C.byref(gk), C.byref(h)))
+        return KeyedGraphQuery(self, h, q)
+
+    def prepare_keyed_wide(self, q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> "KeyedGraphQuery":
+        """The prepared form of scan_agg_keyed_wide (bydb_query_prepare_keyed_wide), for up to 65,536 key values: argument errors
+        are raised here, as scan_agg_keyed_wide raises them; the handle's run() / run_partials() answer as scan_agg_keyed_wide /
+        scan_partials_keyed_wide do at that moment."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gk = _GroupKey(family.encode(), tag.encode(), max_values, value_type)
+        h = C.c_void_p()
+        _check(self._L.bydb_query_prepare_keyed_wide(self._h, C.byref(cq), C.byref(gk), C.byref(h)))
         return KeyedGraphQuery(self, h, q)
 
     def _read_keyed(self, q: Query, r: "_KeyedResult") -> Result:

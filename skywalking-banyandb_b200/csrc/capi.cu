@@ -2327,25 +2327,26 @@ int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *ta
     return 0;
 }
 
-// Steps 1-3 of the wide path, on the slot's stream, synchronised: discovery (w.values), the scan and the order (w.n_comp composite
-// groups).  w.rp then holds everything launch_wide_fold reads but its outputs (table, pairs, perm), and the scratch behind it stays
-// alive in `w`.  No value or no record: w.R = 0 and nothing past discovery ran.
+// The wide path's discovery and scan state.  wide_discover fills values, R, disc_bytes (the discovery scratch `ka`), wk and
+// series_group; wide_scan_order fills rp with everything launch_wide_fold reads but its outputs (table, pairs, perm); wide_pass
+// runs both and sets n_comp.  No value or no record: R = 0 and nothing past discovery ran.
 struct WidePass {
     KeyValues values;
-    size_t R = 0, n_comp = 0;
+    size_t R = 0, n_comp = 0, disc_bytes = 0;
     Scratch ka, sb;           // discovery | scan and order
     WideKeyParams wk;
+    const int32_t *series_group = nullptr;  // [NS] in ka
     WideReduceParams rp;
 };
-int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats &stats,
-              WidePass &w) {
+
+// 1. discovery, on the slot's stream, synchronised: the value table (S slots), each selected block's rank and distinct values,
+// then their exclusive scan (each block's first record; R their sum), and the values read back
+int wide_discover(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats &stats,
+                  WidePass &w) {
     cudaStream_t stream = slot.stream;
     const bool int64_key = key->value_type == BYDB_VT_INT64;
-    const size_t F = plan.fcols.size(), NS = q->n_series, NB = plan.total_blocks, NBp = align_up(std::max<size_t>(NB, 1), 1024);
-    cudaEvent_t *ev = slot.ev;
-    CUDA_TRY(cudaEventRecord(ev[0], stream));
-
-    // 1. discovery: the value table (S slots), each selected block's rank and distinct values, then their exclusive scan
+    const size_t NS = q->n_series, NB = plan.total_blocks, NBp = align_up(std::max<size_t>(NB, 1), 1024);
+    CUDA_TRY(cudaEventRecord(slot.ev[0], stream));
     const size_t S = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(cap), kKeySlots));
     Carve carve;
     const size_t a_sids = carve(NS * 8), a_grp = carve(NS * 4), a_slots = carve(S * 8), a_ctl = carve(32), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
@@ -2353,6 +2354,7 @@ int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uin
                  a_tiles = carve(NBp / 1024 * 4);
     Scratch &ka = w.ka;
     CUDA_TRY(ka.alloc(carve.o, stream));
+    w.disc_bytes = carve.o;
     if (slot.ensure_pinned(std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     WideKeyParams &wk = w.wk;
     memset(&wk, 0, sizeof wk);
@@ -2373,6 +2375,7 @@ int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uin
     wk.slot_id = reinterpret_cast<uint32_t *>(ka.base + a_sid);
     wk.n_by_rank = reinterpret_cast<uint32_t *>(ka.base + a_nbr);
     wk.rank = reinterpret_cast<uint32_t *>(ka.base + a_rank);
+    w.series_group = reinterpret_cast<const int32_t *>(ka.base + a_grp);
     launch_key_values_wide(wk, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
     launch_excl_scan(wk.n_by_rank, static_cast<uint32_t>(NBp), reinterpret_cast<uint32_t *>(ka.base + a_tiles), d_ctl + 4, stream);
     CUDA_TRY(cudaMemcpyAsync(slot.pinned, d_ctl, 32, cudaMemcpyDeviceToHost, stream));
@@ -2396,20 +2399,41 @@ int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uin
     if (V == 0 || R == 0) return 0;  // no block selected: no rows (n_rows = 0)
     if (R > 0x7fffffffull) return fail(BYDB_ENOMEM, "wide group-key query: too many (block, key value) records");
     w.R = R;
+    return 0;
+}
 
-    // 2. the scan: one record per present (block, key value)
-    const size_t rec_bytes = wide_record_bytes(F);
-    const size_t C = pow2_at_least(std::max<size_t>(2 * R, 1024)), N = pow2_at_least(std::max<size_t>(R, 2048));
+// The scratch of the scan and the order over R records of F fields.  The zero page, the composite table and ctl come first, so
+// that one range holds everything they need zeroed, and comp_min (preset to ones) lies right behind it.
+struct WideScanLayout {
+    size_t C, N, zero, comp, ctl, cmin, rec, rslot, keys, heads, tiles, seg, total;
+};
+WideScanLayout wide_scan_layout(size_t R, size_t F) {
+    WideScanLayout L;
+    L.C = pow2_at_least(std::max<size_t>(2 * R, 1024));
+    L.N = pow2_at_least(std::max<size_t>(R, 2048));
     Carve cb;
-    const size_t b_zero = cb(kZeroPageBytes), b_rec = cb(R * rec_bytes), b_comp = cb(C * 8), b_cmin = cb(C * 4), b_rslot = cb(R * 4), b_keys = cb(N * 8),
-                 b_heads = cb(N * 4), b_tiles = cb(N / 1024 * 4), b_ctl = cb(8), b_seg = cb(R * 4);
-    Scratch &sb = w.sb;
-    CUDA_TRY(sb.alloc(cb.o, stream));
-    ZeroPage *z = reinterpret_cast<ZeroPage *>(sb.base + b_zero);
-    CUDA_TRY(cudaMemsetAsync(z, 0, kZeroPageBytes, stream));
-    CUDA_TRY(cudaMemsetAsync(sb.base + b_comp, 0, C * 8, stream));
-    CUDA_TRY(cudaMemsetAsync(sb.base + b_cmin, 0xff, C * 4, stream));
-    CUDA_TRY(cudaMemsetAsync(sb.base + b_ctl, 0, 8, stream));
+    L.zero = cb(kZeroPageBytes);
+    L.comp = cb(L.C * 8);
+    L.ctl = cb(8);
+    L.cmin = cb(L.C * 4);
+    L.rec = cb(R * wide_record_bytes(F));
+    L.rslot = cb(R * 4);
+    L.keys = cb(L.N * 8);
+    L.heads = cb(L.N * 4);
+    L.tiles = cb(L.N / 1024 * 4);
+    L.seg = cb(R * 4);
+    L.total = cb.o;
+    return L;
+}
+
+// 2-3. The scan (one record per present (block, key value)) and the composite groups in insertion order, ENQUEUED on `stream` and
+// nothing else, into the scratch at sb (layout L) with its zero page, composite table and ctl zeroed and comp_min set to ones.
+// Reads discovery's outputs through w.wk and w.series_group; fills w.rp.  `ev` (may be NULL): two events around the scan kernel.
+// `launches` = the kernels launched.
+int wide_scan_order(bydb_ctx *ctx, const bydb_query *q, const Plan &plan, WidePass &w, uint8_t *sb, const WideScanLayout &L, cudaStream_t stream,
+                    cudaEvent_t *ev, uint32_t &launches) {
+    const KeyParams &kp = w.wk.k;
+    ZeroPage *z = reinterpret_cast<ZeroPage *>(sb + L.zero);
     ScanParams sp;
     scan_params_head(ctx, q, plan, kp.q_sids, sp);
     sp.err = z->err;
@@ -2418,50 +2442,69 @@ int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uin
     WideScanParams ws;
     memset(&ws, 0, sizeof ws);
     ws.slots = kp.slots;
-    ws.slot_id = wk.slot_id;
+    ws.slot_id = w.wk.slot_id;
     ws.zero = kp.zero;
-    ws.slot_mask = wk.slot_mask;
-    ws.int64_key = wk.int64_key;
+    ws.slot_mask = w.wk.slot_mask;
+    ws.int64_key = w.wk.int64_key;
     ws.key_name = kp.key_name;
-    ws.rank = wk.rank;
-    ws.rec_off = wk.n_by_rank;
-    ws.series_group = reinterpret_cast<const int32_t *>(ka.base + a_grp);
-    ws.records = sb.base + b_rec;
-    CUDA_TRY(cudaEventRecord(ev[1], stream));
+    ws.rank = w.wk.rank;
+    ws.rec_off = w.wk.n_by_rank;
+    ws.series_group = w.series_group;
+    ws.records = sb + L.rec;
+    if (ev) CUDA_TRY(cudaEventRecord(ev[1], stream));
     launch_scan_keyed_wide(sp, ws, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
-    CUDA_TRY(cudaEventRecord(ev[2], stream));
-
-    // 3. the composite groups in insertion order
+    if (ev) CUDA_TRY(cudaEventRecord(ev[2], stream));
     WideReduceParams &rp = w.rp;
     memset(&rp, 0, sizeof rp);
     rp.records = ws.records;
-    rp.n_records = static_cast<uint32_t>(R);
-    rp.n_fcols = static_cast<uint32_t>(F);
-    rp.comp = reinterpret_cast<unsigned long long *>(sb.base + b_comp);
-    rp.comp_min = reinterpret_cast<uint32_t *>(sb.base + b_cmin);
-    rp.rec_slot = reinterpret_cast<uint32_t *>(sb.base + b_rslot);
-    rp.comp_mask = static_cast<uint32_t>(C - 1);
-    rp.n_sort = static_cast<uint32_t>(N);
-    rp.keys = reinterpret_cast<unsigned long long *>(sb.base + b_keys);
-    rp.heads = reinterpret_cast<uint32_t *>(sb.base + b_heads);
-    rp.tile_sums = reinterpret_cast<uint32_t *>(sb.base + b_tiles);
-    rp.ctl = reinterpret_cast<uint32_t *>(sb.base + b_ctl);
-    rp.seg_start = reinterpret_cast<uint32_t *>(sb.base + b_seg);
+    rp.n_records = static_cast<uint32_t>(w.R);
+    rp.n_fcols = static_cast<uint32_t>(plan.fcols.size());
+    rp.comp = reinterpret_cast<unsigned long long *>(sb + L.comp);
+    rp.comp_min = reinterpret_cast<uint32_t *>(sb + L.cmin);
+    rp.rec_slot = reinterpret_cast<uint32_t *>(sb + L.rslot);
+    rp.comp_mask = static_cast<uint32_t>(L.C - 1);
+    rp.n_sort = static_cast<uint32_t>(L.N);
+    rp.keys = reinterpret_cast<unsigned long long *>(sb + L.keys);
+    rp.heads = reinterpret_cast<uint32_t *>(sb + L.heads);
+    rp.tile_sums = reinterpret_cast<uint32_t *>(sb + L.tiles);
+    rp.ctl = reinterpret_cast<uint32_t *>(sb + L.ctl);
+    rp.seg_start = reinterpret_cast<uint32_t *>(sb + L.seg);
     rp.col_type = z->col_type;
     rp.scan_err = z->err;
     launch_wide_order(rp, stream);
+    uint32_t sort_launches = 0;
+    for (size_t size = 4096; size <= L.N; size <<= 1) sort_launches += 1 + static_cast<uint32_t>(__builtin_ctzll(size) - 11);
+    launches = (plan.total_blocks ? 1u : 0u) + 2u + 1u + sort_launches + 1u + 3u + 1u;
+    return 0;
+}
+
+// Steps 1-3 of the wide path, on the slot's stream, synchronised: discovery (w.values), the scan and the order (w.n_comp composite
+// groups).  The scratch behind w.rp stays alive in `w`.
+int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats &stats,
+              WidePass &w) {
+    cudaStream_t stream = slot.stream;
+    int rc = wide_discover(ctx, q, key, cap, plan, slot, stats, w);
+    if (rc || w.R == 0) return rc;
+    const WideScanLayout L = wide_scan_layout(w.R, plan.fcols.size());
+    Scratch &sb = w.sb;
+    CUDA_TRY(sb.alloc(L.total, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + L.zero, 0, kZeroPageBytes, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + L.comp, 0, L.C * 8, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + L.cmin, 0xff, L.C * 4, stream));
+    CUDA_TRY(cudaMemsetAsync(sb.base + L.ctl, 0, 8, stream));
+    uint32_t launches = 0;
+    rc = wide_scan_order(ctx, q, plan, w, sb.base, L, stream, slot.ev, launches);
+    if (rc) return rc;
     ZeroPage *hz = slot.page(0);
-    CUDA_TRY(cudaMemcpyAsync(hz, z, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, rp.ctl, 8, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(hz, sb.base + L.zero, kZeroPageBytes, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, w.rp.ctl, 8, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     CUDA_TRY(cudaGetLastError());
-    uint32_t sort_launches = 0;
-    for (size_t size = 4096; size <= N; size <<= 1) sort_launches += 1 + static_cast<uint32_t>(__builtin_ctzll(size) - 11);
-    stats.kernel_launches += (NB ? 1u : 0u) + 2u + 1u + sort_launches + 1u + 3u + 1u;
+    stats.kernel_launches += launches;
     stats.d2h_bytes += kZeroPageBytes + 8;
     {
         float ms = 0;
-        cudaEventElapsedTime(&ms, ev[1], ev[2]);
+        cudaEventElapsedTime(&ms, slot.ev[1], slot.ev[2]);
         stats.scan_kernel_ms += ms;
     }
     rc = read_zero_page(*hz, false, &stats);
@@ -2530,6 +2573,8 @@ struct bydb_prepared_keyed {
     uint32_t cap = 0;              // distinct values accepted (check_group_key)
     KeyValues values;              // found when the step was captured: the key table of every replay
     size_t pairs_off = 0, zero_off = 0;  // in the replay's read-back image: the rows' (group, key) pairs, the passes' zero pages
+    bool wide = false;             // bydb_query_prepare_keyed_wide: one scan pass (wide_capture), not one per value
+    size_t n_comp = 0;             // wide: C, the present composite groups found when the step was captured
     ~bydb_prepared_keyed() { prepared_destroy(pq); }
 };
 
@@ -2690,6 +2735,156 @@ int keyed_answer(bydb_prepared_keyed *k, const Plan &shape, const uint8_t *image
     return 0;
 }
 
+// Captures the wide keyed step into k->pq->exec.  Outside the graph, once: the plain path's discovery, scan and order (wide_pass)
+// find the key table, R and C -- functions of the parts the handles name and of the fixed query, so properties of the capture.
+// Then one step state, allocated once and laid out as
+//   discovery's scratch, copied from the eager run (value table, slot ids, ranks, first records, series ids and groups) |
+//   the table of the C composite groups | perm | (partial) their (group, key) pairs | the scan and order's scratch, zero page first |
+//   the tail: the finalisation over C groups with the zero page gathered behind it and the pairs behind that, or the row image,
+// and the graph: keyed_step_reset_kernel (zero page, composite table, ctl; comp_min) -> wide_scan_order -> wide_fold_kernel -> the
+// finalisation and ONE copy of rows, zero page and pairs; or keyed_partial_rows_kernel and rows_to_host_kernel bringing the pairs,
+// the zero page (one range), the control word and the C rows.  C = 0: the graph ends with a copy of the zero page.
+// Leaves neither a graph nor p->empty_step when this execution, or (capturable cleared) every later one, takes the plain path.
+void wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
+    bydb_prepared *p = k->pq;
+    const bydb_query *q = &p->q;
+    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up
+    Plan plan;
+    if (make_plan(ctx, q, nullptr, plan)) return;
+    ExecSlot &slot = *p->slot;
+    cudaStream_t stream = slot.stream;
+    bydb_stats eager{};
+    WidePass w;
+    if (parts_overlap(plan.parts, q->tmin, q->tmax) || wide_pass(ctx, q, &k->key, k->cap, plan, slot, eager, w)) {
+        p->capturable = false;
+        return;
+    }
+    if (w.R == 0) {
+        k->values = std::move(w.values);
+        p->empty_step = true;
+        p->held = plan.parts;
+        p->held_gen = gen;
+        return;
+    }
+    const size_t F = plan.fcols.size(), A = q->n_aggs, C = w.n_comp;
+    const size_t ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
+    const WideScanLayout L = wide_scan_layout(w.R, F);
+    const TableLayout tl(std::max<size_t>(C, 1), F);
+    const FinalLayout fl = final_layout(C, A, q->top_n);
+    Carve carve;
+    const size_t o_disc = carve(w.disc_bytes), o_table = carve(tl.total), o_perm = carve(C * 4), o_pairs = carve(partial ? C * 8 : 0),
+                 o_scan = carve(L.total), o_tail = carve(C == 0 ? 0 : partial ? ctl_bytes + C * row_bytes : fl.total + kZeroPageBytes + C * 8);
+    const size_t pages = o_scan + L.zero + kZeroPageBytes - o_pairs;  // partial: the pairs, padded, then the zero page
+    p->host_off = 0;  // the staging serves only the read-back: discovery's outputs stay on the device
+    p->read_back = C == 0 ? kZeroPageBytes : partial ? pages + ctl_bytes + C * row_bytes : fl.out_bytes + kZeroPageBytes + C * 8;
+    uint8_t *h_dst = slot.ensure_pinned(p->read_back) ? nullptr : slot.pinned_dev(0);
+    if (!h_dst || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
+        cudaGetLastError();
+        p->step_state = nullptr;
+        p->capturable = false;
+        return;
+    }
+    uint8_t *S = p->step_state, *sb = S + o_scan, *tail = S + o_tail;
+    cudaError_t e = cudaMemcpyAsync(S + o_disc, w.ka.base, w.disc_bytes, cudaMemcpyDeviceToDevice, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    // discovery's device pointers, moved to the copy
+    auto moved = [&](auto *ptr) { return reinterpret_cast<decltype(ptr)>(S + o_disc + (reinterpret_cast<const uint8_t *>(ptr) - w.ka.base)); };
+    KeyParams &kp = w.wk.k;
+    kp.q_sids = moved(kp.q_sids);
+    kp.slots = moved(kp.slots);
+    kp.zero = moved(kp.zero);
+    w.wk.slot_id = moved(w.wk.slot_id);
+    w.wk.rank = moved(w.wk.rank);
+    w.wk.n_by_rank = moved(w.wk.n_by_rank);
+    w.series_group = moved(w.series_group);
+    bydb_stats &cs = p->captured;
+    GraphCapture c;
+    if (e == cudaSuccess) c = capture_graph(stream, &p->exec, [&]() -> int {
+        memset(&cs, 0, sizeof cs);
+        KeyedResetParams rs;
+        memset(&rs, 0, sizeof rs);
+        rs.zero[0] = reinterpret_cast<uint32_t *>(sb + L.zero);
+        rs.n_zero[0] = (L.ctl + 8 - L.zero) / 4;
+        rs.ones[0] = reinterpret_cast<uint32_t *>(sb + L.cmin);
+        rs.n_ones[0] = L.C;
+        launch_keyed_step_reset(rs, stream);
+        uint32_t launches = 0;
+        int rc = wide_scan_order(ctx, q, plan, w, sb, L, stream, nullptr, launches);
+        cs.kernel_launches += 1 + launches;
+        if (rc) return rc;
+        if (C == 0) return cudaMemcpyAsync(slot.pinned, sb + L.zero, kZeroPageBytes, cudaMemcpyDeviceToHost, stream) == cudaSuccess ? 0 : BYDB_EIO;
+        WideReduceParams &rp = w.rp;
+        rp.table = tl.at(S + o_table);
+        rp.perm = reinterpret_cast<int32_t *>(S + o_perm);
+        rp.pairs = reinterpret_cast<int32_t *>(partial ? S + o_pairs : tail + fl.total + kZeroPageBytes);
+        launch_wide_fold(rp, static_cast<uint32_t>(C), stream);
+        cs.kernel_launches += 1;
+        Plan planc = plan;
+        planc.n_groups = static_cast<int32_t>(C);
+        if (partial) {
+            launch_keyed_partial_rows(rows_params(q, planc, 1, rp.table, rp.table.coltype, rp.perm, &rp.ctl[1], tail), C, stream);
+            RowsCopyParams cp;
+            memset(&cp, 0, sizeof cp);
+            cp.pages = S + o_pairs;
+            cp.image = tail;
+            cp.dst = h_dst;
+            cp.page_bytes = pages;
+            cp.ctl_bytes = ctl_bytes;
+            cp.row_bytes = row_bytes;
+            cp.max_rows = static_cast<uint32_t>(C);
+            launch_rows_to_host(cp, stream);
+            cs.kernel_launches += 2;
+            return 0;
+        }
+        Scratch fin;
+        fin.view(tail, fl.total + kZeroPageBytes);
+        FinalLayout flc;
+        uint32_t fin_launches = 0;
+        size_t fin_back = 0;
+        rc = finalize_launch(q, planc, stream, S + o_table, tl, fin, flc, fin_launches, fin_back, sb + L.zero);
+        cs.kernel_launches += fin_launches;
+        if (!rc && cudaMemcpyAsync(slot.pinned, tail + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+        return rc;
+    });
+    if (e != cudaSuccess || c.rc || c.err != cudaSuccess || !p->exec) {
+        cudaGetLastError();
+        drop_step(p);
+        p->capturable = false;
+        return;
+    }
+    // a partial step's read-back is sized by the rows present: the replay counts it
+    cs.d2h_bytes = partial && C ? 0 : p->read_back;
+    p->partial_step = partial;
+    p->fl = fl;
+    p->express = false;  // the wide scan has a lane of its own
+    k->values = std::move(w.values);
+    k->n_comp = C;
+    k->pairs_off = partial ? 0 : fl.out_bytes + kZeroPageBytes;
+    k->zero_off = C == 0 ? 0 : partial ? pages - kZeroPageBytes : fl.out_bytes;
+    p->held = plan.parts;
+    p->held_gen = gen;
+}
+
+// the answer of a replayed wide step from its read-back `image`: the finalised rows, or the row image behind the pairs and the zero
+// page (and the bytes the copy kernel brought back); either way each row's (group, key) pair by its composite group's position
+int wide_answer(bydb_prepared_keyed *k, const Plan &, const uint8_t *image, bydb_keyed_result *out, KeyedOwner *owner) {
+    if (k->n_comp == 0) return 0;
+    const int rc = finalize_parse(image, k->pq->fl, true, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, static_cast<ResultOwner *>(out->base.owner)->group_id, image + k->pairs_off, 8, true);
+    return 0;
+}
+int wide_answer(bydb_prepared_keyed *k, const Plan &shape, const uint8_t *image, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+    if (k->n_comp == 0) return 0;
+    const uint8_t *rows = image + k->zero_off + kZeroPageBytes;
+    const size_t ctl_bytes = keyed_ctl_bytes(shape.fcols.size()), row_bytes = keyed_row_bytes(k->pq->q.n_aggs);
+    out->stats.d2h_bytes += k->zero_off + kZeroPageBytes + ctl_bytes + rows_in(rows, k->n_comp) * row_bytes;
+    const int rc = parse_rows(rows, &k->pq->q, shape, k->n_comp, &out->base);
+    if (rc) return rc;
+    set_row_keys(out, owner, static_cast<PartialRowsOwner *>(out->base.owner)->group_id, image + k->pairs_off, 8, true);
+    return 0;
+}
+
 // One replay, synchronised and parsed: the passes' counters add up and the first pass with a device error decides, as the plain
 // path's pass-by-pass collection has it; then the answer of the step's form (keyed_answer).
 template <class Out>
@@ -2699,18 +2894,43 @@ int keyed_replay(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
     int rc = query_shape(&p->q, shape);
     if (rc) return rc;
     uint8_t *image = p->slot->pinned + p->host_off;
-    const size_t V = k->values.size();
+    const size_t V = k->wide ? 1 : k->values.size();  // zero pages: one per pass
+    const bool row_image = p->partial_step && (!k->wide || k->n_comp);
     // a replay that fails to launch cannot report the previous one's status (nor, in a partial step, its control word)
-    memset(image + k->zero_off, 0, V * kZeroPageBytes + (p->partial_step ? keyed_ctl_bytes(shape.fcols.size()) : 0));
+    memset(image + k->zero_off, 0, V * kZeroPageBytes + (row_image ? keyed_ctl_bytes(shape.fcols.size()) : 0));
     auto page = [&](size_t v) -> const ZeroPage & { return *reinterpret_cast<const ZeroPage *>(image + k->zero_off + v * kZeroPageBytes); };
     bydb_stats &stats = keyed_stats(out);
     rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, false, page(0), &stats);
     for (size_t v = 1; !rc && v < V; ++v) rc = read_zero_page(page(v), false, &stats);
     if (rc) return rc;
     KeyedAnswer<Out> answer(ctx, out, k->values);
-    rc = keyed_answer(k, shape, image, out, answer.owner);
+    rc = k->wide ? wide_answer(k, shape, image, out, answer.owner) : keyed_answer(k, shape, image, out, answer.owner);
     if (rc) return rc;
     answer.done = true;
+    return 0;
+}
+
+// bydb_query_prepare_keyed (wide: bydb_query_prepare_keyed_wide): the argument checks of the unprepared call, in its order, then
+// the handle with its copies of the query and the key
+int prepare_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bool wide, bydb_prepared_keyed **out) {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    *out = nullptr;
+    int rc = validate_query(q, true);
+    if (rc) return rc;
+    uint32_t cap = 0;
+    rc = check_group_key(q, key, wide ? kMaxWideKeyValues : kMaxKeyValues, !wide, cap);
+    if (rc) return rc;
+    std::unique_ptr<bydb_prepared_keyed> k(new bydb_prepared_keyed());
+    rc = bydb_query_prepare(ctx, q, &k->pq);
+    if (rc) return rc;
+    k->family = key->family;
+    k->tag = key->tag;
+    k->key = *key;
+    k->key.family = k->family.c_str();
+    k->key.tag = k->tag.c_str();
+    k->cap = cap;
+    k->wide = wide;
+    *out = k.release();
     return 0;
 }
 
@@ -2725,13 +2945,14 @@ int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
     g_last_dev_err = 0;
     CUDA_TRY(cudaSetDevice(ctx->device));
     const int rc = prepared_step(ctx, p, partial, [&] {
-        keyed_capture(ctx, k, partial);
+        if (k->wide) wide_capture(ctx, k, partial);
+        else keyed_capture(ctx, k, partial);
         return 0;
     });
     if (rc) return rc;
-    if (!p->exec && !p->empty_step) return scan_keyed_impl(ctx, &p->q, &k->key, out);
+    if (!p->exec && !p->empty_step) return k->wide ? scan_keyed_wide_impl(ctx, &p->q, &k->key, out) : scan_keyed_impl(ctx, &p->q, &k->key, out);
     if (p->empty_step) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
-        KeyedAnswer<Out> answer(ctx, out, KeyValues());
+        KeyedAnswer<Out> answer(ctx, out, k->values);
         answer.done = true;
         return 0;
     }
@@ -3004,27 +3225,11 @@ void bydb_keyed_result_free(bydb_ctx *ctx, bydb_keyed_result *r) {
 
 
 int bydb_query_prepare_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out) {
-    return guarded([&]() -> int {
-    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
-    *out = nullptr;
-    // the argument checks of bydb_scan_agg_keyed, in its order
-    int rc = validate_query(q, true);
-    if (rc) return rc;
-    uint32_t cap = 0;
-    rc = check_group_key(q, key, kMaxKeyValues, true, cap);
-    if (rc) return rc;
-    std::unique_ptr<bydb_prepared_keyed> k(new bydb_prepared_keyed());
-    rc = bydb_query_prepare(ctx, q, &k->pq);
-    if (rc) return rc;
-    k->family = key->family;
-    k->tag = key->tag;
-    k->key = *key;
-    k->key.family = k->family.c_str();
-    k->key.tag = k->tag.c_str();
-    k->cap = cap;
-    *out = k.release();
-    return 0;
-    });
+    return guarded([&]() -> int { return prepare_keyed_impl(ctx, q, key, false, out); });
+}
+
+int bydb_query_prepare_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out) {
+    return guarded([&]() -> int { return prepare_keyed_impl(ctx, q, key, true, out); });
 }
 
 void bydb_query_release_keyed(bydb_ctx *ctx, bydb_prepared_keyed *k) {
