@@ -433,9 +433,13 @@ void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r);
  *     BYDB_ENOTSUP).  An int64 key takes every page kind bydb_scan_agg_keyed takes; a block whose key column holds more than 256
  *     distinct values gives BYDB_ENOTSUP, the message naming the block.  A key of the wrong type gives BYDB_EINVAL, parts that
  *     overlap in time BYDB_ENOTSUP.  Up to 8 predicates (the key takes no predicate slot); block size and Top-N as bydb_scan_agg.
- *   - Numbers: counts, int64 values and min / max bit-exact; float sums within 1e-9 relative of the reference and bit-identical
- *     from call to call (the records of a group are folded in scan order by a fixed tree), though not necessarily bit-identical
- *     with bydb_scan_agg_keyed, whose passes fold zero partials for the blocks without the value.
+ *   - Numbers: counts, int64 values and min / max bit-exact; float sums within 1e-9 x (sum of |x| over the group's values) +
+ *     1e-9 x |reference| of the reference, and bit-identical from call to call (the records of a group are folded in scan order
+ *     by a fixed tree), though not necessarily bit-identical with bydb_scan_agg_keyed, whose passes fold zero partials for the
+ *     blocks without the value.  A decimal page's block sum is exact in the integer domain and rounded once, where the reference
+ *     adds the page's doubles in row order, so no bound relative to the reference alone holds where values cancel: 0.1, 0.2 and
+ *     -0.3 in one block sum to 0 here and to 5.55e-17 there.  bydb_scan_agg_keyed and the express lane of bydb_scan_agg sum
+ *     decimal pages the same way and give the same 0.
  *   - Stats (one pass): rows_scanned, blocks_scanned and rows_matched are what bydb_scan_agg reports for the same query without
  *     the key; page_bytes counts every page read once (the key page included).  With cap = max_values, V key values found,
  *     R = sum over the selected blocks of the block's distinct key values, C the composite groups with rows > 0, F distinct
@@ -599,7 +603,8 @@ int bydb_scan_reduce_keyed_partials(bydb_ctx *ctx, const bydb_query *q, const by
  *   - The root's answer is what bydb_scan_agg_keyed_wide (bydb_scan_partials_keyed_wide) answers over all ranks' parts: rows in
  *     the insertion order of the whole scan, or Top-N order with ties to the group inserted first; n_keys = the distinct values
  *     over all ranks' selected blocks; key bytes, nil rules, typing, BYDB_Q_ROW_PATH_TYPES and the sentinels as there.  Counts,
- *     int64 values and min / max are exact, float sums within 1e-9 relative and bit-identical from call to call.  The order of
+ *     int64 values and min / max are exact, float sums within bydb_scan_agg_keyed_wide's bound (1e-9 x the sum of |x| over the
+ *     group's values + 1e-9 x |reference|) and bit-identical from call to call.  The order of
  *     the key table is not part of the contract.  Non-root ranks get n_rows = 0, n_keys = 0 and their own stats.
  *   - Caps and refusals: max_values 0 means 64, 1..65,536 are accepted, above gives BYDB_EINVAL.  More distinct values over all
  *     ranks than max_values gives BYDB_ENOMEM at the root, even when every rank alone is under the cap.  A block with more than
