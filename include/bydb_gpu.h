@@ -459,6 +459,74 @@ void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r);
 int bydb_scan_agg_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_result *out);
 int bydb_scan_partials_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out);
 
+/* Group-by on a TUPLE of 2..4 stored tags in one scan pass ("latency by endpoint and status code"): the reference's computeKey
+ * concatenates one key component per GroupBy tag (aggregation.go:328-337, groupby.go:226-254), so two rows share a group only when
+ * every component is equal.  One stored key is bydb_scan_agg_keyed_wide; this is its answer with the key tuple in place of the key.
+ *   - Answer: that of bydb_scan_agg_keyed_wide / bydb_scan_partials_keyed_wide word for word, with a composite group = (series
+ *     group, key tuple): rows in insertion order or Top-N rank order (ties to the group inserted first), MEAN quirks,
+ *     BYDB_Q_ROW_PATH_TYPES, sentinels, the partial form's wire rule, the float bound and call-to-call bit identity as there.  Each
+ *     component follows the one-key rules: a string nil is "", an int64 nil or a block without the column is 0.  String and int64
+ *     tags mix freely.
+ *   - Keys: one table per tag.  Tag t's values are entries key_base[t] .. key_base[t+1]-1 (entry e is key_bytes[key_off[e] ..
+ *     key_off[e+1]), a string's bytes or an int64's 8 little-endian bytes), in no promised order; tag t of row r is entry
+ *     key_id[r * n_tags + t].  n_tuples counts the distinct tuples over all rows of the selected blocks, before the time trim and
+ *     the predicates (some may have no row), and key_base[t+1] - key_base[t] counts tag t's distinct values on the same terms.
+ *   - Refusals: n_keys outside 2..4, the same (family, tag) twice, a key whose own max_values is not 0, max_values above 65,536,
+ *     or a key failing bydb_scan_agg_keyed_wide's checks: BYDB_EINVAL.  More distinct tuples than max_values (0 = 64): BYDB_ENOMEM,
+ *     even when every tag alone is under it.  A block holding more than 256 distinct tuples: BYDB_ENOTSUP, the message naming the
+ *     block (the block-local index is one byte).  Per tag the one-key rules and codes hold: a plain string page or a 65-byte value
+ *     BYDB_ENOTSUP, a wrong type BYDB_EINVAL, an int64 column with more than 256 values in a block BYDB_ENOTSUP.  Parts that
+ *     overlap in time: BYDB_ENOTSUP.  Up to 8 predicates; the keys take no predicate slot.
+ *   - Stats (one pass): rows_scanned, rows_matched and blocks_scanned are those of bydb_scan_agg for the same query without keys;
+ *     page_bytes counts every page read once (every key page included).  With K tags, V_t tag t's distinct values, T = n_tuples,
+ *     R = sum over the selected blocks of the block's distinct tuples, C the composite groups with rows > 0, F fields, A
+ *     aggregations, NB blocks of the parts:
+ *       kernel_launches = (K + 1) * ((NB > 0) + 1) + 3          discovery: a value kernel and a numbering kernel per table, the scan of R
+ *                         (R = 0: that only), then what bydb_scan_agg_keyed_wide launches after its discovery for the same R and C
+ *       d2h_bytes = 32 * (K + 1) + sum_t V_t * (64 + 4 for a string tag, 8 for an int64 tag) + 8 * T     the discovery read-back
+ *                 + 256 + 8                                                     the scan's status / counter page, C
+ *                 + the finalisation read-back of bydb_scan_agg over C groups   (bydb_scan_agg_keys_wide)
+ *                   or 8 + 8 * F + C * (8 + 16 * A)                             (bydb_scan_partials_keys_wide: control word, rows)
+ *                 + 8 * C                                                       each composite group's (series group, tuple)
+ *     (R = 0: the first term only), and the device scratch of one call is, with cap = max_values and S = pow2(max(2 * cap, 1024)),
+ *     up to 256-byte alignment of each region,
+ *       12 * NS + K * (12 * S + 68 * cap) + 12 * S + 8 * cap + 8 * NB                                     discovery
+ *     + then bydb_scan_agg_keyed_wide's scan, order, composite table and finalisation terms for this R and C.
+ * Free the answers with bydb_keys_result_free / bydb_keys_partial_rows_free.  No prepared, multi-GPU or host-image form. */
+typedef struct {
+    uint32_t n_keys;              /* 2..4 stored GroupBy tags, in the request's GroupBy order                               */
+    uint32_t max_values;          /* distinct key TUPLES accepted over the query; 0 = 64, at most 65,536                    */
+    const bydb_group_key *keys;   /* [n_keys] family, tag, value_type as bydb_group_key; each .max_values must be 0         */
+} bydb_group_keys;
+
+typedef struct {
+    bydb_result base;             /* rows as in bydb_result; base.group_id[r] = series_group of row r                       */
+    uint32_t n_tags;              /* = n_keys                                                                                */
+    int32_t n_tuples;             /* distinct key tuples in the selected blocks (some may have no row)                      */
+    const int32_t *key_id;        /* [base.n_rows * n_tags]: tag t of row r is entry key_id[r * n_tags + t]                 */
+    const int32_t *key_base;      /* [n_tags + 1]: tag t's values are entries key_base[t] .. key_base[t+1]-1                */
+    const uint32_t *key_off;      /* [key_base[n_tags] + 1]: entry e is key_bytes[key_off[e] .. key_off[e+1])               */
+    const uint8_t *key_bytes;
+    void *owner;                  /* private                                                                                 */
+} bydb_keys_result;
+
+typedef struct {
+    bydb_partial_rows base;       /* rows as bydb_partials_rows: base.group_id[r] = series_group of row r                   */
+    uint32_t n_tags;              /* as bydb_keys_result                                                                     */
+    int32_t n_tuples;
+    const int32_t *key_id;
+    const int32_t *key_base;
+    const uint32_t *key_off;
+    const uint8_t *key_bytes;
+    bydb_stats stats;             /* as bydb_keys_result.base.stats                                                          */
+    void *owner;                  /* private                                                                                 */
+} bydb_keys_partial_rows;
+
+int bydb_scan_agg_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, bydb_keys_result *out);
+int bydb_scan_partials_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, bydb_keys_partial_rows *out);
+void bydb_keys_result_free(bydb_ctx *ctx, bydb_keys_result *r);
+void bydb_keys_partial_rows_free(bydb_ctx *ctx, bydb_keys_partial_rows *r);
+
 /* Prepared wide group-by on a stored tag: bydb_scan_agg_keyed_wide for a query executed many times (a dashboard panel grouped by
  * endpoint, instance or status code).  The handle is a bydb_prepared_keyed: bydb_scan_agg_keyed_prepared,
  * bydb_scan_partials_keyed_prepared and bydb_query_release_keyed take it, and on it answer what bydb_scan_agg_keyed_wide /

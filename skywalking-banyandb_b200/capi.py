@@ -78,6 +78,16 @@ class _KeyedResult(C.Structure):
                 ("key_off", C.POINTER(C.c_uint32)), ("key_bytes", C.POINTER(C.c_uint8)), ("owner", C.c_void_p)]
 
 
+class _GroupKeys(C.Structure):
+    _fields_ = [("n_keys", C.c_uint32), ("max_values", C.c_uint32), ("keys", C.POINTER(_GroupKey))]
+
+
+class _KeysResult(C.Structure):
+    _fields_ = [("base", _Result), ("n_tags", C.c_uint32), ("n_tuples", C.c_int32), ("key_id", C.POINTER(C.c_int32)),
+                ("key_base", C.POINTER(C.c_int32)), ("key_off", C.POINTER(C.c_uint32)), ("key_bytes", C.POINTER(C.c_uint8)),
+                ("owner", C.c_void_p)]
+
+
 class _EncodeInput(C.Structure):
     _fields_ = [("value_type", C.c_int32), ("n_blocks", C.c_uint32), ("block_rows", C.c_void_p), ("values", C.c_void_p)]
 
@@ -98,6 +108,12 @@ class _KeyedPartialRows(C.Structure):
                 ("key_off", C.POINTER(C.c_uint32)), ("key_bytes", C.POINTER(C.c_uint8)), ("stats", _Stats), ("owner", C.c_void_p)]
 
 
+class _KeysPartialRows(C.Structure):
+    _fields_ = [("base", _PartialRows), ("n_tags", C.c_uint32), ("n_tuples", C.c_int32), ("key_id", C.POINTER(C.c_int32)),
+                ("key_base", C.POINTER(C.c_int32)), ("key_off", C.POINTER(C.c_uint32)), ("key_bytes", C.POINTER(C.c_uint8)),
+                ("stats", _Stats), ("owner", C.c_void_p)]
+
+
 class _Layout(C.Structure):
     _fields_ = [("total_bytes", C.c_uint64), ("off_sum_f64", C.c_uint64), ("off_max_f64", C.c_uint64),
                 ("off_sum_i64", C.c_uint64), ("off_max_i64", C.c_uint64), ("n_sum_f64", C.c_uint64),
@@ -114,7 +130,8 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_keyed_reduce_slot_bytes", "bydb_scan_reduce_keyed", "bydb_scan_partials_keyed", "bydb_keyed_partial_rows_free",
            "bydb_scan_reduce_keyed_partials", "bydb_scan_agg_keyed_wide", "bydb_scan_partials_keyed_wide",
            "bydb_keyed_wide_reduce_slot_bytes", "bydb_scan_reduce_keyed_wide", "bydb_scan_reduce_keyed_wide_partials",
-           "bydb_query_prepare_keyed_wide",
+           "bydb_query_prepare_keyed_wide", "bydb_scan_agg_keys_wide", "bydb_scan_partials_keys_wide", "bydb_keys_result_free",
+           "bydb_keys_partial_rows_free",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -189,6 +206,12 @@ def load_library():
                                                        C.POINTER(_KeyedPartialRows)]
     L.bydb_keyed_partial_rows_free.argtypes = [C.c_void_p, C.POINTER(_KeyedPartialRows)]
     L.bydb_keyed_partial_rows_free.restype = None
+    L.bydb_scan_agg_keys_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKeys), C.POINTER(_KeysResult)]
+    L.bydb_scan_partials_keys_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKeys), C.POINTER(_KeysPartialRows)]
+    L.bydb_keys_result_free.argtypes = [C.c_void_p, C.POINTER(_KeysResult)]
+    L.bydb_keys_result_free.restype = None
+    L.bydb_keys_partial_rows_free.argtypes = [C.c_void_p, C.POINTER(_KeysPartialRows)]
+    L.bydb_keys_partial_rows_free.restype = None
     _lib = L
     return L
 
@@ -470,6 +493,28 @@ def keyed_wide_reduce_slot_bytes(q: Query, family: str, tag: str, max_values: in
     return out.value
 
 
+def _group_keys(keys: Sequence[tuple], max_values: int, keep: list) -> "_GroupKeys":
+    arr = (_GroupKey * max(len(keys), 1))()
+    for i, (family, tag, value_type) in enumerate(keys):
+        fb, tb = family.encode(), tag.encode()
+        keep += [fb, tb]
+        arr[i] = _GroupKey(fb, tb, 0, value_type)
+    keep.append(arr)
+    return _GroupKeys(len(keys), max_values, arr)
+
+
+def _read_tuples(r, n_rows: int):
+    """-> (each tag's values, each row's tuple of key bytes) of a bydb_keys_result / bydb_keys_partial_rows"""
+    k = r.n_tags
+    if k == 0:
+        return [], []
+    base = [r.key_base[t] for t in range(k + 1)]
+    entries = [bytes(r.key_bytes[r.key_off[e]:r.key_off[e + 1]]) for e in range(base[k])]
+    tables = [entries[base[t]:base[t + 1]] for t in range(k)]
+    ids = _arr(r.key_id, n_rows * k, np.int32).tolist()
+    return tables, [tuple(entries[e] for e in ids[i * k:(i + 1) * k]) for i in range(n_rows)]
+
+
 class Context:
     """bydb_ctx: one device, its streams and the HBM part cache."""
 
@@ -593,6 +638,45 @@ class Context:
             return res
         finally:
             self._L.bydb_keyed_result_free(self._h, C.byref(r))
+
+    def scan_agg_keys_wide(self, q: Query, keys: Sequence[tuple], max_values: int = 0) -> Result:
+        """Group-by on a tuple of 2..4 stored tags in one scan pass (bydb_scan_agg_keys_wide).  keys: (family, tag, value_type)
+        per GroupBy tag, value_type as in scan_agg_keyed.  Each row's `key` is a tuple of the tags' key bytes; `n_tuples` counts
+        the distinct tuples of the selected blocks and `key_tables` holds each tag's values."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gks = _group_keys(keys, max_values, keep)
+        r = _KeysResult()
+        _check(self._L.bydb_scan_agg_keys_wide(self._h, C.byref(cq), C.byref(gks), C.byref(r)))
+        try:
+            if r.base.n_rows == 0 and not r.base.owner:
+                a = len(q.aggs)
+                res = Result(np.zeros(0, np.int32), np.zeros(0, np.int64), np.zeros(a, bool), np.zeros((0, a), np.int64),
+                             np.zeros((0, a), np.float64), Stats.of(r.base.stats))
+            else:
+                res = _read_result(r.base)
+            res.key_tables, res.key = _read_tuples(r, r.base.n_rows)
+            res.n_tuples = r.n_tuples
+            return res
+        finally:
+            self._L.bydb_keys_result_free(self._h, C.byref(r))
+
+    def scan_partials_keys_wide(self, q: Query, keys: Sequence[tuple], max_values: int = 0) -> Dict[str, object]:
+        """Map-phase rows of a tuple group-by (bydb_scan_partials_keys_wide): the arrays of partials_rows plus `key` (a tuple of
+        key bytes per row), `n_tuples`, `key_tables` and `stats`."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gks = _group_keys(keys, max_values, keep)
+        r = _KeysPartialRows()
+        _check(self._L.bydb_scan_partials_keys_wide(self._h, C.byref(cq), C.byref(gks), C.byref(r)))
+        try:
+            out = _read_partial_rows(r.base, len(q.aggs))
+            out["key_tables"], out["key"] = _read_tuples(r, r.base.n_rows)
+            out["n_tuples"] = r.n_tuples
+            out["stats"] = Stats.of(r.stats)
+            return out
+        finally:
+            self._L.bydb_keys_partial_rows_free(self._h, C.byref(r))
 
     def encode_pages(self, values: np.ndarray, block_rows: Sequence[int]):
         """Write side (bydb_encode_pages): int64 / float64 value blocks -> ([page bytes or None per block], device ms).

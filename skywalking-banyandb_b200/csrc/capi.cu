@@ -373,6 +373,7 @@ const char *dev_err_text(uint32_t code) {
         case kErrKeyLong: return "per-row group key: a key value longer than 64 bytes";
         case kErrRankOverlap: return "keyed collective: a series lives on several ranks over time spans that intersect";
         case kErrKeyBlock: return "wide group key: a block whose int64 key column holds more than 256 distinct values";
+        case kErrTupleBlock: return "tuple group key: a block holding more than 256 distinct key tuples";
     }
     return "unknown device error";
 }
@@ -1813,6 +1814,7 @@ struct KeyedOwner {
     std::vector<int32_t> key_id;
     std::vector<uint32_t> key_off;
     std::vector<uint8_t> key_bytes;
+    std::vector<int32_t> key_base;  // a tuple key: where each tag's entries start
 };
 
 // the arrays of a bydb_partial_rows
@@ -1901,6 +1903,8 @@ int partial_rows_to_host(const bydb_query *q, const Plan &plan, ExecSlot &slot, 
 // the two answers of a keyed call: finalised rows (bydb_keyed_result) or map-phase partial rows (bydb_keyed_partial_rows)
 bydb_stats &keyed_stats(bydb_keyed_result *out) { return out->base.stats; }
 bydb_stats &keyed_stats(bydb_keyed_partial_rows *out) { return out->stats; }
+bydb_stats &keyed_stats(bydb_keys_result *out) { return out->base.stats; }
+bydb_stats &keyed_stats(bydb_keys_partial_rows *out) { return out->stats; }
 using KeyValues = std::vector<std::vector<uint8_t>>;
 
 // the checks of a group key that need no device; cap = the distinct values accepted (max_values, 0 = 64), at most max_cap.  A key
@@ -1912,6 +1916,25 @@ int check_group_key(const bydb_query *q, const bydb_group_key *key, uint32_t max
     cap = key->max_values ? key->max_values : 64u;
     if (cap > max_cap) return fail(BYDB_EINVAL, "bydb_group_key.max_values above " + std::to_string(max_cap));
     if (pred_slot && q->n_preds + 1 > kMaxPreds) return fail(BYDB_ENOTSUP, "a group-key query takes at most 7 predicates");
+    return 0;
+}
+// the same for a tuple key (bydb_scan_agg_keys_wide): 2..kMaxKeyTags distinct tags, each checked as a wide key with max_values 0;
+// cap = the distinct tuples accepted (max_values, 0 = 64), at most max_cap
+int check_group_key(const bydb_query *q, const bydb_group_keys *keys, uint32_t max_cap, bool pred_slot, uint32_t &cap) {
+    if (!keys || !keys->keys) return fail(BYDB_EINVAL, "bydb_group_keys without keys");
+    if (keys->n_keys < 2 || keys->n_keys > kMaxKeyTags)
+        return fail(BYDB_EINVAL, "bydb_group_keys.n_keys must be 2..4 (one stored key: bydb_scan_agg_keyed_wide)");
+    for (uint32_t t = 0; t < keys->n_keys; ++t) {
+        const bydb_group_key *k = &keys->keys[t];
+        uint32_t unused = 0;
+        if (int rc = check_group_key(q, k, max_cap, pred_slot, unused)) return rc;
+        if (k->max_values != 0) return fail(BYDB_EINVAL, "bydb_group_keys: a key's own max_values must be 0 (the cap is bydb_group_keys.max_values)");
+        for (uint32_t u = 0; u < t; ++u)
+            if (!strcmp(keys->keys[u].family, k->family) && !strcmp(keys->keys[u].tag, k->tag))
+                return fail(BYDB_EINVAL, std::string("bydb_group_keys: the tag ") + k->family + "/" + k->tag + " is named twice");
+    }
+    cap = keys->max_values ? keys->max_values : 64u;
+    if (cap > max_cap) return fail(BYDB_EINVAL, "bydb_group_keys.max_values above " + std::to_string(max_cap));
     return 0;
 }
 
@@ -2198,6 +2221,8 @@ size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, cons
 
 void keyed_free(bydb_ctx *ctx, bydb_keyed_result *out) { bydb_keyed_result_free(ctx, out); }
 void keyed_free(bydb_ctx *ctx, bydb_keyed_partial_rows *out) { bydb_keyed_partial_rows_free(ctx, out); }
+void keyed_free(bydb_ctx *ctx, bydb_keys_result *out) { bydb_keys_result_free(ctx, out); }
+void keyed_free(bydb_ctx *ctx, bydb_keys_partial_rows *out) { bydb_keys_partial_rows_free(ctx, out); }
 
 // a keyed answer being filled: its owner and key table (value k is values[k]) are set up on construction, and a failure past that
 // point must not leave a half-filled result with the caller, so the answer is freed again unless `done` is set
@@ -2207,19 +2232,18 @@ struct KeyedAnswer {
     Out *out;
     KeyedOwner *owner;
     bool done = false;
-    KeyedAnswer(bydb_ctx *c, Out *o, const KeyValues &values) : ctx(c), out(o), owner(new KeyedOwner()) {
-        out->owner = owner;
-        set_key_table(out, owner, values);
-    }
+    KeyedAnswer(bydb_ctx *c, Out *o, const KeyValues &values) : KeyedAnswer(c, o) { set_key_table(out, owner, values); }
+    KeyedAnswer(bydb_ctx *c, Out *o) : ctx(c), out(o), owner(new KeyedOwner()) { out->owner = owner; }
     ~KeyedAnswer() {
         if (!done) keyed_free(ctx, out);
     }
 };
 
-// The preamble of an unprepared keyed call: the arguments and the key (cap at most max_cap; pred_slot: see check_group_key), the
-// plan, the refusal of parts that overlap in time, the device, the slot and the answer's zeroed stats
-template <class Out>
-int keyed_call(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t max_cap, bool pred_slot, Out *out, uint32_t &cap, Plan &plan,
+// The preamble of an unprepared keyed call: the arguments and the key (a bydb_group_key, or a bydb_group_keys' tuple; cap at most
+// max_cap; pred_slot: see check_group_key), the plan, the refusal of parts that overlap in time, the device, the slot and the
+// answer's zeroed stats
+template <class Out, class Key>
+int keyed_call(bydb_ctx *ctx, const bydb_query *q, const Key *key, uint32_t max_cap, bool pred_slot, Out *out, uint32_t &cap, Plan &plan,
                std::optional<SlotLease> &lease) {
     if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
     memset(out, 0, sizeof *out);
@@ -2288,9 +2312,15 @@ size_t pow2_at_least(size_t n) {
     return p;
 }
 
-// the answer forms over the table of the present composite groups (n_comp groups of layout tl at `table`) that the fold `rp` wrote
-int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const WideReduceParams &rp,
-              bydb_keyed_result *out, KeyedOwner *owner) {
+// the answer forms over the table of the present composite groups (n_comp groups of layout tl at `table`) that the fold `rp` wrote:
+// finalised rows (an answer around a bydb_result) or partial rows (around a bydb_partial_rows)
+template <class Out>
+using FinalisedAnswer = std::enable_if_t<std::is_same<decltype(Out::base), bydb_result>::value, int>;
+template <class Out>
+using PartialAnswer = std::enable_if_t<std::is_same<decltype(Out::base), bydb_partial_rows>::value, int>;
+template <class Out>
+FinalisedAnswer<Out> wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp,
+                               const WideReduceParams &rp, Out *out, KeyedOwner *owner) {
     cudaStream_t stream = slot.stream;
     Plan planc = plan;
     planc.n_groups = static_cast<int32_t>(n_comp);
@@ -2303,8 +2333,9 @@ int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *ta
     set_row_keys(out, owner, static_cast<ResultOwner *>(out->base.owner)->group_id, pairs.data(), 8, true);
     return 0;
 }
-int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp, const WideReduceParams &rp,
-              bydb_keyed_partial_rows *out, KeyedOwner *owner) {
+template <class Out>
+PartialAnswer<Out> wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *table, const TableLayout &tl, size_t n_comp,
+                             const WideReduceParams &rp, Out *out, KeyedOwner *owner) {
     cudaStream_t stream = slot.stream;
     const size_t F = plan.fcols.size(), A = q->n_aggs, ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
     Plan planc = plan;
@@ -2329,7 +2360,8 @@ int wide_emit(const bydb_query *q, const Plan &plan, ExecSlot &slot, uint8_t *ta
 
 // The wide path's discovery and scan state.  wide_discover fills values, R, disc_bytes (the discovery scratch `ka`), wk and
 // series_group; wide_scan_order fills rp with everything launch_wide_fold reads but its outputs (table, pairs, perm); wide_pass
-// runs both and sets n_comp.  No value or no record: R = 0 and nothing past discovery ran.
+// runs both and sets n_comp.  No value or no record: R = 0 and nothing past discovery ran.  A tuple key (tags.n_tags > 0): wk is
+// the tuple table, whose ids the records carry; tag_values and codes hold each tag's values and each tuple's code.
 struct WidePass {
     KeyValues values;
     size_t R = 0, n_comp = 0, disc_bytes = 0;
@@ -2337,29 +2369,50 @@ struct WidePass {
     WideKeyParams wk;
     const int32_t *series_group = nullptr;  // [NS] in ka
     WideReduceParams rp;
+    WideTagSet tags{};
+    std::vector<KeyValues> tag_values;
+    std::vector<uint64_t> codes;
 };
 
 // 1. discovery, on the slot's stream, synchronised: the value table (S slots), each selected block's rank and distinct values,
-// then their exclusive scan (each block's first record; R their sum), and the values read back
-int wide_discover(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats &stats,
-                  WidePass &w) {
+// then their exclusive scan (each block's first record; R their sum), and the values read back.  A tuple key (n_keys > 1) has a
+// table per tag, then one of the tuples, whose kernel writes the blocks' distinct tuples; all tables share the cap.
+int wide_discover(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *keys, uint32_t n_keys, uint32_t cap, const Plan &plan, ExecSlot &slot,
+                  bydb_stats &stats, WidePass &w) {
     cudaStream_t stream = slot.stream;
-    const bool int64_key = key->value_type == BYDB_VT_INT64;
+    const size_t nt = n_keys == 1 ? 1 : n_keys + 1;  // the tables; the last one numbers the records
     const size_t NS = q->n_series, NB = plan.total_blocks, NBp = align_up(std::max<size_t>(NB, 1), 1024);
     CUDA_TRY(cudaEventRecord(slot.ev[0], stream));
     const size_t S = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(cap), kKeySlots));
+    auto is_tuples = [&](size_t t) { return nt > 1 && t + 1 == nt; };
+    auto int64_table = [&](size_t t) { return is_tuples(t) || keys[t].value_type == BYDB_VT_INT64; };
     Carve carve;
-    const size_t a_sids = carve(NS * 8), a_grp = carve(NS * 4), a_slots = carve(S * 8), a_ctl = carve(32), a_vals = carve(static_cast<size_t>(cap) * kMaxLit),
-                 a_lens = carve(static_cast<size_t>(cap) * 4), a_sid = carve(S * 4), a_nbr = carve(NBp * 4), a_rank = carve(NB * 4),
-                 a_tiles = carve(NBp / 1024 * 4);
+    const size_t a_sids = carve(NS * 8), a_grp = carve(NS * 4);
+    size_t a_slots[kMaxKeyTags + 1], a_vals[kMaxKeyTags + 1], a_lens[kMaxKeyTags + 1], a_sid[kMaxKeyTags + 1];
+    for (size_t t = 0; t < nt; ++t) a_slots[t] = carve(S * 8);
+    const size_t a_ctl = carve(32 * nt);
+    for (size_t t = 0; t < nt; ++t) {
+        a_vals[t] = carve(static_cast<size_t>(cap) * (is_tuples(t) ? 8 : kMaxLit));
+        a_lens[t] = carve(is_tuples(t) ? 0 : static_cast<size_t>(cap) * 4);
+        a_sid[t] = carve(S * 4);
+    }
+    const size_t a_nbr = carve(NBp * 4), a_rank = carve(NB * 4), a_tiles = carve(NBp / 1024 * 4);
     Scratch &ka = w.ka;
     CUDA_TRY(ka.alloc(carve.o, stream));
     w.disc_bytes = carve.o;
-    if (slot.ensure_pinned(std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    WideKeyParams &wk = w.wk;
-    memset(&wk, 0, sizeof wk);
-    KeyParams &kp = wk.k;
-    kp = key_params(ctx, q, key, cap, plan, slot.pinned, ka.base, a_sids, a_slots, a_ctl, a_vals, a_lens);
+    const size_t back_max = 32 * nt + (nt > 1 ? (nt - 1) * static_cast<size_t>(cap) * (kMaxLit + 4) + static_cast<size_t>(cap) * 8 : static_cast<size_t>(cap) * (kMaxLit + 4));
+    if (slot.ensure_pinned(std::max<size_t>(NS * 12, back_max) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    WideKeyParams wks[kMaxKeyTags + 1];
+    for (size_t t = 0; t < nt; ++t) {
+        WideKeyParams &wk = wks[t];
+        memset(&wk, 0, sizeof wk);
+        wk.k = key_params(ctx, q, &keys[is_tuples(t) ? 0 : t], cap, plan, slot.pinned, ka.base, a_sids, a_slots[t], a_ctl + 32 * t, a_vals[t], a_lens[t]);
+        wk.slot_mask = static_cast<uint32_t>(S - 1);
+        wk.int64_key = int64_table(t) ? 1u : 0u;
+        wk.slot_id = reinterpret_cast<uint32_t *>(ka.base + a_sid[t]);
+        wk.n_by_rank = reinterpret_cast<uint32_t *>(ka.base + a_nbr);
+        wk.rank = reinterpret_cast<uint32_t *>(ka.base + a_rank);
+    }
     int32_t *hg = reinterpret_cast<int32_t *>(slot.pinned + NS * 8);
     for (size_t i = 0; i < NS; ++i) hg[i] = q->series_group ? q->series_group[i] : 0;
     if (NS) {
@@ -2367,34 +2420,63 @@ int wide_discover(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key,
         CUDA_TRY(cudaMemcpyAsync(ka.base + a_grp, slot.pinned + NS * 8, NS * 4, cudaMemcpyHostToDevice, stream));
     }
     stats.h2d_bytes += NS * 12;
-    CUDA_TRY(cudaMemsetAsync(ka.base + a_slots, 0, a_vals - a_slots, stream));
+    CUDA_TRY(cudaMemsetAsync(ka.base + a_slots[0], 0, a_vals[0] - a_slots[0], stream));
     CUDA_TRY(cudaMemsetAsync(ka.base + a_nbr, 0, NBp * 4, stream));
-    uint32_t *d_ctl = kp.count;  // as discovery's, and [4] R
-    wk.slot_mask = static_cast<uint32_t>(S - 1);
-    wk.int64_key = int64_key ? 1u : 0u;
-    wk.slot_id = reinterpret_cast<uint32_t *>(ka.base + a_sid);
-    wk.n_by_rank = reinterpret_cast<uint32_t *>(ka.base + a_nbr);
-    wk.rank = reinterpret_cast<uint32_t *>(ka.base + a_rank);
+    w.wk = wks[nt - 1];
+    uint32_t *d_ctl = w.wk.k.count;  // as discovery's, and [4] R
     w.series_group = reinterpret_cast<const int32_t *>(ka.base + a_grp);
-    launch_key_values_wide(wk, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
-    launch_excl_scan(wk.n_by_rank, static_cast<uint32_t>(NBp), reinterpret_cast<uint32_t *>(ka.base + a_tiles), d_ctl + 4, stream);
-    CUDA_TRY(cudaMemcpyAsync(slot.pinned, d_ctl, 32, cudaMemcpyDeviceToHost, stream));
+    w.tags = WideTagSet{};
+    if (nt > 1) {
+        w.tags.n_tags = n_keys;
+        for (uint32_t t = 0; t < n_keys; ++t) {
+            launch_key_values_wide(wks[t], ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+            w.tags.tag[t] = WideTag{wks[t].k.slots, wks[t].slot_id, wks[t].slot_mask, wks[t].k.key_name, static_cast<uint8_t>(wks[t].int64_key), 0};
+        }
+        launch_key_tuples_wide(w.wk, w.tags, ctx->sm_count * scan_keys_wide_ctas_per_sm(), stream);
+    } else {
+        launch_key_values_wide(w.wk, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+    }
+    launch_excl_scan(w.wk.n_by_rank, static_cast<uint32_t>(NBp), reinterpret_cast<uint32_t *>(ka.base + a_tiles), d_ctl + 4, stream);
+    CUDA_TRY(cudaMemcpyAsync(slot.pinned, ka.base + a_ctl, 32 * nt, cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     CUDA_TRY(cudaGetLastError());
-    stats.kernel_launches += (NB ? 1u : 0u) + 1u + 3u;
-    stats.d2h_bytes += 32;
-    uint32_t ctl[8];
-    memcpy(ctl, slot.pinned, 32);
-    int rc = discovery_status(ctl);
-    if (rc) return rc;
-    const size_t V = std::min<size_t>(ctl[0], cap), R = ctl[4];
-    if (V) {
-        const size_t vb = V * (int64_key ? 8 : kMaxLit);
-        CUDA_TRY(cudaMemcpyAsync(slot.pinned, kp.vals, vb, cudaMemcpyDeviceToHost, stream));
-        if (!int64_key) CUDA_TRY(cudaMemcpyAsync(slot.pinned + vb, kp.lens, V * 4, cudaMemcpyDeviceToHost, stream));
-        CUDA_TRY(cudaStreamSynchronize(stream));
-        stats.d2h_bytes += vb + (int64_key ? 0 : V * 4);
-        w.values = unpack_values(V, int64_key, slot.pinned, reinterpret_cast<const uint32_t *>(slot.pinned + vb));
+    stats.kernel_launches += static_cast<uint32_t>(nt) * ((NB ? 1u : 0u) + 1u) + 3u;
+    stats.d2h_bytes += 32 * nt;
+    uint32_t ctl[8 * (kMaxKeyTags + 1)];
+    memcpy(ctl, slot.pinned, 32 * nt);
+    for (size_t t = 0; t < nt; ++t) {
+        const uint32_t *c = ctl + 8 * t;
+        if (nt > 1 && c[1] == kErrKeyCap) {
+            g_last_dev_err = c[1];
+            return fail(BYDB_ENOMEM, "tuple group key: more distinct key tuples than bydb_group_keys.max_values (block #" + std::to_string(c[2]) + ")");
+        }
+        if (int rc = discovery_status(c)) return rc;
+    }
+    const size_t V = std::min<size_t>(ctl[8 * (nt - 1)], cap), R = ctl[8 * (nt - 1) + 4];
+    // the values of every table, back to back in the staging, in one synchronised read-back
+    size_t at[kMaxKeyTags + 1], n_vals[kMaxKeyTags + 1], back = 0;
+    for (size_t t = 0; t < nt; ++t) {
+        n_vals[t] = std::min<size_t>(ctl[8 * t], cap);
+        at[t] = back;
+        if (!n_vals[t]) continue;
+        const size_t vb = n_vals[t] * (int64_table(t) ? 8 : kMaxLit);
+        CUDA_TRY(cudaMemcpyAsync(slot.pinned + back, wks[t].k.vals, vb, cudaMemcpyDeviceToHost, stream));
+        if (!int64_table(t)) CUDA_TRY(cudaMemcpyAsync(slot.pinned + back + vb, wks[t].k.lens, n_vals[t] * 4, cudaMemcpyDeviceToHost, stream));
+        back += vb + (int64_table(t) ? 0 : n_vals[t] * 4);
+    }
+    if (back) CUDA_TRY(cudaStreamSynchronize(stream));
+    stats.d2h_bytes += back;
+    auto values_of = [&](size_t t) {
+        const size_t vb = n_vals[t] * (int64_table(t) ? 8 : kMaxLit);
+        return unpack_values(n_vals[t], int64_table(t), slot.pinned + at[t], reinterpret_cast<const uint32_t *>(slot.pinned + at[t] + vb));
+    };
+    if (nt == 1) {
+        w.values = values_of(0);
+    } else {
+        w.tag_values.clear();
+        for (uint32_t t = 0; t < n_keys; ++t) w.tag_values.push_back(values_of(t));
+        w.codes.resize(V);
+        if (V) memcpy(w.codes.data(), slot.pinned + at[nt - 1], V * 8);
     }
     if (V == 0 || R == 0) return 0;  // no block selected: no rows (n_rows = 0)
     if (R > 0x7fffffffull) return fail(BYDB_ENOMEM, "wide group-key query: too many (block, key value) records");
@@ -2452,7 +2534,14 @@ int wide_scan_order(bydb_ctx *ctx, const bydb_query *q, const Plan &plan, WidePa
     ws.series_group = w.series_group;
     ws.records = sb + L.rec;
     if (ev) CUDA_TRY(cudaEventRecord(ev[1], stream));
-    launch_scan_keyed_wide(sp, ws, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+    if (w.tags.n_tags) {
+        WideTupleParams wt;
+        static_cast<WideScanParams &>(wt) = ws;
+        wt.tags = w.tags;
+        launch_scan_keys_wide(sp, wt, ctx->sm_count * scan_keys_wide_ctas_per_sm(), stream);
+    } else {
+        launch_scan_keyed_wide(sp, ws, ctx->sm_count * scan_keyed_wide_ctas_per_sm(), stream);
+    }
     if (ev) CUDA_TRY(cudaEventRecord(ev[2], stream));
     WideReduceParams &rp = w.rp;
     memset(&rp, 0, sizeof rp);
@@ -2480,10 +2569,10 @@ int wide_scan_order(bydb_ctx *ctx, const bydb_query *q, const Plan &plan, WidePa
 
 // Steps 1-3 of the wide path, on the slot's stream, synchronised: discovery (w.values), the scan and the order (w.n_comp composite
 // groups).  The scratch behind w.rp stays alive in `w`.
-int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uint32_t cap, const Plan &plan, ExecSlot &slot, bydb_stats &stats,
-              WidePass &w) {
+int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *keys, uint32_t n_keys, uint32_t cap, const Plan &plan, ExecSlot &slot,
+              bydb_stats &stats, WidePass &w) {
     cudaStream_t stream = slot.stream;
-    int rc = wide_discover(ctx, q, key, cap, plan, slot, stats, w);
+    int rc = wide_discover(ctx, q, keys, n_keys, cap, plan, slot, stats, w);
     if (rc || w.R == 0) return rc;
     const WideScanLayout L = wide_scan_layout(w.R, plan.fcols.size());
     Scratch &sb = w.sb;
@@ -2513,8 +2602,60 @@ int wide_pass(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, uin
     return 0;
 }
 
+// the key tables of a wide answer: one key's values, or a tuple key's tables (tag t's values are entries key_base[t] ..)
 template <class Out>
-int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
+void wide_key_tables(Out *out, KeyedOwner *owner, const WidePass &w) {
+    set_key_table(out, owner, w.values);
+}
+template <class Out>
+void tuple_key_tables(Out *out, KeyedOwner *owner, const WidePass &w) {
+    owner->key_base.assign(1, 0);
+    owner->key_off.assign(1, 0);
+    owner->key_bytes.clear();
+    for (const KeyValues &vals : w.tag_values) {
+        for (const auto &v : vals) {
+            owner->key_bytes.insert(owner->key_bytes.end(), v.begin(), v.end());
+            owner->key_off.push_back(static_cast<uint32_t>(owner->key_bytes.size()));
+        }
+        owner->key_base.push_back(owner->key_base.back() + static_cast<int32_t>(vals.size()));
+    }
+    if (owner->key_bytes.empty()) owner->key_bytes.push_back(0);
+    out->n_tags = static_cast<uint32_t>(w.tag_values.size());
+    out->n_tuples = static_cast<int32_t>(w.codes.size());
+    out->key_base = owner->key_base.data();
+    out->key_off = owner->key_off.data();
+    out->key_bytes = owner->key_bytes.data();
+}
+void wide_key_tables(bydb_keys_result *out, KeyedOwner *owner, const WidePass &w) { tuple_key_tables(out, owner, w); }
+void wide_key_tables(bydb_keys_partial_rows *out, KeyedOwner *owner, const WidePass &w) { tuple_key_tables(out, owner, w); }
+
+// a tuple key's rows carry the tuple id (set_row_keys): each becomes its tags' entries, key_id[r * n_tags + t]
+template <class Out>
+void wide_row_tuples(Out *, KeyedOwner *, const WidePass &) {}
+template <class Out>
+void tuple_row_entries(Out *out, KeyedOwner *owner, const WidePass &w) {
+    const size_t K = w.tag_values.size(), n = owner->key_id.size();
+    std::vector<int32_t> ids(n * K);
+    for (size_t r = 0; r < n; ++r) {
+        const uint64_t code = w.codes[static_cast<size_t>(owner->key_id[r])];
+        for (size_t t = 0; t < K; ++t) ids[r * K + t] = owner->key_base[t] + static_cast<int32_t>((code >> (16 * t)) & 0xffffu);
+    }
+    owner->key_id.swap(ids);
+    out->key_id = owner->key_id.data();
+}
+void wide_row_tuples(bydb_keys_result *out, KeyedOwner *owner, const WidePass &w) { tuple_row_entries(out, owner, w); }
+void wide_row_tuples(bydb_keys_partial_rows *out, KeyedOwner *owner, const WidePass &w) { tuple_row_entries(out, owner, w); }
+
+// the key list of a wide call: a bydb_group_key, or the tags of a bydb_group_keys
+const bydb_group_key *key_list(const bydb_group_key *key) { return key; }
+const bydb_group_key *key_list(const bydb_group_keys *keys) { return keys->keys; }
+uint32_t key_count(const bydb_group_key *) { return 1; }
+uint32_t key_count(const bydb_group_keys *keys) { return keys->n_keys; }
+
+// bydb_scan_agg_keyed_wide / bydb_scan_partials_keyed_wide (Key = bydb_group_key) and bydb_scan_agg_keys_wide /
+// bydb_scan_partials_keys_wide (Key = bydb_group_keys)
+template <class Out, class Key>
+int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const Key *key, Out *out) {
     uint32_t cap = 0;
     Plan plan;
     std::optional<SlotLease> lease;
@@ -2525,9 +2666,10 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     const size_t F = plan.fcols.size();
     bydb_stats &stats = keyed_stats(out);
     WidePass w;
-    rc = wide_pass(ctx, q, key, cap, plan, slot, stats, w);
+    rc = wide_pass(ctx, q, key_list(key), key_count(key), cap, plan, slot, stats, w);
     if (rc) return rc;
-    KeyedAnswer<Out> answer(ctx, out, w.values);
+    KeyedAnswer<Out> answer(ctx, out);
+    wide_key_tables(out, answer.owner, w);
     if (w.R == 0) {  // no block selected: no rows (n_rows = 0)
         answer.done = true;
         return 0;
@@ -2549,6 +2691,7 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_ke
     stats.kernel_launches += 1;
     if (n_comp > 0) rc = wide_emit(q, plan, slot, fb.base + f_table, tl, n_comp, rp, out, answer.owner);
     if (rc) return rc;
+    if (n_comp > 0) wide_row_tuples(out, answer.owner, w);
     {
         float ms = 0;
         cudaEventElapsedTime(&ms, slot.ev[0], slot.ev[3]);
@@ -2755,7 +2898,7 @@ void wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     cudaStream_t stream = slot.stream;
     bydb_stats eager{};
     WidePass w;
-    if (parts_overlap(plan.parts, q->tmin, q->tmax) || wide_pass(ctx, q, &k->key, k->cap, plan, slot, eager, w)) {
+    if (parts_overlap(plan.parts, q->tmin, q->tmax) || wide_pass(ctx, q, &k->key, 1, k->cap, plan, slot, eager, w)) {
         p->capturable = false;
         return;
     }
@@ -3207,6 +3350,29 @@ int bydb_scan_agg_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_grou
 
 int bydb_scan_partials_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_keyed_partial_rows *out) {
     return guarded([&]() -> int { return scan_keyed_wide_impl(ctx, q, key, out); });
+}
+
+// Group-by on a tuple of 2..4 stored tags in one scan pass: see "tuple group key" in scan_kernels.cuh.
+int bydb_scan_agg_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, bydb_keys_result *out) {
+    return guarded([&]() -> int { return scan_keyed_wide_impl(ctx, q, keys, out); });
+}
+
+int bydb_scan_partials_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, bydb_keys_partial_rows *out) {
+    return guarded([&]() -> int { return scan_keyed_wide_impl(ctx, q, keys, out); });
+}
+
+void bydb_keys_result_free(bydb_ctx *ctx, bydb_keys_result *r) {
+    if (!r) return;
+    bydb_result_free(ctx, &r->base);
+    delete static_cast<KeyedOwner *>(r->owner);
+    memset(r, 0, sizeof *r);
+}
+
+void bydb_keys_partial_rows_free(bydb_ctx *ctx, bydb_keys_partial_rows *r) {
+    if (!r) return;
+    bydb_partial_rows_free(ctx, &r->base);
+    delete static_cast<KeyedOwner *>(r->owner);
+    memset(r, 0, sizeof *r);
 }
 
 void bydb_keyed_partial_rows_free(bydb_ctx *ctx, bydb_keyed_partial_rows *r) {
@@ -4528,7 +4694,7 @@ static int scan_reduce_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const
     h.contribute = [&](ExecSlot &es, uint8_t *my_slot) -> int {
         cudaStream_t s = es.stream;
         const size_t F = plan.fcols.size(), NS = q->n_series;
-        int rc = wide_pass(ctx, q, key, cap, plan, es, stats, w);
+        int rc = wide_pass(ctx, q, key, 1, cap, plan, es, stats, w);
         if (rc) return rc;
         const size_t V = w.values.size(), C = w.n_comp;
         const WideSlot ws(F, NS, V, C);

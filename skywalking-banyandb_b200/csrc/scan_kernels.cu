@@ -4890,8 +4890,9 @@ void launch_key_values_wide(const WideKeyParams &p, int grid, cudaStream_t s) {
     key_pack_wide_kernel<<<1, 1024, 0, s>>>(p);
 }
 
-// the id of a value the discovery entered (string: by its bytes, int64: by the value)
-__device__ __forceinline__ uint32_t wide_key_id(const WideScanParams &w, unsigned long long v) {
+// the id of a value the discovery entered (string: by its bytes, int64: by the value) in the table W names (WideScanParams, WideTag)
+template <class W>
+__device__ __forceinline__ uint32_t wide_key_id(const W &w, unsigned long long v) {
     if (w.int64_key) {
         if (v == 0ull) return 0u;
         uint32_t s = key_slot_i64(v, w.slot_mask);
@@ -4912,6 +4913,160 @@ __device__ __forceinline__ uint32_t wide_key_id(const WideScanParams &w, unsigne
         s = (s + 1) & w.slot_mask;
     }
     return w.slot_id[s];
+}
+
+// ---- tuple key: the per-warp shared memory it needs besides WideSmem
+struct __align__(16) TupleSmem {
+    uint8_t tidx[kMaskWords * 32];        // block-local index of each row's tuple over the tags combined so far
+    unsigned long long code[kMaxBlockKeys];  // local tuple k so far: id_0 | id_1 << 16 | ...
+};
+size_t tuple_smem_bytes() { return wide_smem_bytes() + sizeof(TupleSmem) * kWideWarps; }
+__device__ __forceinline__ TupleSmem *tuple_smem(uint8_t *smem_raw) {
+    return reinterpret_cast<TupleSmem *>(smem_raw + (sizeof(WarpSmem) + sizeof(WideSmem)) * kWideWarps) + (threadIdx.x >> 5);
+}
+__device__ __forceinline__ uint32_t pair_home(unsigned long long pr) { return static_cast<uint32_t>((pr * 0x9e3779b97f4a7c15ull) >> 55) & (kLocalSlots - 1); }
+
+// The block's tuples, as wide_block_keys<true> leaves one key: the block-local tuple index of every row in ws->kidx, local tuple k's
+// code in ws->dense[k], their number in ws->n_local.  The tags are taken one at a time: wide_block_keys<true> gives the tag's local
+// index per row, and each row's pair (tuple so far, tag's local index) enters a table of kLocalSlots pairs in ws->u.t (free once
+// wide_block_keys returns), numbered in slot order.  Only pairs that some row shows become tuples.  Returns a DevErr.
+__device__ uint32_t tuple_block_keys(WarpSmem *sm, WideSmem *ws, TupleSmem *ts, const DevPartRef &part, const DevBlock &blk, const WideTagSet &tags,
+                                     int lane) {
+    const uint32_t count = blk.count;
+    if (count > kMaskWords * 32) return kErrBigBlock;
+    unsigned long long *pslot = ws->u.t.val;
+    uint32_t n = 0;
+    for (uint32_t t = 0; t < tags.n_tags; ++t) {
+        const WideTag &tg = tags.tag[t];
+        const uint32_t err = wide_block_keys<true>(sm, ws, part, blk, tg.key_name, tg.int64_key != 0, lane);
+        if (err != kErrNone) return err;
+        const uint32_t nl = ws->n_local;
+        for (uint32_t k = lane; k < nl; k += 32) ws->gid[k] = wide_key_id(tg, ws->dense[k]);
+        __syncwarp();
+        if (t == 0) {
+            for (uint32_t r = lane; r < count; r += 32) ts->tidx[r] = ws->kidx[r];
+            for (uint32_t k = lane; k < nl; k += 32) ts->code[k] = ws->gid[k];
+            n = nl;
+            __syncwarp();
+            continue;
+        }
+        for (uint32_t s = lane; s < kLocalSlots; s += 32) pslot[s] = 0ull;
+        if (lane == 0) ws->over = 0;
+        __syncwarp();
+        for (uint32_t r = lane; r < count; r += 32) {
+            const unsigned long long pr = 1ull + ((static_cast<uint32_t>(ts->tidx[r]) << 8) | ws->kidx[r]);
+            uint32_t s = pair_home(pr), probe = 0;
+            for (; probe < kLocalSlots; ++probe) {
+                unsigned long long cur = reinterpret_cast<volatile unsigned long long *>(pslot)[s];
+                if (cur == 0ull) cur = atomicCAS(&pslot[s], 0ull, pr);
+                if (cur == 0ull || cur == pr) break;
+                s = (s + 1) & (kLocalSlots - 1);
+            }
+            if (probe == kLocalSlots) ws->over = 1u;
+        }
+        __syncwarp();
+        if (ws->over) return kErrTupleBlock;
+        // number the pairs in slot order; the new tuple's code adds the tag's value id at bits 16t
+        uint32_t base = 0;
+        for (uint32_t s0 = 0; s0 < kLocalSlots; s0 += 32) {
+            const unsigned long long pr = pslot[s0 + lane];
+            const uint32_t bal = __ballot_sync(0xffffffffu, pr != 0ull);
+            if (pr != 0ull) {
+                const uint32_t k = base + __popc(bal & ((1u << lane) - 1u));
+                ws->u.t.idx[s0 + lane] = static_cast<uint8_t>(k);
+                if (k < kMaxBlockKeys)
+                    ws->dense[k] = ts->code[(pr - 1ull) >> 8] | (static_cast<unsigned long long>(ws->gid[(pr - 1ull) & 0xffu]) << (16u * t));
+            }
+            base += __popc(bal);
+        }
+        if (base > kMaxBlockKeys) return kErrTupleBlock;
+        __syncwarp();
+        const bool last = t + 1 == tags.n_tags;
+        if (!last)
+            for (uint32_t k = lane; k < base; k += 32) ts->code[k] = ws->dense[k];
+        for (uint32_t r = lane; r < count; r += 32) {
+            const unsigned long long pr = 1ull + ((static_cast<uint32_t>(ts->tidx[r]) << 8) | ws->kidx[r]);
+            uint32_t s = pair_home(pr);
+            for (uint32_t probe = 0; probe < kLocalSlots && pslot[s] != pr; ++probe) s = (s + 1) & (kLocalSlots - 1);
+            if (last) ws->kidx[r] = ws->u.t.idx[s];
+            else ts->tidx[r] = ws->u.t.idx[s];
+        }
+        n = base;
+        __syncwarp();
+    }
+    if (lane == 0) ws->n_local = n;
+    __syncwarp();
+    return kErrNone;
+}
+
+// discovery of a tuple key: key_values_wide_kernel's walk, the block's tuple codes into the tuple table
+__global__ void __launch_bounds__(kWideWarps * 32) key_tuples_wide_kernel(const __grid_constant__ WideKeyParams w, const __grid_constant__ WideTagSet tags) {
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    const KeyParams &p = w.k;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    WarpSmem *sm = reinterpret_cast<WarpSmem *>(smem_raw) + warp;
+    WideSmem *ws = reinterpret_cast<WideSmem *>(smem_raw + sizeof(WarpSmem) * kWideWarps) + warp;
+    TupleSmem *ts = tuple_smem(smem_raw);
+    if (lane == 0) {
+        sm->fault = 0;
+        sm->seq = 0;
+        for (int s = 0; s < kStages; ++s) mbar_init(&sm->bar[s], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const uint32_t n_warps = gridDim.x * kWideWarps;
+    for (uint32_t g = blockIdx.x * kWideWarps + warp; g < p.total_blocks; g += n_warps) {
+        uint32_t stop = lane == 0 ? *reinterpret_cast<volatile uint32_t *>(&p.err[0]) : 0u;
+        stop = __shfl_sync(0xffffffffu, stop, 0);
+        if (stop != 0u) return;  // warp-uniform
+        uint32_t pi = 0;
+        while (pi + 1 < p.n_parts && g >= p.parts[pi + 1].block_base) ++pi;
+        const DevPartRef &part = p.parts[pi];
+        const DevBlock blk = part.blocks[g - part.block_base];
+        int32_t qi;
+        if (!select_block(p.q_sids, p.n_series, p.tmin, p.tmax, blk, qi)) continue;
+        uint32_t err = tuple_block_keys(sm, ws, ts, part, blk, tags, lane);
+        if (sm->fault) err = kErrTmaTimeout;
+        const uint32_t n = ws->n_local;
+        if (err == kErrNone) {
+            for (uint32_t k = lane; k < n; k += 32) {
+                const unsigned long long v = ws->dense[k];
+                key_insert_i64_at(p, v, v == 0ull ? 0u : key_slot_i64(v, w.slot_mask), g, w.slot_mask);
+            }
+            const uint32_t r = scan_rank(p.parts, p.n_parts, pi, g - part.block_base, lane);
+            if (lane == 0) {
+                w.rank[g] = r;
+                w.n_by_rank[r] = n;
+            }
+        } else if (lane == 0) {
+            key_err(p, err, g);
+        }
+        __syncwarp();
+    }
+}
+
+void launch_key_tuples_wide(const WideKeyParams &p, const WideTagSet &tags, int grid, cudaStream_t s) {
+    const size_t smem = tuple_smem_bytes();
+    cudaFuncSetAttribute(key_tuples_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (p.k.total_blocks) key_tuples_wide_kernel<<<grid, kWideWarps * 32, smem, s>>>(p, tags);
+    key_pack_wide_kernel<<<1, 1024, 0, s>>>(p);
+}
+
+// ---- the key stage of scan_keyed_wide_kernel: the block-local index of every row in ws->kidx, the local keys' words in ws->dense
+// (one key: its values; a tuple key: the tuples' codes), their number in ws->n_local; every key page counted once in page_bytes
+__device__ __forceinline__ uint32_t wide_key_stage(WarpSmem *sm, WideSmem *ws, uint8_t *, const DevPartRef &part, const DevBlock &blk,
+                                                   const WideScanParams &w, uint32_t &page_bytes, int lane) {
+    DevCol kcol;
+    if (find_col(part, blk, w.key_name, kcol, lane)) page_bytes += kcol.size;
+    return wide_block_keys<true>(sm, ws, part, blk, w.key_name, w.int64_key != 0, lane);
+}
+__device__ __forceinline__ uint32_t wide_key_stage(WarpSmem *sm, WideSmem *ws, uint8_t *smem_raw, const DevPartRef &part, const DevBlock &blk,
+                                                   const WideTupleParams &w, uint32_t &page_bytes, int lane) {
+    for (uint32_t t = 0; t < w.tags.n_tags; ++t) {
+        DevCol kcol;
+        if (find_col(part, blk, w.tags.tag[t].key_name, kcol, lane)) page_bytes += kcol.size;
+    }
+    return tuple_block_keys(sm, ws, tuple_smem(smem_raw), part, blk, w.tags, lane);
 }
 
 // one surviving row's value into its key's accumulator: 128-bit sum by limbs (each add carries against the value it replaced,
@@ -4938,7 +5093,9 @@ struct WideAggCons {
     }
 };
 
-__global__ void __launch_bounds__(kWideWarps * 32) scan_keyed_wide_kernel(const __grid_constant__ ScanParams p, const __grid_constant__ WideScanParams w) {
+// W: WideScanParams (one key) or WideTupleParams (a tuple key); only the key stage (wide_key_stage) differs
+template <class W>
+__global__ void __launch_bounds__(kWideWarps * 32) scan_keyed_wide_kernel(const __grid_constant__ ScanParams p, const __grid_constant__ W w) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     WarpSmem *sm = reinterpret_cast<WarpSmem *>(smem_raw) + warp;
@@ -5079,12 +5236,8 @@ __global__ void __launch_bounds__(kWideWarps * 32) scan_keyed_wide_kernel(const 
             rows = __reduce_add_sync(0xffffffffu, c);
         }
 
-        // ---- 3. the key column -> block-local index per row, then rows and first row per local key
-        if (err == kErrNone) {
-            DevCol kcol;
-            if (find_col(part, blk, w.key_name, kcol, lane)) page_bytes += kcol.size;
-            err = wide_block_keys<true>(sm, ws, part, blk, w.key_name, w.int64_key != 0, lane);
-        }
+        // ---- 3. the key column(s) -> block-local index per row, then rows and first row per local key
+        if (err == kErrNone) err = wide_key_stage(sm, ws, smem_raw, part, blk, w, page_bytes, lane);
         const uint32_t n_local = err == kErrNone ? ws->n_local : 0u;
         for (uint32_t k = lane; k < n_local; k += 32) {
             ws->gid[k] = wide_key_id(w, ws->dense[k]);
@@ -5282,14 +5435,26 @@ __global__ void __launch_bounds__(kWideWarps * 32) scan_keyed_wide_kernel(const 
 
 void launch_scan_keyed_wide(const ScanParams &p, const WideScanParams &w, int grid, cudaStream_t s) {
     const size_t smem = wide_smem_bytes();
-    cudaFuncSetAttribute(scan_keyed_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (p.total_blocks) scan_keyed_wide_kernel<<<grid, kWideWarps * 32, smem, s>>>(p, w);
+    cudaFuncSetAttribute(scan_keyed_wide_kernel<WideScanParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (p.total_blocks) scan_keyed_wide_kernel<WideScanParams><<<grid, kWideWarps * 32, smem, s>>>(p, w);
 }
 int scan_keyed_wide_ctas_per_sm() {
     const size_t smem = wide_smem_bytes();
-    cudaFuncSetAttribute(scan_keyed_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    cudaFuncSetAttribute(scan_keyed_wide_kernel<WideScanParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, scan_keyed_wide_kernel, kWideWarps * 32, smem) != cudaSuccess || n < 1) n = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, scan_keyed_wide_kernel<WideScanParams>, kWideWarps * 32, smem) != cudaSuccess || n < 1) n = 1;
+    return n;
+}
+void launch_scan_keys_wide(const ScanParams &p, const WideTupleParams &w, int grid, cudaStream_t s) {
+    const size_t smem = tuple_smem_bytes();
+    cudaFuncSetAttribute(scan_keyed_wide_kernel<WideTupleParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (p.total_blocks) scan_keyed_wide_kernel<WideTupleParams><<<grid, kWideWarps * 32, smem, s>>>(p, w);
+}
+int scan_keys_wide_ctas_per_sm() {
+    const size_t smem = tuple_smem_bytes();
+    cudaFuncSetAttribute(scan_keyed_wide_kernel<WideTupleParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, scan_keyed_wide_kernel<WideTupleParams>, kWideWarps * 32, smem) != cudaSuccess || n < 1) n = 1;
     return n;
 }
 

@@ -64,6 +64,7 @@ enum DevErr : uint32_t {
     kErrKeyLong = 13,       // per-row group key: a value longer than kMaxLit bytes
     kErrRankOverlap = 14,   // keyed collective: one series on two ranks over time spans that intersect
     kErrKeyBlock = 15,      // wide group key: a block whose key column holds more than kMaxBlockKeys distinct values
+    kErrTupleBlock = 16,    // tuple group key: a block holding more than kMaxBlockKeys distinct key tuples
 };
 constexpr int kOpEqOrNil = 7;  // internal predicate operator of the group-key passes: the cell is nil or equals the literal
 constexpr uint32_t kKeyAbsent = 0xffffffffu;  // Krow of a series that never shows the value (a block's first row is below it)
@@ -321,6 +322,32 @@ struct WideScanParams {
 // counters: rows_scanned, rows_matched, page_bytes, blocks)
 void launch_scan_keyed_wide(const ScanParams &p, const WideScanParams &w, int grid, cudaStream_t s);
 int scan_keyed_wide_ctas_per_sm();
+
+// ---- tuple group key (bydb_scan_agg_keys_wide): 2..kMaxKeyTags stored tags.  Every tag has a value table of its own (discovered by
+// launch_key_values_wide); a tuple is coded id_0 | id_1 << 16 | id_2 << 32 | id_3 << 48 from its values' ids and enters a table of
+// its own as an int64 key does (the all-zero code takes the zero flag).  A record's value id is then the tuple's id.
+constexpr uint32_t kMaxKeyTags = 4;
+struct WideTag {                  // a tag's value table, as WideScanParams names it
+    const unsigned long long *slots;
+    const uint32_t *slot_id;
+    uint32_t slot_mask;
+    uint16_t key_name;
+    uint8_t int64_key, pad;
+};
+struct WideTagSet {
+    WideTag tag[kMaxKeyTags];
+    uint32_t n_tags, pad;
+};
+// discovery of the tuples (one warp per selected block) and their numbering: w.k is the tuple table (int64 mode), w.rank /
+// w.n_by_rank as for one key, n_by_rank counting the block's distinct tuples
+void launch_key_tuples_wide(const WideKeyParams &w, const WideTagSet &tags, int grid, cudaStream_t s);
+// the scan with a tuple key: the WideScanParams name the tuple table (int64 mode)
+struct WideTupleParams : WideScanParams {
+    WideTagSet tags;
+};
+static_assert(sizeof(ScanParams) + sizeof(WideTupleParams) <= 4096 && sizeof(WideKeyParams) + sizeof(WideTagSet) <= 4096, "kernel-parameter space");
+void launch_scan_keys_wide(const ScanParams &p, const WideTupleParams &w, int grid, cudaStream_t s);
+int scan_keys_wide_ctas_per_sm();
 // the records folded into a partial table of the present composite groups (series group, value id) in insertion order
 struct WideReduceParams {
     const uint8_t *records;
