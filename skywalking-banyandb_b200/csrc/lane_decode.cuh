@@ -2,7 +2,7 @@
 //
 // Everything here is a plain function of one lane's registers (no shuffles, no shared memory), so the very same source is
 // also compiled for the host: tests/native/lane_decode_test.cc (and lane_switch_test.cc for swar_word2) runs it against a byte-at-a-time reference decoder
-// (full chunks, chunks with bytes outside the page, and the two-chain experiment) without a GPU.
+// (full chunks and chunks with bytes outside the page) without a GPU.
 #pragma once
 
 #include <cstdint>
@@ -309,75 +309,6 @@ BYDB_LANE_FN uint32_t swar_end(const SwarLane &s, int32_t &T, int32_t &Rp) {
     T = (s.T0 >> 1) + 64 * s.T1 + 8192 * s.T2;
     Rp = (s.R0 >> 1) + 64 * s.R1 + 8192 * s.R2;
     return static_cast<uint32_t>(s.nterm - 1) + ((s.base & 0xffu) - 1u);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Sparse masked decode (delta_page_sparse in scan_kernels.cu): when a row predicate / time range leaves most 64-byte lane
-// windows of a page without an active row, the warp first runs a LIGHT pass over every window -- the byte-linear sum T of the
-// SWAR decoder without the rank weights, the terminator count and the unfinished tail -- which is all that is needed to know
-// every window's first row and the value in front of it; only the windows that hold an active row are then decoded value by
-// value (fast_lane_decode, started from the previous window's tail), 32 of them at a time, one per lane.
-// ------------------------------------------------------------------------------------------------
-struct SwarLite {
-    int32_t T0, T1, T2;
-    uint32_t wide;
-    int32_t nterm;     // terminators seen so far in this lane
-    uint32_t prev_w;
-};
-BYDB_LANE_FN void swar_lite_begin(SwarLite &s, uint32_t prev_w) {
-    s.T0 = s.T1 = s.T2 = 0;
-    s.wide = 0;
-    s.nterm = 0;
-    s.prev_w = prev_w;
-}
-template <bool kMasked>
-BYDB_LANE_FN void swar_lite_word(SwarLite &s, uint32_t w_in, uint32_t vm) {
-    const uint32_t w = kMasked ? (w_in & vm) : w_in;
-    const uint32_t pw = s.prev_w;
-    const uint32_t p = w & 0x7f7f7f7fu;
-    const uint32_t M1 = lane_prmt(w, pw, 0xA98Fu);
-    const uint32_t M2 = lane_prmt(w, pw, 0x98FEu);
-    const uint32_t sb = imad_u32(w, 128u, 0u);
-    const uint32_t psb = imad_u32(pw, 128u, 0u);
-    const uint32_t S0 = lane_prmt(sb, 0u, 0xBA98u);
-    const uint32_t S1 = lane_prmt(sb, psb, 0xA98Fu);
-    const uint32_t S2 = lane_prmt(sb, psb, 0x98FEu);
-    const uint32_t S12 = (M2 & S2) | (~M2 & S1);
-    const uint32_t x0 = (p ^ S0) & ~M1;
-    const uint32_t p1 = p & M1 & ~M2;
-    const uint32_t q2 = w & M1 & M2;
-    const uint32_t wT = S12 | 0x01010101u;
-    uint32_t t01 = ~mulhi_u32(w, 1u << 25) & 0x01010101u;
-    if (kMasked) t01 &= vm;
-    s.nterm = dp4a_su(0x01010101u, t01, s.nterm);
-    s.T0 = dp4a_su(x0, 0x01010101u, s.T0);
-    s.T1 = dp4a_us(p1, wT, s.T1);
-    s.T2 = dp4a_us(q2, wT, s.T2);
-    s.wide |= q2;
-    s.prev_w = w;
-}
-BYDB_LANE_FN uint32_t swar_lite_end(const SwarLite &s, int32_t &T) {
-    T = (s.T0 >> 1) + 64 * s.T1 + 8192 * s.T2;
-    return static_cast<uint32_t>(s.nterm);
-}
-// The unfinished varint at the end of a lane (narrow pages: at most its first two bytes), from the lane's last word as the
-// decoder saw it (bytes outside the page zeroed): payload bits gathered so far, their count (0 / 7 / 14), and what those
-// bytes contributed to the lane's byte-linear sum T -- so that  T + pv(previous lane) - pv(this lane)  is the sum of the
-// deltas of the values that END in this lane.
-BYDB_LANE_FN void swar_tail(uint32_t lw, uint32_t &accv, uint32_t &sh, int32_t &pv) {
-    const uint32_t b3 = lw >> 24, b2 = (lw >> 16) & 0xffu;
-    accv = 0;
-    sh = 0;
-    pv = 0;
-    if (b3 & 0x80u) {
-        const bool two = (b2 & 0x80u) != 0;
-        const uint32_t p0 = (two ? b2 : b3) & 0x7fu;
-        const uint32_t p1 = two ? (b3 & 0x7fu) : 0u;
-        accv = p0 | (p1 << 7);
-        sh = two ? 14u : 7u;
-        const int32_t mag = static_cast<int32_t>((p0 >> 1) + (p0 & 1u) + 64u * p1);
-        pv = (p0 & 1u) ? -mag : mag;
-    }
 }
 
 // ------------------------------------------------------------------------------------------------

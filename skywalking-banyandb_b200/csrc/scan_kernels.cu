@@ -63,8 +63,6 @@ __device__ __forceinline__ void tma_load_1d(void *dst, const void *src, uint32_t
 // ------------------------------------------------------------------------------------------------
 // per-warp shared memory
 // ------------------------------------------------------------------------------------------------
-constexpr int kSparseQueue = BYDB_SPARSE ? 64 : 1;  // at most 32 windows of the previous chunk + 32 of the current one
-
 struct __align__(128) WarpSmem {
     uint8_t stage[kStages][kStageBytes];
     uint64_t bar[kStages];
@@ -88,10 +86,6 @@ struct __align__(128) WarpSmem {
     // the warp's statistics (lane 0 only), flushed to the query's counters once when the warp runs out of work
     unsigned long long st_rows, st_matched, st_bytes;
     uint32_t st_blocks, st_deferred, st_why, pad2;
-    // delta_page_sparse: the lane windows that hold an active row, waiting to be decoded 32 at a time
-    unsigned long long q_desc[kSparseQueue];  // ring offset | valid range | tail of the previous window (see sparse_desc)
-    long long q_base[kSparseQueue];           // value in front of the window's first ending value
-    unsigned long long q_aw[kSparseQueue];    // bit i = the i-th value that ends in the window is an active row
 };
 
 size_t scan_smem_bytes() { return sizeof(WarpSmem) * kWarpsPerCta; }
@@ -702,6 +696,7 @@ struct SwarChunk {
 // counts, 64-bit multiply-add, stage bookkeeping: ~160 instructions) is paid once per 16 words instead of once per 8.
 constexpr uint32_t kSwarLaneBytes = 64;
 constexpr uint32_t kSwarChunkBytes = 32 * kSwarLaneBytes;
+// delta_page_sum_all and delta_page_sum_masked wait for a stage at its first chunk and release it after its last one
 static_assert(kStageBytes % kSwarChunkBytes == 0, "a TMA stage holds whole SWAR chunks");
 // kClasses: 2 = swar_word2 (wide: a varint of 3+ bytes), 3 = swar_word (wide: a varint of 4+ bytes)
 template <int kClasses, bool kMasked>
@@ -975,252 +970,6 @@ __device__ __noinline__ int delta_page_sum_masked(WarpSmem *sm, int lane) {
     publish_acc(sm, acc, lane);
     last_byte = __shfl_sync(0xffffffffu, last_byte, 0);
     return (tb + 1 == count && last_byte < 0x80u) ? 0 : 2;
-}
-
-// ------------------------------------------------------------------------------------------------
-// Sparse masked decode of an EncodeTypeDelta page (row predicate and / or time range, narrow deltas): the selective pass.
-// With a dictionary predicate that keeps one row in eight, in runs, two thirds of the 64-byte lane windows of a field page hold
-// no active row at all; the serial decoder (delta_page_fast) still walks every byte of every window because the next window's
-// values depend on them.  Here every 2 KB chunk first goes through the LIGHT SWAR pass (lane_decode.cuh: swar_lite_word --
-// terminator count, byte-linear delta sum, unfinished tail; no per-value work), two warp scans turn that into each window's
-// first row and the value in front of it, and only windows with an active row are queued (shared memory: ring offset, base
-// value, 64 active bits, the previous window's tail).  When 32 windows are queued -- or the oldest queued chunk has to leave
-// the TMA ring -- every lane decodes ONE queued window value by value.  Windows wait at most one chunk: the stage of chunk
-// c-1 is handed back to the ring after chunk c's light pass, so the ring needs kStages >= 2 (3 keeps a copy in flight).
-// Returns like delta_page_fast.
-// ------------------------------------------------------------------------------------------------
-static_assert(kStageBytes == kSwarChunkBytes || kStageBytes % kSwarChunkBytes == 0, "a TMA stage holds whole chunks");
-
-__device__ __forceinline__ unsigned long long sparse_desc(uint32_t off, uint32_t lo, uint32_t hi, uint32_t sh, uint32_t accv) {
-    return static_cast<unsigned long long>(off) | (static_cast<unsigned long long>(lo) << 16) | (static_cast<unsigned long long>(hi) << 24) |
-           (static_cast<unsigned long long>(sh) << 32) | (static_cast<unsigned long long>(accv) << 40);
-}
-
-template <int kNeed>
-__device__ __forceinline__ void sparse_flush(WarpSmem *sm, uint32_t m, uint32_t &qn, AggAcc &acc, int lane) {
-    __syncwarp();
-    const bool mine = static_cast<uint32_t>(lane) < m;
-    unsigned long long d = 0, aw = 0;
-    long long base = 0;
-    if (mine) {
-        d = sm->q_desc[lane];
-        aw = sm->q_aw[lane];
-        base = sm->q_base[lane];
-    }
-    const uint32_t lo = static_cast<uint32_t>(d >> 16) & 0xffu, hi = static_cast<uint32_t>(d >> 24) & 0xffu;
-    if (mine) {
-        const uint8_t *src = &sm->stage[0][0] + (static_cast<uint32_t>(d) & 0xffffu);
-        uint32_t accv = static_cast<uint32_t>(d >> 40) & 0x3fffu, sh = static_cast<uint32_t>(d >> 32) & 0xffu;
-        int32_t P = 0, sumP = 0, minP = INT32_MAX, maxP = INT32_MIN;
-        unsigned long long a = aw;
-#pragma unroll 1
-        for (int h = 0; h < 2; ++h) {
-            const uint4 wa = *reinterpret_cast<const uint4 *>(src + 32 * h), wb = *reinterpret_cast<const uint4 *>(src + 32 * h + 16);
-            const int l2 = static_cast<int>(lo) - 32 * h, h2 = static_cast<int>(hi) - 32 * h;
-            const uint32_t valid = low_bits(h2 < 0 ? 0 : (h2 > 32 ? 32 : h2)) & ~low_bits(l2 < 0 ? 0 : (l2 > 32 ? 32 : l2));
-            uint32_t msb = msb4(wa.x);
-            msb = imad_u32(msb4(wa.y), 1u << 4, msb);
-            msb = imad_u32(msb4(wa.z), 1u << 8, msb);
-            msb = imad_u32(msb4(wa.w), 1u << 12, msb);
-            msb = imad_u32(msb4(wb.x), 1u << 16, msb);
-            msb = imad_u32(msb4(wb.y), 1u << 20, msb);
-            msb = imad_u32(msb4(wb.z), 1u << 24, msb);
-            msb = imad_u32(msb4(wb.w), 1u << 28, msb);
-            const uint32_t term = valid & ~msb;
-            const uint32_t nh = __popc(term);
-            const uint32_t a32 = static_cast<uint32_t>(a) & low_bits(nh);
-            // one decode variant (the masked one) for interior and edge windows alike: code size, see delta_page_sparse
-            fast_lane_decode<false, kNeed>(wa, wb, valid, term, a32, accv, sh, P, sumP, minP, maxP);
-            a = nh >= 32 ? (a >> 16) >> 16 : (a >> nh);
-        }
-        const uint32_t cntA = static_cast<uint32_t>(__popcll(aw));
-        if (kNeed & kNeedSum) {
-            acc.add_scaled(base, cntA);
-            const int64_t sp = sumP;
-            const uint64_t usp = static_cast<uint64_t>(sp);
-            acc.lo += usp;
-            acc.hi += (sp >> 63) + (acc.lo < usp ? 1 : 0);
-        }
-        if (kNeed & kNeedMinMax) {
-            const int64_t vmin = base + minP, vmax = base + maxP;
-            acc.mn = vmin < acc.mn ? vmin : acc.mn;
-            acc.mx = vmax > acc.mx ? vmax : acc.mx;
-        }
-        acc.cnt += cntA;
-    }
-    // the rest of the queue moves to the front
-    const uint32_t rest = qn - m;
-    unsigned long long rd = 0, ra = 0;
-    long long rb = 0;
-    if (static_cast<uint32_t>(lane) < rest) {
-        rd = sm->q_desc[m + lane];
-        ra = sm->q_aw[m + lane];
-        rb = sm->q_base[m + lane];
-    }
-    __syncwarp();
-    if (static_cast<uint32_t>(lane) < rest) {
-        sm->q_desc[lane] = rd;
-        sm->q_aw[lane] = ra;
-        sm->q_base[lane] = rb;
-    }
-    qn = rest;
-    __syncwarp();
-}
-
-template <int kMode, int kNeed>
-__device__ __noinline__ int delta_page_sparse(WarpSmem *sm, int lane) {
-    static_assert(kMode != kRowsAll, "every row active: delta_page_sum_all / delta_page_fast");
-    const uint8_t *body = sm->a_body;
-    const uint32_t len = sm->a_len, count = sm->a_count, r0 = sm->a_r0, r1 = sm->a_r1;
-    const int64_t first = sm->a_first;
-    AggAcc acc;
-    acc.init();
-    if (lane == 0) {
-        bool a = true;
-        if (kMode == kRowsRange) a = r0 == 0;
-        if (kMode == kRowsMask) a = sm->mask[0] & 1u;
-        if (a) acc.add(first);
-    }
-    if (len == 0) {
-        publish_acc(sm, acc, lane);
-        return count == 1 ? 0 : 2;
-    }
-    PageStream st;
-    stream_open(st, sm, body, len, lane);
-    const uint32_t nchunks = (st.total + kSwarChunkBytes - 1) / kSwarChunkBytes;
-    constexpr uint32_t kChunksPerStage = kStageBytes / kSwarChunkBytes;
-    int64_t V0 = first;
-    uint32_t row_base = 1, carry_w = 0, carry_acc = 0, carry_sh = 0;
-    int32_t carry_pv = 0;
-    uint32_t qn = 0;
-    const uint8_t *buf = nullptr;
-    for (uint32_t c = 0; c < nchunks; ++c) {
-        const uint32_t k = c / kChunksPerStage;
-        if ((c % kChunksPerStage) == 0) buf = stream_wait(st, sm, k);
-        // ---- light pass over the lane's 64 bytes
-        const uint32_t o = c * kSwarChunkBytes + lane * kSwarLaneBytes;
-        const bool interior = c * kSwarChunkBytes >= st.pstart && (c + 1) * kSwarChunkBytes <= st.pend;  // warp-uniform
-        const uint8_t *src = buf + (o % kStageBytes);
-        int lo_i = static_cast<int>(st.pstart) - static_cast<int>(o);
-        int hi_i = static_cast<int>(st.pend) - static_cast<int>(o);
-        lo_i = lo_i < 0 ? 0 : (lo_i > 64 ? 64 : lo_i);
-        hi_i = hi_i < 0 ? 0 : (hi_i > 64 ? 64 : hi_i);
-        SwarLite sl;
-        uint32_t lastw;
-        // the word loops stay ROLLED (4 words per trip): unrolled, the two light passes and the two decode variants of one
-        // instantiation are ~25 KB of hot code, and a query with two aggregated fields runs two instantiations: the warps then
-        // stall on instruction fetch
-        if (interior) {
-            lastw = *reinterpret_cast<const uint32_t *>(src + kSwarLaneBytes - 4);
-            uint32_t pw = __shfl_up_sync(0xffffffffu, lastw, 1);
-            if (lane == 0) pw = carry_w;
-            swar_lite_begin(sl, pw);
-#pragma unroll 1
-            for (int q = 0; q < 4; ++q) {
-                const uint4 w = *reinterpret_cast<const uint4 *>(src + 16 * q);
-                swar_lite_word<false>(sl, w.x, 0u);
-                swar_lite_word<false>(sl, w.y, 0u);
-                swar_lite_word<false>(sl, w.z, 0u);
-                swar_lite_word<false>(sl, w.w, 0u);
-            }
-        } else {
-            const uint32_t va = low_bits(hi_i > 32 ? 32 : hi_i) & ~low_bits(lo_i > 32 ? 32 : lo_i);
-            const uint32_t vb = low_bits(hi_i > 32 ? hi_i - 32 : 0) & ~low_bits(lo_i > 32 ? lo_i - 32 : 0);
-            lastw = 0;
-            if (o + 48 < st.total) lastw = *reinterpret_cast<const uint32_t *>(src + kSwarLaneBytes - 4) & expand4(vb >> 28);
-            uint32_t pw = __shfl_up_sync(0xffffffffu, lastw, 1);
-            if (lane == 0) pw = carry_w;
-            swar_lite_begin(sl, pw);
-#pragma unroll 1
-            for (int q = 0; q < 4; ++q) {
-                uint4 w = make_uint4(0, 0, 0, 0);
-                if (o + 16 * q < st.total) w = *reinterpret_cast<const uint4 *>(src + 16 * q);
-                const uint32_t v = (q < 2 ? va : vb) >> (16 * (q & 1));
-                swar_lite_word<true>(sl, w.x, expand4(v));
-                swar_lite_word<true>(sl, w.y, expand4(v >> 4));
-                swar_lite_word<true>(sl, w.z, expand4(v >> 8));
-                swar_lite_word<true>(sl, w.w, expand4(v >> 12));
-            }
-        }
-        carry_w = __shfl_sync(0xffffffffu, lastw, 31);
-        if (__any_sync(0xffffffffu, (sl.wide & 0x80808080u) != 0)) {
-            // a varint of four or more bytes: the general decoder takes the page.  Stages issued so far: the initial kStages
-            // plus one per stage handed back (all stages before k - 1)
-            const uint32_t kk = k > 0 ? k - 1 : 0;
-            stream_drain(st, sm, kk);
-            if (lane == 0) sm->seq = st.seq0 + min(st.nstages, kk + static_cast<uint32_t>(kStages));
-            __syncwarp();
-            return 1;
-        }
-        int32_t T;
-        const uint32_t n = swar_lite_end(sl, T);
-        uint32_t t_acc, t_sh;
-        int32_t t_pv;
-        swar_tail(lastw, t_acc, t_sh, t_pv);
-        uint32_t in_acc = __shfl_up_sync(0xffffffffu, t_acc, 1), in_sh = __shfl_up_sync(0xffffffffu, t_sh, 1);
-        int32_t in_pv = __shfl_up_sync(0xffffffffu, t_pv, 1);
-        if (lane == 0) {
-            in_acc = carry_acc;
-            in_sh = carry_sh;
-            in_pv = carry_pv;
-        }
-        carry_acc = __shfl_sync(0xffffffffu, t_acc, 31);
-        carry_sh = __shfl_sync(0xffffffffu, t_sh, 31);
-        carry_pv = __shfl_sync(0xffffffffu, t_pv, 31);
-        const int32_t P = T + in_pv - t_pv;  // deltas of the values that END in this window
-        uint32_t n_in = n;
-        int32_t p_in = P;
-#pragma unroll
-        for (int sft = 1; sft < 32; sft <<= 1) {
-            const uint32_t on = __shfl_up_sync(0xffffffffu, n_in, sft);
-            const int32_t op = __shfl_up_sync(0xffffffffu, p_in, sft);
-            if (lane >= sft) {
-                n_in += on;
-                p_in += op;
-            }
-        }
-        const uint32_t row0 = row_base + n_in - n;
-        unsigned long long aw;
-        const unsigned long long nbits = n >= 64 ? ~0ull : ((1ull << n) - 1ull);
-        if (kMode == kRowsRange) {
-            const uint32_t a = r0 > row0 ? min(r0 - row0, 64u) : 0u;
-            const uint32_t b = r1 + 1u > row0 ? min(r1 + 1u - row0, 64u) : 0u;
-            const unsigned long long mb = b >= 64 ? ~0ull : ((1ull << b) - 1ull), ma = a >= 64 ? ~0ull : ((1ull << a) - 1ull);
-            aw = mb & ~ma & nbits;
-        } else {
-            // a corrupt page can hold more varints than the block has rows: never index past the mask
-            const uint32_t wi = min(row0 >> 5, static_cast<uint32_t>(kMaskWords));
-            const uint32_t m0 = sm->mask[wi], m1 = sm->mask[wi + 1], m2 = sm->mask[wi + 2];
-            const uint32_t sft = row0 & 31u;
-            aw = (static_cast<unsigned long long>(__funnelshift_r(m1, m2, sft)) << 32 | __funnelshift_r(m0, m1, sft)) & nbits;
-        }
-        // ---- queue the windows that hold an active row
-        const bool act = aw != 0;
-        const uint32_t bal = __ballot_sync(0xffffffffu, act);
-        const uint32_t q_old = qn;  // everything queued so far belongs to the previous chunk
-        if (act) {
-            const uint32_t pos = qn + __popc(bal & ((1u << lane) - 1u));
-            sm->q_desc[pos] = sparse_desc(static_cast<uint32_t>(src - &sm->stage[0][0]), static_cast<uint32_t>(lo_i), static_cast<uint32_t>(hi_i), in_sh, in_acc);
-            sm->q_base[pos] = V0 + static_cast<int64_t>(p_in - P);
-            sm->q_aw[pos] = aw;
-        }
-        qn += __popc(bal);
-        V0 += static_cast<int64_t>(__shfl_sync(0xffffffffu, p_in, 31));
-        row_base += __shfl_sync(0xffffffffu, n_in, 31);
-        const bool stage_done = (c % kChunksPerStage) == kChunksPerStage - 1 || c == nchunks - 1;
-        const bool last = c == nchunks - 1;
-        // ---- decode: whenever 32 windows wait, and what is left of the previous stage before that stage goes back to the ring
-        uint32_t old = q_old;
-        while (qn >= 32u || (stage_done && old > 0u) || (last && qn > 0u)) {
-            const uint32_t m = qn < 32u ? qn : 32u;
-            sparse_flush<kNeed>(sm, m, qn, acc, lane);
-            old = old > m ? old - m : 0u;
-        }
-        if (stage_done && k > 0) stream_release(st, sm, k - 1, lane);
-        if (last) stream_release(st, sm, k, lane);
-    }
-    publish_acc(sm, acc, lane);
-    return (row_base == count && carry_sh == 0) ? 0 : 2;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1905,17 +1654,6 @@ __device__ __forceinline__ int masked_sum_dispatch(WarpSmem *sm, int lane) {
     else return delta_page_sum_masked<kMode>(sm, lane);
 }
 
-template <int kMode>
-__device__ __forceinline__ int sparse_dispatch(WarpSmem *sm, uint32_t need, int lane) {
-    if constexpr (kMode == kRowsAll) {
-        return 2;  // not reached: every-row pages take delta_page_sum_all / delta_page_fast
-    } else {
-        if (need == kNeedSum) return delta_page_sparse<kMode, kNeedSum>(sm, lane);
-        if (need == kNeedMinMax) return delta_page_sparse<kMode, kNeedMinMax>(sm, lane);
-        return delta_page_sparse<kMode, kNeedSum | kNeedMinMax>(sm, lane);
-    }
-}
-
 template <int kMode, bool kFastLane>
 // Out of line (one copy per row mode), arguments and result through the warp's shared-memory slots: the block loop of the
 // scan kernel then keeps only its own few values live across the call instead of spilling around an inlined decoder.
@@ -1972,8 +1710,7 @@ __device__ __noinline__ uint32_t agg_field_page(WarpSmem *sm, int lane) {
         __syncwarp();
         if (enc == 3) {
             if (need == kNeedSum && kMode == kRowsAll) rc = delta_page_sum_all(sm, lane);
-            else if (need == kNeedSum && kMode != kRowsAll && kFastLane && BYDB_MASKED_SWAR) rc = masked_sum_dispatch<kMode>(sm, lane);
-            else if (kMode != kRowsAll && kFastLane && BYDB_SPARSE) rc = sparse_dispatch<kMode>(sm, need, lane);
+            else if (need == kNeedSum && kMode != kRowsAll && kFastLane) rc = masked_sum_dispatch<kMode>(sm, lane);
             else if (need == kNeedSum) rc = delta_page_fast<kMode, kNeedSum>(sm, lane);
             else if (need == kNeedMinMax) rc = delta_page_fast<kMode, kNeedMinMax>(sm, lane);
             else rc = delta_page_fast<kMode, kNeedSum | kNeedMinMax>(sm, lane);

@@ -28,12 +28,6 @@ constexpr int kWarpsPerCta = 8;          // 256 threads; every warp is an indepe
 #ifndef BYDB_EXPRESS_DECODE
 #define BYDB_EXPRESS_DECODE 1            // 0: the express lane streams its pages and skips the decode (fetch timing only: WRONG sums)
 #endif
-#ifndef BYDB_SPARSE
-#define BYDB_SPARSE 0                    // 1: masked / ranged delta pages take delta_page_sparse (measured slower, see DESIGN.md 4.2; make variant EXTRA="-DBYDB_SPARSE=1 -DBYDB_STAGES=3")
-#endif
-#ifndef BYDB_MASKED_SWAR
-#define BYDB_MASKED_SWAR 1               // 0: masked / ranged SUM pages keep the serial decoder (A/B timing)
-#endif
 #ifndef BYDB_FAST_CTAS
 #define BYDB_FAST_CTAS 3                 // resident CTAs per SM the fast lane is compiled for (register cap 65536 / (256 x n))
 #endif

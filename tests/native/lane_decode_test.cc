@@ -47,7 +47,7 @@ static Ref reference(const uint8_t *b, uint32_t valid, uint32_t aw) {
 }
 
 template <bool kFull, int kNeed>
-static bool check(const uint8_t *b, uint32_t valid, uint32_t aw, bool dual) {
+static bool check(const uint8_t *b, uint32_t valid, uint32_t aw) {
     uint4 wa, wb;
     uint32_t w[8];
     for (int k = 0; k < 8; ++k) w[k] = b[4 * k] | (b[4 * k + 1] << 8) | (b[4 * k + 2] << 16) | (static_cast<uint32_t>(b[4 * k + 3]) << 24);
@@ -58,14 +58,13 @@ static bool check(const uint8_t *b, uint32_t valid, uint32_t aw, bool dual) {
     const uint32_t term = valid & ~msb;
     uint32_t accv = 0, sh = 0;
     int32_t P = 0, sumP = 0, minP = INT32_MAX, maxP = INT32_MIN;
-    (void)dual;
     fast_lane_decode<kFull, kNeed>(wa, wb, valid, term, aw, accv, sh, P, sumP, minP, maxP);
     const Ref r = reference(b, valid, aw);
     bool ok = accv == r.accv && sh == r.sh && P == r.P;
     if (kNeed & kNeedSum) ok = ok && sumP == r.sumP;
     if (kNeed & kNeedMinMax) ok = ok && minP == r.minP && maxP == r.maxP;
     if (!ok)
-        std::printf("FAIL full=%d need=%d dual=%d valid=%08x aw=%08x: got (%u,%u,%d,%d,%d,%d) want (%u,%u,%d,%d,%d,%d)\n", kFull, kNeed, dual, valid, aw,
+        std::printf("FAIL full=%d need=%d valid=%08x aw=%08x: got (%u,%u,%d,%d,%d,%d) want (%u,%u,%d,%d,%d,%d)\n", kFull, kNeed, valid, aw,
                     accv, sh, P, sumP, minP, maxP, r.accv, r.sh, r.P, r.sumP, r.minP, r.maxP);
     return ok;
 }
@@ -161,148 +160,6 @@ static bool swar_page_check(std::mt19937_64 &rng, int n_values, int max_len) {
     if (tb != static_cast<uint32_t>(n_values) || S != want) {
         std::printf("FAIL swar page: n_values=%d pstart=%u terminators=%u S=%lld want=%lld\n", n_values, pstart, tb, static_cast<long long>(S),
                     static_cast<long long>(want));
-        return false;
-    }
-    return true;
-}
-
-// ---- sparse masked decode (swar_lite_* / swar_tail + fast_lane_decode per active window): a page emulated the way
-// delta_page_sparse walks it -- light pass over every 64-byte window (terminators n, deltas of the values ending in it P, tail),
-// scans of n and P over the lanes, then only the windows with an active row decoded from the previous window's tail --
-// against the plain definition of the masked sum / min / max / count.
-static bool sparse_page_check(std::mt19937_64 &rng, int n_values, int density_pct) {
-    std::vector<int64_t> d;
-    const uint32_t pstart = static_cast<uint32_t>(rng() % 16);
-    std::vector<uint8_t> win(pstart);
-    for (auto &x : win) x = static_cast<uint8_t>(rng());
-    for (int i = 0; i < n_values; ++i) {
-        const int L = 1 + static_cast<int>(rng() % 3);
-        uint32_t u = static_cast<uint32_t>(rng()) & ((1u << (7 * L)) - 1u);
-        if (L > 1 && (u >> (7 * (L - 1))) == 0) u |= 1u << (7 * (L - 1));
-        if (rng() % 7 == 0) u &= ~0x3f80u;
-        if (L > 1 && (u >> (7 * (L - 1))) == 0) u |= 1u << (7 * (L - 1));
-        d.push_back(zz(u));
-        for (int k = 0; k < L; ++k) win.push_back(static_cast<uint8_t>(((u >> (7 * k)) & 0x7f) | (k < L - 1 ? 0x80 : 0)));
-    }
-    const uint32_t pend = static_cast<uint32_t>(win.size());
-    while (win.size() % 16) win.push_back(static_cast<uint8_t>(rng()));
-    const uint32_t total = static_cast<uint32_t>(win.size());
-    win.resize(win.size() + 2048, 0xAB);
-    // active rows: runs, like a dictionary predicate leaves them (row 0 is the page's first value, rows 1.. the deltas)
-    const int64_t first = static_cast<int64_t>(rng() % 2000001) - 1000000;
-    std::vector<uint8_t> act(n_values + 1 + 128, 0);
-    for (size_t r = 0; r < static_cast<size_t>(n_values) + 1;) {
-        const size_t run = 1 + rng() % 40;
-        const bool on = static_cast<int>(rng() % 100) < density_pct;
-        for (size_t k = 0; k < run && r < static_cast<size_t>(n_values) + 1; ++k) act[r++] = on;
-    }
-    // reference
-    int64_t want_sum = 0, want_cnt = 0, want_min = INT64_MAX, want_max = INT64_MIN, v = first;
-    for (int r = 0; r <= n_values; ++r) {
-        if (r > 0) v += d[r - 1];
-        if (act[r]) {
-            want_sum += v;
-            want_cnt++;
-            want_min = v < want_min ? v : want_min;
-            want_max = v > want_max ? v : want_max;
-        }
-    }
-    // emulation
-    int64_t sum = 0, cnt = 0, mn = INT64_MAX, mx = INT64_MIN;
-    if (act[0]) sum += first, cnt++, mn = first, mx = first;
-    int64_t V0 = first;
-    uint32_t row_base = 1, carry_w = 0, carry_acc = 0, carry_sh = 0;
-    int32_t carry_pv = 0;
-    const uint32_t nchunks = (total + 2047) / 2048;
-    for (uint32_t c = 0; c < nchunks; ++c) {
-        const bool interior = c * 2048 >= pstart && (c + 1) * 2048 <= pend;
-        uint32_t nl[32], lastw[32], ta[32], ts[32];
-        int32_t T[32], tp[32];
-        for (int lane = 0; lane < 32; ++lane) {
-            const uint32_t o = c * 2048 + lane * 64;
-            uint32_t w[16];
-            for (int k = 0; k < 16; ++k) {
-                w[k] = 0;
-                if (o + 4 * k < total) memcpy(&w[k], &win[o + 4 * k], 4);
-            }
-            int lo_i = static_cast<int>(pstart) - static_cast<int>(o), hi_i = static_cast<int>(pend) - static_cast<int>(o);
-            lo_i = lo_i < 0 ? 0 : (lo_i > 64 ? 64 : lo_i);
-            hi_i = hi_i < 0 ? 0 : (hi_i > 64 ? 64 : hi_i);
-            const uint64_t valid = (hi_i >= 64 ? ~0ull : ((1ull << hi_i) - 1ull)) & ~(lo_i >= 64 ? ~0ull : ((1ull << lo_i) - 1ull));
-            SwarLite sl;
-            swar_lite_begin(sl, lane == 0 ? carry_w : lastw[lane - 1]);
-            for (int k = 0; k < 16; ++k) {
-                if (interior) swar_lite_word<false>(sl, w[k], 0xffffffffu);
-                else swar_lite_word<true>(sl, w[k], expand4(static_cast<uint32_t>(valid >> (4 * k))));
-            }
-            lastw[lane] = sl.prev_w;
-            nl[lane] = swar_lite_end(sl, T[lane]);
-            if ((sl.wide & 0x80808080u) != 0) {
-                std::printf("FAIL sparse: narrow page flagged wide\n");
-                return false;
-            }
-            swar_tail(lastw[lane], ta[lane], ts[lane], tp[lane]);
-        }
-        uint32_t lb = 0;
-        int64_t pb = 0;
-        for (int lane = 0; lane < 32; ++lane) {
-            const uint32_t acc_in = lane == 0 ? carry_acc : ta[lane - 1], sh_in = lane == 0 ? carry_sh : ts[lane - 1];
-            const int32_t pv_in = lane == 0 ? carry_pv : tp[lane - 1];
-            const int32_t P = T[lane] + pv_in - tp[lane];
-            const int64_t base = V0 + pb;
-            const uint32_t row0 = row_base + lb, n = nl[lane];
-            uint64_t aw = 0;
-            for (uint32_t i = 0; i < n && i < 64; ++i) aw |= static_cast<uint64_t>(act[row0 + i]) << i;
-            if (aw) {
-                // phase 2: the window decoded in two 32-byte halves from the previous lane's tail
-                const uint32_t o = c * 2048 + lane * 64;
-                int lo_i = static_cast<int>(pstart) - static_cast<int>(o), hi_i = static_cast<int>(pend) - static_cast<int>(o);
-                lo_i = lo_i < 0 ? 0 : (lo_i > 64 ? 64 : lo_i);
-                hi_i = hi_i < 0 ? 0 : (hi_i > 64 ? 64 : hi_i);
-                uint32_t accv = acc_in, sh = sh_in;
-                int32_t Pl = 0, sumP = 0, minP = INT32_MAX, maxP = INT32_MIN;
-                uint64_t a = aw;
-                for (int h = 0; h < 2; ++h) {
-                    uint32_t ww[8];
-                    for (int k = 0; k < 8; ++k) {
-                        ww[k] = 0;
-                        if (o + 32 * h + 4 * k < total) memcpy(&ww[k], &win[o + 32 * h + 4 * k], 4);
-                    }
-                    const uint4 wa = make_uint4(ww[0], ww[1], ww[2], ww[3]), wb = make_uint4(ww[4], ww[5], ww[6], ww[7]);
-                    const int l2 = lo_i - 32 * h, h2 = hi_i - 32 * h;
-                    const uint32_t valid = low_bits(h2 < 0 ? 0 : (h2 > 32 ? 32 : h2)) & ~low_bits(l2 < 0 ? 0 : (l2 > 32 ? 32 : l2));
-                    uint32_t msb = 0;
-                    for (int k = 0; k < 8; ++k) msb |= msb4(ww[k]) << (4 * k);
-                    const uint32_t term = valid & ~msb;
-                    const uint32_t nh = lane_popc(term);
-                    const uint32_t a32 = static_cast<uint32_t>(a) & low_bits(nh);
-                    if (valid == 0xffffffffu) fast_lane_decode<true, kNeedSum | kNeedMinMax>(wa, wb, valid, term, a32, accv, sh, Pl, sumP, minP, maxP);
-                    else fast_lane_decode<false, kNeedSum | kNeedMinMax>(wa, wb, valid, term, a32, accv, sh, Pl, sumP, minP, maxP);
-                    a = nh >= 64 ? 0 : (a >> nh);
-                }
-                if (Pl != P) {
-                    std::printf("FAIL sparse: window prefix %d vs light pass %d (chunk %u lane %d)\n", Pl, P, c, lane);
-                    return false;
-                }
-                const int64_t ca = __builtin_popcountll(aw);
-                sum += base * ca + sumP;
-                cnt += ca;
-                mn = base + minP < mn ? base + minP : mn;
-                mx = base + maxP > mx ? base + maxP : mx;
-            }
-            lb += n;
-            pb += P;
-        }
-        V0 += pb;
-        row_base += lb;
-        carry_w = lastw[31];
-        carry_acc = ta[31];
-        carry_sh = ts[31];
-        carry_pv = tp[31];
-    }
-    if (row_base != static_cast<uint32_t>(n_values) + 1 || carry_sh != 0 || sum != want_sum || cnt != want_cnt || (cnt && (mn != want_min || mx != want_max))) {
-        std::printf("FAIL sparse page: n_values=%d pstart=%u rows=%u sum=%lld want=%lld cnt=%lld want=%lld\n", n_values, pstart, row_base,
-                    static_cast<long long>(sum), static_cast<long long>(want_sum), static_cast<long long>(cnt), static_cast<long long>(want_cnt));
         return false;
     }
     return true;
@@ -421,12 +278,12 @@ int main() {
         }
         const uint8_t *b = s.data() + rng() % 4;
         const uint32_t aw = (rng() % 4 == 0) ? 0xffffffffu : (rng() % 5 == 0 ? 0u : static_cast<uint32_t>(rng()));
-        bool ok = check<true, kNeedSum>(b, 0xffffffffu, aw, false) && check<true, kNeedMinMax>(b, 0xffffffffu, aw, false) &&
-                  check<true, kNeedSum | kNeedMinMax>(b, 0xffffffffu, aw, false);
+        bool ok = check<true, kNeedSum>(b, 0xffffffffu, aw) && check<true, kNeedMinMax>(b, 0xffffffffu, aw) &&
+                  check<true, kNeedSum | kNeedMinMax>(b, 0xffffffffu, aw);
         // first / last chunk of a page: a contiguous valid window [lo, hi)
         const uint32_t lo = rng() % 33, hi = lo + rng() % (33 - lo);
         const uint32_t valid = (hi >= 32 ? 0xffffffffu : ((1u << hi) - 1u)) & ~(lo >= 32 ? 0xffffffffu : ((1u << lo) - 1u));
-        ok = ok && check<false, kNeedSum>(b, valid, aw, false) && check<false, kNeedSum | kNeedMinMax>(b, valid, aw, false);
+        ok = ok && check<false, kNeedSum>(b, valid, aw) && check<false, kNeedSum | kNeedMinMax>(b, valid, aw);
         if (!ok) return 1;
         n += 8;
     }
@@ -455,10 +312,6 @@ int main() {
         const int nv = it < 50 ? it : 1 + static_cast<int>(rng() % 9000);
         if (!swar_page_check(rng, nv, 3)) return 1;
         if (it % 10 == 0 && !swar_page_check(rng, nv, 4)) return 1;
-    }
-    for (int it = 0; it < 3000; ++it) {
-        const int nv = it < 50 ? it : 1 + static_cast<int>(rng() % 9000);
-        if (!sparse_page_check(rng, nv, it % 3 == 0 ? 12 : (it % 3 == 1 ? 50 : 100))) return 1;
     }
     for (int it = 0; it < 3000; ++it) {
         const int nv = it < 50 ? it : 1 + static_cast<int>(rng() % 9000);

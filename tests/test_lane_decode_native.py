@@ -1,6 +1,7 @@
 """The per-lane fast decoders of the scan kernel (skywalking-banyandb_b200/csrc/lane_decode.cuh) are plain functions of one lane's
 registers and compile for the host: tests/native/lane_decode_test.cc runs them (multiply-add formulation, masked chunks, the
-two-chain experiment, the head correction) against a byte-at-a-time reference on 200k random windows.  No GPU."""
+head correction) against a byte-at-a-time reference on 200k random windows, and the SWAR sum decoders (all rows, row mask) over
+whole emulated pages against the plain sum.  No GPU."""
 import os
 import shutil
 import subprocess
