@@ -2377,6 +2377,12 @@ struct WidePass {
 // 1. discovery, on the slot's stream, synchronised: the value table (S slots), each selected block's rank and distinct values,
 // then their exclusive scan (each block's first record; R their sum), and the values read back.  A tuple key (n_keys > 1) has a
 // table per tag, then one of the tuples, whose kernel writes the blocks' distinct tuples; all tables share the cap.
+// wide_discover_pinned: its page-locked staging, the series' ids and groups going up or the largest read-back coming back.
+static size_t wide_discover_pinned(size_t NS, uint32_t n_keys, uint32_t cap) {
+    const size_t nt = n_keys == 1 ? 1 : n_keys + 1;
+    const size_t back_max = 32 * nt + (nt > 1 ? (nt - 1) * static_cast<size_t>(cap) * (kMaxLit + 4) + static_cast<size_t>(cap) * 8 : static_cast<size_t>(cap) * (kMaxLit + 4));
+    return std::max<size_t>(NS * 12, back_max) + 256;
+}
 int wide_discover(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *keys, uint32_t n_keys, uint32_t cap, const Plan &plan, ExecSlot &slot,
                   bydb_stats &stats, WidePass &w) {
     cudaStream_t stream = slot.stream;
@@ -2400,8 +2406,7 @@ int wide_discover(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *keys
     Scratch &ka = w.ka;
     CUDA_TRY(ka.alloc(carve.o, stream));
     w.disc_bytes = carve.o;
-    const size_t back_max = 32 * nt + (nt > 1 ? (nt - 1) * static_cast<size_t>(cap) * (kMaxLit + 4) + static_cast<size_t>(cap) * 8 : static_cast<size_t>(cap) * (kMaxLit + 4));
-    if (slot.ensure_pinned(std::max<size_t>(NS * 12, back_max) + 256)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+    if (slot.ensure_pinned(wide_discover_pinned(NS, n_keys, cap))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
     WideKeyParams wks[kMaxKeyTags + 1];
     for (size_t t = 0; t < nt; ++t) {
         WideKeyParams &wk = wks[t];
@@ -4464,6 +4469,40 @@ static uint64_t keyed_fingerprint(const bydb_query *q, const bydb_group_key *key
 // the slot of a rank of a keyed collective that found V key values
 static KeyedSlot keyed_slot(const Plan &plan, size_t V) { return KeyedSlot(plan.tl.G, plan.tl.F, plan.n_series, V); }
 
+// A rank's slot head (SlotHead) in either keyed collective: fingerprint, V, C (0 in the per-value form), the values' lengths and
+// bytes, written from the host (pageable: staged before the copy returns)
+static int put_slot_head(uint8_t *my_slot, uint64_t fp, const KeyValues &values, uint32_t C, cudaStream_t s) {
+    const SlotHead sh(values.size());
+    const SlotHead::Header hd{fp, static_cast<uint32_t>(values.size()), C};
+    std::vector<uint8_t> head(sh.end, 0);
+    memcpy(head.data(), &hd, sizeof hd);
+    for (size_t v = 0; v < values.size(); ++v) {
+        const uint32_t len = static_cast<uint32_t>(values[v].size());
+        memcpy(head.data() + sh.off_lens + 4 * v, &len, 4);
+        if (len) memcpy(head.data() + sh.off_vals + v * kMaxLit, values[v].data(), len);
+    }
+    CUDA_TRY(cudaMemcpyAsync(my_slot, head.data(), head.size(), cudaMemcpyHostToDevice, s));
+    return 0;
+}
+
+// On the root: the header of every rank's slot.  A rank whose fingerprint differs from the root's is refused ("<form>: rank r passed
+// another query or group key<also> (...)"); v_off / row_off: the exclusive scans of the ranks' V_r (clamped to the cap) and C_r.
+static int read_slot_heads(const uint8_t *slots0, size_t slot, uint32_t R, uint64_t fp, uint32_t cap, const char *form, const char *also,
+                           std::vector<uint32_t> &v_off, std::vector<uint32_t> &row_off) {
+    v_off.assign(R + 1, 0);
+    row_off.assign(R + 1, 0);
+    for (uint32_t r = 0; r < R; ++r) {
+        SlotHead::Header hd{};
+        CUDA_TRY(cudaMemcpy(&hd, slots0 + r * slot, sizeof hd, cudaMemcpyDeviceToHost));
+        if (hd.fp != fp)
+            return fail(BYDB_EINVAL, std::string(form) + ": rank " + std::to_string(r) + " passed another query or group key" + also +
+                                         " (only the parts may differ between ranks)");
+        v_off[r + 1] = v_off[r] + std::min(hd.V, cap);
+        row_off[r + 1] = row_off[r] + hd.C;
+    }
+    return 0;
+}
+
 int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t *out) {
     return guarded([&]() -> int {
     if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
@@ -4496,7 +4535,6 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
     Plan plan;
     uint32_t cap = 0;
     KeyValues values;
-    std::vector<uint8_t> header;
     KeyedSlot ks(0, 0, 0, 0);
     uint64_t fp = 0;
     CollectiveHooks h;
@@ -4518,15 +4556,6 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
         // sized for the union (at most cap values) now: the root's finalisation may not allocate page-locked memory later
         if (es.ensure_pinned(keyed_pinned_bytes(q, plan, G * cap, out))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
         fp = keyed_fingerprint(q, key, cap);
-        header.assign(ks.off_vals + V * kMaxLit, 0);
-        const uint32_t v32 = static_cast<uint32_t>(V);
-        memcpy(header.data(), &fp, 8);
-        memcpy(header.data() + 8, &v32, 4);
-        for (size_t v = 0; v < V; ++v) {
-            const uint32_t len = static_cast<uint32_t>(values[v].size());
-            memcpy(header.data() + ks.off_lens + 4 * v, &len, 4);
-            if (len) memcpy(header.data() + ks.off_vals + v * kMaxLit, values[v].data(), len);
-        }
         return 0;
     };
     h.contribute = [&](ExecSlot &es, uint8_t *my_slot) -> int {
@@ -4537,8 +4566,7 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
                                       reinterpret_cast<uint32_t *>(my_slot + ks.off_krow), reinterpret_cast<int64_t *>(my_slot + ks.off_span), &stats);
             if (rc) return rc;
         }
-        CUDA_TRY(cudaMemcpyAsync(my_slot, header.data(), header.size(), cudaMemcpyHostToDevice, es.stream));  // pageable: staged before it returns
-        return 0;
+        return put_slot_head(my_slot, fp, values, 0, es.stream);
     };
     h.collect = [&](ExecSlot &) { return 0; };  // every pass was collected as it ran
     h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &settle, bool &) -> int {
@@ -4546,13 +4574,9 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
         if (rc) return rc;
         cudaStream_t s = es.stream;
         const uint32_t R = static_cast<uint32_t>(ctx->comm.nranks);
-        for (uint32_t r = 0; r < R; ++r) {
-            uint64_t theirs = 0;
-            CUDA_TRY(cudaMemcpy(&theirs, slots0 + r * slot, 8, cudaMemcpyDeviceToHost));
-            if (theirs != fp)
-                return fail(BYDB_EINVAL, "keyed collective: rank " + std::to_string(r) +
-                                             " passed another query or group key (only the parts may differ between ranks)");
-        }
+        std::vector<uint32_t> v_off, row_off;  // unused: the kernels read each rank's V_r from its header
+        rc = read_slot_heads(slots0, slot, R, fp, cap, "keyed collective", "", v_off, row_off);
+        if (rc) return rc;
         // ---- union of the ranks' values, cross-rank span check
         const size_t NS = q->n_series, G = static_cast<size_t>(plan.n_groups), F = plan.fcols.size();
         Carve carve;
@@ -4681,10 +4705,10 @@ static int scan_reduce_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const
         const size_t F = plan.fcols.size(), NS = q->n_series;
         // the staging of this rank's pass; on the root also the union's read-back and the answer over the most composite groups the
         // slots can carry (no page-locked allocation may follow inside the collective)
-        size_t pinned = std::max<size_t>(NS * 12, 32 + static_cast<size_t>(cap) * (kMaxLit + 4)) + 256;
+        size_t pinned = wide_discover_pinned(NS, 1, cap);
         if (ctx->comm.rank == root) {
-            const size_t per_comp = 8 * (7 * F + 1) + 12, fixed = WideSlot(F, NS, 0, 0).total;
-            const size_t fit = slot > fixed ? (slot - fixed) / per_comp : 0;
+            const size_t fixed = WideSlot(F, NS, 0, 0).total;
+            const size_t fit = slot > fixed ? (slot - fixed) / WideSlot::comp_bytes(F) : 0;
             const size_t most = std::min<size_t>(static_cast<size_t>(ctx->comm.nranks) * fit, static_cast<size_t>(plan.n_groups) * cap);
             pinned = std::max({pinned, 32 + static_cast<size_t>(cap) * (kMaxLit + 4), keyed_pinned_bytes(q, plan, std::max<size_t>(most, 1), out)});
         }
@@ -4729,19 +4753,7 @@ static int scan_reduce_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const
         } else {
             CUDA_TRY(cudaMemsetAsync(my_slot + ws.off_table, 0, F * 8, s));  // no table: the column types of nothing
         }
-        // the header, the value lengths and the values (pageable: staged before the call returns)
-        std::vector<uint8_t> head(ws.off_span, 0);
-        const uint32_t v32 = static_cast<uint32_t>(V), c32 = static_cast<uint32_t>(C);
-        memcpy(head.data(), &fp, 8);
-        memcpy(head.data() + 8, &v32, 4);
-        memcpy(head.data() + 12, &c32, 4);
-        for (size_t v = 0; v < V; ++v) {
-            const uint32_t len = static_cast<uint32_t>(w.values[v].size());
-            memcpy(head.data() + ws.off_lens + 4 * v, &len, 4);
-            if (len) memcpy(head.data() + ws.off_vals + v * kMaxLit, w.values[v].data(), len);
-        }
-        CUDA_TRY(cudaMemcpyAsync(my_slot, head.data(), head.size(), cudaMemcpyHostToDevice, s));
-        return 0;
+        return put_slot_head(my_slot, fp, w.values, static_cast<uint32_t>(C), s);
     };
     h.collect = [&](ExecSlot &) { return 0; };  // the pass was collected as it ran
     h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &settle, bool &) -> int {
@@ -4750,18 +4762,9 @@ static int scan_reduce_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const
         cudaStream_t s = es.stream;
         const uint32_t R = static_cast<uint32_t>(ctx->comm.nranks);
         const size_t F = plan.fcols.size(), NS = q->n_series;
-        std::vector<uint32_t> v_off(R + 1, 0), row_off(R + 1, 0);
-        for (uint32_t r = 0; r < R; ++r) {
-            uint32_t hd[4] = {0, 0, 0, 0};
-            CUDA_TRY(cudaMemcpy(hd, slots0 + r * slot, 16, cudaMemcpyDeviceToHost));
-            uint64_t theirs = 0;
-            memcpy(&theirs, hd, 8);
-            if (theirs != fp)
-                return fail(BYDB_EINVAL, "wide keyed collective: rank " + std::to_string(r) +
-                                             " passed another query or group key, or called the per-value keyed collective (only the parts may differ between ranks)");
-            v_off[r + 1] = v_off[r] + std::min(hd[2], cap);
-            row_off[r + 1] = row_off[r] + hd[3];
-        }
+        std::vector<uint32_t> v_off, row_off;
+        rc = read_slot_heads(slots0, slot, R, fp, cap, "wide keyed collective", ", or called the per-value keyed collective", v_off, row_off);
+        if (rc) return rc;
         stats.d2h_bytes += 16ull * R;
         const uint32_t n_vals = v_off[R], n_rows = row_off[R];
         if (n_vals == 0) return 0;  // no rank selected a block: no rows, no keys

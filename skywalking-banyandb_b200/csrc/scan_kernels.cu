@@ -3489,6 +3489,26 @@ __device__ __forceinline__ uint64_t combine_word(uint64_t a, uint64_t b, int kin
     return a;
 }
 
+// Word i of a partial table TableLayout(rows, F) below its column types (i < 7 * rows * F + rows): its region -- sum_f64 |
+// max_f64 | negmin_f64 | sum_i64 | cnt | rows | max_i64 | notmin_i64, TableLayout's order --, how it combines (combine_word),
+// its row and its field (0 in the rows region).
+struct TableWord {
+    int reg, kind;
+    uint64_t row, field;
+};
+__device__ __forceinline__ TableWord table_word(uint64_t i, uint64_t rows, uint64_t F) {
+    const uint64_t RF = rows * F;
+    const int reg = i < 5 * RF ? static_cast<int>(i / RF) : i < 5 * RF + rows ? 5 : static_cast<int>(6 + (i - 5 * RF - rows) / RF);
+    const int kind = reg == 0 ? kWordFsum : reg <= 2 ? kWordFmax : reg <= 5 ? kWordIsum : kWordImax;
+    const uint64_t k = reg < 5 ? i - reg * RF : reg == 5 ? i - 5 * RF : i - 5 * RF - rows - (reg - 6) * RF;
+    return TableWord{reg, kind, reg == 5 ? k : k / F, reg == 5 ? 0 : k % F};
+}
+// the index of (region reg, row, field) in a TableLayout(rows, F): table_word's inverse, for another table's row count
+__device__ __forceinline__ uint64_t table_word_index(int reg, uint64_t row, uint64_t field, uint64_t rows, uint64_t F) {
+    const uint64_t RF = rows * F;
+    return (reg <= 5 ? reg * RF : 5 * RF + rows + (reg - 6) * RF) + (reg == 5 ? row : row * F + field);
+}
+
 // Multi-GPU reduce after ONE all-gather of the per-rank partial tables: every word of the table is
 // combined across ranks in rank order (deterministic float sums, unlike a ring all-reduce), which is
 // the liaison's reduceAccumulator.Combine (measure_plan_aggregation.go:96-124) done on the device.
@@ -4021,11 +4041,16 @@ void launch_rows_to_host(const RowsCopyParams &p, cudaStream_t s) {
 // ranks' tables and first appearances into V_u x G union arrays, and then runs the single-context ordering (key_order_kernel,
 // key_perm_kernel, permute_table_kernel) and finalisation on them unchanged.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t slot_values(const KeyedUnionParams &p, uint32_t r) {
-    const uint32_t v = *reinterpret_cast<const uint32_t *>(p.slots + r * p.slot_stride + 8);
+// rank r's V_r (SlotHead::Header), clamped to the cap, and its slot's layout, in either keyed collective
+template <class P>
+__device__ __forceinline__ uint32_t slot_values(const P &p, uint32_t r) {
+    const uint32_t v = reinterpret_cast<const SlotHead::Header *>(p.slots + r * p.slot_stride)->V;
     return v < p.cap ? v : p.cap;
 }
 __device__ __forceinline__ KeyedSlot slot_layout(const KeyedUnionParams &p, uint32_t r) { return KeyedSlot(p.G, p.F, p.NS, slot_values(p, r)); }
+__device__ __forceinline__ WideSlot slot_layout(const WideUnionParams &p, uint32_t r) {
+    return WideSlot(p.F, p.NS, slot_values(p, r), reinterpret_cast<const SlotHead::Header *>(p.slots + r * p.slot_stride)->C);
+}
 
 // One CTA of kMaxKeyValues threads.  Ranks in rank order, each rank's values in its order: thread v looks value v up in a shared
 // open-addressing table of the values so far (homed by key_home, like key_values_kernel's table; byte equality decides -- the
@@ -4084,8 +4109,9 @@ __global__ void __launch_bounds__(kMaxKeyValues) key_union_kernel(const __grid_c
 }
 
 // [lo, hi] of series i on rank r, clipped to the query's range; false = the rank selects no block of it
-__device__ __forceinline__ bool rank_span(const KeyedUnionParams &p, uint32_t r, uint32_t i, int64_t &lo, int64_t &hi) {
-    if (slot_values(p, r) == 0) return false;  // no selected block at all: the rank ran no pass, its spans were never written
+template <class P>
+__device__ __forceinline__ bool rank_span(const P &p, uint32_t r, uint32_t i, int64_t &lo, int64_t &hi) {
+    if (slot_values(p, r) == 0) return false;  // no selected block at all: the rank's spans were never written
     const int64_t *sp = reinterpret_cast<const int64_t *>(p.slots + r * p.slot_stride + slot_layout(p, r).off_span) + 2 * static_cast<size_t>(i);
     lo = sp[0] > p.tmin ? sp[0] : p.tmin;
     hi = sp[1] < p.tmax ? sp[1] : p.tmax;
@@ -4093,8 +4119,10 @@ __device__ __forceinline__ bool rank_span(const KeyedUnionParams &p, uint32_t r,
 }
 
 // One warp per series: the ranks' spans pairwise (at most 64 ranks, 2016 pairs).  The lowest series index with two intersecting
-// spans goes to ctl[2]: merging first appearances by time (merge_first_kernel) is exact only when the spans are disjoint.
-__global__ void __launch_bounds__(256) rank_span_check_kernel(const __grid_constant__ KeyedUnionParams p) {
+// spans goes to ctl[E + 1], kErrRankOverlap to ctl[E]: the root orders first appearances by time, which is exact only when the
+// spans are disjoint.  KeyedUnionParams: E = 1, WideUnionParams: E = 2.
+template <class P, int E>
+__global__ void __launch_bounds__(256) rank_span_check_kernel(const __grid_constant__ P p) {
     const int lane = threadIdx.x & 31;
     const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (i >= p.NS) return;
@@ -4108,8 +4136,8 @@ __global__ void __launch_bounds__(256) rank_span_check_kernel(const __grid_const
         if (rank_span(p, a, i, alo, ahi) && rank_span(p, b, i, blo, bhi)) hit = (alo > blo ? alo : blo) <= (ahi < bhi ? ahi : bhi);
     }
     if (__any_sync(0xffffffffu, hit) && lane == 0) {
-        atomicMin(&p.ctl[2], i);
-        atomicCAS(&p.ctl[1], 0u, static_cast<uint32_t>(kErrRankOverlap));
+        atomicMin(&p.ctl[E + 1], i);
+        atomicCAS(&p.ctl[E], 0u, static_cast<uint32_t>(kErrRankOverlap));
     }
 }
 
@@ -4131,22 +4159,16 @@ __global__ void combine_keyed_kernel(const __grid_constant__ KeyedUnionParams p)
         p.coltype[i - words] = typ | (err << 8);
         return;
     }
-    // region of the word: sum_f64 | max_f64 | negmin_f64 | sum_i64 | cnt | rows | max_i64 | notmin_i64 (TableLayout's order)
-    const int reg = i < 5 * GF ? static_cast<int>(i / GF) : i < 5 * GF + VG ? 5 : static_cast<int>(6 + (i - 5 * GF - VG) / GF);
-    const int kind = reg == 0 ? kWordFsum : reg <= 2 ? kWordFmax : reg <= 5 ? kWordIsum : kWordImax;
-    const uint64_t k = reg < 5 ? i - reg * GF : reg == 5 ? i - 5 * GF : i - 5 * GF - VG - (reg - 6) * GF;
-    const uint64_t j = reg == 5 ? k : k / F, c = reg == 5 ? 0 : k % F;  // union row j = u * G + g
-    const uint64_t u = j / G, g = j % G;
+    const TableWord tw = table_word(i, VG, F);
+    const uint64_t u = tw.row / G, g = tw.row % G;  // union row u * G + g
     uint64_t a = 0;
     bool first = true;
     for (uint32_t r = 0; r < p.n_ranks; ++r) {
         const int32_t v = p.inv[r * cap + u];
         if (v < 0) continue;
-        const uint64_t VGr = slot_values(p, r) * G, GFr = VGr * F;
-        const uint64_t base = reg <= 5 ? reg * GFr : 5 * GFr + VGr + (reg - 6) * GFr;
-        const uint64_t row = static_cast<uint64_t>(v) * G + g;
-        const uint64_t w = reinterpret_cast<const uint64_t *>(p.slots + r * p.slot_stride + slot_layout(p, r).off_table)[base + (reg == 5 ? row : row * F + c)];
-        a = first ? w : combine_word(a, w, kind);
+        const uint64_t at = table_word_index(tw.reg, static_cast<uint64_t>(v) * G + g, tw.field, slot_values(p, r) * G, F);
+        const uint64_t w = reinterpret_cast<const uint64_t *>(p.slots + r * p.slot_stride + slot_layout(p, r).off_table)[at];
+        a = first ? w : combine_word(a, w, tw.kind);
         first = false;
     }
     p.table[i] = a;
@@ -4180,7 +4202,7 @@ __global__ void merge_first_kernel(const __grid_constant__ KeyedUnionParams p) {
 
 void launch_key_union(const KeyedUnionParams &p, cudaStream_t s) {
     key_union_kernel<<<1, kMaxKeyValues, 0, s>>>(p);
-    if (p.NS && p.n_ranks > 1) rank_span_check_kernel<<<(p.NS + 7) / 8, 256, 0, s>>>(p);
+    if (p.NS && p.n_ranks > 1) rank_span_check_kernel<KeyedUnionParams, 1><<<(p.NS + 7) / 8, 256, 0, s>>>(p);
 }
 void launch_combine_keyed(const KeyedUnionParams &p, cudaStream_t s) {
     const uint64_t VG = static_cast<uint64_t>(p.n_values) * p.G, n = 7 * VG * p.F + VG + static_cast<uint64_t>(p.n_values) * p.F;
@@ -5427,12 +5449,8 @@ void launch_wide_first(const WideFirstParams &p, cudaStream_t s) {
     if (p.n_comp) wide_first_kernel<<<(p.n_comp + 255) / 256, 256, 0, s>>>(p);
 }
 
-// rank r's header words, its value count clamped to the cap, and its slot layout
+// rank r's slot (its layout: slot_layout)
 __device__ __forceinline__ const uint8_t *wide_slot_at(const WideUnionParams &p, uint32_t r) { return p.slots + r * p.slot_stride; }
-__device__ __forceinline__ WideSlot wide_slot_layout(const WideUnionParams &p, uint32_t r) {
-    const uint32_t *h = reinterpret_cast<const uint32_t *>(wide_slot_at(p, r));
-    return WideSlot(p.F, p.NS, h[2] < p.cap ? h[2] : p.cap, h[3]);
-}
 // the rank of flat index t of an exclusive scan over the ranks
 __device__ __forceinline__ uint32_t wide_rank_of(const uint32_t *off, uint32_t n_ranks, uint32_t t) {
     uint32_t r = 0;
@@ -5442,7 +5460,7 @@ __device__ __forceinline__ uint32_t wide_rank_of(const uint32_t *off, uint32_t n
 // value v of rank r: its bytes and length
 __device__ __forceinline__ const uint8_t *wide_value(const WideUnionParams &p, uint32_t r, uint32_t v, uint32_t &len) {
     const uint8_t *slot = wide_slot_at(p, r);
-    const WideSlot ws = wide_slot_layout(p, r);
+    const WideSlot ws = slot_layout(p, r);
     len = min(reinterpret_cast<const uint32_t *>(slot + ws.off_lens)[v], static_cast<uint32_t>(kMaxLit));
     return slot + ws.off_vals + static_cast<size_t>(v) * kMaxLit;
 }
@@ -5496,40 +5514,13 @@ __global__ void wide_union_ids_kernel(const __grid_constant__ WideUnionParams p)
     p.vid[t] = u;
 }
 
-// [lo, hi] of series i on rank r, clipped to the query's range; false = the rank selects no block of it (rank_span's rule)
-__device__ __forceinline__ bool wide_rank_span(const WideUnionParams &p, uint32_t r, uint32_t i, int64_t &lo, int64_t &hi) {
-    if (reinterpret_cast<const uint32_t *>(wide_slot_at(p, r))[2] == 0) return false;  // no selected block: no spans were written
-    const int64_t *sp = reinterpret_cast<const int64_t *>(wide_slot_at(p, r) + wide_slot_layout(p, r).off_span) + 2 * static_cast<size_t>(i);
-    lo = sp[0] > p.tmin ? sp[0] : p.tmin;
-    hi = sp[1] < p.tmax ? sp[1] : p.tmax;
-    return lo <= hi;
-}
-// rank_span_check_kernel over the wide slots: one warp per series, the ranks' spans pairwise
-__global__ void __launch_bounds__(256) wide_span_check_kernel(const __grid_constant__ WideUnionParams p) {
-    const int lane = threadIdx.x & 31;
-    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (i >= p.NS) return;
-    const uint32_t R = p.n_ranks, pairs = R * (R - 1) / 2;
-    bool hit = false;
-    for (uint32_t k = lane; k < pairs && !hit; k += 32) {
-        uint32_t a = 0, rem = k;
-        while (rem >= R - 1 - a) rem -= R - 1 - a++;
-        const uint32_t b = a + 1 + rem;
-        int64_t alo, ahi, blo, bhi;
-        if (wide_rank_span(p, a, i, alo, ahi) && wide_rank_span(p, b, i, blo, bhi)) hit = (alo > blo ? alo : blo) <= (ahi < bhi ? ahi : bhi);
-    }
-    if (__any_sync(0xffffffffu, hit) && lane == 0) {
-        atomicMin(&p.ctl[3], i);
-        atomicCAS(&p.ctl[2], 0u, static_cast<uint32_t>(kErrRankOverlap));
-    }
-}
 // the order of rank r's span among the ranks' spans of series i (by start; a tie, which the span check refuses, by rank)
 __device__ uint32_t wide_span_order(const WideUnionParams &p, uint32_t r, uint32_t i) {
     int64_t lo, hi, olo, ohi;
-    if (!wide_rank_span(p, r, i, lo, hi)) return 0;
+    if (!rank_span(p, r, i, lo, hi)) return 0;
     uint32_t o = 0;
     for (uint32_t q = 0; q < p.n_ranks; ++q)
-        if (q != r && wide_rank_span(p, q, i, olo, ohi) && (olo < lo || (olo == lo && q < r))) ++o;
+        if (q != r && rank_span(p, q, i, olo, ohi) && (olo < lo || (olo == lo && q < r))) ++o;
     return o;
 }
 __device__ __forceinline__ unsigned long long wide_order_key(uint32_t series, uint32_t span_order, uint32_t j) {
@@ -5540,7 +5531,7 @@ __global__ void wide_comp_union_kernel(const __grid_constant__ WideUnionParams p
     if (t >= p.n_rows) return;
     const uint32_t r = wide_rank_of(p.row_off, p.n_ranks, t), j = t - p.row_off[r];
     const uint8_t *slot = wide_slot_at(p, r);
-    const WideSlot ws = wide_slot_layout(p, r);
+    const WideSlot ws = slot_layout(p, r);
     const int32_t *pair = reinterpret_cast<const int32_t *>(slot + ws.off_pairs) + 2 * static_cast<size_t>(j);
     const uint32_t u = p.vid[p.v_off[r] + static_cast<uint32_t>(pair[1])];
     const unsigned long long key = ((static_cast<unsigned long long>(static_cast<uint32_t>(pair[0])) << 32) | u) + 1ull;
@@ -5574,7 +5565,7 @@ __global__ void wide_comp_place_kernel(const __grid_constant__ WideUnionParams p
     const uint32_t series = static_cast<uint32_t>(k >> 33), o = static_cast<uint32_t>(k >> 27) & 63u, j = static_cast<uint32_t>(k) & (kWideMaxRankComposites - 1);
     for (uint32_t r = 0; r < p.n_ranks; ++r) {
         int64_t lo, hi;
-        if (j >= p.row_off[r + 1] - p.row_off[r] || !wide_rank_span(p, r, series, lo, hi) || wide_span_order(p, r, series) != o) continue;
+        if (j >= p.row_off[r + 1] - p.row_off[r] || !rank_span(p, r, series, lo, hi) || wide_span_order(p, r, series) != o) continue;
         const uint32_t t = p.row_off[r] + j, s = p.row_slot[t];
         if (p.row_key[t] != k) continue;
         const unsigned long long key = p.comp[s] - 1ull;
@@ -5605,29 +5596,24 @@ __global__ void wide_comp_fold_kernel(const __grid_constant__ WideUnionParams p,
         const uint32_t c = static_cast<uint32_t>(i - words);
         int64_t typ = 0, err = 0;
         for (uint32_t r = 0; r < p.n_ranks; ++r) {
-            const WideSlot ws = wide_slot_layout(p, r);
+            const WideSlot ws = slot_layout(p, r);
             const uint64_t Cr = p.row_off[r + 1] - p.row_off[r];
             merge_coltype(reinterpret_cast<const int64_t *>(wide_slot_at(p, r) + ws.off_table)[7 * Cr * F + Cr + c], typ, err);
         }
         p.table.coltype[c] = typ | (err << 8);
         return;
     }
-    // region of the word: sum_f64 | max_f64 | negmin_f64 | sum_i64 | cnt | rows | max_i64 | notmin_i64 (TableLayout's order)
-    const int reg = i < 5 * CF ? static_cast<int>(i / CF) : i < 5 * CF + n_comp ? 5 : static_cast<int>(6 + (i - 5 * CF - n_comp) / CF);
-    const int kind = reg == 0 ? kWordFsum : reg <= 2 ? kWordFmax : reg <= 5 ? kWordIsum : kWordImax;
-    const uint64_t k = reg < 5 ? i - reg * CF : reg == 5 ? i - 5 * CF : i - 5 * CF - n_comp - (reg - 6) * CF;
-    const uint64_t c = reg == 5 ? k : k / F, f = reg == 5 ? 0 : k % F;
-    const uint32_t lo = p.seg[c], hi = c + 1 < n_comp ? p.seg[c + 1] : p.n_rows;
+    const TableWord tw = table_word(i, n_comp, F);  // row: the union composite c
+    const uint32_t lo = p.seg[tw.row], hi = tw.row + 1 < n_comp ? p.seg[tw.row + 1] : p.n_rows;
     uint64_t a = 0;
     bool first = true;
     for (uint32_t e = lo; e < hi; ++e) {
         const uint32_t t = p.order[e];
         if (t >= p.n_rows) continue;  // only under a span intersection, which fails the call
         const uint32_t r = wide_rank_of(p.row_off, p.n_ranks, t);
-        const uint64_t j = t - p.row_off[r], Cr = p.row_off[r + 1] - p.row_off[r], CFr = Cr * F;
-        const uint64_t base = reg <= 5 ? reg * CFr : 5 * CFr + Cr + (reg - 6) * CFr;
-        const uint64_t w = reinterpret_cast<const uint64_t *>(wide_slot_at(p, r) + wide_slot_layout(p, r).off_table)[base + (reg == 5 ? j : j * F + f)];
-        a = first ? w : combine_word(a, w, kind);
+        const uint64_t at = table_word_index(tw.reg, t - p.row_off[r], tw.field, p.row_off[r + 1] - p.row_off[r], F);
+        const uint64_t w = reinterpret_cast<const uint64_t *>(wide_slot_at(p, r) + slot_layout(p, r).off_table)[at];
+        a = first ? w : combine_word(a, w, tw.kind);
         first = false;
     }
     reinterpret_cast<uint64_t *>(p.table.sum_f64)[i] = a;  // the regions lie back to back from sum_f64 on
@@ -5644,7 +5630,7 @@ uint32_t launch_wide_union(const WideUnionParams &p, cudaStream_t s) {
         n += 6;
     }
     if (p.NS && p.n_ranks > 1) {
-        wide_span_check_kernel<<<(p.NS + 7) / 8, 256, 0, s>>>(p);
+        rank_span_check_kernel<WideUnionParams, 2><<<(p.NS + 7) / 8, 256, 0, s>>>(p);
         n += 1;
     }
     if (p.n_rows) {
@@ -5882,7 +5868,7 @@ void preload_kernels() {
     (void)cudaFuncGetAttributes(&ka, present_groups_kernel);
     (void)cudaFuncGetAttributes(&ka, rows_to_host_kernel);
     (void)cudaFuncGetAttributes(&ka, key_union_kernel);
-    (void)cudaFuncGetAttributes(&ka, rank_span_check_kernel);
+    (void)cudaFuncGetAttributes(&ka, rank_span_check_kernel<KeyedUnionParams, 1>);
     (void)cudaFuncGetAttributes(&ka, combine_keyed_kernel);
     (void)cudaFuncGetAttributes(&ka, merge_first_kernel);
     cudaFuncAttributes a;

@@ -440,21 +440,30 @@ struct RowsCopyParams {
     uint32_t max_rows, pad;
 };
 void launch_rows_to_host(const RowsCopyParams &p, cudaStream_t s);
-// ---- keyed collective (bydb_scan_reduce_keyed): the slot of a rank that found V key values, in the root's mailbox, for G groups,
-// F fields and NS series.  Every region is sized by V, so a rank's need grows with the values it found; the root derives each
-// rank's layout from the V_r in its header.
-//   header    u64 query fingerprint | u32 V_r | u32 pad, then lens[V] u32 and values[V][kMaxLit]
+// ---- the head of a rank's slot in the root's mailbox, in both keyed collectives (KeyedSlot, WideSlot), for V key values.  Every
+// region starts on a 256-byte boundary; the root derives a rank's layout from the V_r (and C_r) in its header.
+//   header    Header, in 256 bytes
+//   lens      [V] u32, values [V][kMaxLit] (an int64 key's 8 little-endian bytes, length 8)
+struct SlotHead {
+    struct Header {
+        uint64_t fp;  // the query's fingerprint
+        uint32_t V, C;  // V_r; C_r (WideSlot) or 0 (KeyedSlot)
+    };
+    size_t off_lens, off_vals, end;  // end: where the slot's own regions begin
+    __host__ __device__ static size_t up(size_t o) { return (o + 255) / 256 * 256; }
+    __host__ __device__ explicit SlotHead(size_t V) : off_lens(256), off_vals(up(256 + V * 4)), end(up(off_vals + V * kMaxLit)) {}
+};
+// ---- keyed collective (bydb_scan_reduce_keyed): the slot of a rank that found V key values, for G groups, F fields and NS
+// series.  Every region is sized by V, so a rank's need grows with the values it found.
+//   head      SlotHead(V)
 //   coltype   [V * F] the passes' column types + status
 //   Kts, Krow [V * NS] where each series first shows each value (ReduceParams::Kts / Krow)
 //   span      [NS][2] the series' selected blocks (ReduceParams::span)
 //   table     the composite table TableLayout(V * G, F)
-struct KeyedSlot {
-    size_t off_lens, off_vals, off_coltype, off_kts, off_krow, off_span, off_table, total;
-    __host__ __device__ static size_t up(size_t o) { return (o + 255) / 256 * 256; }
-    __host__ __device__ KeyedSlot(size_t G, size_t F, size_t NS, size_t V) {
-        off_lens = 256;
-        off_vals = up(off_lens + V * 4);
-        off_coltype = up(off_vals + V * kMaxLit);
+struct KeyedSlot : SlotHead {
+    size_t off_coltype, off_kts, off_krow, off_span, off_table, total;
+    __host__ __device__ KeyedSlot(size_t G, size_t F, size_t NS, size_t V) : SlotHead(V) {
+        off_coltype = end;
         off_kts = up(off_coltype + V * F * 8);
         off_krow = up(off_kts + V * NS * 8);
         off_span = up(off_krow + V * NS * 4);
@@ -482,25 +491,23 @@ void launch_key_union(const KeyedUnionParams &p, cudaStream_t s);
 // combine_keyed_kernel and merge_first_kernel into table / coltype / Kts / Krow (p.n_values = V_u > 0)
 void launch_combine_keyed(const KeyedUnionParams &p, cudaStream_t s);
 // ---- wide keyed collective (bydb_scan_reduce_keyed_wide): the slot of a rank that found V key values and C present composite
-// groups, for F fields and NS series.  Every region starts on a 256-byte boundary; the root derives a rank's layout from the
-// V_r and C_r in its header.
-//   header    u64 query fingerprint | u32 V_r | u32 C_r
-//   lens      [V] u32, values [V][kMaxLit] (an int64 key's 8 little-endian bytes, length 8)
+// groups, for F fields and NS series.
+//   head      SlotHead(V)
 //   span      [NS][2] i64 the series' selected blocks (as ReduceParams::span)
 //   pairs     [C][2] i32 (series group, value id) of composite j, in the rank's insertion order (wide_fold_kernel)
 //   first     [C] u32 the series index of composite j's first row
 //   table     the rank's composite table TableLayout(C, F) in its insertion order (wide_fold_kernel)
-struct WideSlot {
-    size_t off_lens, off_vals, off_span, off_pairs, off_first, off_table, total;
-    __host__ __device__ WideSlot(size_t F, size_t NS, size_t V, size_t C) {
-        off_lens = 256;
-        off_vals = KeyedSlot::up(off_lens + V * 4);
-        off_span = KeyedSlot::up(off_vals + V * kMaxLit);
-        off_pairs = KeyedSlot::up(off_span + NS * 16);
-        off_first = KeyedSlot::up(off_pairs + C * 8);
-        off_table = KeyedSlot::up(off_first + C * 4);
+struct WideSlot : SlotHead {
+    size_t off_span, off_pairs, off_first, off_table, total;
+    __host__ __device__ WideSlot(size_t F, size_t NS, size_t V, size_t C) : SlotHead(V) {
+        off_span = end;
+        off_pairs = up(off_span + NS * 16);
+        off_first = up(off_pairs + C * 8);
+        off_table = up(off_first + C * 4);
         total = off_table + 8 * (C * (7 * F + 1) + F);  // TableLayout(C, F).total
     }
+    // what one more composite group adds to the slot (pairs, first, table row), before the regions' rounding
+    static size_t comp_bytes(size_t F) { return 8 + 4 + 8 * (7 * F + 1); }
 };
 // A rank's first appearances: ranks whose records the scan wrote (WideKeyParams::rank, WideScanParams::rec_off) back to series.
 //   wide_series_kernel: thread i < NS writes span[i] (the series' selected blocks over every part); thread g < total_blocks writes
@@ -523,8 +530,8 @@ void launch_wide_first(const WideFirstParams &p, cudaStream_t s);
 // The root of the wide collective.  Flat indices: rank r's value v is v_off[r] + v, its composite row j is row_off[r] + j.
 //   1. the union of the values (launch_wide_union): every (r, v) enters a table homed by key_home over its bytes; the slot keeps the
 //      least (r, v) with those bytes; the least ones are numbered by an exclusive scan in (r, v) order -- ranks in rank order, each
-//      rank's values in its order -- and write the union values; vid[r, v] = the union id.  wide_span_check_kernel is
-//      rank_span_check_kernel's rule over the wide slots.  wide_comp_union_kernel enters each row's composite (g, union id) into a
+//      rank's values in its order -- and write the union values; vid[r, v] = the union id.  rank_span_check_kernel checks the
+//      spans as in the per-value collective.  wide_comp_union_kernel enters each row's composite (g, union id) into a
 //      composite table (ctl[1] = C_u) with its order key, the least key of a composite and the set of ranks that hold it.
 //   2. the merge (launch_wide_merge): the composites sorted by their least order key are the insertion order of the whole scan;
 //      each composite's rows are laid out in rank order, and wide_comp_fold_kernel folds them with combine_word into row c of a

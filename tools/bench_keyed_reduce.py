@@ -84,7 +84,7 @@ def root_kernels_ms(ctxs, qs, calls):
         us = getattr(e, "device_time_total", None)
         if us is None:
             us = getattr(e, "cuda_time_total", 0)
-        name = e.key.split("(")[0].replace("void ", "").replace("bydb::", "")
+        name = e.key.split("(")[0].split("<")[0].replace("void ", "").replace("bydb::", "")
         if name in ROOT_KERNELS:
             out[name] = round(us / 1e3 / calls, 4)
     return out
