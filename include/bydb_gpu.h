@@ -492,7 +492,8 @@ int bydb_scan_partials_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb
  *     up to 256-byte alignment of each region,
  *       12 * NS + K * (12 * S + 68 * cap) + 12 * S + 8 * cap + 8 * NB                                     discovery
  *     + then bydb_scan_agg_keyed_wide's scan, order, composite table and finalisation terms for this R and C.
- * Free the answers with bydb_keys_result_free / bydb_keys_partial_rows_free.  No prepared, multi-GPU or host-image form. */
+ * Free the answers with bydb_keys_result_free / bydb_keys_partial_rows_free.  The multi-GPU form is bydb_scan_reduce_keys_wide;
+ * there is no prepared or host-image form. */
 typedef struct {
     uint32_t n_keys;              /* 2..4 stored GroupBy tags, in the request's GroupBy order                               */
     uint32_t max_values;          /* distinct key TUPLES accepted over the query; 0 = 64, at most 65,536                    */
@@ -710,6 +711,64 @@ int bydb_keyed_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_key 
 int bydb_scan_reduce_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out);
 int bydb_scan_reduce_keyed_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root,
                                          bydb_keyed_partial_rows *out);
+
+/* The collective form of bydb_scan_agg_keys_wide / bydb_scan_partials_keys_wide: group-by on a tuple of 2..4 stored tags across the
+ * ranks of the peer mailboxes ("latency by endpoint and status code" over a node whose GPUs shard its parts).  Every rank runs
+ * bydb_scan_agg_keys_wide's discovery, scan and order over ITS parts and writes its present composite groups (series group, tuple)
+ * -- their table in its insertion order, their first series, the series' spans, each tag's values and its tuples' codes in its own
+ * tag ids -- straight into its slot of the root's mailbox.  The root takes the union of each tag's values, then of the tuples,
+ * rebuilds the insertion order of the whole scan, folds each composite group's rows in rank order (deterministic float sums) and
+ * answers once.
+ *   - Every rank passes the SAME series_ids, series_group, n_groups, tmin / tmax, predicates, aggregations, Top-N, flags and *keys
+ *     (every key's family, tag and value type in GroupBy order, and max_values); only `parts` differ.  The fingerprint covers them
+ *     and names the tuple form: a rank passing other keys, the same keys in another order, or calling bydb_scan_reduce_keyed_wide in
+ *     the same collective makes the root fail with BYDB_EINVAL.  The two calls below may be mixed: every rank contributes the same
+ *     bytes, the root's call decides its answer's form.
+ *   - The root's answer is what bydb_scan_agg_keys_wide (bydb_scan_partials_keys_wide) answers over all ranks' parts: rows in the
+ *     insertion order of the whole scan, or Top-N order with ties to the group inserted first; n_tuples = the distinct tuples over
+ *     all ranks' selected blocks, key_base[t+1] - key_base[t] = tag t's distinct values over all ranks; the per-component nil
+ *     rules, typing, BYDB_Q_ROW_PATH_TYPES, the sentinels and the partial form's wire rule as there.  Counts, int64 values and
+ *     min / max are exact, float sums within bydb_scan_agg_keyed_wide's bound and bit-identical from call to call.  The order inside
+ *     each tag's table and the numbering of the tuples are not part of the contract: identify rows by their key bytes.  Non-root
+ *     ranks get n_rows = 0, n_tuples = 0 (and n_tags = 0) and their own stats.
+ *   - Caps and refusals: every argument refusal of bydb_scan_agg_keys_wide, with the same codes.  More distinct tuples over all
+ *     ranks than max_values (0 = 64) gives BYDB_ENOMEM at the root, even when every rank alone is under the cap; so does a tag with
+ *     more distinct values over all ranks than max_values, which is refused before any tuple is recoded (a union tag id must fit
+ *     16 bits).  The per-block and per-tag BYDB_ENOTSUP rules hold on the rank where the block lives; parts of one rank that
+ *     overlap in time give BYDB_ENOTSUP; a series whose clipped spans on two ranks intersect gives BYDB_ENOTSUP at the root, naming
+ *     the series.  Insertion order and its limits as in bydb_scan_reduce_keyed_wide.
+ *   - Slots: bydb_keys_wide_reduce_slot_bytes (host only) gives the slot a rank needs at T = V_t = max_values (every tag's values
+ *     and the tuples at the cap) and max_present present composite groups; pass it (or the largest over the queries to come) to
+ *     bydb_comm_export as max_table_bytes.  A rank whose values, tuples and present groups do not fit the exported slot fails with
+ *     BYDB_EINVAL, and so does the root.  Every failure keeps the ranks' epochs in step: plain, keyed, wide and tuple collectives may
+ *     follow, with any roots.
+ *   - Stats of every rank, with K tags, V_t,r, T_r, R_r, C_r the V_t, T, R, C of bydb_scan_agg_keys_wide over the rank's parts, NB its
+ *     parts' blocks and sort(N) as for bydb_scan_reduce_keyed_wide: rows_scanned, rows_matched, blocks_scanned and page_bytes are
+ *     those of its one wide pass;
+ *       d2h_bytes = 32 * (K + 1) + sum_t V_t,r * (64 + 4 for a string tag, 8 for an int64 tag) + 8 * T_r, + 256 + 8 when T_r > 0
+ *       kernel_launches = (K + 1) * ((NB > 0) + 1) + 3, and when T_r > 0: + (NB > 0) + 10 + sort(pow2(max(R_r, 2048))) + (C_r > 0)
+ *     A rank's tables, spans, values and codes travel to the root's mailbox device to device (the head, values and codes from the
+ *     host) and are not counted.  The root adds, with V_u,t, T_u, C_u the union's tag-t values, tuples and composite groups, R ranks,
+ *     sum T and sum C over the ranks:
+ *       d2h_bytes += 36 * R, and when sum T > 0: + 48 + 48 + sum_t V_u,t * (64 + 4) + 8 * T_u, and when C_u > 0: + the
+ *                    finalisation read-back of bydb_scan_agg over C_u groups (or 8 + 8 * F + C_u * (8 + 16 * A) for the partial
+ *                    form) + 8 * C_u
+ *       kernel_launches += when sum T > 0: 6 * K + (NS > 0 and R > 1) + 6 + (sum C > 0), and when C_u > 0: + 8 +
+ *                    sort(pow2(max(sum C, 2048))) + the finalisation's kernels (or 1 for the partial form)
+ *       h2d_bytes += 4 * (K + 2) * (R + 1) when sum T > 0
+ *     (a refusal at the root stops these sums where it is found).  The root's merge takes, up to 256-byte alignment of each region,
+ *     with pow2(x) the least power of two >= x and sum V_t the ranks' tag-t values summed,
+ *       64 + 4 * (K + 2) * (R + 1) + sum_t (8 * pow2(max(2 * sum V_t, 1024)) + 4 * sum V_t + 68 * cap) + 8 * pow2(max(2 * sum T, 1024))
+ *       + 4 * sum T + 4 * max(max_t sum V_t, sum T) + 8 * cap + 28 * pow2(max(2 * sum C, 1024)) + 20 * sum C
+ *       + 8 * pow2(max(sum C, 2048)) (+ the exclusive scans' tile sums)                                    the unions and the order
+ *       + 8 * (C_u * (7 * F + 1) + F) + 12 * C_u                                                           the folded table
+ *       + the finalisation's scratch over C_u groups (or the row image, 8 + 8 * F + C_u * (8 + 16 * A))
+ *     of device scratch, and a rank 4 * (NB + C_r) beside its wide pass.  The root's page-locked staging is sized before the
+ *     collective for the unions' read-back and the most composite groups the slots can carry. */
+int bydb_keys_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_keys *keys, uint64_t max_present, uint64_t *out);
+int bydb_scan_reduce_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root, bydb_keys_result *out);
+int bydb_scan_reduce_keys_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root,
+                                        bydb_keys_partial_rows *out);
 
 const char *bydb_last_error(void);
 const char *bydb_version(void);

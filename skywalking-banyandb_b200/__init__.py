@@ -19,7 +19,7 @@ The directory name contains a hyphen, so the package is registered under the imp
 from .capi import (  # noqa: F401
     AGG_COUNT, AGG_MAX, AGG_MEAN, AGG_MIN, AGG_SUM, OP_EQ, OP_GE, OP_GT, OP_LE, OP_LT, OP_NE,
     VT_BINARY, VT_FLOAT64, VT_INT64, VT_STR, BydbError, Context, Pred, PreparedQuery, Query, Result, Stats,
-    keyed_reduce_slot_bytes, keyed_wide_reduce_slot_bytes, library_path, load_library,
+    keyed_reduce_slot_bytes, keyed_wide_reduce_slot_bytes, keys_wide_reduce_slot_bytes, library_path, load_library,
 )
 from .scan_operator import (  # noqa: F401
     AggCount, AggFunc, AggMax, AggMean, AggMin, AggSpec, AggSum, BatchSchema, ColumnDef, ColumnType,

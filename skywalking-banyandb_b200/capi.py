@@ -131,7 +131,7 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_scan_reduce_keyed_partials", "bydb_scan_agg_keyed_wide", "bydb_scan_partials_keyed_wide",
            "bydb_keyed_wide_reduce_slot_bytes", "bydb_scan_reduce_keyed_wide", "bydb_scan_reduce_keyed_wide_partials",
            "bydb_query_prepare_keyed_wide", "bydb_scan_agg_keys_wide", "bydb_scan_partials_keys_wide", "bydb_keys_result_free",
-           "bydb_keys_partial_rows_free",
+           "bydb_keys_partial_rows_free", "bydb_keys_wide_reduce_slot_bytes", "bydb_scan_reduce_keys_wide", "bydb_scan_reduce_keys_wide_partials",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -212,6 +212,10 @@ def load_library():
     L.bydb_keys_result_free.restype = None
     L.bydb_keys_partial_rows_free.argtypes = [C.c_void_p, C.POINTER(_KeysPartialRows)]
     L.bydb_keys_partial_rows_free.restype = None
+    L.bydb_keys_wide_reduce_slot_bytes.argtypes = [C.POINTER(_Query), C.POINTER(_GroupKeys), C.c_uint64, C.POINTER(C.c_uint64)]
+    L.bydb_scan_reduce_keys_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKeys), C.c_int32, C.POINTER(_KeysResult)]
+    L.bydb_scan_reduce_keys_wide_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKeys), C.c_int32,
+                                                      C.POINTER(_KeysPartialRows)]
     _lib = L
     return L
 
@@ -503,6 +507,17 @@ def _group_keys(keys: Sequence[tuple], max_values: int, keep: list) -> "_GroupKe
     return _GroupKeys(len(keys), max_values, arr)
 
 
+def keys_wide_reduce_slot_bytes(q: Query, keys: Sequence[tuple], max_values: int = 0, max_present: int = 0) -> int:
+    """bydb_keys_wide_reduce_slot_bytes (host only): the mailbox slot a rank of the tuple collective needs with every tag's values
+    and the tuples at max_values and max_present present composite groups.  keys: (family, tag, value_type) per GroupBy tag."""
+    keep: list = []
+    cq = _mk_query(q, keep)
+    gks = _group_keys(keys, max_values, keep)
+    out = C.c_uint64()
+    _check(load_library().bydb_keys_wide_reduce_slot_bytes(C.byref(cq), C.byref(gks), max_present, C.byref(out)))
+    return out.value
+
+
 def _read_tuples(r, n_rows: int):
     """-> (each tag's values, each row's tuple of key bytes) of a bydb_keys_result / bydb_keys_partial_rows"""
     k = r.n_tags
@@ -648,6 +663,9 @@ class Context:
         gks = _group_keys(keys, max_values, keep)
         r = _KeysResult()
         _check(self._L.bydb_scan_agg_keys_wide(self._h, C.byref(cq), C.byref(gks), C.byref(r)))
+        return self._read_keys(q, r)
+
+    def _read_keys(self, q: Query, r: "_KeysResult") -> Result:
         try:
             if r.base.n_rows == 0 and not r.base.owner:
                 a = len(q.aggs)
@@ -669,6 +687,9 @@ class Context:
         gks = _group_keys(keys, max_values, keep)
         r = _KeysPartialRows()
         _check(self._L.bydb_scan_partials_keys_wide(self._h, C.byref(cq), C.byref(gks), C.byref(r)))
+        return self._read_keys_partials(q, r)
+
+    def _read_keys_partials(self, q: Query, r: "_KeysPartialRows") -> Dict[str, object]:
         try:
             out = _read_partial_rows(r.base, len(q.aggs))
             out["key_tables"], out["key"] = _read_tuples(r, r.base.n_rows)
@@ -868,6 +889,31 @@ class Context:
         r = _KeyedPartialRows()
         _check(self._L.bydb_scan_reduce_keyed_wide_partials(self._h, C.byref(cq), C.byref(gk), root, C.byref(r)))
         return self._read_keyed_partials(q, r)
+
+    def keys_wide_reduce_slot_bytes(self, q: Query, keys: Sequence[tuple], max_values: int = 0, max_present: int = 0) -> int:
+        """Mailbox slot bytes the tuple collective needs (bydb_keys_wide_reduce_slot_bytes): pass it to comm_export."""
+        return keys_wide_reduce_slot_bytes(q, keys, max_values, max_present)
+
+    def scan_reduce_keys_wide(self, q: Query, keys: Sequence[tuple], root: int = 0, max_values: int = 0) -> Result:
+        """Collective group-by on a tuple of 2..4 stored tags (bydb_scan_reduce_keys_wide): every rank passes the same query and
+        keys but its parts.  The root gets scan_agg_keys_wide's answer over all ranks' parts; the others an empty result
+        (n_tuples 0, no key tables) with their own scan statistics."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gks = _group_keys(keys, max_values, keep)
+        r = _KeysResult()
+        _check(self._L.bydb_scan_reduce_keys_wide(self._h, C.byref(cq), C.byref(gks), root, C.byref(r)))
+        return self._read_keys(q, r)
+
+    def scan_reduce_keys_wide_partials(self, q: Query, keys: Sequence[tuple], root: int = 0, max_values: int = 0) -> Dict[str, object]:
+        """The tuple collective with the root emitting partial rows (bydb_scan_reduce_keys_wide_partials): the root gets
+        scan_partials_keys_wide's rows over all ranks' parts; the others no rows, no tuples and their own scan statistics."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gks = _group_keys(keys, max_values, keep)
+        r = _KeysPartialRows()
+        _check(self._L.bydb_scan_reduce_keys_wide_partials(self._h, C.byref(cq), C.byref(gks), root, C.byref(r)))
+        return self._read_keys_partials(q, r)
 
     def partials_combine(self, q, d_ptr: int, n_tables: int, bytes_each: int, stream: int = 0) -> None:
         cq, keep = _cq(q)

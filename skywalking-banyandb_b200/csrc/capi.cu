@@ -2218,6 +2218,12 @@ size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, cons
 size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keyed_partial_rows *) {
     return std::max(stage_layout(q->n_series, static_cast<size_t>(plan.n_groups)).stride, keyed_ctl_bytes(plan.fcols.size()) + GP * keyed_row_bytes(q->n_aggs));
 }
+size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keys_result *) {
+    return keyed_pinned_bytes(q, plan, GP, static_cast<const bydb_keyed_result *>(nullptr));
+}
+size_t keyed_pinned_bytes(const bydb_query *q, const Plan &plan, size_t GP, const bydb_keys_partial_rows *) {
+    return keyed_pinned_bytes(q, plan, GP, static_cast<const bydb_keyed_partial_rows *>(nullptr));
+}
 
 void keyed_free(bydb_ctx *ctx, bydb_keyed_result *out) { bydb_keyed_result_free(ctx, out); }
 void keyed_free(bydb_ctx *ctx, bydb_keyed_partial_rows *out) { bydb_keyed_partial_rows_free(ctx, out); }
@@ -4471,9 +4477,10 @@ static KeyedSlot keyed_slot(const Plan &plan, size_t V) { return KeyedSlot(plan.
 
 // A rank's slot head (SlotHead) in either keyed collective: fingerprint, V, C (0 in the per-value form), the values' lengths and
 // bytes, written from the host (pageable: staged before the copy returns)
-static int put_slot_head(uint8_t *my_slot, uint64_t fp, const KeyValues &values, uint32_t C, cudaStream_t s) {
+// the bytes of such a head with Header.V = V (the tuple collective's head holds its tags' values but counts its tuples)
+static std::vector<uint8_t> slot_head(uint64_t fp, const KeyValues &values, uint32_t V, uint32_t C) {
     const SlotHead sh(values.size());
-    const SlotHead::Header hd{fp, static_cast<uint32_t>(values.size()), C};
+    const SlotHead::Header hd{fp, V, C};
     std::vector<uint8_t> head(sh.end, 0);
     memcpy(head.data(), &hd, sizeof hd);
     for (size_t v = 0; v < values.size(); ++v) {
@@ -4481,24 +4488,34 @@ static int put_slot_head(uint8_t *my_slot, uint64_t fp, const KeyValues &values,
         memcpy(head.data() + sh.off_lens + 4 * v, &len, 4);
         if (len) memcpy(head.data() + sh.off_vals + v * kMaxLit, values[v].data(), len);
     }
+    return head;
+}
+static int put_slot_head(uint8_t *my_slot, uint64_t fp, const KeyValues &values, uint32_t C, cudaStream_t s) {
+    const std::vector<uint8_t> head = slot_head(fp, values, static_cast<uint32_t>(values.size()), C);
     CUDA_TRY(cudaMemcpyAsync(my_slot, head.data(), head.size(), cudaMemcpyHostToDevice, s));
     return 0;
 }
 
 // On the root: the header of every rank's slot.  A rank whose fingerprint differs from the root's is refused ("<form>: rank r passed
 // another query or group key<also> (...)"); v_off / row_off: the exclusive scans of the ranks' V_r (clamped to the cap) and C_r.
+// tags (the tuple collective): each rank's TupleSlot::Tags too, read in the same copy as its header.
 static int read_slot_heads(const uint8_t *slots0, size_t slot, uint32_t R, uint64_t fp, uint32_t cap, const char *form, const char *also,
-                           std::vector<uint32_t> &v_off, std::vector<uint32_t> &row_off) {
+                           std::vector<uint32_t> &v_off, std::vector<uint32_t> &row_off, std::vector<TupleSlot::Tags> *tags = nullptr) {
     v_off.assign(R + 1, 0);
     row_off.assign(R + 1, 0);
+    if (tags) tags->assign(R, TupleSlot::Tags{});
     for (uint32_t r = 0; r < R; ++r) {
-        SlotHead::Header hd{};
-        CUDA_TRY(cudaMemcpy(&hd, slots0 + r * slot, sizeof hd, cudaMemcpyDeviceToHost));
-        if (hd.fp != fp)
+        struct {
+            SlotHead::Header hd;
+            TupleSlot::Tags tg;
+        } h{};
+        CUDA_TRY(cudaMemcpy(&h, slots0 + r * slot, sizeof h.hd + (tags ? sizeof h.tg : 0), cudaMemcpyDeviceToHost));
+        if (h.hd.fp != fp)
             return fail(BYDB_EINVAL, std::string(form) + ": rank " + std::to_string(r) + " passed another query or group key" + also +
                                          " (only the parts may differ between ranks)");
-        v_off[r + 1] = v_off[r] + std::min(hd.V, cap);
-        row_off[r + 1] = row_off[r] + hd.C;
+        v_off[r + 1] = v_off[r] + std::min(h.hd.V, cap);
+        row_off[r + 1] = row_off[r] + h.hd.C;
+        if (tags) (*tags)[r] = h.tg;
     }
     return 0;
 }
@@ -4675,6 +4692,41 @@ static uint64_t keyed_wide_fingerprint(const bydb_query *q, const bydb_group_key
     return h;
 }
 
+// A rank's present composite groups after its wide pass, into the WideSlot regions of its slot in the root's mailbox (a TupleSlot's
+// are the same): wide_fold_kernel the table and pairs, wide_series_kernel the series' spans, wide_first_kernel each group's first
+// series.  No record: only the table's column types (of nothing).
+static int put_wide_rank(const Plan &plan, WidePass &w, uint8_t *my_slot, const WideSlot &ws, bydb_stats &stats, cudaStream_t s) {
+    const size_t F = plan.fcols.size(), C = w.n_comp;
+    if (!w.R) {
+        CUDA_TRY(cudaMemsetAsync(my_slot + ws.off_table, 0, F * 8, s));
+        return 0;
+    }
+    WideReduceParams &rp = w.rp;
+    rp.table = TableLayout(C, F).at(my_slot + ws.off_table);
+    rp.pairs = reinterpret_cast<int32_t *>(my_slot + ws.off_pairs);
+    Scratch pb;
+    CUDA_TRY(pb.alloc(C * 4, s));
+    rp.perm = reinterpret_cast<int32_t *>(pb.base);
+    launch_wide_fold(rp, static_cast<uint32_t>(C), s);
+    Scratch rs;
+    CUDA_TRY(rs.alloc(std::max<size_t>(plan.total_blocks, 1) * 4, s));
+    WideFirstParams fp1;
+    memset(&fp1, 0, sizeof fp1);
+    fp1.rank = w.wk.rank;
+    fp1.rank_series = reinterpret_cast<uint32_t *>(rs.base);
+    fp1.span = reinterpret_cast<int64_t *>(my_slot + ws.off_span);
+    fp1.keys = rp.keys;
+    fp1.seg_start = rp.seg_start;
+    fp1.rec_off = w.wk.n_by_rank;
+    fp1.n_blocks = static_cast<uint32_t>(plan.total_blocks);
+    fp1.n_comp = static_cast<uint32_t>(C);
+    fp1.first = reinterpret_cast<uint32_t *>(my_slot + ws.off_first);
+    launch_wide_series(w.wk.k, fp1, s);
+    launch_wide_first(fp1, s);
+    stats.kernel_launches += 1 + 1 + (C ? 1 : 0);
+    return 0;
+}
+
 // The wide keyed collective: on every rank the wide path's discovery, scan and order (wide_pass), then wide_fold_kernel writes the
 // rank's present composite groups straight into its slot of the root's mailbox (layout WideSlot), wide_series_kernel the series'
 // spans and wide_first_kernel each composite's first series; on the root the union of the values, the span check, the union
@@ -4726,33 +4778,8 @@ static int scan_reduce_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const
             return fail(BYDB_EINVAL, "wide keyed collective: this rank's " + std::to_string(V) + " key values and " + std::to_string(C) +
                                          " composite groups need " + std::to_string(ws.total) +
                                          " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keyed_wide_reduce_slot_bytes)");
-        if (w.R) {
-            WideReduceParams &rp = w.rp;
-            rp.table = TableLayout(C, F).at(my_slot + ws.off_table);
-            rp.pairs = reinterpret_cast<int32_t *>(my_slot + ws.off_pairs);
-            Scratch pb;
-            CUDA_TRY(pb.alloc(C * 4, s));
-            rp.perm = reinterpret_cast<int32_t *>(pb.base);
-            launch_wide_fold(rp, static_cast<uint32_t>(C), s);
-            Scratch rs;
-            CUDA_TRY(rs.alloc(std::max<size_t>(plan.total_blocks, 1) * 4, s));
-            WideFirstParams fp1;
-            memset(&fp1, 0, sizeof fp1);
-            fp1.rank = w.wk.rank;
-            fp1.rank_series = reinterpret_cast<uint32_t *>(rs.base);
-            fp1.span = reinterpret_cast<int64_t *>(my_slot + ws.off_span);
-            fp1.keys = rp.keys;
-            fp1.seg_start = rp.seg_start;
-            fp1.rec_off = w.wk.n_by_rank;
-            fp1.n_blocks = static_cast<uint32_t>(plan.total_blocks);
-            fp1.n_comp = static_cast<uint32_t>(C);
-            fp1.first = reinterpret_cast<uint32_t *>(my_slot + ws.off_first);
-            launch_wide_series(w.wk.k, fp1, s);
-            launch_wide_first(fp1, s);
-            stats.kernel_launches += 1 + 1 + (C ? 1 : 0);
-        } else {
-            CUDA_TRY(cudaMemsetAsync(my_slot + ws.off_table, 0, F * 8, s));  // no table: the column types of nothing
-        }
+        rc = put_wide_rank(plan, w, my_slot, ws, stats, s);
+        if (rc) return rc;
         return put_slot_head(my_slot, fp, w.values, static_cast<uint32_t>(C), s);
     };
     h.collect = [&](ExecSlot &) { return 0; };  // the pass was collected as it ran
@@ -4878,6 +4905,305 @@ int bydb_scan_reduce_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_g
 int bydb_scan_reduce_keyed_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root,
                                          bydb_keyed_partial_rows *out) {
     return guarded([&]() -> int { return scan_reduce_keyed_wide_impl(ctx, q, key, root, out); });
+}
+
+int bydb_keys_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_keys *keys, uint64_t max_present, uint64_t *out) {
+    return guarded([&]() -> int {
+    if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
+    int rc = validate_query(q, false);
+    uint32_t cap = 0;
+    if (!rc) rc = check_group_key(q, keys, kMaxWideKeyValues, false, cap);
+    if (rc) return rc;
+    Plan plan;
+    rc = query_shape(q, plan);
+    if (rc) return rc;
+    *out = TupleSlot(plan.fcols.size(), q->n_series, static_cast<size_t>(keys->n_keys) * cap, cap, max_present).total;
+    return 0;
+    });
+}
+}  // extern "C"
+
+// the fingerprint of the tuple collective: the query, every key (family, tag, value type) in GroupBy order, the cap and the form
+static uint64_t keys_wide_fingerprint(const bydb_query *q, const bydb_group_keys *keys, uint32_t cap) {
+    uint64_t h = keyed_fingerprint(q, &keys->keys[0], cap);
+    auto mix = [&](const void *p, size_t n) {
+        const uint8_t *b = static_cast<const uint8_t *>(p);
+        for (size_t i = 0; i < n; ++i) h = (h ^ b[i]) * 0x100000001b3ull;
+    };
+    const uint64_t K = keys->n_keys;
+    mix(&K, sizeof K);
+    for (uint32_t t = 1; t < keys->n_keys; ++t) {
+        const bydb_group_key &k = keys->keys[t];
+        const uint64_t nf = strlen(k.family), nt = strlen(k.tag), vt = k.value_type;
+        mix(&nf, 8);
+        mix(k.family, nf);
+        mix(&nt, 8);
+        mix(k.tag, nt);
+        mix(&vt, 8);
+    }
+    mix("tuple", 5);
+    return h;
+}
+
+// The tuple collective: on every rank bydb_scan_agg_keys_wide's discovery, scan and order (wide_pass with the key list), its present
+// composite groups into its slot as the wide keyed collective writes them (put_wide_rank), and a head with its tags' values and its
+// tuple codes (layout TupleSlot).  On the root: each tag's value union and the span check (launch_tuple_tag_union), then -- every
+// tag's union within the cap, so that a union id fits 16 bits -- the tuple union and the composite union (launch_tuple_union), the
+// wide collective's merge over the union tuple ids, and wide_emit with the union tag tables and codes.  The root's call decides the
+// answer's form; ranks may mix the two calls in one collective.
+template <class Out>
+static int scan_reduce_keys_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root, Out *out) {
+    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
+    memset(out, 0, sizeof *out);
+    g_last_dev_err = 0;
+    KeyedAnswer<Out> answer(ctx, out);
+    bydb_stats &stats = keyed_stats(out);
+    Plan plan;
+    uint32_t cap = 0, K = 0;
+    uint64_t fp = 0;
+    size_t slot_bytes = 0;
+    WidePass w;
+    CollectiveHooks h;
+    h.prepare = [&](ExecSlot &es, size_t slot) -> int {
+        slot_bytes = slot;
+        int rc = validate_query(q, true);
+        if (!rc) rc = check_group_key(q, keys, kMaxWideKeyValues, false, cap);
+        if (!rc) rc = make_plan(ctx, q, nullptr, plan);
+        if (rc) return rc;
+        if (parts_overlap(plan.parts, q->tmin, q->tmax))
+            return fail(BYDB_ENOTSUP, "group-key query over parts of one rank that overlap in time (version dedup) is not supported on the device path");
+        K = keys->n_keys;
+        fp = keys_wide_fingerprint(q, keys, cap);
+        const size_t F = plan.fcols.size(), NS = q->n_series;
+        // the staging of this rank's pass; on the root also the unions' read-back (control words, K tag tables, the tuple codes)
+        // and the answer over the most composite groups the slots can carry (no page-locked allocation may follow inside the
+        // collective)
+        size_t pinned = wide_discover_pinned(NS, K, cap);
+        if (ctx->comm.rank == root) {
+            const size_t fixed = TupleSlot(F, NS, 0, 0, 0).total;
+            const size_t fit = slot > fixed ? (slot - fixed) / WideSlot::comp_bytes(F) : 0;
+            const size_t most = std::min<size_t>(static_cast<size_t>(ctx->comm.nranks) * fit, static_cast<size_t>(plan.n_groups) * cap);
+            pinned = std::max({pinned, 64 + K * static_cast<size_t>(cap) * (kMaxLit + 4) + static_cast<size_t>(cap) * 8,
+                               keyed_pinned_bytes(q, plan, std::max<size_t>(most, 1), out)});
+        }
+        if (es.ensure_pinned(pinned)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
+        return 0;
+    };
+    h.contribute = [&](ExecSlot &es, uint8_t *my_slot) -> int {
+        cudaStream_t s = es.stream;
+        const size_t F = plan.fcols.size(), NS = q->n_series;
+        int rc = wide_pass(ctx, q, keys->keys, K, cap, plan, es, stats, w);
+        if (rc) return rc;
+        KeyValues all;  // the tags' values back to back
+        TupleSlot::Tags tg{};
+        tg.K = K;
+        for (uint32_t t = 0; t < K && t < w.tag_values.size(); ++t) {
+            tg.V[t] = static_cast<uint32_t>(w.tag_values[t].size());
+            all.insert(all.end(), w.tag_values[t].begin(), w.tag_values[t].end());
+        }
+        const size_t T = w.codes.size(), C = w.n_comp;
+        const TupleSlot ts(F, NS, all.size(), T, C);
+        if (ts.total > slot_bytes || C >= kWideMaxRankComposites)
+            return fail(BYDB_EINVAL, "tuple collective: this rank's " + std::to_string(all.size()) + " tag values, " + std::to_string(T) + " tuples and " +
+                                         std::to_string(C) + " composite groups need " + std::to_string(ts.total) +
+                                         " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keys_wide_reduce_slot_bytes)");
+        rc = put_wide_rank(plan, w, my_slot, ts, stats, s);
+        if (rc) return rc;
+        std::vector<uint8_t> head = slot_head(fp, all, static_cast<uint32_t>(T), static_cast<uint32_t>(C));
+        memcpy(head.data() + sizeof(SlotHead::Header), &tg, sizeof tg);
+        CUDA_TRY(cudaMemcpyAsync(my_slot, head.data(), head.size(), cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
+        if (T) CUDA_TRY(cudaMemcpyAsync(my_slot + ts.off_codes, w.codes.data(), T * 8, cudaMemcpyHostToDevice, s));
+        return 0;
+    };
+    h.collect = [&](ExecSlot &) { return 0; };  // the pass was collected as it ran
+    h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &settle, bool &) -> int {
+        int rc = settle();  // a failed rank's slot holds nothing to read
+        if (rc) return rc;
+        cudaStream_t s = es.stream;
+        const uint32_t R = static_cast<uint32_t>(ctx->comm.nranks);
+        const size_t F = plan.fcols.size(), NS = q->n_series;
+        std::vector<uint32_t> t_off, row_off;
+        std::vector<TupleSlot::Tags> tags;
+        rc = read_slot_heads(slots0, slot, R, fp, cap, "tuple collective", ", or called the one-key wide collective", t_off, row_off, &tags);
+        if (rc) return rc;
+        stats.d2h_bytes += (sizeof(SlotHead::Header) + sizeof(TupleSlot::Tags)) * R;
+        WidePass u;  // the union's tag tables and tuple codes, in the shape tuple_key_tables / tuple_row_entries read
+        u.tag_values.assign(K, KeyValues());
+        const uint32_t n_tup = t_off[R], n_rows = row_off[R];
+        if (n_tup == 0) {  // no rank selected a block: no rows, K empty tag tables
+            wide_key_tables(out, answer.owner, u);
+            return 0;
+        }
+        // per tag: the exclusive scan of the ranks' V_t (each at most the cap)
+        std::vector<uint32_t> offs(t_off);
+        offs.insert(offs.end(), row_off.begin(), row_off.end());
+        uint32_t tv[kMaxKeyTags] = {}, tv_max = 0;
+        for (uint32_t t = 0; t < K; ++t) {
+            offs.push_back(0);
+            for (uint32_t r = 0; r < R; ++r) offs.push_back(offs.back() + std::min(tags[r].V[t], cap));
+            tv[t] = offs.back();
+            tv_max = std::max(tv_max, tv[t]);
+        }
+        const size_t nh = align_up(std::max(tv_max, n_tup), 1024), nr = align_up(std::max<uint32_t>(n_rows, 1), 1024);
+        size_t VS[kMaxKeyTags] = {};
+        for (uint32_t t = 0; t < K; ++t) VS[t] = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(tv[t]), 1024));
+        const size_t TS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_tup), 1024));
+        const size_t CS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_rows), 1024)), N = pow2_at_least(std::max<size_t>(n_rows, 2048));
+        Carve carve;
+        const size_t u_ctl = carve(64), u_off = carve(4 * offs.size());
+        size_t u_vslot[kMaxKeyTags] = {}, u_vid[kMaxKeyTags] = {}, u_vals[kMaxKeyTags] = {}, u_lens[kMaxKeyTags] = {};
+        for (uint32_t t = 0; t < K; ++t) u_vslot[t] = carve(VS[t] * 8);
+        const size_t u_tslot = carve(TS * 8);  // every hash table lies in [u_vslot[0], u_tslot + TS * 8): one memset
+        for (uint32_t t = 0; t < K; ++t) {
+            u_vid[t] = carve(tv[t] * 4);
+            u_vals[t] = carve(static_cast<size_t>(cap) * kMaxLit);
+            u_lens[t] = carve(static_cast<size_t>(cap) * 4);
+        }
+        const size_t u_tid = carve(n_tup * 4), u_head = carve(nh * 4), u_tiles = carve(std::max(nh, nr) / 1024 * 4), u_codes = carve(static_cast<size_t>(cap) * 8),
+                     u_comp = carve(CS * 8), u_cranks = carve(CS * 8), u_cfirst = carve(CS * 8), u_cidx = carve(CS * 4), u_rslot = carve(n_rows * 4),
+                     u_rkey = carve(n_rows * 8), u_keys = carve(N * 8), u_seg = carve(nr * 4), u_order = carve(n_rows * 4);
+        Scratch us;
+        CUDA_TRY(us.alloc(carve.o, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl, 0, 64, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl + 12, 0xff, 4, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_vslot[0], 0, u_tslot + TS * 8 - u_vslot[0], s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_comp, 0, CS * 16, s));  // comp, cranks
+        CUDA_TRY(cudaMemsetAsync(us.base + u_cfirst, 0xff, u_rslot - u_cfirst, s));  // cfirst, cidx
+        CUDA_TRY(cudaMemsetAsync(us.base + u_seg, 0, nr * 4, s));
+        CUDA_TRY(cudaMemsetAsync(us.base + u_order, 0xff, n_rows * 4, s));
+        CUDA_TRY(cudaMemcpyAsync(us.base + u_off, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
+        stats.h2d_bytes += offs.size() * 4;
+        const uint32_t *d_off = reinterpret_cast<const uint32_t *>(us.base + u_off);
+        TupleUnionParams up;
+        memset(&up, 0, sizeof up);
+        up.slots = slots0;
+        up.slot_stride = slot;
+        up.F = static_cast<uint32_t>(F);
+        up.NS = static_cast<uint32_t>(NS);
+        up.cap = cap;
+        up.n_ranks = R;
+        up.tmin = q->tmin;
+        up.tmax = q->tmax;
+        up.v_off = d_off;  // the ranks' tuples
+        up.row_off = d_off + (R + 1);
+        up.n_vals = n_tup;
+        up.n_rows = n_rows;
+        up.vmask = static_cast<uint32_t>(TS - 1);
+        up.cmask = static_cast<uint32_t>(CS - 1);
+        up.vslot = reinterpret_cast<unsigned long long *>(us.base + u_tslot);
+        up.vid = reinterpret_cast<uint32_t *>(us.base + u_tid);
+        up.vhead = reinterpret_cast<uint32_t *>(us.base + u_head);
+        up.tiles = reinterpret_cast<uint32_t *>(us.base + u_tiles);
+        up.comp = reinterpret_cast<unsigned long long *>(us.base + u_comp);
+        up.cranks = reinterpret_cast<unsigned long long *>(us.base + u_cranks);
+        up.cfirst = reinterpret_cast<unsigned long long *>(us.base + u_cfirst);
+        up.cidx = reinterpret_cast<uint32_t *>(us.base + u_cidx);
+        up.row_slot = reinterpret_cast<uint32_t *>(us.base + u_rslot);
+        up.row_key = reinterpret_cast<unsigned long long *>(us.base + u_rkey);
+        up.n_sort = static_cast<uint32_t>(N);
+        up.keys = reinterpret_cast<unsigned long long *>(us.base + u_keys);
+        up.seg = reinterpret_cast<uint32_t *>(us.base + u_seg);
+        up.order = reinterpret_cast<uint32_t *>(us.base + u_order);
+        up.ctl = reinterpret_cast<uint32_t *>(us.base + u_ctl);
+        up.n_tags = K;
+        up.tag_ctl = up.ctl + 8;
+        up.codes = reinterpret_cast<unsigned long long *>(us.base + u_codes);
+        for (uint32_t t = 0; t < K; ++t) {
+            TupleTagUnion &tg = up.tags[t];
+            tg.v_off = d_off + 2 * (R + 1) + t * (R + 1);
+            tg.n_vals = tv[t];
+            tg.vmask = static_cast<uint32_t>(VS[t] - 1);
+            tg.vslot = reinterpret_cast<unsigned long long *>(us.base + u_vslot[t]);
+            tg.vid = reinterpret_cast<uint32_t *>(us.base + u_vid[t]);
+            tg.vals = us.base + u_vals[t];
+            tg.lens = reinterpret_cast<uint32_t *>(us.base + u_lens[t]);
+        }
+        // ---- each tag's union and the span check; a tag whose union exceeds the cap stops the call before any code is packed
+        stats.kernel_launches += launch_tuple_tag_union(up, s);
+        uint32_t ctl[16];
+        auto read_ctl = [&]() -> int {
+            CUDA_TRY(cudaMemcpyAsync(es.pinned, up.ctl, 48, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(cudaStreamSynchronize(s));
+            CUDA_TRY(cudaGetLastError());
+            stats.d2h_bytes += 48;
+            memcpy(ctl, es.pinned, 48);
+            return 0;
+        };
+        rc = read_ctl();
+        if (rc) return rc;
+        for (uint32_t t = 0; t < K; ++t)
+            if (ctl[8 + t] > cap)
+                return fail(BYDB_ENOMEM, std::string("tuple collective: more distinct values of the tag ") + keys->keys[t].family + "/" + keys->keys[t].tag +
+                                             " over all ranks than bydb_group_keys.max_values (" + std::to_string(cap) + ")");
+        if (ctl[2] == kErrRankOverlap) {
+            const uint32_t i = ctl[3];
+            return fail(BYDB_ENOTSUP, "tuple collective: series #" + std::to_string(i) + " (id " + std::to_string(i < NS ? q->series_ids[i] : 0) +
+                                          ") lives on several ranks over time spans that intersect");
+        }
+        // ---- the tuple union and the union composites
+        stats.kernel_launches += launch_tuple_union(up, s);
+        rc = read_ctl();
+        if (rc) return rc;
+        if (ctl[0] > cap)
+            return fail(BYDB_ENOMEM, "tuple collective: more distinct key tuples over all ranks than bydb_group_keys.max_values (" + std::to_string(cap) + ")");
+        const size_t T = ctl[0], C = ctl[1];
+        // ---- the union composites in insertion order, folded over their ranks into a table of C_u groups
+        const TableLayout tl(std::max<size_t>(C, 1), F);
+        Carve cf;
+        const size_t f_table = cf(tl.total), f_pairs = cf(C * 8), f_perm = cf(C * 4);
+        Scratch fb;
+        CUDA_TRY(fb.alloc(cf.o, s));
+        up.table = tl.at(fb.base + f_table);
+        up.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
+        up.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
+        if (C) stats.kernel_launches += launch_wide_merge(up, static_cast<uint32_t>(C), s);
+        // the K union tag tables and the T_u union codes, back to back in the staging, in one synchronised read-back
+        size_t at[kMaxKeyTags] = {}, back = 0;
+        for (uint32_t t = 0; t < K; ++t) {
+            const size_t V = ctl[8 + t];
+            at[t] = back;
+            CUDA_TRY(cudaMemcpyAsync(es.pinned + back, up.tags[t].vals, V * kMaxLit, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(cudaMemcpyAsync(es.pinned + back + V * kMaxLit, up.tags[t].lens, V * 4, cudaMemcpyDeviceToHost, s));
+            back += V * (kMaxLit + 4);
+        }
+        CUDA_TRY(cudaMemcpyAsync(es.pinned + back, up.codes, T * 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaGetLastError());
+        stats.d2h_bytes += back + T * 8;
+        for (uint32_t t = 0; t < K; ++t) {
+            const size_t V = ctl[8 + t];
+            u.tag_values[t] = unpack_values(V, false, es.pinned + at[t], reinterpret_cast<const uint32_t *>(es.pinned + at[t] + V * kMaxLit));
+        }
+        u.codes.resize(T);
+        if (T) memcpy(u.codes.data(), es.pinned + back, T * 8);
+        wide_key_tables(out, answer.owner, u);
+        if (C == 0) return 0;
+        WideReduceParams rp;
+        memset(&rp, 0, sizeof rp);
+        rp.pairs = up.pairs;
+        rp.perm = up.perm;
+        rp.ctl = up.ctl;  // ctl[1] = C_u, the present rows keyed_partial_rows_kernel reads
+        rc = wide_emit(q, plan, es, fb.base + f_table, tl, C, rp, out, answer.owner);
+        if (rc) return rc;
+        wide_row_tuples(out, answer.owner, u);
+        return 0;
+    };
+    h.discard = [] {};  // the result of a failed call is freed by `answer`
+    const int rc = run_collective(ctx, root, 0, h);
+    if (rc) return rc;
+    answer.done = true;
+    return 0;
+}
+
+extern "C" {
+
+int bydb_scan_reduce_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root, bydb_keys_result *out) {
+    return guarded([&]() -> int { return scan_reduce_keys_wide_impl(ctx, q, keys, root, out); });
+}
+
+int bydb_scan_reduce_keys_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root,
+                                        bydb_keys_partial_rows *out) {
+    return guarded([&]() -> int { return scan_reduce_keys_wide_impl(ctx, q, keys, root, out); });
 }
 
 int bydb_scan_reduce(bydb_ctx *ctx, const bydb_query *q, int32_t root, bydb_result *out) {

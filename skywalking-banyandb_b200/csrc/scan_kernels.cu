@@ -4051,6 +4051,16 @@ __device__ __forceinline__ KeyedSlot slot_layout(const KeyedUnionParams &p, uint
 __device__ __forceinline__ WideSlot slot_layout(const WideUnionParams &p, uint32_t r) {
     return WideSlot(p.F, p.NS, slot_values(p, r), reinterpret_cast<const SlotHead::Header *>(p.slots + r * p.slot_stride)->C);
 }
+// rank r's tag counts (TupleSlot::Tags) in the tuple collective
+__device__ __forceinline__ const TupleSlot::Tags &slot_tags(const TupleUnionParams &p, uint32_t r) {
+    return *reinterpret_cast<const TupleSlot::Tags *>(p.slots + r * p.slot_stride + sizeof(SlotHead::Header));
+}
+__device__ __forceinline__ TupleSlot slot_layout(const TupleUnionParams &p, uint32_t r) {
+    const TupleSlot::Tags &tg = slot_tags(p, r);
+    uint32_t n_vals = 0;
+    for (uint32_t t = 0; t < tg.K && t < kMaxKeyTags; ++t) n_vals += tg.V[t];
+    return TupleSlot(p.F, p.NS, n_vals, slot_values(p, r), reinterpret_cast<const SlotHead::Header *>(p.slots + r * p.slot_stride)->C);
+}
 
 // One CTA of kMaxKeyValues threads.  Ranks in rank order, each rank's values in its order: thread v looks value v up in a shared
 // open-addressing table of the values so far (homed by key_home, like key_values_kernel's table; byte equality decides -- the
@@ -5450,22 +5460,34 @@ void launch_wide_first(const WideFirstParams &p, cudaStream_t s) {
 }
 
 // rank r's slot (its layout: slot_layout)
-__device__ __forceinline__ const uint8_t *wide_slot_at(const WideUnionParams &p, uint32_t r) { return p.slots + r * p.slot_stride; }
+template <class P>
+__device__ __forceinline__ const uint8_t *wide_slot_at(const P &p, uint32_t r) { return p.slots + r * p.slot_stride; }
 // the rank of flat index t of an exclusive scan over the ranks
 __device__ __forceinline__ uint32_t wide_rank_of(const uint32_t *off, uint32_t n_ranks, uint32_t t) {
     uint32_t r = 0;
     while (r + 1 < n_ranks && off[r + 1] <= t) ++r;
     return r;
 }
+// where the values a value union reads start among rank r's head values: the key's (0), or tag p.tag's
+__device__ __forceinline__ uint32_t union_value_base(const WideUnionParams &, uint32_t) { return 0; }
+__device__ __forceinline__ uint32_t union_value_base(const TupleUnionParams &p, uint32_t r) {
+    const TupleSlot::Tags &tg = slot_tags(p, r);
+    uint32_t b = 0;
+    for (uint32_t t = 0; t < p.tag; ++t) b += tg.V[t];
+    return b;
+}
 // value v of rank r: its bytes and length
-__device__ __forceinline__ const uint8_t *wide_value(const WideUnionParams &p, uint32_t r, uint32_t v, uint32_t &len) {
+template <class P>
+__device__ __forceinline__ const uint8_t *wide_value(const P &p, uint32_t r, uint32_t v, uint32_t &len) {
     const uint8_t *slot = wide_slot_at(p, r);
-    const WideSlot ws = slot_layout(p, r);
+    const auto ws = slot_layout(p, r);
+    v += union_value_base(p, r);
     len = min(reinterpret_cast<const uint32_t *>(slot + ws.off_lens)[v], static_cast<uint32_t>(kMaxLit));
     return slot + ws.off_vals + static_cast<size_t>(v) * kMaxLit;
 }
 
-__global__ void wide_union_insert_kernel(const __grid_constant__ WideUnionParams p) {
+template <class P>
+__global__ void wide_union_insert_kernel(const __grid_constant__ P p) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= p.n_vals) return;
     const uint32_t r = wide_rank_of(p.v_off, p.n_ranks, t), v = t - p.v_off[r];
@@ -5499,7 +5521,8 @@ __global__ void wide_union_heads_kernel(const __grid_constant__ WideUnionParams 
     }
     p.vhead[t] = head;
 }
-__global__ void wide_union_ids_kernel(const __grid_constant__ WideUnionParams p) {
+template <class P>
+__global__ void wide_union_ids_kernel(const __grid_constant__ P p) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= p.n_vals) return;
     const unsigned long long w = p.vslot[p.vid[t]] - 1ull;
@@ -5515,7 +5538,8 @@ __global__ void wide_union_ids_kernel(const __grid_constant__ WideUnionParams p)
 }
 
 // the order of rank r's span among the ranks' spans of series i (by start; a tie, which the span check refuses, by rank)
-__device__ uint32_t wide_span_order(const WideUnionParams &p, uint32_t r, uint32_t i) {
+template <class P>
+__device__ uint32_t wide_span_order(const P &p, uint32_t r, uint32_t i) {
     int64_t lo, hi, olo, ohi;
     if (!rank_span(p, r, i, lo, hi)) return 0;
     uint32_t o = 0;
@@ -5526,12 +5550,13 @@ __device__ uint32_t wide_span_order(const WideUnionParams &p, uint32_t r, uint32
 __device__ __forceinline__ unsigned long long wide_order_key(uint32_t series, uint32_t span_order, uint32_t j) {
     return (static_cast<unsigned long long>(series) << 33) | (static_cast<unsigned long long>(span_order & 63u) << 27) | (j & (kWideMaxRankComposites - 1));
 }
-__global__ void wide_comp_union_kernel(const __grid_constant__ WideUnionParams p) {
+template <class P>
+__global__ void wide_comp_union_kernel(const __grid_constant__ P p) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= p.n_rows) return;
     const uint32_t r = wide_rank_of(p.row_off, p.n_ranks, t), j = t - p.row_off[r];
     const uint8_t *slot = wide_slot_at(p, r);
-    const WideSlot ws = slot_layout(p, r);
+    const auto ws = slot_layout(p, r);
     const int32_t *pair = reinterpret_cast<const int32_t *>(slot + ws.off_pairs) + 2 * static_cast<size_t>(j);
     const uint32_t u = p.vid[p.v_off[r] + static_cast<uint32_t>(pair[1])];
     const unsigned long long key = ((static_cast<unsigned long long>(static_cast<uint32_t>(pair[0])) << 32) | u) + 1ull;
@@ -5558,7 +5583,8 @@ __global__ void wide_comp_keys_kernel(const __grid_constant__ WideUnionParams p)
     p.keys[t] = t < p.n_rows && p.cfirst[p.row_slot[t]] == p.row_key[t] ? p.row_key[t] : ~0ull;
 }
 // composite c < C_u: the row its least key names (the rank whose span of that series has that order) -> its slot
-__global__ void wide_comp_place_kernel(const __grid_constant__ WideUnionParams p, uint32_t n_comp) {
+template <class P>
+__global__ void wide_comp_place_kernel(const __grid_constant__ P p, uint32_t n_comp) {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n_comp) return;
     const unsigned long long k = p.keys[c];
@@ -5588,7 +5614,8 @@ __global__ void wide_comp_order_kernel(const __grid_constant__ WideUnionParams p
 // One thread per word of the union table (c, field) and per column type: composite c's rows in rank order with
 // combine_tables_kernel's per-word rule (deterministic float sums); the column types of every rank merge (merge_coltype), so a
 // field stored as int64 on one rank and float64 on another fails as it does inside one scan.
-__global__ void wide_comp_fold_kernel(const __grid_constant__ WideUnionParams p, uint32_t n_comp) {
+template <class P>
+__global__ void wide_comp_fold_kernel(const __grid_constant__ P p, uint32_t n_comp) {
     const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     const uint64_t F = p.F, CF = static_cast<uint64_t>(n_comp) * F, words = 7 * CF + n_comp;
     if (i >= words + F) return;
@@ -5596,7 +5623,7 @@ __global__ void wide_comp_fold_kernel(const __grid_constant__ WideUnionParams p,
         const uint32_t c = static_cast<uint32_t>(i - words);
         int64_t typ = 0, err = 0;
         for (uint32_t r = 0; r < p.n_ranks; ++r) {
-            const WideSlot ws = slot_layout(p, r);
+            const auto ws = slot_layout(p, r);
             const uint64_t Cr = p.row_off[r + 1] - p.row_off[r];
             merge_coltype(reinterpret_cast<const int64_t *>(wide_slot_at(p, r) + ws.off_table)[7 * Cr * F + Cr + c], typ, err);
         }
@@ -5619,27 +5646,32 @@ __global__ void wide_comp_fold_kernel(const __grid_constant__ WideUnionParams p,
     reinterpret_cast<uint64_t *>(p.table.sum_f64)[i] = a;  // the regions lie back to back from sum_f64 on
 }
 
-uint32_t launch_wide_union(const WideUnionParams &p, cudaStream_t s) {
+// the union of the values p names (the key's, or one tag's): insert, heads, their exclusive scan into ctl[0], ids
+template <class P>
+static uint32_t wide_value_union(const P &p, cudaStream_t s) {
+    if (!p.n_vals) return 0;
     const uint32_t nv = (p.n_vals + 1023u) / 1024u * 1024u;
-    uint32_t n = 0;
-    if (p.n_vals) {
-        wide_union_insert_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
-        wide_union_heads_kernel<<<nv / 256, 256, 0, s>>>(p, nv);
-        launch_excl_scan(p.vhead, nv, p.tiles, &p.ctl[0], s);
-        wide_union_ids_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
-        n += 6;
-    }
-    if (p.NS && p.n_ranks > 1) {
-        rank_span_check_kernel<WideUnionParams, 2><<<(p.NS + 7) / 8, 256, 0, s>>>(p);
-        n += 1;
-    }
-    if (p.n_rows) {
-        wide_comp_union_kernel<<<(p.n_rows + 255) / 256, 256, 0, s>>>(p);
-        n += 1;
-    }
-    return n;
+    wide_union_insert_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
+    wide_union_heads_kernel<<<nv / 256, 256, 0, s>>>(p, nv);
+    launch_excl_scan(p.vhead, nv, p.tiles, &p.ctl[0], s);
+    wide_union_ids_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
+    return 6;
 }
-uint32_t launch_wide_merge(const WideUnionParams &p, uint32_t n_comp, cudaStream_t s) {
+template <class P>
+static uint32_t wide_span_check(const P &p, cudaStream_t s) {
+    if (!p.NS || p.n_ranks < 2) return 0;
+    rank_span_check_kernel<P, 2><<<(p.NS + 7) / 8, 256, 0, s>>>(p);
+    return 1;
+}
+template <class P>
+static uint32_t wide_comp_union(const P &p, cudaStream_t s) {
+    if (!p.n_rows) return 0;
+    wide_comp_union_kernel<<<(p.n_rows + 255) / 256, 256, 0, s>>>(p);
+    return 1;
+}
+uint32_t launch_wide_union(const WideUnionParams &p, cudaStream_t s) { return wide_value_union(p, s) + wide_span_check(p, s) + wide_comp_union(p, s); }
+template <class P>
+static uint32_t wide_merge(const P &p, uint32_t n_comp, cudaStream_t s) {
     const uint32_t N = p.n_sort, nr = (p.n_rows + 1023u) / 1024u * 1024u;
     uint32_t n = 0;
     wide_comp_keys_kernel<<<N / 256, 256, 0, s>>>(p);
@@ -5656,6 +5688,82 @@ uint32_t launch_wide_merge(const WideUnionParams &p, uint32_t n_comp, cudaStream
     const uint64_t words = (7ull * p.F + 1) * n_comp + p.F;
     wide_comp_fold_kernel<<<static_cast<unsigned>((words + 255) / 256), 256, 0, s>>>(p, n_comp);
     return n + 6;
+}
+uint32_t launch_wide_merge(const WideUnionParams &p, uint32_t n_comp, cudaStream_t s) { return wide_merge(p, n_comp, s); }
+uint32_t launch_wide_merge(const TupleUnionParams &p, uint32_t n_comp, cudaStream_t s) { return wide_merge(p, n_comp, s); }
+
+// ---- the tuple collective's root (bydb_scan_reduce_keys_wide).  Flat tuple index t = v_off[r] + j names rank r's tuple j.
+// The union code of rank r's tuple j: its K components, rank r's own tag ids, each recoded through that tag's union ids.  The
+// host has checked that every tag's union fits the cap (at most 65,536), so each union id fits its 16 bits.
+__device__ __forceinline__ unsigned long long tuple_union_code(const TupleUnionParams &p, uint32_t r, uint32_t j) {
+    const unsigned long long code = reinterpret_cast<const unsigned long long *>(wide_slot_at(p, r) + slot_layout(p, r).off_codes)[j];
+    unsigned long long u = 0;
+    for (uint32_t k = 0; k < p.n_tags; ++k) {
+        const TupleTagUnion &tg = p.tags[k];
+        u |= static_cast<unsigned long long>(tg.vid[tg.v_off[r] + static_cast<uint32_t>((code >> (16 * k)) & 0xffffu)]) << (16 * k);
+    }
+    return u;
+}
+// every (r, j) enters a table homed by key_slot_i64 over its union code; the slot keeps the least (r, j) with that code
+__global__ void tuple_union_insert_kernel(const __grid_constant__ TupleUnionParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= p.n_vals) return;
+    const uint32_t r = wide_rank_of(p.v_off, p.n_ranks, t), j = t - p.v_off[r];
+    const unsigned long long code = tuple_union_code(p, r, j), mine = ((static_cast<unsigned long long>(r) << 32) | j) + 1ull;
+    uint32_t s = key_slot_i64(code, p.vmask);
+    for (;;) {  // the table has twice the tuples' slots: a free one is always ahead
+        unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(&p.vslot[s]);
+        if (cur == 0ull) cur = atomicCAS(&p.vslot[s], 0ull, mine);
+        if (cur == 0ull) break;
+        if (tuple_union_code(p, static_cast<uint32_t>((cur - 1ull) >> 32), static_cast<uint32_t>(cur - 1ull)) == code) {
+            atomicMin(&p.vslot[s], mine);
+            break;
+        }
+        s = (s + 1) & p.vmask;
+    }
+    p.vid[t] = s;
+}
+// after wide_union_heads_kernel and the scan numbered the least (r, j) of each code: union tuple u's code (u < cap), and every
+// rank tuple's union id
+__global__ void tuple_union_ids_kernel(const __grid_constant__ TupleUnionParams p) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= p.n_vals) return;
+    const unsigned long long w = p.vslot[p.vid[t]] - 1ull;
+    const uint32_t ro = static_cast<uint32_t>(w >> 32), jo = static_cast<uint32_t>(w);
+    const uint32_t owner = p.v_off[ro] + jo, u = p.vhead[owner];
+    if (owner == t && u < p.cap) p.codes[u] = tuple_union_code(p, ro, jo);
+    p.vid[t] = u;
+}
+
+uint32_t launch_tuple_tag_union(const TupleUnionParams &p, cudaStream_t s) {
+    uint32_t n = 0;
+    TupleUnionParams q = p;
+    for (uint32_t t = 0; t < p.n_tags; ++t) {
+        const TupleTagUnion &tg = p.tags[t];
+        q.tag = t;
+        q.v_off = tg.v_off;
+        q.n_vals = tg.n_vals;
+        q.vmask = tg.vmask;
+        q.vslot = tg.vslot;
+        q.vid = tg.vid;
+        q.vals = tg.vals;
+        q.lens = tg.lens;
+        q.ctl = p.tag_ctl + t;  // the scan's total: V_u,t
+        n += wide_value_union(q, s);
+    }
+    return n + wide_span_check(p, s);
+}
+uint32_t launch_tuple_union(const TupleUnionParams &p, cudaStream_t s) {
+    uint32_t n = 0;
+    if (p.n_vals) {
+        const uint32_t nv = (p.n_vals + 1023u) / 1024u * 1024u;
+        tuple_union_insert_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
+        wide_union_heads_kernel<<<nv / 256, 256, 0, s>>>(p, nv);
+        launch_excl_scan(p.vhead, nv, p.tiles, &p.ctl[0], s);
+        tuple_union_ids_kernel<<<(p.n_vals + 255) / 256, 256, 0, s>>>(p);
+        n += 6;
+    }
+    return n + wide_comp_union(p, s);
 }
 
 void launch_plan_blocks(const ScanParams &p, cudaStream_t s) {

@@ -573,6 +573,48 @@ struct WideUnionParams {
 // -> kernels launched
 uint32_t launch_wide_union(const WideUnionParams &p, cudaStream_t s);
 uint32_t launch_wide_merge(const WideUnionParams &p, uint32_t n_comp, cudaStream_t s);
+// ---- tuple collective (bydb_scan_reduce_keys_wide): the slot of a rank that found T tuples over K tags (tag t: V_t values, n_vals
+// = the sum of the V_t) and C present composite groups, for F fields and NS series.  It is WideSlot(F, NS, n_vals, C) with the tuple
+// codes behind it: span, pairs, first and table mean what they mean there, a pair naming the rank's own tuple id.
+//   head      SlotHead(n_vals): Header.V = T, Header.C = C, and Tags at byte sizeof(Header); lens / values hold tag 0's V_0
+//             values, then tag 1's, ... (a rank's values of tag t start at entry V_0 + .. + V_{t-1})
+//   span, pairs, first, table   as in WideSlot
+//   codes     [T] u64 the rank's tuple codes id_0 | id_1 << 16 | .. in its own tag ids (WidePass::codes)
+struct TupleSlot : WideSlot {
+    struct Tags {
+        uint32_t K, V[kMaxKeyTags];
+    };
+    size_t off_codes, total;  // total: the whole slot (WideSlot::total ends at the table)
+    __host__ __device__ TupleSlot(size_t F, size_t NS, size_t n_vals, size_t T, size_t C) : WideSlot(F, NS, n_vals, C) {
+        off_codes = up(WideSlot::total);
+        total = off_codes + T * 8;
+    }
+};
+// The root of the tuple collective: the wide collective's root with a union per tag and one of the tuples in place of the value
+// union.  The WideUnionParams fields name, in turn, each tag's value union (launch_tuple_tag_union sets them from tags[t]; its
+// v_off / n_vals / vid then count (rank, tag-t value), and ctl points at tag_ctl[t]) and the tuple union (launch_tuple_union:
+// v_off / n_vals / vid count (rank, tuple), vslot keeps the least (r, tuple) per union code, vhead numbers them), whose ids the
+// composite union, the order and the fold then read as the wide collective reads its value ids.
+struct TupleTagUnion {
+    const uint32_t *v_off;            // [n_ranks + 1] exclusive scan of the ranks' V_t
+    uint32_t n_vals, vmask;           // sum of the ranks' V_t; the value table's slots - 1
+    unsigned long long *vslot;        // [vmask + 1]
+    uint32_t *vid;                    // [n_vals] the union id of (r, value)
+    uint8_t *vals;                    // [cap * kMaxLit] the tag's union values
+    uint32_t *lens;                   // [cap]
+};
+struct TupleUnionParams : WideUnionParams {
+    uint32_t n_tags, tag;             // K; the tag whose values a value union reads
+    TupleTagUnion tags[kMaxKeyTags];
+    uint32_t *tag_ctl;                // [K] each tag's union size V_u,t
+    unsigned long long *codes;        // [cap] union tuple u's code in union tag ids
+};
+// each tag's value union, then the span check (ctl[2], ctl[3] as in the wide collective) -> kernels launched
+uint32_t launch_tuple_tag_union(const TupleUnionParams &p, cudaStream_t s);
+// the tuple union (ctl[0] = T_u; only when every V_u,t is at most cap, so that a union tag id fits its 16 bits), then the composite
+// union (ctl[1] = C_u) -> kernels launched
+uint32_t launch_tuple_union(const TupleUnionParams &p, cudaStream_t s);
+uint32_t launch_wide_merge(const TupleUnionParams &p, uint32_t n_comp, cudaStream_t s);
 // dst[j] = src[perm[j]] for every group row of a partial table; coltype = the passes' column types merged
 void launch_permute_table(const TablePtrs &dst, const TablePtrs &src, const int32_t *perm, uint32_t n_groups, uint32_t n_fcols,
                           const int64_t *pass_coltype, uint32_t n_passes, cudaStream_t s);
