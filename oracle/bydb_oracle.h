@@ -188,6 +188,15 @@ typedef struct {
     int func;                /* OB_AGG_* */
 } ob_agg;
 
+/* one component of a group key: a stored tag and its declared type (OB_VT_STR / OB_VT_BINARY or OB_VT_INT64); a block whose
+ * column has another type makes the query fail */
+enum { OB_MAX_GROUP_KEYS = 4 };
+typedef struct {
+    const char *family;
+    const char *tag;
+    int value_type;
+} ob_group_key;
+
 typedef struct {
     int n_parts;
     ob_part *const *parts;
@@ -205,11 +214,13 @@ typedef struct {
     int top_desc;                /* 1 = largest first */
     int threads;                 /* decode threads (goroutine-per-block analogue, query_batch.go:195); <=1 serial */
     int per_thread_partials;     /* 0 = reference-shaped (single-thread merge+agg), 1 = best-effort all-core */
-    /* per-row group key: a stored string / binary tag (NULL = none).  A row's group is (group of its series, tag value);
-     * groups are emitted in insertion order (pkg/query/vectorized/measure/aggregation.go:193-254); a null cell and ""
-     * are the same key (groupby.go:226-254).  Runs the serial fold. */
-    const char *key_family;
-    const char *key_tag;
+    /* per-row group key: a tuple of 1..OB_MAX_GROUP_KEYS stored tags in GroupBy order (n_keys = 0: none).  A row's group is
+     * (group of its series, encoded key); groups are emitted in insertion order (pkg/query/vectorized/measure/aggregation.go:
+     * 193-254).  The key is encoded as computeKey encodes it (aggregation.go:328-337, appendKeyComponent groupby.go:217-254):
+     * an int64 component as 8 little-endian bytes (a nil cell or a block without the column: 0), a string / binary component
+     * as a 4-byte little-endian length and the bytes (nil: "").  Runs the serial fold. */
+    int n_keys;
+    const ob_group_key *keys;
 } ob_query;
 
 typedef struct {
@@ -223,10 +234,10 @@ typedef struct {
     uint64_t rows_scanned;       /* rows decoded from selected blocks (before time trim) */
     uint64_t rows_matched;       /* rows folded */
     uint64_t blocks_scanned;
-    /* only with a group-key tag: group_id[r] is then the SERIES group of row r, key_id[r] its key value */
-    int32_t *key_id;             /* [n_rows] index into keys */
+    /* only with a group key: group_id[r] is then the SERIES group of row r, key[r * n_keys + k] its k-th component -- a
+     * string's bytes, or an int64's 8 little-endian bytes */
     int32_t n_keys;
-    ob_bytes *keys;              /* distinct key values, first-seen order */
+    ob_bytes *key;               /* [n_rows * n_keys] owned */
 } ob_result;
 
 int ob_query_run(const ob_query *q, ob_result *out);

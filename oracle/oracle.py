@@ -60,13 +60,17 @@ class _Agg(C.Structure):
     _fields_ = [("field", C.c_char_p), ("func", C.c_int)]
 
 
+class _GroupKey(C.Structure):
+    _fields_ = [("family", C.c_char_p), ("tag", C.c_char_p), ("value_type", C.c_int)]
+
+
 class _Query(C.Structure):
     _fields_ = [("n_parts", C.c_int), ("parts", C.POINTER(C.c_void_p)), ("n_series", C.c_size_t),
                 ("sids", C.c_void_p), ("groups", C.c_void_p), ("n_groups", C.c_int32),
                 ("tmin", C.c_int64), ("tmax", C.c_int64), ("n_preds", C.c_int), ("preds", C.POINTER(_Pred)),
                 ("n_aggs", C.c_int), ("aggs", C.POINTER(_Agg)), ("top_n", C.c_int), ("top_agg", C.c_int),
                 ("top_desc", C.c_int), ("threads", C.c_int), ("per_thread_partials", C.c_int),
-                ("key_family", C.c_char_p), ("key_tag", C.c_char_p)]
+                ("n_keys", C.c_int), ("keys", C.POINTER(_GroupKey))]
 
 
 class _Result(C.Structure):
@@ -74,7 +78,7 @@ class _Result(C.Structure):
                 ("rows", C.POINTER(C.c_int64)), ("is_float", C.POINTER(C.c_uint8)),
                 ("val_i64", C.POINTER(C.c_int64)), ("val_f64", C.POINTER(C.c_double)),
                 ("rows_scanned", C.c_uint64), ("rows_matched", C.c_uint64), ("blocks_scanned", C.c_uint64),
-                ("key_id", C.POINTER(C.c_int32)), ("n_keys", C.c_int32), ("keys", C.POINTER(_Bytes))]
+                ("n_keys", C.c_int32), ("key", C.POINTER(_Bytes))]
 
 
 class _Rows(C.Structure):
@@ -533,7 +537,9 @@ class Query:
     top_desc: bool = True
     threads: int = 1
     per_thread_partials: bool = False
-    group_key: Optional[Tuple[str, str]] = None  # (family, tag): per-row group key, a stored string / binary tag
+    group_key: Optional[Tuple[str, str]] = None  # (family, tag): shorthand for group_keys=[(family, tag, VT_STR)]
+    # per-row group key: 1..4 stored tags (family, tag, VT_STR / VT_BINARY / VT_INT64) in GroupBy order
+    group_keys: Optional[Sequence[Tuple[str, str, int]]] = None
 
 
 @dataclass
@@ -546,7 +552,9 @@ class Result:
     rows_scanned: int
     rows_matched: int
     blocks_scanned: int
-    key: Optional[List[bytes]] = None  # [n_rows] key value of each row (queries with group_key)
+    # [n_rows] key of each row (queries with a group key): with one component its bytes, with K >= 2 a tuple of K components;
+    # a string component is its bytes, an int64 one its 8 little-endian bytes
+    key: Optional[List[object]] = None
 
     def value(self, row: int, agg: int):
         return float(self.val_f64[row, agg]) if self.is_float[agg] else int(self.val_i64[row, agg])
@@ -599,11 +607,23 @@ def _mk_query(q: Query):
     cq.n_aggs, cq.aggs = len(q.aggs), aggs
     cq.top_n, cq.top_agg, cq.top_desc = q.top_n, q.top_agg, int(q.top_desc)
     cq.threads, cq.per_thread_partials = q.threads, int(q.per_thread_partials)
-    if q.group_key is not None:
-        kf, kt = q.group_key[0].encode(), q.group_key[1].encode()
-        keep.extend([kf, kt])
-        cq.key_family, cq.key_tag = kf, kt
+    gks = _group_keys(q)
+    keys = (_GroupKey * max(len(gks), 1))()
+    for i, (fam, tag, vt) in enumerate(gks):
+        fb, tb = fam.encode(), tag.encode()
+        keep.extend([fb, tb])
+        keys[i].family, keys[i].tag, keys[i].value_type = fb, tb, vt
+    keep.append(keys)
+    cq.n_keys, cq.keys = len(gks), keys
     return cq, keep
+
+
+def _group_keys(q: Query) -> List[Tuple[str, str, int]]:
+    if q.group_keys is not None:
+        if q.group_key is not None:
+            raise ValueError("group_key and group_keys both set")
+        return list(q.group_keys)
+    return [] if q.group_key is None else [(q.group_key[0], q.group_key[1], VT_STR)]
 
 
 def run_query(q: Query) -> Result:
@@ -619,9 +639,10 @@ def run_query(q: Query) -> Result:
         val_i64=np.ctypeslib.as_array(r.val_i64, (max(n, 1) * max(a, 1),))[:n * a].copy().reshape(n, a),
         val_f64=np.ctypeslib.as_array(r.val_f64, (max(n, 1) * max(a, 1),))[:n * a].copy().reshape(n, a),
         rows_scanned=r.rows_scanned, rows_matched=r.rows_matched, blocks_scanned=r.blocks_scanned)
-    if q.group_key is not None:
-        keys = [C.string_at(r.keys[k].p, r.keys[k].len) if r.keys[k].len > 0 else b"" for k in range(r.n_keys)]
-        res.key = [keys[r.key_id[i]] for i in range(n)]
+    K = r.n_keys
+    if K:
+        parts = [C.string_at(r.key[j].p, r.key[j].len) if r.key[j].len > 0 else b"" for j in range(n * K)]
+        res.key = parts if K == 1 else [tuple(parts[i * K:(i + 1) * K]) for i in range(n)]
     lib().ob_result_free(C.byref(r))
     return res
 

@@ -189,8 +189,8 @@ static int decode_numeric(const uint8_t *src, size_t srclen, int value_type, siz
     return 0;
 }
 
-/* tag columns a cursor loads: one per predicate, plus the group-key tag (last) when the query has one */
-static int n_tag_cols(const ob_query *q) { return q->n_preds + (q->key_tag ? 1 : 0); }
+/* tag columns a cursor loads: one per predicate, then one per group-key component */
+static int n_tag_cols(const ob_query *q) { return q->n_preds + q->n_keys; }
 
 static void cursor_free(cursor *c, int n_fcols, int n_preds) {
     free(c->ts);
@@ -297,8 +297,8 @@ static int load_cursor(scan *s, cursor *c) {
     const int n_tcols = n_tag_cols(q);
     c->tags = (tcol *)calloc((size_t)(n_tcols ? n_tcols : 1), sizeof(tcol));
     for (int t = 0; t < n_tcols; t++) {
-        const char *t_family = t < q->n_preds ? q->preds[t].family : q->key_family;
-        const char *t_tag = t < q->n_preds ? q->preds[t].tag : q->key_tag;
+        const char *t_family = t < q->n_preds ? q->preds[t].family : q->keys[t - q->n_preds].family;
+        const char *t_tag = t < q->n_preds ? q->preds[t].tag : q->keys[t - q->n_preds].tag;
         const obi_fammeta *fm = NULL;
         for (size_t k = 0; k < c->bm.n_fams; k++)
             if (strcmp(c->bm.fams[k].name, t_family) == 0) fm = &c->bm.fams[k];
@@ -475,76 +475,110 @@ typedef struct {
 /* ------------------------------------------------------------------ per-series merge (query.go:912-1025) */
 typedef struct {
     int32_t gid;    /* group of the row's series */
-    int32_t key_id; /* index into folder.keys */
+    uint64_t hash;  /* comp_hash(gid, key) */
+    ob_bytes key;   /* encoded key (owned) */
 } comp;
 
 typedef struct {
     scan *s;
-    group *groups;   /* [n_groups]; with a group-key tag: [n_comp], one per (series group, key value) in first-seen order */
+    group *groups;   /* [n_groups]; with a group key: [n_comp], one per (series group, encoded key) in first-seen order */
     int *agg_float;  /* [n_aggs] -1 unknown, 0 int, 1 float */
     uint64_t rows_matched;
     ob_rows *rows_out; /* optional raw dump */
     size_t rows_cap;
-    /* per-row group key (a stored tag): pkg/query/vectorized/measure/aggregation.go:193-254 -- the group of a row is found by
-     * its encoded key (groupby.go:226-254: strings / bytes as length + raw bytes, so a null cell and "" are the same key),
-     * new groups are appended to the insertion list and emitted in that order */
+    /* per-row group key: pkg/query/vectorized/measure/aggregation.go:193-254 -- the group of a row is found by its encoded key
+     * (encode_key); new groups are appended to the insertion list and emitted in that order */
     int keyed;
     comp *comps;
     size_t n_comp, cap_comp, last_comp;
-    ob_bytes *keys; /* distinct key values, first-seen order; owned copies */
-    size_t n_keys, cap_keys;
+    int32_t *slots; /* open addressing over comps by hash, -1 = empty; at most half full */
+    size_t slot_mask;
+    ob_buf kbuf;    /* the current row's encoded key */
     int key_bad_type;
 } folder;
 
+static uint64_t comp_hash(int32_t gid, const uint8_t *p, size_t n) {
+    uint64_t h = (0xcbf29ce484222325ull ^ (uint32_t)gid) * 0x100000001b3ull;
+    for (size_t i = 0; i < n; i++) h = (h ^ p[i]) * 0x100000001b3ull;
+    return h ^ (h >> 29);
+}
+
+/* computeKey (aggregation.go:328-337) with appendKeyComponent (groupby.go:217-254), one component per key in GroupBy order:
+ * int64 -> 8 little-endian bytes (a nil cell or a block without the column: 0); string / binary -> 4-byte little-endian length,
+ * then the bytes (nil: "").  -1 when a block stores a key column with another type than the key declares. */
+static int encode_key(const ob_query *q, const cursor *c, size_t row, ob_buf *dst) {
+    ob_buf_reset(dst);
+    for (int k = 0; k < q->n_keys; k++) {
+        const tcol *kc = &c->tags[q->n_preds + k];
+        const ob_bytes *cell = kc->present && kc->cells[row].len >= 0 ? &kc->cells[row] : NULL;
+        uint8_t b[8];
+        if (q->keys[k].value_type == OB_VT_INT64) {
+            if (kc->present && kc->value_type != OB_VT_INT64) return -1;
+            if (cell && cell->len != 8) return -1;
+            uint64_t v = cell ? (uint64_t)ob_conv_bytes_to_int64(cell->p) : 0;
+            for (int i = 0; i < 8; i++) b[i] = (uint8_t)(v >> (8 * i));
+            ob_buf_append(dst, b, 8);
+        } else {
+            if (kc->present && kc->value_type != OB_VT_STR && kc->value_type != OB_VT_BINARY) return -1;
+            uint32_t n = cell ? (uint32_t)cell->len : 0;
+            for (int i = 0; i < 4; i++) b[i] = (uint8_t)(n >> (8 * i));
+            ob_buf_append(dst, b, 4);
+            if (n) ob_buf_append(dst, cell->p, n);
+        }
+    }
+    return 0;
+}
+
+static void slots_resize(folder *fo, size_t n_slots) {
+    free(fo->slots);
+    fo->slots = (int32_t *)malloc(sizeof(int32_t) * n_slots);
+    for (size_t i = 0; i < n_slots; i++) fo->slots[i] = -1;
+    fo->slot_mask = n_slots - 1;
+    for (size_t ci = 0; ci < fo->n_comp; ci++) {
+        size_t s = fo->comps[ci].hash & fo->slot_mask;
+        while (fo->slots[s] >= 0) s = (s + 1) & fo->slot_mask;
+        fo->slots[s] = (int32_t)ci;
+    }
+}
+
 static int32_t keyed_group(folder *fo, const cursor *c, size_t row, int32_t gid) {
     const ob_query *q = fo->s->q;
-    const tcol *kc = &c->tags[q->n_preds];
-    const uint8_t *kp = NULL;
-    size_t kl = 0;
-    if (kc->present) {
-        if (kc->value_type != OB_VT_STR && kc->value_type != OB_VT_BINARY) {
-            fo->key_bad_type = 1;
-            return -1;
-        }
-        if (kc->cells[row].len > 0) {
-            kp = kc->cells[row].p;
-            kl = (size_t)kc->cells[row].len;
-        }
+    if (encode_key(q, c, row, &fo->kbuf) != 0) {
+        fo->key_bad_type = 1;
+        return -1;
     }
+    const uint8_t *kp = fo->kbuf.p;
+    const size_t kl = fo->kbuf.len; /* >= 4: every key has a component */
     if (fo->n_comp) { /* runs of equal keys are the common case */
         const comp *lc = &fo->comps[fo->last_comp];
-        const ob_bytes *lk = &fo->keys[lc->key_id];
-        if (lc->gid == gid && (size_t)lk->len == kl && (kl == 0 || memcmp(lk->p, kp, kl) == 0)) return (int32_t)fo->last_comp;
+        if (lc->gid == gid && (size_t)lc->key.len == kl && memcmp(lc->key.p, kp, kl) == 0) return (int32_t)fo->last_comp;
     }
-    size_t kid = 0;
-    for (; kid < fo->n_keys; kid++)
-        if ((size_t)fo->keys[kid].len == kl && (kl == 0 || memcmp(fo->keys[kid].p, kp, kl) == 0)) break;
-    if (kid == fo->n_keys) {
-        if (fo->n_keys == fo->cap_keys) {
-            fo->cap_keys = fo->cap_keys ? fo->cap_keys * 2 : 16;
-            fo->keys = (ob_bytes *)realloc(fo->keys, sizeof(ob_bytes) * fo->cap_keys);
+    if (2 * (fo->n_comp + 1) > fo->slot_mask + 1) slots_resize(fo, fo->slots ? 2 * (fo->slot_mask + 1) : 1024);
+    const uint64_t h = comp_hash(gid, kp, kl);
+    size_t s = h & fo->slot_mask;
+    for (; fo->slots[s] >= 0; s = (s + 1) & fo->slot_mask) {
+        const comp *cc = &fo->comps[fo->slots[s]];
+        if (cc->hash == h && cc->gid == gid && (size_t)cc->key.len == kl && memcmp(cc->key.p, kp, kl) == 0) {
+            fo->last_comp = (size_t)fo->slots[s];
+            return fo->slots[s];
         }
-        uint8_t *cp = (uint8_t *)malloc(kl ? kl : 1);
-        if (kl) memcpy(cp, kp, kl);
-        fo->keys[kid].p = cp;
-        fo->keys[kid].len = (int64_t)kl;
-        fo->n_keys++;
     }
-    size_t ci = 0;
-    for (; ci < fo->n_comp; ci++)
-        if (fo->comps[ci].gid == gid && (size_t)fo->comps[ci].key_id == kid) break;
-    if (ci == fo->n_comp) {
-        if (fo->n_comp == fo->cap_comp) {
-            fo->cap_comp = fo->cap_comp ? fo->cap_comp * 2 : 16;
-            fo->comps = (comp *)realloc(fo->comps, sizeof(comp) * fo->cap_comp);
-            fo->groups = (group *)realloc(fo->groups, sizeof(group) * fo->cap_comp);
-        }
-        fo->comps[ci].gid = gid;
-        fo->comps[ci].key_id = (int32_t)kid;
-        memset(&fo->groups[ci], 0, sizeof(group));
-        fo->groups[ci].slots = (slot *)calloc((size_t)(q->n_aggs ? q->n_aggs : 1), sizeof(slot));
-        fo->n_comp++;
+    const size_t ci = fo->n_comp;
+    if (ci == fo->cap_comp) {
+        fo->cap_comp = fo->cap_comp ? fo->cap_comp * 2 : 16;
+        fo->comps = (comp *)realloc(fo->comps, sizeof(comp) * fo->cap_comp);
+        fo->groups = (group *)realloc(fo->groups, sizeof(group) * fo->cap_comp);
     }
+    uint8_t *cp = (uint8_t *)malloc(kl);
+    memcpy(cp, kp, kl);
+    fo->comps[ci].gid = gid;
+    fo->comps[ci].hash = h;
+    fo->comps[ci].key.p = cp;
+    fo->comps[ci].key.len = (int64_t)kl;
+    memset(&fo->groups[ci], 0, sizeof(group));
+    fo->groups[ci].slots = (slot *)calloc((size_t)(q->n_aggs ? q->n_aggs : 1), sizeof(slot));
+    fo->slots[s] = (int32_t)ci;
+    fo->n_comp++;
     fo->last_comp = ci;
     return (int32_t)ci;
 }
@@ -776,9 +810,10 @@ static void folder_free(folder *fo, int32_t n_groups) {
     for (int32_t g = 0; g < n_groups; g++) free(fo->groups[g].slots);
     free(fo->groups);
     free(fo->agg_float);
-    for (size_t k = 0; k < fo->n_keys; k++) free((void *)fo->keys[k].p);
-    free(fo->keys);
+    for (size_t k = 0; k < fo->n_comp; k++) free((void *)fo->comps[k].key.p);
     free(fo->comps);
+    free(fo->slots);
+    ob_buf_free(&fo->kbuf);
 }
 
 typedef struct {
@@ -807,6 +842,17 @@ int ob_query_run(const ob_query *q, ob_result *out) {
         ob_set_error("too many aggregations");
         return -1;
     }
+    if (q->n_keys < 0 || q->n_keys > OB_MAX_GROUP_KEYS) {
+        ob_set_error("a group key has 1 to 4 components");
+        return -1;
+    }
+    for (int k = 0; k < q->n_keys; k++) {
+        const int vt = q->keys[k].value_type;
+        if (vt != OB_VT_STR && vt != OB_VT_BINARY && vt != OB_VT_INT64) {
+            ob_set_error("group key type must be string, binary or int64");
+            return -1;
+        }
+    }
     int32_t ng = q->groups ? q->n_groups : 1;
     if (ng < 1) ng = 1;
     scan s;
@@ -821,7 +867,7 @@ int ob_query_run(const ob_query *q, ob_result *out) {
     for (size_t i = 0; i < s.n_cur; i++) sorted[i] = &s.cur[i];
     qsort(sorted, s.n_cur, sizeof(cursor *), cursor_cmp);
 
-    const int keyed = q->key_tag != NULL;
+    const int keyed = q->n_keys > 0;
     folder total = folder_new(&s, keyed ? 0 : ng);
     total.keyed = keyed;
     int rc = 0;
@@ -882,7 +928,7 @@ int ob_query_run(const ob_query *q, ob_result *out) {
         }
     }
     if (rc == 0 && total.key_bad_type) {
-        ob_set_error("group key must be a string / binary tag");
+        ob_set_error("group key tag stored with another value type than the key declares");
         rc = -1;
     }
     if (rc != 0) {
@@ -924,15 +970,8 @@ int ob_query_run(const ob_query *q, ob_result *out) {
     }
     out->n_rows = nrows;
     if (keyed) {
-        out->key_id = (int32_t *)calloc((size_t)(nrows ? nrows : 1), sizeof(int32_t));
-        out->n_keys = (int32_t)total.n_keys;
-        out->keys = (ob_bytes *)calloc(total.n_keys ? total.n_keys : 1, sizeof(ob_bytes));
-        for (size_t k2 = 0; k2 < total.n_keys; k2++) {
-            uint8_t *cp = (uint8_t *)malloc(total.keys[k2].len ? (size_t)total.keys[k2].len : 1);
-            memcpy(cp, total.keys[k2].p, (size_t)total.keys[k2].len);
-            out->keys[k2].p = cp;
-            out->keys[k2].len = total.keys[k2].len;
-        }
+        out->n_keys = q->n_keys;
+        out->key = (ob_bytes *)calloc((size_t)(nrows ? nrows : 1) * (size_t)q->n_keys, sizeof(ob_bytes));
     }
     out->group_id = (int32_t *)calloc((size_t)(nrows ? nrows : 1), sizeof(int32_t));
     out->rows = (int64_t *)calloc((size_t)(nrows ? nrows : 1), sizeof(int64_t));
@@ -942,7 +981,21 @@ int ob_query_run(const ob_query *q, ob_result *out) {
     for (int32_t r = 0; r < nrows; r++) {
         int32_t g = ents[r].g;
         out->group_id[r] = keyed ? total.comps[g].gid : g;
-        if (keyed) out->key_id[r] = total.comps[g].key_id;
+        if (keyed) { /* the encoded key back into its components */
+            const uint8_t *kp = total.comps[g].key.p;
+            for (int k = 0; k < q->n_keys; k++) {
+                size_t n = 8;
+                if (q->keys[k].value_type != OB_VT_INT64) {
+                    n = (size_t)kp[0] | (size_t)kp[1] << 8 | (size_t)kp[2] << 16 | (size_t)kp[3] << 24;
+                    kp += 4;
+                }
+                uint8_t *cp = (uint8_t *)malloc(n ? n : 1);
+                if (n) memcpy(cp, kp, n);
+                kp += n;
+                out->key[(size_t)r * (size_t)q->n_keys + (size_t)k].p = cp;
+                out->key[(size_t)r * (size_t)q->n_keys + (size_t)k].len = (int64_t)n;
+            }
+        }
         out->rows[r] = total.groups[g].rows;
         for (int a = 0; a < q->n_aggs; a++) {
             const slot *sl = &total.groups[g].slots[a];
@@ -960,9 +1013,9 @@ int ob_query_run(const ob_query *q, ob_result *out) {
 }
 
 void ob_result_free(ob_result *r) {
-    for (int32_t k = 0; k < r->n_keys; k++) free((void *)r->keys[k].p);
-    free(r->keys);
-    free(r->key_id);
+    if (r->key)
+        for (size_t k = 0; k < (size_t)r->n_rows * (size_t)r->n_keys; k++) free((void *)r->key[k].p);
+    free(r->key);
     free(r->group_id);
     free(r->rows);
     free(r->is_float);

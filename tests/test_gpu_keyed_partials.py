@@ -88,9 +88,10 @@ GID = {1: 0, 2: 1, 3: 0, 4: 1}
 def oracle_rows(oq, aggs, okey):
     """the rows a node answers with, made from the oracle's keyed queries: Partial.Value per function (MEAN: SUM's), Partial.Count
     (MEAN: COUNT's), typed like the field (COUNT of a float field is a float).  The oracle takes at most 30 aggregations: it runs
-    the distinct ones."""
+    the distinct ones.  okey: the string tag to key on, or None for the group key oq already names."""
     uniq = list(dict.fromkeys(aggs))
-    own = {fn: O.run_query(dataclasses.replace(oq, aggs=[(f, fn) for f, _ in uniq], group_key=(FAM, okey))) for fn in (SUM, COUNT, MIN, MAX)}
+    key = {} if okey is None else dict(group_key=(FAM, okey))
+    own = {fn: O.run_query(dataclasses.replace(oq, aggs=[(f, fn) for f, _ in uniq], **key)) for fn in (SUM, COUNT, MIN, MAX)}
     s = own[SUM]
     n, A = s.group_id.size, len(aggs)
     col = [uniq.index(x) for x in aggs]
