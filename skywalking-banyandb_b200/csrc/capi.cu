@@ -2270,6 +2270,35 @@ int keyed_call(bydb_ctx *ctx, const bydb_query *q, const Key *key, uint32_t max_
     return 0;
 }
 
+// The same preamble in the prepare hook of a keyed collective (run_collective holds the device, the slot and the answer): the
+// arguments and the key, the plan, and the refusal of parts of this rank that overlap in time
+template <class Key>
+int keyed_collective_call(bydb_ctx *ctx, const bydb_query *q, const Key *key, uint32_t max_cap, bool pred_slot, uint32_t &cap, Plan &plan) {
+    int rc = validate_query(q, true);
+    if (!rc) rc = check_group_key(q, key, max_cap, pred_slot, cap);
+    if (!rc) rc = make_plan(ctx, q, nullptr, plan);
+    if (rc) return rc;
+    if (parts_overlap(plan.parts, q->tmin, q->tmax))
+        return fail(BYDB_ENOTSUP, "group-key query over parts of one rank that overlap in time (version dedup) is not supported on the device path");
+    return 0;
+}
+
+// A bydb_*_reduce_slot_bytes call (host only): the arguments, the key (as keyed_call checks it) and the query's shape, then
+// *out = size(plan, cap)
+template <class Key, class Size>
+int reduce_slot_bytes(const bydb_query *q, const Key *key, uint32_t max_cap, bool pred_slot, uint64_t *out, Size size) {
+    return guarded([&]() -> int {
+        if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
+        int rc = validate_query(q, false);
+        uint32_t cap = 0;
+        if (!rc) rc = check_group_key(q, key, max_cap, pred_slot, cap);
+        Plan plan;
+        if (!rc) rc = query_shape(q, plan);
+        if (!rc) *out = size(plan, cap);
+        return rc;
+    });
+}
+
 // bydb_scan_agg_keyed and bydb_scan_partials_keyed: discovery, the per-value passes, the order, then the form's own answer
 template <class Out>
 int scan_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, Out *out) {
@@ -2663,6 +2692,20 @@ const bydb_group_key *key_list(const bydb_group_keys *keys) { return keys->keys;
 uint32_t key_count(const bydb_group_key *) { return 1; }
 uint32_t key_count(const bydb_group_keys *keys) { return keys->n_keys; }
 
+// What a wide fold (WideReduceParams) or the wide collective's merge (WideUnionParams) writes for C composite groups: the table of
+// layout tl = TableLayout(max(C, 1), F) at fb.base, then pairs [2C] and perm [C], in one scratch allocation; sets p.table / pairs /
+// perm
+template <class P>
+int fold_table(const TableLayout &tl, size_t C, Scratch &fb, P &p, cudaStream_t s) {
+    Carve cf;
+    const size_t f_table = cf(tl.total), f_pairs = cf(C * 8), f_perm = cf(C * 4);
+    CUDA_TRY(fb.alloc(cf.o, s));
+    p.table = tl.at(fb.base + f_table);
+    p.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
+    p.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
+    return 0;
+}
+
 // bydb_scan_agg_keyed_wide / bydb_scan_partials_keyed_wide (Key = bydb_group_key) and bydb_scan_agg_keys_wide /
 // bydb_scan_partials_keys_wide (Key = bydb_group_keys)
 template <class Out, class Key>
@@ -2690,17 +2733,13 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const Key *key, Out
     const size_t n_comp = w.n_comp;
     WideReduceParams &rp = w.rp;
     const TableLayout tl(std::max<size_t>(n_comp, 1), F);
-    Carve cf;
-    const size_t f_table = cf(tl.total), f_pairs = cf(n_comp * 8), f_perm = cf(n_comp * 4);
     Scratch fb;
-    CUDA_TRY(fb.alloc(cf.o, stream));
-    rp.table = tl.at(fb.base + f_table);
-    rp.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
-    rp.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
+    rc = fold_table(tl, n_comp, fb, rp, stream);
+    if (rc) return rc;
     launch_wide_fold(rp, static_cast<uint32_t>(n_comp), stream);
     CUDA_TRY(cudaEventRecord(slot.ev[3], stream));
     stats.kernel_launches += 1;
-    if (n_comp > 0) rc = wide_emit(q, plan, slot, fb.base + f_table, tl, n_comp, rp, out, answer.owner);
+    if (n_comp > 0) rc = wide_emit(q, plan, slot, fb.base, tl, n_comp, rp, out, answer.owner);
     if (rc) return rc;
     if (n_comp > 0) wide_row_tuples(out, answer.owner, w);
     {
@@ -4521,18 +4560,7 @@ static int read_slot_heads(const uint8_t *slots0, size_t slot, uint32_t R, uint6
 }
 
 int bydb_keyed_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t *out) {
-    return guarded([&]() -> int {
-    if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
-    int rc = validate_query(q, false);
-    uint32_t cap = 0;
-    if (!rc) rc = check_group_key(q, key, kMaxKeyValues, true, cap);
-    if (rc) return rc;
-    Plan plan;
-    rc = query_shape(q, plan);
-    if (rc) return rc;
-    *out = keyed_slot(plan, cap).total;
-    return 0;
-    });
+    return reduce_slot_bytes(q, key, kMaxKeyValues, true, out, [](const Plan &plan, uint32_t cap) { return keyed_slot(plan, cap).total; });
 }
 
 // The keyed collective: discovery and the per-value passes of bydb_scan_agg_keyed on every rank, written into its slot of the
@@ -4556,13 +4584,8 @@ static int scan_reduce_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb
     uint64_t fp = 0;
     CollectiveHooks h;
     h.prepare = [&](ExecSlot &es, size_t slot) -> int {
-        int rc = validate_query(q, true);
-        if (!rc) rc = check_group_key(q, key, kMaxKeyValues, true, cap);
-        if (!rc) rc = make_plan(ctx, q, nullptr, plan);
-        if (rc) return rc;
-        if (parts_overlap(plan.parts, q->tmin, q->tmax))
-            return fail(BYDB_ENOTSUP, "group-key query over parts of one rank that overlap in time (version dedup) is not supported on the device path");
-        rc = discover_keys(ctx, q, key, cap, plan, es, &stats, values);
+        int rc = keyed_collective_call(ctx, q, key, kMaxKeyValues, true, cap, plan);
+        if (!rc) rc = discover_keys(ctx, q, key, cap, plan, es, &stats, values);
         if (rc) return rc;
         const size_t V = values.size(), G = static_cast<size_t>(plan.n_groups), F = plan.fcols.size();
         if (G * cap > 0x7fffffffull / std::max<size_t>(F, 1)) return fail(BYDB_ENOMEM, "group-key query: too many composite groups");
@@ -4670,26 +4693,321 @@ int bydb_scan_reduce_keyed_partials(bydb_ctx *ctx, const bydb_query *q, const by
 }
 
 int bydb_keyed_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_key *key, uint64_t max_present, uint64_t *out) {
-    return guarded([&]() -> int {
-    if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
-    int rc = validate_query(q, false);
-    uint32_t cap = 0;
-    if (!rc) rc = check_group_key(q, key, kMaxWideKeyValues, false, cap);
-    if (rc) return rc;
-    Plan plan;
-    rc = query_shape(q, plan);
-    if (rc) return rc;
-    *out = WideSlot(plan.fcols.size(), q->n_series, cap, max_present).total;
-    return 0;
+    return reduce_slot_bytes(q, key, kMaxWideKeyValues, false, out,
+                             [&](const Plan &plan, uint32_t cap) { return WideSlot(plan.fcols.size(), q->n_series, cap, max_present).total; });
+}
+
+int bydb_keys_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_keys *keys, uint64_t max_present, uint64_t *out) {
+    return reduce_slot_bytes(q, keys, kMaxWideKeyValues, false, out, [&](const Plan &plan, uint32_t cap) {
+        return TupleSlot(plan.fcols.size(), q->n_series, static_cast<size_t>(keys->n_keys) * cap, cap, max_present).total;
     });
 }
 }  // extern "C"
 
-// the keyed fingerprint of the wide form: a rank of the per-value collective in the same round does not match it
-static uint64_t keyed_wide_fingerprint(const bydb_query *q, const bydb_group_key *key, uint32_t cap) {
+// ---- the wide collective over one key (bydb_group_key) or a tuple key (bydb_group_keys): scan_reduce_wide_impl.  What depends on
+// the key's form is in the overloads that follow, one per form.
+
+// The fingerprint of a form: the keyed fingerprint of its (first) key, then "wide" -- a rank of the per-value collective in the same
+// round does not match it -- or K, every other key (family, tag, value type) in GroupBy order and "tuple"
+static uint64_t wide_fingerprint(const bydb_query *q, const bydb_group_key *key, uint32_t cap) {
     uint64_t h = keyed_fingerprint(q, key, cap);
     for (const char *s = "wide"; *s; ++s) h = (h ^ static_cast<uint8_t>(*s)) * 0x100000001b3ull;
     return h;
+}
+static uint64_t wide_fingerprint(const bydb_query *q, const bydb_group_keys *keys, uint32_t cap) {
+    uint64_t h = keyed_fingerprint(q, &keys->keys[0], cap);
+    auto mix = [&](const void *p, size_t n) {
+        const uint8_t *b = static_cast<const uint8_t *>(p);
+        for (size_t i = 0; i < n; ++i) h = (h ^ b[i]) * 0x100000001b3ull;
+    };
+    const uint64_t K = keys->n_keys;
+    mix(&K, sizeof K);
+    for (uint32_t t = 1; t < keys->n_keys; ++t) {
+        const bydb_group_key &k = keys->keys[t];
+        const uint64_t nf = strlen(k.family), nt = strlen(k.tag), vt = k.value_type;
+        mix(&nf, 8);
+        mix(k.family, nf);
+        mix(&nt, 8);
+        mix(k.tag, nt);
+        mix(&vt, 8);
+    }
+    mix("tuple", 5);
+    return h;
+}
+
+// the values a tuple key's pass found over all its tags
+static size_t tag_value_count(const WidePass &w) {
+    size_t n = 0;
+    for (const KeyValues &vals : w.tag_values) n += vals.size();
+    return n;
+}
+
+// A rank's slot after its pass `w`: a WideSlot over its values, or a TupleSlot over its tags' values and its tuples.  A pass that
+// found nothing gives the slot's fixed part.
+static WideSlot rank_slot(const bydb_group_key *, const Plan &plan, const WidePass &w) {
+    return WideSlot(plan.fcols.size(), plan.n_series, w.values.size(), w.n_comp);
+}
+static TupleSlot rank_slot(const bydb_group_keys *, const Plan &plan, const WidePass &w) {
+    return TupleSlot(plan.fcols.size(), plan.n_series, tag_value_count(w), w.codes.size(), w.n_comp);
+}
+
+// the refusal of a rank whose slot needs `bytes`, more than the mailbox slots (or whose list of composite groups is too long)
+static std::string slot_refusal(const bydb_group_key *, const WidePass &w, size_t bytes) {
+    return "wide keyed collective: this rank's " + std::to_string(w.values.size()) + " key values and " + std::to_string(w.n_comp) +
+           " composite groups need " + std::to_string(bytes) +
+           " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keyed_wide_reduce_slot_bytes)";
+}
+static std::string slot_refusal(const bydb_group_keys *, const WidePass &w, size_t bytes) {
+    return "tuple collective: this rank's " + std::to_string(tag_value_count(w)) + " tag values, " + std::to_string(w.codes.size()) + " tuples and " +
+           std::to_string(w.n_comp) + " composite groups need " + std::to_string(bytes) +
+           " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keys_wide_reduce_slot_bytes)";
+}
+
+// A rank's slot head: its values (put_slot_head); or its tags' values back to back with Header.V = T, each tag's count in the Tags
+// behind the header, and its tuple codes behind the table
+static int put_wide_head(const bydb_group_key *, uint8_t *my_slot, const WideSlot &, uint64_t fp, const WidePass &w, cudaStream_t s) {
+    return put_slot_head(my_slot, fp, w.values, static_cast<uint32_t>(w.n_comp), s);
+}
+static int put_wide_head(const bydb_group_keys *keys, uint8_t *my_slot, const TupleSlot &ts, uint64_t fp, const WidePass &w, cudaStream_t s) {
+    KeyValues all;
+    TupleSlot::Tags tg{};
+    tg.K = keys->n_keys;
+    for (uint32_t t = 0; t < tg.K && t < w.tag_values.size(); ++t) {
+        tg.V[t] = static_cast<uint32_t>(w.tag_values[t].size());
+        all.insert(all.end(), w.tag_values[t].begin(), w.tag_values[t].end());
+    }
+    const size_t T = w.codes.size();
+    std::vector<uint8_t> head = slot_head(fp, all, static_cast<uint32_t>(T), static_cast<uint32_t>(w.n_comp));
+    memcpy(head.data() + sizeof(SlotHead::Header), &tg, sizeof tg);
+    CUDA_TRY(cudaMemcpyAsync(my_slot, head.data(), head.size(), cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
+    if (T) CUDA_TRY(cudaMemcpyAsync(my_slot + ts.off_codes, w.codes.data(), T * 8, cudaMemcpyHostToDevice, s));
+    return 0;
+}
+
+// the root's staging for the read-backs of its unions: the control words and the union values, or the control words, each tag's
+// union values and the union tuple codes
+static size_t union_pinned_bytes(const bydb_group_key *, uint32_t cap) { return 32 + static_cast<size_t>(cap) * (kMaxLit + 4); }
+static size_t union_pinned_bytes(const bydb_group_keys *keys, uint32_t cap) {
+    return 64 + keys->n_keys * static_cast<size_t>(cap) * (kMaxLit + 4) + static_cast<size_t>(cap) * 8;
+}
+
+// The root of the wide collective: what its unions read, where they count, and what the ranks' slot heads say
+struct WideRoot {
+    const bydb_query *q;
+    size_t F;
+    uint32_t cap, R;
+    const uint8_t *slots0;
+    size_t slot;
+    ExecSlot &es;
+    bydb_stats &stats;
+    std::vector<uint32_t> v_off = {}, row_off = {};  // exclusive scans of the ranks' V_r (a tuple key: T_r) and C_r
+    std::vector<TupleSlot::Tags> tags = {};         // a tuple key: each rank's V_t
+};
+
+// the R slot heads (read_slot_heads), counted; a tuple key's carry each rank's Tags too
+static int read_wide_heads(const bydb_group_key *, WideRoot &wr, uint64_t fp) {
+    const int rc = read_slot_heads(wr.slots0, wr.slot, wr.R, fp, wr.cap, "wide keyed collective", ", or called the per-value keyed collective", wr.v_off,
+                                   wr.row_off);
+    if (!rc) wr.stats.d2h_bytes += sizeof(SlotHead::Header) * wr.R;
+    return rc;
+}
+static int read_wide_heads(const bydb_group_keys *, WideRoot &wr, uint64_t fp) {
+    const int rc = read_slot_heads(wr.slots0, wr.slot, wr.R, fp, wr.cap, "tuple collective", ", or called the one-key wide collective", wr.v_off,
+                                   wr.row_off, &wr.tags);
+    if (!rc) wr.stats.d2h_bytes += (sizeof(SlotHead::Header) + sizeof(TupleSlot::Tags)) * wr.R;
+    return rc;
+}
+
+// the first n bytes of the root's control words, synchronised and counted
+static int read_union_ctl(WideRoot &wr, const uint32_t *d_ctl, size_t n, uint32_t *ctl) {
+    cudaStream_t s = wr.es.stream;
+    CUDA_TRY(cudaMemcpyAsync(wr.es.pinned, d_ctl, n, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaGetLastError());
+    wr.stats.d2h_bytes += n;
+    memcpy(ctl, wr.es.pinned, n);
+    return 0;
+}
+
+// the span check's verdict (ctl[2], ctl[3]): a series that lives on several ranks over time spans that intersect is refused by name
+static int rank_overlap(const char *form, const bydb_query *q, const uint32_t *ctl) {
+    if (ctl[2] != kErrRankOverlap) return 0;
+    const uint32_t i = ctl[3];
+    return fail(BYDB_ENOTSUP, std::string(form) + ": series #" + std::to_string(i) + " (id " + std::to_string(i < q->n_series ? q->series_ids[i] : 0) +
+                                  ") lives on several ranks over time spans that intersect");
+}
+
+// The root's scratch, behind the regions a key union has carved: the control words (ctl_bytes, preset 0 but ctl[3] = ~0), the
+// offsets (the ranks' V_r or T_r, C_r, then tag_off) uploaded, the union table over the V_r (T_r) entries preset empty, the heads
+// of the exclusive scans (n_head entries, the longest) and their tile sums, and the regions of the composite union and the order,
+// preset.  Fills in every WideUnionParams field but the union values (vals / lens).
+static int wide_union_scratch(WideRoot &wr, Carve &carve, size_t ctl_bytes, const std::vector<uint32_t> &tag_off, size_t n_head, Scratch &us,
+                              WideUnionParams &up) {
+    cudaStream_t s = wr.es.stream;
+    const uint32_t R = wr.R, n_vals = wr.v_off[R], n_rows = wr.row_off[R];
+    std::vector<uint32_t> offs(wr.v_off);
+    offs.insert(offs.end(), wr.row_off.begin(), wr.row_off.end());
+    offs.insert(offs.end(), tag_off.begin(), tag_off.end());
+    const size_t nh = align_up(n_head, 1024), nr = align_up(std::max<uint32_t>(n_rows, 1), 1024);
+    const size_t VS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_vals), 1024)), CS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_rows), 1024));
+    const size_t N = pow2_at_least(std::max<size_t>(n_rows, 2048));
+    const size_t u_ctl = carve(ctl_bytes), u_off = carve(4 * offs.size()), u_vslot = carve(VS * 8), u_vid = carve(n_vals * 4), u_vhead = carve(nh * 4),
+                 u_tiles = carve(std::max(nh, nr) / 1024 * 4), u_comp = carve(CS * 8), u_cranks = carve(CS * 8), u_cfirst = carve(CS * 8),
+                 u_cidx = carve(CS * 4), u_rslot = carve(n_rows * 4), u_rkey = carve(n_rows * 8), u_keys = carve(N * 8), u_seg = carve(nr * 4),
+                 u_order = carve(n_rows * 4);
+    CUDA_TRY(us.alloc(carve.o, s));
+    CUDA_TRY(cudaMemsetAsync(us.base + u_ctl, 0, ctl_bytes, s));
+    CUDA_TRY(cudaMemsetAsync(us.base + u_ctl + 12, 0xff, 4, s));
+    CUDA_TRY(cudaMemsetAsync(us.base + u_vslot, 0, VS * 8, s));
+    CUDA_TRY(cudaMemsetAsync(us.base + u_comp, 0, CS * 16, s));  // comp, cranks
+    CUDA_TRY(cudaMemsetAsync(us.base + u_cfirst, 0xff, u_rslot - u_cfirst, s));  // cfirst, cidx
+    CUDA_TRY(cudaMemsetAsync(us.base + u_seg, 0, nr * 4, s));
+    CUDA_TRY(cudaMemsetAsync(us.base + u_order, 0xff, n_rows * 4, s));
+    CUDA_TRY(cudaMemcpyAsync(us.base + u_off, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
+    wr.stats.h2d_bytes += offs.size() * 4;
+    up.slots = wr.slots0;
+    up.slot_stride = wr.slot;
+    up.F = static_cast<uint32_t>(wr.F);
+    up.NS = static_cast<uint32_t>(wr.q->n_series);
+    up.cap = wr.cap;
+    up.n_ranks = R;
+    up.tmin = wr.q->tmin;
+    up.tmax = wr.q->tmax;
+    up.v_off = reinterpret_cast<const uint32_t *>(us.base + u_off);
+    up.row_off = up.v_off + (R + 1);
+    up.n_vals = n_vals;
+    up.n_rows = n_rows;
+    up.vmask = static_cast<uint32_t>(VS - 1);
+    up.cmask = static_cast<uint32_t>(CS - 1);
+    up.vslot = reinterpret_cast<unsigned long long *>(us.base + u_vslot);
+    up.vid = reinterpret_cast<uint32_t *>(us.base + u_vid);
+    up.vhead = reinterpret_cast<uint32_t *>(us.base + u_vhead);
+    up.tiles = reinterpret_cast<uint32_t *>(us.base + u_tiles);
+    up.comp = reinterpret_cast<unsigned long long *>(us.base + u_comp);
+    up.cranks = reinterpret_cast<unsigned long long *>(us.base + u_cranks);
+    up.cfirst = reinterpret_cast<unsigned long long *>(us.base + u_cfirst);
+    up.cidx = reinterpret_cast<uint32_t *>(us.base + u_cidx);
+    up.row_slot = reinterpret_cast<uint32_t *>(us.base + u_rslot);
+    up.row_key = reinterpret_cast<unsigned long long *>(us.base + u_rkey);
+    up.n_sort = static_cast<uint32_t>(N);
+    up.keys = reinterpret_cast<unsigned long long *>(us.base + u_keys);
+    up.seg = reinterpret_cast<uint32_t *>(us.base + u_seg);
+    up.order = reinterpret_cast<uint32_t *>(us.base + u_order);
+    up.ctl = reinterpret_cast<uint32_t *>(us.base + u_ctl);
+    return 0;
+}
+
+// The root's key union, the span check and the union composites (ctl[1] = C_u), whose ids the merge reads.  One key: the union of
+// the ranks' values (launch_wide_union, ctl[0] = V_u).  A tuple key: each tag's value union (launch_tuple_tag_union, ctl[8 + t] =
+// V_u,t), then -- every tag's union within the cap, so that a union tag id fits its 16 bits -- the tuple union (launch_tuple_union,
+// ctl[0] = T_u).
+static int wide_key_union(const bydb_group_key *, WideRoot &wr, Scratch &us, WideUnionParams &up, uint32_t *ctl) {
+    Carve carve;
+    const size_t u_vals = carve(static_cast<size_t>(wr.cap) * kMaxLit), u_lens = carve(static_cast<size_t>(wr.cap) * 4);
+    int rc = wide_union_scratch(wr, carve, 32, {}, wr.v_off[wr.R], us, up);
+    if (rc) return rc;
+    up.vals = us.base + u_vals;
+    up.lens = reinterpret_cast<uint32_t *>(us.base + u_lens);
+    wr.stats.kernel_launches += launch_wide_union(up, wr.es.stream);
+    rc = read_union_ctl(wr, up.ctl, 16, ctl);
+    if (rc) return rc;
+    if (ctl[0] > wr.cap)
+        return fail(BYDB_ENOMEM, "wide keyed collective: more distinct key values over all ranks than bydb_group_key.max_values (" + std::to_string(wr.cap) + ")");
+    return rank_overlap("wide keyed collective", wr.q, ctl);
+}
+static int wide_key_union(const bydb_group_keys *keys, WideRoot &wr, Scratch &us, TupleUnionParams &up, uint32_t *ctl) {
+    cudaStream_t s = wr.es.stream;
+    const uint32_t K = keys->n_keys, R = wr.R, cap = wr.cap;
+    // per tag: the exclusive scan of the ranks' V_t (each at most the cap)
+    std::vector<uint32_t> tag_off;
+    uint32_t tv[kMaxKeyTags] = {}, tv_max = 0;
+    for (uint32_t t = 0; t < K; ++t) {
+        tag_off.push_back(0);
+        for (uint32_t r = 0; r < R; ++r) tag_off.push_back(tag_off.back() + std::min(wr.tags[r].V[t], cap));
+        tv[t] = tag_off.back();
+        tv_max = std::max(tv_max, tv[t]);
+    }
+    Carve carve;
+    size_t VS[kMaxKeyTags] = {}, u_vslot[kMaxKeyTags] = {}, u_vid[kMaxKeyTags] = {}, u_vals[kMaxKeyTags] = {}, u_lens[kMaxKeyTags] = {};
+    for (uint32_t t = 0; t < K; ++t) {
+        VS[t] = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(tv[t]), 1024));
+        u_vslot[t] = carve(VS[t] * 8);
+        u_vid[t] = carve(tv[t] * 4);
+        u_vals[t] = carve(static_cast<size_t>(cap) * kMaxLit);
+        u_lens[t] = carve(static_cast<size_t>(cap) * 4);
+    }
+    const size_t u_codes = carve(static_cast<size_t>(cap) * 8);
+    int rc = wide_union_scratch(wr, carve, 64, tag_off, std::max(tv_max, wr.v_off[R]), us, up);
+    if (rc) return rc;
+    up.n_tags = K;
+    up.tag_ctl = up.ctl + 8;
+    up.codes = reinterpret_cast<unsigned long long *>(us.base + u_codes);
+    for (uint32_t t = 0; t < K; ++t) {
+        TupleTagUnion &tg = up.tags[t];
+        CUDA_TRY(cudaMemsetAsync(us.base + u_vslot[t], 0, VS[t] * 8, s));
+        tg.v_off = up.v_off + (2 + t) * (R + 1);
+        tg.n_vals = tv[t];
+        tg.vmask = static_cast<uint32_t>(VS[t] - 1);
+        tg.vslot = reinterpret_cast<unsigned long long *>(us.base + u_vslot[t]);
+        tg.vid = reinterpret_cast<uint32_t *>(us.base + u_vid[t]);
+        tg.vals = us.base + u_vals[t];
+        tg.lens = reinterpret_cast<uint32_t *>(us.base + u_lens[t]);
+    }
+    wr.stats.kernel_launches += launch_tuple_tag_union(up, s);
+    rc = read_union_ctl(wr, up.ctl, 48, ctl);
+    if (rc) return rc;
+    for (uint32_t t = 0; t < K; ++t)
+        if (ctl[8 + t] > cap)
+            return fail(BYDB_ENOMEM, std::string("tuple collective: more distinct values of the tag ") + keys->keys[t].family + "/" + keys->keys[t].tag +
+                                         " over all ranks than bydb_group_keys.max_values (" + std::to_string(cap) + ")");
+    rc = rank_overlap("tuple collective", wr.q, ctl);
+    if (rc) return rc;
+    wr.stats.kernel_launches += launch_tuple_union(up, s);
+    rc = read_union_ctl(wr, up.ctl, 48, ctl);
+    if (rc) return rc;
+    if (ctl[0] > cap)
+        return fail(BYDB_ENOMEM, "tuple collective: more distinct key tuples over all ranks than bydb_group_keys.max_values (" + std::to_string(cap) + ")");
+    return 0;
+}
+
+// The union's key tables after the merge, in one synchronised read-back: the union values into u.values, or each tag's union
+// values into u.tag_values and the union codes into u.codes
+static int read_union_keys(const bydb_group_key *, WideRoot &wr, const WideUnionParams &up, const uint32_t *ctl, WidePass &u) {
+    cudaStream_t s = wr.es.stream;
+    uint8_t *pinned = wr.es.pinned;
+    const size_t V = ctl[0];
+    CUDA_TRY(cudaMemcpyAsync(pinned, up.vals, V * kMaxLit, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(pinned + V * kMaxLit, up.lens, V * 4, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaGetLastError());
+    wr.stats.d2h_bytes += V * (kMaxLit + 4);
+    u.values = unpack_values(V, false, pinned, reinterpret_cast<const uint32_t *>(pinned + V * kMaxLit));
+    return 0;
+}
+static int read_union_keys(const bydb_group_keys *keys, WideRoot &wr, const TupleUnionParams &up, const uint32_t *ctl, WidePass &u) {
+    cudaStream_t s = wr.es.stream;
+    uint8_t *pinned = wr.es.pinned;
+    const uint32_t K = keys->n_keys;
+    const size_t T = ctl[0];
+    size_t at[kMaxKeyTags] = {}, back = 0;
+    for (uint32_t t = 0; t < K; ++t) {
+        const size_t V = ctl[8 + t];
+        at[t] = back;
+        CUDA_TRY(cudaMemcpyAsync(pinned + back, up.tags[t].vals, V * kMaxLit, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(pinned + back + V * kMaxLit, up.tags[t].lens, V * 4, cudaMemcpyDeviceToHost, s));
+        back += V * (kMaxLit + 4);
+    }
+    CUDA_TRY(cudaMemcpyAsync(pinned + back, up.codes, T * 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaGetLastError());
+    wr.stats.d2h_bytes += back + T * 8;
+    for (uint32_t t = 0; t < K; ++t) {
+        const size_t V = ctl[8 + t];
+        u.tag_values[t] = unpack_values(V, false, pinned + at[t], reinterpret_cast<const uint32_t *>(pinned + at[t] + V * kMaxLit));
+    }
+    u.codes.resize(T);
+    if (T) memcpy(u.codes.data(), pinned + back, T * 8);
+    return 0;
 }
 
 // A rank's present composite groups after its wide pass, into the WideSlot regions of its slot in the root's mailbox (a TupleSlot's
@@ -4727,455 +5045,83 @@ static int put_wide_rank(const Plan &plan, WidePass &w, uint8_t *my_slot, const 
     return 0;
 }
 
-// The wide keyed collective: on every rank the wide path's discovery, scan and order (wide_pass), then wide_fold_kernel writes the
-// rank's present composite groups straight into its slot of the root's mailbox (layout WideSlot), wide_series_kernel the series'
-// spans and wide_first_kernel each composite's first series; on the root the union of the values, the span check, the union
-// composites in insertion order and their fold in rank order (launch_wide_union / launch_wide_merge), then wide_emit as in
-// bydb_scan_agg_keyed_wide.  The root's call decides the answer's form; ranks may mix the two calls in one collective.
-template <class Out>
-static int scan_reduce_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, Out *out) {
-    if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
-    memset(out, 0, sizeof *out);
-    g_last_dev_err = 0;
-    KeyedAnswer<Out> answer(ctx, out, {});
-    bydb_stats &stats = keyed_stats(out);
-    Plan plan;
-    uint32_t cap = 0;
-    uint64_t fp = 0;
-    size_t slot_bytes = 0;
-    WidePass w;
-    CollectiveHooks h;
-    h.prepare = [&](ExecSlot &es, size_t slot) -> int {
-        slot_bytes = slot;
-        int rc = validate_query(q, true);
-        if (!rc) rc = check_group_key(q, key, kMaxWideKeyValues, false, cap);
-        if (!rc) rc = make_plan(ctx, q, nullptr, plan);
-        if (rc) return rc;
-        if (parts_overlap(plan.parts, q->tmin, q->tmax))
-            return fail(BYDB_ENOTSUP, "group-key query over parts of one rank that overlap in time (version dedup) is not supported on the device path");
-        fp = keyed_wide_fingerprint(q, key, cap);
-        const size_t F = plan.fcols.size(), NS = q->n_series;
-        // the staging of this rank's pass; on the root also the union's read-back and the answer over the most composite groups the
-        // slots can carry (no page-locked allocation may follow inside the collective)
-        size_t pinned = wide_discover_pinned(NS, 1, cap);
-        if (ctx->comm.rank == root) {
-            const size_t fixed = WideSlot(F, NS, 0, 0).total;
-            const size_t fit = slot > fixed ? (slot - fixed) / WideSlot::comp_bytes(F) : 0;
-            const size_t most = std::min<size_t>(static_cast<size_t>(ctx->comm.nranks) * fit, static_cast<size_t>(plan.n_groups) * cap);
-            pinned = std::max({pinned, 32 + static_cast<size_t>(cap) * (kMaxLit + 4), keyed_pinned_bytes(q, plan, std::max<size_t>(most, 1), out)});
-        }
-        if (es.ensure_pinned(pinned)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-        return 0;
-    };
-    h.contribute = [&](ExecSlot &es, uint8_t *my_slot) -> int {
-        cudaStream_t s = es.stream;
-        const size_t F = plan.fcols.size(), NS = q->n_series;
-        int rc = wide_pass(ctx, q, key, 1, cap, plan, es, stats, w);
-        if (rc) return rc;
-        const size_t V = w.values.size(), C = w.n_comp;
-        const WideSlot ws(F, NS, V, C);
-        if (ws.total > slot_bytes || C >= kWideMaxRankComposites)
-            return fail(BYDB_EINVAL, "wide keyed collective: this rank's " + std::to_string(V) + " key values and " + std::to_string(C) +
-                                         " composite groups need " + std::to_string(ws.total) +
-                                         " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keyed_wide_reduce_slot_bytes)");
-        rc = put_wide_rank(plan, w, my_slot, ws, stats, s);
-        if (rc) return rc;
-        return put_slot_head(my_slot, fp, w.values, static_cast<uint32_t>(C), s);
-    };
-    h.collect = [&](ExecSlot &) { return 0; };  // the pass was collected as it ran
-    h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &settle, bool &) -> int {
-        int rc = settle();  // a failed rank's slot holds nothing to read
-        if (rc) return rc;
-        cudaStream_t s = es.stream;
-        const uint32_t R = static_cast<uint32_t>(ctx->comm.nranks);
-        const size_t F = plan.fcols.size(), NS = q->n_series;
-        std::vector<uint32_t> v_off, row_off;
-        rc = read_slot_heads(slots0, slot, R, fp, cap, "wide keyed collective", ", or called the per-value keyed collective", v_off, row_off);
-        if (rc) return rc;
-        stats.d2h_bytes += 16ull * R;
-        const uint32_t n_vals = v_off[R], n_rows = row_off[R];
-        if (n_vals == 0) return 0;  // no rank selected a block: no rows, no keys
-        // ---- the union of the values, the span check, the union composites
-        const size_t nv = align_up(n_vals, 1024), nr = align_up(std::max<uint32_t>(n_rows, 1), 1024);
-        const size_t VS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_vals), 1024)), CS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_rows), 1024));
-        const size_t N = pow2_at_least(std::max<size_t>(n_rows, 2048));
-        Carve carve;
-        const size_t u_ctl = carve(32), u_off = carve(8 * (R + 1)), u_vslot = carve(VS * 8), u_vid = carve(n_vals * 4), u_vhead = carve(nv * 4),
-                     u_tiles = carve(std::max(nv, nr) / 1024 * 4), u_vals = carve(static_cast<size_t>(cap) * kMaxLit), u_lens = carve(static_cast<size_t>(cap) * 4),
-                     u_comp = carve(CS * 8), u_cranks = carve(CS * 8), u_cfirst = carve(CS * 8), u_cidx = carve(CS * 4), u_rslot = carve(n_rows * 4),
-                     u_rkey = carve(n_rows * 8), u_keys = carve(N * 8), u_seg = carve(nr * 4), u_order = carve(n_rows * 4);
-        Scratch us;
-        CUDA_TRY(us.alloc(carve.o, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl, 0, 32, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl + 12, 0xff, 4, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_vslot, 0, VS * 8, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_comp, 0, CS * 16, s));  // comp, cranks
-        CUDA_TRY(cudaMemsetAsync(us.base + u_cfirst, 0xff, u_rslot - u_cfirst, s));  // cfirst, cidx
-        CUDA_TRY(cudaMemsetAsync(us.base + u_seg, 0, nr * 4, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_order, 0xff, n_rows * 4, s));
-        std::vector<uint32_t> offs(v_off);
-        offs.insert(offs.end(), row_off.begin(), row_off.end());
-        CUDA_TRY(cudaMemcpyAsync(us.base + u_off, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
-        stats.h2d_bytes += offs.size() * 4;
-        WideUnionParams up;
-        memset(&up, 0, sizeof up);
-        up.slots = slots0;
-        up.slot_stride = slot;
-        up.F = static_cast<uint32_t>(F);
-        up.NS = static_cast<uint32_t>(NS);
-        up.cap = cap;
-        up.n_ranks = R;
-        up.tmin = q->tmin;
-        up.tmax = q->tmax;
-        up.v_off = reinterpret_cast<const uint32_t *>(us.base + u_off);
-        up.row_off = up.v_off + (R + 1);
-        up.n_vals = n_vals;
-        up.n_rows = n_rows;
-        up.vmask = static_cast<uint32_t>(VS - 1);
-        up.cmask = static_cast<uint32_t>(CS - 1);
-        up.vslot = reinterpret_cast<unsigned long long *>(us.base + u_vslot);
-        up.vid = reinterpret_cast<uint32_t *>(us.base + u_vid);
-        up.vhead = reinterpret_cast<uint32_t *>(us.base + u_vhead);
-        up.tiles = reinterpret_cast<uint32_t *>(us.base + u_tiles);
-        up.vals = us.base + u_vals;
-        up.lens = reinterpret_cast<uint32_t *>(us.base + u_lens);
-        up.comp = reinterpret_cast<unsigned long long *>(us.base + u_comp);
-        up.cranks = reinterpret_cast<unsigned long long *>(us.base + u_cranks);
-        up.cfirst = reinterpret_cast<unsigned long long *>(us.base + u_cfirst);
-        up.cidx = reinterpret_cast<uint32_t *>(us.base + u_cidx);
-        up.row_slot = reinterpret_cast<uint32_t *>(us.base + u_rslot);
-        up.row_key = reinterpret_cast<unsigned long long *>(us.base + u_rkey);
-        up.n_sort = static_cast<uint32_t>(N);
-        up.keys = reinterpret_cast<unsigned long long *>(us.base + u_keys);
-        up.seg = reinterpret_cast<uint32_t *>(us.base + u_seg);
-        up.order = reinterpret_cast<uint32_t *>(us.base + u_order);
-        up.ctl = reinterpret_cast<uint32_t *>(us.base + u_ctl);
-        stats.kernel_launches += launch_wide_union(up, s);
-        CUDA_TRY(cudaMemcpyAsync(es.pinned, up.ctl, 16, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaStreamSynchronize(s));
-        CUDA_TRY(cudaGetLastError());
-        stats.d2h_bytes += 16;
-        uint32_t ctl[4];
-        memcpy(ctl, es.pinned, 16);
-        if (ctl[0] > cap)
-            return fail(BYDB_ENOMEM, "wide keyed collective: more distinct key values over all ranks than bydb_group_key.max_values (" + std::to_string(cap) + ")");
-        if (ctl[2] == kErrRankOverlap) {
-            const uint32_t i = ctl[3];
-            return fail(BYDB_ENOTSUP, "wide keyed collective: series #" + std::to_string(i) + " (id " + std::to_string(i < NS ? q->series_ids[i] : 0) +
-                                          ") lives on several ranks over time spans that intersect");
-        }
-        const size_t V = ctl[0], C = ctl[1];
-        // ---- the union composites in insertion order, folded over their ranks into a table of C_u groups
-        const TableLayout tl(std::max<size_t>(C, 1), F);
-        Carve cf;
-        const size_t f_table = cf(tl.total), f_pairs = cf(C * 8), f_perm = cf(C * 4);
-        Scratch fb;
-        CUDA_TRY(fb.alloc(cf.o, s));
-        up.table = tl.at(fb.base + f_table);
-        up.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
-        up.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
-        if (C) stats.kernel_launches += launch_wide_merge(up, static_cast<uint32_t>(C), s);
-        CUDA_TRY(cudaMemcpyAsync(es.pinned, up.vals, V * kMaxLit, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaMemcpyAsync(es.pinned + V * kMaxLit, up.lens, V * 4, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaStreamSynchronize(s));
-        CUDA_TRY(cudaGetLastError());
-        stats.d2h_bytes += V * (kMaxLit + 4);
-        set_key_table(out, answer.owner, unpack_values(V, false, es.pinned, reinterpret_cast<const uint32_t *>(es.pinned + V * kMaxLit)));
-        if (C == 0) return 0;
-        WideReduceParams rp;
-        memset(&rp, 0, sizeof rp);
-        rp.pairs = up.pairs;
-        rp.perm = up.perm;
-        rp.ctl = up.ctl;  // ctl[1] = C_u, the present rows keyed_partial_rows_kernel reads
-        return wide_emit(q, plan, es, fb.base + f_table, tl, C, rp, out, answer.owner);
-    };
-    h.discard = [] {};  // the result of a failed call is freed by `answer`
-    const int rc = run_collective(ctx, root, 0, h);
-    if (rc) return rc;
-    answer.done = true;
-    return 0;
-}
-
-extern "C" {
-
-int bydb_scan_reduce_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out) {
-    return guarded([&]() -> int { return scan_reduce_keyed_wide_impl(ctx, q, key, root, out); });
-}
-
-int bydb_scan_reduce_keyed_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root,
-                                         bydb_keyed_partial_rows *out) {
-    return guarded([&]() -> int { return scan_reduce_keyed_wide_impl(ctx, q, key, root, out); });
-}
-
-int bydb_keys_wide_reduce_slot_bytes(const bydb_query *q, const bydb_group_keys *keys, uint64_t max_present, uint64_t *out) {
-    return guarded([&]() -> int {
-    if (!q || !out) return fail(BYDB_EINVAL, "NULL argument");
-    int rc = validate_query(q, false);
-    uint32_t cap = 0;
-    if (!rc) rc = check_group_key(q, keys, kMaxWideKeyValues, false, cap);
-    if (rc) return rc;
-    Plan plan;
-    rc = query_shape(q, plan);
-    if (rc) return rc;
-    *out = TupleSlot(plan.fcols.size(), q->n_series, static_cast<size_t>(keys->n_keys) * cap, cap, max_present).total;
-    return 0;
-    });
-}
-}  // extern "C"
-
-// the fingerprint of the tuple collective: the query, every key (family, tag, value type) in GroupBy order, the cap and the form
-static uint64_t keys_wide_fingerprint(const bydb_query *q, const bydb_group_keys *keys, uint32_t cap) {
-    uint64_t h = keyed_fingerprint(q, &keys->keys[0], cap);
-    auto mix = [&](const void *p, size_t n) {
-        const uint8_t *b = static_cast<const uint8_t *>(p);
-        for (size_t i = 0; i < n; ++i) h = (h ^ b[i]) * 0x100000001b3ull;
-    };
-    const uint64_t K = keys->n_keys;
-    mix(&K, sizeof K);
-    for (uint32_t t = 1; t < keys->n_keys; ++t) {
-        const bydb_group_key &k = keys->keys[t];
-        const uint64_t nf = strlen(k.family), nt = strlen(k.tag), vt = k.value_type;
-        mix(&nf, 8);
-        mix(k.family, nf);
-        mix(&nt, 8);
-        mix(k.tag, nt);
-        mix(&vt, 8);
-    }
-    mix("tuple", 5);
-    return h;
-}
-
-// The tuple collective: on every rank bydb_scan_agg_keys_wide's discovery, scan and order (wide_pass with the key list), its present
-// composite groups into its slot as the wide keyed collective writes them (put_wide_rank), and a head with its tags' values and its
-// tuple codes (layout TupleSlot).  On the root: each tag's value union and the span check (launch_tuple_tag_union), then -- every
-// tag's union within the cap, so that a union id fits 16 bits -- the tuple union and the composite union (launch_tuple_union), the
-// wide collective's merge over the union tuple ids, and wide_emit with the union tag tables and codes.  The root's call decides the
-// answer's form; ranks may mix the two calls in one collective.
-template <class Out>
-static int scan_reduce_keys_wide_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root, Out *out) {
+// The wide collective, with one key (bydb_scan_reduce_keyed_wide) or a tuple key (bydb_scan_reduce_keys_wide), and the partial form
+// of each.  On every rank the wide path's discovery, scan and order (wide_pass, as bydb_scan_agg_keyed_wide / bydb_scan_agg_keys_wide
+// run them), then its present composite groups into its slot of the root's mailbox (put_wide_rank) and its head: its values, or its
+// tags' values and its tuple codes (layout WideSlot / TupleSlot).  On the root the key union, the span check and the union
+// composites (wide_key_union), their fold in rank order in the insertion order of the whole scan (launch_wide_merge), and the answer
+// as on one context (wide_emit).  The root's call decides the answer's form; ranks may mix the two calls of a key form in one
+// collective.
+template <class Out, class Key>
+static int scan_reduce_wide_impl(bydb_ctx *ctx, const bydb_query *q, const Key *key, int32_t root, Out *out) {
+    using UnionParams = std::conditional_t<std::is_same<Key, bydb_group_keys>::value, TupleUnionParams, WideUnionParams>;
     if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
     memset(out, 0, sizeof *out);
     g_last_dev_err = 0;
     KeyedAnswer<Out> answer(ctx, out);
+    wide_key_tables(out, answer.owner, WidePass());  // empty on every rank until the root's union fills them
     bydb_stats &stats = keyed_stats(out);
     Plan plan;
-    uint32_t cap = 0, K = 0;
+    uint32_t cap = 0;
     uint64_t fp = 0;
     size_t slot_bytes = 0;
     WidePass w;
     CollectiveHooks h;
     h.prepare = [&](ExecSlot &es, size_t slot) -> int {
         slot_bytes = slot;
-        int rc = validate_query(q, true);
-        if (!rc) rc = check_group_key(q, keys, kMaxWideKeyValues, false, cap);
-        if (!rc) rc = make_plan(ctx, q, nullptr, plan);
+        int rc = keyed_collective_call(ctx, q, key, kMaxWideKeyValues, false, cap, plan);
         if (rc) return rc;
-        if (parts_overlap(plan.parts, q->tmin, q->tmax))
-            return fail(BYDB_ENOTSUP, "group-key query over parts of one rank that overlap in time (version dedup) is not supported on the device path");
-        K = keys->n_keys;
-        fp = keys_wide_fingerprint(q, keys, cap);
-        const size_t F = plan.fcols.size(), NS = q->n_series;
-        // the staging of this rank's pass; on the root also the unions' read-back (control words, K tag tables, the tuple codes)
-        // and the answer over the most composite groups the slots can carry (no page-locked allocation may follow inside the
-        // collective)
-        size_t pinned = wide_discover_pinned(NS, K, cap);
+        fp = wide_fingerprint(q, key, cap);
+        // the staging of this rank's pass; on the root also the unions' read-back and the answer over the most composite groups the
+        // slots can carry (no page-locked allocation may follow inside the collective)
+        size_t pinned = wide_discover_pinned(q->n_series, key_count(key), cap);
         if (ctx->comm.rank == root) {
-            const size_t fixed = TupleSlot(F, NS, 0, 0, 0).total;
-            const size_t fit = slot > fixed ? (slot - fixed) / WideSlot::comp_bytes(F) : 0;
+            const size_t fixed = rank_slot(key, plan, WidePass()).total;
+            const size_t fit = slot > fixed ? (slot - fixed) / WideSlot::comp_bytes(plan.fcols.size()) : 0;
             const size_t most = std::min<size_t>(static_cast<size_t>(ctx->comm.nranks) * fit, static_cast<size_t>(plan.n_groups) * cap);
-            pinned = std::max({pinned, 64 + K * static_cast<size_t>(cap) * (kMaxLit + 4) + static_cast<size_t>(cap) * 8,
-                               keyed_pinned_bytes(q, plan, std::max<size_t>(most, 1), out)});
+            pinned = std::max({pinned, union_pinned_bytes(key, cap), keyed_pinned_bytes(q, plan, std::max<size_t>(most, 1), out)});
         }
         if (es.ensure_pinned(pinned)) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
         return 0;
     };
     h.contribute = [&](ExecSlot &es, uint8_t *my_slot) -> int {
-        cudaStream_t s = es.stream;
-        const size_t F = plan.fcols.size(), NS = q->n_series;
-        int rc = wide_pass(ctx, q, keys->keys, K, cap, plan, es, stats, w);
+        int rc = wide_pass(ctx, q, key_list(key), key_count(key), cap, plan, es, stats, w);
         if (rc) return rc;
-        KeyValues all;  // the tags' values back to back
-        TupleSlot::Tags tg{};
-        tg.K = K;
-        for (uint32_t t = 0; t < K && t < w.tag_values.size(); ++t) {
-            tg.V[t] = static_cast<uint32_t>(w.tag_values[t].size());
-            all.insert(all.end(), w.tag_values[t].begin(), w.tag_values[t].end());
-        }
-        const size_t T = w.codes.size(), C = w.n_comp;
-        const TupleSlot ts(F, NS, all.size(), T, C);
-        if (ts.total > slot_bytes || C >= kWideMaxRankComposites)
-            return fail(BYDB_EINVAL, "tuple collective: this rank's " + std::to_string(all.size()) + " tag values, " + std::to_string(T) + " tuples and " +
-                                         std::to_string(C) + " composite groups need " + std::to_string(ts.total) +
-                                         " bytes, more than the mailbox slots (bydb_comm_export max_table_bytes, see bydb_keys_wide_reduce_slot_bytes)");
-        rc = put_wide_rank(plan, w, my_slot, ts, stats, s);
+        const auto rs = rank_slot(key, plan, w);
+        if (rs.total > slot_bytes || w.n_comp >= kWideMaxRankComposites) return fail(BYDB_EINVAL, slot_refusal(key, w, rs.total));
+        rc = put_wide_rank(plan, w, my_slot, rs, stats, es.stream);
         if (rc) return rc;
-        std::vector<uint8_t> head = slot_head(fp, all, static_cast<uint32_t>(T), static_cast<uint32_t>(C));
-        memcpy(head.data() + sizeof(SlotHead::Header), &tg, sizeof tg);
-        CUDA_TRY(cudaMemcpyAsync(my_slot, head.data(), head.size(), cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
-        if (T) CUDA_TRY(cudaMemcpyAsync(my_slot + ts.off_codes, w.codes.data(), T * 8, cudaMemcpyHostToDevice, s));
-        return 0;
+        return put_wide_head(key, my_slot, rs, fp, w, es.stream);
     };
     h.collect = [&](ExecSlot &) { return 0; };  // the pass was collected as it ran
     h.reduce = [&](ExecSlot &es, uint8_t *slots0, size_t slot, const std::function<int()> &settle, bool &) -> int {
         int rc = settle();  // a failed rank's slot holds nothing to read
         if (rc) return rc;
         cudaStream_t s = es.stream;
-        const uint32_t R = static_cast<uint32_t>(ctx->comm.nranks);
-        const size_t F = plan.fcols.size(), NS = q->n_series;
-        std::vector<uint32_t> t_off, row_off;
-        std::vector<TupleSlot::Tags> tags;
-        rc = read_slot_heads(slots0, slot, R, fp, cap, "tuple collective", ", or called the one-key wide collective", t_off, row_off, &tags);
+        WideRoot wr{q, plan.fcols.size(), cap, static_cast<uint32_t>(ctx->comm.nranks), slots0, slot, es, stats};
+        rc = read_wide_heads(key, wr, fp);
         if (rc) return rc;
-        stats.d2h_bytes += (sizeof(SlotHead::Header) + sizeof(TupleSlot::Tags)) * R;
-        WidePass u;  // the union's tag tables and tuple codes, in the shape tuple_key_tables / tuple_row_entries read
-        u.tag_values.assign(K, KeyValues());
-        const uint32_t n_tup = t_off[R], n_rows = row_off[R];
-        if (n_tup == 0) {  // no rank selected a block: no rows, K empty tag tables
+        WidePass u;  // the union's key tables, in the shape wide_key_tables / wide_row_tuples read (a tuple key: K tag tables)
+        u.tag_values.assign(key_count(key), KeyValues());
+        if (wr.v_off[wr.R] == 0) {  // no rank selected a block: no rows, empty key tables
             wide_key_tables(out, answer.owner, u);
             return 0;
         }
-        // per tag: the exclusive scan of the ranks' V_t (each at most the cap)
-        std::vector<uint32_t> offs(t_off);
-        offs.insert(offs.end(), row_off.begin(), row_off.end());
-        uint32_t tv[kMaxKeyTags] = {}, tv_max = 0;
-        for (uint32_t t = 0; t < K; ++t) {
-            offs.push_back(0);
-            for (uint32_t r = 0; r < R; ++r) offs.push_back(offs.back() + std::min(tags[r].V[t], cap));
-            tv[t] = offs.back();
-            tv_max = std::max(tv_max, tv[t]);
-        }
-        const size_t nh = align_up(std::max(tv_max, n_tup), 1024), nr = align_up(std::max<uint32_t>(n_rows, 1), 1024);
-        size_t VS[kMaxKeyTags] = {};
-        for (uint32_t t = 0; t < K; ++t) VS[t] = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(tv[t]), 1024));
-        const size_t TS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_tup), 1024));
-        const size_t CS = pow2_at_least(std::max<size_t>(2 * static_cast<size_t>(n_rows), 1024)), N = pow2_at_least(std::max<size_t>(n_rows, 2048));
-        Carve carve;
-        const size_t u_ctl = carve(64), u_off = carve(4 * offs.size());
-        size_t u_vslot[kMaxKeyTags] = {}, u_vid[kMaxKeyTags] = {}, u_vals[kMaxKeyTags] = {}, u_lens[kMaxKeyTags] = {};
-        for (uint32_t t = 0; t < K; ++t) u_vslot[t] = carve(VS[t] * 8);
-        const size_t u_tslot = carve(TS * 8);  // every hash table lies in [u_vslot[0], u_tslot + TS * 8): one memset
-        for (uint32_t t = 0; t < K; ++t) {
-            u_vid[t] = carve(tv[t] * 4);
-            u_vals[t] = carve(static_cast<size_t>(cap) * kMaxLit);
-            u_lens[t] = carve(static_cast<size_t>(cap) * 4);
-        }
-        const size_t u_tid = carve(n_tup * 4), u_head = carve(nh * 4), u_tiles = carve(std::max(nh, nr) / 1024 * 4), u_codes = carve(static_cast<size_t>(cap) * 8),
-                     u_comp = carve(CS * 8), u_cranks = carve(CS * 8), u_cfirst = carve(CS * 8), u_cidx = carve(CS * 4), u_rslot = carve(n_rows * 4),
-                     u_rkey = carve(n_rows * 8), u_keys = carve(N * 8), u_seg = carve(nr * 4), u_order = carve(n_rows * 4);
-        Scratch us;
-        CUDA_TRY(us.alloc(carve.o, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl, 0, 64, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_ctl + 12, 0xff, 4, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_vslot[0], 0, u_tslot + TS * 8 - u_vslot[0], s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_comp, 0, CS * 16, s));  // comp, cranks
-        CUDA_TRY(cudaMemsetAsync(us.base + u_cfirst, 0xff, u_rslot - u_cfirst, s));  // cfirst, cidx
-        CUDA_TRY(cudaMemsetAsync(us.base + u_seg, 0, nr * 4, s));
-        CUDA_TRY(cudaMemsetAsync(us.base + u_order, 0xff, n_rows * 4, s));
-        CUDA_TRY(cudaMemcpyAsync(us.base + u_off, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, s));  // pageable: staged before it returns
-        stats.h2d_bytes += offs.size() * 4;
-        const uint32_t *d_off = reinterpret_cast<const uint32_t *>(us.base + u_off);
-        TupleUnionParams up;
+        UnionParams up;
         memset(&up, 0, sizeof up);
-        up.slots = slots0;
-        up.slot_stride = slot;
-        up.F = static_cast<uint32_t>(F);
-        up.NS = static_cast<uint32_t>(NS);
-        up.cap = cap;
-        up.n_ranks = R;
-        up.tmin = q->tmin;
-        up.tmax = q->tmax;
-        up.v_off = d_off;  // the ranks' tuples
-        up.row_off = d_off + (R + 1);
-        up.n_vals = n_tup;
-        up.n_rows = n_rows;
-        up.vmask = static_cast<uint32_t>(TS - 1);
-        up.cmask = static_cast<uint32_t>(CS - 1);
-        up.vslot = reinterpret_cast<unsigned long long *>(us.base + u_tslot);
-        up.vid = reinterpret_cast<uint32_t *>(us.base + u_tid);
-        up.vhead = reinterpret_cast<uint32_t *>(us.base + u_head);
-        up.tiles = reinterpret_cast<uint32_t *>(us.base + u_tiles);
-        up.comp = reinterpret_cast<unsigned long long *>(us.base + u_comp);
-        up.cranks = reinterpret_cast<unsigned long long *>(us.base + u_cranks);
-        up.cfirst = reinterpret_cast<unsigned long long *>(us.base + u_cfirst);
-        up.cidx = reinterpret_cast<uint32_t *>(us.base + u_cidx);
-        up.row_slot = reinterpret_cast<uint32_t *>(us.base + u_rslot);
-        up.row_key = reinterpret_cast<unsigned long long *>(us.base + u_rkey);
-        up.n_sort = static_cast<uint32_t>(N);
-        up.keys = reinterpret_cast<unsigned long long *>(us.base + u_keys);
-        up.seg = reinterpret_cast<uint32_t *>(us.base + u_seg);
-        up.order = reinterpret_cast<uint32_t *>(us.base + u_order);
-        up.ctl = reinterpret_cast<uint32_t *>(us.base + u_ctl);
-        up.n_tags = K;
-        up.tag_ctl = up.ctl + 8;
-        up.codes = reinterpret_cast<unsigned long long *>(us.base + u_codes);
-        for (uint32_t t = 0; t < K; ++t) {
-            TupleTagUnion &tg = up.tags[t];
-            tg.v_off = d_off + 2 * (R + 1) + t * (R + 1);
-            tg.n_vals = tv[t];
-            tg.vmask = static_cast<uint32_t>(VS[t] - 1);
-            tg.vslot = reinterpret_cast<unsigned long long *>(us.base + u_vslot[t]);
-            tg.vid = reinterpret_cast<uint32_t *>(us.base + u_vid[t]);
-            tg.vals = us.base + u_vals[t];
-            tg.lens = reinterpret_cast<uint32_t *>(us.base + u_lens[t]);
-        }
-        // ---- each tag's union and the span check; a tag whose union exceeds the cap stops the call before any code is packed
-        stats.kernel_launches += launch_tuple_tag_union(up, s);
+        Scratch us;
         uint32_t ctl[16];
-        auto read_ctl = [&]() -> int {
-            CUDA_TRY(cudaMemcpyAsync(es.pinned, up.ctl, 48, cudaMemcpyDeviceToHost, s));
-            CUDA_TRY(cudaStreamSynchronize(s));
-            CUDA_TRY(cudaGetLastError());
-            stats.d2h_bytes += 48;
-            memcpy(ctl, es.pinned, 48);
-            return 0;
-        };
-        rc = read_ctl();
+        rc = wide_key_union(key, wr, us, up, ctl);
         if (rc) return rc;
-        for (uint32_t t = 0; t < K; ++t)
-            if (ctl[8 + t] > cap)
-                return fail(BYDB_ENOMEM, std::string("tuple collective: more distinct values of the tag ") + keys->keys[t].family + "/" + keys->keys[t].tag +
-                                             " over all ranks than bydb_group_keys.max_values (" + std::to_string(cap) + ")");
-        if (ctl[2] == kErrRankOverlap) {
-            const uint32_t i = ctl[3];
-            return fail(BYDB_ENOTSUP, "tuple collective: series #" + std::to_string(i) + " (id " + std::to_string(i < NS ? q->series_ids[i] : 0) +
-                                          ") lives on several ranks over time spans that intersect");
-        }
-        // ---- the tuple union and the union composites
-        stats.kernel_launches += launch_tuple_union(up, s);
-        rc = read_ctl();
-        if (rc) return rc;
-        if (ctl[0] > cap)
-            return fail(BYDB_ENOMEM, "tuple collective: more distinct key tuples over all ranks than bydb_group_keys.max_values (" + std::to_string(cap) + ")");
-        const size_t T = ctl[0], C = ctl[1];
         // ---- the union composites in insertion order, folded over their ranks into a table of C_u groups
-        const TableLayout tl(std::max<size_t>(C, 1), F);
-        Carve cf;
-        const size_t f_table = cf(tl.total), f_pairs = cf(C * 8), f_perm = cf(C * 4);
+        const size_t C = ctl[1];
+        const TableLayout tl(std::max<size_t>(C, 1), wr.F);
         Scratch fb;
-        CUDA_TRY(fb.alloc(cf.o, s));
-        up.table = tl.at(fb.base + f_table);
-        up.pairs = reinterpret_cast<int32_t *>(fb.base + f_pairs);
-        up.perm = reinterpret_cast<int32_t *>(fb.base + f_perm);
+        rc = fold_table(tl, C, fb, up, s);
+        if (rc) return rc;
         if (C) stats.kernel_launches += launch_wide_merge(up, static_cast<uint32_t>(C), s);
-        // the K union tag tables and the T_u union codes, back to back in the staging, in one synchronised read-back
-        size_t at[kMaxKeyTags] = {}, back = 0;
-        for (uint32_t t = 0; t < K; ++t) {
-            const size_t V = ctl[8 + t];
-            at[t] = back;
-            CUDA_TRY(cudaMemcpyAsync(es.pinned + back, up.tags[t].vals, V * kMaxLit, cudaMemcpyDeviceToHost, s));
-            CUDA_TRY(cudaMemcpyAsync(es.pinned + back + V * kMaxLit, up.tags[t].lens, V * 4, cudaMemcpyDeviceToHost, s));
-            back += V * (kMaxLit + 4);
-        }
-        CUDA_TRY(cudaMemcpyAsync(es.pinned + back, up.codes, T * 8, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(cudaStreamSynchronize(s));
-        CUDA_TRY(cudaGetLastError());
-        stats.d2h_bytes += back + T * 8;
-        for (uint32_t t = 0; t < K; ++t) {
-            const size_t V = ctl[8 + t];
-            u.tag_values[t] = unpack_values(V, false, es.pinned + at[t], reinterpret_cast<const uint32_t *>(es.pinned + at[t] + V * kMaxLit));
-        }
-        u.codes.resize(T);
-        if (T) memcpy(u.codes.data(), es.pinned + back, T * 8);
+        rc = read_union_keys(key, wr, up, ctl, u);
+        if (rc) return rc;
         wide_key_tables(out, answer.owner, u);
         if (C == 0) return 0;
         WideReduceParams rp;
@@ -5183,7 +5129,7 @@ static int scan_reduce_keys_wide_impl(bydb_ctx *ctx, const bydb_query *q, const 
         rp.pairs = up.pairs;
         rp.perm = up.perm;
         rp.ctl = up.ctl;  // ctl[1] = C_u, the present rows keyed_partial_rows_kernel reads
-        rc = wide_emit(q, plan, es, fb.base + f_table, tl, C, rp, out, answer.owner);
+        rc = wide_emit(q, plan, es, fb.base, tl, C, rp, out, answer.owner);
         if (rc) return rc;
         wide_row_tuples(out, answer.owner, u);
         return 0;
@@ -5197,13 +5143,22 @@ static int scan_reduce_keys_wide_impl(bydb_ctx *ctx, const bydb_query *q, const 
 
 extern "C" {
 
+int bydb_scan_reduce_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root, bydb_keyed_result *out) {
+    return guarded([&]() -> int { return scan_reduce_wide_impl(ctx, q, key, root, out); });
+}
+
+int bydb_scan_reduce_keyed_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, int32_t root,
+                                         bydb_keyed_partial_rows *out) {
+    return guarded([&]() -> int { return scan_reduce_wide_impl(ctx, q, key, root, out); });
+}
+
 int bydb_scan_reduce_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root, bydb_keys_result *out) {
-    return guarded([&]() -> int { return scan_reduce_keys_wide_impl(ctx, q, keys, root, out); });
+    return guarded([&]() -> int { return scan_reduce_wide_impl(ctx, q, keys, root, out); });
 }
 
 int bydb_scan_reduce_keys_wide_partials(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, int32_t root,
                                         bydb_keys_partial_rows *out) {
-    return guarded([&]() -> int { return scan_reduce_keys_wide_impl(ctx, q, keys, root, out); });
+    return guarded([&]() -> int { return scan_reduce_wide_impl(ctx, q, keys, root, out); });
 }
 
 int bydb_scan_reduce(bydb_ctx *ctx, const bydb_query *q, int32_t root, bydb_result *out) {
