@@ -1572,6 +1572,28 @@ int scan_agg_impl(bydb_ctx *ctx, const bydb_query *q, const std::vector<std::sha
 // into a CUDA graph and replayed.  A query executed many times (dashboards, alert rules) then costs one graph launch and
 // one synchronisation instead of ~20 runtime calls.  Everything here is additive: bydb_scan_agg is untouched.
 // ------------------------------------------------------------------------------------------------
+
+// One captured step: its graph, the device memory it runs in, and everything a replay reads.
+struct Step {
+    cudaGraphExec_t exec = nullptr;
+    // StepState: the device memory of the captured step, one allocation that lives as long as the graph (NULL: the graph runs in
+    // memory of its own, as the collective's does in the mailboxes)
+    uint8_t *step_state = nullptr;
+    FinalLayout fl;                    // a finalised step: the layout of its finalisation, whose read-back starts at rows_off
+    bydb_stats captured{};             // host-side counters of one step (launch counts, byte counts)
+    bool express = false;              // the captured step launches the express lane
+    bool partial = false;              // the captured step answers with map-phase rows (bydb_scan_partials[_keyed]_prepared)
+    bool empty = false;                // a keyed step whose discovery found no value: it holds its parts, needs no graph, answers empty
+    std::vector<std::shared_ptr<Part>> held;  // the parts whose device pointers are baked into the graph stay alive with it
+    uint64_t held_gen = 0;             // bydb_ctx::parts_gen at which `held` was last compared with the handles
+    // The read-back, set at capture: the image the graph leaves at the slot's pinned staging + image_off, and in it n_zero zero
+    // pages at zero_off; the rows at rows_off (a finalised step's finalisation read-back, or a partial step's control word and rows
+    // behind it), at most max_rows of them (0: the step answers no rows); and a keyed step's (group, key) pair of row r at
+    // pairs_off + j * pairs_stride, with j = r, or j = the row's group_id (by_position: rows carry their composite group's position).
+    size_t image_off = 0, zero_off = 0, n_zero = 0, rows_off = 0, max_rows = 0, pairs_off = 0, pairs_stride = 0;
+    bool by_position = false;
+    bool carried_status = false;       // the rows' table carries a status that is the outcome (finalize_parse)
+};
 }  // namespace
 
 struct bydb_prepared {
@@ -1586,76 +1608,47 @@ struct bydb_prepared {
     bydb_query q{};
     std::mutex mu;                     // one execution at a time per prepared query
     std::unique_ptr<ExecSlot> slot;    // dedicated stream + pinned staging: their addresses are baked into the graph
-    cudaGraphExec_t exec = nullptr;
     cudaEvent_t t0 = nullptr, t1 = nullptr;
-    FinalLayout fl;
-    size_t host_off = 0;
-    std::vector<std::shared_ptr<Part>> held;  // the parts whose device pointers are baked into the graph stay alive with it
-    uint64_t held_gen = 0;             // bydb_ctx::parts_gen at which `held` was last compared with the handles
-    // StepState: the device memory of the captured step, one allocation that lives as long as the graph.  Carved as
-    // partial table | run_scan's scratch (scan_layout) | finalize_enqueue's (final_layout) | the zero page's read-back image, or for
-    // a partial step | emit_plain_rows' (rows_layout);
-    // the staging (sids | order | group_start) is uploaded into run_scan's region once, before the capture.
-    uint8_t *step_state = nullptr;
-    size_t zero_image_off = 0;         // where in the slot's pinned memory a replay's zero page lands
-    size_t read_back = 0;              // bytes of the replay's one device-to-host copy
-    bydb_stats captured{};             // host-side counters of one step (launch counts, byte counts)
-    bool express = false;              // the captured step launches the express lane
-    bool partial_step = false;         // the captured step answers with map-phase rows (bydb_scan_partials[_keyed]_prepared)
-    bool empty_step = false;           // a keyed step whose discovery found no value: it holds its parts, needs no graph, answers empty
+    Step step;                         // the single-context step, of the form last asked for
     uint64_t runs = 0;
     bool capturable = true;
     // the collective form (bydb_scan_reduce_prepared): one captured graph per (root, slot parity)
-    struct ReduceGraph {
-        cudaGraphExec_t exec = nullptr;
-        FinalLayout fl;
-        bydb_stats captured{};
-        bool express = false;
-        std::vector<std::shared_ptr<Part>> held;
-    };
-    std::unordered_map<int, ReduceGraph> reduce_graphs;  // key = root * 2 + parity
+    std::unordered_map<int, Step> reduce_graphs;  // key = root * 2 + parity
     uint64_t reduce_runs = 0;
     bool reduce_capturable = true;
 };
 
 namespace {
 
-// drops the captured step: the graph first, then the memory it runs in.  The slot's stream is idle (every replay synchronises).
-void drop_step(bydb_prepared *p) {
-    if (p->exec) cudaGraphExecDestroy(p->exec);
-    p->exec = nullptr;
-    if (p->step_state) cudaFree(p->step_state);
-    p->step_state = nullptr;
-    p->held.clear();
-    p->empty_step = false;
+// drops a captured step: the graph first, then the memory it runs in, and with them what was set at its capture.  The slot's
+// stream is idle (every replay synchronises).
+void drop_step(Step &s) {
+    if (s.exec) cudaGraphExecDestroy(s.exec);
+    if (s.step_state) cudaFree(s.step_state);
+    s = Step();
 }
 
 void prepared_destroy(bydb_prepared *p) {
     if (!p) return;
-    drop_step(p);
-    for (auto &kv : p->reduce_graphs)
-        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+    drop_step(p->step);
+    for (auto &kv : p->reduce_graphs) drop_step(kv.second);
     if (p->t0) cudaEventDestroy(p->t0);
     if (p->t1) cudaEventDestroy(p->t1);
     delete p;  // and with it the slot
 }
 
 // A graph reads its parts through the device pointers captured with it, so it may only replay while every handle still names
-// the very part object it captured (`held`).  Otherwise the graph is dropped, to be captured again; returns false when a handle
+// the very part object it captured (`held`).  Otherwise the step is dropped, to be captured again; returns false when a handle
 // names no part any more (a released part makes the call fail like the plain path would).
-bool check_held_parts(bydb_ctx *ctx, const std::vector<bydb_part_h> &parts, cudaGraphExec_t &exec, std::vector<std::shared_ptr<Part>> &held) {
+bool check_held_parts(bydb_ctx *ctx, const std::vector<bydb_part_h> &parts, Step &s) {
     std::lock_guard<std::mutex> lk(ctx->mu);
-    bool same = held.size() == parts.size(), missing = false;
+    bool same = s.held.size() == parts.size(), missing = false;
     for (size_t i = 0; i < parts.size(); ++i) {
         auto it = ctx->parts.find(parts[i]);
         if (it == ctx->parts.end()) missing = true;
-        else if (same && it->second != held[i]) same = false;
+        else if (same && it->second != s.held[i]) same = false;
     }
-    if (missing || !same) {
-        if (exec) cudaGraphExecDestroy(exec);  // a keyed step that found no key value holds parts but no graph
-        exec = nullptr;
-        held.clear();
-    }
+    if (missing || !same) drop_step(s);
     return !missing;
 }
 
@@ -1684,7 +1677,6 @@ struct GraphCapture {
     cudaError_t err = cudaSuccess;
     const char *failed = nullptr;
 };
-constexpr const char *kBeginCapture = "begin capture";
 
 // Captures what enqueue() (returning 0 or a code) puts on stream `s` as one graph, instantiated into *exec.  The file's only capture:
 // the stream always leaves capture mode again.
@@ -1693,7 +1685,7 @@ GraphCapture capture_graph(cudaStream_t s, cudaGraphExec_t *exec, Enqueue &&enqu
     GraphCapture c;
     c.err = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
     if (c.err != cudaSuccess) {
-        c.failed = kBeginCapture;
+        c.failed = "begin capture";
         return c;
     }
     c.rc = enqueue();
@@ -1708,104 +1700,125 @@ GraphCapture capture_graph(cudaStream_t s, cudaGraphExec_t *exec, Enqueue &&enqu
     return c;
 }
 
-// Allocates the step state p->step_state (`bytes`) and uploads the query's staging (layout st) into it at `sids_off`, synchronised: the
-// captured kernels read the staging from there on every replay.  False when the state cannot be had; else `e` is the upload's error.
-bool make_step_state(bydb_prepared *p, size_t bytes, const StageLayout &st, size_t sids_off, cudaError_t &e) {
-    if (cudaMalloc(reinterpret_cast<void **>(&p->step_state), bytes) != cudaSuccess) return false;
-    ExecSlot &slot = *p->slot;
-    stage_series(&p->q, st, slot.pinned);
-    e = cudaMemcpyAsync(p->step_state + sids_off, slot.pinned, st.bytes, cudaMemcpyHostToDevice, slot.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(slot.stream);
-    return true;
-}
+// A capture of a single-context step (prepared_capture, keyed_capture, wide_capture) is these plain steps in order, around its own
+// layout and the body it enqueues:
+//   capture_begin    the parts' generation, the plan, the refusal of parts that overlap in time
+//   (keyed)          discovery, and a step with no key value, which needs no graph (capture_finish with ok set and p->step.empty)
+//   step_memory      the pinned staging and the step state, with or without the staging upload
+//   capture_finish   the one failure policy and the one commit
+// A capture returns make_plan's code, else 0 whether or not it left a step to replay.
 
-// captures one step into p->exec, building the StepState it runs in; returns 0, or a code after leaving the stream out of
-// capture mode.  0 with p->exec == NULL: this query keeps the uncaptured path.  The tail after group_reduce: finalisation, row
-// selection and one read-back copy, or (partial) emit_plain_rows, whose last kernel writes the zero page and the rows to the staging.
-int prepared_capture(bydb_ctx *ctx, bydb_prepared *p, bool partial) {
-    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up: a later change is seen by the next run
-    Plan plan;
-    int rc = make_plan(ctx, &p->q, nullptr, plan);
-    if (rc) return rc;
-    // the version-dedup precheck of run_scan synchronises: parts that overlap in time keep the uncaptured path
-    if (parts_overlap(plan.parts, p->q.tmin, p->q.tmax)) {
+// The one end of every capture.  After the plan is made, any failure (ok false: a refusal, discovery, the staging or the state; a
+// failed enqueue; a failed capture) drops the step and leaves the handle on the unprepared path for good, this execution included.
+// Else the step is committed: it holds the parts it was planned over, as of `gen`.
+int capture_finish(bydb_prepared *p, const Plan &plan, uint64_t gen, bool ok, const GraphCapture &c = GraphCapture()) {
+    Step &s = p->step;
+    if (!ok || c.rc || c.err != cudaSuccess || !(s.exec || s.empty)) {
+        cudaGetLastError();
+        drop_step(s);
         p->capturable = false;
         return 0;
     }
+    s.held = plan.parts;
+    s.held_gen = gen;
+    return 0;
+}
+
+// The head of every capture: the parts' generation, read before the handles are looked up (a later change is seen by the next
+// execution), and the plan.  Parts that overlap in time are refused for good: run_scan's version-dedup precheck synchronises.
+int capture_begin(bydb_ctx *ctx, bydb_prepared *p, Plan &plan, uint64_t &gen) {
+    gen = ctx->parts_gen.load(std::memory_order_acquire);
+    const int rc = make_plan(ctx, &p->q, nullptr, plan);
+    if (!rc && parts_overlap(plan.parts, p->q.tmin, p->q.tmax)) capture_finish(p, plan, gen, false);
+    return rc;
+}
+
+// The memory of the step being captured: the slot's pinned staging grown to `pinned` bytes (h_dst, when asked for: the device
+// address of the step's image there, through which rows_to_host_kernel writes) and the step state of `bytes`.  `st` given: the
+// query's staging is uploaded into the state at `sids_off`, synchronised, and the captured kernels read it from there on every
+// replay.  False when any of it cannot be had.
+bool step_memory(bydb_prepared *p, size_t pinned, size_t bytes, const StageLayout *st, size_t sids_off, uint8_t **h_dst) {
+    ExecSlot &slot = *p->slot;
+    Step &s = p->step;
+    if (slot.ensure_pinned(pinned) || (h_dst && !(*h_dst = slot.pinned_dev(s.image_off)))) return false;
+    if (cudaMalloc(reinterpret_cast<void **>(&s.step_state), bytes) != cudaSuccess) {
+        s.step_state = nullptr;
+        return false;
+    }
+    if (!st) return true;
+    stage_series(&p->q, *st, slot.pinned);
+    return cudaMemcpyAsync(s.step_state + sids_off, slot.pinned, st->bytes, cudaMemcpyHostToDevice, slot.stream) == cudaSuccess &&
+           cudaStreamSynchronize(slot.stream) == cudaSuccess;
+}
+
+// Captures the plain step.  Step state: partial table | run_scan's scratch (scan_layout), the staging (sids | order | group_start)
+// uploaded into it | finalize_enqueue's (final_layout) and the zero page's image, or for a partial step emit_plain_rows'
+// (rows_layout).  The tail after group_reduce: finalisation, row selection and one read-back copy of [rows | zero page], or
+// (partial) emit_plain_rows, whose last kernel writes [zero page | control word | rows] to the staging.  Either lands behind the
+// staging area.
+int prepared_capture(bydb_ctx *ctx, bydb_prepared *p, bool partial) {
+    Plan plan;
+    uint64_t gen = 0;
+    if (int rc = capture_begin(ctx, p, plan, gen); rc || !p->capturable) return rc;
+    Step &s = p->step;
     ExecSlot &slot = *p->slot;
     const TableLayout &tl = plan.tl;
     const StageLayout st = stage_layout(p->q.n_series, tl.G);
     const ScanLayout sl = scan_layout(st, plan.total_blocks, plan.fcols.size(), plan.parts.size(), false);
     const FinalLayout fl = final_layout(tl.G, p->q.n_aggs, p->q.top_n);
     const RowsLayout rl = rows_layout(&p->q, plan);
-    p->host_off = st.stride;  // the read-back lands behind the staging area
-    if (slot.ensure_pinned(partial ? partial_pinned_bytes(&p->q, plan) : step_pinned_bytes(&p->q, tl.G, tl.G))) return fail(BYDB_ENOMEM, "cudaMallocHost failed");
-    uint8_t *h_dst = partial ? slot.pinned_dev(p->host_off) : nullptr;
     Carve carve;
     const size_t off_table = carve(tl.total), off_scan = carve(sl.total), off_fin = carve(partial ? rl.total : fl.total + kZeroPageBytes);
-    cudaError_t e = cudaSuccess;
-    if ((partial && !h_dst) || !make_step_state(p, carve.o, st, off_scan + sl.off_sids, e)) {
-        cudaGetLastError();
-        p->step_state = nullptr;
-        p->capturable = false;
-        return 0;
-    }
-    uint32_t fin_launches = 0;
+    s.partial = partial;
+    s.image_off = st.stride;
+    s.n_zero = 1;
+    s.zero_off = partial ? 0 : fl.out_bytes;
+    s.rows_off = partial ? kZeroPageBytes : 0;
+    s.max_rows = partial ? tl.G : fl.cap;
+    uint8_t *h_dst = nullptr;
+    const bool ok = step_memory(p, partial ? partial_pinned_bytes(&p->q, plan) : step_pinned_bytes(&p->q, tl.G, tl.G), carve.o, &st,
+                                off_scan + sl.off_sids, partial ? &h_dst : nullptr);
     GraphCapture c;
-    if (e == cudaSuccess) c = capture_graph(slot.stream, &p->exec, [&]() -> int {
-        memset(&p->captured, 0, sizeof p->captured);
+    if (ok) c = capture_graph(slot.stream, &s.exec, [&]() -> int {
         Scratch scan, fin;
-        scan.view(p->step_state + off_scan, sl.total);
-        fin.view(p->step_state + off_fin, fl.total + kZeroPageBytes);
-        rc = run_scan(ctx, &p->q, plan, slot, slot.stream, p->step_state + off_table, tl, &p->captured, 0, nullptr, &scan);
-        p->express = slot.express[0];
-        if (!rc && partial) {
-            emit_plain_rows(&p->q, plan, slot.stream, p->step_state + off_table, p->step_state + off_fin, scan.base + sl.off_zero, kZeroPageBytes, h_dst);
-            fin_launches = kPlainRowsLaunches;
-            p->read_back = 0;  // sized by the rows present: the replay counts it
-        } else if (!rc) {
-            rc = finalize_enqueue(&p->q, plan, slot, slot.stream, p->step_state + off_table, tl, p->host_off, fin, p->fl, fin_launches, p->read_back,
-                                  scan.base + sl.off_zero);
+        scan.view(s.step_state + off_scan, sl.total);
+        fin.view(s.step_state + off_fin, fl.total + kZeroPageBytes);
+        int rc = run_scan(ctx, &p->q, plan, slot, slot.stream, s.step_state + off_table, tl, &s.captured, 0, nullptr, &scan);
+        s.express = slot.express[0];
+        if (rc) return rc;
+        if (partial) {  // the read-back is sized by the rows present: the replay counts it
+            emit_plain_rows(&p->q, plan, slot.stream, s.step_state + off_table, s.step_state + off_fin, scan.base + sl.off_zero, kZeroPageBytes, h_dst);
+            s.captured.kernel_launches += kPlainRowsLaunches;
+            return 0;
         }
+        uint32_t launches = 0;  // finalize + select_rows (one fused launch for few groups)
+        size_t read_back = 0;
+        rc = finalize_enqueue(&p->q, plan, slot, slot.stream, s.step_state + off_table, tl, s.image_off, fin, s.fl, launches, read_back,
+                              scan.base + sl.off_zero);
+        s.captured.kernel_launches += launches;
+        s.captured.d2h_bytes += read_back;
         return rc;
     });
-    if (e != cudaSuccess || c.failed == kBeginCapture) {
-        drop_step(p);
-        return fail(BYDB_EIO, std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(e != cudaSuccess ? e : c.err));
-    }
-    if (c.rc || c.err != cudaSuccess || !p->exec) {
-        cudaGetLastError();
-        drop_step(p);
-        p->capturable = false;  // fall back to the uncaptured path for good
-        return c.rc;
-    }
-    p->captured.kernel_launches += fin_launches;  // finalize + select_rows (one fused launch for few groups), or the three row kernels
-    p->captured.d2h_bytes += p->read_back;
-    p->zero_image_off = partial ? p->host_off : p->host_off + p->fl.out_bytes;
-    p->partial_step = partial;
-    p->held = plan.parts;
-    p->held_gen = gen;
-    return 0;
+    return capture_finish(p, plan, gen, ok, c);
 }
 
 // The schedule of a prepared query: its first execution runs the uncaptured path (which also performs the one-time kernel attribute
 // setup), the second one captures, later ones replay.  Makes the step of the form asked for (partial: map-phase rows) ready to replay,
 // capturing it with capture() when there is none: a step of the other form gives way (one step per handle), and a step whose handles
-// stopped naming its parts is captured again.  Returns a code (BYDB_ENOENT: a handle names no part), or 0 with neither p->exec nor
-// p->empty_step when this execution takes the uncaptured path.
+// stopped naming its parts is captured again.  Returns a code (BYDB_ENOENT: a handle names no part), or 0 with neither a graph
+// nor an empty step when this execution takes the uncaptured path.
 template <class Capture>
 int prepared_step(bydb_ctx *ctx, bydb_prepared *p, bool partial, Capture &&capture) {
+    Step &s = p->step;
     if (p->runs++ == 0 || !p->capturable) return 0;
-    if (p->exec && p->partial_step != partial) drop_step(p);
-    if (!p->exec && !p->empty_step) return capture();
+    if (s.exec && s.partial != partial) drop_step(s);
+    if (!s.exec && !s.empty) return capture();
     // the handles can only have changed their parts if one was registered or released since `held` was last compared
     const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);
-    if (gen != p->held_gen) {
-        const bool all_there = check_held_parts(ctx, p->parts, p->exec, p->held);
-        if (!p->exec && p->held.empty()) drop_step(p);  // the state is sized for the parts it was captured with
-        if (!all_there) return fail(BYDB_ENOENT, "unknown part handle");
-        p->held_gen = gen;
-        if (!p->exec && !p->empty_step) return capture();
+    if (gen != s.held_gen) {
+        if (!check_held_parts(ctx, p->parts, s)) return fail(BYDB_ENOENT, "unknown part handle");
+        s.held_gen = gen;
+        if (!s.exec && !s.empty) return capture();
     }
     return 0;
 }
@@ -2751,6 +2764,57 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const Key *key, Out
     return 0;
 }
 
+// One replay of a captured step, synchronised.  The regions of its image that the graph writes are zeroed first -- the zero pages,
+// and a partial step's control word (ctl_bytes) -- so that a replay that fails to launch cannot report the previous one's status or
+// rows.  Then replay_graph, with the counters and device error of the first zero page; the other pages are folded in as the plain
+// path collects its passes: the counters add up and the first pass with a device error decides.
+int replay_step(bydb_prepared *p, const Step &s, size_t ctl_bytes, bydb_stats *stats) {
+    uint8_t *image = p->slot->pinned + s.image_off;
+    memset(image + s.zero_off, 0, s.n_zero * kZeroPageBytes);
+    if (s.partial && s.max_rows) memset(image + s.rows_off, 0, ctl_bytes);
+    auto page = [&](size_t v) -> const ZeroPage & { return *reinterpret_cast<const ZeroPage *>(image + s.zero_off + v * kZeroPageBytes); };
+    int rc = replay_graph(s.exec, *p->slot, p->t0, p->t1, s.captured, s.express, page(0), stats);
+    for (size_t v = 1; !rc && v < s.n_zero; ++v) rc = read_zero_page(page(v), false, stats);
+    return rc;
+}
+
+// the rows of an answer: a plain answer is its rows, a keyed one holds them in `base`
+bydb_result *rows_of(bydb_result *out) { return out; }
+bydb_result *rows_of(bydb_keyed_result *out) { return &out->base; }
+bydb_partial_rows *rows_of(bydb_partial_rows *out) { return out; }
+bydb_partial_rows *rows_of(bydb_keyed_partial_rows *out) { return &out->base; }
+
+// The answer of a replayed finalised step from its image: the result rows, then a keyed answer's (group, key) pairs (its owner and
+// key table are set up already)
+template <class Out>
+int finalised_answer(const bydb_prepared *p, const Step &s, Out *out) {
+    if (!s.max_rows) return 0;
+    const uint8_t *image = p->slot->pinned + s.image_off;
+    bydb_result *r = rows_of(out);
+    const int rc = finalize_parse(image + s.rows_off, s.fl, s.carried_status, r);
+    if constexpr (std::is_same<Out, bydb_keyed_result>::value)
+        if (!rc)
+            set_row_keys(out, static_cast<KeyedOwner *>(out->owner), static_cast<ResultOwner *>(r->owner)->group_id, image + s.pairs_off, s.pairs_stride,
+                         s.by_position);
+    return rc;
+}
+
+// The answer of a replayed partial step from its image, over the query's shape: the bytes the copy kernel brought back into
+// `stats`, the row image (its status, then the rows), then a keyed answer's (group, key) pairs
+template <class Out>
+int partial_answer(const bydb_prepared *p, const Step &s, const Plan &shape, Out *out, bydb_stats &stats) {
+    if (!s.max_rows) return 0;
+    const uint8_t *image = p->slot->pinned + s.image_off, *rows = image + s.rows_off;
+    stats.d2h_bytes += s.rows_off + keyed_ctl_bytes(shape.fcols.size()) + rows_in(rows, s.max_rows) * keyed_row_bytes(p->q.n_aggs);
+    bydb_partial_rows *r = rows_of(out);
+    const int rc = parse_rows(rows, &p->q, shape, s.max_rows, r);
+    if constexpr (std::is_same<Out, bydb_keyed_partial_rows>::value)
+        if (!rc)
+            set_row_keys(out, static_cast<KeyedOwner *>(out->owner), static_cast<PartialRowsOwner *>(r->owner)->group_id, image + s.pairs_off,
+                         s.pairs_stride, s.by_position);
+    return rc;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -2760,80 +2824,70 @@ int scan_keyed_wide_impl(bydb_ctx *ctx, const bydb_query *q, const Key *key, Out
 // Everything here is additive: bydb_scan_agg_keyed is untouched.
 // ------------------------------------------------------------------------------------------------
 struct bydb_prepared_keyed {
-    bydb_prepared *pq = nullptr;   // the query's deep copy, its slot, events, graph, step state and held parts
+    bydb_prepared *pq = nullptr;   // the query's deep copy, its slot, events and captured step
     std::string family, tag;       // the key's strings: key.family / key.tag point here
     bydb_group_key key{};
     uint32_t cap = 0;              // distinct values accepted (check_group_key)
     KeyValues values;              // found when the step was captured: the key table of every replay
-    size_t pairs_off = 0, zero_off = 0;  // in the replay's read-back image: the rows' (group, key) pairs, the passes' zero pages
     bool wide = false;             // bydb_query_prepare_keyed_wide: one scan pass (wide_capture), not one per value
-    size_t n_comp = 0;             // wide: C, the present composite groups found when the step was captured
     ~bydb_prepared_keyed() { prepared_destroy(pq); }
 };
 
 namespace {
-// Discovers the key values and captures the keyed step into k->pq->exec, in a step state of its own:
+// Discovers the key values and captures the keyed step, in a step state of its own:
 //   composite table | permuted table | the passes' column types | Kts | Krow | the order's slots, first_series, perm, n_present |
 //   one scan scratch (scan_layout, the passes run one after another) | finalisation over V x G groups, then the rows' (group, key)
 //   pairs and the V zero pages, so that one copy reads back the rows, their pairs and the passes' counters and errors.
 // `partial` (bydb_scan_partials_keyed_prepared) selects the other tail: no permuted table and no finalisation; behind the order,
 // keyed_partial_rows_kernel writes the row image (control word, rows) right behind the V zero pages, and rows_to_host_kernel
-// brings the pages, the control word and exactly the present rows to the staging.
-// Leaves neither a graph nor p->empty_step when this execution, or (capturable cleared) every later one, takes the plain path: a part
-// is missing, the parts overlap, discovery fails (its refusal is the plain call's), or the state or the capture cannot be had.
-void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
+// brings the pages, the control word and exactly the present rows to the staging.  A discovery that fails (its refusal is the
+// plain call's) keeps the unprepared path.
+int keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     bydb_prepared *p = k->pq;
     const bydb_query *q = &p->q;
-    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up
     Plan plan;
-    if (make_plan(ctx, q, nullptr, plan)) return;
+    uint64_t gen = 0;
+    if (int rc = capture_begin(ctx, p, plan, gen); rc || !p->capturable) return rc;
+    Step &s = p->step;
     ExecSlot &slot = *p->slot;
     cudaStream_t stream = slot.stream;
     bydb_stats discovery{};
-    KeyValues values;
-    if (parts_overlap(plan.parts, q->tmin, q->tmax) || discover_keys(ctx, q, &k->key, k->cap, plan, slot, &discovery, values)) {
-        p->capturable = false;
-        return;
-    }
-    const size_t V = values.size(), F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
+    if (discover_keys(ctx, q, &k->key, k->cap, plan, slot, &discovery, k->values)) return capture_finish(p, plan, gen, false);
+    const size_t V = k->values.size(), F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
     if (V == 0) {
-        k->values.clear();
-        p->empty_step = true;
-        p->held = plan.parts;
-        p->held_gen = gen;
-        return;
+        s.empty = true;
+        return capture_finish(p, plan, gen, true);
     }
-    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) {
-        p->capturable = false;
-        return;
-    }
+    if (GP > 0x7fffffffull / std::max<size_t>(F, 1)) return capture_finish(p, plan, gen, false);
     const TableLayout tlc(GP, F);
     const StageLayout st = stage_layout(NS, G);
     const ScanLayout sl = scan_layout(st, plan.total_blocks, F, plan.parts.size(), true);
     const FinalLayout fl = final_layout(GP, q->n_aggs, q->top_n);
-    const size_t b_pairs = align_up(fl.cap * 8, 256), b_zero = V * kZeroPageBytes;
-    const size_t b_rows = keyed_ctl_bytes(F) + GP * keyed_row_bytes(q->n_aggs);  // partial: the row image
+    const size_t ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(q->n_aggs);
+    const size_t b_pairs = align_up(fl.cap * 8, 256), b_zero = V * kZeroPageBytes, b_rows = ctl_bytes + GP * row_bytes;  // partial: the row image
     Carve carve;
     const size_t o_src = carve(tlc.total), o_dst = carve(partial ? 0 : tlc.total), o_ct = carve(V * F * 8), o_kts = carve(V * NS * 8),
                  o_krow = carve(V * NS * 4), o_slot = carve(NS * V * 4), o_first = carve(GP * 4), o_perm = carve(GP * 4), o_np = carve(16),
                  o_scan = carve(sl.total), o_fin = carve(partial ? b_zero + b_rows : fl.total + b_pairs + b_zero);
-    p->host_off = st.stride;  // the read-back lands behind the staging area, as in the plain prepared step
-    p->read_back = partial ? b_zero + b_rows : fl.out_bytes + b_pairs + b_zero;  // partial: the most the copy kernel may write
-    // sized before the capture: the graph writes the staging through its device address
-    uint8_t *h_dst = slot.ensure_pinned(p->host_off + p->read_back) ? nullptr : slot.pinned_dev(p->host_off);
-    cudaError_t e = cudaSuccess;
-    if (!h_dst || !make_step_state(p, carve.o, st, o_scan + sl.off_sids, e)) {
-        cudaGetLastError();
-        p->step_state = nullptr;
-        p->capturable = false;
-        return;
-    }
-    uint8_t *S = p->step_state, *fin_base = S + o_fin, *zero_pages = partial ? fin_base : fin_base + fl.total + b_pairs;
-    bydb_stats &cs = p->captured;
-    uint32_t fin_launches = 0;
+    // the read-back lands behind the staging area, as in the plain prepared step: [rows | pairs | V zero pages], or (partial) the
+    // most the copy kernel may write, [V zero pages | control word | rows]
+    const size_t read_back = partial ? b_zero + b_rows : fl.out_bytes + b_pairs + b_zero;
+    s.partial = partial;
+    s.fl = fl;
+    s.image_off = st.stride;
+    s.n_zero = V;
+    s.zero_off = partial ? 0 : fl.out_bytes + b_pairs;
+    s.rows_off = partial ? b_zero : 0;
+    s.max_rows = partial ? GP : fl.cap;
+    s.pairs_off = partial ? b_zero + ctl_bytes : fl.out_bytes;
+    s.pairs_stride = partial ? row_bytes : 8;
+    s.carried_status = true;
+    uint8_t *h_dst = nullptr;
+    const bool ok = step_memory(p, s.image_off + read_back, carve.o, &st, o_scan + sl.off_sids, partial ? &h_dst : nullptr);
+    bydb_stats &cs = s.captured;
     GraphCapture c;
-    if (e == cudaSuccess) c = capture_graph(stream, &p->exec, [&]() -> int {
-        memset(&cs, 0, sizeof cs);
+    if (ok) c = capture_graph(stream, &s.exec, [&]() -> int {
+        uint8_t *S = s.step_state, *fin_base = S + o_fin, *zero_pages = partial ? fin_base : fin_base + fl.total + b_pairs;
         int64_t *ct = reinterpret_cast<int64_t *>(S + o_ct), *kts = reinterpret_cast<int64_t *>(S + o_kts);
         uint32_t *krow = reinterpret_cast<uint32_t *>(S + o_krow);
         KeyedResetParams rp;
@@ -2851,7 +2905,7 @@ void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
         Scratch scan, kb, fin;
         scan.view(S + o_scan, sl.total);
         fin.view(fin_base, fl.total + b_pairs + b_zero);
-        int rc = run_keyed_passes(ctx, q, &k->key, plan, slot, values, tlc, S + o_src, ct, kts, krow, nullptr, &cs, &scan, zero_pages);
+        int rc = run_keyed_passes(ctx, q, &k->key, plan, slot, k->values, tlc, S + o_src, ct, kts, krow, nullptr, &cs, &scan, zero_pages);
         KeyOrderParams res, ko;
         memset(&res, 0, sizeof res);
         res.order = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_order);
@@ -2861,9 +2915,7 @@ void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
         res.perm = reinterpret_cast<int32_t *>(S + o_perm);
         res.n_present = reinterpret_cast<uint32_t *>(S + o_np);
         if (!rc) rc = keyed_order(q, plan, slot, V, kts, krow, kb, ko, cs, &res);
-        FinalLayout flc;
-        size_t fin_back = 0;
-        if (!rc && partial) {
+        if (!rc && partial) {  // the read-back is sized by the rows present: the replay counts it
             launch_keyed_partial_rows(rows_params(q, plan, V, tlc.at(S + o_src), ct, ko.perm, ko.n_present, zero_pages + b_zero), GP, stream);
             RowsCopyParams cp;
             memset(&cp, 0, sizeof cp);
@@ -2871,93 +2923,59 @@ void keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
             cp.image = zero_pages + b_zero;
             cp.dst = h_dst;
             cp.page_bytes = b_zero;
-            cp.ctl_bytes = keyed_ctl_bytes(F);
-            cp.row_bytes = keyed_row_bytes(q->n_aggs);
+            cp.ctl_bytes = ctl_bytes;
+            cp.row_bytes = row_bytes;
             cp.max_rows = static_cast<uint32_t>(GP);
             launch_rows_to_host(cp, stream);
+            cs.kernel_launches += 2;
         } else if (!rc) {
             launch_permute_table(tlc.at(S + o_dst), tlc.at(S + o_src), ko.perm, static_cast<uint32_t>(GP), static_cast<uint32_t>(F), ct,
                                  static_cast<uint32_t>(V), stream);
             Plan planc = plan;
             planc.n_groups = static_cast<int32_t>(GP);
+            FinalLayout flc;
+            uint32_t fin_launches = 0;
+            size_t fin_back = 0;
             rc = finalize_launch(q, planc, stream, S + o_dst, tlc, fin, flc, fin_launches, fin_back);
             if (!rc) {
                 launch_keyed_row_map(reinterpret_cast<const int32_t *>(fin_base + fl.o_sg), reinterpret_cast<const uint32_t *>(fin_base + fl.o_cnt),
                                      ko.perm, static_cast<uint32_t>(G), static_cast<uint32_t>(fl.cap), reinterpret_cast<int32_t *>(fin_base + fl.total), stream);
-                if (cudaMemcpyAsync(slot.pinned + p->host_off, fin_base + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+                if (cudaMemcpyAsync(slot.pinned + s.image_off, fin_base + fl.o_out, read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+                cs.kernel_launches += 1 + fin_launches + 1;  // permute_table, finalisation + row selection, the row mapping
+                cs.d2h_bytes += read_back;
             }
         }
         return rc;
     });
-    if (e != cudaSuccess || c.rc || c.err != cudaSuccess || !p->exec) {
-        cudaGetLastError();
-        drop_step(p);
-        p->capturable = false;
-        return;
-    }
-    // permute_table, finalisation + row selection, the row mapping; or the row kernel and the copy kernel.  A partial step's read-back
-    // is sized by the rows present: the replay counts it.
-    cs.kernel_launches += partial ? 2 : 1 + fin_launches + 1;
-    cs.d2h_bytes = partial ? 0 : p->read_back;
-    p->partial_step = partial;
-    p->fl = fl;
-    p->express = false;  // the key predicate keeps every pass off the express lane
-    k->values = std::move(values);
-    k->pairs_off = fl.out_bytes;
-    k->zero_off = partial ? 0 : fl.out_bytes + b_pairs;
-    p->held = plan.parts;
-    p->held_gen = gen;
+    return capture_finish(p, plan, gen, ok, c);
 }
 
-// the answer of a replayed keyed step from its read-back `image`, after the passes' zero pages: the finalised rows and their
-// (group, key) pairs, or the row image (table status, rows, their key values) and the bytes the copy kernel brought back
-int keyed_answer(bydb_prepared_keyed *k, const Plan &, const uint8_t *image, bydb_keyed_result *out, KeyedOwner *owner) {
-    const int rc = finalize_parse(image, k->pq->fl, true, &out->base);
-    if (rc) return rc;
-    set_row_keys(out, owner, static_cast<ResultOwner *>(out->base.owner)->group_id, image + k->pairs_off, 8, false);
-    return 0;
-}
-int keyed_answer(bydb_prepared_keyed *k, const Plan &shape, const uint8_t *image, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
-    const size_t V = k->values.size(), GP = V * shape.tl.G, A = k->pq->q.n_aggs;
-    const uint8_t *rows = image + V * kZeroPageBytes;
-    const size_t ctl_bytes = keyed_ctl_bytes(shape.fcols.size()), row_bytes = keyed_row_bytes(A);
-    out->stats.d2h_bytes += V * kZeroPageBytes + ctl_bytes + rows_in(rows, GP) * row_bytes;
-    const int rc = parse_rows(rows, &k->pq->q, shape, GP, &out->base);
-    if (rc) return rc;
-    set_row_keys(out, owner, static_cast<PartialRowsOwner *>(out->base.owner)->group_id, rows + ctl_bytes, row_bytes, false);
-    return 0;
-}
-
-// Captures the wide keyed step into k->pq->exec.  Outside the graph, once: the plain path's discovery, scan and order (wide_pass)
-// find the key table, R and C -- functions of the parts the handles name and of the fixed query, so properties of the capture.
-// Then one step state, allocated once and laid out as
+// Captures the wide keyed step.  Outside the graph, once: the plain path's discovery, scan and order (wide_pass) find the key
+// table, R and C -- functions of the parts the handles name and of the fixed query, so properties of the capture.  Then one step
+// state, laid out as
 //   discovery's scratch, copied from the eager run (value table, slot ids, ranks, first records, series ids and groups) |
 //   the table of the C composite groups | perm | (partial) their (group, key) pairs | the scan and order's scratch, zero page first |
 //   the tail: the finalisation over C groups with the zero page gathered behind it and the pairs behind that, or the row image,
 // and the graph: keyed_step_reset_kernel (zero page, composite table, ctl; comp_min) -> wide_scan_order -> wide_fold_kernel -> the
 // finalisation and ONE copy of rows, zero page and pairs; or keyed_partial_rows_kernel and rows_to_host_kernel bringing the pairs,
-// the zero page (one range), the control word and the C rows.  C = 0: the graph ends with a copy of the zero page.
-// Leaves neither a graph nor p->empty_step when this execution, or (capturable cleared) every later one, takes the plain path.
-void wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
+// the zero page (one range), the control word and the C rows.  C = 0: the graph ends with a copy of the zero page.  A wide_pass
+// that fails (its refusal is the plain call's) keeps the unprepared path.
+int wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     bydb_prepared *p = k->pq;
     const bydb_query *q = &p->q;
-    const uint64_t gen = ctx->parts_gen.load(std::memory_order_acquire);  // before the handles are looked up
     Plan plan;
-    if (make_plan(ctx, q, nullptr, plan)) return;
+    uint64_t gen = 0;
+    if (int rc = capture_begin(ctx, p, plan, gen); rc || !p->capturable) return rc;
+    Step &s = p->step;
     ExecSlot &slot = *p->slot;
     cudaStream_t stream = slot.stream;
     bydb_stats eager{};
     WidePass w;
-    if (parts_overlap(plan.parts, q->tmin, q->tmax) || wide_pass(ctx, q, &k->key, 1, k->cap, plan, slot, eager, w)) {
-        p->capturable = false;
-        return;
-    }
+    if (wide_pass(ctx, q, &k->key, 1, k->cap, plan, slot, eager, w)) return capture_finish(p, plan, gen, false);
+    k->values = std::move(w.values);
     if (w.R == 0) {
-        k->values = std::move(w.values);
-        p->empty_step = true;
-        p->held = plan.parts;
-        p->held_gen = gen;
-        return;
+        s.empty = true;
+        return capture_finish(p, plan, gen, true);
     }
     const size_t F = plan.fcols.size(), A = q->n_aggs, C = w.n_comp;
     const size_t ctl_bytes = keyed_ctl_bytes(F), row_bytes = keyed_row_bytes(A);
@@ -2968,32 +2986,39 @@ void wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     const size_t o_disc = carve(w.disc_bytes), o_table = carve(tl.total), o_perm = carve(C * 4), o_pairs = carve(partial ? C * 8 : 0),
                  o_scan = carve(L.total), o_tail = carve(C == 0 ? 0 : partial ? ctl_bytes + C * row_bytes : fl.total + kZeroPageBytes + C * 8);
     const size_t pages = o_scan + L.zero + kZeroPageBytes - o_pairs;  // partial: the pairs, padded, then the zero page
-    p->host_off = 0;  // the staging serves only the read-back: discovery's outputs stay on the device
-    p->read_back = C == 0 ? kZeroPageBytes : partial ? pages + ctl_bytes + C * row_bytes : fl.out_bytes + kZeroPageBytes + C * 8;
-    uint8_t *h_dst = slot.ensure_pinned(p->read_back) ? nullptr : slot.pinned_dev(0);
-    if (!h_dst || cudaMalloc(reinterpret_cast<void **>(&p->step_state), carve.o) != cudaSuccess) {
-        cudaGetLastError();
-        p->step_state = nullptr;
-        p->capturable = false;
-        return;
+    // the staging serves only the read-back: [rows | zero page | pairs], or (partial) [pairs | zero page | control word | rows] at
+    // most, or (C = 0) the zero page alone.  Discovery's outputs stay on the device.
+    const size_t read_back = C == 0 ? kZeroPageBytes : partial ? pages + ctl_bytes + C * row_bytes : fl.out_bytes + kZeroPageBytes + C * 8;
+    s.partial = partial;
+    s.fl = fl;
+    s.n_zero = 1;
+    s.zero_off = C == 0 ? 0 : partial ? pages - kZeroPageBytes : fl.out_bytes;
+    s.rows_off = partial ? pages : 0;
+    s.max_rows = partial ? C : fl.cap;
+    s.pairs_off = partial ? 0 : fl.out_bytes + kZeroPageBytes;
+    s.pairs_stride = 8;
+    s.by_position = true;
+    s.carried_status = true;
+    uint8_t *h_dst = nullptr;
+    bool ok = step_memory(p, read_back, carve.o, nullptr, 0, partial ? &h_dst : nullptr);
+    if (ok) {  // discovery's scratch into the state, and its device pointers moved to the copy
+        uint8_t *S = s.step_state;
+        ok = cudaMemcpyAsync(S + o_disc, w.ka.base, w.disc_bytes, cudaMemcpyDeviceToDevice, stream) == cudaSuccess &&
+             cudaStreamSynchronize(stream) == cudaSuccess;
+        auto moved = [&](auto *ptr) { return reinterpret_cast<decltype(ptr)>(S + o_disc + (reinterpret_cast<const uint8_t *>(ptr) - w.ka.base)); };
+        KeyParams &kp = w.wk.k;
+        kp.q_sids = moved(kp.q_sids);
+        kp.slots = moved(kp.slots);
+        kp.zero = moved(kp.zero);
+        w.wk.slot_id = moved(w.wk.slot_id);
+        w.wk.rank = moved(w.wk.rank);
+        w.wk.n_by_rank = moved(w.wk.n_by_rank);
+        w.series_group = moved(w.series_group);
     }
-    uint8_t *S = p->step_state, *sb = S + o_scan, *tail = S + o_tail;
-    cudaError_t e = cudaMemcpyAsync(S + o_disc, w.ka.base, w.disc_bytes, cudaMemcpyDeviceToDevice, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    // discovery's device pointers, moved to the copy
-    auto moved = [&](auto *ptr) { return reinterpret_cast<decltype(ptr)>(S + o_disc + (reinterpret_cast<const uint8_t *>(ptr) - w.ka.base)); };
-    KeyParams &kp = w.wk.k;
-    kp.q_sids = moved(kp.q_sids);
-    kp.slots = moved(kp.slots);
-    kp.zero = moved(kp.zero);
-    w.wk.slot_id = moved(w.wk.slot_id);
-    w.wk.rank = moved(w.wk.rank);
-    w.wk.n_by_rank = moved(w.wk.n_by_rank);
-    w.series_group = moved(w.series_group);
-    bydb_stats &cs = p->captured;
+    bydb_stats &cs = s.captured;
     GraphCapture c;
-    if (e == cudaSuccess) c = capture_graph(stream, &p->exec, [&]() -> int {
-        memset(&cs, 0, sizeof cs);
+    if (ok) c = capture_graph(stream, &s.exec, [&]() -> int {
+        uint8_t *S = s.step_state, *sb = S + o_scan, *tail = S + o_tail;
         KeyedResetParams rs;
         memset(&rs, 0, sizeof rs);
         rs.zero[0] = reinterpret_cast<uint32_t *>(sb + L.zero);
@@ -3005,7 +3030,10 @@ void wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
         int rc = wide_scan_order(ctx, q, plan, w, sb, L, stream, nullptr, launches);
         cs.kernel_launches += 1 + launches;
         if (rc) return rc;
-        if (C == 0) return cudaMemcpyAsync(slot.pinned, sb + L.zero, kZeroPageBytes, cudaMemcpyDeviceToHost, stream) == cudaSuccess ? 0 : BYDB_EIO;
+        if (C == 0) {
+            cs.d2h_bytes += kZeroPageBytes;
+            return cudaMemcpyAsync(slot.pinned, sb + L.zero, kZeroPageBytes, cudaMemcpyDeviceToHost, stream) == cudaSuccess ? 0 : BYDB_EIO;
+        }
         WideReduceParams &rp = w.rp;
         rp.table = tl.at(S + o_table);
         rp.perm = reinterpret_cast<int32_t *>(S + o_perm);
@@ -3014,7 +3042,7 @@ void wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
         cs.kernel_launches += 1;
         Plan planc = plan;
         planc.n_groups = static_cast<int32_t>(C);
-        if (partial) {
+        if (partial) {  // the read-back is sized by the rows present: the replay counts it
             launch_keyed_partial_rows(rows_params(q, planc, 1, rp.table, rp.table.coltype, rp.perm, &rp.ctl[1], tail), C, stream);
             RowsCopyParams cp;
             memset(&cp, 0, sizeof cp);
@@ -3036,71 +3064,11 @@ void wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
         size_t fin_back = 0;
         rc = finalize_launch(q, planc, stream, S + o_table, tl, fin, flc, fin_launches, fin_back, sb + L.zero);
         cs.kernel_launches += fin_launches;
-        if (!rc && cudaMemcpyAsync(slot.pinned, tail + fl.o_out, p->read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
+        cs.d2h_bytes += read_back;
+        if (!rc && cudaMemcpyAsync(slot.pinned, tail + fl.o_out, read_back, cudaMemcpyDeviceToHost, stream) != cudaSuccess) rc = BYDB_EIO;
         return rc;
     });
-    if (e != cudaSuccess || c.rc || c.err != cudaSuccess || !p->exec) {
-        cudaGetLastError();
-        drop_step(p);
-        p->capturable = false;
-        return;
-    }
-    // a partial step's read-back is sized by the rows present: the replay counts it
-    cs.d2h_bytes = partial && C ? 0 : p->read_back;
-    p->partial_step = partial;
-    p->fl = fl;
-    p->express = false;  // the wide scan has a lane of its own
-    k->values = std::move(w.values);
-    k->n_comp = C;
-    k->pairs_off = partial ? 0 : fl.out_bytes + kZeroPageBytes;
-    k->zero_off = C == 0 ? 0 : partial ? pages - kZeroPageBytes : fl.out_bytes;
-    p->held = plan.parts;
-    p->held_gen = gen;
-}
-
-// the answer of a replayed wide step from its read-back `image`: the finalised rows, or the row image behind the pairs and the zero
-// page (and the bytes the copy kernel brought back); either way each row's (group, key) pair by its composite group's position
-int wide_answer(bydb_prepared_keyed *k, const Plan &, const uint8_t *image, bydb_keyed_result *out, KeyedOwner *owner) {
-    if (k->n_comp == 0) return 0;
-    const int rc = finalize_parse(image, k->pq->fl, true, &out->base);
-    if (rc) return rc;
-    set_row_keys(out, owner, static_cast<ResultOwner *>(out->base.owner)->group_id, image + k->pairs_off, 8, true);
-    return 0;
-}
-int wide_answer(bydb_prepared_keyed *k, const Plan &shape, const uint8_t *image, bydb_keyed_partial_rows *out, KeyedOwner *owner) {
-    if (k->n_comp == 0) return 0;
-    const uint8_t *rows = image + k->zero_off + kZeroPageBytes;
-    const size_t ctl_bytes = keyed_ctl_bytes(shape.fcols.size()), row_bytes = keyed_row_bytes(k->pq->q.n_aggs);
-    out->stats.d2h_bytes += k->zero_off + kZeroPageBytes + ctl_bytes + rows_in(rows, k->n_comp) * row_bytes;
-    const int rc = parse_rows(rows, &k->pq->q, shape, k->n_comp, &out->base);
-    if (rc) return rc;
-    set_row_keys(out, owner, static_cast<PartialRowsOwner *>(out->base.owner)->group_id, image + k->pairs_off, 8, true);
-    return 0;
-}
-
-// One replay, synchronised and parsed: the passes' counters add up and the first pass with a device error decides, as the plain
-// path's pass-by-pass collection has it; then the answer of the step's form (keyed_answer).
-template <class Out>
-int keyed_replay(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
-    bydb_prepared *p = k->pq;
-    Plan shape;
-    int rc = query_shape(&p->q, shape);
-    if (rc) return rc;
-    uint8_t *image = p->slot->pinned + p->host_off;
-    const size_t V = k->wide ? 1 : k->values.size();  // zero pages: one per pass
-    const bool row_image = p->partial_step && (!k->wide || k->n_comp);
-    // a replay that fails to launch cannot report the previous one's status (nor, in a partial step, its control word)
-    memset(image + k->zero_off, 0, V * kZeroPageBytes + (row_image ? keyed_ctl_bytes(shape.fcols.size()) : 0));
-    auto page = [&](size_t v) -> const ZeroPage & { return *reinterpret_cast<const ZeroPage *>(image + k->zero_off + v * kZeroPageBytes); };
-    bydb_stats &stats = keyed_stats(out);
-    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, false, page(0), &stats);
-    for (size_t v = 1; !rc && v < V; ++v) rc = read_zero_page(page(v), false, &stats);
-    if (rc) return rc;
-    KeyedAnswer<Out> answer(ctx, out, k->values);
-    rc = k->wide ? wide_answer(k, shape, image, out, answer.owner) : keyed_answer(k, shape, image, out, answer.owner);
-    if (rc) return rc;
-    answer.done = true;
-    return 0;
+    return capture_finish(p, plan, gen, ok, c);
 }
 
 // bydb_query_prepare_keyed (wide: bydb_query_prepare_keyed_wide): the argument checks of the unprepared call, in its order, then
@@ -3132,24 +3100,30 @@ template <class Out>
 int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
     if (!ctx || !k || !out) return fail(BYDB_EINVAL, "NULL argument");
     memset(out, 0, sizeof *out);
-    const bool partial = std::is_same<Out, bydb_keyed_partial_rows>::value;
+    constexpr bool partial = std::is_same<Out, bydb_keyed_partial_rows>::value;
     bydb_prepared *p = k->pq;
     std::lock_guard<std::mutex> lk(p->mu);
     g_last_dev_err = 0;
     CUDA_TRY(cudaSetDevice(ctx->device));
-    const int rc = prepared_step(ctx, p, partial, [&] {
-        if (k->wide) wide_capture(ctx, k, partial);
-        else keyed_capture(ctx, k, partial);
-        return 0;
-    });
+    int rc = prepared_step(ctx, p, partial, [&] { return k->wide ? wide_capture(ctx, k, partial) : keyed_capture(ctx, k, partial); });
     if (rc) return rc;
-    if (!p->exec && !p->empty_step) return k->wide ? scan_keyed_wide_impl(ctx, &p->q, &k->key, out) : scan_keyed_impl(ctx, &p->q, &k->key, out);
-    if (p->empty_step) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
+    const Step &s = p->step;
+    if (!s.exec && !s.empty) return k->wide ? scan_keyed_wide_impl(ctx, &p->q, &k->key, out) : scan_keyed_impl(ctx, &p->q, &k->key, out);
+    if (s.empty) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
         KeyedAnswer<Out> answer(ctx, out, k->values);
         answer.done = true;
         return 0;
     }
-    return keyed_replay(ctx, k, out);
+    Plan shape;
+    rc = query_shape(&p->q, shape);
+    if (!rc) rc = replay_step(p, s, keyed_ctl_bytes(shape.fcols.size()), &keyed_stats(out));
+    if (rc) return rc;
+    KeyedAnswer<Out> answer(ctx, out, k->values);
+    if constexpr (partial) rc = partial_answer(p, s, shape, out, out->stats);
+    else rc = finalised_answer(p, s, out);
+    if (rc) return rc;
+    answer.done = true;
+    return 0;
 }
 }  // namespace
 
@@ -4065,12 +4039,9 @@ int bydb_scan_agg_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_result *out) {
     CUDA_TRY(cudaSetDevice(ctx->device));
     int rc = prepared_step(ctx, p, false, [&] { return prepared_capture(ctx, p, false); });
     if (rc) return rc;
-    if (!p->exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
-    uint8_t *image = p->slot->pinned + p->zero_image_off;
-    memset(image, 0, kZeroPageBytes);
-    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, *reinterpret_cast<const ZeroPage *>(image), &out->stats);
-    if (rc) return rc;
-    return finalize_parse(p->slot->pinned + p->host_off, p->fl, false, out);
+    if (!p->step.exec) return scan_agg_impl(ctx, &p->q, nullptr, out, 0);
+    rc = replay_step(p, p->step, 0, &out->stats);
+    return rc ? rc : finalised_answer(p, p->step, out);
     });
 }
 
@@ -4109,20 +4080,13 @@ int bydb_scan_partials_prepared(bydb_ctx *ctx, bydb_prepared *p, bydb_partial_ro
     CUDA_TRY(cudaSetDevice(ctx->device));
     int rc = prepared_step(ctx, p, true, [&] { return prepared_capture(ctx, p, true); });
     if (rc) return rc;
-    if (!p->exec) return scan_partials_rows_impl(ctx, &p->q, out, stats);
+    if (!p->step.exec) return scan_partials_rows_impl(ctx, &p->q, out, stats);
     Plan shape;
     rc = query_shape(&p->q, shape);
     if (rc) return rc;
-    const size_t ctl_bytes = keyed_ctl_bytes(shape.fcols.size());
-    uint8_t *image = p->slot->pinned + p->host_off;  // the zero page, then the row image (control word, rows)
-    memset(image, 0, kZeroPageBytes + ctl_bytes);  // a replay that fails to launch cannot report the previous one's status or rows
     bydb_stats local{};
-    rc = replay_graph(p->exec, *p->slot, p->t0, p->t1, p->captured, p->express, *reinterpret_cast<const ZeroPage *>(image), &local);
-    const uint8_t *rows = image + kZeroPageBytes;
-    if (!rc) {
-        local.d2h_bytes += kZeroPageBytes + ctl_bytes + rows_in(rows, shape.tl.G) * keyed_row_bytes(p->q.n_aggs);
-        rc = parse_rows(rows, &p->q, shape, shape.tl.G, out);
-    }
+    rc = replay_step(p, p->step, keyed_ctl_bytes(shape.fcols.size()), &local);
+    if (!rc) rc = partial_answer(p, p->step, shape, out, local);
     if (stats) *stats = local;
     return rc;
     });
@@ -5197,9 +5161,9 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
         lk.unlock();
         return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
     }
-    auto &rg = p->reduce_graphs[root * 2 + static_cast<int>(mb.parity)];
+    Step &rg = p->reduce_graphs[root * 2 + static_cast<int>(mb.parity)];
     // a graph reads its parts through the pointers captured with it (same rule as bydb_scan_agg_prepared)
-    if (rg.exec) (void)check_held_parts(ctx, p->parts, rg.exec, rg.held);  // a missing part fails in make_plan below
+    if (rg.exec) (void)check_held_parts(ctx, p->parts, rg);  // a missing part fails in make_plan below
     if (!rg.exec) {
         Plan plan;
         int rc = make_plan(ctx, &p->q, nullptr, plan);
@@ -5208,14 +5172,13 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
             return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);  // takes part in the collective and reports the failure
         }
         const TableLayout &tl = plan.tl;
-        p->host_off = stage_layout(p->q.n_series, tl.G).stride;
         // the version-dedup precheck synchronises: such queries keep the plain path
         if (parts_overlap(plan.parts, p->q.tmin, p->q.tmax) || tl.total > mb.slot_bytes || es.ensure_pinned(step_pinned_bytes(&p->q, tl.G, tl.G))) {
             p->reduce_capturable = false;
             lk.unlock();
             return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
         }
-        memset(&rg.captured, 0, sizeof rg.captured);
+        rg.image_off = stage_layout(p->q.n_series, tl.G).stride;  // the root's result rows; its zero page lands in the slot's page 0
         cudaStream_t s = es.stream;
         cudaGetLastError();  // a stale error of an earlier call must not be blamed on the capture
         const char *bad_step = nullptr;  // first step of the capture the runtime objected to (BYDB_TRACE prints it)
@@ -5243,7 +5206,7 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
                 step("combine", true);
                 uint32_t fin_launches = 0;
                 size_t read_back = 0;
-                step("finalize", finalize_enqueue(&p->q, plan, es, s, mb.slots0, tl, p->host_off, fin, rg.fl, fin_launches, read_back) == 0);
+                step("finalize", finalize_enqueue(&p->q, plan, es, s, mb.slots0, tl, rg.image_off, fin, rg.fl, fin_launches, read_back) == 0);
                 launch_comm_done_args(mb.done, d_args, s);
                 step("done word", true);
                 step("status read-back",
@@ -5262,13 +5225,14 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
             static const bool trace = getenv("BYDB_TRACE") != nullptr;
             if (trace) fprintf(stderr, "[bydb] prepared collective: capture failed at '%s' (%s); keeping the plain path\n", bad_step ? bad_step : "?", cudaGetErrorString(e));
             cudaGetLastError();
-            if (rg.exec) cudaGraphExecDestroy(rg.exec);
-            rg.exec = nullptr;
+            drop_step(rg);
             p->reduce_capturable = false;  // the plain path from here on
             lk.unlock();
             return scan_reduce_impl(ctx, &p->q, nullptr, 0, 0, root, out);
         }
         rg.held = plan.parts;
+        rg.max_rows = rg.fl.cap;
+        rg.carried_status = true;
     }
     // ---- replay
     cm.epoch = epoch;
@@ -5284,7 +5248,7 @@ int bydb_scan_reduce_prepared(bydb_ctx *ctx, bydb_prepared *p, int32_t root, byd
     if (cm.rank != root) return 0;
     const int prc = peer_failure(reinterpret_cast<const unsigned long long *>(h_back + 8), cm.nranks, epoch, " failed before its scan");
     if (prc) return prc;
-    return finalize_parse(es.pinned + p->host_off, rg.fl, true, out);
+    return finalised_answer(p, rg, out);
     });
 }
 
