@@ -492,8 +492,8 @@ int bydb_scan_partials_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb
  *     up to 256-byte alignment of each region,
  *       12 * NS + K * (12 * S + 68 * cap) + 12 * S + 8 * cap + 8 * NB                                     discovery
  *     + then bydb_scan_agg_keyed_wide's scan, order, composite table and finalisation terms for this R and C.
- * Free the answers with bydb_keys_result_free / bydb_keys_partial_rows_free.  The multi-GPU form is bydb_scan_reduce_keys_wide;
- * there is no prepared or host-image form. */
+ * Free the answers with bydb_keys_result_free / bydb_keys_partial_rows_free.  The prepared form is bydb_query_prepare_keys_wide,
+ * the multi-GPU form bydb_scan_reduce_keys_wide; there is no host-image form. */
 typedef struct {
     uint32_t n_keys;              /* 2..4 stored GroupBy tags, in the request's GroupBy order                               */
     uint32_t max_values;          /* distinct key TUPLES accepted over the query; 0 = 64, at most 65,536                    */
@@ -562,6 +562,41 @@ void bydb_keys_partial_rows_free(bydb_ctx *ctx, bydb_keys_partial_rows *r);
  *       + (finalised) the finalisation's scratch over C groups + 256 + 8*C,  or  (partial) 8*C + (8 + 8*F) + C*(8 + 16*A)
  *     (C = 0: no finalisation or row image).  The handle's page-locked staging holds the read-back. */
 int bydb_query_prepare_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out);
+
+/* Prepared group-by on a TUPLE of 2..4 stored tags: bydb_scan_agg_keys_wide for a query executed many times (a dashboard panel or an
+ * alert rule grouped by endpoint and status code).  The handle is a bydb_prepared_keyed that bydb_scan_agg_keys_prepared,
+ * bydb_scan_partials_keys_prepared and bydb_query_release_keyed take; the one-key executors (bydb_scan_agg_keyed_prepared,
+ * bydb_scan_partials_keyed_prepared) refuse it with BYDB_EINVAL, and the tuple executors refuse a one-key handle with BYDB_EINVAL, the
+ * message naming the executor to use.  Every execution answers what bydb_scan_agg_keys_wide / bydb_scan_partials_keys_wide answer at
+ * that moment for the handle's query and keys: code and device-error text, rows in the same order, each row's series group and each
+ * tag's key bytes, values bit for bit, n_tuples and each tag's value count (key_base[t+1] - key_base[t]), and the counters
+ * (rows_scanned, rows_matched, page_bytes, blocks_scanned).  The key tables found at the capture answer every replay; their order is
+ * not part of the contract, as for the unprepared call.
+ *   - Arguments: checked at prepare as bydb_scan_agg_keys_wide checks them, in its order and with its codes (n_keys outside 2..4, the
+ *     same (family, tag) twice, a key whose own max_values is not 0, max_values above 65,536, each tag's type, up to 8 predicates);
+ *     the query and the keys are copied, strings included.  A refusal that depends on the data (more tuples than max_values:
+ *     BYDB_ENOMEM; a block holding more than 256 tuples, a plain string page, a 65-byte value, an int64 column with more than 256 values
+ *     in a block, parts that overlap in time: BYDB_ENOTSUP) comes at every execution as the unprepared call gives it, and the handle
+ *     keeps the unprepared path for good.
+ *   - Schedule: the first execution runs the unprepared path; the second runs the discovery, scan and order once with the key list
+ *     to learn each tag's table, the tuples' codes, R and C, captures the step -- the reset kernel, the tuple scan, the order, the fold
+ *     into C composite groups (series group, tuple), the form's tail and its read-back -- as ONE CUDA graph, and answers from its first
+ *     replay; later executions replay it.  T = 0 (no block selected) needs no graph: no rows, no tuples, zero stats.  C = 0 captures
+ *     only a copy of the zero page.  Part lifecycle (a handle that stops naming its captured part drops the step and captures again;
+ *     one that names no part gives BYDB_ENOENT), one step per handle of the form last asked for, one execution at a time per handle:
+ *     as the keyed prepared forms above.
+ *   - Stats of a replay: h2d_bytes = 0; scan_kernel_ms = 0 and device_ms = the whole graph; kernel_launches and d2h_bytes as for
+ *     bydb_query_prepare_keyed_wide's replay, with C counting (series group, tuple) groups: a replay launches the unprepared call's
+ *     kernels, except that discovery's (K + 1) * ((NB > 0) + 1) + 3 launches give way to the reset kernel.
+ *   - Device memory a captured step keeps until bydb_query_release_keyed, or until the step is dropped; it is not charged to
+ *     hbm_budget_bytes.  With K tags, nt = K + 1 tables, cap = max_values, S = pow2(max(2*cap, 1024)) and NBp = NB rounded up to a
+ *     multiple of 1,024 (at least 1,024), each term rounded up to 256 B,
+ *       12*NS + nt*12*S + 32*nt + K*68*cap + 8*cap + 4*NBp + 4*NB + 4*NBp/1024                   discovery's outputs (a copy)
+ *     then the table of C groups, perm, scan and order and the tail of bydb_query_prepare_keyed_wide's step.  The handle's page-locked
+ *     staging holds the read-back. */
+int bydb_query_prepare_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, bydb_prepared_keyed **out);
+int bydb_scan_agg_keys_prepared(bydb_ctx *ctx, bydb_prepared_keyed *pq, bydb_keys_result *out);
+int bydb_scan_partials_keys_prepared(bydb_ctx *ctx, bydb_prepared_keyed *pq, bydb_keys_partial_rows *out);
 
 /* Prepared map-phase answers: what a data node answers, refresh after refresh, for a query the liaison pushes down with
  * agg_return_partial (a dashboard panel or an alert rule in a cluster).  The handles are those of the finalised forms above.

@@ -17,9 +17,11 @@
 // buildAggOutputSchema's (aggregation.go:402-418): the projected tag columns in schema order, then one RoleField column per
 // AggSpec typed by aggOutputType (COUNT -> int64, otherwise the input field's type); group rows come in first-appearance
 // order of the scan (reversed for an order-by DESC request), non-key projected tags carry the first-seen value.
-// A GroupBy key column with per-series values (ScanSpec::SeriesTags: entity / indexed tags) is densified per series; at most
-// one key column may be a stored tag (a tag column absent from SeriesTags), and then the operator calls bydb_scan_agg_keyed, which adds
-// the row's value of that tag to the group.  Such a key takes the ascending series order only (no OrderDesc).
+// A GroupBy key column with per-series values (ScanSpec::SeriesTags: entity / indexed tags) is densified per series; a key column
+// that is a stored tag (a tag column absent from SeriesTags) makes the operator call bydb_scan_agg_keyed(_wide), which adds the row's
+// value of that tag to the group.  With MaxKeyValues above 256, two to four stored key columns go to bydb_scan_agg_keys_wide as a
+// tuple, in GroupBy order; at 256 or below only one may be a stored tag.  Stored keys take the ascending series order only (no
+// OrderDesc).
 // tests/native/operator_test.cc drives it; the Python mirror (skywalking-banyandb_b200/scan_operator.py) follows the same code.
 #pragma once
 
@@ -189,11 +191,13 @@ class GPUScanAgg final : public PullOperator {
             const ColumnDef &cd = in_.Columns[static_cast<size_t>(ti)];
             Column col;
             col.Type = cd.Type;
-            if (ti == stored_key_) {
+            const auto sk = std::find(stored_keys_.begin(), stored_keys_.end(), ti);
+            if (sk != stored_keys_.end()) {
+                const size_t t = static_cast<size_t>(sk - stored_keys_.begin());
                 for (size_t r = lo; r < hi; ++r) {  // the row's key bytes (groupby.go:226-254); a nil cell came back as 0 / ""
-                    const int32_t k = kres_.key_id[r];
-                    const uint8_t *kb = kres_.key_bytes + kres_.key_off[k];
-                    const size_t klen = kres_.key_off[k + 1] - kres_.key_off[k];
+                    const uint8_t *kb = nullptr;
+                    size_t klen = 0;
+                    key_entry(r, t, kb, klen);
                     if (cd.Type == ColumnType::ColumnTypeInt64) {
                         uint64_t u = 0;
                         for (size_t i = 0; i < klen && i < 8; ++i) u |= static_cast<uint64_t>(kb[i]) << (8 * i);
@@ -237,7 +241,8 @@ class GPUScanAgg final : public PullOperator {
 
     Status Close() override {  // idempotent; releases the result exactly once
         if (have_result_) {
-            if (stored_key_ >= 0) bydb_keyed_result_free(ctx_, &kres_);
+            if (stored_keys_.size() > 1) bydb_keys_result_free(ctx_, &tres_);
+            else if (stored_keys_.size() == 1) bydb_keyed_result_free(ctx_, &kres_);
             else bydb_result_free(ctx_, &res_);
             have_result_ = false;
         }
@@ -249,7 +254,15 @@ class GPUScanAgg final : public PullOperator {
 
   private:
     Status fail(int code, std::string msg) { return Error{code, std::move(msg)}; }
-    const bydb_result &result() const { return stored_key_ >= 0 ? kres_.base : res_; }
+    const bydb_result &result() const { return stored_keys_.size() > 1 ? tres_.base : stored_keys_.size() == 1 ? kres_.base : res_; }
+    // stored key t of row r: one key's entry key_id[r], or a tuple's entry key_id[r * n_tags + t]
+    void key_entry(size_t r, size_t t, const uint8_t *&bytes, size_t &len) const {
+        const bool tuple = stored_keys_.size() > 1;
+        const int32_t e = tuple ? tres_.key_id[r * tres_.n_tags + t] : kres_.key_id[r];
+        const uint32_t *off = tuple ? tres_.key_off : kres_.key_off;
+        bytes = (tuple ? tres_.key_bytes : kres_.key_bytes) + off[e];
+        len = off[e + 1] - off[e];
+    }
 
     Status run() {
         ran_ = true;
@@ -258,23 +271,27 @@ class GPUScanAgg final : public PullOperator {
         const size_t ns = scan_.SeriesIDs.size();
         // group key per series = tuple of the key columns' values; dense ids in first-appearance order of the scan
         // (aggregation.go:211-213); an order-by DESC request visits the series list backwards
-        // A tag key column without per-series values is a stored tag: bydb_scan_agg_keyed adds its row value to the group.
-        // Any other key column (a field) still needs per-series values.
+        // A tag key column without per-series values is a stored tag: bydb_scan_agg_keyed adds its row value to the group, and
+        // above 256 values bydb_scan_agg_keys_wide adds the tuple of two to four of them.  Any other key column (a field) still
+        // needs per-series values.
         std::vector<const std::vector<std::string> *> keyvals;
-        stored_key_ = -1;
+        stored_keys_.clear();
         for (int ki : keys_) {
             const ColumnDef &cd = in_.Columns[static_cast<size_t>(ki)];
             const auto it = scan_.SeriesTags.find({cd.TagFamily, cd.Name});
             if (it == scan_.SeriesTags.end() && cd.Role == ColumnRole::RoleTag) {
-                if (stored_key_ >= 0) return fail(BYDB_ENOTSUP, "GroupBy key " + cd.TagFamily + "/" + cd.Name + ": at most one stored-tag key per query");
-                stored_key_ = ki;
+                if (!stored_keys_.empty() && scan_.MaxKeyValues <= 256)
+                    return fail(BYDB_ENOTSUP, "GroupBy key " + cd.TagFamily + "/" + cd.Name + ": at most one stored-tag key per query");
+                if (stored_keys_.size() == kMaxStoredKeys)
+                    return fail(BYDB_ENOTSUP, "GroupBy key " + cd.TagFamily + "/" + cd.Name + ": at most four stored-tag keys per query");
+                stored_keys_.push_back(ki);
                 continue;
             }
             if (it == scan_.SeriesTags.end() || it->second.size() != ns)
                 return fail(BYDB_EINVAL, "GroupBy key " + cd.TagFamily + "/" + cd.Name + " needs one value per series (entity / indexed tag)");
             keyvals.push_back(&it->second);
         }
-        if (stored_key_ >= 0 && scan_.OrderDesc) return fail(BYDB_ENOTSUP, "a stored-tag GroupBy key takes the ascending series order only (OrderDesc)");
+        if (!stored_keys_.empty() && scan_.OrderDesc) return fail(BYDB_ENOTSUP, "a stored-tag GroupBy key takes the ascending series order only (OrderDesc)");
         std::map<std::vector<std::string>, int32_t> group_of;
         std::vector<int32_t> gids(ns, 0);
         group_first_series_.clear();
@@ -338,17 +355,25 @@ class GPUScanAgg final : public PullOperator {
         q.top_agg = top_ ? top_->AggIndex : 0;
         q.top_desc = top_ ? (top_->Desc ? 1 : 0) : 1;
         int rc;
-        if (stored_key_ < 0) {
-            rc = bydb_scan_agg(ctx_, &q, &res_);
-        } else {
-            const ColumnDef &cd = in_.Columns[static_cast<size_t>(stored_key_)];
+        const bool tuple = stored_keys_.size() > 1;  // MaxKeyValues then counts the distinct tuples; each tag's own max_values is 0
+        std::vector<bydb_group_key> ckeys;
+        for (int ki : stored_keys_) {
+            const ColumnDef &cd = in_.Columns[static_cast<size_t>(ki)];
             bydb_group_key key{};
             key.family = cd.TagFamily.c_str();
             key.tag = cd.Name.c_str();
-            key.max_values = scan_.MaxKeyValues;
+            key.max_values = tuple ? 0 : scan_.MaxKeyValues;
             key.value_type = cd.Type == ColumnType::ColumnTypeInt64 ? BYDB_VT_INT64 : 0;
+            ckeys.push_back(key);
+        }
+        if (ckeys.empty()) {
+            rc = bydb_scan_agg(ctx_, &q, &res_);
+        } else if (!tuple) {
             // above the per-value passes' 256 values, the one-pass form (which answers the same rows)
-            rc = scan_.MaxKeyValues > 256 ? bydb_scan_agg_keyed_wide(ctx_, &q, &key, &kres_) : bydb_scan_agg_keyed(ctx_, &q, &key, &kres_);
+            rc = scan_.MaxKeyValues > 256 ? bydb_scan_agg_keyed_wide(ctx_, &q, &ckeys[0], &kres_) : bydb_scan_agg_keyed(ctx_, &q, &ckeys[0], &kres_);
+        } else {
+            bydb_group_keys keys{static_cast<uint32_t>(ckeys.size()), scan_.MaxKeyValues, ckeys.data()};
+            rc = bydb_scan_agg_keys_wide(ctx_, &q, &keys, &tres_);
         }
         if (rc != 0) return fail(rc, bydb_last_error() ? bydb_last_error() : "bydb_scan_agg failed");
         have_result_ = true;
@@ -374,8 +399,10 @@ class GPUScanAgg final : public PullOperator {
     std::optional<TopSpec> top_;
     std::optional<LimitSpec> limit_;
     bydb_result res_{};
-    bydb_keyed_result kres_{};  // the result when a GroupBy key is a stored tag
-    int stored_key_ = -1;       // input column of that key, -1 = none
+    static constexpr size_t kMaxStoredKeys = 4;  // the tags of a bydb_group_keys tuple
+    bydb_keyed_result kres_{};  // the result when one GroupBy key is a stored tag
+    bydb_keys_result tres_{};   // the result when two to four are
+    std::vector<int> stored_keys_;  // input columns of those keys, in GroupBy order
     bydb_stats stats_{};
     std::vector<int> group_first_series_;
     size_t cursor_ = 0, row_end_ = 0;

@@ -132,6 +132,7 @@ EXPORTS = ["bydb_init", "bydb_shutdown", "bydb_part_register", "bydb_part_releas
            "bydb_keyed_wide_reduce_slot_bytes", "bydb_scan_reduce_keyed_wide", "bydb_scan_reduce_keyed_wide_partials",
            "bydb_query_prepare_keyed_wide", "bydb_scan_agg_keys_wide", "bydb_scan_partials_keys_wide", "bydb_keys_result_free",
            "bydb_keys_partial_rows_free", "bydb_keys_wide_reduce_slot_bytes", "bydb_scan_reduce_keys_wide", "bydb_scan_reduce_keys_wide_partials",
+           "bydb_query_prepare_keys_wide", "bydb_scan_agg_keys_prepared", "bydb_scan_partials_keys_prepared",
            "bydb_encode_pages", "bydb_encoded_pages_free", "bydb_last_error", "bydb_version"]
 
 _lib = None
@@ -216,6 +217,9 @@ def load_library():
     L.bydb_scan_reduce_keys_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKeys), C.c_int32, C.POINTER(_KeysResult)]
     L.bydb_scan_reduce_keys_wide_partials.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKeys), C.c_int32,
                                                       C.POINTER(_KeysPartialRows)]
+    L.bydb_query_prepare_keys_wide.argtypes = [C.c_void_p, C.POINTER(_Query), C.POINTER(_GroupKeys), C.POINTER(C.c_void_p)]
+    L.bydb_scan_agg_keys_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_KeysResult)]
+    L.bydb_scan_partials_keys_prepared.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_KeysPartialRows)]
     _lib = L
     return L
 
@@ -476,6 +480,30 @@ class KeyedGraphQuery:
             self._h = None
 
 
+class KeysGraphQuery:
+    """A group-by on a tuple of stored tags held by the library (bydb_query_prepare_keys_wide): its scan, order, fold and answer are
+    replayed as one CUDA graph from its second run on.  run() / run_partials() give what Context.scan_agg_keys_wide /
+    scan_partials_keys_wide give at that moment."""
+
+    def __init__(self, ctx: "Context", handle, q: Query):
+        self._ctx, self._h, self._q = ctx, handle, q
+
+    def run(self) -> Result:
+        r = _KeysResult()
+        _check(self._ctx._L.bydb_scan_agg_keys_prepared(self._ctx._h, self._h, C.byref(r)))
+        return self._ctx._read_keys(self._q, r)
+
+    def run_partials(self) -> Dict[str, object]:
+        r = _KeysPartialRows()
+        _check(self._ctx._L.bydb_scan_partials_keys_prepared(self._ctx._h, self._h, C.byref(r)))
+        return self._ctx._read_keys_partials(self._q, r)
+
+    def release(self):
+        if self._h:
+            self._ctx._L.bydb_query_release_keyed(self._ctx._h, self._h)
+            self._h = None
+
+
 def keyed_reduce_slot_bytes(q: Query, family: str, tag: str, max_values: int = 0, value_type: int = 0) -> int:
     """bydb_keyed_reduce_slot_bytes (host only): the mailbox slot a rank of a keyed collective needs at max_values key values."""
     keep: list = []
@@ -664,6 +692,17 @@ class Context:
         r = _KeysResult()
         _check(self._L.bydb_scan_agg_keys_wide(self._h, C.byref(cq), C.byref(gks), C.byref(r)))
         return self._read_keys(q, r)
+
+    def prepare_keys_wide(self, q: Query, keys: Sequence[tuple], max_values: int = 0) -> "KeysGraphQuery":
+        """The prepared form of scan_agg_keys_wide (bydb_query_prepare_keys_wide): argument errors are raised here, as
+        scan_agg_keys_wide raises them; the handle's run() / run_partials() answer as scan_agg_keys_wide / scan_partials_keys_wide
+        do at that moment."""
+        keep: list = []
+        cq = _mk_query(q, keep)
+        gks = _group_keys(keys, max_values, keep)
+        h = C.c_void_p()
+        _check(self._L.bydb_query_prepare_keys_wide(self._h, C.byref(cq), C.byref(gks), C.byref(h)))
+        return KeysGraphQuery(self, h, q)
 
     def _read_keys(self, q: Query, r: "_KeysResult") -> Result:
         try:

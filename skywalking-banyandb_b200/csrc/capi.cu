@@ -2661,11 +2661,11 @@ void wide_key_tables(Out *out, KeyedOwner *owner, const WidePass &w) {
     set_key_table(out, owner, w.values);
 }
 template <class Out>
-void tuple_key_tables(Out *out, KeyedOwner *owner, const WidePass &w) {
+void tuple_key_tables(Out *out, KeyedOwner *owner, const std::vector<KeyValues> &tag_values, const std::vector<uint64_t> &codes) {
     owner->key_base.assign(1, 0);
     owner->key_off.assign(1, 0);
     owner->key_bytes.clear();
-    for (const KeyValues &vals : w.tag_values) {
+    for (const KeyValues &vals : tag_values) {
         for (const auto &v : vals) {
             owner->key_bytes.insert(owner->key_bytes.end(), v.begin(), v.end());
             owner->key_off.push_back(static_cast<uint32_t>(owner->key_bytes.size()));
@@ -2673,31 +2673,31 @@ void tuple_key_tables(Out *out, KeyedOwner *owner, const WidePass &w) {
         owner->key_base.push_back(owner->key_base.back() + static_cast<int32_t>(vals.size()));
     }
     if (owner->key_bytes.empty()) owner->key_bytes.push_back(0);
-    out->n_tags = static_cast<uint32_t>(w.tag_values.size());
-    out->n_tuples = static_cast<int32_t>(w.codes.size());
+    out->n_tags = static_cast<uint32_t>(tag_values.size());
+    out->n_tuples = static_cast<int32_t>(codes.size());
     out->key_base = owner->key_base.data();
     out->key_off = owner->key_off.data();
     out->key_bytes = owner->key_bytes.data();
 }
-void wide_key_tables(bydb_keys_result *out, KeyedOwner *owner, const WidePass &w) { tuple_key_tables(out, owner, w); }
-void wide_key_tables(bydb_keys_partial_rows *out, KeyedOwner *owner, const WidePass &w) { tuple_key_tables(out, owner, w); }
+void wide_key_tables(bydb_keys_result *out, KeyedOwner *owner, const WidePass &w) { tuple_key_tables(out, owner, w.tag_values, w.codes); }
+void wide_key_tables(bydb_keys_partial_rows *out, KeyedOwner *owner, const WidePass &w) { tuple_key_tables(out, owner, w.tag_values, w.codes); }
 
 // a tuple key's rows carry the tuple id (set_row_keys): each becomes its tags' entries, key_id[r * n_tags + t]
 template <class Out>
 void wide_row_tuples(Out *, KeyedOwner *, const WidePass &) {}
 template <class Out>
-void tuple_row_entries(Out *out, KeyedOwner *owner, const WidePass &w) {
-    const size_t K = w.tag_values.size(), n = owner->key_id.size();
+void tuple_row_entries(Out *out, KeyedOwner *owner, const std::vector<KeyValues> &tag_values, const std::vector<uint64_t> &codes) {
+    const size_t K = tag_values.size(), n = owner->key_id.size();
     std::vector<int32_t> ids(n * K);
     for (size_t r = 0; r < n; ++r) {
-        const uint64_t code = w.codes[static_cast<size_t>(owner->key_id[r])];
+        const uint64_t code = codes[static_cast<size_t>(owner->key_id[r])];
         for (size_t t = 0; t < K; ++t) ids[r * K + t] = owner->key_base[t] + static_cast<int32_t>((code >> (16 * t)) & 0xffffu);
     }
     owner->key_id.swap(ids);
     out->key_id = owner->key_id.data();
 }
-void wide_row_tuples(bydb_keys_result *out, KeyedOwner *owner, const WidePass &w) { tuple_row_entries(out, owner, w); }
-void wide_row_tuples(bydb_keys_partial_rows *out, KeyedOwner *owner, const WidePass &w) { tuple_row_entries(out, owner, w); }
+void wide_row_tuples(bydb_keys_result *out, KeyedOwner *owner, const WidePass &w) { tuple_row_entries(out, owner, w.tag_values, w.codes); }
+void wide_row_tuples(bydb_keys_partial_rows *out, KeyedOwner *owner, const WidePass &w) { tuple_row_entries(out, owner, w.tag_values, w.codes); }
 
 // the key list of a wide call: a bydb_group_key, or the tags of a bydb_group_keys
 const bydb_group_key *key_list(const bydb_group_key *key) { return key; }
@@ -2781,18 +2781,20 @@ int replay_step(bydb_prepared *p, const Step &s, size_t ctl_bytes, bydb_stats *s
 // the rows of an answer: a plain answer is its rows, a keyed one holds them in `base`
 bydb_result *rows_of(bydb_result *out) { return out; }
 bydb_result *rows_of(bydb_keyed_result *out) { return &out->base; }
+bydb_result *rows_of(bydb_keys_result *out) { return &out->base; }
 bydb_partial_rows *rows_of(bydb_partial_rows *out) { return out; }
 bydb_partial_rows *rows_of(bydb_keyed_partial_rows *out) { return &out->base; }
+bydb_partial_rows *rows_of(bydb_keys_partial_rows *out) { return &out->base; }
 
 // The answer of a replayed finalised step from its image: the result rows, then a keyed answer's (group, key) pairs (its owner and
-// key table are set up already)
+// key table are set up already; a tuple answer's pairs carry the tuple id)
 template <class Out>
 int finalised_answer(const bydb_prepared *p, const Step &s, Out *out) {
     if (!s.max_rows) return 0;
     const uint8_t *image = p->slot->pinned + s.image_off;
     bydb_result *r = rows_of(out);
     const int rc = finalize_parse(image + s.rows_off, s.fl, s.carried_status, r);
-    if constexpr (std::is_same<Out, bydb_keyed_result>::value)
+    if constexpr (!std::is_same<Out, bydb_result>::value)
         if (!rc)
             set_row_keys(out, static_cast<KeyedOwner *>(out->owner), static_cast<ResultOwner *>(r->owner)->group_id, image + s.pairs_off, s.pairs_stride,
                          s.by_position);
@@ -2808,7 +2810,7 @@ int partial_answer(const bydb_prepared *p, const Step &s, const Plan &shape, Out
     stats.d2h_bytes += s.rows_off + keyed_ctl_bytes(shape.fcols.size()) + rows_in(rows, s.max_rows) * keyed_row_bytes(p->q.n_aggs);
     bydb_partial_rows *r = rows_of(out);
     const int rc = parse_rows(rows, &p->q, shape, s.max_rows, r);
-    if constexpr (std::is_same<Out, bydb_keyed_partial_rows>::value)
+    if constexpr (!std::is_same<Out, bydb_partial_rows>::value)
         if (!rc)
             set_row_keys(out, static_cast<KeyedOwner *>(out->owner), static_cast<PartialRowsOwner *>(r->owner)->group_id, image + s.pairs_off,
                          s.pairs_stride, s.by_position);
@@ -2825,15 +2827,23 @@ int partial_answer(const bydb_prepared *p, const Step &s, const Plan &shape, Out
 // ------------------------------------------------------------------------------------------------
 struct bydb_prepared_keyed {
     bydb_prepared *pq = nullptr;   // the query's deep copy, its slot, events and captured step
-    std::string family, tag;       // the key's strings: key.family / key.tag point here
-    bydb_group_key key{};
-    uint32_t cap = 0;              // distinct values accepted (check_group_key)
-    KeyValues values;              // found when the step was captured: the key table of every replay
-    bool wide = false;             // bydb_query_prepare_keyed_wide: one scan pass (wide_capture), not one per value
+    std::string family[kMaxKeyTags], tag[kMaxKeyTags];  // the keys' strings: key[t].family / key[t].tag point here
+    bydb_group_key key[kMaxKeyTags]{};  // the key, or a tuple key's tags in GroupBy order
+    bydb_group_keys keys{};        // a tuple key (bydb_query_prepare_keys_wide): n_keys 2..4, keys = key; else n_keys = 0
+    uint32_t cap = 0;              // distinct values (a tuple key: tuples) accepted (check_group_key)
+    // found when the step was captured, the key tables of every replay: the key's values, or each tag's values and each tuple's code
+    KeyValues values;
+    std::vector<KeyValues> tag_values;
+    std::vector<uint64_t> codes;
+    bool wide = false;             // bydb_query_prepare_keyed_wide / _keys_wide: one scan pass (wide_capture), not one per value
     ~bydb_prepared_keyed() { prepared_destroy(pq); }
 };
 
 namespace {
+// the key list of a prepared handle: its key, or its tuple key's tags
+const bydb_group_key *key_list(const bydb_prepared_keyed *k) { return k->key; }
+uint32_t key_count(const bydb_prepared_keyed *k) { return k->keys.n_keys ? k->keys.n_keys : 1; }
+
 // Discovers the key values and captures the keyed step, in a step state of its own:
 //   composite table | permuted table | the passes' column types | Kts | Krow | the order's slots, first_series, perm, n_present |
 //   one scan scratch (scan_layout, the passes run one after another) | finalisation over V x G groups, then the rows' (group, key)
@@ -2852,7 +2862,7 @@ int keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     ExecSlot &slot = *p->slot;
     cudaStream_t stream = slot.stream;
     bydb_stats discovery{};
-    if (discover_keys(ctx, q, &k->key, k->cap, plan, slot, &discovery, k->values)) return capture_finish(p, plan, gen, false);
+    if (discover_keys(ctx, q, k->key, k->cap, plan, slot, &discovery, k->values)) return capture_finish(p, plan, gen, false);
     const size_t V = k->values.size(), F = plan.fcols.size(), NS = q->n_series, G = static_cast<size_t>(plan.n_groups), GP = G * V;
     if (V == 0) {
         s.empty = true;
@@ -2905,7 +2915,7 @@ int keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
         Scratch scan, kb, fin;
         scan.view(S + o_scan, sl.total);
         fin.view(fin_base, fl.total + b_pairs + b_zero);
-        int rc = run_keyed_passes(ctx, q, &k->key, plan, slot, k->values, tlc, S + o_src, ct, kts, krow, nullptr, &cs, &scan, zero_pages);
+        int rc = run_keyed_passes(ctx, q, k->key, plan, slot, k->values, tlc, S + o_src, ct, kts, krow, nullptr, &cs, &scan, zero_pages);
         KeyOrderParams res, ko;
         memset(&res, 0, sizeof res);
         res.order = reinterpret_cast<const int32_t *>(S + o_scan + sl.off_sids + st.off_order);
@@ -2950,10 +2960,10 @@ int keyed_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     return capture_finish(p, plan, gen, ok, c);
 }
 
-// Captures the wide keyed step.  Outside the graph, once: the plain path's discovery, scan and order (wide_pass) find the key
-// table, R and C -- functions of the parts the handles name and of the fixed query, so properties of the capture.  Then one step
-// state, laid out as
-//   discovery's scratch, copied from the eager run (value table, slot ids, ranks, first records, series ids and groups) |
+// Captures the wide keyed step, of one key or a tuple key.  Outside the graph, once: the plain path's discovery, scan and order
+// (wide_pass) find the key table (a tuple key: each tag's table and the tuples' codes), R and C -- functions of the parts the
+// handles name and of the fixed query, so properties of the capture.  Then one step state, laid out as
+//   discovery's scratch, copied from the eager run (value tables, slot ids, ranks, first records, series ids and groups) |
 //   the table of the C composite groups | perm | (partial) their (group, key) pairs | the scan and order's scratch, zero page first |
 //   the tail: the finalisation over C groups with the zero page gathered behind it and the pairs behind that, or the row image,
 // and the graph: keyed_step_reset_kernel (zero page, composite table, ctl; comp_min) -> wide_scan_order -> wide_fold_kernel -> the
@@ -2971,8 +2981,10 @@ int wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     cudaStream_t stream = slot.stream;
     bydb_stats eager{};
     WidePass w;
-    if (wide_pass(ctx, q, &k->key, 1, k->cap, plan, slot, eager, w)) return capture_finish(p, plan, gen, false);
+    if (wide_pass(ctx, q, key_list(k), key_count(k), k->cap, plan, slot, eager, w)) return capture_finish(p, plan, gen, false);
     k->values = std::move(w.values);
+    k->tag_values = std::move(w.tag_values);
+    k->codes = std::move(w.codes);
     if (w.R == 0) {
         s.empty = true;
         return capture_finish(p, plan, gen, true);
@@ -3001,7 +3013,7 @@ int wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     s.carried_status = true;
     uint8_t *h_dst = nullptr;
     bool ok = step_memory(p, read_back, carve.o, nullptr, 0, partial ? &h_dst : nullptr);
-    if (ok) {  // discovery's scratch into the state, and its device pointers moved to the copy
+    if (ok) {  // discovery's scratch into the state, and every device pointer into it moved to the copy
         uint8_t *S = s.step_state;
         ok = cudaMemcpyAsync(S + o_disc, w.ka.base, w.disc_bytes, cudaMemcpyDeviceToDevice, stream) == cudaSuccess &&
              cudaStreamSynchronize(stream) == cudaSuccess;
@@ -3009,11 +3021,19 @@ int wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
         KeyParams &kp = w.wk.k;
         kp.q_sids = moved(kp.q_sids);
         kp.slots = moved(kp.slots);
+        kp.count = moved(kp.count);
+        kp.err = moved(kp.err);
         kp.zero = moved(kp.zero);
+        kp.vals = moved(kp.vals);
+        kp.lens = moved(kp.lens);
         w.wk.slot_id = moved(w.wk.slot_id);
         w.wk.rank = moved(w.wk.rank);
         w.wk.n_by_rank = moved(w.wk.n_by_rank);
         w.series_group = moved(w.series_group);
+        for (uint32_t t = 0; t < w.tags.n_tags; ++t) {  // a tuple key: the tags' value tables, which the scan reads too
+            w.tags.tag[t].slots = moved(w.tags.tag[t].slots);
+            w.tags.tag[t].slot_id = moved(w.tags.tag[t].slot_id);
+        }
     }
     bydb_stats &cs = s.captured;
     GraphCapture c;
@@ -3071,9 +3091,10 @@ int wide_capture(bydb_ctx *ctx, bydb_prepared_keyed *k, bool partial) {
     return capture_finish(p, plan, gen, ok, c);
 }
 
-// bydb_query_prepare_keyed (wide: bydb_query_prepare_keyed_wide): the argument checks of the unprepared call, in its order, then
-// the handle with its copies of the query and the key
-int prepare_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bool wide, bydb_prepared_keyed **out) {
+// bydb_query_prepare_keyed (wide: bydb_query_prepare_keyed_wide; Key = bydb_group_keys: bydb_query_prepare_keys_wide): the argument
+// checks of the unprepared call, in its order, then the handle with its copies of the query and the key(s)
+template <class Key>
+int prepare_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const Key *key, bool wide, bydb_prepared_keyed **out) {
     if (!ctx || !out) return fail(BYDB_EINVAL, "ctx/out is NULL");
     *out = nullptr;
     int rc = validate_query(q, true);
@@ -3084,23 +3105,35 @@ int prepare_keyed_impl(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key 
     std::unique_ptr<bydb_prepared_keyed> k(new bydb_prepared_keyed());
     rc = bydb_query_prepare(ctx, q, &k->pq);
     if (rc) return rc;
-    k->family = key->family;
-    k->tag = key->tag;
-    k->key = *key;
-    k->key.family = k->family.c_str();
-    k->key.tag = k->tag.c_str();
+    for (uint32_t t = 0; t < key_count(key); ++t) {
+        const bydb_group_key &kt = key_list(key)[t];
+        k->family[t] = kt.family;
+        k->tag[t] = kt.tag;
+        k->key[t] = kt;
+        k->key[t].family = k->family[t].c_str();
+        k->key[t].tag = k->tag[t].c_str();
+    }
+    if constexpr (std::is_same<Key, bydb_group_keys>::value) {
+        k->keys = *key;
+        k->keys.keys = k->key;
+    }
     k->cap = cap;
     k->wide = wide;
     *out = k.release();
     return 0;
 }
 
-// bydb_scan_agg_keyed_prepared and bydb_scan_partials_keyed_prepared: one captured step per handle, of the form last asked for
+// bydb_scan_agg_keyed_prepared / bydb_scan_partials_keyed_prepared on a one-key handle, bydb_scan_agg_keys_prepared /
+// bydb_scan_partials_keys_prepared on a tuple handle: one captured step per handle, of the form last asked for
 template <class Out>
 int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
     if (!ctx || !k || !out) return fail(BYDB_EINVAL, "NULL argument");
     memset(out, 0, sizeof *out);
-    constexpr bool partial = std::is_same<Out, bydb_keyed_partial_rows>::value;
+    constexpr bool tuple = std::is_same<Out, bydb_keys_result>::value || std::is_same<Out, bydb_keys_partial_rows>::value;
+    constexpr bool partial = std::is_same<Out, bydb_keyed_partial_rows>::value || std::is_same<Out, bydb_keys_partial_rows>::value;
+    if (tuple != (k->keys.n_keys > 0))
+        return fail(BYDB_EINVAL, tuple ? (partial ? "a one-key handle: use bydb_scan_partials_keyed_prepared" : "a one-key handle: use bydb_scan_agg_keyed_prepared")
+                                       : (partial ? "a tuple-key handle: use bydb_scan_partials_keys_prepared" : "a tuple-key handle: use bydb_scan_agg_keys_prepared"));
     bydb_prepared *p = k->pq;
     std::lock_guard<std::mutex> lk(p->mu);
     g_last_dev_err = 0;
@@ -3108,9 +3141,18 @@ int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
     int rc = prepared_step(ctx, p, partial, [&] { return k->wide ? wide_capture(ctx, k, partial) : keyed_capture(ctx, k, partial); });
     if (rc) return rc;
     const Step &s = p->step;
-    if (!s.exec && !s.empty) return k->wide ? scan_keyed_wide_impl(ctx, &p->q, &k->key, out) : scan_keyed_impl(ctx, &p->q, &k->key, out);
+    if (!s.exec && !s.empty) {
+        if constexpr (tuple) return scan_keyed_wide_impl(ctx, &p->q, &k->keys, out);
+        else return k->wide ? scan_keyed_wide_impl(ctx, &p->q, k->key, out) : scan_keyed_impl(ctx, &p->q, k->key, out);
+    }
+    // the key tables found at the capture
+    auto key_tables = [&](KeyedAnswer<Out> &answer) {
+        if constexpr (tuple) tuple_key_tables(out, answer.owner, k->tag_values, k->codes);
+        else set_key_table(out, answer.owner, k->values);
+    };
     if (s.empty) {  // no block selected: no rows, no keys (n_rows = 0), nothing launched
-        KeyedAnswer<Out> answer(ctx, out, k->values);
+        KeyedAnswer<Out> answer(ctx, out);
+        key_tables(answer);
         answer.done = true;
         return 0;
     }
@@ -3118,10 +3160,13 @@ int keyed_prepared_impl(bydb_ctx *ctx, bydb_prepared_keyed *k, Out *out) {
     rc = query_shape(&p->q, shape);
     if (!rc) rc = replay_step(p, s, keyed_ctl_bytes(shape.fcols.size()), &keyed_stats(out));
     if (rc) return rc;
-    KeyedAnswer<Out> answer(ctx, out, k->values);
+    KeyedAnswer<Out> answer(ctx, out);
+    key_tables(answer);
     if constexpr (partial) rc = partial_answer(p, s, shape, out, out->stats);
     else rc = finalised_answer(p, s, out);
     if (rc) return rc;
+    if constexpr (tuple)
+        if (s.max_rows) tuple_row_entries(out, answer.owner, k->tag_values, k->codes);
     answer.done = true;
     return 0;
 }
@@ -3420,6 +3465,18 @@ int bydb_query_prepare_keyed(bydb_ctx *ctx, const bydb_query *q, const bydb_grou
 
 int bydb_query_prepare_keyed_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_key *key, bydb_prepared_keyed **out) {
     return guarded([&]() -> int { return prepare_keyed_impl(ctx, q, key, true, out); });
+}
+
+int bydb_query_prepare_keys_wide(bydb_ctx *ctx, const bydb_query *q, const bydb_group_keys *keys, bydb_prepared_keyed **out) {
+    return guarded([&]() -> int { return prepare_keyed_impl(ctx, q, keys, true, out); });
+}
+
+int bydb_scan_agg_keys_prepared(bydb_ctx *ctx, bydb_prepared_keyed *k, bydb_keys_result *out) {
+    return guarded([&]() -> int { return keyed_prepared_impl(ctx, k, out); });
+}
+
+int bydb_scan_partials_keys_prepared(bydb_ctx *ctx, bydb_prepared_keyed *k, bydb_keys_partial_rows *out) {
+    return guarded([&]() -> int { return keyed_prepared_impl(ctx, k, out); });
 }
 
 void bydb_query_release_keyed(bydb_ctx *ctx, bydb_prepared_keyed *k) {

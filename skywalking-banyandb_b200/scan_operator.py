@@ -9,9 +9,10 @@ into libbydbgpu.so.  Names and contracts follow the reference:
   output schema = buildAggOutputSchema               aggregation.go:402-418
   Top semantics                                       pkg/query/vectorized/measure/top.go:145-214
 
-A GroupBy key column with per-series values (ScanSpec.series_tags: entity / indexed tags) is densified per series.  At most
-one key column may be a stored tag (a tag column absent from series_tags): the operator then calls bydb_scan_agg_keyed, which adds the
-row's value of that tag to the group (include/bydb_operator.hpp follows the same rules).
+A GroupBy key column with per-series values (ScanSpec.series_tags: entity / indexed tags) is densified per series.  A key column
+that is a stored tag (a tag column absent from series_tags) makes the operator call bydb_scan_agg_keyed(_wide), which adds the row's
+value of that tag to the group.  With max_key_values above 256, two to four stored key columns go to bydb_scan_agg_keys_wide as a
+tuple, in GroupBy order; at 256 or below only one may be a stored tag (include/bydb_operator.hpp follows the same rules).
 """
 from __future__ import annotations
 
@@ -118,7 +119,11 @@ class ScanSpec:
     #   projected tags take their first-seen value) from the far end -- aggregation.go:211-213 on a reversed stream
     max_key_values: int = 0
     # ^ distinct values a stored-tag GroupBy key may take over the query (bydb_group_key.max_values; 0 = the library's 64):
-    #   up to 256 the per-value passes of scan_agg_keyed answer, up to 65,536 the one pass of scan_agg_keyed_wide
+    #   up to 256 the per-value passes of scan_agg_keyed answer, up to 65,536 the one pass of scan_agg_keyed_wide; with two to
+    #   four stored keys (above 256 only) the distinct key tuples (bydb_group_keys.max_values) of scan_agg_keys_wide
+
+
+_MAX_STORED_KEYS = 4   # the tags of a bydb_group_keys tuple
 
 
 def _key_cell(t: ColumnType, k: bytes):
@@ -156,7 +161,7 @@ class GPUScanAgg:
         self._out = BatchSchema(defs)
         self._result: Optional[capi.Result] = None
         self._group_first_series: List[int] = []
-        self._stored_key: Optional[int] = None   # input column of the stored-tag GroupBy key, if any
+        self._stored_keys: List[int] = []   # input columns of the stored-tag GroupBy keys, in GroupBy order
         self._cursor = 0
         self._closed = False
         self._err: Optional[Exception] = None
@@ -194,8 +199,10 @@ class GPUScanAgg:
         cols: List[object] = []
         for ti in self._tag_idx:
             cdef = self._in.Columns[ti]
-            if ti == self._stored_key:
-                cols.append([_key_cell(cdef.Type, k) for k in r.key[lo:hi]])
+            if ti in self._stored_keys:
+                t = self._stored_keys.index(ti)
+                tuple_key = len(self._stored_keys) > 1   # a row's key is then the tuple of its tags' key bytes
+                cols.append([_key_cell(cdef.Type, k[t] if tuple_key else k) for k in r.key[lo:hi]])
                 continue
             vals = self._scan.series_tags.get((cdef.TagFamily, cdef.Name))
             cols.append([None if vals is None else vals[self._group_first_series[g]] for g in r.group_id[lo:hi]])
@@ -208,22 +215,25 @@ class GPUScanAgg:
         sids = np.asarray(sc.series_ids, dtype=np.uint64)
         # group key per series = tuple of key-column values; dense ids in first-appearance order
         # (aggregation.go:211-213; series-major scan order for group-by-entity).  A tag key column without per-series values
-        # is a stored tag: its value changes from row to row, and bydb_scan_agg_keyed adds it to the series group.  Any other
-        # key column (a field) still needs per-series values.
+        # is a stored tag: its value changes from row to row, and bydb_scan_agg_keyed adds it to the series group (above 256
+        # values bydb_scan_agg_keys_wide adds the tuple of two to four of them).  Any other key column (a field) still needs
+        # per-series values.
         keyvals = []
-        self._stored_key = None
+        self._stored_keys = []
         for ki in self._keys:
             cdef = self._in.Columns[ki]
             vals = sc.series_tags.get((cdef.TagFamily, cdef.Name))
             if vals is None and cdef.Role == ColumnRole.RoleTag:
-                if self._stored_key is not None:
+                if self._stored_keys and sc.max_key_values <= 256:
                     raise capi.BydbError(capi.ENOTSUP, f"GroupBy key {cdef.TagFamily}/{cdef.Name}: at most one stored-tag key per query")
-                self._stored_key = ki
+                if len(self._stored_keys) == _MAX_STORED_KEYS:
+                    raise capi.BydbError(capi.ENOTSUP, f"GroupBy key {cdef.TagFamily}/{cdef.Name}: at most four stored-tag keys per query")
+                self._stored_keys.append(ki)
                 continue
             if vals is None or len(vals) != len(sids):
                 raise ValueError(f"GroupBy key {cdef.TagFamily}/{cdef.Name} needs one value per series (entity / indexed tag)")
             keyvals.append(vals)
-        if self._stored_key is not None and sc.order_desc:
+        if self._stored_keys and sc.order_desc:
             raise capi.BydbError(capi.ENOTSUP, "a stored-tag GroupBy key takes the ascending series order only (order_desc)")
         group_of: Dict[tuple, int] = {}
         gids = np.zeros(len(sids), dtype=np.int32)
@@ -245,14 +255,19 @@ class GPUScanAgg:
                        top_desc=self._top.Desc if self._top else True)
         if not self._keys:
             self._group_first_series = ([len(sids) - 1] if sc.order_desc else [0]) if len(sids) else []
-        if self._stored_key is None:
+        ckeys = []
+        for ki in self._stored_keys:
+            cdef = self._in.Columns[ki]
+            ckeys.append((cdef.TagFamily, cdef.Name, capi.VT_INT64 if cdef.Type == ColumnType.ColumnTypeInt64 else 0))
+        if not ckeys:
             self._result = self._ctx.scan_agg(q)
-        else:
-            cdef = self._in.Columns[self._stored_key]
-            vt = capi.VT_INT64 if cdef.Type == ColumnType.ColumnTypeInt64 else 0
+        elif len(ckeys) == 1:
+            family, tag, vt = ckeys[0]
             # above the per-value passes' 256 values, the one-pass form (which answers the same rows)
             keyed = self._ctx.scan_agg_keyed_wide if sc.max_key_values > 256 else self._ctx.scan_agg_keyed
-            self._result = keyed(q, cdef.TagFamily, cdef.Name, sc.max_key_values, vt)
+            self._result = keyed(q, family, tag, sc.max_key_values, vt)
+        else:   # max_key_values counts the distinct tuples
+            self._result = self._ctx.scan_agg_keys_wide(q, ckeys, sc.max_key_values)
         self.stats = self._result.stats
         # offset / limit window over the (Top-ordered) output rows, limit.go:56-73
         n = len(self._result.group_id)
